@@ -4,6 +4,7 @@ hot path (waveform -> log-mel -> two-head conformer -> decoded notes), BASELINE.
 configs/two_head_model.yaml, 64 x 30 s synthetic 44.1 kHz mono clips per GPU, bf16 operands / fp32 accumulate.
 
     python bench.py --gpus N --steps K --warmup W            # this repo (libsome_b200.so kernels)
+    python bench.py ... --dump-outputs DIR                   # + the outputs of the last timed step as DIR/*.npy
     python bench.py --impl reference ...                     # the reference algorithm on the host CPU cores
 
 A "step" = one pass of the hot path over one batch (64 clips x 30 s = 1920 audio-seconds per GPU; weak
@@ -47,7 +48,8 @@ def load_peaks():
         return {'hbm_gbs': p['hbm_gbs'], 'tf_burst': p['bf16_tflops'], 'tf_sustained': p['bf16_tflops_sustained'],
                 'source': 'measured (MEASURED_PEAKS.json)'}
     except Exception:
-        return {'hbm_gbs': 6650.0, 'tf_burst': 1590.0, 'tf_sustained': 1400.0, 'source': 'fallback (B200_PROFILING.md)'}
+        # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16 tensor rate; not a measured figure
+        return {'hbm_gbs': 3350.0, 'tf_burst': 989.0, 'tf_sustained': 989.0, 'source': 'H100 SXM data sheet'}
 
 
 def make_clips(first_index, count, seconds):
@@ -118,8 +120,8 @@ class ClockSampler:
 def time_cpu_reference(config_name, clips, threads=None):
     """Times the reference ALGORITHM on the host cores: the oracle port (oracle/decode.infer = the serial batch-1 loop of
     inference/base_infer.py:46-53 in fp32 torch, with the vectorised decode forms that match the speed of the reference's
-    torch ops and the mel basis built once).  /root/reference itself is not on the GPU box; the port is pinned to it by
-    tests/golden (also at 30 s / 10 s clips)."""
+    torch ops and the mel basis built once).  The port is pinned to the reference by the golden vectors under tests/golden
+    (also at 30 s / 10 s clips)."""
     from oracle import decode as odecode
     if threads:
         torch.set_num_threads(threads)
@@ -196,9 +198,35 @@ def _pinned(clips):
     return out
 
 
-def measure_batch(ins, config_name, clips_per_gpu, seconds, steps, warmup, rank, world, dev, full, sampler=None):
+DUMP_PROB_ROWS = 16384   # seeded sample of probs rows written by --dump-outputs (the full [frames, 128] array is ~85 MB)
+
+
+def dump_outputs(eng, ws, cu, m, note_count, dump_dir):
+    """What the timed device path hands its caller after its last step: the decoded notes of every clip (concatenated in
+    clip order, with the per-clip counts), the bounds of every frame and a fixed seeded sample of the probs rows."""
+    os.makedirs(dump_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    nc = note_count.cpu().numpy()
+    notes = eng.unpack(cu, nc, ws.note_midi[:m].cpu().numpy(), ws.note_dur[:m].cpu().numpy(), ws.note_rest[:m].cpu().numpy())
+    rows = np.sort(np.random.default_rng(0).choice(m, size=min(m, DUMP_PROB_ROWS), replace=False))
+    arrays = {
+        'note_count': nc.astype(np.float32),
+        'note_midi': np.concatenate([n['note_midi'] for n in notes]).astype(np.float32),
+        'note_dur': np.concatenate([n['note_dur'] for n in notes]).astype(np.float64),
+        'note_rest': np.concatenate([n['note_rest'] for n in notes]).astype(np.float32),
+        'bounds': ws.bounds[:m].cpu().numpy().astype(np.float32),
+        'probs_rows': rows.astype(np.float64),
+        'probs_sample': ws.probs[torch.from_numpy(rows).to(ws.probs.device)].cpu().numpy().astype(np.float32),
+    }
+    for name, a in arrays.items():
+        np.save(os.path.join(dump_dir, f'{name}.npy'), a)
+
+
+def measure_batch(ins, config_name, clips_per_gpu, seconds, steps, warmup, rank, world, dev, full, sampler=None,
+                  dump_dir=None):
     """Device-resident value, end-to-end value and per-kernel roofline of one (config, batch) on this rank; `full` adds the
-    pageable-input variant, the e2e breakdown, the strong-scaling figure and the parity check of the headline line."""
+    pageable-input variant, the e2e breakdown, the strong-scaling figure and the parity check of the headline line.
+    dump_dir: rank 0 writes the outputs of the last timed step there (dump_outputs)."""
     import torch.distributed as dist
     from some_b200 import dist as sdist
     eng = ins.model
@@ -239,6 +267,8 @@ def measure_batch(ins, config_name, clips_per_gpu, seconds, steps, warmup, rank,
     barrier()
     dev_ms = ev0.elapsed_time(ev1)
     launches = eng.launches - launches0
+    if dump_dir is not None and rank == 0:
+        dump_outputs(eng, ws, cu, m, note_count, dump_dir)
     # second pass of the same K steps with CUDA events around every launch (recorded by the sequencer itself) for the roofline
     eng.start_profile(cu)
     barrier()
@@ -453,7 +483,8 @@ def run_ours(args, rank, world, local_rank):
     ins = build_plugin(args.config, local_rank)
     eng = ins.model
     sampler = ClockSampler(local_rank) if rank == 0 else None
-    meas = measure_batch(ins, args.config, args.clips, args.seconds, args.steps, args.warmup, rank, world, dev, True, sampler)
+    meas = measure_batch(ins, args.config, args.clips, args.seconds, args.steps, args.warmup, rank, world, dev, True, sampler,
+                         args.dump_outputs)
     s = summarise(meas, args.steps, world, peaks)
 
     extra = {}
@@ -492,16 +523,6 @@ def run_ours(args, rank, world, local_rank):
     if rank != 0:
         return
 
-    traffic, traffic_src = None, None
-    for name in ('r02_gemm_traffic.json', 'r01_gemm_traffic.json'):
-        try:
-            with open(os.path.join(REPO, 'profiles', name)) as f:
-                traffic = json.load(f).get('dram_bytes_per_launch')
-                traffic_src = (f'profiles/{name} (ncu dram__bytes_read.sum + dram__bytes_write.sum of the same command; '
-                               f'not re-measured in this run)')
-                break
-        except Exception:
-            pass
     m = meas['frames']
     line = {
         'metric': METRIC, 'value': s['value'], 'unit': 'audio-s/s', 'n_gpus': world, 'steps': args.steps,
@@ -509,7 +530,7 @@ def run_ours(args, rank, world, local_rank):
         'scaling': 'weak', 'vs_baseline': None, 'dtype': 'bf16', 'data': 'synthetic',
         'config': {'workload': workload_name(args.config, args.clips, args.seconds), 'clips_per_gpu': args.clips,
                    'clip_seconds': args.seconds, 'frames_per_gpu': m, 'parallelism': f'dp{world}',
-                   'l2': f'inputs ({meas["audio_mb"]:.0f} MB audio, {m * 512 * 4 * 2 / 1e9:.1f} GB residual streams) exceed the 126 MB L2',
+                   'l2': f'inputs ({meas["audio_mb"]:.0f} MB audio, {m * 512 * 4 * 2 / 1e9:.1f} GB residual streams) exceed the 50 MB L2',
                    'weights': 'seeded random (no pretrained checkpoint offline)',
                    'ln_fold': bool(eng.ln_fold), 'bias_correction': bool(eng.bias_correction)},
         'e2e': {'value': s['e2e_value'], 'unit': 'audio-s/s', 'h2d_bytes_per_step': meas['h2d'], 'd2h_bytes_per_step': meas['d2h'],
@@ -517,9 +538,9 @@ def run_ours(args, rank, world, local_rank):
                 'pageable_value': (meas['audio_seconds_rank'] / meas['pageable_s']) if meas.get('pageable_s') else None},
         'e2e_breakdown': meas.get('e2e_breakdown'),
         'gpu_launches': meas['launches'],
-        'roofline': {'kernel': 'some_gemm (tcgen05, all shapes of a step)', 'bound': 'tensor', 'achieved': s['gemm_tf'],
+        'roofline': {'kernel': 'some_gemm (wgmma, all shapes of a step)', 'bound': 'tensor', 'achieved': s['gemm_tf'],
                      'peak': s['peak_tf'], 'unit': 'TFLOP/s', 'frac': s['gemm_tf'] / s['peak_tf'] if s['peak_tf'] else None,
-                     'traffic': traffic, 'traffic_source': traffic_src, 'peak_source': peaks['source'] + ', sustained bf16',
+                     'peak_source': peaks['source'] + ', sustained bf16',
                      'measured_in': 'second pass of the same K steps with CUDA events around every launch (some_profiler)'},
         'kernels': s['kernels'],
         'gemm_shapes': s['gemm_shapes'],
@@ -550,6 +571,8 @@ def main():
     ap.add_argument('--config', default='two_head', choices=['two_head', 'quant_two_head', 'midi_conformer'])
     ap.add_argument('--clips', type=int, default=64, help='clips per GPU')
     ap.add_argument('--seconds', type=float, default=30.0, help='clip length')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step of the headline workload as DIR/<name>.npy')
     args = ap.parse_args()
     rank = int(os.environ.get('RANK', '0'))
     world = int(os.environ.get('WORLD_SIZE', '1'))

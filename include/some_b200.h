@@ -1,8 +1,8 @@
-/* some_b200.h — C ABI of libsome_b200.so: the B200 (sm_100a) kernels behind SOME's inference hot path.
+/* some_b200.h — C ABI of libsome_b200.so: the H100 (sm_90a) kernels behind SOME's inference hot path.
  *
- * The reference (openvpi/SOME, /root/reference) is pure Python/PyTorch and has NO native FFI; the
+ * The reference (openvpi/SOME) is pure Python/PyTorch and has NO native FFI; the
  * "operator interface" of this path is the set of torch calls listed below.  Each entry point names
- * the reference call site (file:line under /root/reference) it replaces.  INTEGRATION.md shows the
+ * the reference call site (file:line in the reference repository) it replaces.  INTEGRATION.md shows the
  * ctypes binding the reference's inference/ package uses to call them.
  *
  * Conventions
@@ -98,7 +98,7 @@ typedef struct {
 } some_ln_args;
 int some_layernorm(const some_ln_args* args, cudaStream_t stream);
 
-/* ---- K-gemm: C = epilogue(A[M,K] . W[N,K]^T), bf16 operands, fp32 accumulation on tcgen05 tensor cores.
+/* ---- K-gemm: C = epilogue(A[M,K] . W[N,K]^T), bf16 operands, fp32 accumulation on the tensor cores (wgmma).
  * Replaces every nn.Linear / 1x1 Conv1d of the trunk (see gemm.cu header for the call sites). */
 enum some_epilogue {
   SOME_EPI_STORE_BF16 = 0,     /* out bf16 [M,N]   = acc (+ bias)                       to_q|to_kv          */

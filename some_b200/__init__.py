@@ -1,4 +1,4 @@
-"""some_b200 — SOME's inference hot path on B200 (sm_100a).
+"""some_b200 — SOME's inference hot path on H100 (sm_90a).
 
 Public surface (nothing is imported eagerly; the CUDA library is loaded on first use and there is no CPU fallback):
 

@@ -157,7 +157,7 @@ def load():
     if not LIB_PATH.is_file():
         raise SomeB200Error(
             f'{LIB_PATH} not found: build it with `python -c "import __graft_entry__ as g; g.build()"` '
-            f'or `make -C {_HERE / "csrc"}` (nvcc, sm_100a). some_b200 has no CPU fallback.')
+            f'or `make -C {_HERE / "csrc"}` (nvcc, sm_90a). some_b200 has no CPU fallback.')
     lib = C.CDLL(os.fspath(LIB_PATH))
     for name, (restype, argtypes) in EXPORTS.items():
         fn = getattr(lib, name)  # AttributeError if the header and the library disagree

@@ -1,4 +1,4 @@
-"""Dataset-level driver (SURVEY.md §8f-2): the B200 counterpart of batch_infer.py.
+"""Dataset-level driver (SURVEY.md §8f-2): the GPU counterpart of batch_infer.py.
 
 The reference transcribes a DiffSinger dataset strictly one file at a time (batch_infer.py:164-176: librosa.load -> Slicer ->
 infer on that file's chunks, a handful of 5-15 s clips per launch sequence).  Here the chunks of MANY recordings form one

@@ -1,7 +1,7 @@
 """Configuration and checkpoint-schema helpers for the SOME inference hot path.
 
 * ``flatten_config`` restates the ``base_config`` inheritance of
-  /root/reference/utils/config_utils.py:11-41 (read_full_config / override_dict) so the
+  the reference's utils/config_utils.py:11-41 (read_full_config / override_dict) so the
   stock ``configs/*.yaml`` chain can be flattened into the ``config.yaml`` the reference
   writes beside a checkpoint (train.py:42-43) and that infer.py:21 reads back.
 * ``model_param_shapes`` is the strict ``state_dict`` schema of
@@ -17,7 +17,7 @@ from typing import Dict, Tuple
 
 import yaml
 
-# The model geometry the sm_100a kernels are specialised for (every shipped config uses it:
+# The model geometry the sm_90a kernels are specialised for (every shipped config uses it:
 # configs/{two_head_model,quant_two_head_model,midi_conformer,continuous,discrete}.yaml).
 DIM = 512
 HEADS = 8

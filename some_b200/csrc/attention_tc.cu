@@ -1,29 +1,20 @@
-// K-attn (tcgen05): per-clip (var-len) multi-head self-attention softmax(Q K^T / 8) V, no mask, 8 heads x 64
+// K-attn (wgmma): per-clip (var-len) multi-head self-attention softmax(Q K^T / 8) V, no mask, 8 heads x 64
 // (base_attention.py:34-45; conform_blocke never forwards a mask: Gconform.py:83-84,133).
 //
 // Input: the fused to_q|to_kv GEMM output qkv bf16 [M, 1536] = [q | k | v] (heads 64-wide, contiguous);
 // output bf16 [M, 512] = 'b h t c -> b t (h c)'.  No head-major copies are made: Q/K/V tiles are TMA boxes cut
 // straight out of qkv.
 //
-// CTA = 128 query rows of one (clip, head), 64-key tiles; 2 CTAs per SM (98 KB smem, 256 TMEM columns each).
-// The kernel is bound by the MUFU pipe (one ex2 per score: 8192 per tile = 512 clk/SM against 256 clk of tensor work),
-// so the design goal is to keep the four XU pipes fed: TWO independent softmax warpgroups per CTA, each owning every
-// other key tile with its OWN running maximum, row sum and O accumulator (split-K inside the CTA, merged once at the
-// end), so that while one group waits for its PV / next QK^T the other one is exponentiating.
-// Roles (320 threads):
-//   warp 0    TMA producer: Q once, then (K_j, V_j) 64-key tiles into a 5-stage ring (128-B swizzle)
-//   warp 1    MMA issuer (one thread):  S_j = Q K_j^T (tcgen05.mma M128 N64 K16 x4, both operands K-major) into S[j & 1];
-//             O[j & 1] += P_j V_j (M128 N64 K16 x4, A = P from TENSOR MEMORY, B = V MN-major); QK_{j+2} right behind PV_j
-//   warps 2-5 softmax group 0 (even tiles), warps 6-9 group 1 (odd tiles); thread = query row (TMEM lane): online
-//             softmax in base 2 (packed f32x2 scale/sum, ex2.approx), P -> bf16 pairs -> tcgen05.st over the first half of
-//             the S buffer just read.  There is NO row-maximum pass in the steady state: the exp pass runs against the
-//             group's stale reference maximum (exact: the final division by the row sum removes the reference) and a tile
-//             whose row sum exceeds 2^14 (some p > 2^8, +inf on overflow) is redone the slow way -- row maximum, O rescaled
-//             in TMEM (tcgen05.ld / st), l rescaled, exp pass again (S_j is intact: P is stored last).  The first tile of a
-//             group takes the slow path.  warp 2 also owns the TMEM allocation: S0 | S1 | O0 | O1, 64 columns each.
+// CTA = 128 query rows of one (clip, head), 64-key tiles; 2 CTAs per SM (81 KB smem each).
+// Roles (288 threads):
+//   warps 0-7   two consumer warpgroups, 64 query rows each (wgmma M = 64).  Per key tile:
+//               S = Q K_j^T (wgmma m64n64k16 x4, both operands K-major in shared memory) into 32 fp32 registers,
+//               online softmax in base 2 on the registers (row = a quad of lanes), P -> bf16 pairs that are already in
+//               the register layout of a wgmma A operand, O += P V_j (wgmma m64n64k16 x4, A from registers, B = V MN-major)
+//   warp 8      TMA producer: Q once, then (K_j, V_j) 64-key tiles into a 4-stage ring (128-B swizzle)
 // Rows of K/V beyond the clip end are masked (p = 0); rows beyond M are zero-filled by TMA.
 #include "host_common.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 #include "../../include/some_b200.h"
 
@@ -33,12 +24,10 @@ constexpr int TC_BM = 128;                 // queries per CTA
 constexpr int TC_BN = 64;                  // keys per tile
 constexpr int TC_QTILE = 128 * 64 * 2;     // 16 KB
 constexpr int TC_KTILE = TC_BN * 64 * 2;   // 8 KB (K or V tile)
-constexpr int TC_STAGES = 5;  // K/V tile j+3 is requested when PV_{j-1} retires: two tile periods to cover the TMA latency
-constexpr int TC_THREADS = 320;
+constexpr int TC_STAGES = 4;
+constexpr int TC_THREADS = 288;
 constexpr int TC_BAR_BYTES = 256;
-constexpr int TC_SMEM = TC_QTILE + TC_STAGES * 2 * TC_KTILE + TC_BAR_BYTES + 2 * TC_BM * 8 /*group stats*/;
-constexpr uint32_t TC_TMEM_COLS = 256;
-constexpr uint32_t TC_O_COL = 128;
+constexpr int TC_SMEM = 1024 /*align slack*/ + TC_QTILE + TC_STAGES * 2 * TC_KTILE + TC_BAR_BYTES;
 
 struct AttnTcParams {
   __nv_bfloat16* out[2];
@@ -51,120 +40,49 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// 2^x for a packed pair on the FMA / ALU pipes instead of the MUFU pipe (the kernel's bottleneck): Cody-Waite split with
-// the 1.5 * 2^23 rounding constant, degree-3 polynomial on [-0.5, 0.5] (max relative error 7.7e-5, well inside the bf16
-// rounding of P), exponent spliced in with an integer add.  TC_POLY_OF_8 of every 8 scores take this path.
-__device__ __forceinline__ void exp2_poly2(uint64_t y2, float& p0, float& p1) {
-  float a, b;
-  f2_unpack(y2, a, b);
-  a = fminf(fmaxf(a, -126.f), 126.f);   // upper clamp: an overflowing score must show up as a huge p (it is detected from the row sum)
-  b = fminf(fmaxf(b, -126.f), 126.f);
-  const uint64_t y = f2_pack(a, b);
-  const uint64_t xf = f2_add(y, f2_pack(12582912.f, 12582912.f));
-  const uint64_t n = f2_add(xf, f2_pack(-12582912.f, -12582912.f));
-  const uint64_t r = f2_fma(n, f2_pack(-1.f, -1.f), y);
-  uint64_t q = f2_fma(f2_pack(0.05508868396282196f, 0.05508868396282196f), r, f2_pack(0.24260404706001282f, 0.24260404706001282f));
-  q = f2_fma(q, r, f2_pack(0.6932762265205383f, 0.6932762265205383f));
-  q = f2_fma(q, r, f2_pack(0.9999289512634277f, 0.9999289512634277f));
-  float qa, qb, xa, xb;
-  f2_unpack(q, qa, qb);
-  f2_unpack(xf, xa, xb);
-  p0 = __int_as_float(__float_as_int(qa) + (__float_as_int(xa) << 23));
-  p1 = __int_as_float(__float_as_int(qb) + (__float_as_int(xb) << 23));
-}
-#ifndef TC_POLY_OF_8
-#define TC_POLY_OF_8 2
-#endif
-
-#ifdef SOME_ATTN_TRACE
-// debug build only (tools/attn_trace.py): SM-clock timestamps of one CTA's softmax groups and MMA thread
-__device__ long long* g_attn_trace = nullptr;
-#define ATTN_TRACE(role, tile, ev)                                                                  \
-  do {                                                                                              \
-    if (trace_on && (tile) < 64) g_attn_trace[(((role) * 64) + (tile)) * 4 + (ev)] = clock64();   \
-  } while (0)
-#else
-#define ATTN_TRACE(role, tile, ev) do { } while (0)
-#endif
 
 __global__ void __launch_bounds__(TC_THREADS, 2)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmq0, const __grid_constant__ CUtensorMap tmkv0,
                     const __grid_constant__ CUtensorMap tmq1, const __grid_constant__ CUtensorMap tmkv1,
                     const AttnTcParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
   uint8_t* sKV = smem + TC_QTILE;                                  // stage s: K at +s * 2 * KTILE, V right after it
   uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + TC_STAGES * 2 * TC_KTILE);
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;                      // [TC_STAGES]
   uint64_t* kv_empty = kv_full + TC_STAGES;          // [TC_STAGES]
-  uint64_t* s_full = kv_empty + TC_STAGES;           // [2]
-  uint64_t* p_full = s_full + 2;                     // [2]
-  uint64_t* all_done = p_full + 2;                   // every PV retired
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(all_done + 1);
-  static_assert(8 * (1 + 2 * TC_STAGES + 6) <= TC_BAR_BYTES, "barrier block too small");
-  float2* stats = reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(bars) + TC_BAR_BYTES);  // [2][128] (max, row sum) per group
+  static_assert(8 * (1 + 2 * TC_STAGES) <= TC_BAR_BYTES, "barrier block too small");
 
-  // Role index: 0 = TMA producer, 1 = MMA issuer, 2..9 = softmax.  The sub-partition arbiter favours the HIGHEST warp id, and
-  // the producer / issuer threads sit on the kernel's critical hand-off chain, so with TC_MMA_HIGH_WARP they are hardware warps
-  // 8 and 9 (softmax = hardware warps 0..7) instead of 0 and 1.
-#ifdef TC_MMA_HIGH_WARP
-  const int hw_warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int warp = hw_warp >= 8 ? hw_warp - 8 : hw_warp + 2;
-#else
-  const int hw_warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int warp = hw_warp;
-#endif
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int clip = blockIdx.x / p.tiles_per_clip;
   const int qt = blockIdx.x - clip * p.tiles_per_clip;
   const int row_begin = p.cu_frames[clip];
   const int T = p.cu_frames[clip + 1] - row_begin;
   const int q0 = qt * TC_BM;
-  if (q0 >= T) return;  // whole CTA, before any barrier / TMEM use
+  if (q0 >= T) return;  // whole CTA, before any barrier use
   const int head = blockIdx.y;
   const int grp = blockIdx.z;
   const CUtensorMap* tmq = grp == 0 ? &tmq0 : &tmq1;
   const CUtensorMap* tmkv = grp == 0 ? &tmkv0 : &tmkv1;
   const int n_tiles = (T + TC_BN - 1) / TC_BN;
-#ifdef SOME_ATTN_TRACE
-  const bool trace_on = g_attn_trace != nullptr && blockIdx.x == 7 && blockIdx.y == 3 && blockIdx.z == 0 &&
-                        (lane == 0 || warp == 1) && (warp == 1 || warp == 2 || warp == 6);
-#endif
 
   if (threadIdx.x == 0) {
-    if ((smem_u32(smem) & 1023u) != 0) {
-      printf("some_b200: attention smem base not 1024-byte aligned\n");
-      __trap();
-    }
     tma_prefetch_desc(tmq);
     tma_prefetch_desc(tmkv);
-  }
-  if (warp == 1 && lane == 0) {
     mbar_init(q_full, 1);
     for (int i = 0; i < TC_STAGES; ++i) {
       mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
+      mbar_init(&kv_empty[i], 8);   // one arrival per consumer warp
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_full[i], 4);
-    }
-    mbar_init(all_done, 1);
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc<TC_TMEM_COLS>(tmem_slot);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_launch();     // programmatic dependent launch (host_common.h): qkv is read only after the producing GEMM has completed
   griddep_wait();
 
-#ifdef SOME_ATTN_DIAG_NOMMA
-  if (warp < 2) {
-  } else
-#endif
-  if (warp == 0) {
+  if (warp == 8) {
     if (elect_one_sync()) {
       mbar_arrive_expect_tx(q_full, TC_QTILE);
       tma_load_2d(sQ, tmq, q_full, head * 64, row_begin + q0);
@@ -172,13 +90,6 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmq0, const __grid_const
       uint32_t ph = 0;
       for (int j = 0; j < n_tiles; ++j) {
         mbar_wait(&kv_empty[s], ph ^ 1);
-#ifdef SOME_ATTN_SKIPKV  // timing experiment only (wrong results): half of the K/V traffic
-        if (j >= TC_STAGES && (j & 1)) {
-          mbar_arrive(&kv_full[s]);
-          if (++s == TC_STAGES) s = 0, ph ^= 1;
-          continue;
-        }
-#endif
         mbar_arrive_expect_tx(&kv_full[s], 2 * TC_KTILE);
         uint8_t* dst = sKV + s * 2 * TC_KTILE;
         tma_load_2d(dst, tmkv, &kv_full[s], SOME_DIM + head * 64, row_begin + j * TC_BN);
@@ -187,271 +98,104 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmq0, const __grid_const
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (elect_one_sync()) {
-      constexpr uint32_t idesc_qk = umma_idesc_bf16_f32(TC_BM, TC_BN);
-      constexpr uint32_t idesc_pv = umma_idesc_bf16_f32(TC_BM, 64, 0, 1);  // B = V is MN-major
-      const uint64_t qdesc = umma_desc_kmajor_sw128(smem_u32(sQ));
-      // The serial chain between a group's p_full arrival and its next s_full sits on the critical path of that group
-      // (clock64 timeline, profiles/r02_attention_notes.txt), so it is kept as short as possible:
-      //   * the K/V tile of QK_{j+2} is awaited BEFORE the p_full wait (the thread is idle there anyway),
-      //   * PV_j and QK_{j+2} are issued back to back, the commits follow (kv_empty last: nobody waits for it soon).
-      auto wait_kv = [&](int t) {
-        mbar_wait(&kv_full[t % TC_STAGES], (t / TC_STAGES) & 1);
-        tc_fence_after_sync();
-      };
-      auto issue_qk = [&](int t) {  // S[t & 1] = Q K_t^T   (kv_full[t] already awaited)
-        const int s = t % TC_STAGES;
-        const uint64_t kdesc = umma_desc_kmajor_sw128(smem_u32(sKV + s * 2 * TC_KTILE));
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16_ss(tmem_base + (t & 1) * TC_BN, qdesc + 2 * k, kdesc + 2 * k, idesc_qk, k != 0);
-        umma_commit(&s_full[t & 1]);
-      };
-      mbar_wait(q_full, 0);
-      wait_kv(0);
-      issue_qk(0);
-      if (n_tiles > 1) {
-        wait_kv(1);
-        issue_qk(1);
-      }
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j % TC_STAGES;
-        if (j + 2 < n_tiles) wait_kv(j + 2);      // off the critical path: before the p_full wait
-        ATTN_TRACE(2, j, 0);
-        mbar_wait(&p_full[j & 1], (j >> 1) & 1);  // P_j in tensor memory (and O rescaled if it had to be)
-        tc_fence_after_sync();
-        ATTN_TRACE(2, j, 1);
-        const uint64_t vdesc = umma_desc_mnmajor_sw128(smem_u32(sKV + s * 2 * TC_KTILE + TC_KTILE), 1024);
-        const uint32_t p_tmem = tmem_base + (j & 1) * TC_BN;  // P_j (bf16, two keys per column) overwrote S_j's first 32 columns
-#pragma unroll
-        for (int k = 0; k < 4; ++k)  // 16 keys per MMA: A +8 TMEM columns, B +16 key rows = 2 KB (+128)
-          umma_bf16_ts(tmem_base + TC_O_COL + (j & 1) * 64, p_tmem + 8 * k, vdesc + 128 * k, idesc_pv, j >= 2 || k != 0);
-        ATTN_TRACE(2, j, 2);
-        // S[j & 1] has been consumed (p_full_j): refill it two tiles ahead, right behind PV_j on the in-order tensor pipe
-        if (j + 2 < n_tiles) issue_qk(j + 2);
-        umma_commit(&kv_empty[s]);
-        ATTN_TRACE(2, j, 3);
-      }
-      umma_commit(all_done);
-    }
-    __syncwarp();
-  } else {
-    const int g = (warp - 2) >> 2;  // softmax group: 0 = even key tiles, 1 = odd key tiles
-    const int quad = hw_warp & 3;   // the TMEM lane quadrant this warp may touch
-    const int r = quad * 32 + lane; // query row inside the tile == TMEM lane
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(quad * 32) << 16);
-    const uint32_t t_s = t_lane + g * TC_BN;
-    const uint32_t t_o = t_lane + TC_O_COL + g * 64;
-    const float c = 0.125f * 1.4426950408889634f;  // dim_head^-0.5 * log2(e)
-    const uint64_t c2 = f2_pack(c, c);
-    float m_used = -INFINITY, l = 0.f;
-    int it = 0;
-    for (int j = g; j < n_tiles; j += 2, ++it) {
-      const int valid = min(TC_BN, T - j * TC_BN);  // keys of this tile inside the clip
-#ifndef SOME_ATTN_DIAG_NOMMA     // timing experiment only (wrong results): softmax warps free-running, no MMA / TMA
-      mbar_wait(&s_full[g], it & 1);  // also: PV_{j-2} (this group's previous tile) has retired, O[g] is quiescent
-#endif
-      tc_fence_after_sync();
-#ifdef SOME_ATTN_DIAG_NOSOFTMAX  // timing experiment only (wrong results): hand-off chain and tensor work alone
-      if (true) {
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[g]);
-        continue;
-      }
-#endif
-      ATTN_TRACE(g, j, 0);
-      // The exp pass runs against the STALE reference m_used WITHOUT looking for this tile's maximum first.  That is exact as
-      // long as nothing overflows (the final division by the row sum removes the reference).  A tile whose row sum exceeds 2^14
-      // (=> some p > 2^8; +inf when a score sits more than 2^126 above the reference) is redone the slow way: row maximum, O and
-      // l brought to the new reference, exp pass again -- S_j is still intact in tensor memory because P is stored last.
-      uint32_t pk[32];
-      float tile_sum;
-      bool with_max = (it == 0);
-#pragma unroll 1
-      for (;;) {
-        if (with_max) {
-          uint32_t v[32];
-          float mx = -INFINITY;
-          {
-            uint32_t u[32];
-            tmem_ld_32x32(t_s, v);  // both halves in flight before the single wait
-            tmem_ld_32x32(t_s + 32, u);
-            tmem_ld_wait();
-            if (valid == TC_BN) {  // eight independent chains (a single fmax chain is 32 dependent FMNMX3)
-              float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-              float m4 = -INFINITY, m5 = -INFINITY, m6 = -INFINITY, m7 = -INFINITY;
-#pragma unroll
-              for (int i = 0; i < 32; i += 8) {
-                m0 = fmaxf(m0, fmaxf(__uint_as_float(v[i]), __uint_as_float(v[i + 1])));
-                m1 = fmaxf(m1, fmaxf(__uint_as_float(v[i + 2]), __uint_as_float(v[i + 3])));
-                m2 = fmaxf(m2, fmaxf(__uint_as_float(v[i + 4]), __uint_as_float(v[i + 5])));
-                m3 = fmaxf(m3, fmaxf(__uint_as_float(v[i + 6]), __uint_as_float(v[i + 7])));
-                m4 = fmaxf(m4, fmaxf(__uint_as_float(u[i]), __uint_as_float(u[i + 1])));
-                m5 = fmaxf(m5, fmaxf(__uint_as_float(u[i + 2]), __uint_as_float(u[i + 3])));
-                m6 = fmaxf(m6, fmaxf(__uint_as_float(u[i + 4]), __uint_as_float(u[i + 5])));
-                m7 = fmaxf(m7, fmaxf(__uint_as_float(u[i + 6]), __uint_as_float(u[i + 7])));
-              }
-              mx = fmaxf(fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)), fmaxf(fmaxf(m4, m5), fmaxf(m6, m7)));
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) {
-                if (i < valid) mx = fmaxf(mx, __uint_as_float(v[i]));
-                if (32 + i < valid) mx = fmaxf(mx, __uint_as_float(u[i]));
-              }
-            }
-          }
-          const float m_new = fmaxf(m_used, mx);
-          const float alpha = (it == 0) ? 0.f : ex2_approx((m_used - m_new) * c);
-          m_used = m_new;
-          l *= alpha;
-          if (it > 0 && __any_sync(0xffffffffu, alpha != 1.0f)) {  // O[g] *= alpha (PV_{j-2} has retired: s_full covers it)
-#pragma unroll 1
-            for (int h = 0; h < 2; ++h) {
-              tmem_ld_32x32(t_o + 32 * h, v);
-              tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-              tmem_st_32x32(t_o + 32 * h, v);
-            }
-            tmem_st_wait();
-          }
-        }
-        ATTN_TRACE(g, j, 1);
-        const float mc = m_used * c;
-        const uint64_t nmc2 = f2_pack(-mc, -mc);
-        // ---- pass 2: p = 2^(s c - m c), row sum, bf16 pack
-        uint64_t rs_a = f2_pack(0.f, 0.f), rs_b = rs_a;
-        // 16-column quarters, software-pipelined: the tcgen05.ld of quarter q + 1 is in flight while quarter q is exponentiated
-        auto quarter = [&](const uint32_t(&x)[16], int q) {
-          if (valid == TC_BN) {
-  #pragma unroll
-            for (int i = 0; i < 16; i += 4) {
-              const uint64_t ya = f2_fma(f2_pack(__uint_as_float(x[i]), __uint_as_float(x[i + 1])), c2, nmc2);
-              const uint64_t yb = f2_fma(f2_pack(__uint_as_float(x[i + 2]), __uint_as_float(x[i + 3])), c2, nmc2);
-              float p0, p1, p2, p3;
-              {
-                float y0, y1;
-                f2_unpack(ya, y0, y1);
-                p0 = ex2_approx(y0);
-                p1 = ex2_approx(y1);
-              }
-              if (TC_POLY_OF_8 >= 4 || ((i & 4) && TC_POLY_OF_8 >= 2)) {  // compile-time after unrolling: pair(s) of every 8 scores
-                exp2_poly2(yb, p2, p3);
-              } else {
-                float y2, y3;
-                f2_unpack(yb, y2, y3);
-                p2 = ex2_approx(y2);
-                p3 = ex2_approx(y3);
-              }
-              rs_a = f2_add(rs_a, f2_pack(p0, p1));
-              rs_b = f2_add(rs_b, f2_pack(p2, p3));
-              pk[8 * q + (i >> 1)] = pack_bf16x2(p0, p1);
-              pk[8 * q + (i >> 1) + 1] = pack_bf16x2(p2, p3);
-            }
-          } else {
-  #pragma unroll
-            for (int i = 0; i < 16; i += 2) {
-              float p0 = ex2_approx(fmaf(__uint_as_float(x[i]), c, -mc));
-              float p1 = ex2_approx(fmaf(__uint_as_float(x[i + 1]), c, -mc));
-              if (16 * q + i >= valid) p0 = 0.f;
-              if (16 * q + i + 1 >= valid) p1 = 0.f;
-              rs_a = f2_add(rs_a, f2_pack(p0, p1));
-              pk[8 * q + (i >> 1)] = pack_bf16x2(p0, p1);
-            }
-          }
-        };
-        {
-          uint32_t xa[16], xb[16];
-          tmem_ld_32x16(t_s, xa);
-          tmem_ld_wait();
-          tmem_ld_32x16(t_s + 16, xb);
-          quarter(xa, 0);
-          tmem_ld_wait();
-          tmem_ld_32x16(t_s + 32, xa);
-          quarter(xb, 1);
-          tmem_ld_wait();
-          tmem_ld_32x16(t_s + 48, xb);
-          quarter(xa, 2);
-          tmem_ld_wait();
-          quarter(xb, 3);
-        }
-        {
-          float s0, s1, s2, s3;
-          f2_unpack(rs_a, s0, s1);
-          f2_unpack(rs_b, s2, s3);
-          tile_sum = (s0 + s1) + (s2 + s3);
-        }
-        if (with_max || !__any_sync(0xffffffffu, !(tile_sum <= 16384.f))) break;
-        with_max = true;
-      }
-      l += tile_sum;
-      // ---- P -> TMEM: bf16 pairs into the first 32 columns of this row's S buffer (all 64 scores have been consumed); the
-      //      PV MMA takes its A operand straight from tensor memory, so P never touches shared memory.  QK_{j+2} overwrites
-      //      these columns only after PV_j (the MMA pipe executes in issue order).
-      ATTN_TRACE(g, j, 2);
-      tmem_st_32x32(t_s, pk);
-      tmem_st_wait();
-      tc_fence_before_sync();
-      __syncwarp();
-#ifndef SOME_ATTN_DIAG_NOMMA
-      if (lane == 0) mbar_arrive(&p_full[g]);
-#endif
-      ATTN_TRACE(g, j, 3);
-    }
-    // ---- merge the two groups and write O / l -> bf16 -> out[row, head * 64 ..]; group g writes channels [32 g, 32 g + 32)
-    stats[g * TC_BM + r] = make_float2(m_used, l);
-#ifndef SOME_ATTN_DIAG_NOMMA
-    mbar_wait(all_done, 0);
-#endif
-    tc_fence_after_sync();
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    const float2 sa = stats[r], sb = stats[TC_BM + r];
-    const bool two = n_tiles > 1;
-    const float m = fmaxf(sa.x, sb.x);
-    float wa = ex2_approx((sa.x - m) * c);
-    float wb = two ? ex2_approx((sb.x - m) * c) : 0.f;
-    const float inv = 1.0f / (sa.y * wa + sb.y * wb);
-    wa *= inv;
-    wb *= inv;
-    const int qrow = q0 + r;
-    __nv_bfloat16* dst = p.out[grp] + (size_t)(row_begin + qrow) * SOME_DIM + head * 64 + 32 * g;
-    uint32_t oa[32], ob[32];
-    tmem_ld_32x32(t_lane + TC_O_COL + 32 * g, oa);
-    if (two) tmem_ld_32x32(t_lane + TC_O_COL + 64 + 32 * g, ob);
-    tmem_ld_wait();
-    if (qrow < T) {
-      float o[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) o[i] = __uint_as_float(oa[i]) * wa;
-      if (two) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = fmaf(__uint_as_float(ob[i]), wb, o[i]);
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        reinterpret_cast<uint4*>(dst)[i] = make_uint4(pack_bf16x2(o[8 * i], o[8 * i + 1]), pack_bf16x2(o[8 * i + 2], o[8 * i + 3]),
-                                                      pack_bf16x2(o[8 * i + 4], o[8 * i + 5]), pack_bf16x2(o[8 * i + 6], o[8 * i + 7]));
-    }
-    tc_fence_before_sync();
+    return;
   }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc<TC_TMEM_COLS>(tmem_base);
+
+  // ---- consumers: warpgroup cw owns query rows [64 cw, 64 cw + 64) of the tile; this thread rows r and r + 8 (quad = row)
+  const int cw = warp >> 2;
+  const int q = lane & 3;
+  const int r = cw * 64 + (warp & 3) * 16 + (lane >> 2);
+  const float c = 0.125f * 1.4426950408889634f;  // dim_head^-0.5 * log2(e)
+  const uint64_t qdesc = gmma_desc_kmajor_sw128(smem_u32(sQ + cw * 64 * 128));
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // per row half: running maximum (raw score), partial row sum
+
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < n_tiles; ++j) {
+    const int s = j % TC_STAGES;
+    mbar_wait(&kv_full[s], (j / TC_STAGES) & 1);
+    const uint32_t k_addr = smem_u32(sKV + s * 2 * TC_KTILE);
+    const uint64_t kdesc = gmma_desc_kmajor_sw128(k_addr);
+    float sc[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_m64n64k16_ss(sc, qdesc + 2 * k, kdesc + 2 * k, k != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence(sc);
+
+    // ---- online softmax: sc[4 jj + 2 h + e] = score of row r + 8 h, key 8 jj + 2 q + e of the tile
+    const int valid = min(TC_BN, T - j * TC_BN);  // keys of this tile inside the clip
+    if (valid < TC_BN) {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * jj + 2 * q + e >= valid) sc[4 * jj + e] = sc[4 * jj + 2 + e] = -INFINITY;
+    }
+    uint32_t pa[4][4];   // P as the A operand of PV: k-slice kk = keys [16 kk, 16 kk + 16)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(sc[4 * jj + 2 * h], sc[4 * jj + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx);   // finite: every tile has at least one valid key
+      const float alpha = ex2_approx((m_run[h] - m_new) * c);   // 0 on the first tile (-inf)
+      m_run[h] = m_new;
+      const float mc = m_new * c;
+      float ts = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const float p0 = ex2_approx(fmaf(sc[4 * jj + 2 * h], c, -mc));
+        const float p1 = ex2_approx(fmaf(sc[4 * jj + 2 * h + 1], c, -mc));
+        ts += p0 + p1;
+        // A fragment of wgmma k16: regs {row r k 2q.., row r+8 k 2q.., row r k 8+2q.., row r+8 k 8+2q..}
+        pa[jj >> 1][(jj & 1) * 2 + h] = pack_bf16x2(p0, p1);
+      }
+      l[h] = fmaf(l[h], alpha, ts);
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        o[4 * jj + 2 * h] *= alpha;
+        o[4 * jj + 2 * h + 1] *= alpha;
+      }
+    }
+
+    // ---- O += P V_j: 16 keys per MMA, B = V rows (keys) 16 kk .. : +2 KB
+    const uint32_t v_addr = k_addr + TC_KTILE;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs_tb(o, pa[kk], gmma_desc_mnmajor_sw128(v_addr + kk * 2048, 1024));
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[s]);
+  }
+
+  // ---- O / l -> bf16 -> out[row, head * 64 ..]
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float lt = l[h];
+    lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+    lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+    const float inv = 1.0f / lt;
+    const int qrow = q0 + r + 8 * h;
+    if (qrow < T) {
+      __nv_bfloat16* dst = p.out[grp] + (size_t)(row_begin + qrow) * SOME_DIM + head * 64 + 2 * q;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+    }
   }
 }
 
 }  // namespace some
 
 using namespace some;
-
-#ifdef SOME_ATTN_TRACE
-extern "C" int some_attention_set_trace(long long* buf) {
-  return cudaMemcpyToSymbol(some::g_attn_trace, &buf, sizeof(buf)) == cudaSuccess ? 0 : -1;
-}
-#endif
 
 extern "C" int some_attention_varlen(const some_attn_args* a, cudaStream_t stream) {
   SOME_REQUIRE(a != nullptr && (a->groups == 1 || a->groups == 2), "some_attention_varlen: bad args");
@@ -473,7 +217,7 @@ extern "C" int some_attention_varlen(const some_attn_args* a, cudaStream_t strea
   if (!configured[dev_]) {
     cudaError_t e = cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM);
     SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(attention_tc): %s", cudaGetErrorString(e));
-    // two CTAs per SM need the full shared-memory carveout (2 x 113 KB)
+    // two CTAs per SM need more than the default shared-memory carveout
     e = cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
                              cudaSharedmemCarveoutMaxShared);
     SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(attention_tc carveout): %s", cudaGetErrorString(e));

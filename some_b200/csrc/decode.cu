@@ -13,10 +13,9 @@
 //   phase C  decode_notes_kernel, DEC_NOTE_CTAS CTAs per clip (warp per note; notes are contiguous frame ranges, so no
 //            atomics on global memory): duration, unmasked duration, 128-bin histogram of round(value) -> mode (first
 //            maximal bin), sequential fp32 sum of the values within +-0.5 of the mode (CPU scatter_add order), mean.
-// (Round 1 ran all three phases in ONE CTA per clip: 64 CTAs on 148 SMs, 0.65 ms per 64 x 30 s batch, 2 % of the HBM rate.)
 // Outputs are packed per clip at offset cu_frames[b] (a clip never has more notes than frames).
 #include "host_common.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 #include "../../include/some_b200.h"
 

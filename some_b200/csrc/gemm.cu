@@ -1,21 +1,20 @@
-// K-gemm: persistent, warp-specialised bf16 GEMM on the 5th-gen tensor cores (tcgen05) for every dense
-// contraction of the SOME conformer (reference call sites: Gconform.py:29-34 conform_ffn,
-// base_attention.py:31-32,46 to_q/to_kv/to_out, base_conv.py:65,69 pointwise convs, Gconform.py:85-87
-// glu1/glu2, Gconform.py:124-125,135-136 inln/inln1/outln).
+// K-gemm: persistent, warp-specialised bf16 GEMM on the Hopper tensor cores (wgmma) for every dense contraction of the
+// SOME conformer (reference call sites: Gconform.py:29-34 conform_ffn, base_attention.py:31-32,46 to_q/to_kv/to_out,
+// base_conv.py:65,69 pointwise convs, Gconform.py:85-87 glu1/glu2, Gconform.py:124-125,135-136 inln/inln1/outln).
 //
 //   C[M, N] = epilogue(A[M, K] . W[N, K]^T)        A, W bf16 row-major (both K-major), fp32 accumulate
 //
-// Roles (384 threads, 1 CTA / SM, grid = #SMs, static round-robin tile schedule, N fastest):
-//   warp 0      TMA producer: A box 128x64 + W box BLOCK_Nx64 (128-B swizzle) into a 4-stage smem ring
-//   warp 1      MMA issuer: one thread, tcgen05.mma cta_group::1 kind::f16, M=128, N=BLOCK_N, K=16 x4 per stage
-//   warp 2      TMEM allocator (512 columns = 2 accumulator stages x 256)
-//   warps 4-11  epilogue: tcgen05.ld 32x32b (thread = one output row), fused bias / SiLU / GLU / residual /
-//               sigmoid / softmax, direct vectorised global stores; overlaps the next tile's mainloop
-//               through the double-buffered accumulator.
-// Up to two independent problems (the "midi" and "bound" streams: same shapes, different weights) run in
-// one launch (groups = 2).
+// Roles (384 threads = 3 warpgroups, 1 CTA / SM, grid = #SMs, static round-robin schedule over 128 x 256 tiles, N fastest):
+//   warpgroup 0     TMA producer (one thread): A box 128x64 + W box 256x64 (128-B swizzle) into a 4-stage smem ring;
+//                   gives its registers to the consumers (setmaxnreg)
+//   warpgroups 1-2  consumers: rows [64 c, 64 c + 64) of the tile, wgmma m64n256k16 from shared memory into 128 fp32
+//                   registers per thread, one k-block in flight while the previous one's stage is released; then the fused
+//                   epilogue (bias / SiLU / GLU / residual / LayerNorm fold / sigmoid / softmax) straight from the
+//                   accumulator registers: each quad of lanes stores 8 consecutive columns of a row (32 B in fp32, 16 B in bf16).
+// Up to two independent problems (the "midi" and "bound" streams: same shapes, different weights) run in one launch
+// (groups = 2).
 #include "host_common.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 #include <string.h>
 
@@ -24,11 +23,17 @@
 namespace some {
 
 constexpr int BLOCK_M = 128;
+constexpr int BLOCK_N = 256;
 constexpr int BLOCK_K = 64;
-constexpr int UMMA_K = 16;
+constexpr int WGMMA_K = 16;
 constexpr int STAGES = 4;
-constexpr int EPI_WARPS = 8;
-constexpr int GEMM_THREADS = 128 + EPI_WARPS * 32;
+constexpr int GEMM_THREADS = 384;
+constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;   // 16 KB
+constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;   // 32 KB
+constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+constexpr int GEMM_SMEM = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+static_assert(GEMM_SMEM <= 232448, "gemm_kernel: shared memory over the 227 KB per-CTA limit");
+constexpr int ACC = BLOCK_N / 2;   // accumulator registers per consumer thread
 
 struct GemmGroup {
   const float* bias;   // [N] in packed-column order, or nullptr
@@ -36,6 +41,7 @@ struct GemmGroup {
   const float* resid;  // f32 [M, ld_out] or nullptr (may alias out)
   const float* ln_s;   // LayerNorm-folded consumers: column sums of W' [N]
   float* ln_stats;     // f32 [M][SOME_LN_SLOTS][2] partial (sum x, sum x^2): written by producers, read by consumers
+  __nv_bfloat16* out_bf16;   // LayerNorm producers: bf16 copy of out, row pitch ld_out
 };
 
 struct GemmParams {
@@ -48,379 +54,20 @@ struct GemmParams {
   GemmGroup g[2];
 };
 
-template <int BLOCK_N>
-struct GemmSmem {
-  static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
-  static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-};
-
-// ---------------------------------------------------------------------------------------------------
-// Epilogue for one 32-column chunk of one row.  `col` = first packed output column of the chunk.
 template <int EPI>
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const GemmGroup& g, int row, bool row_ok, int col,
-                                               const uint32_t (&r)[32]) {
-  float v[32];
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-  if (g.bias != nullptr) {
-    const float4* b4 = reinterpret_cast<const float4*>(g.bias + col);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      float4 b = __ldg(b4 + i);
-      v[4 * i + 0] += b.x;
-      v[4 * i + 1] += b.y;
-      v[4 * i + 2] += b.z;
-      v[4 * i + 3] += b.w;
-    }
-  }
-  if constexpr (EPI == SOME_EPI_STORE_BF16 || EPI == SOME_EPI_SILU_BF16) {
-    if constexpr (EPI == SOME_EPI_SILU_BF16) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = silu_fast(v[i]);
-    }
-    if (row_ok) {
-      uint4* dst = reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(g.out) + (size_t)row * p.ld_out + col);
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        dst[i] = make_uint4(pack_bf16x2(v[8 * i + 0], v[8 * i + 1]), pack_bf16x2(v[8 * i + 2], v[8 * i + 3]),
-                            pack_bf16x2(v[8 * i + 4], v[8 * i + 5]), pack_bf16x2(v[8 * i + 6], v[8 * i + 7]));
-    }
-  } else if constexpr (EPI == SOME_EPI_GLU_BF16 || EPI == SOME_EPI_GLU_RESID_F32) {
-    // packed columns: [col, col+16) = "out" channels, [col+16, col+32) = their "gate" channels
-    float o[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) o[i] = v[i] * sigmoid_fast(v[16 + i]);
-    const int oc = col >> 1;  // output channel of o[0]
-    if (row_ok) {
-      if constexpr (EPI == SOME_EPI_GLU_BF16) {
-        uint4* dst = reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(g.out) + (size_t)row * p.ld_out + oc);
-#pragma unroll
-        for (int i = 0; i < 2; ++i)
-          dst[i] = make_uint4(pack_bf16x2(o[8 * i + 0], o[8 * i + 1]), pack_bf16x2(o[8 * i + 2], o[8 * i + 3]),
-                              pack_bf16x2(o[8 * i + 4], o[8 * i + 5]), pack_bf16x2(o[8 * i + 6], o[8 * i + 7]));
-      } else {
-        const float4* rs = reinterpret_cast<const float4*>(g.resid + (size_t)row * p.ld_out + oc);
-        float4* dst = reinterpret_cast<float4*>(static_cast<float*>(g.out) + (size_t)row * p.ld_out + oc);
-        float4 x[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) x[i] = rs[i];
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          dst[i] = make_float4(x[i].x + o[4 * i + 0], x[i].y + o[4 * i + 1], x[i].z + o[4 * i + 2],
-                               x[i].w + o[4 * i + 3]);
-      }
-    }
-  } else if constexpr (EPI == SOME_EPI_RESID_F32) {
-    if (row_ok) {
-      const float4* rs = reinterpret_cast<const float4*>(g.resid + (size_t)row * p.ld_out + col);
-      float4* dst = reinterpret_cast<float4*>(static_cast<float*>(g.out) + (size_t)row * p.ld_out + col);
-      float4 x[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) x[i] = rs[i];
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        dst[i] = make_float4(fmaf(p.alpha, v[4 * i + 0], x[i].x), fmaf(p.alpha, v[4 * i + 1], x[i].y),
-                             fmaf(p.alpha, v[4 * i + 2], x[i].z), fmaf(p.alpha, v[4 * i + 3], x[i].w));
-    }
-  } else if constexpr (EPI == SOME_EPI_BIAS_F32 || EPI == SOME_EPI_SIGMOID_F32) {
-    if constexpr (EPI == SOME_EPI_SIGMOID_F32) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = 1.0f / (1.0f + __expf(-v[i]));
-    }
-    if (row_ok) {
-      float* dst = static_cast<float*>(g.out) + (size_t)row * p.ld_out + col;
-      if (col + 32 <= p.n_valid && (p.ld_out & 3) == 0) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          reinterpret_cast<float4*>(dst)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (col + i < p.n_valid) dst[i] = v[i];
-      }
-    }
-  }
-}
-
-template <int BLOCK_N, int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
-            const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1, const GemmParams p) {
-  using S = GemmSmem<BLOCK_N>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES);
-  uint64_t* full_bar = bars;                    // [STAGES]
-  uint64_t* empty_bar = bars + STAGES;          // [STAGES]
-  uint64_t* tmem_full = bars + 2 * STAGES;      // [2]
-  uint64_t* tmem_empty = bars + 2 * STAGES + 2; // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  const int num_m = (p.M + BLOCK_M - 1) / BLOCK_M;
-  const int num_n = (p.N + BLOCK_N - 1) / BLOCK_N;
-  const int tiles_per_group = num_m * num_n;
-  const int num_tiles = tiles_per_group * p.groups;
-  const int num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA0);
-    tma_prefetch_desc(&tmB0);
-    if (p.groups > 1) {
-      tma_prefetch_desc(&tmA1);
-      tma_prefetch_desc(&tmB1);
-    }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], EPI_WARPS);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 2) tmem_alloc<512>(tmem_slot);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-  griddep_launch();
-  griddep_wait();
-
-  if (warp == 0) {
-    if (elect_one_sync()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int grp = tile / tiles_per_group;
-        const int t = tile - grp * tiles_per_group;
-        const int m_blk = t / num_n, n_blk = t - m_blk * num_n;
-        const CUtensorMap* ta = grp == 0 ? &tmA0 : &tmA1;
-        const CUtensorMap* tb = grp == 0 ? &tmB0 : &tmB1;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], S::STAGE_BYTES);
-          uint8_t* sa = smem + stage * S::STAGE_BYTES;
-          tma_load_2d(sa, ta, &full_bar[stage], kb * BLOCK_K, m_blk * BLOCK_M);
-          tma_load_2d(sa + S::A_BYTES, tb, &full_bar[stage], kb * BLOCK_K, n_blk * BLOCK_N);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (elect_one_sync()) {
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(BLOCK_M, BLOCK_N);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after_sync();
-          const uint32_t sa = smem_u32(smem + stage * S::STAGE_BYTES);
-          const uint64_t adesc = umma_desc_kmajor_sw128(sa);
-          const uint64_t bdesc = umma_desc_kmajor_sw128(sa + S::A_BYTES);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            // advance 16 bf16 = 32 B along K inside the 128-B swizzle atom: +2 in the (addr >> 4) field
-            umma_bf16_ss(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // smem slot reusable once these MMAs have read it
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);  // accumulator complete
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int ew = warp - 4;
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may access
-    const int half = ew >> 2;   // column half of the tile
-    constexpr int COLS_PER_WARP = BLOCK_N / 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int grp = tile / tiles_per_group;
-      const int t = tile - grp * tiles_per_group;
-      const int m_blk = t / num_n, n_blk = t - m_blk * num_n;
-      const GemmGroup& g = p.g[grp];
-      const int row = m_blk * BLOCK_M + quad * 32 + lane;
-      const bool row_ok = row < p.M;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after_sync();
-      const uint32_t t_row = tmem_base + acc * BLOCK_N + (static_cast<uint32_t>(quad * 32) << 16);
-      if constexpr (EPI == SOME_EPI_SOFTMAX_F32) {
-        // whole row in one thread: pass 1 max, pass 2 sum, pass 3 write (TMEM re-reads are cheap)
-        if (half == 0) {
-          uint32_t r[32];
-          float mx = -INFINITY;
-          for (int c = 0; c < p.n_valid; c += 32) {
-            tmem_ld_32x32(t_row + c, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (c + i < p.n_valid) mx = fmaxf(mx, __uint_as_float(r[i]) + (g.bias ? __ldg(g.bias + c + i) : 0.f));
-          }
-          float sum = 0.f;
-          for (int c = 0; c < p.n_valid; c += 32) {
-            tmem_ld_32x32(t_row + c, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (c + i < p.n_valid) sum += __expf(__uint_as_float(r[i]) + (g.bias ? __ldg(g.bias + c + i) : 0.f) - mx);
-          }
-          const float inv = 1.0f / sum;
-          for (int c = 0; c < p.n_valid; c += 32) {
-            tmem_ld_32x32(t_row + c, r);
-            tmem_ld_wait();
-            if (row_ok) {
-              float* dst = static_cast<float*>(g.out) + (size_t)row * p.ld_out + c;
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (c + i < p.n_valid)
-                  dst[i] = __expf(__uint_as_float(r[i]) + (g.bias ? __ldg(g.bias + c + i) : 0.f) - mx) * inv;
-            }
-          }
-        }
-      } else {
-#pragma unroll 1
-        for (int c = 0; c < COLS_PER_WARP; c += 32) {
-          const int col_in_tile = half * COLS_PER_WARP + c;
-          const int col = n_blk * BLOCK_N + col_in_tile;
-          if (col >= p.N) break;  // ragged last N tile (heads): nothing to store (warp-uniform)
-          uint32_t r[32];
-          tmem_ld_32x32(t_row + col_in_tile, r);
-          tmem_ld_wait();
-          epilogue_chunk<EPI>(p, g, row, row_ok, col, r);
-        }
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc<512>(tmem_base);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// Staged epilogue of the trunk GEMMs.  tcgen05.ld hands every thread ONE ROW of the accumulator, so storing (or
-// reading the residual) straight from that mapping makes each 16-byte access of a warp hit 32 different rows:
-// 32 LSU wavefronts per instruction, which made the epilogue as slow as a K = 512 mainloop
-// (profiles/r01_gemm_epilogue_lsu.txt).  Instead each epilogue warp transposes through a private 32 x 128-byte
-// shared-memory tile (16-byte chunks XOR-swizzled with the row, conflict-free both ways) and then moves it with
-// fully coalesced 128-byte rows: lane -> (row = 4 it + lane / 8, 16-byte chunk = lane % 8).
-__device__ __forceinline__ uint32_t stage_off(int row, int chunk) { return row * 128 + ((chunk ^ (row & 7)) << 4); }
-
-// Hands one staged 32-row x 128-byte tile (bf16 outputs, 128-byte swizzle = the layout stage_off() writes) to a TMA store.
-// Two tiles per warp alternate, so the only wait is for the store issued two flushes ago (lane 0 owns the bulk groups).
-struct StageRing {
-  uint8_t* base;            // two 4 KB tiles of this warp
-  const CUtensorMap* map;   // bf16 output of the current group, box 32 rows x 64 columns
-  uint32_t count;           // flushes so far (across tiles)
-  __device__ __forceinline__ uint8_t* tile() const { return base + (count & 1) * 4096; }
-  // call before the first write into tile(): the store that last read it has finished reading shared memory
-  __device__ __forceinline__ void acquire(int lane) {
-    if (lane == 0) bulk_wait_group_read<1>();
-    __syncwarp();
-  }
-  __device__ __forceinline__ void flush(int lane, int col, int row_base) {
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-      tma_store_2d(map, tile(), col, row_base);
-      bulk_commit_group();
-    }
-    ++count;
-  }
+struct EpiCfg {
+  static constexpr bool LNP = EPI == SOME_EPI_RESID_F32_LN || EPI == SOME_EPI_GLU_RESID_F32_LN;
+  static constexpr bool LNC = EPI == SOME_EPI_LN_STORE_BF16 || EPI == SOME_EPI_LN_SILU_BF16 || EPI == SOME_EPI_LN_GLU_BF16;
+  // the LayerNorm variants share the store path of their plain epilogue
+  static constexpr int BASE = LNC ? EPI - SOME_EPI_LN_STORE_BF16
+                              : EPI == SOME_EPI_RESID_F32_LN ? SOME_EPI_RESID_F32
+                              : EPI == SOME_EPI_GLU_RESID_F32_LN ? SOME_EPI_GLU_RESID_F32 : EPI;
 };
-__device__ __forceinline__ void add_bias32(const float* bias, int col, float (&v)[32]) {
-  if (bias == nullptr) return;
-  const float4* b4 = reinterpret_cast<const float4*>(bias + col);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float4 b = __ldg(b4 + i);
-    v[4 * i + 0] += b.x, v[4 * i + 1] += b.y, v[4 * i + 2] += b.z, v[4 * i + 3] += b.w;
-  }
-}
-__device__ __forceinline__ uint64_t u2_pair(uint32_t lo, uint32_t hi) {   // two accumulator registers as one packed f32x2
-  return f2_pack(__uint_as_float(lo), __uint_as_float(hi));
-}
-// 32 accumulator columns of this thread's row -> 16 packed pairs with the bias (or the folded LayerNorm) applied.
-// LayerNorm folded into the consumer GEMM (Gconform.py:57-62: ffn(norm(x)), att(norm(x)), conv(norm(x))): the accumulator
-// was taken over bf16(x) and W' = W * gamma, so   LN(x) . W^T + bias = rstd * (acc - mean * s_n) + bias'_n   with
-// s_n = sum_k W'[n,k] (ln_s) and bias' = bias + W . beta (passed as bias).  ra2 = (rstd, rstd), nmu2 = (-mean, -mean) of
-// THIS thread's row.  Everything on the packed f32x2 pipes: 2 FFMA2 per pair (the plain bias add is 1 FADD2).
-template <bool kLn, int NC = 32>
-__device__ __forceinline__ void bias_or_ln32(const GemmGroup& g, int col, const uint32_t (&acc)[NC], uint64_t (&v)[NC / 2],
-                                             uint64_t ra2, uint64_t nmu2) {
-  if constexpr (!kLn) {
-    if (g.bias == nullptr) {
-#pragma unroll
-      for (int i = 0; i < NC / 2; ++i) v[i] = u2_pair(acc[2 * i], acc[2 * i + 1]);
-    } else {
-      const float4* b4 = reinterpret_cast<const float4*>(g.bias + col);
-#pragma unroll
-      for (int i = 0; i < NC / 4; ++i) {
-        const float4 b = __ldg(b4 + i);
-        v[2 * i] = f2_add(u2_pair(acc[4 * i], acc[4 * i + 1]), f2_pack(b.x, b.y));
-        v[2 * i + 1] = f2_add(u2_pair(acc[4 * i + 2], acc[4 * i + 3]), f2_pack(b.z, b.w));
-      }
-    }
-  } else {
-    const float4* b4 = reinterpret_cast<const float4*>(g.bias + col);
-    const float4* s4 = reinterpret_cast<const float4*>(g.ln_s + col);
-#pragma unroll
-    for (int i = 0; i < NC / 4; ++i) {
-#ifdef SOME_DIAG_LNC_NOS       // timing experiment only (wrong results)
-      const float4 b = __ldg(b4 + i), s = b;
-#else
-      const float4 b = __ldg(b4 + i), s = __ldg(s4 + i);
-#endif
-      v[2 * i] = f2_fma(f2_fma(f2_pack(s.x, s.y), nmu2, u2_pair(acc[4 * i], acc[4 * i + 1])), ra2, f2_pack(b.x, b.y));
-      v[2 * i + 1] = f2_fma(f2_fma(f2_pack(s.z, s.w), nmu2, u2_pair(acc[4 * i + 2], acc[4 * i + 3])), ra2, f2_pack(b.z, b.w));
-    }
-  }
-}
+
 // Row statistics of the LayerNorm input from the producers' partial sums (nn.LayerNorm: biased variance, eps 1e-5).
-__device__ __forceinline__ void ln_row_coeffs(const GemmParams& p, const GemmGroup& g, int row, uint64_t& ra2, uint64_t& nmu2) {
+__device__ __forceinline__ void ln_row_coeffs(const GemmParams& p, const GemmGroup& g, int row, float& ra, float& nmu) {
   float s = 0.f, q = 0.f;
-#ifdef SOME_DIAG_LNC_NOSTATS   // timing experiment only (wrong results)
-  if (false) {
-#else
   if (row < p.M) {
-#endif
     const float2* st = reinterpret_cast<const float2*>(g.ln_stats) + (size_t)row * SOME_LN_SLOTS;
     for (int i = 0; i < p.ln_parts; ++i) {
       const float2 t = st[i];
@@ -430,177 +77,221 @@ __device__ __forceinline__ void ln_row_coeffs(const GemmParams& p, const GemmGro
   const float inv_d = 1.0f / static_cast<float>(p.K);
   const float mean = s * inv_d;
   const float var = fmaxf(fmaf(-mean, mean, q * inv_d), 0.f);
-  const float ra = rsqrtf(var + 1e-5f);
-  ra2 = f2_pack(ra, ra);
-  nmu2 = f2_pack(-mean, -mean);
+  ra = rsqrtf(var + 1e-5f);
+  nmu = -mean;
 }
 
-// One epilogue warp: rows [row_base, +32) x accumulator columns [col0, col0 + 128) of the tile (col_tile = first packed
-// column of the tile).  t_row = TMEM address of the warp's lane quadrant in the current accumulator stage.
-// EPI = SOME_EPI_STORE_BF16 / SILU_BF16 / GLU_BF16; kLn = LayerNorm-folded consumer (SOME_EPI_LN_*).
-template <int EPI, bool kLn>
-__device__ __forceinline__ void epilogue_warp_staged(const GemmParams& p, const GemmGroup& g, int row_base, int lane,
-                                                     uint32_t t_row, int col0, int col_tile, StageRing& ring) {
-  const int r = lane;  // row inside the warp's 32-row slab == TMEM lane offset
-  uint64_t ra2 = 0, nmu2 = 0;
-  if constexpr (kLn) ln_row_coeffs(p, g, row_base + r, ra2, nmu2);
-  // The warp's 128 accumulator columns go through in eight 16-column granules with the tcgen05.ld of granule i + 1 in flight
-  // while granule i is processed (these epilogues are latency bound: one warp per 32 rows, the K = 512 GEMMs spend more
-  // time here than in their mainloop; a serial ld -> wait -> math chain per 32 columns cost ~20 %).
-  uint32_t a0[16], a1[16];
-  tmem_ld_32x16(t_row + col0, a0);
-  [[maybe_unused]] uint64_t keep[8];   // GLU: the "out" half of a packed 32-column group waits here for its gates
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+
+// Epilogue of one consumer thread: acc holds rows row0 and row0 + 8, columns col_tile + 8 j + 2 q + {0, 1} (j < 32).
+// GLU: packed columns come in 32-column groups [16 "out" | 16 "gate"], so the gate of acc[4 j + i] is acc[4 (j + 2) + i]
+// (j % 4 < 2) and output channel (col_tile + 32 G) / 2 + 8 jj + 2 q + e belongs to group G, j = 4 G + jj.
+// LayerNorm producers: slot col / 128 of ln_stats gets (sum x, sum x^2) of the row over those 128 accumulator columns.
+template <int EPI>
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const GemmGroup& g, float (&acc)[ACC], int row0,
+                                              int col_tile, int q) {
+  using Cfg = EpiCfg<EPI>;
+  constexpr int BASE = Cfg::BASE;
+  const int rows[2] = {row0, row0 + 8};
+  const bool row_ok[2] = {rows[0] < p.M, rows[1] < p.M};
+
+  // ---- bias, or the folded LayerNorm:  LN(x) . W^T + bias = rstd * (acc - mean * s_n) + bias'_n  (s_n = ln_s, bias' = bias)
+  [[maybe_unused]] float ra[2] = {1.f, 1.f}, nmu[2] = {0.f, 0.f};
+  if constexpr (Cfg::LNC) {
+    ln_row_coeffs(p, g, rows[0], ra[0], nmu[0]);
+    ln_row_coeffs(p, g, rows[1], ra[1], nmu[1]);
+  }
+  if (Cfg::LNC || g.bias != nullptr) {
 #pragma unroll
-  for (int gi = 0; gi < 8; ++gi) {
-    tmem_ld_wait();
-    if (gi + 1 < 8) {
-      if (gi & 1) tmem_ld_32x16(t_row + col0 + 16 * (gi + 1), a0);
-      else tmem_ld_32x16(t_row + col0 + 16 * (gi + 1), a1);
-    }
-    uint64_t v[8];
-    if (gi & 1) bias_or_ln32<kLn, 16>(g, col_tile + col0 + 16 * gi, a1, v, ra2, nmu2);
-    else bias_or_ln32<kLn, 16>(g, col_tile + col0 + 16 * gi, a0, v, ra2, nmu2);
-    if constexpr (EPI == SOME_EPI_STORE_BF16 || EPI == SOME_EPI_SILU_BF16) {
-      if constexpr (EPI == SOME_EPI_SILU_BF16) {
+    for (int j = 0; j < ACC / 4; ++j) {
+      const int col = col_tile + 8 * j + 2 * q;
+      if (col >= p.N) continue;   // ragged head tile: bias arrays are padded to 32 floats, not to the tile
+      const float2 b = __ldg(reinterpret_cast<const float2*>(g.bias + col));
+      if constexpr (Cfg::LNC) {
+        const float2 sn = __ldg(reinterpret_cast<const float2*>(g.ln_s + col));
 #pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = silu_fast2(v[i]);
-      }
-      // 16 columns -> 16 bf16 = two 16-byte cells of the 128-byte staged row (64 columns per row)
-      if ((gi & 3) == 0) ring.acquire(lane);
-      uint8_t* stage = ring.tile();
-#pragma unroll
-      for (int q = 0; q < 2; ++q)
-        *reinterpret_cast<uint4*>(stage + stage_off(r, (gi & 3) * 2 + q)) =
-            make_uint4(pack_bf16x2(v[4 * q]), pack_bf16x2(v[4 * q + 1]), pack_bf16x2(v[4 * q + 2]), pack_bf16x2(v[4 * q + 3]));
-      if ((gi & 3) == 3) ring.flush(lane, col_tile + col0 + 64 * (gi >> 2), row_base);
-    } else {
-      static_assert(EPI == SOME_EPI_GLU_BF16, "staged epilogue: STORE / SILU / GLU only");
-      // packed columns: even granule = 16 "out" channels, odd granule = their 16 gates -> 16 bf16 outputs = two cells
-      if ((gi & 1) == 0) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) keep[i] = v[i];
+        for (int h = 0; h < 2; ++h) {
+          acc[4 * j + 2 * h] = fmaf(fmaf(sn.x, nmu[h], acc[4 * j + 2 * h]), ra[h], b.x);
+          acc[4 * j + 2 * h + 1] = fmaf(fmaf(sn.y, nmu[h], acc[4 * j + 2 * h + 1]), ra[h], b.y);
+        }
       } else {
-        uint32_t o[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) o[i] = pack_bf16x2(f2_mul(keep[i], sigmoid_fast2(v[i])));
-        if (gi == 1) ring.acquire(lane);
-        uint8_t* stage = ring.tile();
-#pragma unroll
-        for (int q = 0; q < 2; ++q)
-          *reinterpret_cast<uint4*>(stage + stage_off(r, (gi >> 1) * 2 + q)) = make_uint4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]);
+        for (int h = 0; h < 2; ++h) {
+          acc[4 * j + 2 * h] += b.x;
+          acc[4 * j + 2 * h + 1] += b.y;
+        }
       }
-      if (gi == 7) ring.flush(lane, (col_tile + col0) >> 1, row_base);
+    }
+  }
+
+  if constexpr (BASE == SOME_EPI_STORE_BF16 || BASE == SOME_EPI_SILU_BF16) {
+#pragma unroll
+    for (int j = 0; j < ACC / 4; ++j) {
+      const int col = col_tile + 8 * j + 2 * q;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if constexpr (BASE == SOME_EPI_SILU_BF16) v0 = silu_fast(v0), v1 = silu_fast(v1);
+        if (row_ok[h])
+          *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(g.out) + (size_t)rows[h] * p.ld_out + col) = pack_bf16x2(v0, v1);
+      }
+    }
+  } else if constexpr (BASE == SOME_EPI_GLU_BF16) {
+#pragma unroll
+    for (int G = 0; G < ACC / 16; ++G) {
+#pragma unroll
+      for (int jj = 0; jj < 2; ++jj) {
+        const int j = 4 * G + jj;
+        const int oc = (col_tile >> 1) + 16 * G + 8 * jj + 2 * q;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float o0 = acc[4 * j + 2 * h] * sigmoid_fast(acc[4 * (j + 2) + 2 * h]);
+          const float o1 = acc[4 * j + 2 * h + 1] * sigmoid_fast(acc[4 * (j + 2) + 2 * h + 1]);
+          if (row_ok[h])
+            *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(g.out) + (size_t)rows[h] * p.ld_out + oc) = pack_bf16x2(o0, o1);
+        }
+      }
+    }
+  } else if constexpr (BASE == SOME_EPI_RESID_F32 || BASE == SOME_EPI_GLU_RESID_F32) {
+    constexpr bool GLU = BASE == SOME_EPI_GLU_RESID_F32;
+    [[maybe_unused]] float st_s[2][2] = {}, st_q[2][2] = {};   // [row half][128-column slot of the tile]
+#pragma unroll
+    for (int j = 0; j < ACC / 4; ++j) {
+      if (GLU && (j & 3) >= 2) continue;   // gate columns: consumed with their "out" partners
+      const int oc = GLU ? (col_tile >> 1) + 16 * (j >> 2) + 8 * (j & 3) + 2 * q : col_tile + 8 * j + 2 * q;
+      const int slot = j >> 4;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if constexpr (GLU) {
+          v0 *= sigmoid_fast(acc[4 * (j + 2) + 2 * h]);
+          v1 *= sigmoid_fast(acc[4 * (j + 2) + 2 * h + 1]);
+        }
+        if (row_ok[h]) {
+          const size_t off = (size_t)rows[h] * p.ld_out + oc;
+          const float2 r = *reinterpret_cast<const float2*>(g.resid + off);
+          float2 x;
+          if constexpr (GLU) x = make_float2(r.x + v0, r.y + v1);
+          else x = make_float2(fmaf(v0, p.alpha, r.x), fmaf(v1, p.alpha, r.y));   // alpha * (acc + bias) + resid
+          *reinterpret_cast<float2*>(static_cast<float*>(g.out) + off) = x;
+          if constexpr (Cfg::LNP) {
+            st_s[h][slot] += x.x + x.y;
+            st_q[h][slot] = fmaf(x.x, x.x, fmaf(x.y, x.y, st_q[h][slot]));
+            *reinterpret_cast<uint32_t*>(g.out_bf16 + off) = pack_bf16x2(x.x, x.y);
+          }
+        }
+      }
+    }
+    if constexpr (Cfg::LNP) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int sl = 0; sl < 2; ++sl) {
+          const float s = quad_sum(st_s[h][sl]), qq = quad_sum(st_q[h][sl]);
+          if (q == 0 && row_ok[h])
+            reinterpret_cast<float2*>(g.ln_stats)[(size_t)rows[h] * SOME_LN_SLOTS + (col_tile >> 7) + sl] = make_float2(s, qq);
+        }
+      }
+    }
+  } else if constexpr (BASE == SOME_EPI_BIAS_F32 || BASE == SOME_EPI_SIGMOID_F32) {
+#pragma unroll
+    for (int j = 0; j < ACC / 4; ++j) {
+      const int col = col_tile + 8 * j + 2 * q;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float v = acc[4 * j + 2 * h + e];
+          if constexpr (BASE == SOME_EPI_SIGMOID_F32) v = 1.0f / (1.0f + __expf(-v));
+          if (row_ok[h] && col + e < p.n_valid) static_cast<float*>(g.out)[(size_t)rows[h] * p.ld_out + col + e] = v;
+        }
+      }
+    }
+  } else {
+    static_assert(BASE == SOME_EPI_SOFTMAX_F32, "unknown epilogue");
+    // the whole row is in this tile (N <= 256): a quad of lanes holds it
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < ACC / 4; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * j + 2 * q + e < p.n_valid) mx = fmaxf(mx, acc[4 * j + 2 * h + e]);
+      mx = quad_max(mx);
+      float sum = 0.f;   // exponentials in place: the row is read once more only to be scaled and stored
+#pragma unroll
+      for (int j = 0; j < ACC / 4; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& v = acc[4 * j + 2 * h + e];
+          v = 8 * j + 2 * q + e < p.n_valid ? __expf(v - mx) : 0.f;
+          sum += v;
+        }
+      const float inv = 1.0f / quad_sum(sum);
+      if (row_ok[h]) {
+        float* dst = static_cast<float*>(g.out) + (size_t)rows[h] * p.ld_out;
+#pragma unroll
+        for (int j = 0; j < ACC / 4; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * j + 2 * q + e;
+            if (col < p.n_valid) dst[col] = acc[4 * j + 2 * h + e] * inv;
+          }
+      }
     }
   }
 }
 
-// ---------------------------------------------------------------------------------------------------
-// CTA-pair variant (cta_group::2): a cluster of two CTAs computes a 256 x 256 tile with M = 256 MMAs.  Each CTA
-// loads its own 128 rows of A and only HALF of the W tile (128 rows), so the L2 -> SM traffic per MAC drops
-// from (128 + 256) / (128 * 256) to (128 + 128) / (128 * 256) operand rows: the single-CTA kernel is capped by
-// the ~6300 B/clk L2 -> SM fabric at ~45 % of the tensor peak (profiles/r01_gemm_ncu_full_summary.csv).
-//   producer (warp 0, both CTAs): TMA with .cta_group::2, completion bytes land on the LEADER's full barrier
-//   MMA (warp 1, leader only): tcgen05.mma.cta_group::2 M256 N256 K16; commits are multicast to both CTAs
-//   epilogue (warps 4-11, both CTAs): own 128 TMEM lanes; tmem_empty arrivals go to the leader (remote arrive)
-//
-// Residual epilogues (RESID_F32, GLU_RESID_F32 and their LayerNorm-producer variants) move ALL of their global traffic
-// with TMA.  Per epilogue warp and 32-column chunk: the fp32 residual slab (32 rows x 128 B) is TMA-loaded one chunk ahead
-// into a 128-byte-swizzled shared-memory slab, so the thread that owns accumulator row r (tcgen05.ld: thread = row) reads
-// its row's residual conflict-free, adds alpha * (acc + bias) IN PLACE, and one elected lane TMA-stores the slab.  Nothing
-// goes through the LSU to global memory and no residual registers are held (the round-1 epilogue kept 32 and sat at ~0.69
-// of the HBM floor on the N = K = 512 GEMMs, profiles/r01_gemm_epilogue_lsu.txt).  Because the final row values pass
-// through the row-owning thread, the LayerNorm-producer variants get the row statistics for free: each thread sums x and
-// x^2 over its 128 (RESID) / 64 (GLU) columns of the tile, writes the pair into its slot of ln_stats, and also packs
-// bf16(x) into a third swizzled tile that is TMA-stored every second chunk (the consumer GEMM's A operand).
-constexpr int PAIR_BN = 256;
-constexpr int PAIR_STAGE_BYTES = BLOCK_M * BLOCK_K * 2 + (PAIR_BN / 2) * BLOCK_K * 2;  // 16 KB A + 16 KB half W
-constexpr int PAIR_BAR_BYTES = 512;
-
-struct EpiMaps {        // tensor maps of the TMA epilogues, per group: residual (load), out (store), bf16 copy (store)
-  CUtensorMap r[2], o[2], xb[2];
-};
-
 template <int EPI>
-struct PairCfg {
-  static constexpr bool LNP = EPI == SOME_EPI_RESID_F32_LN || EPI == SOME_EPI_GLU_RESID_F32_LN;
-  static constexpr bool GLU_R = EPI == SOME_EPI_GLU_RESID_F32 || EPI == SOME_EPI_GLU_RESID_F32_LN;
-  static constexpr bool TMA_EPI = LNP || EPI == SOME_EPI_RESID_F32 || EPI == SOME_EPI_GLU_RESID_F32;
-  static constexpr bool LNC = EPI == SOME_EPI_LN_STORE_BF16 || EPI == SOME_EPI_LN_SILU_BF16 || EPI == SOME_EPI_LN_GLU_BF16;
-  static constexpr int BASE = LNC ? EPI - SOME_EPI_LN_STORE_BF16 : EPI;   // staged epilogues: STORE / SILU / GLU
-  static constexpr int STAGES = LNP ? 4 : 5;
-  // per epilogue warp: two 32 x 128 B output tiles, or two residual slabs (+ the bf16 tile of the LN producers)
-  static constexpr int WARP_BYTES = TMA_EPI ? (LNP ? 12288 : 8192) : 8192;   // staged: two alternating 4 KB tiles
-  static constexpr int EPI_BYTES = EPI_WARPS * WARP_BYTES;
-  static constexpr int SMEM = STAGES * PAIR_STAGE_BYTES + EPI_BYTES + 1024 + PAIR_BAR_BYTES;
-  static_assert(SMEM <= 232448, "gemm_pair_kernel: shared memory over the 227 KB per-CTA limit");
-};
-
-template <int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
-                 const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1,
-                 const __grid_constant__ EpiMaps em, const GemmParams p) {
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
+            const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  using Cfg = PairCfg<EPI>;
-  constexpr int PAIR_STAGES = Cfg::STAGES;
-  uint8_t* epi_stage = smem + PAIR_STAGES * PAIR_STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(epi_stage + Cfg::EPI_BYTES);
-  uint64_t* full_bar = bars;                               // [STAGES]  (used in the leader)
-  uint64_t* empty_bar = bars + PAIR_STAGES;                // [STAGES]  (local, multicast commit)
-  uint64_t* tmem_full = bars + 2 * PAIR_STAGES;            // [2]       (local, multicast commit)
-  uint64_t* tmem_empty = bars + 2 * PAIR_STAGES + 2;       // [2]       (used in the leader)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * PAIR_STAGES + 4);
-  [[maybe_unused]] uint64_t* ld_bar = bars + 2 * PAIR_STAGES + 6;      // [EPI_WARPS][2] residual slabs (TMA epilogues)
-  static_assert(8 * (2 * PAIR_STAGES + 6 + 2 * EPI_WARPS) <= PAIR_BAR_BYTES, "barrier block too small");
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);   // [STAGES]
+  uint64_t* empty_bar = full_bar + STAGES;                                          // [STAGES]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
+  const int wg = threadIdx.x >> 7;
 
-  const int num_m = (p.M + 2 * BLOCK_M - 1) / (2 * BLOCK_M);
-  const int num_n = p.N / PAIR_BN;
+  const int num_m = (p.M + BLOCK_M - 1) / BLOCK_M;
+  const int num_n = (p.N + BLOCK_N - 1) / BLOCK_N;
   const int tiles_per_group = num_m * num_n;
   const int num_tiles = tiles_per_group * p.groups;
   const int num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
-  const int pair = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA0);
     tma_prefetch_desc(&tmB0);
     if (p.groups > 1) {
       tma_prefetch_desc(&tmA1);
       tma_prefetch_desc(&tmB1);
     }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < PAIR_STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);   // the leader's producer arrives and expects the bytes of BOTH CTAs
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 2 * EPI_WARPS);
-    }
-    if constexpr (Cfg::TMA_EPI) {
-      for (int i = 0; i < 2 * EPI_WARPS; ++i) mbar_init(&ld_bar[i], 1);
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);   // one arrival per consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc_pair<512>(tmem_slot);
-  tc_fence_before_sync();
-  cluster_sync_all();   // barrier inits + TMEM allocation of BOTH CTAs visible before any remote arrive / multicast
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   griddep_launch();     // programmatic dependent launch: the next kernel may start its own prologue ...
   griddep_wait();       // ... and this one touches activations only after its predecessor has completed
 
-  if (warp == 0) {
-    if (elect_one_sync()) {
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one_sync()) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int grp = tile / tiles_per_group;
         const int t = tile - grp * tiles_per_group;
         const int m_blk = t / num_n, n_blk = t - m_blk * num_n;
@@ -608,14 +299,11 @@ gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
         const CUtensorMap* tb = grp == 0 ? &tmB0 : &tmB1;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          const uint32_t full_leader = mapa_u32(smem_u32(&full_bar[stage]), 0);
-          // The follower never arrives: its bytes may land before the leader's expect_tx (the transaction count goes
-          // negative transiently) but the phase cannot complete until the leader has arrived and all bytes are in.
-          if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * PAIR_STAGE_BYTES);
-          uint8_t* sa = smem + stage * PAIR_STAGE_BYTES;
-          tma_load_2d_pair(sa, ta, full_leader, kb * BLOCK_K, m_blk * 2 * BLOCK_M + rank * BLOCK_M);
-          tma_load_2d_pair(sa + BLOCK_M * BLOCK_K * 2, tb, full_leader, kb * BLOCK_K, n_blk * PAIR_BN + rank * (PAIR_BN / 2));
-          if (++stage == PAIR_STAGES) {
+          mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);   // out-of-bounds rows are zero-filled and still counted
+          uint8_t* sa = smem + stage * STAGE_BYTES;
+          tma_load_2d(sa, ta, &full_bar[stage], kb * BLOCK_K, m_blk * BLOCK_M);
+          tma_load_2d(sa + A_BYTES, tb, &full_bar[stage], kb * BLOCK_K, n_blk * BLOCK_N);
+          if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
           }
@@ -623,247 +311,53 @@ gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (leader && elect_one_sync()) {
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(2 * BLOCK_M, PAIR_BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + acc * PAIR_BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after_sync();
-          const uint32_t sa = smem_u32(smem + stage * PAIR_STAGE_BYTES);
-          const uint64_t adesc = umma_desc_kmajor_sw128(sa);
-          const uint64_t bdesc = umma_desc_kmajor_sw128(sa + BLOCK_M * BLOCK_K * 2);
+  } else {
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1;   // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int grp = tile / tiles_per_group;
+      const int t = tile - grp * tiles_per_group;
+      const int m_blk = t / num_n, n_blk = t - m_blk * num_n;
+      float acc[ACC];
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+        const uint64_t adesc = gmma_desc_kmajor_sw128(sa + cw * 64 * 128);
+        const uint64_t bdesc = gmma_desc_kmajor_sw128(sa + A_BYTES);
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-            umma_bf16_ss_pair(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          umma_commit_pair(&empty_bar[stage], 0b11);   // both CTAs' producers may refill this slot
-          if (++stage == PAIR_STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit_pair(&tmem_full[acc], 0b11);        // both CTAs' epilogues may read their accumulator half
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
+        for (int k = 0; k < BLOCK_K / WGMMA_K; ++k)   // +16 bf16 = 32 B along K inside the 128-B swizzle atom: +2 in (addr >> 4)
+          wgmma_m64n256k16_ss(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous k-block's MMAs have finished reading their stage
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
         }
       }
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      const GemmGroup g = grp == 0 ? p.g[0] : p.g[1];   // no dynamic index into the parameter space (a local copy)
+      epilogue_tile<EPI>(p, g, acc, m_blk * BLOCK_M + cw * 64 + (warp & 3) * 16 + (lane >> 2), n_blk * BLOCK_N,
+                         lane & 3);
     }
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int ew = warp - 4;
-    const int quad = warp & 3;
-    const int half = ew >> 2;
-    constexpr int COLS_PER_WARP = PAIR_BN / 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    if constexpr (Cfg::TMA_EPI) {
-      constexpr int NCH = Cfg::GLU_R ? 2 : 4;            // 32-output-column chunks per tile visit of this warp
-      uint8_t* wbase = epi_stage + ew * Cfg::WARP_BYTES;  // slab 0 | slab 1 | (bf16 tile)
-      uint64_t* lbar = ld_bar + 2 * ew;
-      // first output column / first row of chunk `ch` of tile `tile_` for this warp
-      auto coords = [&](int tile_, int ch, int& grp_, int& col_, int& row0_) {
-        grp_ = tile_ / tiles_per_group;
-        const int t_ = tile_ - grp_ * tiles_per_group;
-        const int m_ = t_ / num_n, n_ = t_ - m_ * num_n;
-        row0_ = m_ * 2 * BLOCK_M + rank * BLOCK_M + quad * 32;
-        col_ = Cfg::GLU_R ? n_ * (PAIR_BN / 2) + half * 64 + ch * 32 : n_ * PAIR_BN + half * COLS_PER_WARP + ch * 32;
-      };
-      auto issue_load = [&](int tile_, int ch, int slab) {   // lane 0 only: the bulk groups belong to the issuing thread
-        if (tile_ >= num_tiles) return;
-        int grp_, col_, row0_;
-        coords(tile_, ch, grp_, col_, row0_);
-        mbar_arrive_expect_tx(&lbar[slab], 4096);             // rows beyond M are zero-filled and still counted
-        tma_load_2d(wbase + slab * 4096, grp_ == 0 ? &em.r[0] : &em.r[1], &lbar[slab], col_, row0_);
-      };
-      uint32_t q = 0;   // chunk counter of this warp across tiles: chunk q lives in slab q & 1
-      if (lane == 0) issue_load(pair, 0, 0);
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        int grp, col_first, row_base;
-        coords(tile, 0, grp, col_first, row_base);
-        const int t = tile - grp * tiles_per_group;
-        const int n_blk = t - (t / num_n) * num_n;
-        const GemmGroup& g = p.g[grp];
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after_sync();
-        const uint32_t t_row = tmem_base + acc * PAIR_BN + (static_cast<uint32_t>(quad * 32) << 16) + half * COLS_PER_WARP;
-        // LayerNorm producers: sum x, sum x^2 of this thread's row over the warp's columns (two lanes each, added at the end)
-        [[maybe_unused]] uint64_t rs2 = f2_pack(0.f, 0.f), rq2 = rs2;
-#pragma unroll 1
-        for (int ch = 0; ch < NCH; ++ch, ++q) {
-          const int slab = q & 1;
-          // this chunk's 32 output columns of the thread's row, before the residual: 16 packed pairs
-          uint64_t v[16];
-          if constexpr (!Cfg::GLU_R) {
-            uint32_t a[32];
-            tmem_ld_32x32(t_row + ch * 32, a);
-            tmem_ld_wait();
-            bias_or_ln32<false>(g, n_blk * PAIR_BN + half * COLS_PER_WARP + ch * 32, a, v, 0, 0);
-          } else {
-            // 64 packed accumulator columns (2 x [16 out | 16 gate]) -> 32 outputs
-#pragma unroll
-            for (int sub = 0; sub < 2; ++sub) {
-              uint32_t a[32];
-              tmem_ld_32x32(t_row + ch * 64 + sub * 32, a);
-              tmem_ld_wait();
-              uint64_t w[16];
-              bias_or_ln32<false>(g, n_blk * PAIR_BN + half * COLS_PER_WARP + ch * 64 + sub * 32, a, w, 0, 0);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) v[sub * 8 + i] = f2_mul(w[i], sigmoid_fast2(w[8 + i]));
-            }
-          }
-          // the other slab (and the bf16 tile) were handed to TMA stores by the previous chunk: once those have read
-          // shared memory, prefetch the next chunk's residual into that slab
-          if (lane == 0) {
-            bulk_wait_group_read<0>();
-            if (ch + 1 < NCH) issue_load(tile, ch + 1, slab ^ 1);
-            else issue_load(tile + num_pairs, 0, slab ^ 1);
-          }
-          __syncwarp();
-          mbar_wait(&lbar[slab], (q >> 1) & 1);   // this chunk's residual has landed
-          uint8_t* sl = wbase + slab * 4096;
-          [[maybe_unused]] uint32_t pk[16];
-          const uint64_t alpha2 = f2_pack(p.alpha, p.alpha);
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            ulonglong2* cell = reinterpret_cast<ulonglong2*>(sl + stage_off(lane, k));
-            ulonglong2 x = *cell;                     // residual: 4 consecutive columns as two packed pairs
-            if constexpr (Cfg::GLU_R) {
-              x.x = f2_add(x.x, v[2 * k]);
-              x.y = f2_add(x.y, v[2 * k + 1]);
-            } else {
-              x.x = f2_fma(v[2 * k], alpha2, x.x);    // alpha * (acc + bias) + resid
-              x.y = f2_fma(v[2 * k + 1], alpha2, x.y);
-            }
-            *cell = x;
-            if constexpr (Cfg::LNP) {
-#ifndef SOME_DIAG_LNP_NOSTATS  // timing experiment only (wrong results)
-              rs2 = f2_add(rs2, f2_add(x.x, x.y));
-              rq2 = f2_fma(x.x, x.x, f2_fma(x.y, x.y, rq2));
-#endif
-#ifndef SOME_DIAG_LNP_NOXB
-              pk[2 * k] = pack_bf16x2(x.x);
-              pk[2 * k + 1] = pack_bf16x2(x.y);
-#endif
-            }
-          }
-#ifndef SOME_DIAG_LNP_NOXB
-          if constexpr (Cfg::LNP) {
-            uint8_t* xt = wbase + 8192;   // 32 rows x 64 bf16: chunk ch fills the 16-byte cells 4 (ch & 1) .. + 3 of each row
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              *reinterpret_cast<uint4*>(xt + stage_off(lane, (ch & 1) * 4 + j)) =
-                  make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-          }
-#endif
-          fence_proxy_async_smem();   // generic-proxy writes above -> visible to the TMA (async proxy) reads below
-          __syncwarp();
-          if (lane == 0) {
-            const int col = col_first + ch * 32;
-            tma_store_2d(grp == 0 ? &em.o[0] : &em.o[1], sl, col, row_base);
-#ifndef SOME_DIAG_LNP_NOXB
-            if constexpr (Cfg::LNP) {
-              if (ch & 1) tma_store_2d(grp == 0 ? &em.xb[0] : &em.xb[1], wbase + 8192, col - 32, row_base);
-            }
-#endif
-            bulk_commit_group();
-          }
-        }
-        if constexpr (Cfg::LNP) {
-          float s0, s1, q0, q1;
-          f2_unpack(rs2, s0, s1);
-          f2_unpack(rq2, q0, q1);
-          if (row_base + lane < p.M)
-            reinterpret_cast<float2*>(g.ln_stats)[(size_t)(row_base + lane) * SOME_LN_SLOTS + n_blk * 2 + half] =
-                make_float2(s0 + s1, q0 + q1);
-        }
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&tmem_empty[acc]), 0));
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-      if (lane == 0) bulk_wait_group_read<0>();   // shared memory must outlive the last TMA stores' reads
-    } else {
-      StageRing ring{epi_stage + ew * Cfg::WARP_BYTES, nullptr, 0};
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        const int grp = tile / tiles_per_group;
-        const int t = tile - grp * tiles_per_group;
-        const int m_blk = t / num_n, n_blk = t - m_blk * num_n;
-        const GemmGroup& g = p.g[grp];
-        ring.map = grp == 0 ? &em.o[0] : &em.o[1];
-        const int row_base = m_blk * 2 * BLOCK_M + rank * BLOCK_M + quad * 32;
-        if constexpr (Cfg::LNC) {
-          // The row statistics of the NEXT tile are pulled into L2 now: read at the start of that tile's epilogue they would
-          // cost a DRAM round trip with nothing to overlap it.
-          const int nt = tile + num_pairs;
-          if (nt < num_tiles) {
-            const int ng = nt / tiles_per_group;
-            const int nrow = ((nt - ng * tiles_per_group) / num_n) * 2 * BLOCK_M + rank * BLOCK_M + quad * 32 + lane;
-            if (nrow < p.M)
-              asm volatile("prefetch.global.L2 [%0];" ::"l"(p.g[ng].ln_stats + (size_t)nrow * SOME_LN_SLOTS * 2));
-          }
-        }
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after_sync();
-        const uint32_t t_row = tmem_base + acc * PAIR_BN + (static_cast<uint32_t>(quad * 32) << 16);
-        epilogue_warp_staged<Cfg::BASE, Cfg::LNC>(p, g, row_base, lane, t_row, half * COLS_PER_WARP, n_blk * PAIR_BN, ring);
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&tmem_empty[acc]), 0));
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-      if (lane == 0) bulk_wait_group_read<0>();   // shared memory must outlive the last TMA stores' reads
-    }
-  }
-
-  tc_fence_before_sync();
-  cluster_sync_all();   // no CTA of the pair may free TMEM / exit while its peer still uses it
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc_pair<512>(tmem_base);
   }
 }
 
 template <int EPI>
-static int launch_gemm_pair(const CUtensorMap* maps, const EpiMaps& em, const GemmParams& p, cudaStream_t stream) {
-  auto kern = gemm_pair_kernel<EPI>;
-  static bool configured[kMaxDevices] = {};   // function attributes are per device
-  const int dev_ = device_index();
-  if (!configured[dev_]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PairCfg<EPI>::SMEM);
-    SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(gemm_pair, %d B smem): %s", PairCfg<EPI>::SMEM, cudaGetErrorString(e));
-    configured[dev_] = true;
-  }
-  const int num_m = (p.M + 2 * BLOCK_M - 1) / (2 * BLOCK_M);
-  const int tiles = num_m * (p.N / PAIR_BN) * p.groups;
-  int pairs = num_sms() / 2;
-  if (tiles < pairs) pairs = tiles;
-  launch_pdl(kern, dim3(2 * pairs), dim3(GEMM_THREADS), PairCfg<EPI>::SMEM, stream, maps[0], maps[1], maps[2], maps[3], em, p);
-  return check_launch("some_gemm(pair)");
-}
-
-template <int BLOCK_N, int EPI>
 static int launch_gemm(const CUtensorMap* maps, const GemmParams& p, cudaStream_t stream) {
-  using S = GemmSmem<BLOCK_N>;
-  auto kern = gemm_kernel<BLOCK_N, EPI>;
+  auto kern = gemm_kernel<EPI>;
   static bool configured[kMaxDevices] = {};   // function attributes are per device
   const int dev_ = device_index();
   if (!configured[dev_]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
-    SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(gemm, %d B smem): %s", S::TOTAL, cudaGetErrorString(e));
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM);
+    SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(gemm, %d B smem): %s", GEMM_SMEM, cudaGetErrorString(e));
     configured[dev_] = true;
   }
   const int num_m = (p.M + BLOCK_M - 1) / BLOCK_M;
@@ -871,7 +365,7 @@ static int launch_gemm(const CUtensorMap* maps, const GemmParams& p, cudaStream_
   const int tiles = num_m * num_n * p.groups;
   int grid = num_sms();
   if (tiles < grid) grid = tiles;
-  launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), S::TOTAL, stream, maps[0], maps[1], maps[2], maps[3], p);
+  launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), GEMM_SMEM, stream, maps[0], maps[1], maps[2], maps[3], p);
   return check_launch("some_gemm");
 }
 
@@ -905,57 +399,51 @@ extern "C" int some_gemm(const some_gemm_args* a, cudaStream_t stream) {
   if (ln_consumer)
     SOME_REQUIRE(a->ln_parts >= 1 && a->ln_parts <= SOME_LN_SLOTS, "some_gemm: ln_parts must be in [1, %d] (got %d)",
                  SOME_LN_SLOTS, a->ln_parts);
+  // one slot per 128 accumulator columns (= 128 outputs, or 64 after a GLU)
   if (ln_producer)
-    SOME_REQUIRE((glu_resid ? a->N / 2 : a->N) / 128 <= SOME_LN_SLOTS, "some_gemm: LayerNorm producer output too wide (N=%d)", a->N);
-  const bool use_pair = !head;   // 256 x 256 CTA-pair tiles for every trunk GEMM; heads / input projection stay 1-CTA
+    SOME_REQUIRE(a->N / 128 <= SOME_LN_SLOTS, "some_gemm: LayerNorm producer output too wide (N=%d)", a->N);
   CUtensorMap maps[4];
-  EpiMaps em;
-  memset(&em, 0, sizeof(em));
   for (int g = 0; g < 2; ++g) {
     const int s = g < a->groups ? g : 0;
     SOME_REQUIRE(a->A[s] != nullptr && a->W[s] != nullptr && a->out[s] != nullptr, "some_gemm: null pointer in group %d", s);
     if (make_tmap_bf16_2d(&maps[2 * g], a->A[s], a->M, a->K, a->lda, BLOCK_M)) return -1;
-    if (make_tmap_bf16_2d(&maps[2 * g + 1], a->W[s], a->N, a->K, a->K, use_pair ? 128 : 256)) return -1;
+    if (make_tmap_bf16_2d(&maps[2 * g + 1], a->W[s], a->N, a->K, a->K, BLOCK_N)) return -1;
     p.g[g].bias = a->bias[s];
     p.g[g].out = a->out[s];
     p.g[g].resid = a->resid[s];
     p.g[g].ln_s = a->ln_s[s];
     p.g[g].ln_stats = a->ln_stats[s];
+    p.g[g].out_bf16 = reinterpret_cast<__nv_bfloat16*>(a->out_bf16[s]);
     if (needs_resid) {
       const int out_cols = glu_resid ? a->N / 2 : a->N;
       SOME_REQUIRE(a->resid[s] != nullptr, "some_gemm: epilogue %d needs a residual pointer (group %d)", epi, s);
       SOME_REQUIRE(a->ld_out % 4 == 0 && out_cols <= a->ld_out, "some_gemm: bad ld_out %d for %d output columns", a->ld_out, out_cols);
-      if (make_tmap_2d(&em.r[g], 4, a->resid[s], a->M, out_cols, a->ld_out, 32, 32)) return -1;
-      if (make_tmap_2d(&em.o[g], 4, a->out[s], a->M, out_cols, a->ld_out, 32, 32)) return -1;
-      if (ln_producer) {
+      if (ln_producer)
         SOME_REQUIRE(a->out_bf16[s] != nullptr && a->ln_stats[s] != nullptr,
                      "some_gemm: LayerNorm producer epilogue %d needs out_bf16 and ln_stats (group %d)", epi, s);
-        if (make_tmap_2d(&em.xb[g], 2, a->out_bf16[s], a->M, out_cols, a->ld_out, 32, 64)) return -1;
-      }
     }
-    if (!head && !needs_resid) {   // staged bf16 epilogues: TMA-stored 32-row x 64-column tiles
+    if (!head && !needs_resid) {   // bf16 epilogues: bf16 pairs stored as 32-bit words
       const int out_cols = (epi == SOME_EPI_GLU_BF16 || epi == SOME_EPI_LN_GLU_BF16) ? a->N / 2 : a->N;
       SOME_REQUIRE(a->ld_out % 8 == 0 && out_cols <= a->ld_out, "some_gemm: bad ld_out %d for %d bf16 output columns", a->ld_out, out_cols);
-      if (make_tmap_2d(&em.o[g], 2, a->out[s], a->M, out_cols, a->ld_out, 32, 64)) return -1;
     }
     if (ln_consumer)
       SOME_REQUIRE(a->ln_s[s] != nullptr && a->ln_stats[s] != nullptr && a->bias[s] != nullptr,
                    "some_gemm: LayerNorm consumer epilogue %d needs bias, ln_s and ln_stats (group %d)", epi, s);
   }
   switch (epi) {
-    case SOME_EPI_STORE_BF16: return launch_gemm_pair<SOME_EPI_STORE_BF16>(maps, em, p, stream);
-    case SOME_EPI_SILU_BF16: return launch_gemm_pair<SOME_EPI_SILU_BF16>(maps, em, p, stream);
-    case SOME_EPI_GLU_BF16: return launch_gemm_pair<SOME_EPI_GLU_BF16>(maps, em, p, stream);
-    case SOME_EPI_RESID_F32: return launch_gemm_pair<SOME_EPI_RESID_F32>(maps, em, p, stream);
-    case SOME_EPI_GLU_RESID_F32: return launch_gemm_pair<SOME_EPI_GLU_RESID_F32>(maps, em, p, stream);
-    case SOME_EPI_LN_STORE_BF16: return launch_gemm_pair<SOME_EPI_LN_STORE_BF16>(maps, em, p, stream);
-    case SOME_EPI_LN_SILU_BF16: return launch_gemm_pair<SOME_EPI_LN_SILU_BF16>(maps, em, p, stream);
-    case SOME_EPI_LN_GLU_BF16: return launch_gemm_pair<SOME_EPI_LN_GLU_BF16>(maps, em, p, stream);
-    case SOME_EPI_RESID_F32_LN: return launch_gemm_pair<SOME_EPI_RESID_F32_LN>(maps, em, p, stream);
-    case SOME_EPI_GLU_RESID_F32_LN: return launch_gemm_pair<SOME_EPI_GLU_RESID_F32_LN>(maps, em, p, stream);
-    case SOME_EPI_BIAS_F32: return launch_gemm<256, SOME_EPI_BIAS_F32>(maps, p, stream);
-    case SOME_EPI_SIGMOID_F32: return launch_gemm<256, SOME_EPI_SIGMOID_F32>(maps, p, stream);
-    case SOME_EPI_SOFTMAX_F32: return launch_gemm<256, SOME_EPI_SOFTMAX_F32>(maps, p, stream);
+    case SOME_EPI_STORE_BF16: return launch_gemm<SOME_EPI_STORE_BF16>(maps, p, stream);
+    case SOME_EPI_SILU_BF16: return launch_gemm<SOME_EPI_SILU_BF16>(maps, p, stream);
+    case SOME_EPI_GLU_BF16: return launch_gemm<SOME_EPI_GLU_BF16>(maps, p, stream);
+    case SOME_EPI_RESID_F32: return launch_gemm<SOME_EPI_RESID_F32>(maps, p, stream);
+    case SOME_EPI_GLU_RESID_F32: return launch_gemm<SOME_EPI_GLU_RESID_F32>(maps, p, stream);
+    case SOME_EPI_LN_STORE_BF16: return launch_gemm<SOME_EPI_LN_STORE_BF16>(maps, p, stream);
+    case SOME_EPI_LN_SILU_BF16: return launch_gemm<SOME_EPI_LN_SILU_BF16>(maps, p, stream);
+    case SOME_EPI_LN_GLU_BF16: return launch_gemm<SOME_EPI_LN_GLU_BF16>(maps, p, stream);
+    case SOME_EPI_RESID_F32_LN: return launch_gemm<SOME_EPI_RESID_F32_LN>(maps, p, stream);
+    case SOME_EPI_GLU_RESID_F32_LN: return launch_gemm<SOME_EPI_GLU_RESID_F32_LN>(maps, p, stream);
+    case SOME_EPI_BIAS_F32: return launch_gemm<SOME_EPI_BIAS_F32>(maps, p, stream);
+    case SOME_EPI_SIGMOID_F32: return launch_gemm<SOME_EPI_SIGMOID_F32>(maps, p, stream);
+    case SOME_EPI_SOFTMAX_F32: return launch_gemm<SOME_EPI_SOFTMAX_F32>(maps, p, stream);
     default: SOME_REQUIRE(false, "some_gemm: unknown epilogue %d", epi);
   }
   return -1;

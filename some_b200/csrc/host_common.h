@@ -29,7 +29,7 @@ int device_index();
 int num_sms();
 
 // Programmatic dependent launch (some_set_pdl): a kernel launched through launch_pdl() may become resident while its
-// predecessor in the stream is still running; it executes its prologue (barrier init, TMEM allocation, tensor-map prefetch) and
+// predecessor in the stream is still running; it executes its prologue (barrier init, tensor-map prefetch) and
 // blocks in griddep_wait() -- which every such kernel calls before its first access to activations -- until the predecessor has
 // completed and flushed.  Pays on small batches, where a step is ~70 dependent launches of a few microseconds each.
 bool pdl_enabled();

@@ -15,7 +15,7 @@
 // No CTA barrier after the table load; a CTA is just MEL_WARPS independent warps sharing the 19 KB of tables.
 // Algorithmic traffic: 512 x 4 B in + 80 x 4 B out per frame (2368 B); ~60 kFLOP per frame keep it issue-bound.
 #include "host_common.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 #include "../../include/some_b200.h"
 

@@ -5,7 +5,7 @@
 //                                                                 base_conv.py:66-68
 // Roofline: HBM.  LN reads 2 KB and writes 1-3 KB per row; dwconv reads/writes 1 KB + 1 KB per row.
 #include "host_common.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 #include "../../include/some_b200.h"
 
@@ -145,27 +145,39 @@ __global__ void __launch_bounds__(256) row_stats_kernel(const RowStatsParams p) 
   }
 }
 
-// K-colmeans (calibration only, load time): column means of a GEMM's (effective) A operand.  One thread per column, rows
-// strided over blockIdx.y, partial sums combined with atomics into a zeroed buffer; the caller divides by M.
-__global__ void __launch_bounds__(128)
+// K-colmeans (calibration only, load time): column means of a GEMM's (effective) A operand.  A block owns 32 columns; its 8
+// warps take every 8th row and their partial sums are added in a fixed order, so the result (and with it the bias
+// correction of every layer) is the same bit for bit on every run.
+constexpr int CM_COLS = 32, CM_WARPS = 8;
+__global__ void __launch_bounds__(CM_COLS * CM_WARPS)
 col_means_kernel(const __nv_bfloat16* __restrict__ a, int M, int K, int lda, const float* __restrict__ stats, int parts,
                  float inv_m, float* __restrict__ out) {
-  const int k = blockIdx.x * 128 + threadIdx.x;
-  if (k >= K) return;
+  __shared__ float part[CM_WARPS][CM_COLS];
+  const int c = threadIdx.x % CM_COLS, w = threadIdx.x / CM_COLS;
+  const int k = blockIdx.x * CM_COLS + c;
   float acc = 0.f;
-  for (int row = blockIdx.y; row < M; row += gridDim.y) {
-    float v = __bfloat162float(a[(size_t)row * lda + k]);
-    if (stats != nullptr) {
-      float s = 0.f, q = 0.f;
-      const float2* st = reinterpret_cast<const float2*>(stats) + (size_t)row * SOME_LN_SLOTS;
-      for (int i = 0; i < parts; ++i) s += st[i].x, q += st[i].y;
-      const float mean = s / K;
-      const float var = fmaxf(q / K - mean * mean, 0.f);
-      v = (v - mean) * rsqrtf(var + 1e-5f);
+  if (k < K) {
+    for (int row = w; row < M; row += CM_WARPS) {
+      float v = __bfloat162float(a[(size_t)row * lda + k]);
+      if (stats != nullptr) {
+        float s = 0.f, q = 0.f;
+        const float2* st = reinterpret_cast<const float2*>(stats) + (size_t)row * SOME_LN_SLOTS;
+        for (int i = 0; i < parts; ++i) s += st[i].x, q += st[i].y;
+        const float mean = s / K;
+        const float var = fmaxf(q / K - mean * mean, 0.f);
+        v = (v - mean) * rsqrtf(var + 1e-5f);
+      }
+      acc += v;
     }
-    acc += v;
   }
-  atomicAdd(out + k, acc * inv_m);
+  part[w][c] = acc;
+  __syncthreads();
+  if (w == 0 && k < K) {
+    float sum = 0.f;
+#pragma unroll
+    for (int i = 0; i < CM_WARPS; ++i) sum += part[i][c];
+    out[k] = sum * inv_m;
+  }
 }
 
 __global__ void __launch_bounds__(256)
@@ -196,7 +208,7 @@ bound_head_kernel(const float* __restrict__ x, const float* __restrict__ gamma, 
 // the clip read as zero).  Persistent CTAs: a CTA keeps ONE channel block for its whole life, so the 31 x 2 BN-folded
 // taps of each thread are loaded into registers once, and it walks over frame tiles with a cp.async double buffer
 // (the (128 + 30) x 64 bf16 window of the next tile streams in while the current one is computed).  Each thread owns a
-// channel pair and 16 consecutive frames: 16 packed-f32x2 accumulators, the 46 input rows stream through once
+// channel pair and 16 consecutive frames: 16 fp32-pair accumulators, the 46 input rows stream through once
 // (row-major accumulation, fully unrolled, no per-tap predicates).
 constexpr int DW_T = 128;     // frames per tile
 constexpr int DW_C = 64;      // channels per CTA
@@ -247,7 +259,7 @@ __global__ void __launch_bounds__(256) dwconv_kernel(const DwParams p) {
     }
   };
 
-  // Packed fp32x2 FMAs (sm_100 FFMA2): {a[c], a[c+1]} += {w[c], w[c+1]} * {x[c], x[c+1]} in ONE instruction per lane.
+  // fp32 pairs: {a[c], a[c+1]} += {w[c], w[c+1]} * {x[c], x[c+1]}
   uint64_t w[SOME_CONV_K];
 #pragma unroll
   for (int k = 0; k < SOME_CONV_K; ++k) w[k] = __ldg(reinterpret_cast<const unsigned long long*>(p.w[grp] + k * D + c));
@@ -273,12 +285,12 @@ __global__ void __launch_bounds__(256) dwconv_kernel(const DwParams p) {
 #pragma unroll
       for (int r = 0; r < DW_FR + SOME_CONV_K - 1; ++r) {
         const uint32_t xb = *reinterpret_cast<const uint32_t*>(tb + (f0 + r) * DW_C + 2 * lane);  // bf16x2
-        // bf16 -> f32 is a 16-bit shift: {lo, hi} as packed f32x2
+        // bf16 -> f32 is a 16-bit shift: {lo, hi} as an fp32 pair
         const uint64_t xv = (static_cast<uint64_t>(xb & 0xffff0000u) << 32) | static_cast<uint64_t>(xb << 16);
 #pragma unroll
         for (int f = 0; f < DW_FR; ++f) {
           const int k = r - f;  // tap index: output frame f reads tile rows f .. f + 30
-          if (k >= 0 && k < SOME_CONV_K) asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(a[f]) : "l"(w[k]), "l"(xv));
+          if (k >= 0 && k < SOME_CONV_K) a[f] = f2_fma(w[k], xv, a[f]);
         }
       }
 #pragma unroll
@@ -338,10 +350,7 @@ extern "C" int some_col_means(const uint16_t* a, int M, int K, int lda, const fl
                               cudaStream_t stream) {
   SOME_REQUIRE(a != nullptr && out != nullptr && M > 0 && K > 0 && K <= SOME_CALIB_K, "some_col_means: bad arguments");
   SOME_REQUIRE(ln_stats == nullptr || (ln_parts >= 1 && ln_parts <= SOME_LN_SLOTS), "some_col_means: bad ln_parts");
-  cudaError_t e = cudaMemsetAsync(out, 0, sizeof(float) * K, stream);
-  SOME_REQUIRE(e == cudaSuccess, "some_col_means: %s", cudaGetErrorString(e));
-  dim3 grid((K + 127) / 128, M < 64 ? M : 64);
-  col_means_kernel<<<grid, 128, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(a), M, K, lda, ln_stats, ln_parts,
+  col_means_kernel<<<(K + CM_COLS - 1) / CM_COLS, CM_COLS * CM_WARPS, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(a), M, K, lda, ln_stats, ln_parts,
                                              1.0f / M, out);
   return check_launch("some_col_means");
 }

@@ -1,4 +1,4 @@
-"""Batched SOME inference engine: packs clips var-len, launches the sm_100a kernels of
+"""Batched SOME inference engine: packs clips var-len, launches the sm_90a kernels of
 libsome_b200.so in order on the current CUDA stream and unpacks the decoded notes.
 
 Equivalent to running the reference's batch-1 loop (inference/base_infer.py:46-53) once per clip:
@@ -9,8 +9,7 @@ The trunk is sequenced natively (csrc/forward.cu: some_forward); per conform_blo
     GEMM(to_out)+x -> LN3 -> GEMM(pointwise_conv1)+GLU -> dwconv+BN+SiLU -> GEMM(pointwise_conv2)+x ->
     LN4 -> GEMM(ffn2.ln1)+SiLU -> GEMM(ffn2.ln2)*0.5+x -> LN5
 SOME_B200_LN_FOLD=1 selects the variant with norm1..norm4 folded into the GEMMs around them (11 instead of 15 launches per
-block; measured 0.9 ms SLOWER per 64 x 30 s step on B200 because the K = 512 consumer GEMMs are epilogue-bound:
-profiles/r02_ln_fold.md), kept as a validated option.
+block), kept as a validated option; stand-alone LayerNorm launches are the default.
 The residual stream x is fp32 [M, 512]; GEMM operands are bf16; accumulation is fp32.
 """
 from __future__ import annotations
@@ -76,7 +75,7 @@ class Engine:
         self.config = config
         self.device = torch.device(device)
         if self.device.type != 'cuda':
-            raise _lib.SomeB200Error('some_b200 runs on CUDA devices only (sm_100a); there is no CPU path')
+            raise _lib.SomeB200Error('some_b200 runs on CUDA devices only (sm_90a); there is no CPU path')
         self.quantized = False
         self._state_dict = state_dict        # fp32 masters for the validation path (infer_accurate), built lazily
         self._f32 = None

@@ -1,11 +1,11 @@
-"""B200-native drop-in for the reference's ``inference`` plugin package
-(/root/reference/inference/{base_infer,me_infer,me_quant_infer}.py, registry __init__.py:5-8).
+"""H100-native drop-in for the reference's ``inference`` plugin package
+(the reference's inference/{base_infer,me_infer,me_quant_infer}.py, registry __init__.py:5-8).
 
 Same class names, constructor signature, attributes and method contracts, so that infer.py:24-37,
 batch_infer.py:26-34,54 and webui.py:28-54 run unchanged when this repo precedes the reference on
 ``sys.path`` (the top-level ``inference`` package of this repo re-exports these classes).
 
-All compute goes through libsome_b200.so (hand-written sm_100a kernels).  ``infer()`` runs the whole
+All compute goes through libsome_b200.so (hand-written sm_90a kernels).  ``infer()`` runs the whole
 list of clips as ONE var-len batch (mel -> trunk -> decode) instead of the reference's serial
 batch-1 loop; the per-clip methods ``preprocess / forward_model / postprocess`` keep the reference's
 tensor contracts and also run on the GPU kernels.  There is no CPU fallback.
@@ -35,7 +35,7 @@ class BaseInference:
         self.device = device
         if torch.device(device).type != 'cuda':
             raise _lib.SomeB200Error(
-                f"some_b200 plugin needs a CUDA (sm_100a) device, got device='{device}'. "
+                f"some_b200 plugin needs a CUDA (sm_90a) device, got device='{device}'. "
                 "It has no CPU path; use the reference implementation on CPU.")
         self.timestep = self.config['hop_size'] / self.config['audio_sample_rate']   # base_infer.py:20
         self._lock = threading.Lock()     # webui.py:104 runs up to 10 concurrent callers on one instance

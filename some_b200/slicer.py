@@ -1,4 +1,4 @@
-"""Silence slicer in front of the path (SURVEY.md §8f-1): the B200 counterpart of utils/slicer2.py.
+"""Silence slicer in front of the path (SURVEY.md §8f-1): the GPU counterpart of utils/slicer2.py.
 
 The reference computes the short-time RMS with numpy (slicer2.py:5-38: ~53 M multiply-adds and a 200 MB temporary for a
 5-minute recording) and then walks the RMS list frame by frame in Python (:84-127).  Here

@@ -1,4 +1,4 @@
-"""Drop-in for the reference's ``modules.rmvpe.spec.MelSpectrogram`` (modules/rmvpe/spec.py:7-72) on the sm_100a mel kernels:
+"""Drop-in for the reference's ``modules.rmvpe.spec.MelSpectrogram`` (modules/rmvpe/spec.py:7-72) on the sm_90a mel kernels:
 same constructor, same ``forward(audio, keyshift=0, speed=1, center=True)`` contract (float32 ``[B, n_mels, T]``), including
 the key-shift / speed path the binarizer uses for pitch augmentation (preprocessing/me_binarizer.py:235-247; SURVEY.md §8f-4).
 
@@ -50,7 +50,7 @@ class MelSpectrogram(torch.nn.Module):
     @torch.no_grad()
     def forward(self, audio: torch.Tensor, keyshift=0, speed=1, center=True) -> torch.Tensor:
         if not audio.is_cuda:
-            raise _lib.SomeB200Error('some_b200.spec.MelSpectrogram runs on CUDA tensors only (sm_100a kernels, no CPU path)')
+            raise _lib.SomeB200Error('some_b200.spec.MelSpectrogram runs on CUDA tensors only (sm_90a kernels, no CPU path)')
         lib = _lib.load()
         squeeze = audio.dim() == 1
         x = (audio.unsqueeze(0) if squeeze else audio).to(torch.float32).contiguous()

@@ -1,5 +1,5 @@
 """Host-side packing of a reference checkpoint (``state_dict`` of
-``modules.model.Gmidi_conform.midi_conforms``) into the device layouts the sm_100a kernels consume:
+``modules.model.Gmidi_conform.midi_conforms``) into the device layouts the sm_90a kernels consume:
 
 * every nn.Linear / 1x1 Conv1d weight -> bf16 [N, K] (K-major, exactly nn.Linear's own layout);
 * to_q | to_kv concatenated to one [1536, 512] matrix (base_attention.py:31-32: q, then k, then v);

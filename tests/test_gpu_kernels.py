@@ -1,4 +1,4 @@
-"""GPU parity tests of the individual sm_100a kernels, each called THROUGH THE C ABI
+"""GPU parity tests of the individual sm_90a kernels, each called THROUGH THE C ABI
 (libsome_b200.so via ctypes) and compared with a plain fp32 torch restatement of the same op on the
 same (bf16-rounded) inputs.  Tolerances are written at each comparison."""
 import ctypes as C
@@ -228,7 +228,30 @@ def test_row_stats(lib):
         torch.testing.assert_close(st[i][:, 0, 1], (x[i] * x[i]).sum(1), atol=1e-2, rtol=1e-5)
 
 
-@pytest.mark.parametrize('n,epi', [(128, 'sigmoid'), (129, 'softmax'), (128, 'logits'), (129, 'logits')])
+@pytest.mark.parametrize('normalised', [False, True])
+def test_col_means_match_and_repeat_bit_for_bit(lib, normalised):
+    """The load-time bias correction is built from these means: they must not depend on the run (fixed summation order)."""
+    torch.manual_seed(41)
+    m, k = 3001, 2048
+    a = (torch.randn(m, k, device=DEV) * 1.5 + 0.2).to(torch.bfloat16)
+    af = a.float()
+    st = torch.zeros(m, _lib.LN_SLOTS, 2, device=DEV)
+    st[:, 0, 0], st[:, 0, 1] = af.sum(1), (af * af).sum(1)
+    outs = []
+    for _ in range(3):
+        out = torch.full((k,), float('nan'), device=DEV)
+        _lib.check(lib.some_col_means(a.data_ptr(), m, k, k, st.data_ptr() if normalised else None, 1, out.data_ptr(),
+                                      stream()), 'some_col_means')
+        outs.append(out)
+    torch.cuda.synchronize()
+    assert all(torch.equal(outs[0], o) for o in outs[1:])
+    if normalised:
+        mean = af.mean(1, keepdim=True)
+        af = (af - mean) * torch.rsqrt((af * af).mean(1, keepdim=True) - mean * mean + 1e-5)
+    torch.testing.assert_close(outs[0], af.mean(0), atol=2e-5, rtol=1e-4)
+
+
+@pytest.mark.parametrize('n,epi',[(128, 'sigmoid'), (129, 'softmax'), (128, 'logits'), (129, 'logits')])
 def test_gemm_heads(lib, n, epi):
     torch.manual_seed(4)
     m, k = 333, 512
@@ -327,7 +350,7 @@ def test_attention_varlen(lib, frames, impl):
 
 def test_attention_growing_max_forces_rescale(lib):
     """Scores whose row maximum jumps by far more than 2^8 from one key tile to the next: exercises the lazy
-    O-rescale path of the tcgen05 kernel on every tile (a race there shows up as wrong rows)."""
+    O-rescale path of the attention kernel on every tile (a race there shows up as wrong rows)."""
     torch.manual_seed(8)
     frames = [1500, 333]
     cu = _cu(frames)

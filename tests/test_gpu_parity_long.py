@@ -16,8 +16,7 @@ from oracle.metrics import note_agreement
 pytestmark = pytest.mark.gpu
 
 CASES = {   # cfg: (batch clips, min frame agreement, min exact-boundary agreement) — thresholds = measured - margin
-    # measured on B200 (round 2, with the load-time bias correction): two_head 0.95-0.99 / 0.58-0.93, quant 0.995-1.0 / 0.51-0.93,
-    # midi_conformer 0.95-0.99 / 0.73-0.81 (without the correction: 0.89 / 0.40-0.49 on two_head).  With seeded random weights
+    # thresholds sit below the agreement measured with the load-time bias correction on.  With seeded random weights
     # `bounds` hovers around 0.5 on every frame (a boundary every 2-3 frames), the worst case for cumsum().round(): a residual
     # mean error of +-1e-4 (input dependent) is a drift of up to 0.3 over 2584 frames and moves boundaries by one frame.
     # The fp32 validation mode decodes exactly the oracle's notes (tests/test_gpu_accurate.py).

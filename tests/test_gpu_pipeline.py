@@ -116,7 +116,7 @@ def test_ln_fold_matches_standalone_layernorm(tmp_path):
         assert launches[fold] == eng.trunk_launches
         out[fold] = (ws.probs[:m].clone(), ws.bounds[:m].clone())
         assert not torch.isnan(out[fold][0]).any() and not torch.isnan(out[fold][1]).any()
-    eng.set_ln_fold(False)                     # the product default (the folded variant measured slower: profiles/r02_ln_fold.md)
+    eng.set_ln_fold(False)                     # the product default
     lay = eng.w.lay
     assert launches[True] == 15 + 12 * lay and launches[False] == 18 + 16 * lay
     # two bf16 evaluations of the same fp32 function: each is within ~2.5e-3 of it (tests/test_gpu_parity_long.py)
