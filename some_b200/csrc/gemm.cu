@@ -9,8 +9,11 @@
 //                   gives its registers to the consumers (setmaxnreg)
 //   warpgroups 1-2  consumers: rows [64 c, 64 c + 64) of the tile, wgmma m64n256k16 from shared memory into 128 fp32
 //                   registers per thread, one k-block in flight while the previous one's stage is released; then the fused
-//                   epilogue (bias / SiLU / GLU / residual / LayerNorm fold / sigmoid / softmax) straight from the
-//                   accumulator registers: each quad of lanes stores 8 consecutive columns of a row (32 B in fp32, 16 B in bf16).
+//                   epilogue (bias / SiLU / GLU / residual / LayerNorm fold / sigmoid / softmax).
+// Epilogue stores: the bf16 and residual epilogues leave through shared memory.  Each consumer warpgroup fills slabs of
+// 64 rows x 128 B (64 bf16 or 32 fp32 columns, 128-byte swizzle) and one thread sends each slab with a TMA store; the
+// residual epilogues first TMA-load the residual slab (the next slab loads while this one is worked on) and add into it
+// in place.  The head epilogues (ragged N) store straight from the accumulator registers.
 // Up to two independent problems (the "midi" and "bound" streams: same shapes, different weights) run in one launch
 // (groups = 2).
 #include "host_common.h"
@@ -26,22 +29,25 @@ constexpr int BLOCK_M = 128;
 constexpr int BLOCK_N = 256;
 constexpr int BLOCK_K = 64;
 constexpr int WGMMA_K = 16;
-constexpr int STAGES = 4;
 constexpr int GEMM_THREADS = 384;
 constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;   // 16 KB
 constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;   // 32 KB
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int GEMM_SMEM = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-static_assert(GEMM_SMEM <= 232448, "gemm_kernel: shared memory over the 227 KB per-CTA limit");
 constexpr int ACC = BLOCK_N / 2;   // accumulator registers per consumer thread
+constexpr int SLAB_ROWS = 64;      // epilogue slab: the rows of one consumer warpgroup ...
+constexpr int SLAB_BYTES = SLAB_ROWS * 128;   // ... by 128 B (one 128-byte swizzle row)
 
 struct GemmGroup {
   const float* bias;   // [N] in packed-column order, or nullptr
-  void* out;           // bf16 or f32, row pitch ld_out elements
-  const float* resid;  // f32 [M, ld_out] or nullptr (may alias out)
+  void* out;           // head epilogues: f32, row pitch ld_out elements (the others store through GemmMaps::out)
   const float* ln_s;   // LayerNorm-folded consumers: column sums of W' [N]
   float* ln_stats;     // f32 [M][SOME_LN_SLOTS][2] partial (sum x, sum x^2): written by producers, read by consumers
-  __nv_bfloat16* out_bf16;   // LayerNorm producers: bf16 copy of out, row pitch ld_out
+};
+
+// Tensor maps of one group.  resid / out: f32 boxes of 64 x 32 (residual epilogues) or bf16 boxes of 64 x 64 (out of
+// the bf16 epilogues); out_bf16: bf16 64 x 64 (LayerNorm producers).  Maps an epilogue does not use are zero.
+struct GemmMaps {
+  CUtensorMap a, b, resid, out, out_bf16;
 };
 
 struct GemmParams {
@@ -62,6 +68,20 @@ struct EpiCfg {
   static constexpr int BASE = LNC ? EPI - SOME_EPI_LN_STORE_BF16
                               : EPI == SOME_EPI_RESID_F32_LN ? SOME_EPI_RESID_F32
                               : EPI == SOME_EPI_GLU_RESID_F32_LN ? SOME_EPI_GLU_RESID_F32 : EPI;
+  static constexpr bool STAGED = BASE <= SOME_EPI_GLU_RESID_F32;   // everything but the heads goes through slabs
+  static constexpr bool RESID = BASE == SOME_EPI_RESID_F32 || BASE == SOME_EPI_GLU_RESID_F32;
+  static constexpr bool GLU = BASE == SOME_EPI_GLU_BF16 || BASE == SOME_EPI_GLU_RESID_F32;
+  static constexpr int ELEM = RESID ? 4 : 2;            // bytes per output element in the slab
+  static constexpr int SLAB_COLS = 128 / ELEM;
+  static constexpr int SLABS = STAGED ? (GLU ? BLOCK_N / 2 : BLOCK_N) / SLAB_COLS : 0;   // per warpgroup and tile
+  // Slab buffers per consumer warpgroup: two, so that one is filled (or loaded) while the other is stored.  The
+  // LayerNorm producers add two bf16 slabs for the copy of out; they do not fit beside a 4-stage ring, and 64-byte
+  // (32-column) bf16 slabs would need a second swizzle mode in the maps and the fragment mapping, so those two epilogues
+  // run a 3-stage ring instead (ln_fold only; K = 512 gives 8 k-blocks per tile).
+  static constexpr int SLAB_BUFS = !STAGED ? 0 : LNP ? 4 : 2;
+  static constexpr int STAGES = LNP ? 3 : 4;
+  static constexpr int SMEM = STAGES * STAGE_BYTES + 2 * SLAB_BUFS * SLAB_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(SMEM <= 232448, "gemm_kernel: shared memory over the 227 KB per-CTA limit");
 };
 
 // Row statistics of the LayerNorm input from the producers' partial sums (nn.LayerNorm: biased variance, eps 1e-5).
@@ -90,16 +110,135 @@ __device__ __forceinline__ float quad_max(float v) {
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
 
-// Epilogue of one consumer thread: acc holds rows row0 and row0 + 8, columns col_tile + 8 j + 2 q + {0, 1} (j < 32).
+// Slab state of one consumer warpgroup: its SLAB_BUFS buffers (0-1 staging, 2-3 the LayerNorm producers' bf16 copy),
+// the mbarriers of the residual loads into buffers 0-1, the number of slabs it has used so far (buffer = count & 1,
+// barrier parity = (count >> 1) & 1), and whether this thread is the one that issues the warpgroup's TMA operations
+// (always the same thread: bulk groups belong to the thread that commits them).
+struct Slabs {
+  uint8_t* buf;
+  uint64_t* bar;
+  uint32_t count;
+  bool leader;
+};
+
+// Shared address of this thread's columns 2 q, 2 q + 1 in slab row r, in the 128-byte swizzle of the tensor maps (the
+// 16-byte chunk index is XORed with r % 8).  Column 8 u + 2 q of the row is then at slab_row(...) ^ (8 u * ELEM): the
+// constant only flips chunk bits 4-6 (8 u * ELEM < 128), so one base per slab and row serves every column group, and
+// the row r + 8 is at + 1024 (same r % 8).  The 8 rows of a warp (r % 8 = lane / 4) put one 8-column group into 8
+// different chunks: a warp's bf16 stores hit 32 distinct banks, its fp32 pairs (256 B) each bank twice.
+template <int ELEM>
+__device__ __forceinline__ uint32_t slab_row(const uint8_t* slab, int r, int q) {
+  constexpr int Q = 2 * ELEM;   // bytes per column pair
+  return smem_u32(slab) + r * 128 + ((((Q * q) >> 4) ^ (r & 7)) << 4) + ((Q * q) & 15);
+}
+
+// Sends a residual slab's load (buffer count & 1).  Called by the leader only.
+__device__ __forceinline__ void slab_load(const GemmMaps& tm, const Slabs& sl, uint32_t count, int col, int row) {
+  uint64_t* bar = &sl.bar[count & 1];
+  mbar_arrive_expect_tx(bar, SLAB_BYTES);   // rows past M are zero-filled and still counted
+  tma_load_2d(sl.buf + (count & 1) * SLAB_BYTES, &tm.resid, bar, col, row);
+}
+
+// Staged epilogue of one consumer warpgroup (64 rows x 256 accumulator columns of the tile, starting at row_base):
+// output columns are cut into Cfg::SLABS slabs of SLAB_COLS.  Per slab: (residual: wait for its TMA load, start the
+// next one), each thread writes its values into the slab (in place: alpha * (acc + bias) + resid), fence.proxy.async,
+// named barrier over the warpgroup, one TMA store.  Rows past M are clipped by the store.  The residual slab is read and
+// written by this warpgroup only, and its load completes before its store is issued, so resid may alias out.
+template <int EPI>
+__device__ __forceinline__ void epilogue_staged(const GemmParams& p, const GemmGroup& g, const GemmMaps& tm,
+                                                float (&acc)[ACC], Slabs& sl, int row_base, int lrow, int col_tile,
+                                                int q, int cw) {
+  using Cfg = EpiCfg<EPI>;
+  constexpr int BASE = Cfg::BASE;
+  constexpr int SC = Cfg::SLAB_COLS;
+  const int col_out = Cfg::GLU ? col_tile / 2 : col_tile;   // first output column of the tile
+  [[maybe_unused]] float st_s[2] = {}, st_q[2] = {};   // [row half]: (sum x, sum x^2) of the current ln_stats slot
+#pragma unroll
+  for (int c = 0; c < Cfg::SLABS; ++c) {
+    const uint32_t count = sl.count + c;
+    uint8_t* buf = sl.buf + (count & 1) * SLAB_BYTES;
+    [[maybe_unused]] uint8_t* buf16 = sl.buf + (2 + ((count >> 1) & 1)) * SLAB_BYTES;   // LN producers: 2 slabs per copy
+    if constexpr (Cfg::RESID) {
+      mbar_wait(&sl.bar[count & 1], (count >> 1) & 1);
+      if (sl.leader) {
+        bulk_wait_group_read<0>();   // the previous slab's store has read the other buffer
+        if (c + 1 < Cfg::SLABS) slab_load(tm, sl, count + 1, col_out + (c + 1) * SC, row_base);
+      }
+    }
+    const uint32_t row = slab_row<Cfg::ELEM>(buf, lrow, q);
+    [[maybe_unused]] const uint32_t row16 = slab_row<2>(buf16, lrow, q);
+#pragma unroll
+    for (int u = 0; u < SC / 8; ++u) {
+      // 8-column output group og of the warpgroup -> accumulator group j (GLU: "out" half of packed group og / 2)
+      const int og = c * (SC / 8) + u;
+      const int j = Cfg::GLU ? 4 * (og >> 1) + (og & 1) : og;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t addr = (row ^ (8 * u * Cfg::ELEM)) + 1024 * h;
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if constexpr (BASE == SOME_EPI_SILU_BF16) v0 = silu_fast(v0), v1 = silu_fast(v1);
+        if constexpr (Cfg::GLU) {
+          v0 *= sigmoid_fast(acc[4 * (j + 2) + 2 * h]);
+          v1 *= sigmoid_fast(acc[4 * (j + 2) + 2 * h + 1]);
+        }
+        if constexpr (Cfg::RESID) {
+          const float2 rs = lds_f2(addr);
+          float2 x;
+          if constexpr (Cfg::GLU) x = make_float2(rs.x + v0, rs.y + v1);
+          else x = make_float2(fmaf(v0, p.alpha, rs.x), fmaf(v1, p.alpha, rs.y));   // alpha * (acc + bias) + resid
+          sts_f2(addr, x);
+          if constexpr (Cfg::LNP) {
+            st_s[h] += x.x + x.y;
+            st_q[h] = fmaf(x.x, x.x, fmaf(x.y, x.y, st_q[h]));
+            sts_u32((row16 ^ (2 * ((c & 1) * SC + 8 * u))) + 1024 * h, pack_bf16x2(x.x, x.y));
+          }
+        } else {
+          sts_u32(addr, pack_bf16x2(v0, v1));
+        }
+      }
+    }
+    fence_proxy_async_smem();   // this thread's slab writes -> visible to the TMA store
+    if constexpr (!Cfg::RESID)
+      if (sl.leader) bulk_wait_group_read<0>();   // the previous slab's store has read the buffer the next slab fills
+    named_bar_sync(1 + cw, 128);
+    if (sl.leader) {
+      tma_store_2d(&tm.out, buf, col_out + c * SC, row_base);
+      if constexpr (Cfg::LNP)
+        if (c & 1) tma_store_2d(&tm.out_bf16, buf16, col_out + (c - 1) * SC, row_base);
+      bulk_commit_group();
+    }
+    if constexpr (Cfg::LNP) {
+      // slot j / 16 of the tile (128 accumulator columns) is complete after its last slab
+      constexpr int G8 = SC / 8;
+      const int slot = (Cfg::GLU ? 4 * ((c * G8) >> 1) : c * G8) >> 4;
+      const int next = (Cfg::GLU ? 4 * (((c + 1) * G8) >> 1) : (c + 1) * G8) >> 4;
+      if (c + 1 == Cfg::SLABS || next != slot) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = row_base + lrow + 8 * h;
+          const float sum = quad_sum(st_s[h]), sq = quad_sum(st_q[h]);
+          if (q == 0 && row < p.M)
+            reinterpret_cast<float2*>(g.ln_stats)[(size_t)row * SOME_LN_SLOTS + (col_tile >> 7) + slot] = make_float2(sum, sq);
+          st_s[h] = st_q[h] = 0.f;
+        }
+      }
+    }
+  }
+  sl.count += Cfg::SLABS;
+}
+
+// Epilogue of one consumer thread: acc holds rows row0 and row0 + 8, columns col_tile + 8 j + 2 q + {0, 1} (j < 32),
+// where row0 = row_base + lrow.
 // GLU: packed columns come in 32-column groups [16 "out" | 16 "gate"], so the gate of acc[4 j + i] is acc[4 (j + 2) + i]
 // (j % 4 < 2) and output channel (col_tile + 32 G) / 2 + 8 jj + 2 q + e belongs to group G, j = 4 G + jj.
 // LayerNorm producers: slot col / 128 of ln_stats gets (sum x, sum x^2) of the row over those 128 accumulator columns.
 template <int EPI>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const GemmGroup& g, float (&acc)[ACC], int row0,
-                                              int col_tile, int q) {
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const GemmGroup& g, const GemmMaps& tm,
+                                              float (&acc)[ACC], Slabs& sl, int row_base, int lrow, int col_tile, int q,
+                                              int cw) {
   using Cfg = EpiCfg<EPI>;
   constexpr int BASE = Cfg::BASE;
-  const int rows[2] = {row0, row0 + 8};
+  const int rows[2] = {row_base + lrow, row_base + lrow + 8};
   const bool row_ok[2] = {rows[0] < p.M, rows[1] < p.M};
 
   // ---- bias, or the folded LayerNorm:  LN(x) . W^T + bias = rstd * (acc - mean * s_n) + bias'_n  (s_n = ln_s, bias' = bias)
@@ -131,75 +270,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const GemmGro
     }
   }
 
-  if constexpr (BASE == SOME_EPI_STORE_BF16 || BASE == SOME_EPI_SILU_BF16) {
-#pragma unroll
-    for (int j = 0; j < ACC / 4; ++j) {
-      const int col = col_tile + 8 * j + 2 * q;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if constexpr (BASE == SOME_EPI_SILU_BF16) v0 = silu_fast(v0), v1 = silu_fast(v1);
-        if (row_ok[h])
-          *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(g.out) + (size_t)rows[h] * p.ld_out + col) = pack_bf16x2(v0, v1);
-      }
-    }
-  } else if constexpr (BASE == SOME_EPI_GLU_BF16) {
-#pragma unroll
-    for (int G = 0; G < ACC / 16; ++G) {
-#pragma unroll
-      for (int jj = 0; jj < 2; ++jj) {
-        const int j = 4 * G + jj;
-        const int oc = (col_tile >> 1) + 16 * G + 8 * jj + 2 * q;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const float o0 = acc[4 * j + 2 * h] * sigmoid_fast(acc[4 * (j + 2) + 2 * h]);
-          const float o1 = acc[4 * j + 2 * h + 1] * sigmoid_fast(acc[4 * (j + 2) + 2 * h + 1]);
-          if (row_ok[h])
-            *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(g.out) + (size_t)rows[h] * p.ld_out + oc) = pack_bf16x2(o0, o1);
-        }
-      }
-    }
-  } else if constexpr (BASE == SOME_EPI_RESID_F32 || BASE == SOME_EPI_GLU_RESID_F32) {
-    constexpr bool GLU = BASE == SOME_EPI_GLU_RESID_F32;
-    [[maybe_unused]] float st_s[2][2] = {}, st_q[2][2] = {};   // [row half][128-column slot of the tile]
-#pragma unroll
-    for (int j = 0; j < ACC / 4; ++j) {
-      if (GLU && (j & 3) >= 2) continue;   // gate columns: consumed with their "out" partners
-      const int oc = GLU ? (col_tile >> 1) + 16 * (j >> 2) + 8 * (j & 3) + 2 * q : col_tile + 8 * j + 2 * q;
-      const int slot = j >> 4;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if constexpr (GLU) {
-          v0 *= sigmoid_fast(acc[4 * (j + 2) + 2 * h]);
-          v1 *= sigmoid_fast(acc[4 * (j + 2) + 2 * h + 1]);
-        }
-        if (row_ok[h]) {
-          const size_t off = (size_t)rows[h] * p.ld_out + oc;
-          const float2 r = *reinterpret_cast<const float2*>(g.resid + off);
-          float2 x;
-          if constexpr (GLU) x = make_float2(r.x + v0, r.y + v1);
-          else x = make_float2(fmaf(v0, p.alpha, r.x), fmaf(v1, p.alpha, r.y));   // alpha * (acc + bias) + resid
-          *reinterpret_cast<float2*>(static_cast<float*>(g.out) + off) = x;
-          if constexpr (Cfg::LNP) {
-            st_s[h][slot] += x.x + x.y;
-            st_q[h][slot] = fmaf(x.x, x.x, fmaf(x.y, x.y, st_q[h][slot]));
-            *reinterpret_cast<uint32_t*>(g.out_bf16 + off) = pack_bf16x2(x.x, x.y);
-          }
-        }
-      }
-    }
-    if constexpr (Cfg::LNP) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-#pragma unroll
-        for (int sl = 0; sl < 2; ++sl) {
-          const float s = quad_sum(st_s[h][sl]), qq = quad_sum(st_q[h][sl]);
-          if (q == 0 && row_ok[h])
-            reinterpret_cast<float2*>(g.ln_stats)[(size_t)rows[h] * SOME_LN_SLOTS + (col_tile >> 7) + sl] = make_float2(s, qq);
-        }
-      }
-    }
+  if constexpr (Cfg::STAGED) {
+    epilogue_staged<EPI>(p, g, tm, acc, sl, row_base, lrow, col_tile, q, cw);
   } else if constexpr (BASE == SOME_EPI_BIAS_F32 || BASE == SOME_EPI_SIGMOID_F32) {
 #pragma unroll
     for (int j = 0; j < ACC / 4; ++j) {
@@ -252,12 +324,15 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const GemmGro
 
 template <int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
-            const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1, const GemmParams p) {
+gemm_kernel(const __grid_constant__ GemmMaps tm0, const __grid_constant__ GemmMaps tm1, const GemmParams p) {
+  using Cfg = EpiCfg<EPI>;
+  constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);   // [STAGES]
-  uint64_t* empty_bar = full_bar + STAGES;                                          // [STAGES]
+  uint8_t* slabs = smem + STAGES * STAGE_BYTES;                                           // [2][SLAB_BUFS] slabs
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(slabs + 2 * Cfg::SLAB_BUFS * SLAB_BYTES);   // [STAGES]
+  uint64_t* empty_bar = full_bar + STAGES;                                                // [STAGES]
+  uint64_t* slab_bar = empty_bar + STAGES;                                                // [2][2] residual loads
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -270,16 +345,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CU
   const int num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
 
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA0);
-    tma_prefetch_desc(&tmB0);
-    if (p.groups > 1) {
-      tma_prefetch_desc(&tmA1);
-      tma_prefetch_desc(&tmB1);
+    for (int i = 0; i < p.groups; ++i) {
+      const GemmMaps* tm = i == 0 ? &tm0 : &tm1;
+      tma_prefetch_desc(&tm->a);
+      tma_prefetch_desc(&tm->b);
+      if constexpr (Cfg::RESID) tma_prefetch_desc(&tm->resid);
+      if constexpr (Cfg::STAGED) tma_prefetch_desc(&tm->out);
     }
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);   // one arrival per consumer warp
     }
+    for (int i = 0; i < 4; ++i) mbar_init(&slab_bar[i], 1);
     fence_mbar_init();
   }
   __syncthreads();
@@ -295,14 +372,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CU
         const int grp = tile / tiles_per_group;
         const int t = tile - grp * tiles_per_group;
         const int m_blk = t / num_n, n_blk = t - m_blk * num_n;
-        const CUtensorMap* ta = grp == 0 ? &tmA0 : &tmA1;
-        const CUtensorMap* tb = grp == 0 ? &tmB0 : &tmB1;
+        const GemmMaps* tm = grp == 0 ? &tm0 : &tm1;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);   // out-of-bounds rows are zero-filled and still counted
           uint8_t* sa = smem + stage * STAGE_BYTES;
-          tma_load_2d(sa, ta, &full_bar[stage], kb * BLOCK_K, m_blk * BLOCK_M);
-          tma_load_2d(sa + A_BYTES, tb, &full_bar[stage], kb * BLOCK_K, n_blk * BLOCK_N);
+          tma_load_2d(sa, &tm->a, &full_bar[stage], kb * BLOCK_K, m_blk * BLOCK_M);
+          tma_load_2d(sa + A_BYTES, &tm->b, &full_bar[stage], kb * BLOCK_K, n_blk * BLOCK_N);
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
@@ -314,12 +390,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CU
   } else {
     setmaxnreg_inc<232>();
     const int cw = wg - 1;   // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
+    Slabs sl{slabs + cw * Cfg::SLAB_BUFS * SLAB_BYTES, slab_bar + 2 * cw, 0u, (threadIdx.x & 127) == 0};
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int grp = tile / tiles_per_group;
       const int t = tile - grp * tiles_per_group;
       const int m_blk = t / num_n, n_blk = t - m_blk * num_n;
+      const GemmMaps* tm = grp == 0 ? &tm0 : &tm1;
+      const int row_base = m_blk * BLOCK_M + cw * SLAB_ROWS;
+      // the tile's first residual slab loads while the MMAs run (its buffer's last store was waited for, .read, in the
+      // previous tile's last slab)
+      if constexpr (Cfg::RESID)
+        if (sl.leader) slab_load(*tm, sl, sl.count, Cfg::GLU ? n_blk * BLOCK_N / 2 : n_blk * BLOCK_N, row_base);
       float acc[ACC];
       int prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
@@ -344,20 +427,23 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CU
       wgmma_reg_fence(acc);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
       const GemmGroup g = grp == 0 ? p.g[0] : p.g[1];   // no dynamic index into the parameter space (a local copy)
-      epilogue_tile<EPI>(p, g, acc, m_blk * BLOCK_M + cw * 64 + (warp & 3) * 16 + (lane >> 2), n_blk * BLOCK_N,
-                         lane & 3);
+      epilogue_tile<EPI>(p, g, *tm, acc, sl, row_base, (warp & 3) * 16 + (lane >> 2), n_blk * BLOCK_N, lane & 3, cw);
     }
+    // all stores performed before the CTA exits: a dependent kernel (programmatic launch) may read them at once
+    if constexpr (Cfg::STAGED)
+      if (sl.leader) bulk_wait_group<0>();
   }
 }
 
 template <int EPI>
-static int launch_gemm(const CUtensorMap* maps, const GemmParams& p, cudaStream_t stream) {
+static int launch_gemm(const GemmMaps* maps, const GemmParams& p, cudaStream_t stream) {
   auto kern = gemm_kernel<EPI>;
+  constexpr int smem = EpiCfg<EPI>::SMEM;
   static bool configured[kMaxDevices] = {};   // function attributes are per device
   const int dev_ = device_index();
   if (!configured[dev_]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM);
-    SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(gemm, %d B smem): %s", GEMM_SMEM, cudaGetErrorString(e));
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(gemm, %d B smem): %s", smem, cudaGetErrorString(e));
     configured[dev_] = true;
   }
   const int num_m = (p.M + BLOCK_M - 1) / BLOCK_M;
@@ -365,7 +451,7 @@ static int launch_gemm(const CUtensorMap* maps, const GemmParams& p, cudaStream_
   const int tiles = num_m * num_n * p.groups;
   int grid = num_sms();
   if (tiles < grid) grid = tiles;
-  launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), GEMM_SMEM, stream, maps[0], maps[1], maps[2], maps[3], p);
+  launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), smem, stream, maps[0], maps[1], p);
   return check_launch("some_gemm");
 }
 
@@ -402,29 +488,41 @@ extern "C" int some_gemm(const some_gemm_args* a, cudaStream_t stream) {
   // one slot per 128 accumulator columns (= 128 outputs, or 64 after a GLU)
   if (ln_producer)
     SOME_REQUIRE(a->N / 128 <= SOME_LN_SLOTS, "some_gemm: LayerNorm producer output too wide (N=%d)", a->N);
-  CUtensorMap maps[4];
+  GemmMaps maps[2];
+  memset(maps, 0, sizeof(maps));
+  const auto aligned16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   for (int g = 0; g < 2; ++g) {
     const int s = g < a->groups ? g : 0;
     SOME_REQUIRE(a->A[s] != nullptr && a->W[s] != nullptr && a->out[s] != nullptr, "some_gemm: null pointer in group %d", s);
-    if (make_tmap_bf16_2d(&maps[2 * g], a->A[s], a->M, a->K, a->lda, BLOCK_M)) return -1;
-    if (make_tmap_bf16_2d(&maps[2 * g + 1], a->W[s], a->N, a->K, a->K, BLOCK_N)) return -1;
+    if (make_tmap_bf16_2d(&maps[g].a, a->A[s], a->M, a->K, a->lda, BLOCK_M)) return -1;
+    if (make_tmap_bf16_2d(&maps[g].b, a->W[s], a->N, a->K, a->K, BLOCK_N)) return -1;
     p.g[g].bias = a->bias[s];
     p.g[g].out = a->out[s];
-    p.g[g].resid = a->resid[s];
     p.g[g].ln_s = a->ln_s[s];
     p.g[g].ln_stats = a->ln_stats[s];
-    p.g[g].out_bf16 = reinterpret_cast<__nv_bfloat16*>(a->out_bf16[s]);
+    // the staged epilogues store (and the residual ones load) through tensor maps: 16-byte aligned bases and pitches
     if (needs_resid) {
       const int out_cols = glu_resid ? a->N / 2 : a->N;
       SOME_REQUIRE(a->resid[s] != nullptr, "some_gemm: epilogue %d needs a residual pointer (group %d)", epi, s);
       SOME_REQUIRE(a->ld_out % 4 == 0 && out_cols <= a->ld_out, "some_gemm: bad ld_out %d for %d output columns", a->ld_out, out_cols);
-      if (ln_producer)
+      SOME_REQUIRE(aligned16(a->resid[s]) && aligned16(a->out[s]),
+                   "some_gemm: resid and out must be 16-byte aligned (group %d)", s);
+      if (make_tmap_2d(&maps[g].resid, 4, a->resid[s], a->M, out_cols, a->ld_out, SLAB_ROWS, 32)) return -1;
+      if (make_tmap_2d(&maps[g].out, 4, a->out[s], a->M, out_cols, a->ld_out, SLAB_ROWS, 32)) return -1;
+      if (ln_producer) {
         SOME_REQUIRE(a->out_bf16[s] != nullptr && a->ln_stats[s] != nullptr,
                      "some_gemm: LayerNorm producer epilogue %d needs out_bf16 and ln_stats (group %d)", epi, s);
+        SOME_REQUIRE(a->ld_out % 8 == 0 && aligned16(a->out_bf16[s]),
+                     "some_gemm: out_bf16 needs a 16-byte aligned base and ld_out %% 8 == 0 (ld_out %d, group %d)",
+                     a->ld_out, s);
+        if (make_tmap_2d(&maps[g].out_bf16, 2, a->out_bf16[s], a->M, out_cols, a->ld_out, SLAB_ROWS, 64)) return -1;
+      }
     }
-    if (!head && !needs_resid) {   // bf16 epilogues: bf16 pairs stored as 32-bit words
+    if (!head && !needs_resid) {
       const int out_cols = (epi == SOME_EPI_GLU_BF16 || epi == SOME_EPI_LN_GLU_BF16) ? a->N / 2 : a->N;
       SOME_REQUIRE(a->ld_out % 8 == 0 && out_cols <= a->ld_out, "some_gemm: bad ld_out %d for %d bf16 output columns", a->ld_out, out_cols);
+      SOME_REQUIRE(aligned16(a->out[s]), "some_gemm: out must be 16-byte aligned (group %d)", s);
+      if (make_tmap_2d(&maps[g].out, 2, a->out[s], a->M, out_cols, a->ld_out, SLAB_ROWS, 64)) return -1;
     }
     if (ln_consumer)
       SOME_REQUIRE(a->ln_s[s] != nullptr && a->ln_stats[s] != nullptr && a->bias[s] != nullptr,

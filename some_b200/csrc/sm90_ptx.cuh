@@ -125,6 +125,29 @@ template <int kPending>
 __device__ __forceinline__ void bulk_wait_group_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(kPending) : "memory");
 }
+// waits until at most kPending of this thread's committed bulk groups are incomplete (their global writes performed)
+template <int kPending>
+__device__ __forceinline__ void bulk_wait_group() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(kPending) : "memory");
+}
+
+// ------------------------------------------------------------------ shared memory by 32-bit address
+__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void sts_f2(uint32_t addr, float2 v) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
+}
+__device__ __forceinline__ float2 lds_f2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
+
+// ------------------------------------------------------------------ named barriers (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 // ------------------------------------------------------------------ register reallocation (whole warpgroup)
 template <uint32_t kRegs>
