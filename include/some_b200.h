@@ -237,6 +237,57 @@ int some_slicer_rms(const float* wave, long long n_samples, int frame_length, in
 int some_resample_kaiser(const float* x, const int64_t* x_start, const int64_t* x_len, float* y, const int64_t* y_start, int B,
                          long long max_out, int sr_orig, int sr_new, const double* win, int nwin, cudaStream_t stream);
 
+/* ---- K-flac (the step in front of K-resample): the FLAC decode of librosa.load (soundfile -> libsndfile -> libFLAC) for
+ * many recordings in one set of launches, from slices of one device byte buffer `data` (restated in oracle/flac.py).
+ * Streams with more than 24 bits per sample are the caller's to refuse; so is parsing the metadata blocks.
+ *   streams  device [n_streams], sorted by audio_start, disjoint: recording s's frames lie in [audio_start, end) of data
+ *            and must agree with its STREAMINFO channels, bps and max block size.
+ * some_flac_scan: every byte position of every recording's audio range where a frame header starts that is syntactically
+ * valid, has a correct CRC-8 and agrees with the STREAMINFO is a candidate; *count (device int) = their number, and the
+ * first min(count, capacity) are written to frames[] in byte order with pos, number, stream, blocksize, header_len,
+ * chan_code, variable filled.  Each written candidate is then parsed (subframe syntax, zero padding, CRC-16): status =
+ * SOME_FLAC_OK and end = one past its CRC-16, or another status and end = the byte where the problem was found.  A
+ * candidate never reads outside its recording's range.  If count > capacity, the call must be repeated with a larger
+ * capacity.  workspace: some_flac_scan_workspace_bytes(n_bytes) bytes of device memory.
+ * some_flac_decode: decodes frames[chain[k]] (k < n_chain, each parsed OK) into scratch[scratch_off[k] ..] as int32
+ * [channels][blocksize], then writes x * 2^-(bps-1) to out: mono (out[out_off[k] + i], np.mean's float32 order over the
+ * channels) or interleaved (out[(out_off[k] + i) * channels + c]).  *status (device int, zero on entry) is set if a
+ * chained frame fails to decode. */
+enum {
+  SOME_FLAC_OK = 0,
+  SOME_FLAC_TRUNCATED = 1,           /* the frame runs past the end of its recording */
+  SOME_FLAC_BAD_CRC16 = 2,
+  SOME_FLAC_BAD_PADDING = 3,         /* a subframe's zero bit or the frame's byte-alignment bits are not 0 */
+  SOME_FLAC_RESERVED_SUBFRAME = 4,   /* reserved subframe type or FIXED order > 4 */
+  SOME_FLAC_BAD_WASTED_BITS = 5,     /* wasted bits >= the subframe's bits per sample */
+  SOME_FLAC_BAD_ORDER = 6,           /* predictor order > block size */
+  SOME_FLAC_BAD_LPC = 7,             /* LPC precision code 1111 or negative shift */
+  SOME_FLAC_BAD_RESIDUAL = 8,        /* reserved residual coding method */
+  SOME_FLAC_BAD_PARTITION = 9        /* partition order does not divide the block, or its first partition < order */
+};
+typedef struct {
+  int64_t audio_start;
+  int64_t end;
+  int32_t channels, bps, max_blocksize, reserved;
+} some_flac_stream;
+typedef struct {
+  int64_t pos;                       /* byte offset of the frame header in data */
+  int64_t number;                    /* coded frame number (fixed blocking) or first sample number (variable blocking) */
+  int64_t end;
+  int32_t stream;
+  int32_t blocksize;
+  int16_t header_len;
+  uint8_t chan_code;                 /* 0-7 independent channels, 8 left/side, 9 side/right, 10 mid/side */
+  uint8_t variable;                  /* blocking strategy bit */
+  int32_t status;
+} some_flac_frame;
+uint64_t some_flac_scan_workspace_bytes(long long n_bytes);
+int some_flac_scan(const uint8_t* data, long long n_bytes, const some_flac_stream* streams, int n_streams,
+                   some_flac_frame* frames, int capacity, int* count, void* workspace, cudaStream_t stream);
+int some_flac_decode(const uint8_t* data, const some_flac_stream* streams, const some_flac_frame* frames, const int32_t* chain,
+                     const int64_t* scratch_off, const int64_t* out_off, int n_chain, int32_t* scratch, float* out, int mono,
+                     int* status, cudaStream_t stream);
+
 /* ---- some_forward: the whole trunk Gmidi_conform.forward (Gconform.py:119-140) + head activation
  * (Gmidi_conform.py:30-40) as one call that enqueues the launch sequence above on `stream`.
  * All pointers are device pointers owned by the caller (packed by some_b200/weights.py); the structs themselves are

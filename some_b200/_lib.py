@@ -129,6 +129,9 @@ EXPORTS = {
     'some_decode_notes': (C.c_int, [C.POINTER(DecodeArgs), _vp]),
     'some_slicer_rms': (C.c_int, [_vp, C.c_longlong, C.c_int, C.c_int, _vp, C.c_int, _vp]),
     'some_resample_kaiser': (C.c_int, [_vp, _vp, _vp, _vp, _vp, C.c_int, C.c_longlong, C.c_int, C.c_int, _vp, C.c_int, _vp]),
+    'some_flac_scan_workspace_bytes': (C.c_uint64, [C.c_longlong]),
+    'some_flac_scan': (C.c_int, [_vp, C.c_longlong, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp]),
+    'some_flac_decode': (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp, C.c_int, _vp, _vp]),
     'some_row_stats': (C.c_int, [C.POINTER(RowStatsArgs), _vp]),
     'some_col_means': (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, _vp]),
     'some_forward': (C.c_int, [C.POINTER(ModelC), C.POINTER(WorkspaceC), C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp,

@@ -5,18 +5,23 @@
 - ``decode_wav`` / ``to_mono``: libsndfile's integer -> float32 scaling for RIFF/WAVE files and librosa.to_mono.
 - ``resample``: librosa.resample(res_type='kaiser_best') on the GPU (csrc/resample.cu, some_resample_kaiser), BIT-identical to
   resampy's float32 loop; numpy in -> numpy out, CUDA tensor in -> CUDA tensor out on the current stream.
-- ``load``: librosa.load for RIFF/WAVE files (PCM 8/16/24/32-bit, float32/64, WAVE_FORMAT_EXTENSIBLE).  Other containers
-  (FLAC, OGG, MP3, AIFF, ...) raise: librosa decodes those through libsndfile / audioread, which this module does not restate.
+- ``read_encoded`` / ``EncodedAudio`` / ``FlacBatch`` / ``decode_flac``: FLAC files (libsndfile reads them through libFLAC)
+  decoded on the GPU (csrc/flac.cu): the file's bytes and its STREAMINFO are read on the host, the frames are found,
+  checked and decoded on the device, many recordings in one set of launches, straight to mono if wanted.
+- ``load``: librosa.load for RIFF/WAVE files (PCM 8/16/24/32-bit, float32/64, WAVE_FORMAT_EXTENSIBLE) and for FLAC files
+  (``fLaC``, optionally behind an ID3v2 tag; up to 24 bits per sample), chosen by the file's content.  Other containers
+  (Ogg, MP3, AIFF, ...) raise: librosa decodes those through libsndfile / audioread, which this module does not restate.
 - ``load_native``: the decoded recording at its own rate, for batch.batch_infer_dataset's device-resident resampling.
 
-The arithmetic is restated in oracle/resample.py (test infrastructure), which documents what was restated and what could
-not be compared with the libraries themselves.
+The arithmetic is restated in oracle/resample.py and oracle/flac.py (test infrastructure), which document what was
+restated and what could not be compared with the libraries themselves.
 """
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import functools
-from typing import Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -162,10 +167,248 @@ def resample(y, orig_sr: int, target_sr: int):
     return dst.cpu().numpy() if is_np else dst
 
 
+# ---------------------------------------------------------------------------------------------- FLAC (host metadata)
+@dataclasses.dataclass(frozen=True, eq=False)
+class EncodedAudio:
+    """A FLAC recording as read from disk, not yet decoded: the file's bytes and its STREAMINFO.  ``length`` is the
+    STREAMINFO sample count (0 = not stated: known once the frames are decoded)."""
+    name: str
+    data: bytes
+    rate: int
+    channels: int
+    bps: int
+    length: int
+    audio_offset: int           # byte offset of the first frame (after any ID3v2 tag, 'fLaC' and the metadata blocks)
+    min_blocksize: int
+    max_blocksize: int
+
+
+def _id3_size(data: bytes) -> int:
+    """Length of an ID3v2 tag at the start of ``data`` (0 if none): 10 + its syncsafe size, + 10 with a footer (0x10)."""
+    if len(data) < 10 or data[:3] != b'ID3':
+        return 0
+    size = (data[6] & 0x7F) << 21 | (data[7] & 0x7F) << 14 | (data[8] & 0x7F) << 7 | (data[9] & 0x7F)
+    return 10 + size + (10 if data[5] & 0x10 else 0)
+
+
+def parse_flac(data: bytes, name: str = '<bytes>') -> EncodedAudio:
+    """The metadata of a FLAC stream (host; raises ValueError naming FLAC and the byte offset on malformed input): the
+    first block must be a 34-byte STREAMINFO; PADDING, APPLICATION, SEEKTABLE, VORBIS_COMMENT, CUESHEET, PICTURE and unknown
+    blocks are skipped; type 127 is invalid.  Streams of more than 24 bits per sample are refused."""
+    off = _id3_size(data)
+    if data[off:off + 4] != b'fLaC':
+        raise ValueError(f'{name}: not a FLAC stream (no fLaC marker at byte offset {off})')
+    p, info, first = off + 4, None, True
+    while True:
+        if p + 4 > len(data):
+            raise ValueError(f'{name}: FLAC metadata block header truncated at byte offset {p}')
+        last, kind, size = data[p] >> 7, data[p] & 0x7F, int.from_bytes(data[p + 1:p + 4], 'big')
+        if first and (kind != 0 or size != 34):
+            raise ValueError(f'{name}: FLAC stream does not start with a 34-byte STREAMINFO block (type {kind}, {size} '
+                             f'bytes at byte offset {p})')
+        if not first and kind in (0, 127):
+            raise ValueError(f'{name}: {"second STREAMINFO" if kind == 0 else "invalid"} FLAC metadata block at byte offset {p}')
+        if p + 4 + size > len(data):
+            raise ValueError(f'{name}: FLAC metadata block truncated at byte offset {p}')
+        if first:
+            b = int.from_bytes(data[p + 4:p + 22], 'big')               # the 144 bits in front of the MD5
+            info = dict(min_blocksize=b >> 128, max_blocksize=(b >> 112) & 0xFFFF, rate=(b >> 44) & 0xFFFFF,
+                        channels=((b >> 41) & 7) + 1, bps=((b >> 36) & 31) + 1, length=b & ((1 << 36) - 1))
+            first = False
+        p += 4 + size
+        if last:
+            break
+    if info['bps'] > 24:
+        raise ValueError(f'{name}: FLAC stream of {info["bps"]} bits per sample (at byte offset {off + 8}); only up to 24 '
+                         f'bits are decoded (libsndfile\'s float scaling is exact up to 24 bits)')
+    if info['rate'] == 0 or info['max_blocksize'] == 0:
+        raise ValueError(f'{name}: invalid FLAC STREAMINFO (sample rate {info["rate"]}, max block size '
+                         f'{info["max_blocksize"]}) at byte offset {off + 8}')
+    return EncodedAudio(name=name, data=bytes(data), audio_offset=p, **info)
+
+
+def _sniff(path) -> str:
+    """'flac' for 'fLaC' (optionally behind an ID3v2 tag), else 'other'."""
+    with open(path, 'rb') as f:
+        head = f.read(10)
+        off = _id3_size(head)
+        if off:
+            f.seek(off)
+            head = f.read(4)
+    return 'flac' if head[:4] == b'fLaC' else 'other'
+
+
+def read_encoded(path, sr=None) -> EncodedAudio:
+    """Reads a FLAC file and parses its metadata on the host; no decoding happens here.  The second argument is the rate
+    the caller wants (batch.batch_infer_dataset passes it) and is ignored: the dataset driver decodes the records on the
+    device and resamples them straight into the batch's wave buffer."""
+    with open(path, 'rb') as f:
+        return parse_flac(f.read(), str(path))
+
+
+# ---------------------------------------------------------------------------------------------- FLAC (device)
+_STREAM_DTYPE = np.dtype([('audio_start', '<i8'), ('end', '<i8'), ('channels', '<i4'), ('bps', '<i4'),
+                          ('max_blocksize', '<i4'), ('reserved', '<i4')])                       # some_flac_stream
+_FRAME_DTYPE = np.dtype([('pos', '<i8'), ('number', '<i8'), ('end', '<i8'), ('stream', '<i4'), ('blocksize', '<i4'),
+                         ('header_len', '<i2'), ('chan_code', 'u1'), ('variable', 'u1'), ('status', '<i4')])  # some_flac_frame
+_FLAC_REASONS = {1: 'truncated frame', 2: 'CRC-16 mismatch', 3: 'non-zero padding bits', 4: 'reserved subframe type',
+                 5: 'invalid wasted-bits count', 6: 'predictor order larger than the block',
+                 7: 'invalid LPC precision or shift', 8: 'reserved residual coding method', 9: 'invalid partition order'}
+
+
+class FlacBatch:
+    """FLAC recordings uploaded into one device buffer, their frames found, checked and chained (some_flac_scan, then one
+    device-to-host copy of the candidate list and the chain on the host).  Raises ValueError naming the file, FLAC and the
+    byte offset for a corrupt stream.  ``lengths`` are then known, and ``emit`` enqueues the decode of any of the
+    recordings into slices of a float32 CUDA tensor on the current stream, without synchronising."""
+
+    def __init__(self, records: Sequence[EncodedAudio], device):
+        import torch
+        from . import _lib
+        self.records = list(records)
+        self.device = torch.device(device)
+        sizes = [len(r.data) for r in self.records]
+        bases = np.zeros(len(sizes) + 1, dtype=np.int64)
+        np.cumsum(sizes, out=bases[1:])
+        streams = np.zeros(len(self.records), _STREAM_DTYPE)
+        for i, r in enumerate(self.records):
+            streams[i] = (bases[i] + r.audio_offset, bases[i + 1], r.channels, r.bps, r.max_blocksize, 0)
+        lib = _lib.load()
+        stream = torch.cuda.current_stream(self.device)
+        host = np.empty(max(int(bases[-1]), 1), np.uint8)
+        for r, a in zip(self.records, bases):
+            host[a:a + len(r.data)] = np.frombuffer(r.data, np.uint8)
+        self.data = torch.from_numpy(host).to(self.device)
+        self.streams = torch.from_numpy(streams.view(np.uint8).copy()).to(self.device)
+        ws = torch.empty(int(lib.some_flac_scan_workspace_bytes(int(bases[-1]))), dtype=torch.uint8, device=self.device)
+        count = torch.zeros(1, dtype=torch.int32, device=self.device)
+        # real frames: at most length / min block size + 1 each; false sync patterns are rare (a CRC-8 and the STREAMINFO
+        # must both match), and a larger list is made if they do not fit
+        capacity = 64 + sum((r.length // max(r.min_blocksize, 1) + 2) if r.length else (len(r.data) // 16 + 2)
+                            for r in self.records)
+        while True:
+            frames = torch.empty(capacity * _FRAME_DTYPE.itemsize, dtype=torch.uint8, device=self.device)
+            _lib.check(lib.some_flac_scan(self.data.data_ptr(), int(bases[-1]), self.streams.data_ptr(), len(self.records),
+                                          frames.data_ptr(), capacity, count.data_ptr(), ws.data_ptr(),
+                                          C.c_void_p(stream.cuda_stream)), 'some_flac_scan')
+            n = int(count.item())                                             # syncs
+            if n <= capacity:
+                break
+            capacity = n
+        self.frames, self.n_candidates = frames, n
+        fr = frames[:n * _FRAME_DTYPE.itemsize].cpu().numpy().view(_FRAME_DTYPE)
+        self._chain(fr, bases)
+
+    def _chain(self, fr, bases):
+        """Walks every recording from its first audio byte: each next frame starts where the current one ends and carries
+        the next frame number (fixed blocking) or sample number (variable blocking)."""
+        pos, end, status = fr['pos'].tolist(), fr['end'].tolist(), fr['status'].tolist()
+        number, variable, bs = fr['number'].tolist(), fr['variable'].tolist(), fr['blocksize'].tolist()
+        n = len(pos)
+        self.chains: List[np.ndarray] = []
+        self.lengths: List[int] = []
+        i = 0
+        for r, rec in enumerate(self.records):
+            base, p, stop, total = int(bases[r]), int(bases[r]) + rec.audio_offset, int(bases[r + 1]), rec.length
+            chain, got, strategy = [], 0, None
+            while not (total and got == total) and not (not total and p == stop):
+                if p >= stop:
+                    raise ValueError(f'{rec.name}: FLAC stream ends at byte offset {p - base} after {got} of {total} samples')
+                while i < n and pos[i] < p:
+                    i += 1
+                if i >= n or pos[i] != p:
+                    raise ValueError(f'{rec.name}: no valid FLAC frame header (sync, reserved code, CRC-8 or STREAMINFO '
+                                     f'mismatch) at byte offset {p - base}')
+                if status[i]:
+                    raise ValueError(f'{rec.name}: FLAC frame at byte offset {p - base}: '
+                                     f'{_FLAC_REASONS.get(status[i], status[i])} (at byte offset {end[i] - base})')
+                strategy = variable[i] if strategy is None else strategy
+                want = got if variable[i] else len(chain)
+                if variable[i] != strategy or number[i] != want:
+                    raise ValueError(f'{rec.name}: FLAC frame at byte offset {p - base}: {"sample" if variable[i] else "frame"} '
+                                     f'number {number[i]}, expected {want} (gap, overlap or changed blocking strategy)')
+                got += bs[i]
+                if total and got > total:
+                    raise ValueError(f'{rec.name}: FLAC frame at byte offset {p - base} decodes past the {total} samples '
+                                     f'STREAMINFO states')
+                chain.append(i)
+                p = end[i]
+            self.chains.append(np.asarray(chain, dtype=np.int32))
+            self.lengths.append(got)
+        self._bs = np.asarray(bs, dtype=np.int64)
+
+    def emit(self, out, starts: Dict[int, int], mono: bool = True):
+        """Decodes recording r into out[starts[r] : + lengths[r]] (mono: np.mean's float32 order over the channels, i.e.
+        to_mono(decode_flac(...).T)) or, with mono=False, out[starts[r] * channels : + lengths[r] * channels] interleaved
+        [n, channels]; one some_flac_decode call for all of ``starts`` on the current stream.  Returns the device status
+        word (0 unless a chained frame failed to decode)."""
+        import torch
+        from . import _lib
+        assert out.dtype == torch.float32 and out.device == self.device
+        idx, off = [], []
+        for r, start in starts.items():
+            ch = 1 if mono else self.records[r].channels
+            assert 0 <= start and (start + self.lengths[r]) * ch <= out.numel(), 'recording outside its buffer'
+            c = self.chains[r]
+            idx.append(c)
+            off.append(start + np.concatenate([[0], np.cumsum(self._bs[c])[:-1]]).astype(np.int64) if len(c) else
+                       np.zeros(0, np.int64))
+        status = torch.zeros(1, dtype=torch.int32, device=self.device)
+        chain = np.concatenate(idx) if idx else np.zeros(0, np.int32)
+        if not len(chain):
+            return status
+        ch_of = np.array([r.channels for r in self.records], np.int64)
+        fr_stream = np.concatenate([np.full(len(c), r, np.int64) for r, c in zip(starts, idx)])
+        slot = self._bs[chain] * ch_of[fr_stream]
+        scratch_off = np.concatenate([[0], np.cumsum(slot)[:-1]]).astype(np.int64)
+        meta = torch.from_numpy(np.stack([scratch_off, np.concatenate(off)])).to(self.device)
+        chain_d = torch.from_numpy(chain).to(self.device)
+        scratch = torch.empty(max(int(slot.sum()), 1), dtype=torch.int32, device=self.device)
+        lib = _lib.load()
+        _lib.check(lib.some_flac_decode(self.data.data_ptr(), self.streams.data_ptr(), self.frames.data_ptr(),
+                                        chain_d.data_ptr(), meta[0].data_ptr(), meta[1].data_ptr(), len(chain),
+                                        scratch.data_ptr(), out.data_ptr(), int(mono), status.data_ptr(),
+                                        C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)), 'some_flac_decode')
+        return status
+
+
+def _check_status(status) -> None:
+    if int(status.item()):
+        raise RuntimeError(f'some_flac_decode: a chained frame failed to decode (status {int(status.item())})')
+
+
+def _flac_device(rec: EncodedAudio, mono: bool):
+    """(CUDA float32 tensor: [n] mono / single channel or [channels, n], FlacBatch) for one record."""
+    import torch
+    dev = torch.device('cuda', torch.cuda.current_device())
+    fb = FlacBatch([rec], dev)
+    n, ch = fb.lengths[0], (1 if mono else rec.channels)
+    y = torch.empty(max(n * ch, 1), dtype=torch.float32, device=dev)
+    status = fb.emit(y, {0: 0}, mono=mono)
+    y = y[:n * ch]
+    _check_status(status)
+    return (y if ch == 1 else y.view(n, ch).t().contiguous()), fb
+
+
+def decode_flac(path) -> Tuple[np.ndarray, int]:
+    """(samples, native rate) of a FLAC file as libsndfile hands them to librosa.load, decoded on the GPU: float32 [n]
+    (one channel) or [n, channels], x * 2^-(bps - 1)."""
+    rec = read_encoded(path)
+    y, _ = _flac_device(rec, mono=False)
+    return (y.cpu().numpy() if y.ndim == 1 else y.t().contiguous().cpu().numpy()), rec.rate
+
+
 # ---------------------------------------------------------------------------------------------- librosa.load
 def load(path, sr=22050, mono: bool = True):
-    """librosa.load(path, sr=sr, mono=mono) (librosa 0.9, res_type='kaiser_best') for RIFF/WAVE files: (y, rate).
-    ``sr=None`` keeps the native rate; otherwise the decoded (and down-mixed) samples are resampled on the GPU."""
+    """librosa.load(path, sr=sr, mono=mono) (librosa 0.9, res_type='kaiser_best') for RIFF/WAVE and FLAC files: (y, rate).
+    ``sr=None`` keeps the native rate; otherwise the decoded (and down-mixed) samples are resampled on the GPU.  FLAC files
+    are decoded and down-mixed on the GPU too."""
+    if _sniff(path) == 'flac':
+        rec = read_encoded(path)
+        y, _ = _flac_device(rec, mono)
+        if sr is not None and as_rate(sr) != rec.rate:
+            return resample(y, rec.rate, as_rate(sr)).cpu().numpy(), as_rate(sr)
+        return y.cpu().numpy(), rec.rate
     x, native = decode_wav(path)
     y = x.T                                                  # librosa's (channels, n)
     if mono:

@@ -17,6 +17,10 @@ sharps, ``unicode=False``) and ``librosa.load(path, sr=audio_sample_rate, mono=T
   are uploaded as they are and ``transcribe_recordings(..., rates=...)`` resamples them on the device with resampy's
   ``kaiser_best`` filter (librosa's default ``res_type``), bit-identical to librosa.load, straight into the batch's wave
   buffer (some_b200/audio.py, csrc/resample.cu);
+- FLAC: ``load_audio=audio.read_encoded`` returns each FLAC file's bytes and metadata (``audio.EncodedAudio``) without
+  decoding them; ``transcribe_recordings`` uploads the bytes of all of them into one buffer and decodes them on the device
+  (csrc/flac.cu), straight to mono at their native rate, bit-identical to librosa.load, into the batch's wave buffer or
+  the resampler's input;
 - default ``load_wav``: the same WAV decode, then scipy's polyphase resampling on the host.  Files that are already at
   ``audio_sample_rate`` give librosa's samples exactly; other rates go through a different filter from librosa's, so their
   notes may differ at the margin.
@@ -154,8 +158,8 @@ def row_notes(ph_dur_field: str, ph_num_field: str, notes: List[dict], round_mid
 
 
 # ---------------------------------------------------------------------------------------------- GPU part
-def transcribe_recordings(infer_ins, waveforms: Sequence[np.ndarray], slicer: Optional[Slicer] = None,
-                          rates: Optional[Sequence[int]] = None):
+def transcribe_recordings(infer_ins, waveforms: Sequence, slicer: Optional[Slicer] = None,
+                          rates: Optional[Sequence[Optional[int]]] = None):
     """[(chunk offsets in seconds, per-chunk notes)] for several mono recordings, as ONE var-len batch.
 
     Equivalent to ``[ (offsets, infer_ins.infer(chunks)) for chunks in (Slicer.slice(w) for w in waveforms) ]``
@@ -165,20 +169,35 @@ def transcribe_recordings(infer_ins, waveforms: Sequence[np.ndarray], slicer: Op
     ``rates``: each recording's native sample rate (default: all at ``audio_sample_rate``).  A recording at another rate is
     uploaded as it is and resampled on the device, grouped by rate, straight into the batch's wave buffer, exactly as
     librosa.load(sr=audio_sample_rate) would have resampled it (audio.resample); slicing and inference then run on the
-    resampled samples."""
+    resampled samples.
+
+    ``waveforms`` may also hold ``audio.EncodedAudio`` records (FLAC files read by ``audio.read_encoded``).  Their rates
+    come from the records (a ``rates`` entry for one must be None or equal it); the bytes of all of them are uploaded into
+    one buffer and decoded on the device, straight to mono at their native rate (audio.FlacBatch), into the wave buffer or
+    the resampler's input."""
     import torch
     eng = infer_ins.model
     target_sr = int(infer_ins.config['audio_sample_rate'])
     slicer = slicer or Slicer(sr=target_sr, max_sil_kept=1000)                                 # batch_infer.py:52
     quantized = bool(getattr(infer_ins, 'quantized', False))
-    waves = [np.ascontiguousarray(w, dtype=np.float32) for w in waveforms]
+    enc = {i: w for i, w in enumerate(waveforms) if isinstance(w, audio.EncodedAudio)}
+    waves = [None if i in enc else np.ascontiguousarray(w, dtype=np.float32) for i, w in enumerate(waveforms)]
     for w in waves:
-        assert w.ndim == 1, 'mono recordings expected (librosa.load(..., mono=True), batch_infer.py:51)'
+        assert w is None or w.ndim == 1, 'mono recordings expected (librosa.load(..., mono=True), batch_infer.py:51)'
     if rates is None:
-        rates = [target_sr] * len(waves)
-    rates = [audio.as_rate(r) for r in rates]
+        rates = [None] * len(waves)
     assert len(rates) == len(waves), 'one rate per recording'
-    lens = [audio.resampled_length(int(w.shape[0]), r, target_sr) for w, r in zip(waves, rates)]
+    for i, rec in enc.items():
+        if rates[i] is not None and audio.as_rate(rates[i]) != rec.rate:
+            raise ValueError(f'{rec.name}: rate {rates[i]} given for a FLAC record of {rec.rate} Hz')
+    rates = [enc[i].rate if i in enc else audio.as_rate(target_sr if r is None else r) for i, r in enumerate(rates)]
+    flac = None
+    if enc:                                                        # scan + chain: one device-to-host copy, one sync
+        with torch.cuda.device(eng.device):
+            flac = audio.FlacBatch(list(enc.values()), eng.device)
+    slot = {i: k for k, i in enumerate(enc)}                       # recording -> its index in the FlacBatch
+    native_lens = [flac.lengths[slot[i]] if i in enc else int(w.shape[0]) for i, w in enumerate(waves)]
+    lens = [audio.resampled_length(n, r, target_sr) for n, r in zip(native_lens, rates)]
     bases = np.zeros(len(waves) + 1, dtype=np.int64)
     np.cumsum([(n + 3) & ~3 for n in lens], out=bases[1:])
     lock = getattr(infer_ins, '_lock', None)
@@ -188,17 +207,25 @@ def transcribe_recordings(infer_ins, waveforms: Sequence[np.ndarray], slicer: Op
         with torch.cuda.device(eng.device):
             wave_d = torch.empty(max(int(bases[-1]), 4), dtype=torch.float32, device=eng.device)
             for w, b, n, r in zip(waves, bases, lens, rates):
-                if n and r == target_sr:
+                if n and r == target_sr and w is not None:
                     src = torch.from_numpy(w)
                     wave_d[b:b + n].copy_(src, non_blocking=src.is_pinned())
+            flac_status = []
+            direct = {slot[i]: int(bases[i]) for i in enc if rates[i] == target_sr}
+            if direct:
+                flac_status.append(flac.emit(wave_d, direct))
             for r in sorted(set(rates) - {target_sr}):                # one resampling launch per native rate
                 group = [i for i, ri in enumerate(rates) if ri == r]
                 starts = np.zeros(len(group) + 1, dtype=np.int64)
-                np.cumsum([waves[i].shape[0] for i in group], out=starts[1:])
+                np.cumsum([native_lens[i] for i in group], out=starts[1:])
                 native_d = torch.empty(max(int(starts[-1]), 1), dtype=torch.float32, device=eng.device)
                 for i, a in zip(group, starts):
-                    native_d[a:a + waves[i].shape[0]].copy_(torch.from_numpy(waves[i]))
-                audio.resample_into(native_d, starts[:-1].tolist(), [waves[i].shape[0] for i in group], wave_d,
+                    if i not in enc:
+                        native_d[a:a + native_lens[i]].copy_(torch.from_numpy(waves[i]))
+                to_decode = {slot[i]: int(a) for i, a in zip(group, starts) if i in enc}
+                if to_decode:
+                    flac_status.append(flac.emit(native_d, to_decode))
+                audio.resample_into(native_d, starts[:-1].tolist(), [native_lens[i] for i in group], wave_d,
                                     [int(bases[i]) for i in group], r, target_sr)
             need = [i for i, n in enumerate(lens) if (n + slicer.hop_size - 1) // slicer.hop_size > slicer.min_length]
             rms_lists = eng.rms_frames_many([wave_d[bases[i]:bases[i] + lens[i]] for i in need], slicer.win_size, slicer.hop_size)
@@ -211,6 +238,8 @@ def transcribe_recordings(infer_ins, waveforms: Sequence[np.ndarray], slicer: Op
                 slab, cu, layout, _ = eng.enqueue(None, quantized, resident=(wave_d, flat))
                 host = slab.cpu().numpy()                                                    # one D2H + sync
                 results = eng.unpack_slab(host, cu, layout)
+            for st in flac_status:                                                           # already complete
+                audio._check_status(st)
     finally:
         if lock is not None:
             lock.release()
@@ -240,9 +269,11 @@ def batch_infer_dataset(dataset, infer_ins, config: dict, round_midi: bool = Fal
     """batch_infer.py's command (:149-226) with dataset-level batching.  ``dataset`` = DiffSinger raw data dir with
     ``transcriptions.csv`` and ``wavs/``; writes ``csv`` (default: the dataset's own transcriptions.csv).
 
-    ``load_audio(path, sr)`` returns the mono waveform at ``sr``, or a ``(waveform, native_rate)`` pair: such recordings are
-    resampled on the device (transcribe_recordings(rates=...)).  ``load_audio=audio.load_native`` is librosa.load's exact
-    result; the default ``load_wav`` resamples with scipy on the host."""
+    ``load_audio(path, sr)`` returns the mono waveform at ``sr``, a ``(waveform, native_rate)`` pair, or an
+    ``audio.EncodedAudio`` record: pairs are resampled on the device (transcribe_recordings(rates=...)), records are also
+    decoded there.  ``load_audio=audio.load_native`` is librosa.load's exact result for WAV files and
+    ``load_audio=audio.read_encoded`` for FLAC files; the default ``load_wav`` resamples with scipy on the host.  (Dataset
+    items are still found as ``wavs/{name}.wav``, whatever the files hold.)"""
     data_path = pathlib.Path(dataset)
     csv_path = pathlib.Path(csv) if csv is not None else data_path / 'transcriptions.csv'
     if csv_path.exists() and not overwrite:
@@ -287,9 +318,13 @@ def batch_infer_dataset(dataset, infer_ins, config: dict, round_midi: bool = Fal
         while pending:
             row, fut = pending.popleft()
             wave = fut.result()
-            wave, rate = wave if isinstance(wave, tuple) else (wave, sr)
+            if isinstance(wave, audio.EncodedAudio):                   # decoded on the device; its rate is its own
+                rate, n = None, wave.length * int(sr) // wave.rate
+            else:
+                wave, rate = wave if isinstance(wave, tuple) else (wave, sr)
+                n = audio.resampled_length(len(wave), audio.as_rate(rate), int(sr))
             refill()
-            t = 1 + audio.resampled_length(len(wave), audio.as_rate(rate), int(sr)) // 512
+            t = 1 + n // 512
             if group and frames + t > max_frames_per_batch:
                 flush()
             group.append((row, wave, rate))
