@@ -213,6 +213,50 @@ typedef struct {
 uint64_t some_decode_scratch_bytes(int M);
 int some_decode_notes(const some_decode_args* args, cudaStream_t stream);
 
+/* ---- K-eval: the validation losses and MIDI accuracy of the training tasks (training/me_task.py:72-154, continuous;
+ * training/me_quant_task.py:43-120, quantized) for B labelled clips in one launch, one CTA per clip, without materialising
+ * the [M, N] target.  Per clip b (frames [cu_frames[b], cu_frames[b+1]), T = their number):
+ *   midi_loss[b]   continuous: sum over T x N of BCEWithLogits(logit, gaussian-blurred target of the collater, me_task.py:26-49),
+ *                  max(x,0) - x*y + log1p(exp(-|x|)); quantized: sum over T of CrossEntropy(logits row, note class) with a
+ *                  stable log-softmax (every frame has a class: unit2note > 0, so ignore_index never applies)
+ *   bound_loss[b]  sum over T of |cumsum(bounds) / sqrt(T) - cumsum(gt) / sqrt(T)|, gt = diff(unit2note, prepend 0) > 0
+ *                  (BinaryEMDLoss, modules/losses/bound_loss.py:6-19; the bounds prefix is accumulated in double and rounded
+ *                  to float per frame like ATen's CPU cumsum)
+ *   correct[b]     frames where MIDIAccuracy(tolerance=0.5).update (modules/metrics/midi_acc.py:16-35) counts a hit:
+ *                  neither the prediction nor the label is a rest and |midi_pred - midi_gt| <= 0.5; the prediction is the
+ *                  validation step's decode of the activated head (continuous: gaussian-blurred decode, rest = max < threshold;
+ *                  quantized: argmax, rest = 128).  The total is T.
+ * The sums are the caller's to divide (T * N, T, T).  Reductions run in a fixed order (frame-strided warps, then warps in
+ * order) with no atomics: a clip's results do not depend on the other clips of the launch.
+ *   logits     f32 [M, N] raw head (SOME_EPI_BIAS_F32), bounds f32 [M] (sigmoid, as the trunk writes them)
+ *   unit2note  i32 [M], 1-based note index within the clip, in [1, cu_notes[b+1] - cu_notes[b]]
+ *   cu_notes   i32 [B+1]; note_midi f32 (continuous: MIDI with rests interpolated; quantized: class 0..128, rest = 128),
+ *              note_rest u8 (continuous only), both [cu_notes[B]]
+ *   head       SOME_EVAL_HEAD_TC: sigmoid / softmax exactly as the tensor-core GEMM's head epilogues compute them (some_forward);
+ *              SOME_EVAL_HEAD_F32: as the fp32 validation path's head kernel computes them (some_forward_f32)
+ *   probs      optional f32 [M, N] (may equal logits): the activated head, bit-identical to what the chosen forward would
+ *              have written with the sigmoid / softmax head, for some_decode_notes
+ * A frame whose unit2note is out of range makes its clip's three results NaN / -1. */
+enum { SOME_EVAL_HEAD_TC = 0, SOME_EVAL_HEAD_F32 = 1 };
+typedef struct {
+  const float* logits;
+  const float* bounds;
+  const int32_t* cu_frames;
+  const int32_t* unit2note;
+  const int32_t* cu_notes;
+  const float* note_midi;
+  const uint8_t* note_rest;
+  int B, M, N;
+  int quantized;
+  int head;
+  float vmin, vmax, deviation, threshold; /* midi_min, midi_max, midi_prob_deviation, rest_threshold */
+  double* midi_loss;
+  double* bound_loss;
+  int32_t* correct;
+  float* probs;
+} some_eval_args;
+int some_eval_clips(const some_eval_args* args, cudaStream_t stream);
+
 /* ---- K-rms (row §8f-1, the step in front of the path): short-time RMS for the silence slicer.
  * Replaces get_rms (utils/slicer2.py:5-38) as called by Slicer.slice (slicer2.py:81): zero padding of frame_length / 2 on
  * both sides, frames of frame_length samples every hop samples, sqrt(mean(x^2)) in float32 with numpy's pairwise summation

@@ -70,6 +70,17 @@ class DecodeArgs(C.Structure):
                 ('dbg_rest', _vp), ('scratch', _vp)]
 
 
+EVAL_HEAD_TC, EVAL_HEAD_F32 = 0, 1
+
+
+class EvalArgs(C.Structure):
+    _fields_ = [('logits', _vp), ('bounds', _vp), ('cu_frames', _vp), ('unit2note', _vp), ('cu_notes', _vp),
+                ('note_midi', _vp), ('note_rest', _vp), ('B', C.c_int), ('M', C.c_int), ('N', C.c_int),
+                ('quantized', C.c_int), ('head', C.c_int), ('vmin', C.c_float), ('vmax', C.c_float),
+                ('deviation', C.c_float), ('threshold', C.c_float), ('midi_loss', _vp), ('bound_loss', _vp),
+                ('correct', _vp), ('probs', _vp)]
+
+
 class BlockWeightsC(C.Structure):
     _fields_ = [('ln_g', _vp * 5), ('ln_b', _vp * 5), ('ffn_w1', _vp * 2), ('ffn_b1', _vp * 2), ('ffn_w2', _vp * 2),
                 ('ffn_b2', _vp * 2), ('w_qkv', _vp), ('w_out', _vp), ('b_out', _vp), ('w_pw1', _vp), ('b_pw1', _vp),
@@ -127,6 +138,7 @@ EXPORTS = {
     'some_bound_head': (C.c_int, [_vp, _vp, _vp, _vp, C.c_float, C.c_int, _vp, _vp]),
     'some_decode_scratch_bytes': (C.c_uint64, [C.c_int]),
     'some_decode_notes': (C.c_int, [C.POINTER(DecodeArgs), _vp]),
+    'some_eval_clips': (C.c_int, [C.POINTER(EvalArgs), _vp]),
     'some_slicer_rms': (C.c_int, [_vp, C.c_longlong, C.c_int, C.c_int, _vp, C.c_int, _vp]),
     'some_resample_kaiser': (C.c_int, [_vp, _vp, _vp, _vp, _vp, C.c_int, C.c_longlong, C.c_int, C.c_int, _vp, C.c_int, _vp]),
     'some_flac_scan_workspace_bytes': (C.c_uint64, [C.c_longlong]),

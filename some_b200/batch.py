@@ -29,6 +29,7 @@ from __future__ import annotations
 
 import concurrent.futures
 import pathlib
+import re
 from csv import DictReader, DictWriter
 from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
@@ -41,10 +42,42 @@ _NOTE_NAMES = ('C', 'C#', 'D', 'D#', 'E', 'F', 'F#', 'G', 'G#', 'A', 'A#', 'B')
 
 
 # ---------------------------------------------------------------------------------------------- strings / rounding
-def midi_to_note(midi: float) -> str:
-    """librosa.midi_to_note(midi, unicode=False) for a scalar (octave on, cents off, key C:maj)."""
+def midi_to_note(midi: float, cents: bool = False) -> str:
+    """librosa.midi_to_note(midi, cents=cents, unicode=False) for a scalar (octave on, key C:maj).  With ``cents`` the
+    signed cent offset ``int(100 * np.around(midi - round(midi), 2))`` follows as ``{:+02d}`` (``C4+0``, ``A#3-25``).
+    Restated from librosa 0.9 (not installed here): the cents form could not be checked against librosa itself."""
     num = int(np.round(midi))
-    return '{:s}{:0d}'.format(_NOTE_NAMES[num % 12], int(num / 12) - 1)
+    note = '{:s}{:0d}'.format(_NOTE_NAMES[num % 12], int(num / 12) - 1)
+    if cents:
+        note = '{:s}{:+02d}'.format(note, int(100 * np.around(midi - num, 2)))
+    return note
+
+
+_PITCH_CLASSES = {'C': 0, 'D': 2, 'E': 4, 'F': 5, 'G': 7, 'A': 9, 'B': 11}
+_ACCIDENTALS = {'#': 1, '': 0, 'b': -1, '!': -1, '\u266f': 1, '\U0001d12a': 2, '\u266d': -1, '\U0001d12b': -2, '\u266e': 0}
+_NOTE_RE = re.compile('^(?P<note>[A-Ga-g])(?P<accidental>[#\u266f\U0001d12ab!\u266d\U0001d12b\u266e]*)(?P<octave>[+-]?\\d+)?'
+                      '(?P<cents>[+-]\\d+)?$')
+
+
+def note_to_midi(note: str, round_midi: bool = True):
+    """librosa.note_to_midi(note, round_midi=round_midi) for one note name: pitch class, any accidentals (``#``, ``b``,
+    ``!`` and the unicode signs), optional octave (default 0) and optional signed cents, as
+    ``12 * (octave + 1) + pitch + accidentals + cents * 1e-2`` (rounded half to even to an int with ``round_midi``).  Raises
+    ValueError for a malformed name.  Restated from librosa 0.9 (not installed here) and not checked against librosa
+    itself; the DiffSinger labels it reads use the plain forms (``C#4``, ``A3+25``, ``rest`` is the caller's)."""
+    match = _NOTE_RE.match(note)
+    if not match:
+        raise ValueError(f'Improper note format: {note:s}')
+    pitch = match.group('note').upper()
+    offset = np.sum([_ACCIDENTALS[o] for o in match.group('accidental')])
+    octave = match.group('octave')
+    cents = match.group('cents')
+    octave = int(octave) if octave else 0
+    cents = int(cents) * 1e-2 if cents else 0
+    note_value = 12 * (octave + 1) + _PITCH_CLASSES[pitch] + offset + cents
+    if round_midi:
+        note_value = int(np.round(note_value))
+    return note_value
 
 
 def calc_seq(note_midi: float, note_rest: bool) -> str:
@@ -158,6 +191,57 @@ def row_notes(ph_dur_field: str, ph_num_field: str, notes: List[dict], round_mid
 
 
 # ---------------------------------------------------------------------------------------------- GPU part
+def stage_recordings(eng, target_sr: int, waveforms: Sequence, rates: Optional[Sequence[Optional[int]]]):
+    """Uploads mono recordings (numpy arrays, or ``audio.EncodedAudio`` FLAC records) into ONE device buffer at
+    ``target_sr``, as transcribe_recordings describes: recordings at another rate are resampled on the device, FLAC records
+    decoded there.  Call on the engine's device.  Returns (wave_d, bases int64 [n + 1], lens, flac_status): recording i is
+    wave_d[bases[i] : bases[i] + lens[i]]; the FLAC status words are checked with audio._check_status once the stream has
+    passed them."""
+    import torch
+    enc = {i: w for i, w in enumerate(waveforms) if isinstance(w, audio.EncodedAudio)}
+    waves = [None if i in enc else np.ascontiguousarray(w, dtype=np.float32) for i, w in enumerate(waveforms)]
+    for w in waves:
+        assert w is None or w.ndim == 1, 'mono recordings expected (librosa.load(..., mono=True), batch_infer.py:51)'
+    if rates is None:
+        rates = [None] * len(waves)
+    assert len(rates) == len(waves), 'one rate per recording'
+    for i, rec in enc.items():
+        if rates[i] is not None and audio.as_rate(rates[i]) != rec.rate:
+            raise ValueError(f'{rec.name}: rate {rates[i]} given for a FLAC record of {rec.rate} Hz')
+    rates = [enc[i].rate if i in enc else audio.as_rate(target_sr if r is None else r) for i, r in enumerate(rates)]
+    flac = None
+    if enc:                                                        # scan + chain: one device-to-host copy, one sync
+        flac = audio.FlacBatch(list(enc.values()), eng.device)
+    slot = {i: k for k, i in enumerate(enc)}                       # recording -> its index in the FlacBatch
+    native_lens = [flac.lengths[slot[i]] if i in enc else int(w.shape[0]) for i, w in enumerate(waves)]
+    lens = [audio.resampled_length(n, r, target_sr) for n, r in zip(native_lens, rates)]
+    bases = np.zeros(len(waves) + 1, dtype=np.int64)
+    np.cumsum([(n + 3) & ~3 for n in lens], out=bases[1:])
+    wave_d = torch.empty(max(int(bases[-1]), 4), dtype=torch.float32, device=eng.device)
+    for w, b, n, r in zip(waves, bases, lens, rates):
+        if n and r == target_sr and w is not None:
+            src = torch.from_numpy(w)
+            wave_d[b:b + n].copy_(src, non_blocking=src.is_pinned())
+    flac_status = []
+    direct = {slot[i]: int(bases[i]) for i in enc if rates[i] == target_sr}
+    if direct:
+        flac_status.append(flac.emit(wave_d, direct))
+    for r in sorted(set(rates) - {target_sr}):                # one resampling launch per native rate
+        group = [i for i, ri in enumerate(rates) if ri == r]
+        starts = np.zeros(len(group) + 1, dtype=np.int64)
+        np.cumsum([native_lens[i] for i in group], out=starts[1:])
+        native_d = torch.empty(max(int(starts[-1]), 1), dtype=torch.float32, device=eng.device)
+        for i, a in zip(group, starts):
+            if i not in enc:
+                native_d[a:a + native_lens[i]].copy_(torch.from_numpy(waves[i]))
+        to_decode = {slot[i]: int(a) for i, a in zip(group, starts) if i in enc}
+        if to_decode:
+            flac_status.append(flac.emit(native_d, to_decode))
+        audio.resample_into(native_d, starts[:-1].tolist(), [native_lens[i] for i in group], wave_d,
+                            [int(bases[i]) for i in group], r, target_sr)
+    return wave_d, bases, lens, flac_status
+
+
 def transcribe_recordings(infer_ins, waveforms: Sequence, slicer: Optional[Slicer] = None,
                           rates: Optional[Sequence[Optional[int]]] = None):
     """[(chunk offsets in seconds, per-chunk notes)] for several mono recordings, as ONE var-len batch.
@@ -180,53 +264,12 @@ def transcribe_recordings(infer_ins, waveforms: Sequence, slicer: Optional[Slice
     target_sr = int(infer_ins.config['audio_sample_rate'])
     slicer = slicer or Slicer(sr=target_sr, max_sil_kept=1000)                                 # batch_infer.py:52
     quantized = bool(getattr(infer_ins, 'quantized', False))
-    enc = {i: w for i, w in enumerate(waveforms) if isinstance(w, audio.EncodedAudio)}
-    waves = [None if i in enc else np.ascontiguousarray(w, dtype=np.float32) for i, w in enumerate(waveforms)]
-    for w in waves:
-        assert w is None or w.ndim == 1, 'mono recordings expected (librosa.load(..., mono=True), batch_infer.py:51)'
-    if rates is None:
-        rates = [None] * len(waves)
-    assert len(rates) == len(waves), 'one rate per recording'
-    for i, rec in enc.items():
-        if rates[i] is not None and audio.as_rate(rates[i]) != rec.rate:
-            raise ValueError(f'{rec.name}: rate {rates[i]} given for a FLAC record of {rec.rate} Hz')
-    rates = [enc[i].rate if i in enc else audio.as_rate(target_sr if r is None else r) for i, r in enumerate(rates)]
-    flac = None
-    if enc:                                                        # scan + chain: one device-to-host copy, one sync
-        with torch.cuda.device(eng.device):
-            flac = audio.FlacBatch(list(enc.values()), eng.device)
-    slot = {i: k for k, i in enumerate(enc)}                       # recording -> its index in the FlacBatch
-    native_lens = [flac.lengths[slot[i]] if i in enc else int(w.shape[0]) for i, w in enumerate(waves)]
-    lens = [audio.resampled_length(n, r, target_sr) for n, r in zip(native_lens, rates)]
-    bases = np.zeros(len(waves) + 1, dtype=np.int64)
-    np.cumsum([(n + 3) & ~3 for n in lens], out=bases[1:])
     lock = getattr(infer_ins, '_lock', None)
     if lock is not None:
         lock.acquire()
     try:
         with torch.cuda.device(eng.device):
-            wave_d = torch.empty(max(int(bases[-1]), 4), dtype=torch.float32, device=eng.device)
-            for w, b, n, r in zip(waves, bases, lens, rates):
-                if n and r == target_sr and w is not None:
-                    src = torch.from_numpy(w)
-                    wave_d[b:b + n].copy_(src, non_blocking=src.is_pinned())
-            flac_status = []
-            direct = {slot[i]: int(bases[i]) for i in enc if rates[i] == target_sr}
-            if direct:
-                flac_status.append(flac.emit(wave_d, direct))
-            for r in sorted(set(rates) - {target_sr}):                # one resampling launch per native rate
-                group = [i for i, ri in enumerate(rates) if ri == r]
-                starts = np.zeros(len(group) + 1, dtype=np.int64)
-                np.cumsum([native_lens[i] for i in group], out=starts[1:])
-                native_d = torch.empty(max(int(starts[-1]), 1), dtype=torch.float32, device=eng.device)
-                for i, a in zip(group, starts):
-                    if i not in enc:
-                        native_d[a:a + native_lens[i]].copy_(torch.from_numpy(waves[i]))
-                to_decode = {slot[i]: int(a) for i, a in zip(group, starts) if i in enc}
-                if to_decode:
-                    flac_status.append(flac.emit(native_d, to_decode))
-                audio.resample_into(native_d, starts[:-1].tolist(), [native_lens[i] for i in group], wave_d,
-                                    [int(bases[i]) for i in group], r, target_sr)
+            wave_d, bases, lens, flac_status = stage_recordings(eng, target_sr, waveforms, rates)
             need = [i for i, n in enumerate(lens) if (n + slicer.hop_size - 1) // slicer.hop_size > slicer.min_length]
             rms_lists = eng.rms_frames_many([wave_d[bases[i]:bases[i] + lens[i]] for i in need], slicer.win_size, slicer.hop_size)
             per_rec: List[List[Tuple[int, int]]] = [[(0, n)] for n in lens]               # slicer2.py:79-80 (short: one chunk)
@@ -264,6 +307,48 @@ def load_wav(path, sr: int) -> np.ndarray:
     return np.ascontiguousarray(x, dtype=np.float32)
 
 
+def load_groups(todo: Sequence[Tuple[object, pathlib.Path]], load_audio: Callable, sr: int, max_frames_per_batch: int,
+                workers: int):
+    """Reads the audio of ``todo = [(key, path), ...]`` with ``load_audio(path, sr)`` on a thread pool and yields groups
+    ``[(key, waveform or EncodedAudio, native rate or None), ...]`` of about ``max_frames_per_batch`` frames, in order, to be
+    run as one var-len batch each: decoding overlaps the GPU work on the previous group.  Only a bounded window of decoded
+    recordings is ever held (the reference streams one file at a time; an unbounded list of futures would keep the whole
+    dataset's audio in host memory)."""
+    import collections
+    with concurrent.futures.ThreadPoolExecutor(max_workers=workers) as pool:
+        window = max(2 * workers, 4)
+        pending: 'collections.deque' = collections.deque()
+        it = iter(todo)
+
+        def refill():
+            while len(pending) < window:
+                nxt = next(it, None)
+                if nxt is None:
+                    return
+                pending.append((nxt[0], pool.submit(load_audio, nxt[1], sr)))
+
+        group: List[tuple] = []
+        frames = 0
+        refill()
+        while pending:
+            key, fut = pending.popleft()
+            wave = fut.result()
+            if isinstance(wave, audio.EncodedAudio):                   # decoded on the device; its rate is its own
+                rate, n = None, wave.length * int(sr) // wave.rate
+            else:
+                wave, rate = wave if isinstance(wave, tuple) else (wave, sr)
+                n = audio.resampled_length(len(wave), audio.as_rate(rate), int(sr))
+            refill()
+            t = 1 + n // 512
+            if group and frames + t > max_frames_per_batch:
+                yield group
+                group, frames = [], 0
+            group.append((key, wave, rate))
+            frames += t
+        if group:
+            yield group
+
+
 def batch_infer_dataset(dataset, infer_ins, config: dict, round_midi: bool = False, csv=None, overwrite: bool = False,
                         load_audio: Callable = load_wav, max_frames_per_batch: int = 400_000, workers: int = 4) -> pathlib.Path:
     """batch_infer.py's command (:149-226) with dataset-level batching.  ``dataset`` = DiffSinger raw data dir with
@@ -288,48 +373,10 @@ def batch_infer_dataset(dataset, infer_ins, config: dict, round_midi: bool = Fal
             print(f'WARNING: audio file does not exist: \'{wav_path}\'')
             continue
         todo.append((row, wav_path))
-    with concurrent.futures.ThreadPoolExecutor(max_workers=workers) as pool:
-        # decoding overlaps the GPU work below; only a bounded window of decoded recordings is ever held (the reference
-        # streams one file at a time; an unbounded list of futures would keep the whole dataset's audio in host memory)
-        import collections
-        window = max(2 * workers, 4)
-        pending: 'collections.deque' = collections.deque()
-        it = iter(todo)
-
-        def refill():
-            while len(pending) < window:
-                nxt = next(it, None)
-                if nxt is None:
-                    return
-                pending.append((nxt[0], pool.submit(load_audio, nxt[1], sr)))
-
-        group: List[Tuple[dict, np.ndarray, int]] = []
-        frames = 0
-
-        def flush():
-            nonlocal group, frames
-            if group:
-                results = transcribe_recordings(infer_ins, [w for _, w, _ in group], rates=[r for _, _, r in group])
-                for (row, _, _), (offsets, segments) in zip(group, results):
-                    row['note_seq'], row['note_dur'] = row_notes(row['ph_dur'], row['ph_num'], note_timeline(offsets, segments), round_midi)
-            group, frames = [], 0
-
-        refill()
-        while pending:
-            row, fut = pending.popleft()
-            wave = fut.result()
-            if isinstance(wave, audio.EncodedAudio):                   # decoded on the device; its rate is its own
-                rate, n = None, wave.length * int(sr) // wave.rate
-            else:
-                wave, rate = wave if isinstance(wave, tuple) else (wave, sr)
-                n = audio.resampled_length(len(wave), audio.as_rate(rate), int(sr))
-            refill()
-            t = 1 + n // 512
-            if group and frames + t > max_frames_per_batch:
-                flush()
-            group.append((row, wave, rate))
-            frames += t
-        flush()
+    for group in load_groups(todo, load_audio, sr, max_frames_per_batch, workers):
+        results = transcribe_recordings(infer_ins, [w for _, w, _ in group], rates=[r for _, _, r in group])
+        for (row, _, _), (offsets, segments) in zip(group, results):
+            row['note_seq'], row['note_dur'] = row_notes(row['ph_dur'], row['ph_num'], note_timeline(offsets, segments), round_midi)
     with open(csv_path, 'w', encoding='utf8', newline='') as f:
         writer = DictWriter(f, fieldnames=['name', 'ph_seq', 'ph_dur', 'ph_num', 'note_seq', 'note_dur'])
         writer.writeheader()

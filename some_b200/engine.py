@@ -16,7 +16,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Dict, List, Optional, Sequence
+from typing import Callable, Dict, List, Optional, Sequence
 
 import numpy as np
 import torch
@@ -412,7 +412,7 @@ class Engine:
         return cu, layout, off
 
     def enqueue(self, waveforms: Sequence[np.ndarray], quantized: bool = False, return_intermediates: bool = False,
-                resident=None, out: Optional[torch.Tensor] = None):
+                resident=None, out: Optional[torch.Tensor] = None, logits_hook: Optional[Callable] = None):
         """Stages, copies and enqueues the whole batch WITHOUT synchronising.  Returns (device slab uint8 [nbytes], cu, layout,
         extra): the decoded notes land in the device slab (see slab_layout); the caller copies it to the host (infer) or
         hands it to the all-gather (dist.infer_sharded).
@@ -427,7 +427,13 @@ class Engine:
 
         ``resident = (wave_d, ranges)``: the audio is already on the device (f32 tensor) and the clips are the sample ranges
         ``[(begin, end), ...]`` inside it (``waveforms`` is ignored): no staging, no audio H2D — the slicer path
-        (infer_sliced) cuts the recording where it lies."""
+        (infer_sliced) cuts the recording where it lies.
+
+        ``logits_hook``: optional ``hook(ws, c0, c1, mc, cu_d)``, enqueued for every pipeline chunk (clips c0..c1, mc frames,
+        chunk-relative cu_frames cu_d) between the trunk and the decode.  With a hook the trunk writes the raw logits
+        (SOME_EPI_BIAS_F32) into ``ws.probs[:mc]`` and the hook must leave there the probabilities the decode reads
+        (some_eval_clips does both in one pass: the evaluator, some_b200/evaluate.py).  Without one (the default) the trunk
+        applies the sigmoid / softmax head itself."""
         dev = self.device
         if resident is not None:
             wave_res, ranges = resident
@@ -525,13 +531,17 @@ class Engine:
                 self.run_mel(wave_d[lo:], tab_dev[:bc], tab_dev[bc:2 * bc], cu_d, bc, max_frames, mel_f32, ws.units)
                 was = self.lib.some_set_pdl(1) if pdl else 0    # programmatic dependent launch of the trunk kernels
                 try:
-                    self.run_trunk(ws, mc, bc, cu_d, max_frames, 'softmax' if quantized else 'sigmoid')
+                    self.run_trunk(ws, mc, bc, cu_d, max_frames,
+                                   'logits' if logits_hook is not None else 'softmax' if quantized else 'sigmoid')
                 finally:
                     if pdl:
                         self.lib.some_set_pdl(was)
+                if logits_hook is not None:
+                    logits_hook(ws, c0, c1, mc, cu_d)
                 self.run_decode(ws, mc, bc, cu_d, note_count, quantized, out=(note_midi, note_dur, note_rest))
 
-            if mc <= self.GRAPH_MAX_FRAMES and self.use_graphs and self.prof is None and not return_intermediates:
+            if (mc <= self.GRAPH_MAX_FRAMES and self.use_graphs and self.prof is None and not return_intermediates
+                    and logits_hook is None):
                 # small batches are launch-bound (~56 launches of a few microseconds each): replay them as ONE CUDA graph,
                 # keyed by everything the captured kernel arguments depend on
                 self._graphed((wave_d.data_ptr() + 4 * lo, tab_dev.data_ptr(), cu_d.data_ptr(), o.data_ptr(), ws.serial, bc, mc,
@@ -639,38 +649,49 @@ class Engine:
         csrc/accurate.cu) — no bf16, no tensor cores, exact activations.  Asserts the "within 1e-3 fp32" line of the contract
         (tests/test_gpu_accurate.py) and shows that operand rounding is the only source of note differences in the product
         path.  ~100x slower than infer(); one clip at a time; returns mel / probs / bounds with the notes."""
-        from .weights import build_f32_model
         dev = self.device
         out = []
         with torch.cuda.device(dev):
-            if self._f32 is None:
-                self._f32 = build_f32_model(self._state_dict, self.config, dev)
-            cmodel = self._f32[0]
-            head = _lib.EPI_SOFTMAX_F32 if quantized else _lib.EPI_SIGMOID_F32
             for w in waveforms:
                 host, tables, cu = self.pack([w])
-                m = int(cu[-1])
-                wave_d, tab_d, cu_d = host.to(dev), tables.to(dev), torch.from_numpy(cu).to(dev)
-                f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
-                t = {'x': f(2, m, DIM), 'a': f(2, m, DIM), 'h': f(2, m, FFN_DIM), 'qkv': f(2, m, 3 * DIM), 'g': f(2, m, DIM),
-                     'y': f(2, m, 2 * DIM), 'units': f(m, 80), 'probs': f(m, self.outdim), 'bounds': f(m)}
-                c = _lib.WorkspaceF32C()
-                for s in range(2):
-                    for k in ('x', 'a', 'h', 'qkv', 'g', 'y'):
-                        getattr(c, k)[s] = t[k][s].data_ptr()
-                c.units, c.probs, c.bounds = t['units'].data_ptr(), t['probs'].data_ptr(), t['bounds'].data_ptr()
-                self.run_mel(wave_d, tab_d[:1], tab_d[1:], cu_d, 1, m, t['units'], None)
-                _lib.check(self.lib.some_forward_f32(C.byref(cmodel), C.byref(c), m, 1, cu_d.data_ptr(), m, head, self._stream),
-                           'some_forward_f32')
-                ws = self.workspace(m)
-                nc = torch.empty(1, dtype=torch.int32, device=dev)
-                self.run_decode(ws, m, 1, cu_d, nc, quantized, probs=t['probs'], bounds=t['bounds'])
-                n = int(nc.item())
+                wave_d, tab_d = host.to(dev), tables.to(dev)
+                t, ws, n = self.accurate_clip(wave_d, tab_d[:1], tab_d[1:], int(cu[-1]), quantized)
                 out.append({'note_midi': ws.note_midi[:n].cpu().numpy(),
                             'note_dur': ws.note_dur[:n].cpu().numpy().astype(np.int64) * self.timestep,
                             'note_rest': ws.note_rest[:n].cpu().numpy().astype(bool),
                             'mel': t['units'].cpu().numpy(), 'probs': t['probs'].cpu().numpy(), 'bounds': t['bounds'].cpu().numpy()})
         return out
+
+    def accurate_clip(self, wave_d: torch.Tensor, start_d: torch.Tensor, len_d: torch.Tensor, m: int, quantized: bool,
+                      logits_hook: Optional[Callable] = None):
+        """One clip (samples wave_d[start : start + len], int64 device scalars; m frames) through mel -> some_forward_f32 ->
+        decode, on the current device.  Returns (the fp32 tensors {units, probs, bounds, ...}, the workspace holding the notes
+        at rows [0, n), n).  ``logits_hook(t, cu_d)``: as in enqueue(), run between the trunk (which then writes raw logits
+        into t['probs']) and the decode."""
+        from .weights import build_f32_model
+        dev = self.device
+        if self._f32 is None:
+            self._f32 = build_f32_model(self._state_dict, self.config, dev)
+        cmodel = self._f32[0]
+        head = _lib.EPI_BIAS_F32 if logits_hook is not None else _lib.EPI_SOFTMAX_F32 if quantized else _lib.EPI_SIGMOID_F32
+        cu_d = torch.tensor([0, m], dtype=torch.int32, device=dev)
+        f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
+        t = {'x': f(2, m, DIM), 'a': f(2, m, DIM), 'h': f(2, m, FFN_DIM), 'qkv': f(2, m, 3 * DIM), 'g': f(2, m, DIM),
+             'y': f(2, m, 2 * DIM), 'units': f(m, 80), 'probs': f(m, self.outdim), 'bounds': f(m)}
+        c = _lib.WorkspaceF32C()
+        for s in range(2):
+            for k in ('x', 'a', 'h', 'qkv', 'g', 'y'):
+                getattr(c, k)[s] = t[k][s].data_ptr()
+        c.units, c.probs, c.bounds = t['units'].data_ptr(), t['probs'].data_ptr(), t['bounds'].data_ptr()
+        self.run_mel(wave_d, start_d, len_d, cu_d, 1, m, t['units'], None)
+        _lib.check(self.lib.some_forward_f32(C.byref(cmodel), C.byref(c), m, 1, cu_d.data_ptr(), m, head, self._stream),
+                   'some_forward_f32')
+        if logits_hook is not None:
+            logits_hook(t, cu_d)
+        ws = self.workspace(m)
+        nc = torch.empty(1, dtype=torch.int32, device=dev)
+        self.run_decode(ws, m, 1, cu_d, nc, quantized, probs=t['probs'], bounds=t['bounds'])
+        return t, ws, int(nc.item())
 
     def unpack(self, cu, nc, nm, nd, nr, extra=None) -> List[Dict[str, np.ndarray]]:
         # The slab has room for one note per FRAME (notes of clip j start at row cu[j]); only ~1 row in 5 is used.  Gather the

@@ -164,3 +164,94 @@ def write_checkpoint(directory, config: dict, seed: int = 1234) -> pathlib.Path:
     with open(directory / 'config.yaml', 'w', encoding='utf8') as f:
         yaml.safe_dump(config, f, sort_keys=False, allow_unicode=True)
     return path
+
+
+def synth_labelled(seed: int, seconds: float, sr: int = SR):
+    """Seeded sung-note waveform together with the DiffSinger labels the generator used: returns
+    ``(waveform f32, {'note_seq': [...], 'note_dur': [...], 'note_slur': [...]})``.  Notes last U(0.12, 0.7) s (durations
+    rounded to 0.1 ms, the last one cut so that they sum to ``seconds``), pitch is a random walk in [48, 72] MIDI with a
+    cent offset on one note in four, one note in seven is a rest and one in five a slur of the note before it (within a
+    semitone).  Rendering as in ``synth_waveform``: 6 harmonics, 5.5 Hz vibrato, 10 ms note edges, peak 0.5, noise at
+    -50 dBFS."""
+    from .batch import midi_to_note
+    rng = np.random.default_rng(seed)
+    names, durs, slurs, pitches = [], [], [], []
+    total, pitch = 0.0, float(rng.integers(55, 66))
+    while total < seconds - 1e-4:
+        d = min(round(float(rng.uniform(0.12, 0.7)), 4), round(seconds - total, 4))
+        slur = bool(names) and names[-1] != 'rest' and rng.random() < 0.2
+        if slur:
+            p = pitches[-1] + float(rng.choice([-1.0, -0.25, 0.0, 0.25, 1.0]))
+        elif rng.random() < 1 / 7 and names and names[-1] != 'rest':
+            p = None
+        else:
+            pitch = float(np.clip(pitch + rng.integers(-4, 5), 48, 72))
+            p = pitch + (float(rng.choice([-0.25, 0.25, 0.4])) if rng.random() < 0.25 else 0.0)
+        names.append('rest' if p is None else midi_to_note(p, cents=True))
+        pitches.append(p)
+        durs.append(d)
+        slurs.append(int(slur))
+        total = round(total + d, 4)
+    n = int(round(seconds * sr))
+    out = np.zeros(n, dtype=np.float64)
+    phase = np.zeros(6)
+    t0 = 0
+    acc = 0.0
+    for p, d in zip(pitches, durs):
+        acc += d
+        t1 = min(n, int(round(acc * sr)))
+        m = t1 - t0
+        if p is not None and m > 0:
+            tt = (np.arange(m) + t0) / sr
+            f = 440.0 * 2.0 ** ((p - 69.0 + 0.3 * np.sin(2 * np.pi * 5.5 * tt)) / 12.0)
+            base = np.cumsum(2 * np.pi * f / sr)
+            seg = np.zeros(m)
+            for k in range(1, 7):
+                seg += np.sin(phase[k - 1] + k * base) / k
+                phase[k - 1] = (phase[k - 1] + k * base[-1]) % (2 * np.pi)
+            edge = min(int(0.010 * sr), m // 2)
+            env = np.ones(m)
+            if edge > 0:
+                ramp = 0.5 - 0.5 * np.cos(np.pi * np.arange(edge) / edge)
+                env[:edge] = ramp
+                env[m - edge:] = ramp[::-1]
+            out[t0:t1] = seg * env
+        t0 = t1
+    peak = np.abs(out).max()
+    if peak > 0:
+        out *= 0.5 / peak
+    out += rng.standard_normal(n) * (10.0 ** (-50.0 / 20.0))
+    return out.astype(np.float32), {'note_seq': names, 'note_dur': durs, 'note_slur': slurs}
+
+
+def write_wav16(path, samples: np.ndarray, sr: int = SR) -> np.ndarray:
+    """Writes mono 16-bit PCM; returns the samples as librosa.load reads them back (int16 / 32768)."""
+    import wave
+    q = np.clip(np.round(np.asarray(samples, dtype=np.float64) * 32768.0), -32768, 32767).astype('<i2')
+    with wave.open(str(path), 'wb') as f:
+        f.setnchannels(1)
+        f.setsampwidth(2)
+        f.setframerate(int(sr))
+        f.writeframes(q.tobytes())
+    return (q.astype(np.float32) / np.float32(32768.0)).astype(np.float32)
+
+
+def write_labelled_dataset(directory, items, sr: int = SR) -> pathlib.Path:
+    """A DiffSinger raw data directory (``transcriptions.csv``, ``wavs/{name}.wav`` as 16-bit PCM, ``wavs/{name}.ds``) from
+    ``items = [(name, waveform, labels), ...]`` with labels as ``synth_labelled`` returns them (extra keys, e.g.
+    ``note_glide``, are written to the .ds as well)."""
+    import csv
+    import json
+    directory = pathlib.Path(directory)
+    (directory / 'wavs').mkdir(parents=True, exist_ok=True)
+    with open(directory / 'transcriptions.csv', 'w', encoding='utf8', newline='') as f:
+        w = csv.writer(f)
+        w.writerow(['name', 'ph_seq', 'ph_dur', 'ph_num'])
+        for name, wave_, lab in items:
+            secs = sum(lab['note_dur'])
+            w.writerow([name, 'SP', f'{secs:.4f}', '1'])
+            write_wav16(directory / 'wavs' / f'{name}.wav', wave_, sr)
+            ds = {k: ' '.join(str(x) for x in v) if isinstance(v, (list, tuple)) else v for k, v in lab.items()}
+            with open(directory / 'wavs' / f'{name}.ds', 'w', encoding='utf8') as g:
+                json.dump(ds, g)
+    return directory
