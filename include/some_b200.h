@@ -30,7 +30,7 @@ extern "C" {
 typedef struct CUstream_st* cudaStream_t;
 #endif
 
-/* Model geometry the kernels are specialised for (all shipped configs: configs/*.yaml). */
+/* Model geometry the kernels are specialised for (all shipped configs under configs/). */
 #define SOME_DIM 512
 #define SOME_HEADS 8
 #define SOME_HEAD_DIM 64
@@ -510,6 +510,62 @@ typedef struct {
 } some_workspace_f32;
 int some_forward_f32(const some_model_f32* model, const some_workspace_f32* ws, int M, int B, const int32_t* cu_frames,
                      int max_frames, int head, cudaStream_t stream);
+
+/* ---- Native inference session (csrc/session.cu): the export/deployment path of the reference (export.py + deployment/) for
+ * hosts without Python.  `python -m some_b200.export --model CKPT` writes a checkpoint, its load-time bias correction applied
+ * (Engine.calibrate), into one self-contained model file (format: INTEGRATION.md "Deploying without Python"); a session opens
+ * that file and transcribes recordings with the kernels above, enqueued in the order of some_b200/engine.py, so its notes are
+ * bit-identical to plugin.infer() / Engine.infer_sliced.  Host memory in, host memory out; the session owns its streams and
+ * buffers, and calls on one session are serialised on a mutex (several threads may share it, each with its own result).
+ *
+ * some_session_open       reads and validates the whole file before any CUDA call (magic, format version, ABI, directory
+ *                         bounds, every tensor present with the shape implied by lay / outdim, file size); refuses a device
+ *                         that is not sm_90; uploads the weights.  < 0 on failure, some_last_error() names the file and problem.
+ * some_session_transcribe B mono float32 clips at the model's sample rate -> one entry per clip in `out`, in input order.  The
+ *                         clips are staged through pinned memory; the upload of each pipeline chunk overlaps the kernels of
+ *                         the previous one (Engine.enqueue).  Clips are independent: results do not depend on the batch.
+ * some_session_transcribe_sliced
+ *                         one mono recording at any integer rate (resampled on the device as librosa.load does when the rate
+ *                         differs; too-short inputs are refused as resampy does), cut by the silence slicer (params NULL:
+ *                         Slicer(sr, max_sil_kept=1000) as in infer.py) and transcribed where it lies: one entry per chunk,
+ *                         with its sample range in the (resampled) recording.
+ * some_notes_get          a clip's notes: note_midi f32, note_dur in frames (seconds = dur * timestep, the float64 product of
+ *                         me_infer.py:95), note_rest u8; the pointers stay valid until the next call that fills `n`. */
+typedef struct some_session some_session;
+typedef struct some_notes some_notes;
+typedef struct {
+  int sample_rate, hop, outdim, quantized, bias_corrected;
+  double timestep; /* hop / sample_rate */
+} some_session_info;
+/* Slicer constructor arguments (utils/slicer2.py), in milliseconds / dB like Slicer(sr, threshold, min_length, min_interval,
+ * hop_size, max_sil_kept) */
+typedef struct {
+  double threshold_db, min_length_ms, min_interval_ms, hop_size_ms, max_sil_kept_ms;
+} some_slicer_params;
+/* ... and the frame counts Slicer derives from them (Python's round, half to even) */
+typedef struct {
+  float threshold; /* 10^(dB / 20) rounded to float32: `rms < threshold` compares in float32 */
+  int hop_size, win_size, min_length, min_interval, max_sil_kept;
+} some_slicer_frames;
+
+int some_session_open(const char* path, int device, some_session** out);
+int some_session_close(some_session* s);
+int some_session_get_info(const some_session* s, some_session_info* info);
+int some_session_transcribe(some_session* s, const float* const* clips, const int64_t* lens, int B, some_notes* out);
+int some_session_transcribe_sliced(some_session* s, const float* samples, long long n, int sample_rate,
+                                   const some_slicer_params* params, some_notes* out);
+int some_notes_create(some_notes** out);
+int some_notes_destroy(some_notes* n);
+int some_notes_clips(const some_notes* n); /* number of clips / chunks (< 0: error) */
+int some_notes_get(const some_notes* n, int clip, int* count, const float** note_midi, const int32_t** note_dur,
+                   const uint8_t** note_rest, int64_t* begin, int64_t* end); /* any output pointer may be NULL */
+/* The slicer's decisions on the HOST (no CUDA call): some_slicer_derive fills the frame counts for a sample rate (params NULL:
+ * the session's defaults); some_slicer_ranges turns the RMS list of a recording of n_samples samples (some_slicer_rms) into the
+ * [begin, end) sample ranges of its chunks, ranges[2 k], ranges[2 k + 1] (silence_tags + chunk_ranges of some_b200/slicer.py).
+ * *count = the number of ranges; capacity n_frames / 2 + 2 always suffices. */
+int some_slicer_derive(int sample_rate, const some_slicer_params* params, some_slicer_frames* out);
+int some_slicer_ranges(const float* rms, int n_frames, long long n_samples, const some_slicer_frames* frames, int64_t* ranges,
+                       int capacity, int* count);
 
 #ifdef __cplusplus
 }

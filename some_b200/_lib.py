@@ -117,6 +117,21 @@ class WorkspaceF32C(C.Structure):
                 ('units', _vp), ('probs', _vp), ('bounds', _vp)]
 
 
+class SessionInfo(C.Structure):
+    _fields_ = [('sample_rate', C.c_int), ('hop', C.c_int), ('outdim', C.c_int), ('quantized', C.c_int),
+                ('bias_corrected', C.c_int), ('timestep', C.c_double)]
+
+
+class SlicerParams(C.Structure):
+    _fields_ = [('threshold_db', C.c_double), ('min_length_ms', C.c_double), ('min_interval_ms', C.c_double),
+                ('hop_size_ms', C.c_double), ('max_sil_kept_ms', C.c_double)]
+
+
+class SlicerFrames(C.Structure):
+    _fields_ = [('threshold', C.c_float), ('hop_size', C.c_int), ('win_size', C.c_int), ('min_length', C.c_int),
+                ('min_interval', C.c_int), ('max_sil_kept', C.c_int)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     'some_version': (C.c_int, []),
@@ -156,6 +171,19 @@ EXPORTS = {
     'some_profiler_destroy': (C.c_int, [_vp]),
     'some_profiler_reset': (C.c_int, [_vp]),
     'some_profiler_read': (C.c_int, [_vp, C.c_int, C.POINTER(ProfileRecord)]),
+    'some_session_open': (C.c_int, [C.c_char_p, C.c_int, C.POINTER(_vp)]),
+    'some_session_close': (C.c_int, [_vp]),
+    'some_session_get_info': (C.c_int, [_vp, C.POINTER(SessionInfo)]),
+    'some_session_transcribe': (C.c_int, [_vp, _vp, _vp, C.c_int, _vp]),
+    'some_session_transcribe_sliced': (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.POINTER(SlicerParams), _vp]),
+    'some_notes_create': (C.c_int, [C.POINTER(_vp)]),
+    'some_notes_destroy': (C.c_int, [_vp]),
+    'some_notes_clips': (C.c_int, [_vp]),
+    'some_notes_get': (C.c_int, [_vp, C.c_int, C.POINTER(C.c_int), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp),
+                                 C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    'some_slicer_derive': (C.c_int, [C.c_int, C.POINTER(SlicerParams), C.POINTER(SlicerFrames)]),
+    'some_slicer_ranges': (C.c_int, [_vp, C.c_int, C.c_longlong, C.POINTER(SlicerFrames), _vp, C.c_int,
+                                     C.POINTER(C.c_int)]),
 }
 
 _lib = None

@@ -1,0 +1,898 @@
+// Native inference session: a model file written by `python -m some_b200.export` in, notes out, with no Python or torch in
+// between.  Host code only; the work is done by the sm_90a kernels of this library, enqueued in the order Engine.enqueue
+// (some_b200/engine.py) and Engine.infer_sliced use:
+//   [some_resample_kaiser] -> [some_slicer_rms + the slicer's decisions on the host] -> per pipeline chunk:
+//   some_mel_logmel -> some_forward (stand-alone LayerNorms, sigmoid / softmax head) -> some_decode_notes.
+//
+// The model file (little-endian; INTEGRATION.md "Deploying without Python" has the table):
+//   header     128 bytes: magic "SOMEB200", format version, ABI number, file size, directory offset, tensor count, the scalars
+//              of the model (lay, outdim, quantized, sample rate, hop, win, midi_min, midi_max, midi_prob_deviation,
+//              rest_threshold, bias correction applied) and the offset of the data section
+//   directory  128 bytes per tensor: name (NUL-padded, 64 bytes), dtype, ndim, shape[4], offset, byte length
+//   data       every tensor at a 256-byte aligned offset; the data section is uploaded as one block
+// The whole file is read and validated before any CUDA call.
+#include "host_common.h"
+
+#include <math.h>
+#include <stdio.h>
+#include <string.h>
+
+#include <algorithm>
+#include <condition_variable>
+#include <functional>
+#include <map>
+#include <memory>
+#include <mutex>
+#include <string>
+#include <thread>
+#include <vector>
+
+#include "../../include/some_b200.h"
+
+using namespace some;
+
+namespace {
+
+constexpr char kMagic[8] = {'S', 'O', 'M', 'E', 'B', '2', '0', '0'};
+constexpr uint32_t kFormat = 1;
+constexpr uint64_t kHeaderBytes = 128, kEntryBytes = 128, kAlign = 256;
+constexpr int kNameBytes = 64;
+enum { DT_F32 = 1, DT_BF16 = 2, DT_I32 = 3, DT_F64 = 4 };
+constexpr int kKaiserTaps = 32769;   // resampy kaiser_best: 64 zero crossings x 512 + 1
+
+// Engine's pipeline split (engine.py CHUNK_FRACTIONS / MIN_CHUNK_FRAMES): a small first chunk gets the GPU going while the
+// next chunk is staged and copied.
+constexpr double kChunkFractions[2] = {0.125, 0.375};
+constexpr int kMinChunkFrames = 16384;
+
+template <class T>
+T rd(const uint8_t* p) {
+  T v;
+  memcpy(&v, p, sizeof(T));
+  return v;
+}
+
+int dtype_bytes(uint32_t dt) { return dt == DT_F32 || dt == DT_I32 ? 4 : dt == DT_BF16 ? 2 : dt == DT_F64 ? 8 : 0; }
+const char* dtype_name(uint32_t dt) {
+  return dt == DT_F32 ? "f32" : dt == DT_BF16 ? "bf16" : dt == DT_I32 ? "i32" : dt == DT_F64 ? "f64" : "?";
+}
+
+struct Spec {
+  std::string name;
+  uint32_t dtype;
+  std::vector<uint64_t> shape;
+};
+
+// The tensors a file of this geometry must hold (some_b200/export.py: tensor_specs writes the same list).
+std::vector<Spec> expected_tensors(int lay, int outdim) {
+  const uint64_t D = SOME_DIM, F = 4 * SOME_DIM;
+  std::vector<Spec> v;
+  for (int s = 0; s < 2; ++s) {
+    v.push_back({"w_in." + std::to_string(s), DT_BF16, {D, SOME_N_MELS}});
+    v.push_back({"b_in." + std::to_string(s), DT_F32, {D}});
+  }
+  for (int j = 0; j < 2 * (lay + 1); ++j) {
+    const std::string p = "blk" + std::to_string(j) + ".";
+    for (int k = 0; k < 5; ++k) {
+      v.push_back({p + "ln_g." + std::to_string(k), DT_F32, {D}});
+      v.push_back({p + "ln_b." + std::to_string(k), DT_F32, {D}});
+    }
+    for (int k = 0; k < 2; ++k) {
+      const std::string q = "." + std::to_string(k);
+      v.push_back({p + "ffn_w1" + q, DT_BF16, {F, D}});
+      v.push_back({p + "ffn_b1" + q, DT_F32, {F}});
+      v.push_back({p + "ffn_w2" + q, DT_BF16, {D, F}});
+      v.push_back({p + "ffn_b2" + q, DT_F32, {D}});
+    }
+    v.push_back({p + "w_qkv", DT_BF16, {3 * D, D}});
+    v.push_back({p + "w_out", DT_BF16, {D, D}});
+    v.push_back({p + "b_out", DT_F32, {D}});
+    v.push_back({p + "w_pw1", DT_BF16, {2 * D, D}});
+    v.push_back({p + "b_pw1", DT_F32, {2 * D}});
+    v.push_back({p + "w_dw", DT_F32, {SOME_CONV_K, D}});
+    v.push_back({p + "b_dw", DT_F32, {D}});
+    v.push_back({p + "w_pw2", DT_BF16, {D, D}});
+    v.push_back({p + "b_pw2", DT_F32, {D}});
+  }
+  for (int j = 0; j < 2 * lay; ++j) {
+    v.push_back({"glu" + std::to_string(j) + ".w", DT_BF16, {2 * D, D}});
+    v.push_back({"glu" + std::to_string(j) + ".b", DT_F32, {2 * D}});
+  }
+  v.push_back({"w_head", DT_BF16, {static_cast<uint64_t>(outdim), D}});
+  v.push_back({"b_head", DT_F32, {static_cast<uint64_t>((outdim + 31) / 32 * 32)}});
+  v.push_back({"w_cut", DT_F32, {D}});
+  v.push_back({"b_cut", DT_F32, {1}});
+  v.push_back({"mel_start", DT_I32, {SOME_N_MELS}});
+  v.push_back({"mel_count", DT_I32, {SOME_N_MELS}});
+  v.push_back({"mel_weights", DT_F32, {SOME_N_MELS, SOME_MEL_MAXW}});
+  v.push_back({"twiddle", DT_F32, {SOME_MEL_TW, 2}});
+  v.push_back({"window", DT_F32, {SOME_N_FFT}});
+  v.push_back({"kaiser_best", DT_F64, {kKaiserTaps}});
+  return v;
+}
+
+std::string shape_str(const std::vector<uint64_t>& s) {
+  std::string r = "[";
+  for (size_t i = 0; i < s.size(); ++i) r += (i ? ", " : "") + std::to_string(s[i]);
+  return r + "]";
+}
+
+// Grow-only device / pinned buffers.
+struct DevBuf {
+  void* p = nullptr;
+  size_t cap = 0;
+  int ensure(size_t bytes, const char* what) {
+    if (bytes <= cap) return 0;
+    const size_t want = std::max(bytes, cap + cap / 4);
+    if (p) cudaFree(p);
+    p = nullptr, cap = 0;
+    cudaError_t e = cudaMalloc(&p, want);
+    SOME_REQUIRE(e == cudaSuccess, "session: cudaMalloc(%zu) for %s: %s", want, what, cudaGetErrorString(e));
+    cap = want;
+    return 0;
+  }
+  void release() {
+    if (p) cudaFree(p);
+    p = nullptr, cap = 0;
+  }
+};
+struct PinBuf {
+  void* p = nullptr;
+  size_t cap = 0;
+  int ensure(size_t bytes, const char* what) {
+    if (bytes <= cap) return 0;
+    const size_t want = std::max(bytes, cap + cap / 4);
+    if (p) cudaFreeHost(p);
+    p = nullptr, cap = 0;
+    cudaError_t e = cudaHostAlloc(&p, want, cudaHostAllocDefault);
+    SOME_REQUIRE(e == cudaSuccess, "session: cudaHostAlloc(%zu) for %s: %s", want, what, cudaGetErrorString(e));
+    cap = want;
+    return 0;
+  }
+  void release() {
+    if (p) cudaFreeHost(p);
+    p = nullptr, cap = 0;
+  }
+};
+
+// Makes `dev` current for the scope of a call and restores the caller's device afterwards.
+struct DeviceScope {
+  int prev = -1;
+  cudaError_t err;
+  explicit DeviceScope(int dev) {
+    cudaGetDevice(&prev);
+    err = cudaSetDevice(dev);
+  }
+  ~DeviceScope() {
+    if (prev >= 0) cudaSetDevice(prev);
+  }
+};
+
+#define SOME_CUDA(call, what)                                                           \
+  do {                                                                                  \
+    cudaError_t e_ = (call);                                                            \
+    SOME_REQUIRE(e_ == cudaSuccess, "session: %s: %s", what, cudaGetErrorString(e_));   \
+  } while (0)
+
+struct Chunk {
+  int c0, c1;
+  uint64_t off;
+  int bc, mc;
+};
+
+// A fixed set of worker threads for the host copies (staging of clips and recordings into pinned memory), kept for the
+// session's lifetime like Engine._pool, so that no call creates threads.  run(n, fn) runs fn(0 .. n-1), lane 0 on the calling
+// thread, and returns when every lane has finished; calls are serialised by the session's mutex.
+class WorkerPool {
+ public:
+  explicit WorkerPool(int n) : size_(std::max(1, n)) {
+    for (int lane = 1; lane < size_; ++lane) threads_.emplace_back([this, lane] { loop(lane); });
+  }
+  ~WorkerPool() {
+    {
+      std::lock_guard<std::mutex> l(mu_);
+      stop_ = true;
+      ++gen_;
+    }
+    wake_.notify_all();
+    for (auto& t : threads_) t.join();
+  }
+  int size() const { return size_; }
+  void run(int n, const std::function<void(int)>& fn) {
+    n = std::min(n, size_);
+    if (n <= 1) {
+      if (n == 1) fn(0);
+      return;
+    }
+    {
+      std::lock_guard<std::mutex> l(mu_);
+      fn_ = &fn, lanes_ = n, pending_ = n - 1;
+      ++gen_;
+    }
+    wake_.notify_all();
+    fn(0);
+    std::unique_lock<std::mutex> l(mu_);
+    done_.wait(l, [this] { return pending_ == 0; });
+    fn_ = nullptr;
+  }
+
+ private:
+  void loop(int lane) {
+    uint64_t seen = 0;
+    for (;;) {
+      const std::function<void(int)>* fn = nullptr;
+      {
+        std::unique_lock<std::mutex> l(mu_);
+        wake_.wait(l, [&] { return gen_ != seen; });
+        seen = gen_;
+        if (stop_) return;
+        if (lane >= lanes_) continue;        // not needed for this job
+        fn = fn_;
+      }
+      (*fn)(lane);
+      std::lock_guard<std::mutex> l(mu_);
+      if (--pending_ == 0) done_.notify_one();
+    }
+  }
+  int size_;
+  std::vector<std::thread> threads_;
+  std::mutex mu_;
+  std::condition_variable wake_, done_;
+  uint64_t gen_ = 0;
+  bool stop_ = false;
+  int lanes_ = 0, pending_ = 0;
+  const std::function<void(int)>* fn_ = nullptr;
+};
+
+}  // namespace
+
+struct some_notes {
+  std::vector<int64_t> first;   // [clips + 1] prefix sums of the note counts
+  std::vector<int64_t> range;   // [2 clips] sample range of each clip (sliced: in the resampled recording)
+  std::vector<float> midi;
+  std::vector<int32_t> dur;
+  std::vector<uint8_t> rest;
+};
+
+struct some_session {
+  std::mutex mu;
+  int device = 0;
+  some_session_info info{};
+  float vmin = 0.f, vmax = 0.f, deviation = 1.f, threshold = 0.1f;
+  void* weights = nullptr;
+  std::vector<some_block_weights> blocks;
+  std::vector<const uint16_t*> glu_w;
+  std::vector<const float*> glu_b;
+  some_model model{};
+  const int32_t *mel_start = nullptr, *mel_count = nullptr;
+  const float *mel_weights = nullptr, *twiddle = nullptr, *window = nullptr;
+  std::vector<double> kaiser;             // host copy of the float64 table (scaled per rate pair on upload)
+  std::vector<double> table_host;         // the scaled table of the current rate pair (source of its upload)
+  cudaStream_t stream = nullptr, copy_stream = nullptr;
+  cudaEvent_t ev[4] = {};
+  // grow-only buffers
+  DevBuf ws_block, scratch, wave_d, tab_d, cu_d, slab_d, native_d, table_d, meta_d, rms_d;
+  PinBuf wave_h, tab_h, cu_h, slab_h, meta_h, rms_h;
+  int ws_m = 0;
+  some_workspace ws{};
+  double table_ratio = 0.0;
+  std::unique_ptr<WorkerPool> pool;
+};
+
+namespace {
+
+void destroy(some_session* s) {
+  {
+    DeviceScope scope(s->device);
+    if (s->stream) cudaStreamSynchronize(s->stream);
+    if (s->copy_stream) cudaStreamSynchronize(s->copy_stream);
+    for (DevBuf* b : {&s->ws_block, &s->scratch, &s->wave_d, &s->tab_d, &s->cu_d, &s->slab_d, &s->native_d, &s->table_d,
+                      &s->meta_d, &s->rms_d})
+      b->release();
+    for (PinBuf* b : {&s->wave_h, &s->tab_h, &s->cu_h, &s->slab_h, &s->meta_h, &s->rms_h}) b->release();
+    for (cudaEvent_t& e : s->ev)
+      if (e) cudaEventDestroy(e);
+    if (s->stream) cudaStreamDestroy(s->stream);
+    if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
+    if (s->weights) cudaFree(s->weights);
+  }
+  delete s;
+}
+
+// Engine._chunks: up to three pipeline chunks of whole clips, a small first one.
+std::vector<std::pair<int, int>> split_chunks(const std::vector<int32_t>& cu) {
+  const int b = static_cast<int>(cu.size()) - 1;
+  const int64_t m = cu[b];
+  if (b < 2 || m < 2 * kMinChunkFrames) return {{0, b}};
+  std::vector<int> bounds{0};
+  double acc = 0.0;
+  for (double f : kChunkFractions) {
+    acc += f;
+    const double target = acc * static_cast<double>(m);
+    int i = static_cast<int>(std::lower_bound(cu.begin(), cu.end(), target,
+                                              [](int32_t v, double t) { return static_cast<double>(v) < t; }) -
+                             cu.begin());
+    i = std::min(std::max(i, bounds.back() + 1), b - 1);
+    if (cu[i] - cu[bounds.back()] >= kMinChunkFrames / 2 && i > bounds.back()) bounds.push_back(i);
+  }
+  bounds.push_back(b);
+  std::vector<std::pair<int, int>> out;
+  for (size_t i = 0; i + 1 < bounds.size(); ++i)
+    if (bounds[i + 1] > bounds[i]) out.push_back({bounds[i], bounds[i + 1]});
+  return out;
+}
+
+// One var-len batch through mel -> trunk -> decode, pipelined like Engine.enqueue.  Host clips (`host` != NULL: clip i is
+// host[i][0 .. lens[i])) are staged through pinned memory and copied on the copy stream while the previous chunk's kernels
+// run; resident clips (`resident` != NULL) are the sample ranges [starts[i], starts[i] + lens[i]) of that device buffer.
+int run_batch(some_session* s, const float* const* host, const float* resident, const int64_t* res_starts,
+              const int64_t* lens, int B, some_notes* out) {
+  std::vector<int32_t> cu(B + 1, 0);
+  std::vector<int64_t> starts(B, 0);
+  int64_t total = 0;
+  for (int i = 0; i < B; ++i) {
+    SOME_REQUIRE(lens[i] >= 0, "session: clip %d has a negative length", i);
+    const int64_t frames = 1 + lens[i] / SOME_HOP;
+    SOME_REQUIRE(cu[i] + frames < (int64_t(1) << 31), "session: the batch has more than 2^31 frames");
+    cu[i + 1] = static_cast<int32_t>(cu[i] + frames);
+    if (host) {
+      starts[i] = total;
+      total += (lens[i] + 3) & ~int64_t(3);     // 16-byte aligned clip starts, as Engine.tables
+    } else {
+      starts[i] = res_starts[i];
+    }
+  }
+  const auto spans = split_chunks(cu);
+  std::vector<Chunk> layout;
+  uint64_t slab_bytes = 0;
+  int max_mc = 1;
+  for (const auto& sp : spans) {
+    const int bc = sp.second - sp.first, mc = cu[sp.second] - cu[sp.first];
+    layout.push_back({sp.first, sp.second, slab_bytes, bc, mc});
+    slab_bytes += (4ull * bc + 9ull * mc + 15) & ~uint64_t(15);
+    max_mc = std::max(max_mc, mc);
+  }
+  // buffers
+  if (max_mc > s->ws_m) {
+    const uint64_t bytes = some_workspace_bytes(max_mc, s->info.outdim, 0);
+    if (s->ws_block.ensure(bytes, "the workspace")) return -1;
+    if (some_workspace_carve(s->ws_block.p, s->ws_block.cap, max_mc, s->info.outdim, 0, &s->ws)) return -1;
+    if (s->scratch.ensure(some_decode_scratch_bytes(max_mc), "the decode scratch")) return -1;
+    s->ws_m = max_mc;
+  }
+  if (s->tab_h.ensure(16ull * B + 16, "tables") || s->tab_d.ensure(16ull * B + 16, "tables") ||
+      s->cu_h.ensure(4ull * (B + layout.size()) + 4, "cu_frames") || s->cu_d.ensure(4ull * (B + layout.size()) + 4, "cu_frames") ||
+      s->slab_h.ensure(slab_bytes + 16, "the note slab") || s->slab_d.ensure(slab_bytes + 16, "the note slab"))
+    return -1;
+  if (host && (s->wave_h.ensure(4ull * total + 16, "the staged audio") || s->wave_d.ensure(4ull * total + 16, "the audio")))
+    return -1;
+  float* wave_h = static_cast<float*>(s->wave_h.p);
+  const float* wave = host ? static_cast<const float*>(s->wave_d.p) : resident;
+  int64_t* tab_h = static_cast<int64_t*>(s->tab_h.p);
+  int64_t* tab_d = static_cast<int64_t*>(s->tab_d.p);
+  int32_t* cu_h = static_cast<int32_t*>(s->cu_h.p);
+  int32_t* cu_d = static_cast<int32_t*>(s->cu_d.p);
+  uint8_t* slab = static_cast<uint8_t*>(s->slab_d.p);
+  const int head = s->info.quantized ? SOME_EPI_SOFTMAX_F32 : SOME_EPI_SIGMOID_F32;
+
+  for (size_t ci = 0; ci < layout.size(); ++ci) {
+    const Chunk& ch = layout[ci];
+    const int64_t lo = starts[ch.c0];
+    if (host) {                                  // stage this chunk's clips; the GPU is still busy with the previous chunk
+      const int nt = std::min(s->pool->size(), ch.bc);
+      s->pool->run(nt, [&](int t) {
+        for (int i = ch.c0 + t; i < ch.c1; i += nt)
+          if (lens[i]) memcpy(wave_h + starts[i], host[i], 4ull * lens[i]);
+      });
+    }
+    int64_t* tab = tab_h + 2 * ch.c0;
+    int max_frames = 1;
+    for (int i = 0; i < ch.bc; ++i) {
+      tab[i] = starts[ch.c0 + i] - lo;
+      tab[ch.bc + i] = lens[ch.c0 + i];
+      max_frames = std::max(max_frames, cu[ch.c0 + i + 1] - cu[ch.c0 + i]);
+    }
+    int32_t* cuc = cu_h + ch.c0 + ci;            // chunk ci owns entries [c0 + ci, c1 + ci]
+    for (int i = 0; i <= ch.bc; ++i) cuc[i] = cu[ch.c0 + i] - cu[ch.c0];
+    const int64_t hi = host ? starts[ch.c1 - 1] + ((lens[ch.c1 - 1] + 3) & ~int64_t(3)) : lo;
+    if (hi > lo)
+      SOME_CUDA(cudaMemcpyAsync(static_cast<float*>(s->wave_d.p) + lo, wave_h + lo, 4ull * (hi - lo), cudaMemcpyHostToDevice,
+                                s->copy_stream), "audio upload");
+    SOME_CUDA(cudaMemcpyAsync(tab_d + 2 * ch.c0, tab, 16ull * ch.bc, cudaMemcpyHostToDevice, s->copy_stream), "table upload");
+    SOME_CUDA(cudaMemcpyAsync(cu_d + ch.c0 + ci, cuc, 4ull * (ch.bc + 1), cudaMemcpyHostToDevice, s->copy_stream),
+              "cu_frames upload");
+    SOME_CUDA(cudaEventRecord(s->ev[ci], s->copy_stream), "event record");
+    SOME_CUDA(cudaStreamWaitEvent(s->stream, s->ev[ci], 0), "stream wait");
+
+    const int32_t* cud = cu_d + ch.c0 + ci;
+    uint8_t* o = slab + ch.off;
+    if (some_mel_logmel(wave + lo, tab_d + 2 * ch.c0, tab_d + 2 * ch.c0 + ch.bc, cud, ch.bc, max_frames, s->mel_start,
+                        s->mel_count, s->mel_weights, s->twiddle, s->window, nullptr, const_cast<uint16_t*>(s->ws.units), 1e-5f,
+                        s->stream))
+      return -1;
+    if (some_forward(&s->model, &s->ws, ch.mc, ch.bc, cud, max_frames, head, nullptr, nullptr, s->stream)) return -1;
+    some_decode_args d{};
+    d.probs = s->ws.probs, d.bounds = s->ws.bounds, d.cu_frames = cud;
+    d.B = ch.bc, d.M = ch.mc, d.N = s->info.outdim, d.quantized = s->info.quantized;
+    d.vmin = s->vmin, d.vmax = s->vmax, d.deviation = s->deviation, d.threshold = s->threshold;
+    d.note_count = reinterpret_cast<int32_t*>(o);
+    d.note_dur = reinterpret_cast<int32_t*>(o + 4ull * ch.bc);
+    d.note_midi = reinterpret_cast<float*>(o + 4ull * ch.bc + 4ull * ch.mc);
+    d.note_rest = o + 4ull * ch.bc + 8ull * ch.mc;
+    d.scratch = s->scratch.p;
+    if (some_decode_notes(&d, s->stream)) return -1;
+  }
+  if (slab_bytes) SOME_CUDA(cudaMemcpyAsync(s->slab_h.p, slab, slab_bytes, cudaMemcpyDeviceToHost, s->stream), "note download");
+  SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+
+  // unpack: the notes of clip b start at its first frame's row of the chunk slab
+  out->first.assign(1, 0);
+  out->range.clear();
+  out->midi.clear(), out->dur.clear(), out->rest.clear();
+  const uint8_t* h = static_cast<const uint8_t*>(s->slab_h.p);
+  for (const Chunk& ch : layout) {
+    const uint8_t* o = h + ch.off;
+    for (int b = 0; b < ch.bc; ++b) {
+      const int32_t n = rd<int32_t>(o + 4ull * b);
+      const int64_t row = cu[ch.c0 + b] - cu[ch.c0];
+      SOME_REQUIRE(n >= 0 && row + n <= ch.mc, "session: decode returned %d notes for a clip of %d frames", n,
+                   cu[ch.c0 + b + 1] - cu[ch.c0 + b]);
+      for (int j = 0; j < n; ++j) {
+        const uint64_t r = static_cast<uint64_t>(row + j);
+        out->dur.push_back(rd<int32_t>(o + 4ull * ch.bc + 4 * r));
+        out->midi.push_back(rd<float>(o + 4ull * ch.bc + 4ull * ch.mc + 4 * r));
+        out->rest.push_back(o[4ull * ch.bc + 8ull * ch.mc + r]);
+      }
+      out->first.push_back(out->first.back() + n);
+      out->range.push_back(host ? 0 : starts[ch.c0 + b]);
+      out->range.push_back(host ? lens[ch.c0 + b] : starts[ch.c0 + b] + lens[ch.c0 + b]);
+    }
+  }
+  return 0;
+}
+
+// Uploads n floats of host memory to `dst` through the pinned staging buffer: in pieces, each copied into pinned memory by the
+// session's threads and then sent while the next piece is copied.
+int upload_staged(some_session* s, float* dst, const float* src, int64_t n) {
+  constexpr int64_t kPiece = int64_t(1) << 22;   // 16 MB
+  float* pin = static_cast<float*>(s->wave_h.p);
+  for (int64_t a = 0; a < n; a += kPiece) {
+    const int64_t len = std::min(kPiece, n - a);
+    const int nt = static_cast<int>(std::min<int64_t>(s->pool->size(), (len + 65535) / 65536));
+    const int64_t per = (len + nt - 1) / nt;
+    s->pool->run(nt, [&](int t) {
+      const int64_t b = a + t * per, e = std::min(a + len, b + per);
+      if (e > b) memcpy(pin + b, src + b, 4ull * (e - b));
+    });
+    SOME_CUDA(cudaMemcpyAsync(dst + a, pin + a, 4ull * len, cudaMemcpyHostToDevice, s->stream), "audio upload");
+  }
+  return 0;
+}
+
+// The first index of the minimum of rms[a, min(b, n)) (numpy's argmin: the first NaN wins).
+int64_t first_min(const float* rms, int64_t n, int64_t a, int64_t b) {
+  b = std::min(b, n);
+  int64_t best = a;
+  for (int64_t i = a; i < b; ++i) {
+    if (isnan(rms[i])) return i;
+    if (rms[i] < rms[best]) best = i;
+  }
+  return best;
+}
+
+}  // namespace
+
+// ---------------------------------------------------------------------------------------------------- slicer decisions
+extern "C" int some_slicer_derive(int sample_rate, const some_slicer_params* p, some_slicer_frames* out) {
+  SOME_REQUIRE(out != nullptr && sample_rate > 0, "some_slicer_derive: bad arguments");
+  some_slicer_params d{-40.0, 5000.0, 300.0, 20.0, 1000.0};    // infer.py: Slicer(sr, max_sil_kept=1000)
+  if (p) d = *p;
+  SOME_REQUIRE(d.min_length_ms >= d.min_interval_ms && d.min_interval_ms >= d.hop_size_ms,
+               "some_slicer_derive: the following condition must be satisfied: min_length >= min_interval >= hop_size");
+  SOME_REQUIRE(d.max_sil_kept_ms >= d.hop_size_ms,
+               "some_slicer_derive: the following condition must be satisfied: max_sil_kept >= hop_size");
+  // Slicer.__init__ (some_b200/slicer.py), with Python's round (half to even: rint in the default rounding mode)
+  const double sr = sample_rate;
+  const double interval = sr * d.min_interval_ms / 1000.0;
+  const double hop = rint(sr * d.hop_size_ms / 1000.0);
+  SOME_REQUIRE(hop >= 1.0, "some_slicer_derive: hop_size of %g ms is less than one sample", d.hop_size_ms);
+  out->threshold = static_cast<float>(pow(10.0, d.threshold_db / 20.0));   // `rms < threshold` compares in float32
+  out->hop_size = static_cast<int>(hop);
+  out->win_size = static_cast<int>(std::min(rint(interval), 4.0 * hop));
+  out->min_length = static_cast<int>(rint(sr * d.min_length_ms / 1000.0 / hop));
+  out->min_interval = static_cast<int>(rint(interval / hop));
+  out->max_sil_kept = static_cast<int>(rint(sr * d.max_sil_kept_ms / 1000.0 / hop));
+  return 0;
+}
+
+extern "C" int some_slicer_ranges(const float* rms, int n_frames, long long n_samples, const some_slicer_frames* f,
+                                  int64_t* ranges, int capacity, int* count) {
+  SOME_REQUIRE((rms != nullptr || n_frames == 0) && f != nullptr && count != nullptr && n_frames >= 0 && n_samples >= 0,
+               "some_slicer_ranges: bad arguments");
+  // silence_tags (some_b200/slicer.py): the rules act on each run of frames with rms < threshold
+  const int64_t total = n_frames, keep = f->max_sil_kept;
+  std::vector<std::pair<int64_t, int64_t>> tags;
+  int64_t clip_from = 0;
+  for (int64_t s = 0; s < total;) {
+    if (!(rms[s] < f->threshold)) {
+      ++s;
+      continue;
+    }
+    int64_t i = s;
+    while (i < total && rms[i] < f->threshold) ++i;     // first voiced frame after the run (total for a trailing run)
+    if (i == total) {
+      if (total - s >= f->min_interval) tags.push_back({first_min(rms, total, s, std::min(total, s + keep) + 1), total + 1});
+      break;
+    }
+    const bool leading = s == 0 && i > keep;
+    const bool middle = i - s >= f->min_interval && i - clip_from >= f->min_length;
+    if (leading || middle) {
+      const int64_t span = i - s;
+      if (span <= keep) {
+        const int64_t cut = first_min(rms, total, s, i + 1);
+        tags.push_back(s == 0 ? std::make_pair(int64_t(0), cut) : std::make_pair(cut, cut));
+        clip_from = cut;
+      } else if (span <= 2 * keep) {
+        const int64_t mid = first_min(rms, total, i - keep, s + keep + 1);
+        const int64_t left = first_min(rms, total, s, s + keep + 1);
+        const int64_t right = first_min(rms, total, i - keep, i + 1);
+        if (s == 0) {
+          tags.push_back({0, right});
+          clip_from = right;
+        } else {
+          tags.push_back({std::min(left, mid), std::max(right, mid)});
+          clip_from = std::max(right, mid);
+        }
+      } else {
+        const int64_t left = first_min(rms, total, s, s + keep + 1);
+        const int64_t right = first_min(rms, total, i - keep, i + 1);
+        tags.push_back(s == 0 ? std::make_pair(int64_t(0), right) : std::make_pair(left, right));
+        clip_from = right;
+      }
+    }
+    s = i;
+  }
+  // chunk_ranges: the frames between the tags, as sample ranges
+  std::vector<std::pair<int64_t, int64_t>> kept;
+  if (tags.empty()) {
+    kept.push_back({0, -1});
+  } else {
+    if (tags[0].first > 0) kept.push_back({0, tags[0].first});
+    for (size_t k = 0; k + 1 < tags.size(); ++k) kept.push_back({tags[k].second, tags[k + 1].first});
+    if (tags.back().second < total) kept.push_back({tags.back().second, total});
+  }
+  *count = static_cast<int>(kept.size());
+  SOME_REQUIRE(ranges != nullptr && capacity >= *count, "some_slicer_ranges: %d ranges do not fit in a capacity of %d", *count,
+               capacity);
+  const int64_t hop = f->hop_size;
+  for (size_t k = 0; k < kept.size(); ++k) {
+    if (kept[k].second < 0) {                   // no tags: the whole recording
+      ranges[2 * k] = 0, ranges[2 * k + 1] = n_samples;
+      continue;
+    }
+    ranges[2 * k] = kept[k].first * hop;
+    ranges[2 * k + 1] = std::min<int64_t>(n_samples, kept[k].second * hop);
+  }
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- results
+extern "C" int some_notes_create(some_notes** out) {
+  SOME_REQUIRE(out != nullptr, "some_notes_create: null pointer");
+  *out = new some_notes();
+  (*out)->first.assign(1, 0);
+  return 0;
+}
+extern "C" int some_notes_destroy(some_notes* n) {
+  delete n;
+  return 0;
+}
+extern "C" int some_notes_clips(const some_notes* n) {
+  SOME_REQUIRE(n != nullptr, "some_notes_clips: null pointer");
+  return static_cast<int>(n->first.size()) - 1;
+}
+extern "C" int some_notes_get(const some_notes* n, int clip, int* count, const float** note_midi, const int32_t** note_dur,
+                              const uint8_t** note_rest, int64_t* begin, int64_t* end) {
+  SOME_REQUIRE(n != nullptr && clip >= 0 && clip + 1 < static_cast<int>(n->first.size()),
+               "some_notes_get: clip %d out of range", clip);
+  const int64_t a = n->first[clip];
+  if (count) *count = static_cast<int>(n->first[clip + 1] - a);
+  if (note_midi) *note_midi = n->midi.data() + a;
+  if (note_dur) *note_dur = n->dur.data() + a;
+  if (note_rest) *note_rest = n->rest.data() + a;
+  if (begin) *begin = n->range[2 * clip];
+  if (end) *end = n->range[2 * clip + 1];
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- session
+extern "C" int some_session_open(const char* path, int device, some_session** out) {
+  SOME_REQUIRE(path != nullptr && out != nullptr, "some_session_open: null pointer");
+  *out = nullptr;
+  FILE* fp = fopen(path, "rb");
+  SOME_REQUIRE(fp != nullptr, "%s: cannot open the model file", path);
+  std::vector<uint8_t> file;
+  {
+    uint8_t buf[1 << 16];
+    size_t got;
+    while ((got = fread(buf, 1, sizeof(buf), fp)) > 0) file.insert(file.end(), buf, buf + got);
+    const bool bad = ferror(fp) != 0;
+    fclose(fp);
+    SOME_REQUIRE(!bad, "%s: read error", path);
+  }
+  const uint64_t size = file.size();
+  const uint8_t* f = file.data();
+  // ---- header
+  SOME_REQUIRE(size >= kHeaderBytes, "%s: truncated header (%llu bytes, a model file starts with %llu)", path,
+               (unsigned long long)size, (unsigned long long)kHeaderBytes);
+  SOME_REQUIRE(memcmp(f, kMagic, 8) == 0, "%s: bad magic: not a some_b200 model file", path);
+  const uint32_t format = rd<uint32_t>(f + 8), abi = rd<uint32_t>(f + 12);
+  SOME_REQUIRE(format == kFormat, "%s: unsupported format version %u (this library reads version %u)", path, format, kFormat);
+  SOME_REQUIRE(abi == SOME_B200_VERSION, "%s: written for ABI %u, this library is ABI %d", path, abi, SOME_B200_VERSION);
+  const uint64_t file_size = rd<uint64_t>(f + 16), dir_off = rd<uint64_t>(f + 24), data_off = rd<uint64_t>(f + 80);
+  const uint32_t n_tensors = rd<uint32_t>(f + 32);
+  const int32_t lay = rd<int32_t>(f + 36), outdim = rd<int32_t>(f + 40), quantized = rd<int32_t>(f + 44);
+  const int32_t sr = rd<int32_t>(f + 48), hop = rd<int32_t>(f + 52), win = rd<int32_t>(f + 56);
+  const int32_t bias_corrected = rd<int32_t>(f + 76);
+  SOME_REQUIRE(dir_off >= kHeaderBytes && dir_off <= size && n_tensors <= (size - dir_off) / kEntryBytes,
+               "%s: truncated directory (%u entries at byte %llu, file of %llu bytes)", path, n_tensors,
+               (unsigned long long)dir_off, (unsigned long long)size);
+  SOME_REQUIRE(file_size == size, "%s: file size %llu does not match the %llu bytes the header records", path,
+               (unsigned long long)size, (unsigned long long)file_size);
+  SOME_REQUIRE(data_off % kAlign == 0 && data_off >= dir_off + uint64_t(n_tensors) * kEntryBytes && data_off <= size,
+               "%s: bad data offset %llu", path, (unsigned long long)data_off);
+  SOME_REQUIRE(lay >= 0 && lay <= 64 && outdim >= 1 && outdim <= 256 && (quantized == 0 || quantized == 1) && sr > 0 &&
+                   hop == SOME_HOP && win == SOME_N_FFT,
+               "%s: unsupported model scalars (lay %d, outdim %d, quantized %d, rate %d, hop %d, win %d)", path, lay, outdim,
+               quantized, sr, hop, win);
+  // ---- directory
+  struct Entry {
+    uint32_t dtype;
+    std::vector<uint64_t> shape;
+    uint64_t off, bytes;
+  };
+  std::map<std::string, Entry> dir;
+  for (uint32_t t = 0; t < n_tensors; ++t) {
+    const uint8_t* e = f + dir_off + uint64_t(t) * kEntryBytes;
+    char name[kNameBytes + 1] = {};
+    memcpy(name, e, kNameBytes);
+    Entry en;
+    en.dtype = rd<uint32_t>(e + 64);
+    const uint32_t ndim = rd<uint32_t>(e + 68);
+    SOME_REQUIRE(ndim <= 4 && dtype_bytes(en.dtype) > 0, "%s: directory entry %u ('%s') has dtype %u / %u dimensions", path, t,
+                 name, en.dtype, ndim);
+    uint64_t elems = 1;
+    for (uint32_t k = 0; k < ndim; ++k) {
+      en.shape.push_back(rd<uint64_t>(e + 72 + 8 * k));
+      SOME_REQUIRE(en.shape.back() < (uint64_t(1) << 40), "%s: tensor '%s' has an absurd shape", path, name);
+      elems *= en.shape.back();
+    }
+    en.off = rd<uint64_t>(e + 104);
+    en.bytes = rd<uint64_t>(e + 112);
+    SOME_REQUIRE(en.off % kAlign == 0 && en.off >= data_off && en.off <= size && en.bytes <= size - en.off,
+                 "%s: tensor '%s' lies outside the data section (bytes %llu + %llu of %llu)", path, name,
+                 (unsigned long long)en.off, (unsigned long long)en.bytes, (unsigned long long)size);
+    SOME_REQUIRE(en.bytes == elems * dtype_bytes(en.dtype), "%s: tensor '%s' holds %llu bytes, its shape needs %llu", path,
+                 name, (unsigned long long)en.bytes, (unsigned long long)(elems * dtype_bytes(en.dtype)));
+    SOME_REQUIRE(dir.emplace(name, en).second, "%s: tensor '%s' appears twice", path, name);
+  }
+  const std::vector<Spec> specs = expected_tensors(lay, outdim);
+  for (const Spec& sp : specs) {
+    auto it = dir.find(sp.name);
+    SOME_REQUIRE(it != dir.end(), "%s: missing tensor '%s'", path, sp.name.c_str());
+    SOME_REQUIRE(it->second.dtype == sp.dtype && it->second.shape == sp.shape,
+                 "%s: tensor '%s' is %s %s, a model with lay %d / outdim %d needs %s %s", path, sp.name.c_str(),
+                 dtype_name(it->second.dtype), shape_str(it->second.shape).c_str(), lay, outdim, dtype_name(sp.dtype),
+                 shape_str(sp.shape).c_str());
+  }
+  SOME_REQUIRE(dir.size() == specs.size(), "%s: %zu tensors, a model with lay %d / outdim %d has %zu", path, dir.size(), lay,
+               outdim, specs.size());
+
+  // ---- the device (first CUDA call)
+  int n_dev = 0;
+  cudaError_t e = cudaGetDeviceCount(&n_dev);
+  SOME_REQUIRE(e == cudaSuccess && device >= 0 && device < n_dev, "some_session_open: no CUDA device %d (%s)", device,
+               e == cudaSuccess ? "out of range" : cudaGetErrorString(e));
+  cudaDeviceProp prop;
+  SOME_CUDA(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties");
+  SOME_REQUIRE(prop.major == 9 && prop.minor == 0, "some_session_open: device %d (%s) is sm_%d%d; the kernels are built for sm_90a",
+               device, prop.name, prop.major, prop.minor);
+  some_session* s = new some_session();
+  s->device = device;
+  DeviceScope scope(device);
+  auto fail = [&](int rc) {
+    destroy(s);
+    return rc;
+  };
+  if (scope.err != cudaSuccess) {
+    set_error("some_session_open: cudaSetDevice(%d): %s", device, cudaGetErrorString(scope.err));
+    return fail(-2);
+  }
+  e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s->copy_stream, cudaStreamNonBlocking);
+  for (cudaEvent_t& ev : s->ev)
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+  // the weights go up on the session's own (non-blocking) stream, which every later kernel of the session runs on; the wait
+  // also keeps the host copy of the file alive until the copy has read it
+  if (e == cudaSuccess) e = cudaMalloc(&s->weights, std::max<uint64_t>(size - data_off, 1));
+  if (e == cudaSuccess) e = cudaMemcpyAsync(s->weights, f + data_off, size - data_off, cudaMemcpyHostToDevice, s->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
+  if (e != cudaSuccess) {
+    set_error("some_session_open: uploading %s: %s", path, cudaGetErrorString(e));
+    return fail(-2);
+  }
+  uint8_t* base = static_cast<uint8_t*>(s->weights);
+  auto dp = [&](const std::string& name) -> const void* { return base + (dir.at(name).off - data_off); };
+  auto bf = [&](const std::string& n) { return static_cast<const uint16_t*>(dp(n)); };
+  auto fl = [&](const std::string& n) { return static_cast<const float*>(dp(n)); };
+  s->blocks.resize(2 * (lay + 1));
+  for (int j = 0; j < 2 * (lay + 1); ++j) {
+    const std::string p = "blk" + std::to_string(j) + ".";
+    some_block_weights& b = s->blocks[j];
+    memset(&b, 0, sizeof(b));
+    for (int k = 0; k < 5; ++k) b.ln_g[k] = fl(p + "ln_g." + std::to_string(k)), b.ln_b[k] = fl(p + "ln_b." + std::to_string(k));
+    for (int k = 0; k < 2; ++k) {
+      const std::string q = "." + std::to_string(k);
+      b.ffn_w1[k] = bf(p + "ffn_w1" + q), b.ffn_b1[k] = fl(p + "ffn_b1" + q);
+      b.ffn_w2[k] = bf(p + "ffn_w2" + q), b.ffn_b2[k] = fl(p + "ffn_b2" + q);
+    }
+    b.w_qkv = bf(p + "w_qkv"), b.w_out = bf(p + "w_out"), b.b_out = fl(p + "b_out");
+    b.w_pw1 = bf(p + "w_pw1"), b.b_pw1 = fl(p + "b_pw1"), b.w_dw = fl(p + "w_dw"), b.b_dw = fl(p + "b_dw");
+    b.w_pw2 = bf(p + "w_pw2"), b.b_pw2 = fl(p + "b_pw2");
+  }
+  for (int j = 0; j < 2 * lay; ++j) {
+    s->glu_w.push_back(bf("glu" + std::to_string(j) + ".w"));
+    s->glu_b.push_back(fl("glu" + std::to_string(j) + ".b"));
+  }
+  if (lay == 0) s->glu_w.push_back(nullptr), s->glu_b.push_back(nullptr);
+  some_model& m = s->model;
+  m.lay = lay, m.outdim = outdim;
+  for (int k = 0; k < 2; ++k) m.w_in[k] = bf("w_in." + std::to_string(k)), m.b_in[k] = fl("b_in." + std::to_string(k));
+  m.blocks = s->blocks.data();
+  m.glu_w = s->glu_w.data();
+  m.glu_b = s->glu_b.data();
+  m.w_head = bf("w_head"), m.b_head = fl("b_head"), m.w_cut = fl("w_cut");
+  const Entry& bc = dir.at("b_cut");
+  m.b_cut = rd<float>(f + bc.off);               // a host scalar of some_model
+  m.ln_fold = 0;                                  // the default stand-alone LayerNorm sequence
+  s->mel_start = static_cast<const int32_t*>(dp("mel_start"));
+  s->mel_count = static_cast<const int32_t*>(dp("mel_count"));
+  s->mel_weights = fl("mel_weights"), s->twiddle = fl("twiddle"), s->window = fl("window");
+  const Entry& kt = dir.at("kaiser_best");
+  s->kaiser.resize(kKaiserTaps);
+  memcpy(s->kaiser.data(), f + kt.off, kt.bytes);
+  s->info.sample_rate = sr;
+  s->info.hop = hop;
+  s->info.outdim = outdim;
+  s->info.quantized = quantized;
+  s->info.bias_corrected = bias_corrected;
+  s->info.timestep = static_cast<double>(hop) / static_cast<double>(sr);    // base_infer.py:20
+  s->vmin = rd<float>(f + 60), s->vmax = rd<float>(f + 64), s->deviation = rd<float>(f + 68), s->threshold = rd<float>(f + 72);
+  const unsigned hw = std::thread::hardware_concurrency();
+  s->pool.reset(new WorkerPool(static_cast<int>(std::min(8u, std::max(2u, hw / 2)))));
+  *out = s;
+  return 0;
+}
+
+extern "C" int some_session_close(some_session* s) {
+  if (s) destroy(s);
+  return 0;
+}
+
+extern "C" int some_session_get_info(const some_session* s, some_session_info* info) {
+  SOME_REQUIRE(s != nullptr && info != nullptr, "some_session_get_info: null pointer");
+  *info = s->info;
+  return 0;
+}
+
+namespace {
+int transcribe_sliced(some_session* s, const float* samples, int64_t n, int sample_rate, int64_t n_out,
+                      const some_slicer_frames& sl, some_notes* out);
+
+// After a failure partway through a call, copies and kernels may still be queued on the session's streams: wait for them, so
+// that the next call cannot rewrite staging or device buffers they still use.  (The error message of the failure is kept.)
+int settle(some_session* s, int rc) {
+  if (rc != 0) {
+    cudaStreamSynchronize(s->copy_stream);
+    cudaStreamSynchronize(s->stream);
+  }
+  return rc;
+}
+}  // namespace
+
+extern "C" int some_session_transcribe(some_session* s, const float* const* clips, const int64_t* lens, int B, some_notes* out) {
+  SOME_REQUIRE(s != nullptr && out != nullptr && B >= 0 && (B == 0 || (clips != nullptr && lens != nullptr)),
+               "some_session_transcribe: bad arguments");
+  for (int i = 0; i < B; ++i) SOME_REQUIRE(lens[i] >= 0 && (lens[i] == 0 || clips[i] != nullptr), "some_session_transcribe: clip %d", i);
+  std::lock_guard<std::mutex> lock(s->mu);
+  if (B == 0) {
+    out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
+    return 0;
+  }
+  DeviceScope scope(s->device);
+  SOME_CUDA(scope.err, "cudaSetDevice");
+  return settle(s, run_batch(s, clips, nullptr, nullptr, lens, B, out));
+}
+
+extern "C" int some_session_transcribe_sliced(some_session* s, const float* samples, long long n, int sample_rate,
+                                              const some_slicer_params* params, some_notes* out) {
+  SOME_REQUIRE(s != nullptr && out != nullptr && n >= 0 && (n == 0 || samples != nullptr) && sample_rate > 0,
+               "some_session_transcribe_sliced: bad arguments");
+  const int sr = s->info.sample_rate;
+  some_slicer_frames sl;
+  if (some_slicer_derive(sr, params, &sl)) return -1;
+  // audio.resampled_length: librosa.load's output length, and resampy's refusal of too-short inputs
+  int64_t n_out = n;
+  const double ratio = static_cast<double>(sr) / sample_rate;
+  if (sample_rate != sr) {
+    SOME_REQUIRE(static_cast<int64_t>(n) * sr / sample_rate >= 1,
+                 "some_session_transcribe_sliced: Input signal length=%lld is too small to resample from %d->%d", n, sample_rate, sr);
+    n_out = static_cast<int64_t>(ceil(static_cast<double>(n) * ratio));
+  }
+  std::lock_guard<std::mutex> lock(s->mu);
+  DeviceScope scope(s->device);
+  SOME_CUDA(scope.err, "cudaSetDevice");
+  return settle(s, transcribe_sliced(s, samples, n, sample_rate, n_out, sl, out));
+}
+
+namespace {
+int transcribe_sliced(some_session* s, const float* samples, int64_t n, int sample_rate, int64_t n_out,
+                      const some_slicer_frames& sl, some_notes* out) {
+  const int sr = s->info.sample_rate;
+  const double ratio = static_cast<double>(sr) / sample_rate;
+  // upload (through pinned memory) and, at another rate, resample into the wave buffer
+  if (s->wave_h.ensure(4ull * n + 16, "the staged audio") || s->wave_d.ensure(4ull * n_out + 16, "the audio")) return -1;
+  float* wave = static_cast<float*>(s->wave_d.p);
+  if (sample_rate == sr) {
+    if (upload_staged(s, wave, samples, n)) return -1;
+  } else {
+    const double key = ratio < 1 ? ratio : 1.0;
+    if (s->table_d.cap == 0 || s->table_ratio != key) {
+      s->table_host = s->kaiser;
+      if (ratio < 1)
+        for (double& v : s->table_host) v = ratio * v;   // audio._device_table: resampy scales the table when downsampling
+      if (s->table_d.ensure(8ull * kKaiserTaps, "the resampling table")) return -1;
+      // on the session's stream, in front of the resampling launch that reads it
+      SOME_CUDA(cudaMemcpyAsync(s->table_d.p, s->table_host.data(), 8ull * kKaiserTaps, cudaMemcpyHostToDevice, s->stream),
+                "table upload");
+      s->table_ratio = key;
+    }
+    if (s->native_d.ensure(4ull * n + 16, "the native audio") || s->meta_h.ensure(32, "resampling tables") ||
+        s->meta_d.ensure(32, "resampling tables"))
+      return -1;
+    int64_t* meta = static_cast<int64_t*>(s->meta_h.p);
+    meta[0] = 0, meta[1] = n, meta[2] = 0;
+    const int64_t* md = static_cast<const int64_t*>(s->meta_d.p);
+    if (upload_staged(s, static_cast<float*>(s->native_d.p), samples, n)) return -1;
+    SOME_CUDA(cudaMemcpyAsync(s->meta_d.p, meta, 24, cudaMemcpyHostToDevice, s->stream), "table upload");
+    if (some_resample_kaiser(static_cast<const float*>(s->native_d.p), md, md + 1, wave, md + 2, 1, n_out, sample_rate, sr,
+                             static_cast<const double*>(s->table_d.p), kKaiserTaps, s->stream))
+      return -1;
+  }
+  // the slicer: a recording no longer than min_length is one chunk (slicer2.py:79-80)
+  std::vector<int64_t> ranges;
+  if ((n_out + sl.hop_size - 1) / sl.hop_size <= sl.min_length) {
+    ranges = {0, n_out};
+  } else {
+    const int64_t frames = 1 + (n_out + 2 * (sl.win_size / 2) - sl.win_size) / sl.hop_size;
+    SOME_REQUIRE(frames < (int64_t(1) << 31), "some_session_transcribe_sliced: recording too long");
+    const int nf = static_cast<int>(frames);
+    if (s->rms_d.ensure(4ull * nf, "the RMS frames") || s->rms_h.ensure(4ull * nf, "the RMS frames")) return -1;
+    if (some_slicer_rms(wave, n_out, sl.win_size, sl.hop_size, static_cast<float*>(s->rms_d.p), nf, s->stream)) return -1;
+    SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * nf, cudaMemcpyDeviceToHost, s->stream), "RMS download");
+    SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+    ranges.resize(2 * (static_cast<size_t>(nf) + 2));
+    int count = 0;
+    if (some_slicer_ranges(static_cast<const float*>(s->rms_h.p), nf, n_out, &sl, ranges.data(), nf + 2, &count)) return -1;
+    ranges.resize(2 * static_cast<size_t>(count));
+  }
+  const int B = static_cast<int>(ranges.size() / 2);
+  if (B == 0) {
+    out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
+    return 0;
+  }
+  std::vector<int64_t> starts(B), lens(B);
+  for (int i = 0; i < B; ++i) starts[i] = ranges[2 * i], lens[i] = std::max<int64_t>(0, ranges[2 * i + 1] - ranges[2 * i]);
+  return run_batch(s, nullptr, wave, starts.data(), lens.data(), B, out);
+}
+}  // namespace

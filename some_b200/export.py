@@ -1,0 +1,173 @@
+"""Export a checkpoint to one self-contained model file for hosts without Python (the counterpart of the reference's
+``export.py`` + ``deployment/``, which write an ONNX graph).
+
+    python -m some_b200.export --model CKPT [--out PATH]
+
+reads ``config.yaml`` beside the checkpoint (export.py:53-55), builds the engine exactly as a default
+``MIDIExtractionInference`` does (default launch sequence, load-time bias correction ``Engine.calibrate``: that step needs a
+CUDA device) and writes the tensors that engine runs with: the device tensors ``build_c_model(w, ln_fold=False)`` points to,
+biases corrected, plus the mel tables and resampy's float64 ``kaiser_best`` table.  ``some_session_open`` (csrc/session.cu)
+is the only reader; the format is documented in INTEGRATION.md ("Deploying without Python").
+
+The file is a pure function of the checkpoint: exporting the same checkpoint twice gives identical bytes.
+"""
+from __future__ import annotations
+
+import argparse
+import pathlib
+import struct
+from typing import Dict, List, Sequence, Tuple
+
+import numpy as np
+
+MAGIC = b'SOMEB200'
+FORMAT_VERSION = 1
+ABI_VERSION = 202
+SUFFIX = '.somemodel'
+HEADER = struct.Struct('<8sIIQQIiiiiiiffffiQ40x')       # 128 bytes
+ENTRY = struct.Struct('<64sII4QQQ8x')                   # 128 bytes
+ALIGN = 256
+DTYPES = {np.dtype('<f4'): 1, np.dtype('<u2'): 2, np.dtype('<i4'): 3, np.dtype('<f8'): 4}   # u2 = raw bfloat16
+KAISER_TAPS = 32769
+DIM, FFN, N_MELS, CONV_K, MEL_MAXW, MEL_TW, N_FFT, HOP = 512, 2048, 80, 31, 24, 1396, 2048, 512
+
+
+def tensor_specs(lay: int, outdim: int) -> List[Tuple[str, np.dtype, Tuple[int, ...]]]:
+    """The tensors of a model file, in file order: (name, dtype, shape).  ``some_session_open`` expects exactly these."""
+    f32, bf, i32, f64 = np.dtype('<f4'), np.dtype('<u2'), np.dtype('<i4'), np.dtype('<f8')
+    v = []
+    for s in range(2):
+        v += [(f'w_in.{s}', bf, (DIM, N_MELS)), (f'b_in.{s}', f32, (DIM,))]
+    for j in range(2 * (lay + 1)):                   # block i of stream s is entry 2 i + s (some_model.blocks)
+        p = f'blk{j}.'
+        for k in range(5):
+            v += [(f'{p}ln_g.{k}', f32, (DIM,)), (f'{p}ln_b.{k}', f32, (DIM,))]
+        for k in range(2):
+            v += [(f'{p}ffn_w1.{k}', bf, (FFN, DIM)), (f'{p}ffn_b1.{k}', f32, (FFN,)),
+                  (f'{p}ffn_w2.{k}', bf, (DIM, FFN)), (f'{p}ffn_b2.{k}', f32, (DIM,))]
+        v += [(p + 'w_qkv', bf, (3 * DIM, DIM)), (p + 'w_out', bf, (DIM, DIM)), (p + 'b_out', f32, (DIM,)),
+              (p + 'w_pw1', bf, (2 * DIM, DIM)), (p + 'b_pw1', f32, (2 * DIM,)), (p + 'w_dw', f32, (CONV_K, DIM)),
+              (p + 'b_dw', f32, (DIM,)), (p + 'w_pw2', bf, (DIM, DIM)), (p + 'b_pw2', f32, (DIM,))]
+    for j in range(2 * lay):                         # 2 i + 0 = glu1 (fed by midi), 2 i + 1 = glu2
+        v += [(f'glu{j}.w', bf, (2 * DIM, DIM)), (f'glu{j}.b', f32, (2 * DIM,))]
+    v += [('w_head', bf, (outdim, DIM)), ('b_head', f32, ((outdim + 31) // 32 * 32,)), ('w_cut', f32, (DIM,)),
+          ('b_cut', f32, (1,)),
+          ('mel_start', i32, (N_MELS,)), ('mel_count', i32, (N_MELS,)), ('mel_weights', f32, (N_MELS, MEL_MAXW)),
+          ('twiddle', f32, (MEL_TW, 2)), ('window', f32, (N_FFT,)), ('kaiser_best', f64, (KAISER_TAPS,))]
+    return v
+
+
+def write_model_file(path, scalars: dict, tensors: Dict[str, np.ndarray]) -> List[dict]:
+    """Writes a model file (the only writer of the format).  ``scalars``: lay, outdim, quantized, audio_sample_rate,
+    hop_size, win_size (512 / 2048: the mel kernel's), midi_min, midi_max, midi_prob_deviation, rest_threshold,
+    bias_corrected.  ``tensors``: name -> array with the dtype and
+    shape ``tensor_specs`` gives (bf16 as its raw uint16 bits).  Returns the directory as written: one dict per tensor with
+    name, dtype code, shape, offset, nbytes and the byte offset of its directory entry."""
+    if int(scalars['hop_size']) != HOP or int(scalars['win_size']) != N_FFT:
+        raise ValueError(f"hop_size / win_size {scalars['hop_size']} / {scalars['win_size']}: the model file describes "
+                         f'models of hop {HOP} and window {N_FFT} only')
+    specs = tensor_specs(int(scalars['lay']), int(scalars['outdim']))
+    names = [n for n, _, _ in specs]
+    if sorted(names) != sorted(tensors):
+        raise ValueError(f'tensor set differs from the format: missing {sorted(set(names) - set(tensors))}, '
+                         f'unexpected {sorted(set(tensors) - set(names))}')
+    dir_off = HEADER.size
+    data_off = (dir_off + ENTRY.size * len(specs) + ALIGN - 1) // ALIGN * ALIGN
+    entries, off = [], data_off
+    for i, (name, dt, shape) in enumerate(specs):
+        a = tensors[name]
+        if a.dtype != dt or tuple(a.shape) != shape:
+            raise ValueError(f'{name}: {a.dtype} {tuple(a.shape)}, the format needs {dt} {shape}')
+        entries.append({'name': name, 'dtype': DTYPES[dt], 'shape': shape, 'offset': off, 'nbytes': int(a.nbytes),
+                        'entry_offset': dir_off + i * ENTRY.size})
+        off = (off + a.nbytes + ALIGN - 1) // ALIGN * ALIGN
+    file_size = off
+    header = HEADER.pack(MAGIC, FORMAT_VERSION, ABI_VERSION, file_size, dir_off, len(specs), int(scalars['lay']),
+                         int(scalars['outdim']), int(bool(scalars['quantized'])), int(scalars['audio_sample_rate']),
+                         int(scalars['hop_size']), int(scalars['win_size']),
+                         float(scalars['midi_min']), float(scalars['midi_max']), float(scalars['midi_prob_deviation']),
+                         float(scalars['rest_threshold']), int(bool(scalars['bias_corrected'])), data_off)
+    with open(path, 'wb') as f:
+        f.write(header)
+        for e in entries:
+            shape4 = list(e['shape']) + [0] * (4 - len(e['shape']))
+            f.write(ENTRY.pack(e['name'].encode('ascii'), e['dtype'], len(e['shape']), *shape4, e['offset'], e['nbytes']))
+        for e in entries:
+            f.write(b'\0' * (e['offset'] - f.tell()))
+            f.write(np.ascontiguousarray(tensors[e['name']]).tobytes())
+        f.write(b'\0' * (file_size - f.tell()))
+    return entries
+
+
+def engine_tensors(engine) -> Dict[str, np.ndarray]:
+    """The device tensors of a built (and calibrated) engine, under the format's names, as host arrays."""
+    import torch
+
+    from .audio import kaiser_best_table
+
+    def host(t):
+        t = t.detach().contiguous().cpu()
+        return t.view(torch.uint16).numpy() if t.dtype == torch.bfloat16 else t.numpy()
+
+    w, out = engine.w, {}
+    for s in range(2):
+        out[f'w_in.{s}'], out[f'b_in.{s}'] = host(w.w_in[s]), host(w.b_in[s])
+    for i, pair in enumerate(w.blocks):
+        for s, bw in enumerate(pair):
+            p = f'blk{2 * i + s}.'
+            for k in range(5):
+                out[f'{p}ln_g.{k}'], out[f'{p}ln_b.{k}'] = host(bw.ln_g[k]), host(bw.ln_b[k])
+            for k in range(2):
+                f = bw.ffn[k]
+                out[f'{p}ffn_w1.{k}'], out[f'{p}ffn_b1.{k}'] = host(f['w1']), host(f['b1'])
+                out[f'{p}ffn_w2.{k}'], out[f'{p}ffn_b2.{k}'] = host(f['w2']), host(f['b2'])
+            for k in ('w_qkv', 'w_out', 'b_out', 'w_pw1', 'b_pw1', 'w_dw', 'b_dw', 'w_pw2', 'b_pw2'):
+                out[p + k] = host(getattr(bw, k))
+    for i in range(w.lay):
+        for s in range(2):
+            out[f'glu{2 * i + s}.w'], out[f'glu{2 * i + s}.b'] = host(w.glu_w[i][s]), host(w.glu_b[i][s])
+    out['w_head'], out['b_head'], out['w_cut'] = host(w.w_head), host(w.b_head), host(w.w_cut)
+    out['b_cut'] = np.array([w.b_cut], dtype='<f4')
+    for k in ('mel_start', 'mel_count', 'mel_weights', 'twiddle', 'window'):
+        out[k] = host(engine.mel[k])
+    out['kaiser_best'] = np.asarray(kaiser_best_table(), dtype='<f8')
+    return out
+
+
+def export(model_path, out_path=None, device='cuda') -> pathlib.Path:
+    """Builds the default plugin for ``model_path`` (config.yaml beside it) on ``device`` and writes its model file to
+    ``out_path`` (default: the checkpoint path with the suffix ``.somemodel``)."""
+    import yaml
+
+    from .plugin import MIDIExtractionInference, QuantizedMIDIExtractionInference, task_inference_mapping
+    model_path = pathlib.Path(model_path)
+    with open(model_path.with_name('config.yaml'), 'r', encoding='utf8') as f:
+        config = yaml.safe_load(f)
+    cls_name = task_inference_mapping[config['task_cls']].rsplit('.', 1)[-1]
+    cls = {'MIDIExtractionInference': MIDIExtractionInference,
+           'QuantizedMIDIExtractionInference': QuantizedMIDIExtractionInference}[cls_name]
+    ins = cls(config=config, model_path=model_path, device=device)
+    eng = ins.model
+    # calibrate() records every GEMM weight it has seen (and corrected the bias of): empty if it did not run
+    corrected = bool(getattr(eng, '_corrected', None))
+    scalars = {'lay': eng.w.lay, 'outdim': eng.outdim, 'quantized': cls.quantized,
+               'audio_sample_rate': config['audio_sample_rate'], 'hop_size': config.get('hop_size', HOP),
+               'win_size': config.get('win_size', N_FFT), 'midi_min': ins.midi_min, 'midi_max': ins.midi_max,
+               'midi_prob_deviation': ins.midi_deviation, 'rest_threshold': ins.rest_threshold,
+               'bias_corrected': corrected}
+    out_path = pathlib.Path(out_path) if out_path is not None else model_path.with_suffix(SUFFIX)
+    write_model_file(out_path, scalars, engine_tensors(eng))
+    return out_path
+
+
+def main(argv: Sequence[str] = None):
+    ap = argparse.ArgumentParser(prog='python -m some_b200.export',
+                                 description='Export a checkpoint to a self-contained model file for some_session_open')
+    ap.add_argument('--model', required=True, metavar='CKPT_PATH', help='Path to the model checkpoint (*.ckpt)')
+    ap.add_argument('--out', required=False, metavar='PATH', help=f'Path to the output model (default: CKPT{SUFFIX})')
+    args = ap.parse_args(argv)
+    print(f'| exported \'{export(args.model, args.out)}\'')
+
+
+if __name__ == '__main__':
+    main()

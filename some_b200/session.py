@@ -1,0 +1,137 @@
+"""ctypes wrapper of the native session (csrc/session.cu, include/some_b200.h): opens a model file written by
+``python -m some_b200.export`` and transcribes with no torch on the path.  C / C++ hosts call the same functions directly
+(examples/some_transcribe.c); this wrapper serves Python callers that want the same results, the tests and bench_session.py.
+
+Results have the plugin's shape: one dict per clip / chunk with ``note_midi`` f32, ``note_dur`` in seconds
+(``dur * timestep``, float64 as me_infer.py:95) and ``note_rest`` bool, plus ``note_frames`` (the durations in frames)."""
+from __future__ import annotations
+
+import ctypes as C
+import os
+from typing import Dict, List, Optional, Sequence, Tuple
+
+import numpy as np
+
+from . import _lib
+
+
+def slicer_params(threshold: float = -40., min_length: float = 5000, min_interval: float = 300, hop_size: float = 20,
+                  max_sil_kept: float = 1000) -> _lib.SlicerParams:
+    """Slicer constructor arguments (ms / dB) for the session; the defaults are infer.py's Slicer(sr, max_sil_kept=1000)."""
+    return _lib.SlicerParams(threshold, min_length, min_interval, hop_size, max_sil_kept)
+
+
+def slicer_frames(sample_rate: int, params: Optional[_lib.SlicerParams] = None) -> _lib.SlicerFrames:
+    """some_slicer_derive: the frame counts the native slicer uses (host only)."""
+    lib = _lib.load()
+    out = _lib.SlicerFrames()
+    _lib.check(lib.some_slicer_derive(int(sample_rate), C.byref(params) if params is not None else None, C.byref(out)),
+               'some_slicer_derive')
+    return out
+
+
+def slicer_ranges(rms: np.ndarray, num_samples: int, frames: _lib.SlicerFrames) -> List[Tuple[int, int]]:
+    """some_slicer_ranges: the native slicer's chunk ranges for an RMS list (host only, no CUDA call)."""
+    lib = _lib.load()
+    rms = np.ascontiguousarray(rms, dtype=np.float32)
+    cap = rms.shape[0] // 2 + 2
+    out = np.zeros(2 * cap, dtype=np.int64)
+    count = C.c_int()
+    _lib.check(lib.some_slicer_ranges(rms.ctypes.data, int(rms.shape[0]), int(num_samples), C.byref(frames), out.ctypes.data,
+                                      cap, C.byref(count)), 'some_slicer_ranges')
+    return [(int(out[2 * k]), int(out[2 * k + 1])) for k in range(count.value)]
+
+
+class Notes:
+    """A caller-owned result object (some_notes_create / some_notes_destroy)."""
+
+    handle = None
+
+    def __init__(self):
+        self.lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(self.lib.some_notes_create(C.byref(h)), 'some_notes_create')
+        self.handle = h
+
+    def close(self):
+        if self.handle is not None:
+            self.lib.some_notes_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        self.close()
+
+    def results(self, timestep: float) -> Tuple[List[Tuple[int, int]], List[Dict[str, np.ndarray]]]:
+        """(sample range of every clip, notes of every clip) copied out of the native object."""
+        n = self.lib.some_notes_clips(self.handle)
+        if n < 0:
+            _lib.check(n, 'some_notes_clips')
+        ranges, out = [], []
+        cnt, nm, nd, nr = C.c_int(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        a, b = C.c_int64(), C.c_int64()
+        for i in range(n):
+            _lib.check(self.lib.some_notes_get(self.handle, i, C.byref(cnt), C.byref(nm), C.byref(nd), C.byref(nr), C.byref(a),
+                                               C.byref(b)), 'some_notes_get')
+            k = cnt.value
+            midi = np.ctypeslib.as_array(C.cast(nm, C.POINTER(C.c_float)), (k,)).copy() if k else np.zeros(0, np.float32)
+            dur = np.ctypeslib.as_array(C.cast(nd, C.POINTER(C.c_int32)), (k,)).copy() if k else np.zeros(0, np.int32)
+            rest = np.ctypeslib.as_array(C.cast(nr, C.POINTER(C.c_uint8)), (k,)).copy() if k else np.zeros(0, np.uint8)
+            ranges.append((a.value, b.value))
+            out.append({'note_midi': midi, 'note_dur': dur * timestep, 'note_rest': rest.astype(bool), 'note_frames': dur})
+        return ranges, out
+
+
+class Session:
+    """some_session_open(path, device) ... some_session_close."""
+
+    handle = None
+
+    def __init__(self, path, device: int = 0):
+        self.lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(self.lib.some_session_open(os.fsencode(os.fspath(path)), int(device), C.byref(h)), 'some_session_open')
+        self.handle = h
+        info = _lib.SessionInfo()
+        _lib.check(self.lib.some_session_get_info(h, C.byref(info)), 'some_session_get_info')
+        self.sample_rate, self.hop, self.outdim = info.sample_rate, info.hop, info.outdim
+        self.quantized, self.bias_corrected, self.timestep = bool(info.quantized), bool(info.bias_corrected), info.timestep
+
+    def close(self):
+        if self.handle is not None:
+            self.lib.some_session_close(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        self.close()
+
+    def transcribe(self, waveforms: Sequence[np.ndarray], notes: Optional[Notes] = None) -> List[Dict[str, np.ndarray]]:
+        """some_session_transcribe: mono float32 clips at the model's rate -> one dict per clip, in input order."""
+        waves = [np.ascontiguousarray(w, dtype=np.float32) for w in waveforms]
+        ptrs = (C.c_void_p * max(len(waves), 1))(*[w.ctypes.data for w in waves])
+        lens = np.array([w.shape[0] for w in waves] or [0], dtype=np.int64)
+        own = notes is None
+        notes = notes or Notes()
+        try:
+            _lib.check(self.lib.some_session_transcribe(self.handle, ptrs, lens.ctypes.data, len(waves), notes.handle),
+                       'some_session_transcribe')
+            return notes.results(self.timestep)[1]
+        finally:
+            if own:
+                notes.close()
+
+    def transcribe_sliced(self, samples: np.ndarray, sample_rate: Optional[int] = None,
+                          params: Optional[_lib.SlicerParams] = None, notes: Optional[Notes] = None):
+        """some_session_transcribe_sliced: one mono recording (any integer rate) -> (chunk offsets in seconds, chunk sample
+        ranges, per-chunk notes), as Engine.infer_sliced returns offsets and notes."""
+        x = np.ascontiguousarray(samples, dtype=np.float32)
+        own = notes is None
+        notes = notes or Notes()
+        try:
+            _lib.check(self.lib.some_session_transcribe_sliced(
+                self.handle, x.ctypes.data, int(x.shape[0]), int(sample_rate or self.sample_rate),
+                C.byref(params) if params is not None else None, notes.handle), 'some_session_transcribe_sliced')
+            ranges, res = notes.results(self.timestep)
+        finally:
+            if own:
+                notes.close()
+        return [a / self.sample_rate for a, _ in ranges], ranges, res
