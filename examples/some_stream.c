@@ -1,0 +1,96 @@
+/* some_stream: transcribe a recording while it arrives, with a model file written by `python -m some_b200.export`, without
+ * Python.
+ *
+ *   some_stream MODEL RATE [DEVICE] < pcm
+ *
+ * Reads raw mono little-endian float32 samples at RATE Hz from stdin in blocks of 100 ms, pushes each block to a
+ * some_stream and prints the notes of every chunk as soon as it is delivered, one line per note:
+ *
+ *   <chunk offset in seconds> <note_midi> <duration in seconds> <rest 0/1>
+ *
+ * the same lines examples/some_transcribe prints for the whole recording.  Live from a microphone:
+ *
+ *   arecord -f FLOAT_LE -c1 -r 44100 | some_stream model.somemodel 44100 */
+#include <stdint.h>
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include "some_b200.h"
+
+static void print_chunks(const some_notes* notes, const some_session_info* info) {
+  const int chunks = some_notes_clips(notes);
+  for (int c = 0; c < chunks; ++c) {
+    int count = 0;
+    const float* midi;
+    const int32_t* dur;
+    const uint8_t* rest;
+    int64_t begin, end;
+    some_notes_get(notes, c, &count, &midi, &dur, &rest, &begin, &end);
+    const double offset = (double)begin / info->sample_rate;
+    for (int k = 0; k < count; ++k)
+      printf("%.17g %.9g %.17g %d\n", offset, midi[k], (double)dur[k] * info->timestep, rest[k] ? 1 : 0);
+  }
+  fflush(stdout);
+}
+
+int main(int argc, char** argv) {
+  if (argc < 3 || atoi(argv[2]) <= 0) {
+    fprintf(stderr, "usage: %s MODEL RATE [DEVICE] < mono float32 little-endian PCM\n", argv[0]);
+    return 2;
+  }
+  const int rate = atoi(argv[2]);
+  const size_t block = (size_t)(rate / 10 > 0 ? rate / 10 : 1);
+  unsigned char* raw = malloc(4 * block);
+  float* samples = malloc(sizeof(float) * block);
+  some_session* s = NULL;
+  some_stream* st = NULL;
+  some_notes* notes = NULL;
+  some_session_info info;
+  int rc = 1;
+  if (!raw || !samples) goto done;
+  if (some_session_open(argv[1], argc > 3 ? atoi(argv[3]) : 0, &s) != 0 || some_session_get_info(s, &info) != 0 ||
+      some_notes_create(&notes) != 0 || some_stream_open(s, rate, NULL, &st) != 0) {
+    fprintf(stderr, "some_stream: %s\n", some_last_error());
+    goto done;
+  }
+  size_t have = 0;                       /* bytes of the current block read so far */
+  for (;;) {
+    const size_t got = fread(raw + have, 1, 4 * block - have, stdin);
+    have += got;
+    const int eof = got == 0;
+    if (have == 4 * block || (eof && have >= 4)) {
+      const size_t n = have / 4;
+      for (size_t i = 0; i < n; ++i) {
+        const unsigned char* p = raw + 4 * i;
+        const uint32_t u = p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24);
+        memcpy(&samples[i], &u, 4);
+      }
+      memmove(raw, raw + 4 * n, have - 4 * n);
+      have -= 4 * n;
+      if (some_stream_push(st, samples, (long long)n, notes) != 0) {
+        fprintf(stderr, "some_stream: %s\n", some_last_error());
+        goto done;
+      }
+      print_chunks(notes, &info);
+    }
+    if (eof) break;
+  }
+  if (ferror(stdin)) {
+    fprintf(stderr, "some_stream: read error\n");
+    goto done;
+  }
+  if (some_stream_finish(st, notes) != 0) {
+    fprintf(stderr, "some_stream: %s\n", some_last_error());
+    goto done;
+  }
+  print_chunks(notes, &info);
+  rc = 0;
+done:
+  some_stream_close(st);
+  some_notes_destroy(notes);
+  some_session_close(s);
+  free(raw);
+  free(samples);
+  return rc;
+}

@@ -265,6 +265,12 @@ int some_eval_clips(const some_eval_args* args, cudaStream_t stream);
  * rms: device f32 [n_frames], n_frames = 1 + (n_samples + 2 * (frame_length / 2) - frame_length) / hop. */
 int some_slicer_rms(const float* wave, long long n_samples, int frame_length, int hop, float* rms, int n_frames,
                     cudaStream_t stream);
+/* The same frames [f_begin, f_end) of a recording of which the buffer holds samples [base, base + held): wave[s - base] is
+ * sample s; rms[f - f_begin] receives frame f.  n_samples: the recording's length, or -1 while it is not known (every frame
+ * must then read samples before base + held only).  The buffer must hold every sample inside the recording the frames read.
+ * Bit-identical to some_slicer_rms on the whole recording. */
+int some_slicer_rms_window(const float* wave, long long base, long long held, long long n_samples, int frame_length, int hop,
+                           float* rms, long long f_begin, long long f_end, cudaStream_t stream);
 
 /* ---- K-resample (the step in front of the slicer): librosa.resample(y, orig_sr, target_sr, res_type='kaiser_best') as
  * librosa.load calls it (infer.py:34, batch_infer.py:51, webui.py:47; librosa<0.10 -> resampy.resample(filter='kaiser_best')
@@ -280,6 +286,18 @@ int some_slicer_rms(const float* wave, long long n_samples, int frame_length, in
  * Downsampling by more than about 11x is rejected (the input window of a tile no longer fits in shared memory). */
 int some_resample_kaiser(const float* x, const int64_t* x_start, const int64_t* x_len, float* y, const int64_t* y_start, int B,
                          long long max_out, int sr_orig, int sr_new, const double* win, int nwin, cudaStream_t stream);
+/* The same resampling of ONE recording whose input arrives in pieces, by absolute positions: x[i - x_first] is input sample i
+ * (x holds [x_first, received)), y[t - y_first] receives output t, for t in [t_begin, t_end).  final = 0: the recording may
+ * go on, and only outputs whose right wing ends within the received input are computed (t_end up to the plan's);
+ * final != 0: the recording is `received` samples long and outputs up to ceil(received * ratio) include fix_length's zeros.
+ * Bit-identical to some_resample_kaiser on the whole recording.
+ * some_resample_window_plan: *t_end = the outputs [0, *t_end) that `received` input samples fix, *x_first = the first input
+ * sample the outputs from t_begin on read (what a host must keep).  Host only. */
+int some_resample_kaiser_window(const float* x, long long x_first, long long received, int final, float* y, long long y_first,
+                                long long t_begin, long long t_end, int sr_orig, int sr_new, const double* win, int nwin,
+                                cudaStream_t stream);
+int some_resample_window_plan(long long received, int final, long long t_begin, int sr_orig, int sr_new, int nwin,
+                              long long* t_end, long long* x_first);
 
 /* ---- K-flac (the step in front of K-resample): the FLAC decode of librosa.load (soundfile -> libsndfile -> libFLAC) for
  * many recordings in one set of launches, from slices of one device byte buffer `data` (restated in oracle/flac.py).
@@ -566,6 +584,65 @@ int some_notes_get(const some_notes* n, int clip, int* count, const float** note
 int some_slicer_derive(int sample_rate, const some_slicer_params* params, some_slicer_frames* out);
 int some_slicer_ranges(const float* rms, int n_frames, long long n_samples, const some_slicer_frames* frames, int64_t* ranges,
                        int capacity, int* count);
+
+/* The slicer on an RMS list that arrives in pieces (host only, no CUDA call): the same decisions as some_slicer_ranges, each
+ * range returned as soon as no later frame can change it.
+ * some_slicer_stream_feed    the next n_frames RMS frames; `fixed` = the samples known so far, which must complete those frames
+ *                            (frame k reads samples up to k hop_size - win_size / 2 + win_size - 1).  Returns the ranges that
+ *                            became final: the range before a cut silent run once the voiced frame after the run is known, or
+ *                            once the run has lasted to frame max(ss + 2 max_sil_kept, ss + min_interval - 1,
+ *                            chunk begin + min_length - 1) (ss: its first frame), whichever comes first; none while no more
+ *                            than min_length * hop_size samples are fixed (a shorter recording is one chunk).
+ * some_slicer_stream_finish  the frames not fed yet (those that read past the end) and the final length: the remaining ranges,
+ *                            after the trailing-silence and short-recording rules.  No feed after it.
+ * some_slicer_stream_keep_from  what a host must keep of the audio: a range not returned yet begins at or after *sample, or
+ *                            (only during a leading silence longer than max_sil_kept frames: the all-silent recording's
+ *                            range) lies within samples [0, *head) (head may be NULL; 0 when there is no such range); and
+ *                            (rms_held, may be NULL) how many RMS values the stream holds: O(max_sil_kept).
+ * The range pointers stay valid until the next call on the stream.  Concatenated over all calls, the ranges equal
+ * some_slicer_ranges on the whole list (with the short-recording rule of some_session_transcribe_sliced). */
+typedef struct some_slicer_stream some_slicer_stream;
+int some_slicer_stream_create(const some_slicer_frames* frames, some_slicer_stream** out);
+int some_slicer_stream_feed(some_slicer_stream* st, const float* rms, int n_frames, long long fixed, const int64_t** ranges,
+                            int* count);
+int some_slicer_stream_finish(some_slicer_stream* st, const float* rms, int n_frames, long long n_samples, const int64_t** ranges,
+                              int* count);
+int some_slicer_stream_keep_from(const some_slicer_stream* st, long long* sample, long long* head, long long* rms_held);
+int some_slicer_stream_destroy(some_slicer_stream* st);
+
+/* ---- Streaming (csrc/session.cu): transcribe a recording while it is still arriving.  Push samples as they come; each push
+ * returns, in `out`, the chunks that became final (zero, one or several), and some_stream_finish the rest.  Concatenated in
+ * order, the chunks of all pushes and the finish equal some_session_transcribe_sliced on the whole recording at the same rate
+ * and params: the same [begin, end) (absolute positions at the model's rate) and bit-identical notes, however the recording is
+ * split into pushes.  A chunk is delivered by the push that makes known the first voiced frame after the silent run that ends
+ * it, or frame max(ss + 2 max_sil_kept, ss + min_interval - 1, chunk begin + min_length - 1) of a longer run (see
+ * some_slicer_stream_feed).  With the default params at 44.1 kHz: when singing resumes after at least 300 ms of silence, or at
+ * the latest about 2.1 s into a longer silence.  A frame is known once the samples it reads are fixed: at the model's rate
+ * when they are received; at another rate once the resampler's right wing behind them has been received (<= 64 input samples
+ * when upsampling, nwin / index_step when downsampling).
+ *   Each push uploads its samples through pinned memory, resamples the outputs they fix (some_resample_kaiser_window),
+ * computes the RMS frames those complete (some_slicer_rms_window), downloads them with one synchronise, takes the slicer's
+ * decisions on the host and transcribes the final chunks where they lie in the stream's device buffer.  The buffer keeps
+ * only what a later chunk or RMS frame can read: `held` stays within the longest chunk plus 2 max_sil_kept frames and the
+ * RMS window (during a long leading silence: the first and the last max_sil_kept frames and the RMS window), plus the push in
+ * progress, however long the recording or its silences; until more than min_length hops are fixed (the recording may still
+ * prove to be one chunk) it holds everything so far.
+ *   Any number of streams may share a session, from different threads: each GPU step takes the session's mutex.  One stream
+ * is used by one thread at a time.  sample_rate: any integer rate (params NULL: Slicer(sr, max_sil_kept=1000)).  At finish, a
+ * recording too short to resample is refused as resampy refuses it; an empty stream finishes like transcribe_sliced on zero
+ * samples.  No push after finish.  Close a session's streams before the session: a stream uses its session's device, streams
+ * and buffers. */
+typedef struct some_stream some_stream;
+typedef struct {
+  int64_t received; /* samples pushed, at the stream's rate */
+  int64_t fixed;    /* model-rate samples whose values can no longer change */
+  int64_t held;     /* model-rate samples resident on the device */
+} some_stream_info;
+int some_stream_open(some_session* s, int sample_rate, const some_slicer_params* params, some_stream** out);
+int some_stream_push(some_stream* st, const float* samples, long long n, some_notes* out);
+int some_stream_finish(some_stream* st, some_notes* out);
+int some_stream_get_info(const some_stream* st, some_stream_info* info);
+int some_stream_close(some_stream* st);
 
 #ifdef __cplusplus
 }

@@ -132,6 +132,10 @@ class SlicerFrames(C.Structure):
                 ('min_interval', C.c_int), ('max_sil_kept', C.c_int)]
 
 
+class StreamInfo(C.Structure):
+    _fields_ = [('received', C.c_int64), ('fixed', C.c_int64), ('held', C.c_int64)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     'some_version': (C.c_int, []),
@@ -156,6 +160,12 @@ EXPORTS = {
     'some_eval_clips': (C.c_int, [C.POINTER(EvalArgs), _vp]),
     'some_slicer_rms': (C.c_int, [_vp, C.c_longlong, C.c_int, C.c_int, _vp, C.c_int, _vp]),
     'some_resample_kaiser': (C.c_int, [_vp, _vp, _vp, _vp, _vp, C.c_int, C.c_longlong, C.c_int, C.c_int, _vp, C.c_int, _vp]),
+    'some_slicer_rms_window': (C.c_int, [_vp, C.c_longlong, C.c_longlong, C.c_longlong, C.c_int, C.c_int, _vp, C.c_longlong,
+                                         C.c_longlong, _vp]),
+    'some_resample_kaiser_window': (C.c_int, [_vp, C.c_longlong, C.c_longlong, C.c_int, _vp, C.c_longlong, C.c_longlong,
+                                              C.c_longlong, C.c_int, C.c_int, _vp, C.c_int, _vp]),
+    'some_resample_window_plan': (C.c_int, [C.c_longlong, C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_int,
+                                            C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]),
     'some_flac_scan_workspace_bytes': (C.c_uint64, [C.c_longlong]),
     'some_flac_scan': (C.c_int, [_vp, C.c_longlong, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp]),
     'some_flac_decode': (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp, C.c_int, _vp, _vp]),
@@ -184,6 +194,17 @@ EXPORTS = {
     'some_slicer_derive': (C.c_int, [C.c_int, C.POINTER(SlicerParams), C.POINTER(SlicerFrames)]),
     'some_slicer_ranges': (C.c_int, [_vp, C.c_int, C.c_longlong, C.POINTER(SlicerFrames), _vp, C.c_int,
                                      C.POINTER(C.c_int)]),
+    'some_slicer_stream_create': (C.c_int, [C.POINTER(SlicerFrames), C.POINTER(_vp)]),
+    'some_slicer_stream_feed': (C.c_int, [_vp, _vp, C.c_int, C.c_longlong, C.POINTER(_vp), C.POINTER(C.c_int)]),
+    'some_slicer_stream_finish': (C.c_int, [_vp, _vp, C.c_int, C.c_longlong, C.POINTER(_vp), C.POINTER(C.c_int)]),
+    'some_slicer_stream_keep_from': (C.c_int, [_vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
+                                               C.POINTER(C.c_longlong)]),
+    'some_slicer_stream_destroy': (C.c_int, [_vp]),
+    'some_stream_open': (C.c_int, [_vp, C.c_int, C.POINTER(SlicerParams), C.POINTER(_vp)]),
+    'some_stream_push': (C.c_int, [_vp, _vp, C.c_longlong, _vp]),
+    'some_stream_finish': (C.c_int, [_vp, _vp]),
+    'some_stream_get_info': (C.c_int, [_vp, C.POINTER(StreamInfo)]),
+    'some_stream_close': (C.c_int, [_vp]),
 }
 
 _lib = None

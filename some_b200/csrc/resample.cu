@@ -16,6 +16,8 @@
 // signal's edges, the end of the table) is skipped, exactly like resampy's loop bounds.
 #include <math.h>
 
+#include <algorithm>
+
 #include "host_common.h"
 
 #include "../../include/some_b200.h"
@@ -43,6 +45,9 @@ struct ResampleParams {
   double scale;      // min(1, ratio)
   int step;          // index_step = int(scale * 512)
   int max_taps;      // nwin / step: the longest wing
+  // window variant (one recording, absolute positions): x[i - x_first] is input sample i, y[t - y_first] output t; the
+  // outputs [t_begin, t_end) of a recording whose input is `len` samples long (as far as the wing limits see it) are written
+  long long x_first, y_first, t_begin, t_end, len;
 };
 
 // One wing (left = taps x[n - i], right = x[n + 1 + k]) for this thread's RS_OPT outputs.  xi[k] is the window index of
@@ -88,24 +93,29 @@ __device__ __forceinline__ void table_pos(double frac, int& off, double& eta) {
   eta = __dsub_rn(index_frac, static_cast<double>(off));
 }
 
+// kWindow = false: the batched form, recording b = blockIdx.y whole.  kWindow = true: outputs [t_begin, t_end) of one recording
+// from a buffer that holds only part of its input.  Every output's arithmetic depends on its absolute position t alone (n, the
+// table position, the wing limits against 0 and len), not on the tile it falls in, so both forms give the same bits.
+template <bool kWindow>
 __global__ void __launch_bounds__(RS_THREADS, 2) resample_kaiser_kernel(const ResampleParams p) {
   extern __shared__ double rs_smem[];
   const int b = blockIdx.y;
-  const long long L = p.x_len[b];
+  const long long L = kWindow ? p.len : p.x_len[b];
   const long long n_total = static_cast<long long>(ceil(__dmul_rn(static_cast<double>(L), p.ratio)));   // fix_length
   const long long n_out = L * p.sr_new / p.sr_orig;                                                       // resampy's length
-  const long long t0 = static_cast<long long>(blockIdx.x) * RS_TILE;
-  if (t0 >= n_total) return;
-  float* y = p.y + p.y_start[b];
+  const long long t0 = (kWindow ? p.t_begin : 0) + static_cast<long long>(blockIdx.x) * RS_TILE;
+  const long long t_stop = kWindow ? min(p.t_end, n_total) : n_total;
+  if (t0 >= t_stop) return;
+  float* y = p.y + (kWindow ? -p.y_first : p.y_start[b]);   // y[t]: output t
   float acc[RS_OPT];
 #pragma unroll
   for (int k = 0; k < RS_OPT; ++k) acc[k] = 0.f;
 
   if (t0 < n_out) {                                         // uniform over the CTA
-    const float* x = p.x + p.x_start[b];
+    const float* x = p.x + (kWindow ? -p.x_first : p.x_start[b]);   // x[i]: input sample i
     double* tab = rs_smem;
     double* xs = rs_smem + RS_CHUNK * p.step + 2;
-    const long long t_last = min(t0 + RS_TILE, n_out) - 1;
+    const long long t_last = min(t0 + RS_TILE, min(t_stop, n_out)) - 1;
     const long long n_first = static_cast<long long>(__dmul_rn(static_cast<double>(t0), p.inc));
     const long long n_last = static_cast<long long>(__dmul_rn(static_cast<double>(t_last), p.inc));
     const long long lo = max(0ll, n_first - p.max_taps + 1);
@@ -122,7 +132,7 @@ __global__ void __launch_bounds__(RS_THREADS, 2) resample_kaiser_kernel(const Re
       frac[k] = __dmul_rn(p.scale, __dsub_rn(tr, static_cast<double>(n)));
       table_pos(frac[k], off[k], eta[k]);
       xi[k] = static_cast<int>(n - lo);
-      lim[k] = t < n_out ? static_cast<int>(min(n + 1, static_cast<long long>((p.nwin - off[k]) / p.step))) : 0;
+      lim[k] = t <= t_last ? static_cast<int>(min(n + 1, static_cast<long long>((p.nwin - off[k]) / p.step))) : 0;
     }
     wing<true>(p, tab, xs, xi, lim, off, eta, acc);
 #pragma unroll
@@ -131,15 +141,60 @@ __global__ void __launch_bounds__(RS_THREADS, 2) resample_kaiser_kernel(const Re
       const long long n = lo + xi[k];
       table_pos(__dsub_rn(p.scale, frac[k]), off[k], eta[k]);
       xi[k] += 1;
-      lim[k] = t < n_out ? static_cast<int>(max(0ll, min(L - n - 1, static_cast<long long>((p.nwin - off[k]) / p.step)))) : 0;
+      lim[k] = t <= t_last ? static_cast<int>(max(0ll, min(L - n - 1, static_cast<long long>((p.nwin - off[k]) / p.step)))) : 0;
     }
     wing<false>(p, tab, xs, xi, lim, off, eta, acc);
   }
 #pragma unroll
   for (int k = 0; k < RS_OPT; ++k) {
     const long long t = t0 + threadIdx.x + k * RS_THREADS;
-    if (t < n_total) y[t] = acc[k];                         // 0 beyond resampy's n_out: fix_length's zero padding
+    if (t < t_stop) y[t] = acc[k];                          // 0 beyond resampy's n_out: fix_length's zero padding
   }
+}
+
+
+// The rate-pair constants of resampy.resample and the kernel's shared-memory size for them.
+int setup(ResampleParams& p, int sr_orig, int sr_new, int nwin, const char* what, double* smem) {
+  SOME_REQUIRE(sr_orig > 0 && sr_new > 0, "%s: invalid sample rates %d -> %d", what, sr_orig, sr_new);
+  SOME_REQUIRE(nwin >= 2, "%s: table of %d entries", what, nwin);
+  p.nwin = nwin;
+  p.sr_orig = sr_orig, p.sr_new = sr_new;
+  p.ratio = static_cast<double>(sr_new) / static_cast<double>(sr_orig);
+  p.inc = 1.0 / p.ratio;
+  p.scale = p.ratio < 1.0 ? p.ratio : 1.0;
+  p.step = static_cast<int>(p.scale * RS_NUM_TABLE);
+  SOME_REQUIRE(p.step >= 1, "%s: %d -> %d is below the table's resolution", what, sr_orig, sr_new);
+  p.max_taps = nwin / p.step;
+  // input window: n_last - n_first <= ceil((RS_TILE - 1) * inc) + 1, plus the taps on both sides
+  const double x_cap = ceil((RS_TILE - 1) * p.inc) + 2.0 * p.max_taps + 4.0;
+  *smem = 8.0 * (RS_CHUNK * p.step + 2 + x_cap);
+  SOME_REQUIRE(*smem <= RS_MAX_SMEM, "%s: %d -> %d needs %.0f B of shared memory (downsampling by more than "
+               "about 11x is not supported)", what, sr_orig, sr_new, *smem);
+  return 0;
+}
+
+// Output t reads input samples floor(t * inc) - max_taps + 1 .. floor(t * inc) + max_taps (clipped to [0, len)), with
+// floor(t * inc) the same double product the kernel forms.
+long long centre(const ResampleParams& p, long long t) { return static_cast<long long>(static_cast<double>(t) * p.inc); }
+
+// The outputs [0, *t_end) that `received` input samples fix, and the first input sample outputs from t_begin on read.  While
+// the recording may go on (final == 0), an output is fixed when its right wing ends before `received`: then its wing limit
+// min(len - n - 1, (nwin - offset) / step) is the table's whatever the final length, and t < received * sr_new / sr_orig
+// keeps it below resampy's n_out.  At the end (final != 0) every output up to fix_length's ceil(len * ratio) is fixed.
+void plan(const ResampleParams& p, long long received, int final, long long t_begin, long long* t_end, long long* x_first) {
+  if (final) {
+    *t_end = static_cast<long long>(ceil(static_cast<double>(received) * p.ratio));
+  } else {
+    const long long last = received - 1 - p.max_taps;       // the largest centre whose right wing is received
+    long long t = 0;
+    if (last >= 0) {
+      t = static_cast<long long>(static_cast<double>(last + 1) * p.ratio);
+      while (t > 0 && centre(p, t - 1) > last) --t;         // centre() is monotone in t
+      while (centre(p, t) <= last) ++t;
+    }
+    *t_end = std::min(t, received * p.sr_new / p.sr_orig);
+  }
+  *x_first = std::max(0ll, centre(p, t_begin) - p.max_taps + 1);
 }
 
 }  // namespace some
@@ -154,24 +209,53 @@ extern "C" int some_resample_kaiser(const float* x, const int64_t* x_start, cons
   SOME_REQUIRE(sr_orig > 0 && sr_new > 0, "some_resample_kaiser: invalid sample rates %d -> %d", sr_orig, sr_new);
   SOME_REQUIRE(nwin >= 2, "some_resample_kaiser: table of %d entries", nwin);
   if (B == 0 || max_out == 0) return 0;
-  ResampleParams p;
-  p.x = x, p.x_start = x_start, p.x_len = x_len, p.y = y, p.y_start = y_start, p.win = win, p.nwin = nwin;
-  p.sr_orig = sr_orig, p.sr_new = sr_new;
-  p.ratio = static_cast<double>(sr_new) / static_cast<double>(sr_orig);
-  p.inc = 1.0 / p.ratio;
-  p.scale = p.ratio < 1.0 ? p.ratio : 1.0;
-  p.step = static_cast<int>(p.scale * RS_NUM_TABLE);
-  SOME_REQUIRE(p.step >= 1, "some_resample_kaiser: %d -> %d is below the table's resolution", sr_orig, sr_new);
-  p.max_taps = nwin / p.step;
-  // input window: n_last - n_first <= ceil((RS_TILE - 1) * inc) + 1, plus the taps on both sides
-  const double x_cap = ceil((RS_TILE - 1) * p.inc) + 2.0 * p.max_taps + 4.0;
-  const double smem = 8.0 * (RS_CHUNK * p.step + 2 + x_cap);
-  SOME_REQUIRE(smem <= RS_MAX_SMEM, "some_resample_kaiser: %d -> %d needs %.0f B of shared memory (downsampling by more than "
-               "about 11x is not supported)", sr_orig, sr_new, smem);
+  ResampleParams p{};
+  double smem;
+  if (setup(p, sr_orig, sr_new, nwin, "some_resample_kaiser", &smem)) return -1;
+  p.x = x, p.x_start = x_start, p.x_len = x_len, p.y = y, p.y_start = y_start, p.win = win;
   const long long tiles = (max_out + RS_TILE - 1) / RS_TILE;
   SOME_REQUIRE(tiles < (1ll << 31), "some_resample_kaiser: grid too large");
-  cudaError_t e = cudaFuncSetAttribute(resample_kaiser_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  cudaError_t e = cudaFuncSetAttribute(resample_kaiser_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(smem));
   SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(resample): %s", cudaGetErrorString(e));
-  resample_kaiser_kernel<<<dim3(static_cast<unsigned>(tiles), B), RS_THREADS, static_cast<size_t>(smem), stream>>>(p);
+  resample_kaiser_kernel<false><<<dim3(static_cast<unsigned>(tiles), B), RS_THREADS, static_cast<size_t>(smem), stream>>>(p);
   return check_launch("some_resample_kaiser");
+}
+
+extern "C" int some_resample_window_plan(long long received, int final, long long t_begin, int sr_orig, int sr_new, int nwin,
+                                         long long* t_end, long long* x_first) {
+  SOME_REQUIRE(t_end && x_first && received >= 0 && t_begin >= 0, "some_resample_window_plan: bad arguments");
+  ResampleParams p{};
+  double smem;
+  if (setup(p, sr_orig, sr_new, nwin, "some_resample_window_plan", &smem)) return -1;
+  plan(p, received, final, t_begin, t_end, x_first);
+  return 0;
+}
+
+extern "C" int some_resample_kaiser_window(const float* x, long long x_first, long long received, int final, float* y,
+                                           long long y_first, long long t_begin, long long t_end, int sr_orig, int sr_new,
+                                           const double* win, int nwin, cudaStream_t stream) {
+  SOME_REQUIRE(x && y && win, "some_resample_kaiser_window: null pointer");
+  ResampleParams p{};
+  double smem;
+  if (setup(p, sr_orig, sr_new, nwin, "some_resample_kaiser_window", &smem)) return -1;
+  long long fixed_end, need_first;
+  plan(p, received, final, t_begin, &fixed_end, &need_first);
+  SOME_REQUIRE(x_first >= 0 && x_first <= received && t_begin >= 0 && t_begin <= t_end && y_first <= t_begin,
+               "some_resample_kaiser_window: bad window (input from %lld of %lld, outputs [%lld, %lld) at %lld)", x_first,
+               received, t_begin, t_end, y_first);
+  SOME_REQUIRE(t_end <= fixed_end, "some_resample_kaiser_window: outputs up to %lld requested, %lld received input samples "
+               "fix %lld%s", t_end, received, fixed_end, final ? "" : " (their right wings would reach past the input)");
+  SOME_REQUIRE(x_first <= need_first || t_begin == t_end, "some_resample_kaiser_window: output %lld reads input from %lld, "
+               "the buffer starts at %lld", t_begin, need_first, x_first);
+  if (t_begin == t_end) return 0;
+  p.x = x, p.y = y, p.win = win;
+  p.x_first = x_first, p.y_first = y_first, p.t_begin = t_begin, p.t_end = t_end, p.len = received;
+  const long long tiles = (t_end - t_begin + RS_TILE - 1) / RS_TILE;
+  SOME_REQUIRE(tiles < (1ll << 31), "some_resample_kaiser_window: grid too large");
+  cudaError_t e = cudaFuncSetAttribute(resample_kaiser_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(smem));
+  SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(resample): %s", cudaGetErrorString(e));
+  resample_kaiser_kernel<true><<<dim3(static_cast<unsigned>(tiles), 1), RS_THREADS, static_cast<size_t>(smem), stream>>>(p);
+  return check_launch("some_resample_kaiser_window");
 }

@@ -10,17 +10,20 @@
 // reference.  13.2 M samples (5 min) -> 15 001 frames x 3528 samples: ~53 M multiply-adds, L1 / L2 resident.
 #include "host_common.h"
 
+#include <algorithm>
+
 #include "../../include/some_b200.h"
 
 namespace some {
 
 struct RmsWindow {
-  const float* wave;
+  const float* wave;  // wave[s - base] is sample s
+  long long base;
   long long n_samples;
   long long first;  // sample index of window element 0 (may be negative: zero padding)
   __device__ __forceinline__ float sq(int k) const {
     const long long s = first + k;
-    const float v = (s >= 0 && s < n_samples) ? __ldg(wave + s) : 0.f;
+    const float v = (s >= 0 && s < n_samples) ? __ldg(wave + (s - base)) : 0.f;
     return __fmul_rn(v, v);
   }
 };
@@ -48,11 +51,15 @@ __device__ __forceinline__ float rms_block(const RmsWindow& w, int lo, int n) {
 
 constexpr int RMS_MAX_DEPTH = 24;  // frame_length < 128 * 2^24
 
-__global__ void __launch_bounds__(128) slicer_rms_kernel(const float* __restrict__ wave, long long n_samples, int frame_length,
-                                                         int hop, float* __restrict__ rms, int n_frames) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= n_frames) return;
-  RmsWindow w{wave, n_samples, static_cast<long long>(f) * hop - frame_length / 2};
+// Frames [f_begin, f_begin + n_frames) into rms[0, n_frames): a frame's value depends on its absolute index and the samples
+// alone, so a window of frames over a buffer holding part of the recording gives the whole-recording bits.
+__global__ void __launch_bounds__(128) slicer_rms_kernel(const float* __restrict__ wave, long long base, long long n_samples,
+                                                         int frame_length, int hop, float* __restrict__ rms, long long f_begin,
+                                                         int n_frames) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_frames) return;
+  const long long f = f_begin + i;
+  RmsWindow w{wave, base, n_samples, f * hop - frame_length / 2};
   float total;
   if (frame_length < 8) {
     total = w.sq(0);
@@ -90,7 +97,7 @@ __global__ void __launch_bounds__(128) slicer_rms_kernel(const float* __restrict
     }
     total = ret;
   }
-  rms[f] = __fsqrt_rn(__fdiv_rn(total, static_cast<float>(frame_length)));
+  rms[i] = __fsqrt_rn(__fdiv_rn(total, static_cast<float>(frame_length)));
 }
 
 }  // namespace some
@@ -106,6 +113,32 @@ extern "C" int some_slicer_rms(const float* wave, long long n_samples, int frame
   SOME_REQUIRE(padded >= frame_length && n_frames == 1 + (padded - frame_length) / hop,
                "some_slicer_rms: n_frames %d does not match %lld samples, window %d, hop %d", n_frames, n_samples, frame_length, hop);
   if (n_frames == 0) return 0;
-  slicer_rms_kernel<<<(n_frames + 127) / 128, 128, 0, stream>>>(wave, n_samples, frame_length, hop, rms, n_frames);
+  slicer_rms_kernel<<<(n_frames + 127) / 128, 128, 0, stream>>>(wave, 0, n_samples, frame_length, hop, rms, 0, n_frames);
   return check_launch("some_slicer_rms");
+}
+
+extern "C" int some_slicer_rms_window(const float* wave, long long base, long long held, long long n_samples, int frame_length,
+                                      int hop, float* rms, long long f_begin, long long f_end, cudaStream_t stream) {
+  SOME_REQUIRE(wave && rms, "some_slicer_rms_window: null pointer");
+  SOME_REQUIRE(base >= 0 && held >= 0 && n_samples >= -1 && frame_length >= 1 && hop >= 1 && f_begin >= 0 && f_end >= f_begin &&
+                   f_end - f_begin < (1ll << 31),
+               "some_slicer_rms_window: bad sizes");
+  if (f_end == f_begin) return 0;
+  const long long half = frame_length / 2;
+  const bool final = n_samples >= 0;
+  if (final) {
+    const long long padded = n_samples + 2 * half;
+    SOME_REQUIRE(padded >= frame_length && f_end <= 1 + (padded - frame_length) / hop,
+                 "some_slicer_rms_window: frame %lld is past the last frame of %lld samples", f_end - 1, n_samples);
+  }
+  // the samples the frames read that lie inside the recording: the buffer must hold them
+  const long long lo = std::max(0ll, f_begin * hop - half);
+  const long long hi = (f_end - 1) * hop - half + frame_length;
+  const long long hi_in = final ? std::min(hi, n_samples) : hi;
+  SOME_REQUIRE(lo >= base && hi_in <= base + held,
+               "some_slicer_rms_window: frames [%lld, %lld) read samples [%lld, %lld), the buffer holds [%lld, %lld)%s", f_begin,
+               f_end, lo, hi_in, base, base + held, final ? "" : " (the recording's length is not known yet)");
+  slicer_rms_kernel<<<static_cast<unsigned>((f_end - f_begin + 127) / 128), 128, 0, stream>>>(
+      wave, base, final ? n_samples : base + held, frame_length, hop, rms, f_begin, static_cast<int>(f_end - f_begin));
+  return check_launch("some_slicer_rms_window");
 }

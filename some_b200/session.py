@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import weakref
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -40,6 +41,56 @@ def slicer_ranges(rms: np.ndarray, num_samples: int, frames: _lib.SlicerFrames) 
     _lib.check(lib.some_slicer_ranges(rms.ctypes.data, int(rms.shape[0]), int(num_samples), C.byref(frames), out.ctypes.data,
                                       cap, C.byref(count)), 'some_slicer_ranges')
     return [(int(out[2 * k]), int(out[2 * k + 1])) for k in range(count.value)]
+
+
+class SlicerStream:
+    """some_slicer_stream_*: the slicer's decisions on an RMS list that arrives in pieces (host only, no CUDA call)."""
+
+    handle = None
+
+    def __init__(self, frames: _lib.SlicerFrames):
+        self.lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(self.lib.some_slicer_stream_create(C.byref(frames), C.byref(h)), 'some_slicer_stream_create')
+        self.handle = h
+
+    @staticmethod
+    def _ranges(ptr, count) -> List[Tuple[int, int]]:
+        if count.value == 0:
+            return []
+        a = np.ctypeslib.as_array(C.cast(ptr, C.POINTER(C.c_int64)), (2 * count.value,))
+        return [(int(a[2 * k]), int(a[2 * k + 1])) for k in range(count.value)]
+
+    def feed(self, rms: np.ndarray, fixed: int) -> List[Tuple[int, int]]:
+        """The next RMS frames and the samples fixed so far -> the [begin, end) sample ranges that became final."""
+        rms = np.ascontiguousarray(rms, dtype=np.float32)
+        ptr, count = C.c_void_p(), C.c_int()
+        _lib.check(self.lib.some_slicer_stream_feed(self.handle, rms.ctypes.data, int(rms.shape[0]), int(fixed), C.byref(ptr),
+                                                    C.byref(count)), 'some_slicer_stream_feed')
+        return self._ranges(ptr, count)
+
+    def finish(self, rms: np.ndarray, num_samples: int) -> List[Tuple[int, int]]:
+        """The frames not fed yet and the final length -> the remaining ranges."""
+        rms = np.ascontiguousarray(rms, dtype=np.float32)
+        ptr, count = C.c_void_p(), C.c_int()
+        _lib.check(self.lib.some_slicer_stream_finish(self.handle, rms.ctypes.data, int(rms.shape[0]), int(num_samples),
+                                                      C.byref(ptr), C.byref(count)), 'some_slicer_stream_finish')
+        return self._ranges(ptr, count)
+
+    def keep_from(self) -> Tuple[int, int, int]:
+        """(sample a range not returned yet begins at or after, unless it lies within [0, head); head; RMS values held)."""
+        a, h, b = C.c_longlong(), C.c_longlong(), C.c_longlong()
+        _lib.check(self.lib.some_slicer_stream_keep_from(self.handle, C.byref(a), C.byref(h), C.byref(b)),
+                   'some_slicer_stream_keep_from')
+        return a.value, h.value, b.value
+
+    def close(self):
+        if self.handle is not None:
+            self.lib.some_slicer_stream_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        self.close()
 
 
 class Notes:
@@ -91,13 +142,17 @@ class Session:
         h = C.c_void_p()
         _lib.check(self.lib.some_session_open(os.fsencode(os.fspath(path)), int(device), C.byref(h)), 'some_session_open')
         self.handle = h
+        self._streams = weakref.WeakSet()      # closed before the session: a stream uses the session's device state
         info = _lib.SessionInfo()
         _lib.check(self.lib.some_session_get_info(h, C.byref(info)), 'some_session_get_info')
         self.sample_rate, self.hop, self.outdim = info.sample_rate, info.hop, info.outdim
         self.quantized, self.bias_corrected, self.timestep = bool(info.quantized), bool(info.bias_corrected), info.timestep
 
     def close(self):
+        """Closes the session and, first, every stream still open on it."""
         if self.handle is not None:
+            for st in list(self._streams):
+                st.close()
             self.lib.some_session_close(self.handle)
             self.handle = None
 
@@ -135,3 +190,59 @@ class Session:
             if own:
                 notes.close()
         return [a / self.sample_rate for a, _ in ranges], ranges, res
+
+    def stream(self, sample_rate: Optional[int] = None, params: Optional[_lib.SlicerParams] = None) -> 'Stream':
+        """some_stream_open: a recording pushed while it arrives (see Stream)."""
+        return Stream(self, sample_rate, params)
+
+
+class Stream:
+    """some_stream_*: push samples as they arrive; push() and finish() return the chunks that became final, in the shape
+    transcribe_sliced returns them (offsets in seconds, sample ranges at the model's rate, notes).  Concatenated over all calls
+    they equal transcribe_sliced on the whole recording.  Also a context manager (close() on exit)."""
+
+    handle = None
+    notes = None
+
+    def __init__(self, session: Session, sample_rate: Optional[int] = None, params: Optional[_lib.SlicerParams] = None):
+        self.lib, self.session = session.lib, session
+        h = C.c_void_p()
+        _lib.check(self.lib.some_stream_open(session.handle, int(sample_rate or session.sample_rate),
+                                             C.byref(params) if params is not None else None, C.byref(h)), 'some_stream_open')
+        self.handle = h
+        self.notes = Notes()
+        session._streams.add(self)
+
+    def _results(self):
+        ranges, res = self.notes.results(self.session.timestep)
+        return [a / self.session.sample_rate for a, _ in ranges], ranges, res
+
+    def push(self, samples: np.ndarray):
+        x = np.ascontiguousarray(samples, dtype=np.float32)
+        _lib.check(self.lib.some_stream_push(self.handle, x.ctypes.data, int(x.shape[0]), self.notes.handle), 'some_stream_push')
+        return self._results()
+
+    def finish(self):
+        _lib.check(self.lib.some_stream_finish(self.handle, self.notes.handle), 'some_stream_finish')
+        return self._results()
+
+    def info(self) -> Dict[str, int]:
+        i = _lib.StreamInfo()
+        _lib.check(self.lib.some_stream_get_info(self.handle, C.byref(i)), 'some_stream_get_info')
+        return {'received': i.received, 'fixed': i.fixed, 'held': i.held}
+
+    def close(self):
+        if self.handle is not None:
+            self.lib.some_stream_close(self.handle)
+            self.handle = None
+        if self.notes is not None:
+            self.notes.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        self.close()
