@@ -32,9 +32,9 @@ def kernel_times(rate, block, sr=44100, reps=200):
     """CUDA-event time of the windowed launches a push of `block` samples makes (resampling when rate != sr, then the RMS
     frames those samples complete), replayed on their own at a fixed position: a stand-in, not a time taken inside a push."""
     import torch
-    from some_b200 import _lib, audio, session as nsess
+    from some_b200 import _lib, audio, slicer
     lib = _lib.load()
-    f = nsess.slicer_frames(sr)
+    f = slicer.slicer_frames(sr)
     x = torch.randn(rate * 4, device='cuda') * 0.1
     stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     out = torch.empty(sr * 4, device='cuda')

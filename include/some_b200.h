@@ -579,14 +579,15 @@ int some_notes_get(const some_notes* n, int clip, int* count, const float** note
                    const uint8_t** note_rest, int64_t* begin, int64_t* end); /* any output pointer may be NULL */
 /* The slicer's decisions on the HOST (no CUDA call): some_slicer_derive fills the frame counts for a sample rate (params NULL:
  * the session's defaults); some_slicer_ranges turns the RMS list of a recording of n_samples samples (some_slicer_rms) into the
- * [begin, end) sample ranges of its chunks, ranges[2 k], ranges[2 k + 1] (silence_tags + chunk_ranges of some_b200/slicer.py).
+ * [begin, end) sample ranges of its chunks, ranges[2 k], ranges[2 k + 1] (the cuts of Slicer.slice, utils/slicer2.py:82-145).
  * *count = the number of ranges; capacity n_frames / 2 + 2 always suffices. */
 int some_slicer_derive(int sample_rate, const some_slicer_params* params, some_slicer_frames* out);
 int some_slicer_ranges(const float* rms, int n_frames, long long n_samples, const some_slicer_frames* frames, int64_t* ranges,
                        int capacity, int* count);
 
 /* The slicer on an RMS list that arrives in pieces (host only, no CUDA call): the same decisions as some_slicer_ranges, each
- * range returned as soon as no later frame can change it.
+ * range returned as soon as no later frame can change it.  Both, and some_slicer_derive, are in csrc/slicer.cu next to the
+ * RMS kernel; the session and the streams below take their cuts from them.
  * some_slicer_stream_feed    the next n_frames RMS frames; `fixed` = the samples known so far, which must complete those frames
  *                            (frame k reads samples up to k hop_size - win_size / 2 + win_size - 1).  Returns the ranges that
  *                            became final: the range before a cut silent run once the voiced frame after the run is known, or
@@ -622,11 +623,11 @@ int some_slicer_stream_destroy(some_slicer_stream* st);
  * when upsampling, nwin / index_step when downsampling).
  *   Each push uploads its samples through pinned memory, resamples the outputs they fix (some_resample_kaiser_window),
  * computes the RMS frames those complete (some_slicer_rms_window), downloads them with one synchronise, takes the slicer's
- * decisions on the host and transcribes the final chunks where they lie in the stream's device buffer.  The buffer keeps
- * only what a later chunk or RMS frame can read: `held` stays within the longest chunk plus 2 max_sil_kept frames and the
- * RMS window (during a long leading silence: the first and the last max_sil_kept frames and the RMS window), plus the push in
- * progress, however long the recording or its silences; until more than min_length hops are fixed (the recording may still
- * prove to be one chunk) it holds everything so far.
+ * decisions on the host (some_slicer_stream_*, csrc/slicer.cu) and transcribes the final chunks where they lie in the
+ * stream's device buffer.  The buffer keeps only what a later chunk or RMS frame can read: `held` stays within the longest
+ * chunk plus 2 max_sil_kept frames and the RMS window (during a long leading silence: the first and the last max_sil_kept
+ * frames and the RMS window), plus the push in progress, however long the recording or its silences; until more than
+ * min_length hops are fixed (the recording may still prove to be one chunk) it holds everything so far.
  *   Any number of streams may share a session, from different threads: each GPU step takes the session's mutex.  One stream
  * is used by one thread at a time.  sample_rate: any integer rate (params NULL: Slicer(sr, max_sil_kept=1000)).  At finish, a
  * recording too short to resample is refused as resampy refuses it; an empty stream finishes like transcribe_sliced on zero

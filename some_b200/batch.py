@@ -36,7 +36,7 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import audio
-from .slicer import Slicer, chunk_ranges, silence_tags
+from .slicer import Slicer, cut_ranges
 
 _NOTE_NAMES = ('C', 'C#', 'D', 'D#', 'E', 'F', 'F#', 'G', 'G#', 'A', 'A#', 'B')
 
@@ -270,11 +270,8 @@ def transcribe_recordings(infer_ins, waveforms: Sequence, slicer: Optional[Slice
     try:
         with torch.cuda.device(eng.device):
             wave_d, bases, lens, flac_status = stage_recordings(eng, target_sr, waveforms, rates)
-            need = [i for i, n in enumerate(lens) if (n + slicer.hop_size - 1) // slicer.hop_size > slicer.min_length]
-            rms_lists = eng.rms_frames_many([wave_d[bases[i]:bases[i] + lens[i]] for i in need], slicer.win_size, slicer.hop_size)
-            per_rec: List[List[Tuple[int, int]]] = [[(0, n)] for n in lens]               # slicer2.py:79-80 (short: one chunk)
-            for i, rms in zip(need, rms_lists):
-                per_rec[i] = chunk_ranges(silence_tags(rms, slicer), rms.shape[0], slicer.hop_size, lens[i])
+            per_rec = cut_ranges(slicer, lens, lambda need: eng.rms_frames_many(
+                [wave_d[bases[i]:bases[i] + lens[i]] for i in need], slicer.win_size, slicer.hop_size))
             flat = [(int(bases[i]) + a, int(bases[i]) + b) for i, rs in enumerate(per_rec) for a, b in rs]
             results: List[Dict[str, np.ndarray]] = []
             if flat:

@@ -8,6 +8,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include "../../include/some_b200.h"
+
 namespace some {
 
 void set_error(const char* fmt, ...);
@@ -55,5 +57,11 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
       return -1;                     \
     }                                \
   } while (0)
+
+// The number of RMS frames whose windows end within the first `fixed` samples (the streaming slicer and the stream).
+inline int64_t frames_within(const some_slicer_frames& f, int64_t fixed) {
+  const int64_t reach = f.win_size - f.win_size / 2;          // frame k reads samples up to k hop - win / 2 + win - 1
+  return fixed < reach ? 0 : (fixed - reach) / f.hop_size + 1;
+}
 
 }  // namespace some

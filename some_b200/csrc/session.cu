@@ -469,325 +469,7 @@ int upload_staged(some_session* s, float* dst, const float* src, int64_t n) {
   return 0;
 }
 
-// The first index of the minimum of rms[a, min(b, n)) (numpy's argmin: the first NaN wins).  `rms` is a pointer to the whole
-// list or a RmsStore of the frames a streaming slicer still holds.
-template <class R>
-int64_t first_min(const R& rms, int64_t n, int64_t a, int64_t b) {
-  b = std::min(b, n);
-  int64_t best = a;
-  for (int64_t i = a; i < b; ++i) {
-    if (isnan(rms[i])) return i;
-    if (rms[i] < rms[best]) best = i;
-  }
-  return best;
-}
-
-using Tag = std::pair<int64_t, int64_t>;
-
-// silence_tags (some_b200/slicer.py, slicer2.py:84-133) for one run of frames with rms < threshold, [s, i): i < total is the
-// voiced frame that ends it, i == total a trailing run.  Returns whether the run is cut, with the frames it removes in `tag`.
-// Reads rms[s .. s + keep] and rms[max(s, i - keep) .. i] only.
-template <class R>
-bool run_tag(const R& rms, int64_t total, const some_slicer_frames& f, int64_t s, int64_t i, int64_t& clip_from, Tag& tag) {
-  const int64_t keep = f.max_sil_kept;
-  if (i == total) {                                       // trailing silence (slicer2.py:129-133)
-    if (total - s < f.min_interval) return false;
-    tag = {first_min(rms, total, s, std::min(total, s + keep) + 1), total + 1};
-    return true;
-  }
-  const bool leading = s == 0 && i > keep;
-  const bool middle = i - s >= f.min_interval && i - clip_from >= f.min_length;
-  if (!(leading || middle)) return false;
-  const int64_t span = i - s;
-  if (span <= keep) {
-    const int64_t cut = first_min(rms, total, s, i + 1);
-    tag = s == 0 ? Tag(0, cut) : Tag(cut, cut);
-    clip_from = cut;
-  } else if (span <= 2 * keep) {
-    const int64_t mid = first_min(rms, total, i - keep, s + keep + 1);
-    const int64_t left = first_min(rms, total, s, s + keep + 1);
-    const int64_t right = first_min(rms, total, i - keep, i + 1);
-    tag = s == 0 ? Tag(0, right) : Tag(std::min(left, mid), std::max(right, mid));
-    clip_from = tag.second;
-  } else {
-    const int64_t left = first_min(rms, total, s, s + keep + 1);
-    const int64_t right = first_min(rms, total, i - keep, i + 1);
-    tag = s == 0 ? Tag(0, right) : Tag(left, right);
-    clip_from = right;
-  }
-  return true;
-}
-
-// The RMS values run_tag can still read while the list arrives frame by frame: none outside a silent run; inside the run
-// that began at frame ss, frames [ss, ss + keep] (`head`, once the run is long) and the last keep + 1 (`tail`), whichever
-// frame ends the run.  O(max_sil_kept) values however long the run.
-class RmsStore {
- public:
-  float operator[](int64_t k) const { return k >= tail_base_ ? tail_[k - tail_base_] : head_[k - head_base_]; }
-  void start(int64_t ss) {
-    head_.clear(), tail_.clear();
-    head_base_ = tail_base_ = ss;
-  }
-  void push(float v, int64_t keep) {
-    tail_.push_back(v);
-    const int64_t end = tail_base_ + static_cast<int64_t>(tail_.size());
-    const int64_t dead = end - keep - 1 - tail_base_;            // frames before the last keep + 1
-    if (dead <= std::max<int64_t>(keep + 1, 64)) return;         // erase in batches
-    if (head_.empty()) head_.assign(tail_.begin(), tail_.begin() + keep + 1);   // tail_base_ == ss here
-    tail_.erase(tail_.begin(), tail_.begin() + dead);
-    tail_base_ += dead;
-  }
-  size_t size() const { return head_.size() + tail_.size(); }
-
- private:
-  std::vector<float> head_, tail_;
-  int64_t head_base_ = 0, tail_base_ = 0;
-};
-
-// silence_tags + chunk_ranges of some_b200/slicer.py on an RMS list that arrives in pieces.  Each range is returned as soon
-// as no later frame can change it:
-//  (a) when the voiced frame that ends a cut run is known: the run's tag, and with it the end of the range before it;
-//  (b) or, for a run that began at ss > 0 and is still silent at frame j = max(ss + 2 keep, ss + min_interval - 1,
-//      clip_from + min_length - 1), at frame j.  Every frame i that can still end the run has i - ss > 2 keep, so the run is
-//      the third case of run_tag (span > 2 keep) with both of its conditions met (i - ss >= min_interval, i - clip_from >=
-//      min_length), and a recording that ends inside the run has total - ss >= min_interval, so the trailing rule cuts it;
-//      both cut the run's start at left = first_min(ss, ss + keep + 1), which frames up to j already fix.  (A run from frame
-//      0 ends no range: the leading rule's (0, right) and the all-silent trailing cut differ, so it waits for (a).)
-// The next range then begins at the run's right cut, which is no earlier than max(ss, i - keep): open_begin().
-// A run from frame 0 that has lasted past frame max(keep, min_interval - 1) (leading_tail()) ends in one of two ways: a voiced
-// frame i > keep makes it a leading cut (0, right) with right >= i - keep, so the next range begins no earlier than
-// known - keep; or the recording ends inside it, and the trailing rule cuts it at left = first_min(0, keep + 1) <= keep, which
-// leaves the one range [0, left) (the all-silent recording).  So during a long leading silence a host keeps the last keep
-// frames and, apart, the first keep frames, not everything since frame 0.
-class SlicerCore {
- public:
-  explicit SlicerCore(const some_slicer_frames& f) : f_(f) {}
-  // frames known() .. known() + n; appends the frame ranges [a, b) that became final to `out`
-  int feed(const float* rms, int64_t n, std::vector<Tag>& out) {
-    const int64_t keep = f_.max_sil_kept;
-    for (int64_t j = 0; j < n; ++j) {
-      const int64_t k = known_++;
-      const float v = rms[j];
-      if (v < f_.threshold) {
-        if (!in_run_) in_run_ = true, ss_ = k, early_ = false, store_.start(k);
-        store_.push(v, keep);
-        if (!early_ && ss_ > 0 &&
-            k >= std::max({ss_ + 2 * keep, ss_ + f_.min_interval - 1, clip_from_ + f_.min_length - 1})) {   // (b)
-          early_first_ = first_min(store_, known_, ss_, ss_ + keep + 1);
-          emit(early_first_, out);
-          early_ = true;
-        }
-      } else if (in_run_) {                                                                                  // (a)
-        store_.push(v, keep);
-        if (end_run(k, out)) return -1;
-      }
-    }
-    return 0;
-  }
-  // the end of the list: the trailing rule and the last range; a range (0, -1) is the whole recording (no cut at all)
-  int finish(std::vector<Tag>& out) {
-    if (in_run_ && end_run(known_, out)) return -1;
-    if (!any_tag_) {
-      out.push_back({0, -1});
-    } else if (prev_ < known_) {
-      out.push_back({prev_, known_});
-    }
-    return 0;
-  }
-  int64_t known() const { return known_; }
-  // the first frame a range not yet returned may begin at
-  int64_t open_begin() const {
-    if (in_run_ && early_) return std::max(ss_, known_ - f_.max_sil_kept);
-    if (leading_tail()) return known_ - f_.max_sil_kept;
-    return any_tag_ ? prev_ : 0;
-  }
-  // a range [0, a) with a <= max_sil_kept may still come besides those from open_begin() on
-  bool leading_tail() const {
-    return in_run_ && ss_ == 0 && known_ > f_.max_sil_kept && known_ >= f_.min_interval;
-  }
-  size_t held() const { return store_.size(); }
-
- private:
-  void emit(int64_t a, std::vector<Tag>& out) {                // chunk_ranges: the frames before a tag starting at a
-    if (any_tag_) {
-      out.push_back({prev_, a});
-    } else if (a > 0) {
-      out.push_back({0, a});
-    }
-  }
-  int end_run(int64_t i, std::vector<Tag>& out) {
-    Tag tag;
-    const bool cut = run_tag(store_, known_, f_, ss_, i, clip_from_, tag);
-    SOME_REQUIRE(!early_ || (cut && tag.first == early_first_),
-                 "slicer: the run from frame %lld was cut early at %lld, its end gives %lld", (long long)ss_,
-                 (long long)early_first_, cut ? (long long)tag.first : -1ll);
-    in_run_ = false;
-    store_.start(known_);
-    if (!cut) return 0;
-    if (!early_) emit(tag.first, out);
-    any_tag_ = true;
-    prev_ = tag.second;
-    return 0;
-  }
-  some_slicer_frames f_;
-  RmsStore store_;
-  int64_t known_ = 0, clip_from_ = 0, ss_ = 0, early_first_ = 0, prev_ = 0;
-  bool in_run_ = false, early_ = false, any_tag_ = false;
-};
-
-// The number of RMS frames whose windows end within the first `fixed` samples.
-int64_t frames_within(const some_slicer_frames& f, int64_t fixed) {
-  const int64_t reach = f.win_size - f.win_size / 2;          // frame k reads samples up to k hop - win / 2 + win - 1
-  return fixed < reach ? 0 : (fixed - reach) / f.hop_size + 1;
-}
-
 }  // namespace
-
-// ---------------------------------------------------------------------------------------------------- slicer decisions
-extern "C" int some_slicer_derive(int sample_rate, const some_slicer_params* p, some_slicer_frames* out) {
-  SOME_REQUIRE(out != nullptr && sample_rate > 0, "some_slicer_derive: bad arguments");
-  some_slicer_params d{-40.0, 5000.0, 300.0, 20.0, 1000.0};    // infer.py: Slicer(sr, max_sil_kept=1000)
-  if (p) d = *p;
-  SOME_REQUIRE(d.min_length_ms >= d.min_interval_ms && d.min_interval_ms >= d.hop_size_ms,
-               "some_slicer_derive: the following condition must be satisfied: min_length >= min_interval >= hop_size");
-  SOME_REQUIRE(d.max_sil_kept_ms >= d.hop_size_ms,
-               "some_slicer_derive: the following condition must be satisfied: max_sil_kept >= hop_size");
-  // Slicer.__init__ (some_b200/slicer.py), with Python's round (half to even: rint in the default rounding mode)
-  const double sr = sample_rate;
-  const double interval = sr * d.min_interval_ms / 1000.0;
-  const double hop = rint(sr * d.hop_size_ms / 1000.0);
-  SOME_REQUIRE(hop >= 1.0, "some_slicer_derive: hop_size of %g ms is less than one sample", d.hop_size_ms);
-  out->threshold = static_cast<float>(pow(10.0, d.threshold_db / 20.0));   // `rms < threshold` compares in float32
-  out->hop_size = static_cast<int>(hop);
-  out->win_size = static_cast<int>(std::min(rint(interval), 4.0 * hop));
-  out->min_length = static_cast<int>(rint(sr * d.min_length_ms / 1000.0 / hop));
-  out->min_interval = static_cast<int>(rint(interval / hop));
-  out->max_sil_kept = static_cast<int>(rint(sr * d.max_sil_kept_ms / 1000.0 / hop));
-  return 0;
-}
-
-extern "C" int some_slicer_ranges(const float* rms, int n_frames, long long n_samples, const some_slicer_frames* f,
-                                  int64_t* ranges, int capacity, int* count) {
-  SOME_REQUIRE((rms != nullptr || n_frames == 0) && f != nullptr && count != nullptr && n_frames >= 0 && n_samples >= 0,
-               "some_slicer_ranges: bad arguments");
-  SlicerCore core(*f);
-  std::vector<Tag> kept;
-  if (core.feed(rms, n_frames, kept) || core.finish(kept)) return -1;
-  *count = static_cast<int>(kept.size());
-  SOME_REQUIRE(ranges != nullptr && capacity >= *count, "some_slicer_ranges: %d ranges do not fit in a capacity of %d", *count,
-               capacity);
-  const int64_t hop = f->hop_size;
-  for (size_t k = 0; k < kept.size(); ++k) {
-    if (kept[k].second < 0) {                   // no tags: the whole recording
-      ranges[2 * k] = 0, ranges[2 * k + 1] = n_samples;
-      continue;
-    }
-    ranges[2 * k] = kept[k].first * hop;
-    ranges[2 * k + 1] = std::min<int64_t>(n_samples, kept[k].second * hop);
-  }
-  return 0;
-}
-
-// ---------------------------------------------------------------------------------------------------- streaming slicer
-// SlicerCore in samples, with the short-recording rule (slicer2.py:78-79): a recording of no more than min_length hops is one
-// chunk, so ranges are held back until more than min_length * hop_size samples are fixed.
-struct some_slicer_stream {
-  some_slicer_frames f;
-  SlicerCore core;
-  std::vector<Tag> queued;                // final ranges (frames) held back by the short-recording rule
-  std::vector<int64_t> out;               // the sample ranges the last call returned
-  int64_t fixed = 0;
-  bool finished = false;
-  explicit some_slicer_stream(const some_slicer_frames& fr) : f(fr), core(fr) {}
-  bool may_slice() const { return fixed > static_cast<int64_t>(f.min_length) * f.hop_size; }
-  // the first model-rate sample a range not yet returned may begin at
-  int64_t keep_from() const { return may_slice() ? core.open_begin() * f.hop_size : 0; }
-  // the samples [0, head()) a range may still need besides those from keep_from() on
-  int64_t head() const { return may_slice() && core.leading_tail() ? static_cast<int64_t>(f.max_sil_kept) * f.hop_size : 0; }
-  void release(int64_t n_samples) {
-    for (const Tag& t : queued) {
-      out.push_back(t.first * f.hop_size);
-      out.push_back(t.second < 0 ? n_samples : std::min(n_samples, t.second * f.hop_size));
-    }
-    queued.clear();
-  }
-};
-
-namespace {
-int slicer_feed(some_slicer_stream* st, const float* rms, int64_t n, int64_t fixed) {
-  SOME_REQUIRE(!st->finished, "some_slicer_stream_feed: the stream has finished");
-  SOME_REQUIRE(fixed >= st->fixed, "some_slicer_stream_feed: fixed went back from %lld to %lld", (long long)st->fixed,
-               (long long)fixed);
-  const int64_t known = frames_within(st->f, fixed);
-  SOME_REQUIRE(st->core.known() + n <= known, "some_slicer_stream_feed: frames up to %lld fed, %lld fixed samples complete %lld",
-               (long long)(st->core.known() + n), (long long)fixed, (long long)known);
-  st->out.clear();
-  if (st->core.feed(rms, n, st->queued)) return -1;
-  st->fixed = fixed;
-  if (st->may_slice()) st->release(fixed);              // ranges that end at a fixed frame: no clamp to the length
-  return 0;
-}
-
-// rms: the frames not fed yet, which need the recording's end (their windows reach into the zero padding)
-int slicer_finish(some_slicer_stream* st, const float* rms, int64_t n, int64_t n_samples) {
-  SOME_REQUIRE(!st->finished, "some_slicer_stream_finish: the stream has finished");
-  SOME_REQUIRE(n_samples >= st->fixed, "some_slicer_stream_finish: %lld samples, %lld were fixed already", (long long)n_samples,
-               (long long)st->fixed);
-  st->out.clear();
-  st->fixed = n_samples;
-  st->finished = true;
-  if (st->core.feed(rms, n, st->queued)) return -1;
-  const int64_t hop = st->f.hop_size;
-  if ((n_samples + hop - 1) / hop <= st->f.min_length) {   // one chunk (slicer2.py:79-80)
-    st->queued.clear();
-    st->out = {0, n_samples};
-    return 0;
-  }
-  const int64_t total = 1 + (n_samples + 2 * (st->f.win_size / 2) - st->f.win_size) / hop;
-  SOME_REQUIRE(st->core.known() == total, "some_slicer_stream_finish: %lld of the %lld frames of %lld samples were fed",
-               (long long)st->core.known(), (long long)total, (long long)n_samples);
-  if (st->core.finish(st->queued)) return -1;
-  st->release(n_samples);
-  return 0;
-}
-}  // namespace
-
-extern "C" int some_slicer_stream_create(const some_slicer_frames* frames, some_slicer_stream** out) {
-  SOME_REQUIRE(frames != nullptr && out != nullptr, "some_slicer_stream_create: null pointer");
-  SOME_REQUIRE(frames->hop_size >= 1 && frames->win_size >= 1 && frames->max_sil_kept >= 1 && frames->min_interval >= 0 &&
-                   frames->min_length >= 0,
-               "some_slicer_stream_create: bad frame counts");
-  *out = new some_slicer_stream(*frames);
-  return 0;
-}
-extern "C" int some_slicer_stream_destroy(some_slicer_stream* st) {
-  delete st;
-  return 0;
-}
-extern "C" int some_slicer_stream_feed(some_slicer_stream* st, const float* rms, int n_frames, long long fixed,
-                                       const int64_t** ranges, int* count) {
-  SOME_REQUIRE(st != nullptr && (rms != nullptr || n_frames == 0) && n_frames >= 0 && ranges != nullptr && count != nullptr,
-               "some_slicer_stream_feed: bad arguments");
-  if (slicer_feed(st, rms, n_frames, fixed)) return -1;
-  *ranges = st->out.data(), *count = static_cast<int>(st->out.size() / 2);
-  return 0;
-}
-extern "C" int some_slicer_stream_finish(some_slicer_stream* st, const float* rms, int n_frames, long long n_samples,
-                                         const int64_t** ranges, int* count) {
-  SOME_REQUIRE(st != nullptr && (rms != nullptr || n_frames == 0) && n_frames >= 0 && ranges != nullptr && count != nullptr,
-               "some_slicer_stream_finish: bad arguments");
-  if (slicer_finish(st, rms, n_frames, n_samples)) return -1;
-  *ranges = st->out.data(), *count = static_cast<int>(st->out.size() / 2);
-  return 0;
-}
-extern "C" int some_slicer_stream_keep_from(const some_slicer_stream* st, long long* sample, long long* head,
-                                            long long* rms_held) {
-  SOME_REQUIRE(st != nullptr && sample != nullptr, "some_slicer_stream_keep_from: bad arguments");
-  *sample = st->keep_from();
-  if (head) *head = st->head();
-  if (rms_held) *rms_held = static_cast<long long>(st->core.held());
-  return 0;
-}
 
 // ---------------------------------------------------------------------------------------------------- results
 extern "C" int some_notes_create(some_notes** out) {
@@ -1153,7 +835,8 @@ struct some_stream {
   some_session* s = nullptr;
   int rate = 0;                           // of the pushed samples
   bool resample = false;
-  some_slicer_stream slicer;
+  some_slicer_stream* slicer = nullptr;   // the slicer's decisions (some_slicer_stream_*)
+  some_slicer_frames f{};                 // its frame counts
   SampleWindow native, wave;              // the input at its own rate (when resampling) and at the model's rate
   PinBuf stage_h, rms_h;
   DevBuf rms_d;
@@ -1161,7 +844,6 @@ struct some_stream {
   int64_t head_len = 0;
   int64_t received = 0, fixed = 0, frames = 0;   // frames: RMS frames computed so far
   bool finished = false;
-  explicit some_stream(const some_slicer_frames& f) : slicer(f) {}
 };
 
 namespace {
@@ -1171,6 +853,7 @@ void destroy(some_stream* st) {
     for (DevBuf* b : {&st->native.buf, &st->wave.buf, &st->rms_d, &st->head_d}) b->release();
     for (PinBuf* b : {&st->stage_h, &st->rms_h}) b->release();
   }
+  some_slicer_stream_destroy(st->slicer);
   delete st;
 }
 
@@ -1179,13 +862,14 @@ void destroy(some_stream* st) {
 // `final`: the recording ends here.
 int stream_step(some_stream* st, int64_t n, bool final, some_notes* out) {
   some_session* s = st->s;
-  const some_slicer_frames& f = st->slicer.f;
+  const some_slicer_frames& f = st->f;
   const int sr = s->info.sample_rate;
+  long long keep_from, head;
+  if (some_slicer_stream_keep_from(st->slicer, &keep_from, &head, nullptr)) return -1;
   // the model-rate samples a later chunk or RMS frame can still read
-  const int64_t keep = std::max<int64_t>(0, std::min(st->slicer.keep_from(), st->frames * f.hop_size - f.win_size / 2));
-  // during a long leading silence, the first max_sil_kept frames go apart before the window drops them (SlicerCore::
-  // leading_tail: the all-silent recording's one range lies there); until then the window holds everything from sample 0
-  const int64_t head = st->slicer.head();
+  const int64_t keep = std::max<int64_t>(0, std::min<int64_t>(keep_from, st->frames * f.hop_size - f.win_size / 2));
+  // during a long leading silence (head > 0), the first max_sil_kept frames go apart before the window drops them (the
+  // all-silent recording's one range lies there); until then the window holds everything from sample 0
   if (head == 0) {
     st->head_len = 0;
   } else if (st->head_len == 0 && keep > st->wave.first) {
@@ -1230,9 +914,11 @@ int stream_step(some_stream* st, int64_t n, bool final, some_notes* out) {
   SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");   // also frees the staging buffer for the next push
   st->frames += nf;
   const float* rms = static_cast<const float*>(st->rms_h.p);
-  if (final ? slicer_finish(&st->slicer, rms, nf, st->fixed) : slicer_feed(&st->slicer, rms, nf, st->fixed)) return -1;
-  const std::vector<int64_t>& ranges = st->slicer.out;
-  const int B = static_cast<int>(ranges.size() / 2);
+  const int64_t* ranges = nullptr;
+  int B = 0;
+  if (final ? some_slicer_stream_finish(st->slicer, rms, static_cast<int>(nf), st->fixed, &ranges, &B)
+            : some_slicer_stream_feed(st->slicer, rms, static_cast<int>(nf), st->fixed, &ranges, &B))
+    return -1;
   if (B == 0) {
     out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
     return 0;
@@ -1278,8 +964,11 @@ extern "C" int some_stream_open(some_session* s, int sample_rate, const some_sli
     long long t_end, x_first;
     if (some_resample_window_plan(0, 0, 0, sample_rate, s->info.sample_rate, kKaiserTaps, &t_end, &x_first)) return -1;
   }
-  some_stream* st = new some_stream(sl);
+  some_slicer_stream* slicer;
+  if (some_slicer_stream_create(&sl, &slicer)) return -1;
+  some_stream* st = new some_stream();
   st->s = s, st->rate = sample_rate, st->resample = sample_rate != s->info.sample_rate;
+  st->slicer = slicer, st->f = sl;
   *out = st;
   return 0;
 }

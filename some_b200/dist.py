@@ -216,7 +216,7 @@ def infer_sliced_sharded(plugin, waveform: np.ndarray, slicer, group=None):
     """C5 across GPUs (SURVEY.md §8d): ONE long recording -> slicer -> the chunks sharded over the ranks -> all ranks return
     (chunk offsets in seconds, notes of every chunk in order).
 
-    Every rank holds the recording and cuts it itself (the device RMS + host run walk cost well under a millisecond of GPU
+    Every rank holds the recording and cuts it itself (the device RMS + host slicer cost well under a millisecond of GPU
     time and are deterministic, so no broadcast of the cut list is needed); the chunks are zero-copy views, each rank stages
     and uploads only its own shard, and the exchange is the same single all-gather of packed notes as ``infer_sharded``."""
     ranges = slicer.ranges(waveform)

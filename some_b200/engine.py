@@ -23,6 +23,7 @@ import torch
 
 from . import _lib
 from .config import DIM, FFN_DIM, check_supported
+from .slicer import cut_ranges
 from .weights import ModelWeights, build_c_model, mel_tables
 
 HOP = 512
@@ -553,20 +554,10 @@ class Engine:
         self._h2d_done = ev if layout else None
         return out_d[:nbytes_total], cu, layout, extra
 
-    def rms_frames(self, wave_d: torch.Tensor, frame_length: int, hop: int) -> np.ndarray:
-        """Short-time RMS of a device-resident f32 waveform (some_slicer_rms), bit-identical to the reference's get_rms
-        (utils/slicer2.py:5-38).  Returns the host copy (one small D2H + sync): the slicer's state machine runs on the host."""
-        n = int(wave_d.numel())
-        n_frames = 1 + (n + 2 * (frame_length // 2) - frame_length) // hop
-        rms_d = torch.empty(n_frames, dtype=torch.float32, device=self.device)
-        _lib.check(self.lib.some_slicer_rms(wave_d.data_ptr(), n, frame_length, hop, rms_d.data_ptr(), n_frames, self._stream),
-                   'some_slicer_rms')
-        self.launches += 1
-        return rms_d.cpu().numpy()
-
     def rms_frames_many(self, waves_d: Sequence[torch.Tensor], frame_length: int, hop: int) -> List[np.ndarray]:
-        """RMS lists of several device-resident recordings: one launch each into ONE buffer, one D2H copy and sync for all
-        (the dataset driver, some_b200/batch.py)."""
+        """Short-time RMS lists of device-resident f32 recordings (some_slicer_rms), bit-identical to the reference's get_rms
+        (utils/slicer2.py:5-38): one launch each into ONE buffer, one D2H copy and sync for all.  The slicer's decisions are
+        taken on the host from these copies."""
         counts = [1 + (int(w.numel()) + 2 * (frame_length // 2) - frame_length) // hop for w in waves_d]
         if not counts:
             return []
@@ -585,26 +576,30 @@ class Engine:
         batch_infer.py:50-54 (Slicer.slice, then infer on the chunks) with the recording uploaded ONCE.  The RMS frames are
         computed on the device, the slicer's decisions are taken on the host from the copied RMS list (15 k floats for 5 min),
         and the chunks are then processed where they lie in device memory as one var-len batch."""
-        from .slicer import chunk_ranges, silence_tags
         samples = np.ascontiguousarray(waveform, dtype=np.float32)
         assert samples.ndim == 1, 'infer_sliced expects a mono waveform (infer.py loads with mono=True)'
         n = int(samples.shape[0])
         dev = self.device
         with torch.cuda.device(dev):
-            if (n + slicer.hop_size - 1) // slicer.hop_size <= slicer.min_length:   # slicer2.py:79-80
+            uploaded = []
+
+            def rms_of(_):                      # only for a recording long enough to be cut
+                src = torch.from_numpy(samples)
+                if not src.is_pinned():
+                    st = self._staging(n, 1, 1 + n // HOP)
+                    st['wave_h'][:n].copy_(src)
+                    src = st['wave_h'][:n]
+                wave_d = torch.empty(n, dtype=torch.float32, device=dev)
+                wave_d.copy_(src, non_blocking=True)
+                uploaded.append(wave_d)
+                return self.rms_frames_many(uploaded, slicer.win_size, slicer.hop_size)
+
+            [ranges] = cut_ranges(slicer, [n], rms_of)
+            if not uploaded:                    # one chunk, the whole recording
                 return [0], self.infer([samples], quantized)
-            src = torch.from_numpy(samples)
-            if not src.is_pinned():
-                st = self._staging(n, 1, 1 + n // HOP)
-                st['wave_h'][:n].copy_(src)
-                src = st['wave_h'][:n]
-            wave_d = torch.empty(n, dtype=torch.float32, device=dev)
-            wave_d.copy_(src, non_blocking=True)
-            rms = self.rms_frames(wave_d, slicer.win_size, slicer.hop_size)
-            ranges = chunk_ranges(silence_tags(rms, slicer), rms.shape[0], slicer.hop_size, n)
             if not ranges:
                 return [], []
-            slab, cu, layout, _ = self.enqueue(None, quantized, resident=(wave_d, ranges))
+            slab, cu, layout, _ = self.enqueue(None, quantized, resident=(uploaded[0], ranges))
             self._staging(0, len(ranges), int(cu[-1]))
             out_h = self._stage['out_h']
             out_h[:slab.numel()].copy_(slab, non_blocking=True)

@@ -1,6 +1,7 @@
 """ctypes wrapper of the native session (csrc/session.cu, include/some_b200.h): opens a model file written by
 ``python -m some_b200.export`` and transcribes with no torch on the path.  C / C++ hosts call the same functions directly
 (examples/some_transcribe.c); this wrapper serves Python callers that want the same results, the tests and bench_session.py.
+The slicer parameters of transcribe_sliced and stream are ``slicer_params(...)`` (defined in some_b200.slicer).
 
 Results have the plugin's shape: one dict per clip / chunk with ``note_midi`` f32, ``note_dur`` in seconds
 (``dur * timestep``, float64 as me_infer.py:95) and ``note_rest`` bool, plus ``note_frames`` (the durations in frames)."""
@@ -14,83 +15,9 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _lib
-
-
-def slicer_params(threshold: float = -40., min_length: float = 5000, min_interval: float = 300, hop_size: float = 20,
-                  max_sil_kept: float = 1000) -> _lib.SlicerParams:
-    """Slicer constructor arguments (ms / dB) for the session; the defaults are infer.py's Slicer(sr, max_sil_kept=1000)."""
-    return _lib.SlicerParams(threshold, min_length, min_interval, hop_size, max_sil_kept)
-
-
-def slicer_frames(sample_rate: int, params: Optional[_lib.SlicerParams] = None) -> _lib.SlicerFrames:
-    """some_slicer_derive: the frame counts the native slicer uses (host only)."""
-    lib = _lib.load()
-    out = _lib.SlicerFrames()
-    _lib.check(lib.some_slicer_derive(int(sample_rate), C.byref(params) if params is not None else None, C.byref(out)),
-               'some_slicer_derive')
-    return out
-
-
-def slicer_ranges(rms: np.ndarray, num_samples: int, frames: _lib.SlicerFrames) -> List[Tuple[int, int]]:
-    """some_slicer_ranges: the native slicer's chunk ranges for an RMS list (host only, no CUDA call)."""
-    lib = _lib.load()
-    rms = np.ascontiguousarray(rms, dtype=np.float32)
-    cap = rms.shape[0] // 2 + 2
-    out = np.zeros(2 * cap, dtype=np.int64)
-    count = C.c_int()
-    _lib.check(lib.some_slicer_ranges(rms.ctypes.data, int(rms.shape[0]), int(num_samples), C.byref(frames), out.ctypes.data,
-                                      cap, C.byref(count)), 'some_slicer_ranges')
-    return [(int(out[2 * k]), int(out[2 * k + 1])) for k in range(count.value)]
-
-
-class SlicerStream:
-    """some_slicer_stream_*: the slicer's decisions on an RMS list that arrives in pieces (host only, no CUDA call)."""
-
-    handle = None
-
-    def __init__(self, frames: _lib.SlicerFrames):
-        self.lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(self.lib.some_slicer_stream_create(C.byref(frames), C.byref(h)), 'some_slicer_stream_create')
-        self.handle = h
-
-    @staticmethod
-    def _ranges(ptr, count) -> List[Tuple[int, int]]:
-        if count.value == 0:
-            return []
-        a = np.ctypeslib.as_array(C.cast(ptr, C.POINTER(C.c_int64)), (2 * count.value,))
-        return [(int(a[2 * k]), int(a[2 * k + 1])) for k in range(count.value)]
-
-    def feed(self, rms: np.ndarray, fixed: int) -> List[Tuple[int, int]]:
-        """The next RMS frames and the samples fixed so far -> the [begin, end) sample ranges that became final."""
-        rms = np.ascontiguousarray(rms, dtype=np.float32)
-        ptr, count = C.c_void_p(), C.c_int()
-        _lib.check(self.lib.some_slicer_stream_feed(self.handle, rms.ctypes.data, int(rms.shape[0]), int(fixed), C.byref(ptr),
-                                                    C.byref(count)), 'some_slicer_stream_feed')
-        return self._ranges(ptr, count)
-
-    def finish(self, rms: np.ndarray, num_samples: int) -> List[Tuple[int, int]]:
-        """The frames not fed yet and the final length -> the remaining ranges."""
-        rms = np.ascontiguousarray(rms, dtype=np.float32)
-        ptr, count = C.c_void_p(), C.c_int()
-        _lib.check(self.lib.some_slicer_stream_finish(self.handle, rms.ctypes.data, int(rms.shape[0]), int(num_samples),
-                                                      C.byref(ptr), C.byref(count)), 'some_slicer_stream_finish')
-        return self._ranges(ptr, count)
-
-    def keep_from(self) -> Tuple[int, int, int]:
-        """(sample a range not returned yet begins at or after, unless it lies within [0, head); head; RMS values held)."""
-        a, h, b = C.c_longlong(), C.c_longlong(), C.c_longlong()
-        _lib.check(self.lib.some_slicer_stream_keep_from(self.handle, C.byref(a), C.byref(h), C.byref(b)),
-                   'some_slicer_stream_keep_from')
-        return a.value, h.value, b.value
-
-    def close(self):
-        if self.handle is not None:
-            self.lib.some_slicer_stream_destroy(self.handle)
-            self.handle = None
-
-    def __del__(self):
-        self.close()
+# The slicer's parameters and host decisions are defined in some_b200.slicer; they stay importable from here because
+# transcribe_sliced and stream take slicer_params(...), and existing callers import them with the session.
+from .slicer import SlicerStream, slicer_frames, slicer_params, slicer_ranges  # noqa: F401
 
 
 class Notes:

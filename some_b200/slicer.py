@@ -5,80 +5,119 @@ The reference computes the short-time RMS with numpy (slicer2.py:5-38: ~53 M mul
 
 * the RMS frames come from ``some_slicer_rms`` (csrc/slicer.cu): the recording is uploaded once — it has to go to the GPU
   for the mel front end anyway — and the kernel reproduces numpy's float32 pairwise summation bit for bit, so every
-  threshold comparison and argmin below sees the reference's numbers;
-* the decisions are taken per SILENT RUN instead of per frame: the reference's loop only acts on the first voiced frame
-  after a run of frames with ``rms < threshold``, so the runs are extracted with vectorised numpy and the (sequential, because
-  of ``clip_start``) rules are applied to a few dozen runs;
+  threshold comparison and argmin sees the reference's numbers;
+* the cuts are decided by the native slicer next to that kernel (``some_slicer_ranges``, csrc/slicer.cu), on the host with no
+  CUDA call: per SILENT RUN instead of per frame, since the reference's loop only acts on the first voiced frame after a run
+  of frames with ``rms < threshold``.  The native session, streaming and the C ABI use the same code, so the cut rules exist
+  once;
 * ``Engine.infer_sliced`` then processes the chunks where they lie in device memory (no second upload).
 
 ``Slicer`` keeps the reference's constructor, derived attributes and ``slice()`` return value (list of
 ``{'offset': seconds, 'waveform': view}``), so ``infer.py``-style callers can use it unchanged.  There is no CPU path:
-the RMS needs the CUDA library.
+the RMS needs the CUDA library.  ``cut_ranges`` applies the cuts of any object with those attributes; ``slicer_params``,
+``slicer_frames``, ``slicer_ranges`` and ``SlicerStream`` wrap the native slicer's C functions (ctypes).
 """
 from __future__ import annotations
 
-from typing import List, Tuple
+import ctypes as C
+from typing import Callable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-
-def silence_tags(rms: np.ndarray, p) -> List[Tuple[int, int]]:
-    """Frame ranges to remove (slicer2.py:82-133).  ``p`` carries threshold, min_length, min_interval, max_sil_kept (frames)."""
-    total = int(rms.shape[0])
-    silent = rms < p.threshold                       # float32 comparison, as the reference's scalar `rms < self.threshold`
-    edges = np.diff(silent.astype(np.int8), prepend=np.int8(0), append=np.int8(0))
-    run_from = np.flatnonzero(edges == 1)
-    run_to = np.flatnonzero(edges == -1)             # first voiced frame after the run (== total for a trailing run)
-    keep = p.max_sil_kept
-    tags: List[Tuple[int, int]] = []
-    clip_from = 0
-
-    def first_min(a: int, b: int) -> int:            # first-index argmin over frames [a, b)
-        return int(rms[a:b].argmin()) + a
-
-    for s, i in zip(run_from.tolist(), run_to.tolist()):
-        if i == total:                               # trailing silence (slicer2.py:129-133)
-            if total - s >= p.min_interval:
-                tags.append((first_min(s, min(total, s + keep) + 1), total + 1))
-            break
-        leading = s == 0 and i > keep
-        middle = i - s >= p.min_interval and i - clip_from >= p.min_length
-        if not (leading or middle):
-            continue
-        span = i - s
-        if span <= keep:
-            cut = first_min(s, i + 1)
-            tags.append((0, cut) if s == 0 else (cut, cut))
-            clip_from = cut
-        elif span <= 2 * keep:
-            mid = first_min(i - keep, s + keep + 1)
-            left = first_min(s, s + keep + 1)
-            right = first_min(i - keep, i + 1)
-            if s == 0:
-                tags.append((0, right))
-                clip_from = right
-            else:
-                tags.append((min(left, mid), max(right, mid)))
-                clip_from = max(right, mid)
-        else:
-            left = first_min(s, s + keep + 1)
-            right = first_min(i - keep, i + 1)
-            tags.append((0, right) if s == 0 else (left, right))
-            clip_from = right
-    return tags
+from . import _lib
 
 
-def chunk_ranges(tags: List[Tuple[int, int]], total_frames: int, hop_size: int, num_samples: int) -> List[Tuple[int, int]]:
-    """[begin, end) SAMPLE ranges that remain after removing the tagged frames (slicer2.py:62-71,135-145)."""
-    if not tags:
-        return [(0, num_samples)]
-    kept = []
-    if tags[0][0] > 0:
-        kept.append((0, tags[0][0]))
-    kept.extend((a[1], b[0]) for a, b in zip(tags[:-1], tags[1:]))
-    if tags[-1][1] < total_frames:
-        kept.append((tags[-1][1], total_frames))
-    return [(f0 * hop_size, min(num_samples, f1 * hop_size)) for f0, f1 in kept]
+def slicer_params(threshold: float = -40., min_length: float = 5000, min_interval: float = 300, hop_size: float = 20,
+                  max_sil_kept: float = 1000) -> _lib.SlicerParams:
+    """Slicer constructor arguments (ms / dB) for the session; the defaults are infer.py's Slicer(sr, max_sil_kept=1000)."""
+    return _lib.SlicerParams(threshold, min_length, min_interval, hop_size, max_sil_kept)
+
+
+def slicer_frames(sample_rate: int, params: Optional[_lib.SlicerParams] = None) -> _lib.SlicerFrames:
+    """some_slicer_derive: the frame counts the native slicer uses (host only)."""
+    lib = _lib.load()
+    out = _lib.SlicerFrames()
+    _lib.check(lib.some_slicer_derive(int(sample_rate), C.byref(params) if params is not None else None, C.byref(out)),
+               'some_slicer_derive')
+    return out
+
+
+def slicer_ranges(rms: np.ndarray, num_samples: int, frames: _lib.SlicerFrames) -> List[Tuple[int, int]]:
+    """some_slicer_ranges: the native slicer's chunk ranges for an RMS list (host only, no CUDA call)."""
+    lib = _lib.load()
+    rms = np.ascontiguousarray(rms, dtype=np.float32)
+    cap = rms.shape[0] // 2 + 2
+    out = np.zeros(2 * cap, dtype=np.int64)
+    count = C.c_int()
+    _lib.check(lib.some_slicer_ranges(rms.ctypes.data, int(rms.shape[0]), int(num_samples), C.byref(frames), out.ctypes.data,
+                                      cap, C.byref(count)), 'some_slicer_ranges')
+    return [(int(out[2 * k]), int(out[2 * k + 1])) for k in range(count.value)]
+
+
+def cut_ranges(slicer, lengths: Sequence[int],
+               rms_of: Callable[[List[int]], Sequence[np.ndarray]]) -> List[List[Tuple[int, int]]]:
+    """[begin, end) sample ranges of the chunks of recordings of the given lengths, cut by ``slicer``: any object with the
+    reference Slicer's attributes (threshold, hop_size, win_size, min_length, min_interval, max_sil_kept).  A recording of no
+    more than min_length hops is one chunk (slicer2.py:79-80); ``rms_of(indices)`` returns the RMS lists of the others, in
+    that order, and is called once, only if there is one, so that short recordings make no device call."""
+    out = [[(0, int(n))] for n in lengths]
+    need = [i for i, n in enumerate(lengths) if (n + slicer.hop_size - 1) // slicer.hop_size > slicer.min_length]
+    if need:
+        frames = _lib.SlicerFrames(np.float32(slicer.threshold), slicer.hop_size, slicer.win_size, slicer.min_length,
+                                   slicer.min_interval, slicer.max_sil_kept)
+        for i, rms in zip(need, rms_of(need)):
+            out[i] = slicer_ranges(rms, lengths[i], frames)
+    return out
+
+
+class SlicerStream:
+    """some_slicer_stream_*: the slicer's decisions on an RMS list that arrives in pieces (host only, no CUDA call)."""
+
+    handle = None
+
+    def __init__(self, frames: _lib.SlicerFrames):
+        self.lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(self.lib.some_slicer_stream_create(C.byref(frames), C.byref(h)), 'some_slicer_stream_create')
+        self.handle = h
+
+    @staticmethod
+    def _ranges(ptr, count) -> List[Tuple[int, int]]:
+        if count.value == 0:
+            return []
+        a = np.ctypeslib.as_array(C.cast(ptr, C.POINTER(C.c_int64)), (2 * count.value,))
+        return [(int(a[2 * k]), int(a[2 * k + 1])) for k in range(count.value)]
+
+    def feed(self, rms: np.ndarray, fixed: int) -> List[Tuple[int, int]]:
+        """The next RMS frames and the samples fixed so far -> the [begin, end) sample ranges that became final."""
+        rms = np.ascontiguousarray(rms, dtype=np.float32)
+        ptr, count = C.c_void_p(), C.c_int()
+        _lib.check(self.lib.some_slicer_stream_feed(self.handle, rms.ctypes.data, int(rms.shape[0]), int(fixed), C.byref(ptr),
+                                                    C.byref(count)), 'some_slicer_stream_feed')
+        return self._ranges(ptr, count)
+
+    def finish(self, rms: np.ndarray, num_samples: int) -> List[Tuple[int, int]]:
+        """The frames not fed yet and the final length -> the remaining ranges."""
+        rms = np.ascontiguousarray(rms, dtype=np.float32)
+        ptr, count = C.c_void_p(), C.c_int()
+        _lib.check(self.lib.some_slicer_stream_finish(self.handle, rms.ctypes.data, int(rms.shape[0]), int(num_samples),
+                                                      C.byref(ptr), C.byref(count)), 'some_slicer_stream_finish')
+        return self._ranges(ptr, count)
+
+    def keep_from(self) -> Tuple[int, int, int]:
+        """(sample a range not returned yet begins at or after, unless it lies within [0, head); head; RMS values held)."""
+        a, h, b = C.c_longlong(), C.c_longlong(), C.c_longlong()
+        _lib.check(self.lib.some_slicer_stream_keep_from(self.handle, C.byref(a), C.byref(h), C.byref(b)),
+                   'some_slicer_stream_keep_from')
+        return a.value, h.value, b.value
+
+    def close(self):
+        if self.handle is not None:
+            self.lib.some_slicer_stream_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        self.close()
 
 
 class Slicer:
@@ -104,7 +143,6 @@ class Slicer:
     def rms(self, samples: np.ndarray) -> np.ndarray:
         """RMS list of a mono float32 waveform, computed on the GPU (bit-identical to get_rms, slicer2.py:5-38)."""
         import torch
-        from . import _lib
         lib = _lib.load()
         if not torch.cuda.is_available():
             raise _lib.SomeB200Error('some_b200.slicer needs a CUDA device (no CPU path)')
@@ -114,7 +152,6 @@ class Slicer:
             n = int(x.numel())
             n_frames = 1 + (n + 2 * (self.win_size // 2) - self.win_size) // self.hop_size
             out = torch.empty(n_frames, dtype=torch.float32, device=dev)
-            import ctypes as C
             stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             _lib.check(lib.some_slicer_rms(x.data_ptr(), n, self.win_size, self.hop_size, out.data_ptr(), n_frames, stream),
                        'some_slicer_rms')
@@ -123,18 +160,11 @@ class Slicer:
     # ------------------------------------------------------------------ reference API
     def ranges(self, waveform: np.ndarray) -> List[Tuple[int, int]]:
         samples = waveform.mean(axis=0) if waveform.ndim > 1 else waveform          # slicer2.py:75-78
-        n = int(samples.shape[0])
-        if (n + self.hop_size - 1) // self.hop_size <= self.min_length:            # slicer2.py:79-80
-            return [(0, n)]
-        rms = self.rms(samples)
-        return chunk_ranges(silence_tags(rms, self), rms.shape[0], self.hop_size, n)
+        return cut_ranges(self, [int(samples.shape[0])], lambda _: [self.rms(samples)])[0]
 
     def slice(self, waveform: np.ndarray):
-        n = waveform.shape[-1]
-        if (n + self.hop_size - 1) // self.hop_size <= self.min_length:
+        ranges = self.ranges(waveform)
+        if ranges == [(0, waveform.shape[-1])]:                     # one chunk: the input itself (slicer2.py:80, :135-136)
             return [{'offset': 0, 'waveform': waveform}]
-        chunks = []
-        for begin, end in self.ranges(waveform):
-            chunks.append({'offset': begin / self.sr,                               # == begin_frame * hop_size / sr
-                           'waveform': waveform[..., begin:end]})
-        return chunks
+        return [{'offset': begin / self.sr,                         # == begin_frame * hop_size / sr
+                 'waveform': waveform[..., begin:end]} for begin, end in ranges]

@@ -1,5 +1,5 @@
-"""CPU tests of the streaming slicer (some_slicer_stream_*, csrc/session.cu): fed the RMS list in any pieces, its ranges,
-concatenated, equal some_slicer_ranges on the whole list (itself checked against some_b200.slicer in test_session_cpu.py),
+"""CPU tests of the streaming slicer (some_slicer_stream_*, csrc/slicer.cu): fed the RMS list in any pieces, its ranges,
+concatenated, equal some_slicer_ranges on the whole list (itself checked against the oracle in test_slicer_cpu.py),
 each range comes back no later than the delivery bound, and the state it keeps stays O(max_sil_kept).  The device half of
 streaming is tested in tests/test_gpu_stream.py."""
 import ctypes as C
@@ -15,13 +15,13 @@ sys.path.insert(0, str(HERE / 'golden'))
 from oracle import slicer as osl  # noqa: E402
 from slicer_cases import CASES, make_case  # noqa: E402
 from some_b200 import _lib  # noqa: E402
-from some_b200 import session as nsess  # noqa: E402
+from some_b200 import slicer as psl  # noqa: E402
 
 DEFAULTS = dict(threshold=-40., min_length=5000, min_interval=300, hop_size=20, max_sil_kept=1000)
 
 
 def frames_for(sr, **kw):
-    return nsess.slicer_frames(sr, nsess.slicer_params(**dict(DEFAULTS, **kw)))
+    return psl.slicer_frames(sr, psl.slicer_params(**dict(DEFAULTS, **kw)))
 
 
 def reach(f):
@@ -33,13 +33,13 @@ def offline(rms, n, f):
     """transcribe_sliced's ranges: the short-recording rule, then some_slicer_ranges."""
     if (n + f.hop_size - 1) // f.hop_size <= f.min_length:
         return [(0, n)]
-    return nsess.slicer_ranges(rms, n, f)
+    return psl.slicer_ranges(rms, n, f)
 
 
 def streamed(rms, n, f, blocks, log=None):
     """Feeds rms in blocks of the given sizes (the frames the n samples complete; the rest at finish).  log collects
     (frames fed, ranges returned, keep_from()) per call.  Every range a call returns lies where keep_from() said before it."""
-    st = nsess.SlicerStream(f)
+    st = psl.SlicerStream(f)
 
     def kept(out, before):
         keep, head, _ = before
@@ -224,7 +224,7 @@ def test_refusals():
     h = C.c_void_p()
     with pytest.raises(_lib.SomeB200Error, match='null pointer'):
         _lib.check(lib.some_slicer_stream_create(None, C.byref(h)), 'some_slicer_stream_create')
-    st = nsess.SlicerStream(f)
+    st = psl.SlicerStream(f)
     ptr, cnt = C.c_void_p(), C.c_int()
     with pytest.raises(_lib.SomeB200Error, match='bad arguments'):
         _lib.check(lib.some_slicer_stream_feed(st.handle, None, 5, 10 ** 6, C.byref(ptr), C.byref(cnt)))
@@ -236,7 +236,7 @@ def test_refusals():
     with pytest.raises(_lib.SomeB200Error, match='frames of'):
         st.finish(np.zeros(0, np.float32), 10 ** 6)                    # not long enough for the short rule, frames missing
     st.close()
-    st = nsess.SlicerStream(f)
+    st = psl.SlicerStream(f)
     assert st.finish(np.zeros(0, np.float32), 100) == [(0, 100)]
     with pytest.raises(_lib.SomeB200Error, match='has finished'):
         st.feed(np.zeros(0, np.float32), 100)
@@ -244,6 +244,6 @@ def test_refusals():
         st.finish(np.zeros(0, np.float32), 100)
     st.close()
     with pytest.raises(_lib.SomeB200Error, match='min_length >= min_interval'):
-        nsess.slicer_frames(44100, nsess.slicer_params(min_length=100, min_interval=300))
+        psl.slicer_frames(44100, psl.slicer_params(min_length=100, min_interval=300))
     with pytest.raises(_lib.SomeB200Error, match='max_sil_kept >= hop_size'):
-        nsess.slicer_frames(44100, nsess.slicer_params(max_sil_kept=10))
+        psl.slicer_frames(44100, psl.slicer_params(max_sil_kept=10))
