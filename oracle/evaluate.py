@@ -54,19 +54,23 @@ def losses(logits, bounds, labels: dict, config: dict, quantized: bool) -> dict:
     return {'midi_loss': float(midi), 'bound_loss': float(bound)}
 
 
-def accuracy_counts(logits, labels: dict, config: dict, quantized: bool):
-    """(correct, total) that MIDIAccuracy(tolerance=0.5).update adds for one item."""
+def accuracy_counts(logits, labels: dict, config: dict, quantized: bool, probs=None):
+    """(correct, total) that MIDIAccuracy(tolerance=0.5).update adds for one item.  ``probs``: the activated head to
+    decode instead of the sigmoid / softmax of ``logits`` (a kernel's own activations, which may differ from torch's in
+    the last ulp)."""
     logits = torch.as_tensor(logits).float()
     u = torch.as_tensor(labels['unit2note']).long()
+    if probs is not None:
+        probs = torch.as_tensor(probs).float()
     if quantized:
-        probs = torch.softmax(logits, dim=-1)
+        probs = torch.softmax(logits, dim=-1) if probs is None else probs
         midi_pred = probs.argmax(dim=-1)
         rest_pred = midi_pred == 128
         midi_pred = midi_pred.float()
         note_midi_gt = torch.as_tensor(labels['note_midi']).float()
         note_midi_gt[torch.as_tensor(labels['note_midi']) == 128] = -torch.inf
     else:
-        probs = torch.sigmoid(logits)
+        probs = torch.sigmoid(logits) if probs is None else probs
         values, rest = odecode.decode_gaussian_blurred_probs_vec(
             probs.numpy(), config['midi_min'], config['midi_max'], config['midi_prob_deviation'], config['rest_threshold'])
         midi_pred, rest_pred = torch.from_numpy(values), torch.from_numpy(rest)

@@ -26,6 +26,9 @@ KERNEL_SIZE = 31
 UNITS_DIM = 80
 FFN_DIM = 4 * DIM
 MAX_OUTDIM = 256
+# the quantized task's classes: MIDI 0..127 and rest (me_quant_infer.py:28-31)
+QUANTIZED_TASK = 'training.QuantizedMIDIExtractionTask'
+QUANTIZED_BINS = 129
 
 
 def override_dict(old: dict, new: dict) -> None:
@@ -73,8 +76,13 @@ def check_supported(config: dict) -> dict:
         problems.append(f"kernel_size={args.get('kernel_size')} (kernels are built for {KERNEL_SIZE})")
     if config['units_dim'] != UNITS_DIM:
         problems.append(f"units_dim={config['units_dim']} (mel front end emits {UNITS_DIM})")
-    if not (1 <= config['midi_num_bins'] <= MAX_OUTDIM):
-        problems.append(f"midi_num_bins={config['midi_num_bins']} (max {MAX_OUTDIM})")
+    bins = config['midi_num_bins']
+    if not (2 <= bins <= MAX_OUTDIM):
+        # interval = (midi_max - midi_min) / (bins - 1) (infer_utils.py:11): one bin has no interval
+        problems.append(f"midi_num_bins={bins} (the decode takes 2 to {MAX_OUTDIM} bins)")
+    elif config.get('task_cls') == QUANTIZED_TASK and bins != QUANTIZED_BINS:
+        problems.append(f"midi_num_bins={bins} for {QUANTIZED_TASK} (its decode takes {QUANTIZED_BINS} classes, "
+                        f"rest = {QUANTIZED_BINS - 1})")
     if config.get('win_size', 2048) != 2048 or config.get('hop_size', 512) != 512:
         problems.append('win_size/hop_size must be 2048/512 (fused STFT kernel)')
     if problems:

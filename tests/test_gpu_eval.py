@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import evaluate as oeval
 from oracle import flac as of
 from some_b200 import _lib, audio, evaluate, plugin, synth
 
@@ -90,6 +91,70 @@ def test_kernel_on_golden_logits(cfg, golden_dir, tmp_path):
             ref = torch.softmax(torch.from_numpy(logits[i]), -1) if quantized else torch.sigmoid(torch.from_numpy(logits[i]))
             np.testing.assert_allclose(probs[cu[i]:cu[i + 1]], ref.numpy(), rtol=1e-5, atol=1e-7)
     assert g['item0_lean_correct'] > 0
+
+
+def _spanning_clip(rng, t, config, quantized):
+    """(logits [t, N], bounds [t], label arrays) of a clip whose notes (20-400 frames, some rests) span every multiple of
+    2048, the chunk of the kernel's bound-loss scan.  Most frames of a pitched note lean towards its pitch, so the
+    accuracy counts are far from 0."""
+    n = config['midi_num_bins']
+    starts = [0]
+    while starts[-1] < t:
+        s = starts[-1] + int(rng.integers(20, 400))
+        if any(s - 60 <= c <= s + 60 for c in range(2048, t, 2048)):
+            s += 150                                                     # no note starts right at a chunk boundary
+        starts.append(s)
+    durs = np.diff(np.minimum(starts, t))
+    durs = durs[durs > 0]
+    k = len(durs)
+    unit2note = np.repeat(np.arange(1, k + 1, dtype=np.int64), durs)
+    rest = rng.random(k) < 0.15
+    if quantized:
+        note_midi = np.where(rest, 128, rng.integers(0, 128, k)).astype(np.int64)
+        target = note_midi[unit2note - 1]
+        logits = rng.standard_normal((t, n)).astype(np.float32) * 2.0
+        lean = rng.random(t) < 0.7
+        logits[np.nonzero(lean)[0], target[lean]] += 6.0
+    else:
+        vmin, vmax = config['midi_min'], config['midi_max']
+        note_midi = rng.uniform(vmin + 1, vmax - 1, k).astype(np.float32)
+        interval = (vmax - vmin) / (n - 1)
+        miu = (note_midi[unit2note - 1] - vmin) / interval
+        bump = np.exp(-((np.arange(n)[None, :] - miu[:, None]) * interval / config['midi_prob_deviation']) ** 2 / 2)
+        lean = (rng.random(t) < 0.7) & ~rest[unit2note - 1]
+        logits = (rng.standard_normal((t, n)) * 1.5 - 3.0 + 9.0 * bump * lean[:, None]).astype(np.float32)
+    bounds = rng.random(t) ** 8 * 0.1                                    # a bound head: high where a note starts
+    bounds[np.cumsum(durs)[:-1]] = rng.uniform(0.6, 1.0, k - 1)
+    bounds = bounds.astype(np.float32)
+    labels = {'unit2note': unit2note, 'note_midi': note_midi, 'note_rest': rest if not quantized else note_midi == 128}
+    for c in range(2048, t, 2048):
+        assert unit2note[c - 1] == unit2note[c]
+    return logits, bounds, labels
+
+
+@pytest.mark.parametrize('head', [_lib.EVAL_HEAD_TC, _lib.EVAL_HEAD_F32])
+@pytest.mark.parametrize('cfg,bins,vmin,vmax', [('two_head', 128, 0, 127), ('two_head', 200, 21, 108),
+                                                ('quant_two_head', 129, 0, 127)])
+def test_kernel_past_one_chunk(cfg, bins, vmin, vmax, head):
+    """Clips of 2047 to 9000 frames, so the bound-loss scan carries its double prefix, note count and previous note across
+    2048-frame chunks: losses against the oracle on the logits, and the accuracy counts exactly against the oracle's on the
+    kernel's own activations (CUDA's exp and torch's can differ by an ulp, which may move a value across +- 0.5)."""
+    config = dict(synth.named_config(cfg), midi_num_bins=bins, midi_min=vmin, midi_max=vmax)
+    quantized = cfg.startswith('quant')
+    rng = np.random.default_rng(bins + head)
+    clips = [_spanning_clip(rng, t, config, quantized) for t in (2047, 2048, 2049, 5000, 9000)]
+    logits, bounds, arrs = (list(x) for x in zip(*clips))
+    ms, bs, cor, probs, cu = _kernel(config, quantized, logits, bounds, arrs, head=head)
+    for i, t in enumerate(len(b) for b in bounds):
+        ref = oeval.losses(logits[i], bounds[i], arrs[i], config, quantized)
+        np.testing.assert_allclose(_per_item(ms[i], t, bins, quantized), ref['midi_loss'], rtol=1e-5)
+        np.testing.assert_allclose(bs[i] / t, ref['bound_loss'], rtol=1e-5)
+        p = probs[cu[i]:cu[i + 1]]
+        act = torch.softmax(torch.from_numpy(logits[i]), -1) if quantized else torch.sigmoid(torch.from_numpy(logits[i]))
+        np.testing.assert_allclose(p, act.numpy(), rtol=1e-5, atol=1e-7)
+        correct, total = oeval.accuracy_counts(logits[i], arrs[i], config, quantized, probs=p)
+        assert total == t and cor[i] == correct, (i, cor[i], correct)
+        assert correct > t // 8, correct
 
 
 @pytest.mark.parametrize('cfg', CFGS)

@@ -139,6 +139,23 @@ def test_state_dict_schema_and_strict_loading(tmp_path):
         sconfig.check_supported(dict(cfg, units_dim=768))
 
 
+def test_check_supported_head_widths():
+    """Widths the decode and scoring kernels refuse are refused when the model is loaded, naming the value: fewer than
+    2 bins (the reference divides by N - 1 = 0), more than 256, and a quantized task with N != 129."""
+    cont, quant = synth.named_config('two_head'), synth.named_config('quant_two_head')
+    for n in (2, 64, 128, 129, 200, 256):
+        sconfig.check_supported(dict(cont, midi_num_bins=n, midi_max=cont['midi_min'] + n - 1))
+    sconfig.check_supported(quant)
+    for n in (1, 0, -3, 257):
+        with pytest.raises(NotImplementedError, match=rf'midi_num_bins={n} \(the decode takes 2 to 256 bins\)'):
+            sconfig.check_supported(dict(cont, midi_num_bins=n))
+        with pytest.raises(NotImplementedError, match=rf'midi_num_bins={n} '):
+            sconfig.check_supported(dict(quant, midi_num_bins=n))
+    for n in (2, 128, 130, 256):
+        with pytest.raises(NotImplementedError, match=rf'midi_num_bins={n} for training.QuantizedMIDIExtractionTask'):
+            sconfig.check_supported(dict(quant, midi_num_bins=n))
+
+
 def test_schema_matches_reference_module():
     # parameter names / shapes of the reference's midi_conforms (tests/golden/make_golden_reference_meta.py)
     ref = json.loads((REPO / 'tests' / 'golden' / 'reference_state_dict_shapes.json').read_text())

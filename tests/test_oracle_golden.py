@@ -1,5 +1,8 @@
 """Pins oracle/ (the CPU restatement) against the golden vectors produced by the unmodified
 reference (tests/golden/make_golden.py) and the SURVEY.md §4 known answers.  CPU only."""
+import pathlib
+import sys
+
 import numpy as np
 import pytest
 import torch
@@ -9,6 +12,9 @@ from oracle import melbank
 from oracle import model as omodel
 from oracle.metrics import note_agreement
 from some_b200 import synth
+
+sys.path.insert(0, str(pathlib.Path(__file__).resolve().parent / 'golden'))
+from decode_bins_cases import DEVIATION, THRESHOLD, WIDTHS, make_probe  # noqa: E402
 
 
 def test_melbank_known_answers(golden_dir):
@@ -27,6 +33,22 @@ def test_melbank_known_answers(golden_dir):
     assert np.abs(w - ta).max() < 2e-7                      # independent implementation
 
 
+def _assert_log_mel_close(got, ref, key, log_atol, floor):
+    """Round-off of an fp32 FFT is absolute: about eps times the frame's energy in every bin, so a band far below the
+    frame's largest one can carry a large relative error, and how large depends on the FFT code the CPU runs.  Between
+    MKL's AVX-512, AVX2 and SSE4.2 paths the oracle differs from the reference's fp32 bands by up to 3.6e-7 of the
+    frame's largest band (and the reference's own bands differ from a float64 STFT by up to 5.5e-3 in the log domain, on
+    the quietest bands of a pure tone).  So every band is compared in the linear domain relative to the largest band of
+    its frame (2e-6), and in the log domain where it is at least ``floor`` of that band (``log_atol``)."""
+    glin, rlin = np.exp(got.astype(np.float64)), np.exp(ref.astype(np.float64))
+    scale = rlin.max(axis=0, keepdims=True)                     # [1, T]: the frame's largest band
+    lin_err = float((np.abs(glin - rlin) / scale).max()) if ref.size else 0.0
+    assert lin_err < 2e-6, (key, lin_err)
+    big = rlin >= floor * scale
+    log_err = float(np.abs(got - ref)[big].max()) if big.any() else 0.0
+    assert log_err < log_atol, (key, log_err)
+
+
 def test_log_mel_matches_reference(golden_dir):
     g = np.load(golden_dir / 'mel.npz')
     clips = synth.edge_case_waveforms()
@@ -35,7 +57,7 @@ def test_log_mel_matches_reference(golden_dir):
         ref = g['mel_' + name]
         got = omodel.log_mel(torch.from_numpy(w).unsqueeze(0))[0].numpy()
         assert got.shape == ref.shape == (80, synth.frames_of(len(w))), name
-        np.testing.assert_allclose(got, ref, rtol=0, atol=2e-4, err_msg=name)
+        _assert_log_mel_close(got, ref, name, log_atol=2e-4, floor=1e-2)
     assert np.all(g['mel_zeros'] == np.float32(np.log(np.float32(1e-5))))   # silence -> log(clamp)
 
 
@@ -156,6 +178,31 @@ def test_vectorised_decode_equals_loops():
                 np.testing.assert_array_equal(x, y)
 
 
+@pytest.mark.parametrize('n,vmin,vmax', WIDTHS)
+def test_decode_head_widths_match_reference_exactly(golden_dir, n, vmin, vmax):
+    """Head widths other than 128 (tests/golden/make_golden_decode_bins.py): the bin values are float32 arithmetic in the
+    reference, so on probes whose sums do not depend on their order the oracle must give the reference's bits."""
+    g = np.load(golden_dir / 'decode_bins.npz')
+    key = f'n{n}_{vmin}_{vmax}'
+    probs, bounds = make_probe(n, vmin, vmax)
+    assert probs.astype(np.float64).sum() == g[f'{key}_probs_checksum']
+    f2i = odecode.decode_bounds_to_alignment(bounds)
+    np.testing.assert_array_equal(f2i, g[f'{key}_frame2item'])
+    for blur, notes in ((odecode.decode_gaussian_blurred_probs, odecode.decode_note_sequence),
+                        (odecode.decode_gaussian_blurred_probs_vec, odecode.decode_note_sequence_vec)):
+        v, r = blur(probs, vmin, vmax, DEVIATION, THRESHOLD)
+        np.testing.assert_array_equal(v, g[f'{key}_values'])
+        np.testing.assert_array_equal(r, g[f'{key}_rest'])
+        nm, nd, nk = notes(f2i, v, ~r)
+        np.testing.assert_array_equal(nm, g[f'{key}_note_midi'])
+        np.testing.assert_array_equal(nd, g[f'{key}_note_dur'])
+        np.testing.assert_array_equal(nk, g[f'{key}_note_mask'])
+    # the probes reach what they are for: every bin value, rests, notes with and without valid frames
+    one_hot = (probs == 1.0).sum(1) == (probs != 0).sum(1)
+    assert set(probs[one_hot].argmax(1)) == set(range(n))
+    assert g[f'{key}_rest'].any() and (~g[f'{key}_note_mask']).any() and g[f'{key}_note_mask'].any()
+
+
 def test_quantised_decode_matches_reference(golden_dir):
     """inference/me_quant_infer.py:21-38 on random 129-bin probabilities: the oracle's quantised decode against the
     reference's own postprocess outputs (decode_quant_kat.npz), exactly."""
@@ -189,4 +236,4 @@ def test_oracle_keyshift_mel_matches_reference(golden_dir):
     for key, kw in cases:
         got = omodel.log_mel(audio, fmin=40, fmax=8000, **kw)[0].numpy()
         assert got.shape == g[key].shape, key
-        assert float(np.abs(got - g[key]).max()) < 2e-5, key        # same torch.stft; summation-order noise only
+        _assert_log_mel_close(got, g[key], key, log_atol=2e-5, floor=0.1)   # same torch.stft: round-off only
