@@ -1,13 +1,23 @@
-"""Measures streaming transcription (some_stream_*): N concurrent streams on one session, one thread each, every stream
-pushing a synthetic recording with silence gaps in fixed-size blocks as fast as it can.  Reports the aggregate audio-seconds
-per second, the wall time of a push (median and p99, split into pushes that delivered a chunk and pushes that did not), the
-CUDA-event time of the windowed front-end kernels for a push of one block (the launches such a push makes, replayed on their
-own outside the streams at a fixed position 1 s into the recording, 200 times back to back: not timed inside the pushes), and
-some_session_transcribe_sliced on the same recordings as the one-shot reference.  Checks that every stream's chunks equal the one-shot result.
+"""Measures streaming transcription (some_stream_*) of N streams on one session, every stream pushing a synthetic recording
+with silence gaps in fixed-size blocks as fast as it can, in two arms run alternately in one process:
 
-    python bench_stream.py [--streams 1,16,128] [--blocks-ms 20,100] [--seconds 300] [--rate 44100]
+- threaded: one thread per stream, each calling Stream.push.  Reports the aggregate audio-seconds per second, the wall time
+  of a push (median and p99, split into pushes that delivered a chunk and pushes that did not), and the CUDA-event time of the
+  windowed front-end kernels for a push of one block (the launches such a push makes, replayed on their own outside the
+  streams at a fixed position 1 s into the recording, 200 times back to back: not timed inside the pushes).
+- push_many: one thread; per tick one Session.push_many call with one block for every stream that still has samples, and
+  finish at each stream's end.  Reports the aggregate audio-seconds per second, the tick wall time (median and p99) and the
+  chunks per forward batch (ticks that delivered chunks).
 
-Prints the card's name and power limit beside the numbers, and one JSON line per configuration."""
+Both arms check that every stream's chunks equal some_session_transcribe_sliced on the same recording, which is also timed
+as the one-shot reference.
+
+    python bench_stream.py [--streams 1,16,128,1024] [--blocks-ms 20,100] [--seconds 300] [--rate 44100]
+                           [--arms threaded,push_many] [--threaded-max 128]
+
+The threaded arm is skipped above --threaded-max streams: its pushes serialise on the session, so 1024 threads take about
+eight times as long as 128 for the same total rate.  Prints the card's name and power limit beside the numbers, and one JSON
+line per configuration and arm."""
 import argparse
 import ctypes as C
 import json
@@ -66,13 +76,100 @@ def kernel_times(rate, block, sr=44100, reps=200):
     return ev[0].elapsed_time(ev[1]) / reps
 
 
+def threaded_arm(sess, pool, want, n, block, block_ms, args, kern):
+    times = [[] for _ in range(n)]
+    errors, mismatches = [], []
+
+    def work(i):
+        w = pool[i % len(pool)]
+        got = []
+        try:
+            with sess.stream(args.rate) as st:
+                for a in range(0, w.shape[0], block):
+                    t0 = time.perf_counter()
+                    o, r, nt = st.push(w[a:a + block])
+                    times[i].append((time.perf_counter() - t0, bool(r)))
+                    got += r
+                got += st.finish()[1]
+            if got != want[i % len(pool)][1]:
+                mismatches.append(i)
+        except Exception as e:         # noqa: BLE001
+            errors.append(repr(e))
+
+    threads = [threading.Thread(target=work, args=(i,)) for i in range(n)]
+    t = time.perf_counter()
+    for th in threads:
+        th.start()
+    for th in threads:
+        th.join()
+    wall = time.perf_counter() - t
+    flat = [x for ts in times for x in ts]
+    dl = np.array([x for x, d in flat if d]) * 1e3
+    nd = np.array([x for x, d in flat if not d]) * 1e3
+    res = {'config': f'stream x{n}', 'arm': 'threaded', 'block_ms': block_ms, 'seconds': args.seconds,
+           'audio_s_per_s': round(n * args.seconds / wall, 1), 'pushes': len(flat),
+           'push_ms_no_chunk_median': round(float(np.median(nd)), 3) if nd.size else None,
+           'push_ms_no_chunk_p99': round(float(np.percentile(nd, 99)), 3) if nd.size else None,
+           'push_ms_chunk_median': round(float(np.median(dl)), 3) if dl.size else None,
+           'push_ms_chunk_p99': round(float(np.percentile(dl, 99)), 3) if dl.size else None,
+           'window_kernels_ms_replayed_push': round(kern, 4), 'identical': not mismatches and not errors}
+    if errors:
+        res['errors'] = errors[:3]
+    return res
+
+
+def push_many_arm(sess, pool, want, n, block, block_ms, args):
+    waves = [pool[i % len(pool)] for i in range(n)]
+    streams = [sess.stream(args.rate) for _ in range(n)]
+    got = [[] for _ in range(n)]
+    pos, live = [0] * n, list(range(n))
+    ticks, batches, errors = [], [], []
+    t = time.perf_counter()
+    try:
+        while live:
+            items, fin = [], []
+            for i in live:
+                part = waves[i][pos[i]:pos[i] + block]
+                pos[i] += part.shape[0]
+                items.append((streams[i], part))
+                fin.append(pos[i] >= waves[i].shape[0])
+            t0 = time.perf_counter()
+            res = sess.push_many(items, fin)
+            ticks.append(time.perf_counter() - t0)
+            chunks = sum(len(r[1]) for r in res)
+            if chunks:
+                batches.append(chunks)
+            for i, r in zip(live, res):
+                got[i] += r[1]
+            live = [i for i, f in zip(live, fin) if not f]
+    except Exception as e:             # noqa: BLE001
+        errors.append(repr(e))
+    wall = time.perf_counter() - t
+    for st in streams:
+        st.close()
+    tk = np.array(ticks) * 1e3
+    res = {'config': f'stream x{n}', 'arm': 'push_many', 'block_ms': block_ms, 'seconds': args.seconds,
+           'audio_s_per_s': round(n * args.seconds / wall, 1), 'ticks': len(ticks),
+           'tick_ms_median': round(float(np.median(tk)), 3) if tk.size else None,
+           'tick_ms_p99': round(float(np.percentile(tk, 99)), 3) if tk.size else None,
+           'chunks_per_batch_mean': round(float(np.mean(batches)), 2) if batches else None,
+           'chunks_per_batch_max': int(max(batches)) if batches else None,
+           'identical': not errors and all(got[i] == want[i % len(pool)][1] for i in range(n))}
+    if errors:
+        res['errors'] = errors[:3]
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument('--streams', default='1,16,128')
+    ap.add_argument('--streams', default='1,16,128,1024')
     ap.add_argument('--blocks-ms', default='20,100')
     ap.add_argument('--seconds', type=float, default=300.0)
     ap.add_argument('--rate', type=int, default=44100)
+    ap.add_argument('--arms', default='threaded,push_many')
+    ap.add_argument('--threaded-max', type=int, default=128)
     args = ap.parse_args()
+    arms = args.arms.split(',')
     import torch
     if not torch.cuda.is_available():
         sys.exit('bench_stream.py needs a CUDA device')
@@ -93,45 +190,10 @@ def main():
             block = args.rate * block_ms // 1000
             kern = kernel_times(args.rate, block)
             for n in counts:
-                times = [[] for _ in range(n)]
-                errors, mismatches = [], []
-
-                def work(i):
-                    w = pool[i % len(pool)]
-                    got = []
-                    try:
-                        with sess.stream(args.rate) as st:
-                            for a in range(0, w.shape[0], block):
-                                t0 = time.perf_counter()
-                                o, r, nt = st.push(w[a:a + block])
-                                times[i].append((time.perf_counter() - t0, bool(r)))
-                                got += r
-                            got += st.finish()[1]
-                        if got != want[i % len(pool)][1]:
-                            mismatches.append(i)
-                    except Exception as e:         # noqa: BLE001
-                        errors.append(repr(e))
-
-                threads = [threading.Thread(target=work, args=(i,)) for i in range(n)]
-                t = time.perf_counter()
-                for th in threads:
-                    th.start()
-                for th in threads:
-                    th.join()
-                wall = time.perf_counter() - t
-                flat = [x for ts in times for x in ts]
-                dl = np.array([x for x, d in flat if d]) * 1e3
-                nd = np.array([x for x, d in flat if not d]) * 1e3
-                res = {'config': f'stream x{n}', 'block_ms': block_ms, 'seconds': args.seconds,
-                       'audio_s_per_s': round(n * args.seconds / wall, 1), 'pushes': len(flat),
-                       'push_ms_no_chunk_median': round(float(np.median(nd)), 3) if nd.size else None,
-                       'push_ms_no_chunk_p99': round(float(np.percentile(nd, 99)), 3) if nd.size else None,
-                       'push_ms_chunk_median': round(float(np.median(dl)), 3) if dl.size else None,
-                       'push_ms_chunk_p99': round(float(np.percentile(dl, 99)), 3) if dl.size else None,
-                       'window_kernels_ms_replayed_push': round(kern, 4), 'identical': not mismatches and not errors}
-                if errors:
-                    res['errors'] = errors[:3]
-                print(json.dumps(res), flush=True)
+                if 'threaded' in arms and n <= args.threaded_max:
+                    print(json.dumps(threaded_arm(sess, pool, want, n, block, block_ms, args, kern)), flush=True)
+                if 'push_many' in arms:
+                    print(json.dumps(push_many_arm(sess, pool, want, n, block, block_ms, args)), flush=True)
         sess.close()
 
 

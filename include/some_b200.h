@@ -271,6 +271,23 @@ int some_slicer_rms(const float* wave, long long n_samples, int frame_length, in
  * Bit-identical to some_slicer_rms on the whole recording. */
 int some_slicer_rms_window(const float* wave, long long base, long long held, long long n_samples, int frame_length, int hop,
                            float* rms, long long f_begin, long long f_end, cudaStream_t stream);
+/* Many frame windows in one launch (the streams of one some_stream_push_many call).  Window i is the call
+ * some_slicer_rms_window(w[i].wave, ..., w[i].f_end) and gets its bits.  Two steps, so that the descriptors can travel in a
+ * host-to-device copy the caller makes anyway:
+ *   some_slicer_rms_windows_pack  checks every window as some_slicer_rms_window does (the message names the window) and
+ *                                 writes the kernel's descriptors to `desc`, host memory of some_slicer_rms_windows_bytes(K) bytes;
+ *   some_slicer_rms_windows       launches, sized by the host copy `desc`, reading the descriptors from `desc_d`, a device
+ *                                 copy of the same bytes (16-byte aligned) that is in place when the launch runs. */
+typedef struct {
+  const float* wave;
+  long long base, held, n_samples;
+  int frame_length, hop;
+  float* rms;
+  long long f_begin, f_end;
+} some_rms_window;
+long long some_slicer_rms_windows_bytes(int K);
+int some_slicer_rms_windows_pack(const some_rms_window* w, int K, void* desc);
+int some_slicer_rms_windows(const void* desc, const void* desc_d, cudaStream_t stream);
 
 /* ---- K-resample (the step in front of the slicer): librosa.resample(y, orig_sr, target_sr, res_type='kaiser_best') as
  * librosa.load calls it (infer.py:34, batch_infer.py:51, webui.py:47; librosa<0.10 -> resampy.resample(filter='kaiser_best')
@@ -298,6 +315,25 @@ int some_resample_kaiser_window(const float* x, long long x_first, long long rec
                                 cudaStream_t stream);
 int some_resample_window_plan(long long received, int final, long long t_begin, int sr_orig, int sr_new, int nwin,
                               long long* t_end, long long* x_first);
+/* Many windows in one launch, each with its own recording, rate pair and table: window i is the call
+ * some_resample_kaiser_window(w[i].x, ..., w[i].nwin) and gets its bits.  The grid lays the windows' tiles end to end; the
+ * dynamic shared memory is the largest the windows' rate pairs need.  Packed and launched in two steps like
+ * some_slicer_rms_windows: some_resample_windows_pack checks every window as some_resample_kaiser_window does (the message
+ * names the window) and writes the descriptors to host memory of some_resample_windows_bytes(K) bytes;
+ * some_resample_kaiser_windows launches from the host copy `desc` and its device copy `desc_d` (16-byte aligned). */
+typedef struct {
+  const float* x;
+  long long x_first, received;
+  int final;
+  float* y;
+  long long y_first, t_begin, t_end;
+  int sr_orig, sr_new;
+  const double* win;
+  int nwin;
+} some_resample_window;
+long long some_resample_windows_bytes(int K);
+int some_resample_windows_pack(const some_resample_window* w, int K, void* desc);
+int some_resample_kaiser_windows(const void* desc, const void* desc_d, cudaStream_t stream);
 
 /* ---- K-flac (the step in front of K-resample): the FLAC decode of librosa.load (soundfile -> libsndfile -> libFLAC) for
  * many recordings in one set of launches, from slices of one device byte buffer `data` (restated in oracle/flac.py).
@@ -621,8 +657,8 @@ int some_slicer_stream_destroy(some_slicer_stream* st);
  * the latest about 2.1 s into a longer silence.  A frame is known once the samples it reads are fixed: at the model's rate
  * when they are received; at another rate once the resampler's right wing behind them has been received (<= 64 input samples
  * when upsampling, nwin / index_step when downsampling).
- *   Each push uploads its samples through pinned memory, resamples the outputs they fix (some_resample_kaiser_window),
- * computes the RMS frames those complete (some_slicer_rms_window), downloads them with one synchronise, takes the slicer's
+ *   Each push uploads its samples through pinned memory, resamples the outputs they fix (some_resample_kaiser_windows),
+ * computes the RMS frames those complete (some_slicer_rms_windows), downloads them with one synchronise, takes the slicer's
  * decisions on the host (some_slicer_stream_*, csrc/slicer.cu) and transcribes the final chunks where they lie in the
  * stream's device buffer.  The buffer keeps only what a later chunk or RMS frame can read: `held` stays within the longest
  * chunk plus 2 max_sil_kept frames and the RMS window (during a long leading silence: the first and the last max_sil_kept
@@ -644,6 +680,22 @@ int some_stream_push(some_stream* st, const float* samples, long long n, some_no
 int some_stream_finish(some_stream* st, some_notes* out);
 int some_stream_get_info(const some_stream* st, some_stream_info* info);
 int some_stream_close(some_stream* st);
+/* Many streams: advances `count` streams of one session in one step.  For stream i, the effect is some_stream_push(streams[i],
+ * samples[i], n[i], out[i]), followed by some_stream_finish when finish != NULL and finish[i] != 0.  out[i] receives the
+ * chunks of both.  finish may be NULL.
+ *   Each stream keeps the contract above, over any mix of push, finish and push_many calls, and gets each chunk in the call in
+ * which some_stream_push would deliver it.  The streams of one call may have different rates and slicer params.  The call
+ * does the GPU work once for all of them: one upload, one resampling and one RMS launch, one synchronise, and every chunk that
+ * became final in any of the streams in one batch through the model.  So every stream of a call waits for the chunks of all.
+ *   Refused, with the index i in the message and no stream changed, when: an array is NULL or count < 0; a stream is NULL,
+ * belongs to another session than stream 0, appears twice or has finished; n[i] < 0, or samples[i] is NULL while n[i] > 0;
+ * two entries share one some_notes; a resampling stream is to finish with too few input samples to resample.  count == 0
+ * does nothing.  A failure after that (a device error) is reported like one of some_stream_push; the session stays usable,
+ * but on every stream of the failed call only some_stream_get_info and some_stream_close remain defined.
+ *   The call takes the session's mutex once.  Threads may call it on disjoint sets of streams of one session, mixed with
+ * single pushes on other streams; one stream is used by one thread at a time. */
+int some_stream_push_many(some_stream* const* streams, const float* const* samples, const long long* n, const int* finish,
+                          int count, some_notes* const* out);
 
 #ifdef __cplusplus
 }

@@ -136,6 +136,18 @@ class StreamInfo(C.Structure):
     _fields_ = [('received', C.c_int64), ('fixed', C.c_int64), ('held', C.c_int64)]
 
 
+class ResampleWindow(C.Structure):
+    _fields_ = [('x', _vp), ('x_first', C.c_longlong), ('received', C.c_longlong), ('final', C.c_int), ('y', _vp),
+                ('y_first', C.c_longlong), ('t_begin', C.c_longlong), ('t_end', C.c_longlong), ('sr_orig', C.c_int),
+                ('sr_new', C.c_int), ('win', _vp), ('nwin', C.c_int)]
+
+
+class RmsWindow(C.Structure):
+    _fields_ = [('wave', _vp), ('base', C.c_longlong), ('held', C.c_longlong), ('n_samples', C.c_longlong),
+                ('frame_length', C.c_int), ('hop', C.c_int), ('rms', _vp), ('f_begin', C.c_longlong),
+                ('f_end', C.c_longlong)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     'some_version': (C.c_int, []),
@@ -166,6 +178,12 @@ EXPORTS = {
                                               C.c_longlong, C.c_int, C.c_int, _vp, C.c_int, _vp]),
     'some_resample_window_plan': (C.c_int, [C.c_longlong, C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_int,
                                             C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]),
+    'some_resample_windows_bytes': (C.c_longlong, [C.c_int]),
+    'some_resample_windows_pack': (C.c_int, [C.POINTER(ResampleWindow), C.c_int, _vp]),
+    'some_resample_kaiser_windows': (C.c_int, [_vp, _vp, _vp]),
+    'some_slicer_rms_windows_bytes': (C.c_longlong, [C.c_int]),
+    'some_slicer_rms_windows_pack': (C.c_int, [C.POINTER(RmsWindow), C.c_int, _vp]),
+    'some_slicer_rms_windows': (C.c_int, [_vp, _vp, _vp]),
     'some_flac_scan_workspace_bytes': (C.c_uint64, [C.c_longlong]),
     'some_flac_scan': (C.c_int, [_vp, C.c_longlong, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp]),
     'some_flac_decode': (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp, C.c_int, _vp, _vp]),
@@ -205,6 +223,7 @@ EXPORTS = {
     'some_stream_finish': (C.c_int, [_vp, _vp]),
     'some_stream_get_info': (C.c_int, [_vp, C.POINTER(StreamInfo)]),
     'some_stream_close': (C.c_int, [_vp]),
+    'some_stream_push_many': (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, _vp]),
 }
 
 _lib = None

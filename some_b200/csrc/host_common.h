@@ -64,4 +64,44 @@ inline int64_t frames_within(const some_slicer_frames& f, int64_t fixed) {
   return fixed < reach ? 0 : (fixed - reach) / f.hop_size + 1;
 }
 
+// Packed descriptors of a many-window launch (some_resample_windows_pack, some_slicer_rms_windows_pack and the stream's
+// upload): a header, the windows' first tiles (K + 1 prefix sums: the grid lays the windows' tiles end to end) and the K
+// kernel parameter blocks P, each part 16-byte aligned.  The host copy sizes the launch; the kernel reads a device copy of
+// the same bytes.
+struct WindowsHeader {
+  long long K, tiles, smem, pad;
+};
+constexpr size_t align16(size_t b) { return (b + 15) & ~size_t(15); }
+template <class P>
+size_t windows_bytes(int K) {
+  return sizeof(WindowsHeader) + align16(8ull * (K + 1)) + sizeof(P) * K;
+}
+inline long long* windows_tile0(void* desc) {
+  return reinterpret_cast<long long*>(static_cast<char*>(desc) + sizeof(WindowsHeader));
+}
+template <class P>
+P* windows_params(void* desc, int K) {
+  return reinterpret_cast<P*>(static_cast<char*>(desc) + sizeof(WindowsHeader) + align16(8ull * (K + 1)));
+}
+
+// Completes the descriptors of K windows whose tile counts the packer left in tile0[1 .. K]: the prefix sums and the header.
+inline void windows_index(void* desc, int K, long long smem) {
+  WindowsHeader* h = static_cast<WindowsHeader*>(desc);
+  long long* tile0 = windows_tile0(desc);
+  tile0[0] = 0;
+  for (int w = 0; w < K; ++w) tile0[w + 1] += tile0[w];
+  h->K = K, h->tiles = tile0[K], h->smem = smem, h->pad = 0;
+}
+
+// The window w with tile0[w] <= tile < tile0[w + 1]: the last of equal prefixes, so windows without tiles are skipped.
+__device__ __forceinline__ int window_of(const long long* __restrict__ tile0, int K, long long tile) {
+  int lo = 0, hi = K - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) / 2;
+    if (__ldg(tile0 + mid) <= tile) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
 }  // namespace some

@@ -93,17 +93,17 @@ __device__ __forceinline__ void table_pos(double frac, int& off, double& eta) {
   eta = __dsub_rn(index_frac, static_cast<double>(off));
 }
 
-// kWindow = false: the batched form, recording b = blockIdx.y whole.  kWindow = true: outputs [t_begin, t_end) of one recording
-// from a buffer that holds only part of its input.  Every output's arithmetic depends on its absolute position t alone (n, the
-// table position, the wing limits against 0 and len), not on the tile it falls in, so both forms give the same bits.
+// kWindow = false: the batched form, recording b whole.  kWindow = true: outputs [t_begin, t_end) of one recording from a
+// buffer that holds only part of its input.  Every output's arithmetic depends on its absolute position t alone (n, the table
+// position, the wing limits against 0 and len), not on the tile it falls in, so both forms, and every kernel that computes
+// its tiles with this function, give the same bits.
 template <bool kWindow>
-__global__ void __launch_bounds__(RS_THREADS, 2) resample_kaiser_kernel(const ResampleParams p) {
+__device__ __forceinline__ void resample_tile(const ResampleParams& p, int b, long long tile) {
   extern __shared__ double rs_smem[];
-  const int b = blockIdx.y;
   const long long L = kWindow ? p.len : p.x_len[b];
   const long long n_total = static_cast<long long>(ceil(__dmul_rn(static_cast<double>(L), p.ratio)));   // fix_length
   const long long n_out = L * p.sr_new / p.sr_orig;                                                       // resampy's length
-  const long long t0 = (kWindow ? p.t_begin : 0) + static_cast<long long>(blockIdx.x) * RS_TILE;
+  const long long t0 = (kWindow ? p.t_begin : 0) + tile * RS_TILE;
   const long long t_stop = kWindow ? min(p.t_end, n_total) : n_total;
   if (t0 >= t_stop) return;
   float* y = p.y + (kWindow ? -p.y_first : p.y_start[b]);   // y[t]: output t
@@ -152,6 +152,19 @@ __global__ void __launch_bounds__(RS_THREADS, 2) resample_kaiser_kernel(const Re
   }
 }
 
+template <bool kWindow>
+__global__ void __launch_bounds__(RS_THREADS, 2) resample_kaiser_kernel(const ResampleParams p) {
+  resample_tile<kWindow>(p, blockIdx.y, blockIdx.x);
+}
+
+// K windows of kWindow form in one grid: the windows' tiles laid end to end, each CTA finds its window from the tile prefix.
+__global__ void __launch_bounds__(RS_THREADS, 2) resample_windows_kernel(const ResampleParams* __restrict__ ps,
+                                                                         const long long* __restrict__ tile0, int K) {
+  const long long tile = blockIdx.x;
+  const int w = window_of(tile0, K, tile);
+  resample_tile<true>(ps[w], 0, tile - tile0[w]);
+}
+
 
 // The rate-pair constants of resampy.resample and the kernel's shared-memory size for them.
 int setup(ResampleParams& p, int sr_orig, int sr_new, int nwin, const char* what, double* smem) {
@@ -197,6 +210,26 @@ void plan(const ResampleParams& p, long long received, int final, long long t_be
   *x_first = std::max(0ll, centre(p, t_begin) - p.max_taps + 1);
 }
 
+// The kernel parameters of one window, with the checks of some_resample_kaiser_window: the buffer must hold every input
+// sample the outputs read, and the received input must fix every output requested.
+int window_params(const some_resample_window& w, const char* what, ResampleParams& p, double* smem) {
+  SOME_REQUIRE(w.x && w.y && w.win, "%s: null pointer", what);
+  p = ResampleParams{};
+  if (setup(p, w.sr_orig, w.sr_new, w.nwin, what, smem)) return -1;
+  long long fixed_end, need_first;
+  plan(p, w.received, w.final, w.t_begin, &fixed_end, &need_first);
+  SOME_REQUIRE(w.x_first >= 0 && w.x_first <= w.received && w.t_begin >= 0 && w.t_begin <= w.t_end && w.y_first <= w.t_begin,
+               "%s: bad window (input from %lld of %lld, outputs [%lld, %lld) at %lld)", what, w.x_first, w.received, w.t_begin,
+               w.t_end, w.y_first);
+  SOME_REQUIRE(w.t_end <= fixed_end, "%s: outputs up to %lld requested, %lld received input samples fix %lld%s", what, w.t_end,
+               w.received, fixed_end, w.final ? "" : " (their right wings would reach past the input)");
+  SOME_REQUIRE(w.x_first <= need_first || w.t_begin == w.t_end, "%s: output %lld reads input from %lld, the buffer starts at "
+               "%lld", what, w.t_begin, need_first, w.x_first);
+  p.x = w.x, p.y = w.y, p.win = w.win;
+  p.x_first = w.x_first, p.y_first = w.y_first, p.t_begin = w.t_begin, p.t_end = w.t_end, p.len = w.received;
+  return 0;
+}
+
 }  // namespace some
 
 using namespace some;
@@ -235,22 +268,11 @@ extern "C" int some_resample_window_plan(long long received, int final, long lon
 extern "C" int some_resample_kaiser_window(const float* x, long long x_first, long long received, int final, float* y,
                                            long long y_first, long long t_begin, long long t_end, int sr_orig, int sr_new,
                                            const double* win, int nwin, cudaStream_t stream) {
-  SOME_REQUIRE(x && y && win, "some_resample_kaiser_window: null pointer");
-  ResampleParams p{};
+  const some_resample_window w{x, x_first, received, final, y, y_first, t_begin, t_end, sr_orig, sr_new, win, nwin};
+  ResampleParams p;
   double smem;
-  if (setup(p, sr_orig, sr_new, nwin, "some_resample_kaiser_window", &smem)) return -1;
-  long long fixed_end, need_first;
-  plan(p, received, final, t_begin, &fixed_end, &need_first);
-  SOME_REQUIRE(x_first >= 0 && x_first <= received && t_begin >= 0 && t_begin <= t_end && y_first <= t_begin,
-               "some_resample_kaiser_window: bad window (input from %lld of %lld, outputs [%lld, %lld) at %lld)", x_first,
-               received, t_begin, t_end, y_first);
-  SOME_REQUIRE(t_end <= fixed_end, "some_resample_kaiser_window: outputs up to %lld requested, %lld received input samples "
-               "fix %lld%s", t_end, received, fixed_end, final ? "" : " (their right wings would reach past the input)");
-  SOME_REQUIRE(x_first <= need_first || t_begin == t_end, "some_resample_kaiser_window: output %lld reads input from %lld, "
-               "the buffer starts at %lld", t_begin, need_first, x_first);
+  if (window_params(w, "some_resample_kaiser_window", p, &smem)) return -1;
   if (t_begin == t_end) return 0;
-  p.x = x, p.y = y, p.win = win;
-  p.x_first = x_first, p.y_first = y_first, p.t_begin = t_begin, p.t_end = t_end, p.len = received;
   const long long tiles = (t_end - t_begin + RS_TILE - 1) / RS_TILE;
   SOME_REQUIRE(tiles < (1ll << 31), "some_resample_kaiser_window: grid too large");
   cudaError_t e = cudaFuncSetAttribute(resample_kaiser_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -258,4 +280,38 @@ extern "C" int some_resample_kaiser_window(const float* x, long long x_first, lo
   SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(resample): %s", cudaGetErrorString(e));
   resample_kaiser_kernel<true><<<dim3(static_cast<unsigned>(tiles), 1), RS_THREADS, static_cast<size_t>(smem), stream>>>(p);
   return check_launch("some_resample_kaiser_window");
+}
+
+extern "C" long long some_resample_windows_bytes(int K) { return K < 0 ? -1 : static_cast<long long>(windows_bytes<ResampleParams>(K)); }
+
+extern "C" int some_resample_windows_pack(const some_resample_window* w, int K, void* desc) {
+  SOME_REQUIRE(desc && K >= 0 && (K == 0 || w), "some_resample_windows_pack: bad arguments");
+  char what[64];
+  ResampleParams* ps = windows_params<ResampleParams>(desc, K);
+  long long* tile0 = windows_tile0(desc);
+  double smem_max = 0.0;
+  for (int i = 0; i < K; ++i) {
+    snprintf(what, sizeof(what), "some_resample_windows_pack: window %d", i);
+    double smem;
+    if (window_params(w[i], what, ps[i], &smem)) return -1;
+    tile0[i + 1] = (w[i].t_end - w[i].t_begin + RS_TILE - 1) / RS_TILE;
+    if (tile0[i + 1]) smem_max = std::max(smem_max, smem);
+  }
+  windows_index(desc, K, static_cast<long long>(smem_max));
+  SOME_REQUIRE(windows_tile0(desc)[K] < (1ll << 31), "some_resample_windows_pack: grid too large");
+  return 0;
+}
+
+extern "C" int some_resample_kaiser_windows(const void* desc, const void* desc_d, cudaStream_t stream) {
+  SOME_REQUIRE(desc && desc_d && reinterpret_cast<uintptr_t>(desc_d) % 16 == 0, "some_resample_kaiser_windows: bad arguments");
+  const WindowsHeader& h = *static_cast<const WindowsHeader*>(desc);
+  if (h.tiles == 0) return 0;
+  const int K = static_cast<int>(h.K);
+  void* d = const_cast<void*>(desc_d);
+  cudaError_t e = cudaFuncSetAttribute(resample_windows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(h.smem));
+  SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(resample): %s", cudaGetErrorString(e));
+  resample_windows_kernel<<<static_cast<unsigned>(h.tiles), RS_THREADS, static_cast<size_t>(h.smem), stream>>>(
+      windows_params<ResampleParams>(d, K), windows_tile0(d), K);
+  return check_launch("some_resample_kaiser_windows");
 }

@@ -1,5 +1,6 @@
 // Native inference session: a model file written by `python -m some_b200.export` in, notes out, with no Python or torch in
-// between.  Host code only; the work is done by the sm_90a kernels of this library, enqueued in the order Engine.enqueue
+// between.  Host code, and the copy kernel that scatters a stream step's upload; the work is done by the sm_90a kernels of
+// this library, enqueued in the order Engine.enqueue
 // (some_b200/engine.py) and Engine.infer_sliced use:
 //   [some_resample_kaiser] -> [some_slicer_rms + the slicer's decisions on the host] -> per pipeline chunk:
 //   some_mel_logmel -> some_forward (stand-alone LayerNorms, sigmoid / softmax head) -> some_decode_notes.
@@ -267,15 +268,21 @@ struct some_session {
   const int32_t *mel_start = nullptr, *mel_count = nullptr;
   const float *mel_weights = nullptr, *twiddle = nullptr, *window = nullptr;
   std::vector<double> kaiser;             // host copy of the float64 table (scaled per rate pair on upload)
-  std::vector<double> table_host;         // the scaled table of the current rate pair (source of its upload)
+  // the device tables by downsampling ratio (1.0: the unscaled table every upsampling pair shares), each kept with the host
+  // copy its upload reads
+  struct Table {
+    DevBuf d;
+    std::vector<double> h;
+  };
+  std::map<double, Table> tables;
   cudaStream_t stream = nullptr, copy_stream = nullptr;
   cudaEvent_t ev[4] = {};
   // grow-only buffers
-  DevBuf ws_block, scratch, wave_d, tab_d, cu_d, slab_d, native_d, table_d, meta_d, rms_d;
-  PinBuf wave_h, tab_h, cu_h, slab_h, meta_h, rms_h;
+  DevBuf ws_block, scratch, wave_d, tab_d, cu_d, slab_d, native_d, meta_d, rms_d, step_d;
+  PinBuf wave_h, tab_h, cu_h, slab_h, meta_h, rms_h, step_h;   // step: the samples and descriptors of a stream step
   int ws_m = 0;
   some_workspace ws{};
-  double table_ratio = 0.0;
+  some_notes chunks;                      // the notes of a stream step's chunks, before they are split by stream
   std::unique_ptr<WorkerPool> pool;
 };
 
@@ -286,10 +293,11 @@ void destroy(some_session* s) {
     DeviceScope scope(s->device);
     if (s->stream) cudaStreamSynchronize(s->stream);
     if (s->copy_stream) cudaStreamSynchronize(s->copy_stream);
-    for (DevBuf* b : {&s->ws_block, &s->scratch, &s->wave_d, &s->tab_d, &s->cu_d, &s->slab_d, &s->native_d, &s->table_d,
-                      &s->meta_d, &s->rms_d})
+    for (DevBuf* b : {&s->ws_block, &s->scratch, &s->wave_d, &s->tab_d, &s->cu_d, &s->slab_d, &s->native_d, &s->meta_d,
+                      &s->rms_d, &s->step_d})
       b->release();
-    for (PinBuf* b : {&s->wave_h, &s->tab_h, &s->cu_h, &s->slab_h, &s->meta_h, &s->rms_h}) b->release();
+    for (auto& t : s->tables) t.second.d.release();
+    for (PinBuf* b : {&s->wave_h, &s->tab_h, &s->cu_h, &s->slab_h, &s->meta_h, &s->rms_h, &s->step_h}) b->release();
     for (cudaEvent_t& e : s->ev)
       if (e) cudaEventDestroy(e);
     if (s->stream) cudaStreamDestroy(s->stream);
@@ -731,21 +739,25 @@ extern "C" int some_session_transcribe_sliced(some_session* s, const float* samp
 }
 
 namespace {
-// The resampling table for sample_rate -> the model's rate, uploaded on the session's stream (in front of the resampling
-// launches that read it) when the last upload was for another ratio.
-int ensure_table(some_session* s, int sample_rate) {
+// The resampling table for sample_rate -> the model's rate: uploaded on the session's stream (in front of the resampling
+// launches that read it) the first time its ratio is used, and kept.  Upsampling reads the table as it is; resampy scales it
+// by the ratio when downsampling (audio._device_table), so each downsampling ratio has its own copy.
+const double* table_for(some_session* s, int sample_rate) {
   const double ratio = static_cast<double>(s->info.sample_rate) / sample_rate;
-  const double key = ratio < 1 ? ratio : 1.0;
-  if (s->table_d.cap == 0 || s->table_ratio != key) {
-    s->table_host = s->kaiser;
+  some_session::Table& t = s->tables[ratio < 1 ? ratio : 1.0];
+  if (t.d.cap == 0) {
+    t.h = s->kaiser;
     if (ratio < 1)
-      for (double& v : s->table_host) v = ratio * v;   // audio._device_table: resampy scales the table when downsampling
-    if (s->table_d.ensure(8ull * kKaiserTaps, "the resampling table")) return -1;
-    SOME_CUDA(cudaMemcpyAsync(s->table_d.p, s->table_host.data(), 8ull * kKaiserTaps, cudaMemcpyHostToDevice, s->stream),
-              "table upload");
-    s->table_ratio = key;
+      for (double& v : t.h) v = ratio * v;
+    if (t.d.ensure(8ull * kKaiserTaps, "the resampling table")) return nullptr;
+    const cudaError_t e = cudaMemcpyAsync(t.d.p, t.h.data(), 8ull * kKaiserTaps, cudaMemcpyHostToDevice, s->stream);
+    if (e != cudaSuccess) {
+      set_error("session: table upload: %s", cudaGetErrorString(e));
+      t.d.release();
+      return nullptr;
+    }
   }
-  return 0;
+  return static_cast<const double*>(t.d.p);
 }
 
 int transcribe_sliced(some_session* s, const float* samples, int64_t n, int sample_rate, int64_t n_out,
@@ -758,7 +770,8 @@ int transcribe_sliced(some_session* s, const float* samples, int64_t n, int samp
   if (sample_rate == sr) {
     if (upload_staged(s, wave, samples, n)) return -1;
   } else {
-    if (ensure_table(s, sample_rate)) return -1;
+    const double* table = table_for(s, sample_rate);
+    if (!table) return -1;
     if (s->native_d.ensure(4ull * n + 16, "the native audio") || s->meta_h.ensure(32, "resampling tables") ||
         s->meta_d.ensure(32, "resampling tables"))
       return -1;
@@ -768,7 +781,7 @@ int transcribe_sliced(some_session* s, const float* samples, int64_t n, int samp
     if (upload_staged(s, static_cast<float*>(s->native_d.p), samples, n)) return -1;
     SOME_CUDA(cudaMemcpyAsync(s->meta_d.p, meta, 24, cudaMemcpyHostToDevice, s->stream), "table upload");
     if (some_resample_kaiser(static_cast<const float*>(s->native_d.p), md, md + 1, wave, md + 2, 1, n_out, sample_rate, sr,
-                             static_cast<const double*>(s->table_d.p), kKaiserTaps, s->stream))
+                             table, kKaiserTaps, s->stream))
       return -1;
   }
   // the slicer: a recording no longer than min_length is one chunk (slicer2.py:79-80)
@@ -829,6 +842,22 @@ struct SampleWindow {
     return 0;
   }
 };
+// The upload scatter of a stream step: entry j copies n samples of the step's device upload into a stream's window.
+struct ScatterParams {
+  const float* src;
+  float* dst;
+  long long n;
+};
+constexpr int kScatterThreads = 256, kScatterTile = 8 * kScatterThreads;
+
+__global__ void __launch_bounds__(kScatterThreads) scatter_kernel(const ScatterParams* __restrict__ ps,
+                                                                  const long long* __restrict__ tile0, int K) {
+  const long long tile = blockIdx.x;
+  const int w = window_of(tile0, K, tile);
+  const ScatterParams& p = ps[w];
+  const long long e = min(p.n, (tile - tile0[w] + 1) * kScatterTile);
+  for (long long i = (tile - tile0[w]) * kScatterTile + threadIdx.x; i < e; i += kScatterThreads) p.dst[i] = __ldg(p.src + i);
+}
 }  // namespace
 
 struct some_stream {
@@ -838,8 +867,6 @@ struct some_stream {
   some_slicer_stream* slicer = nullptr;   // the slicer's decisions (some_slicer_stream_*)
   some_slicer_frames f{};                 // its frame counts
   SampleWindow native, wave;              // the input at its own rate (when resampling) and at the model's rate
-  PinBuf stage_h, rms_h;
-  DevBuf rms_d;
   DevBuf head_d;                          // model-rate samples [0, head_len) kept apart during a long leading silence
   int64_t head_len = 0;
   int64_t received = 0, fixed = 0, frames = 0;   // frames: RMS frames computed so far
@@ -850,108 +877,220 @@ namespace {
 void destroy(some_stream* st) {
   {
     DeviceScope scope(st->s->device);
-    for (DevBuf* b : {&st->native.buf, &st->wave.buf, &st->rms_d, &st->head_d}) b->release();
-    for (PinBuf* b : {&st->stage_h, &st->rms_h}) b->release();
+    for (DevBuf* b : {&st->native.buf, &st->wave.buf, &st->head_d}) b->release();
   }
   some_slicer_stream_destroy(st->slicer);
   delete st;
 }
 
-// One step of a stream, under the session's mutex, with the n new samples in st->stage_h: upload, resample the outputs they
-// fix, compute the RMS frames those complete, take the slicer's decisions and transcribe the chunks that became final.
-// `final`: the recording ends here.
-int stream_step(some_stream* st, int64_t n, bool final, some_notes* out) {
-  some_session* s = st->s;
-  const some_slicer_frames& f = st->f;
+void clear(some_notes* out) {
+  out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
+}
+
+// One stream's part of a step: n new samples, whether the recording ends there, and where its chunks go.
+struct StepItem {
+  some_stream* st;
+  const float* samples;
+  int64_t n;
+  bool final;
+  some_notes* out;
+  int64_t up = 0;               // where its samples lie in the upload (floats)
+  int64_t rms0 = 0, nf = 0;     // its new RMS frames in the session's RMS buffer
+  int c0 = 0, c1 = 0;           // its chunks in the step's batch
+};
+
+// One step of any number of streams of one session, under the session's mutex.  Each stream does what a push of its samples
+// (and a finish, when `final`) does alone, but the GPU work is made once for all of them:
+//   1. per stream on the host: what to keep, the samples set apart during a leading silence, the window plans and room in the
+//      stream's buffers;
+//   2. the samples and the kernel descriptors in one pinned buffer, one host-to-device copy, one scatter launch into the
+//      streams' windows, one resampling launch and one RMS launch for all windows, one download of the RMS frames and one
+//      synchronise;
+//   3. the slicer's decisions for each stream;
+//   4. every chunk that became final, in any stream, copied next to each other and transcribed as one batch.
+int streams_step(some_session* s, std::vector<StepItem>& items) {
   const int sr = s->info.sample_rate;
-  long long keep_from, head;
-  if (some_slicer_stream_keep_from(st->slicer, &keep_from, &head, nullptr)) return -1;
-  // the model-rate samples a later chunk or RMS frame can still read
-  const int64_t keep = std::max<int64_t>(0, std::min<int64_t>(keep_from, st->frames * f.hop_size - f.win_size / 2));
-  // during a long leading silence (head > 0), the first max_sil_kept frames go apart before the window drops them (the
-  // all-silent recording's one range lies there); until then the window holds everything from sample 0
-  if (head == 0) {
-    st->head_len = 0;
-  } else if (st->head_len == 0 && keep > st->wave.first) {
-    SOME_REQUIRE(st->wave.first == 0 && st->wave.len >= head, "stream: samples [0, %lld) are no longer resident",
-                 (long long)head);
-    if (st->head_d.ensure(4ull * head, "the stream's leading samples")) return -1;
-    SOME_CUDA(cudaMemcpyAsync(st->head_d.p, st->wave.at(0), 4ull * head, cudaMemcpyDeviceToDevice, s->stream), "head copy");
-    st->head_len = head;
+  std::vector<some_resample_window> rs;
+  std::vector<some_rms_window> rm;
+  std::vector<ScatterParams> sc;
+  int64_t up_floats = 0, frames = 0;
+  for (StepItem& it : items) {
+    some_stream* st = it.st;
+    const some_slicer_frames& f = st->f;
+    long long keep_from, head;
+    if (some_slicer_stream_keep_from(st->slicer, &keep_from, &head, nullptr)) return -1;
+    // the model-rate samples a later chunk or RMS frame can still read
+    const int64_t keep = std::max<int64_t>(0, std::min<int64_t>(keep_from, st->frames * f.hop_size - f.win_size / 2));
+    // during a long leading silence (head > 0), the first max_sil_kept frames go apart before the window drops them (the
+    // all-silent recording's one range lies there); until then the window holds everything from sample 0
+    if (head == 0) {
+      st->head_len = 0;
+    } else if (st->head_len == 0 && keep > st->wave.first) {
+      SOME_REQUIRE(st->wave.first == 0 && st->wave.len >= head, "stream: samples [0, %lld) are no longer resident",
+                   (long long)head);
+      if (st->head_d.ensure(4ull * head, "the stream's leading samples")) return -1;
+      SOME_CUDA(cudaMemcpyAsync(st->head_d.p, st->wave.at(0), 4ull * head, cudaMemcpyDeviceToDevice, s->stream), "head copy");
+      st->head_len = head;
+    }
+    float* dst;
+    if (st->resample) {
+      long long t_end, x_first;
+      const double* table = table_for(s, st->rate);
+      if (!table) return -1;
+      if (some_resample_window_plan(st->received, 0, st->fixed, st->rate, sr, kKaiserTaps, &t_end, &x_first)) return -1;
+      if (st->native.reserve(s->stream, x_first, it.n, "the stream's input")) return -1;
+      dst = st->native.at(st->received);
+      st->native.len += it.n, st->received += it.n;
+      if (some_resample_window_plan(st->received, it.final, st->fixed, st->rate, sr, kKaiserTaps, &t_end, &x_first)) return -1;
+      if (st->wave.reserve(s->stream, keep, t_end - st->fixed, "the stream's audio")) return -1;
+      rs.push_back({st->native.at(st->native.first), st->native.first, st->received, it.final, st->wave.at(st->wave.first),
+                    st->wave.first, st->fixed, t_end, st->rate, sr, table, kKaiserTaps});
+      st->wave.len += t_end - st->fixed, st->fixed = t_end;
+    } else {
+      if (st->wave.reserve(s->stream, keep, it.n, "the stream's audio")) return -1;
+      dst = st->wave.at(st->received);
+      st->wave.len += it.n, st->received += it.n, st->fixed = st->received;
+    }
+    if (it.n) {
+      it.up = up_floats;
+      up_floats += (it.n + 3) & ~int64_t(3);         // 16-byte aligned
+      sc.push_back({nullptr, dst, it.n});
+    }
+    // the RMS frames the fixed samples complete (at the end: all of them, unless the recording is one chunk anyway)
+    const int64_t hop = f.hop_size;
+    int64_t f_end = frames_within(f, st->fixed);
+    if (it.final && (st->fixed + hop - 1) / hop > f.min_length) f_end = 1 + (st->fixed + 2 * (f.win_size / 2) - f.win_size) / hop;
+    it.nf = std::max<int64_t>(0, f_end - st->frames);
+    it.rms0 = frames;
+    if (it.nf) {
+      rm.push_back({st->wave.at(st->wave.first), st->wave.first, st->wave.len, it.final ? st->fixed : -1, f.win_size,
+                    f.hop_size, nullptr, st->frames, st->frames + it.nf});
+      frames += it.nf;
+    }
   }
-  const float* staged = static_cast<const float*>(st->stage_h.p);
-  if (st->resample) {
-    long long t_end, x_first;
-    if (ensure_table(s, st->rate)) return -1;
-    if (some_resample_window_plan(st->received, 0, st->fixed, st->rate, sr, kKaiserTaps, &t_end, &x_first)) return -1;
-    if (st->native.reserve(s->stream, x_first, n, "the stream's input")) return -1;
-    if (n) SOME_CUDA(cudaMemcpyAsync(st->native.at(st->received), staged, 4ull * n, cudaMemcpyHostToDevice, s->stream), "upload");
-    st->native.len += n, st->received += n;
-    if (some_resample_window_plan(st->received, final, st->fixed, st->rate, sr, kKaiserTaps, &t_end, &x_first)) return -1;
-    if (st->wave.reserve(s->stream, keep, t_end - st->fixed, "the stream's audio")) return -1;
-    if (some_resample_kaiser_window(st->native.at(st->native.first), st->native.first, st->received, final,
-                                    st->wave.at(st->wave.first), st->wave.first, st->fixed, t_end, st->rate, sr,
-                                    static_cast<const double*>(s->table_d.p), kKaiserTaps, s->stream))
-      return -1;
-    st->wave.len += t_end - st->fixed, st->fixed = t_end;
-  } else {
-    if (st->wave.reserve(s->stream, keep, n, "the stream's audio")) return -1;
-    if (n) SOME_CUDA(cudaMemcpyAsync(st->wave.at(st->received), staged, 4ull * n, cudaMemcpyHostToDevice, s->stream), "upload");
-    st->wave.len += n, st->received += n, st->fixed = st->received;
-  }
-  // the RMS frames the fixed samples complete (at the end: all of them, unless the recording is one chunk anyway)
-  const int64_t hop = f.hop_size;
-  int64_t f_end = frames_within(f, st->fixed);
-  if (final && (st->fixed + hop - 1) / hop > f.min_length) f_end = 1 + (st->fixed + 2 * (f.win_size / 2) - f.win_size) / hop;
-  const int64_t nf = std::max<int64_t>(0, f_end - st->frames);
-  if (nf) {
-    if (st->rms_d.ensure(4ull * nf, "the RMS frames") || st->rms_h.ensure(4ull * nf, "the RMS frames")) return -1;
-    if (some_slicer_rms_window(st->wave.at(st->wave.first), st->wave.first, st->wave.len, final ? st->fixed : -1, f.win_size,
-                               hop, static_cast<float*>(st->rms_d.p), st->frames, st->frames + nf, s->stream))
-      return -1;
-    SOME_CUDA(cudaMemcpyAsync(st->rms_h.p, st->rms_d.p, 4ull * nf, cudaMemcpyDeviceToHost, s->stream), "RMS download");
-  }
-  SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");   // also frees the staging buffer for the next push
-  st->frames += nf;
-  const float* rms = static_cast<const float*>(st->rms_h.p);
-  const int64_t* ranges = nullptr;
-  int B = 0;
-  if (final ? some_slicer_stream_finish(st->slicer, rms, static_cast<int>(nf), st->fixed, &ranges, &B)
-            : some_slicer_stream_feed(st->slicer, rms, static_cast<int>(nf), st->fixed, &ranges, &B))
+
+  // the upload: samples, then the scatter, resampling and RMS descriptors
+  const int ks = static_cast<int>(sc.size()), kr = static_cast<int>(rs.size()), km = static_cast<int>(rm.size());
+  const size_t sc_off = 4ull * up_floats;
+  const size_t rs_off = sc_off + align16(windows_bytes<ScatterParams>(ks));
+  const size_t rm_off = rs_off + align16(static_cast<size_t>(some_resample_windows_bytes(kr)));
+  const size_t bytes = rm_off + align16(static_cast<size_t>(some_slicer_rms_windows_bytes(km)));
+  if (s->step_h.ensure(bytes, "the stream upload") || s->step_d.ensure(bytes, "the stream upload") ||
+      s->rms_d.ensure(4ull * frames + 16, "the RMS frames") || s->rms_h.ensure(4ull * frames + 16, "the RMS frames"))
     return -1;
-  if (B == 0) {
-    out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
-    return 0;
+  char* up_h = static_cast<char*>(s->step_h.p);
+  char* up_d = static_cast<char*>(s->step_d.p);
+  {
+    ScatterParams* ps = windows_params<ScatterParams>(up_h + sc_off, ks);
+    long long* tile0 = windows_tile0(up_h + sc_off);
+    int j = 0;
+    for (const StepItem& it : items)
+      if (it.n) {
+        ps[j] = sc[j];
+        ps[j].src = reinterpret_cast<const float*>(up_d) + it.up;
+        tile0[j + 1] = (it.n + kScatterTile - 1) / kScatterTile;
+        ++j;
+      }
+    windows_index(up_h + sc_off, ks, 0);
   }
-  if (ranges[0] < st->wave.first) {                            // the all-silent recording's range, from the samples kept apart
-    SOME_REQUIRE(B == 1 && ranges[0] == 0 && ranges[1] <= st->head_len, "stream: chunk [%lld, %lld) is not resident",
-                 (long long)ranges[0], (long long)ranges[1]);
-    const int64_t start = 0, len = ranges[1];
-    return run_batch(s, nullptr, static_cast<const float*>(st->head_d.p), &start, &len, 1, out);
+  for (int j = 0, at = 0; j < km; at += static_cast<int>(rm[j].f_end - rm[j].f_begin), ++j)   // in item order, as rms0
+    rm[j].rms = static_cast<float*>(s->rms_d.p) + at;
+  if (some_resample_windows_pack(rs.data(), kr, up_h + rs_off) || some_slicer_rms_windows_pack(rm.data(), km, up_h + rm_off))
+    return -1;
+  {                                                // the samples, copied by the session's threads in pieces of up to 1 MB
+    constexpr int64_t kPiece = int64_t(1) << 18;
+    std::vector<std::pair<const StepItem*, int64_t>> pieces;
+    for (const StepItem& it : items)
+      for (int64_t a = 0; a < it.n; a += kPiece) pieces.push_back({&it, a});
+    const int nt = static_cast<int>(std::min<int64_t>(s->pool->size(), (up_floats + kPiece - 1) / kPiece));
+    float* dst = reinterpret_cast<float*>(up_h);
+    s->pool->run(nt, [&](int t) {
+      for (size_t j = t; j < pieces.size(); j += nt) {
+        const StepItem& it = *pieces[j].first;
+        const int64_t a = pieces[j].second;
+        memcpy(dst + it.up + a, it.samples + a, 4ull * std::min(kPiece, it.n - a));
+      }
+    });
   }
-  // the chunks, where they lie in the stream's buffer
-  std::vector<int64_t> starts(B), lens(B);
-  for (int i = 0; i < B; ++i) {
-    SOME_REQUIRE(ranges[2 * i] >= st->wave.first && ranges[2 * i + 1] <= st->wave.first + st->wave.len,
-                 "stream: chunk [%lld, %lld) is not resident ([%lld, %lld))", (long long)ranges[2 * i],
-                 (long long)ranges[2 * i + 1], (long long)st->wave.first, (long long)(st->wave.first + st->wave.len));
-    starts[i] = ranges[2 * i] - st->wave.first, lens[i] = std::max<int64_t>(0, ranges[2 * i + 1] - ranges[2 * i]);
+  SOME_CUDA(cudaMemcpyAsync(up_d, up_h, bytes, cudaMemcpyHostToDevice, s->stream), "stream upload");
+  if (ks) {
+    const WindowsHeader& h = *reinterpret_cast<const WindowsHeader*>(up_h + sc_off);
+    scatter_kernel<<<static_cast<unsigned>(h.tiles), kScatterThreads, 0, s->stream>>>(
+        windows_params<ScatterParams>(up_d + sc_off, ks), windows_tile0(up_d + sc_off), ks);
+    if (check_launch("stream upload scatter")) return -1;
   }
-  if (run_batch(s, nullptr, st->wave.at(st->wave.first), starts.data(), lens.data(), B, out)) return -1;
-  for (int64_t& r : out->range) r += st->wave.first;
+  if (some_resample_kaiser_windows(up_h + rs_off, up_d + rs_off, s->stream) ||
+      some_slicer_rms_windows(up_h + rm_off, up_d + rm_off, s->stream))
+    return -1;
+  if (frames)
+    SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames, cudaMemcpyDeviceToHost, s->stream), "RMS download");
+  SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");   // also frees the upload buffer for the next step
+
+  // the slicer's decisions, and where each chunk that became final lies
+  std::vector<const float*> src;
+  std::vector<int64_t> begin, lens;
+  for (StepItem& it : items) {
+    some_stream* st = it.st;
+    st->frames += it.nf;
+    const float* rms = static_cast<const float*>(s->rms_h.p) + it.rms0;
+    const int64_t* ranges = nullptr;
+    int B = 0;
+    if (it.final ? some_slicer_stream_finish(st->slicer, rms, static_cast<int>(it.nf), st->fixed, &ranges, &B)
+                 : some_slicer_stream_feed(st->slicer, rms, static_cast<int>(it.nf), st->fixed, &ranges, &B))
+      return -1;
+    it.c0 = static_cast<int>(begin.size());
+    if (B && ranges[0] < st->wave.first) {          // the all-silent recording's range, from the samples kept apart
+      SOME_REQUIRE(B == 1 && ranges[0] == 0 && ranges[1] <= st->head_len, "stream: chunk [%lld, %lld) is not resident",
+                   (long long)ranges[0], (long long)ranges[1]);
+      src.push_back(static_cast<const float*>(st->head_d.p)), begin.push_back(0), lens.push_back(ranges[1]);
+    } else {
+      for (int i = 0; i < B; ++i) {
+        SOME_REQUIRE(ranges[2 * i] >= st->wave.first && ranges[2 * i + 1] <= st->wave.first + st->wave.len,
+                     "stream: chunk [%lld, %lld) is not resident ([%lld, %lld))", (long long)ranges[2 * i],
+                     (long long)ranges[2 * i + 1], (long long)st->wave.first, (long long)(st->wave.first + st->wave.len));
+        src.push_back(st->wave.at(ranges[2 * i]));
+        begin.push_back(ranges[2 * i]), lens.push_back(std::max<int64_t>(0, ranges[2 * i + 1] - ranges[2 * i]));
+      }
+    }
+    it.c1 = static_cast<int>(begin.size());
+  }
+  const int B = static_cast<int>(begin.size());
+  if (B) {                                          // the chunks side by side in the audio buffer, then one batch
+    std::vector<int64_t> starts(B);
+    int64_t total = 0;
+    for (int c = 0; c < B; ++c) starts[c] = total, total += (lens[c] + 3) & ~int64_t(3);
+    if (s->wave_d.ensure(4ull * total + 16, "the audio")) return -1;
+    float* wave = static_cast<float*>(s->wave_d.p);
+    for (int c = 0; c < B; ++c)
+      if (lens[c])
+        SOME_CUDA(cudaMemcpyAsync(wave + starts[c], src[c], 4ull * lens[c], cudaMemcpyDeviceToDevice, s->stream), "chunk copy");
+    if (run_batch(s, nullptr, wave, starts.data(), lens.data(), B, &s->chunks)) return -1;
+  }
+  // each stream's notes, with its chunks' ranges
+  const some_notes& all = s->chunks;
+  for (const StepItem& it : items) {
+    some_notes* out = it.out;
+    clear(out);
+    for (int c = it.c0; c < it.c1; ++c) {
+      const int64_t a = all.first[c], b = all.first[c + 1];
+      out->midi.insert(out->midi.end(), all.midi.begin() + a, all.midi.begin() + b);
+      out->dur.insert(out->dur.end(), all.dur.begin() + a, all.dur.begin() + b);
+      out->rest.insert(out->rest.end(), all.rest.begin() + a, all.rest.begin() + b);
+      out->first.push_back(out->first.back() + (b - a));
+      out->range.push_back(begin[c]), out->range.push_back(begin[c] + lens[c]);
+    }
+  }
   return 0;
 }
 
-// Takes the stream's samples into its pinned staging buffer (no lock: the buffer is the stream's own, and the previous step
-// ended with a synchronise), then runs one step under the session's mutex.
+// A step of one stream (some_stream_push, some_stream_finish).
 int stream_call(some_stream* st, const float* samples, int64_t n, bool final, some_notes* out) {
   some_session* s = st->s;
   DeviceScope scope(s->device);
   SOME_CUDA(scope.err, "cudaSetDevice");
-  if (st->stage_h.ensure(4ull * n + 16, "the staged audio")) return -1;
-  if (n) memcpy(st->stage_h.p, samples, 4ull * n);
+  std::vector<StepItem> items{StepItem{st, samples, n, final, out}};
   std::lock_guard<std::mutex> lock(s->mu);
-  return settle(s, stream_step(st, n, final, out));
+  return settle(s, streams_step(s, items));
 }
 }  // namespace
 
@@ -988,6 +1127,45 @@ extern "C" int some_stream_finish(some_stream* st, some_notes* out) {
                st->rate, sr);
   st->finished = true;
   return stream_call(st, nullptr, 0, true, out);
+}
+
+extern "C" int some_stream_push_many(some_stream* const* streams, const float* const* samples, const long long* n,
+                                     const int* finish, int count, some_notes* const* out) {
+  SOME_REQUIRE(streams != nullptr && samples != nullptr && n != nullptr && out != nullptr && count >= 0,
+               "some_stream_push_many: bad arguments");
+  if (count == 0) return 0;
+  // every argument is checked before any stream changes
+  some_session* s = streams[0] ? streams[0]->s : nullptr;
+  std::map<const void*, int> seen, seen_notes;
+  for (int i = 0; i < count; ++i) {
+    const some_stream* st = streams[i];
+    SOME_REQUIRE(st != nullptr, "some_stream_push_many: stream %d is NULL", i);
+    SOME_REQUIRE(st->s == s, "some_stream_push_many: stream %d belongs to another session than stream 0", i);
+    const auto dup = seen.emplace(st, i);
+    SOME_REQUIRE(dup.second, "some_stream_push_many: stream %d appears twice (also at %d)", i, dup.first->second);
+    SOME_REQUIRE(!st->finished, "some_stream_push_many: stream %d has finished", i);
+    SOME_REQUIRE(n[i] >= 0 && (n[i] == 0 || samples[i] != nullptr), "some_stream_push_many: stream %d: %lld samples at %p", i,
+                 n[i], static_cast<const void*>(samples[i]));
+    SOME_REQUIRE(out[i] != nullptr, "some_stream_push_many: stream %d: NULL notes", i);
+    const auto shared = seen_notes.emplace(out[i], i);
+    SOME_REQUIRE(shared.second, "some_stream_push_many: stream %d shares its some_notes with stream %d", i,
+                 shared.first->second);
+    const int sr = s->info.sample_rate;
+    SOME_REQUIRE(!(finish && finish[i]) || !st->resample || (st->received + n[i]) * sr / st->rate >= 1,
+                 "some_stream_push_many: stream %d: Input signal length=%lld is too small to resample from %d->%d", i,
+                 (long long)(st->received + n[i]), st->rate, sr);
+  }
+  std::vector<StepItem> items;
+  items.reserve(count);
+  for (int i = 0; i < count; ++i) {
+    const bool final = finish && finish[i];
+    if (final) streams[i]->finished = true;
+    items.push_back(StepItem{streams[i], samples[i], n[i], final, out[i]});
+  }
+  DeviceScope scope(s->device);
+  SOME_CUDA(scope.err, "cudaSetDevice");
+  std::lock_guard<std::mutex> lock(s->mu);
+  return settle(s, streams_step(s, items));
 }
 
 extern "C" int some_stream_get_info(const some_stream* st, some_stream_info* info) {

@@ -61,14 +61,11 @@ __device__ __forceinline__ float rms_block(const RmsWindow& w, int lo, int n) {
 
 constexpr int RMS_MAX_DEPTH = 24;  // frame_length < 128 * 2^24
 
-// Frames [f_begin, f_begin + n_frames) into rms[0, n_frames): a frame's value depends on its absolute index and the samples
-// alone, so a window of frames over a buffer holding part of the recording gives the whole-recording bits.
-__global__ void __launch_bounds__(128) slicer_rms_kernel(const float* __restrict__ wave, long long base, long long n_samples,
-                                                         int frame_length, int hop, float* __restrict__ rms, long long f_begin,
-                                                         int n_frames) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_frames) return;
-  const long long f = f_begin + i;
+// Frame f of a recording of n_samples samples, wave[s - base] being sample s: its value depends on its absolute index and the
+// samples alone, so a window of frames over a buffer holding part of the recording gives the whole-recording bits.  Not
+// inlined: inlined into the kernels, ptxas unrolled the block sums less (29 global loads instead of 53).
+__device__ __noinline__ float rms_frame(const float* __restrict__ wave, long long base, long long n_samples, int frame_length,
+                                        int hop, long long f) {
   RmsWindow w{wave, base, n_samples, f * hop - frame_length / 2};
   float total;
   if (frame_length < 8) {
@@ -107,7 +104,37 @@ __global__ void __launch_bounds__(128) slicer_rms_kernel(const float* __restrict
     }
     total = ret;
   }
-  rms[i] = __fsqrt_rn(__fdiv_rn(total, static_cast<float>(frame_length)));
+  return __fsqrt_rn(__fdiv_rn(total, static_cast<float>(frame_length)));
+}
+
+// Frames [f_begin, f_begin + n_frames) into rms[0, n_frames).
+__global__ void __launch_bounds__(128) slicer_rms_kernel(const float* __restrict__ wave, long long base, long long n_samples,
+                                                         int frame_length, int hop, float* __restrict__ rms, long long f_begin,
+                                                         int n_frames) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_frames) return;
+  rms[i] = rms_frame(wave, base, n_samples, frame_length, hop, f_begin + i);
+}
+
+// One frame window of the many-window launch: the arguments of slicer_rms_kernel.
+struct RmsParams {
+  const float* wave;
+  long long base, n_samples;
+  float* rms;
+  long long f_begin;
+  int frame_length, hop, n_frames, pad;
+};
+constexpr int RMS_TILE = 128;   // frames per CTA, one thread each
+
+// K frame windows in one grid: the windows' tiles of RMS_TILE frames laid end to end.
+__global__ void __launch_bounds__(RMS_TILE) slicer_rms_windows_kernel(const RmsParams* __restrict__ ps,
+                                                                      const long long* __restrict__ tile0, int K) {
+  const long long tile = blockIdx.x;
+  const int w = window_of(tile0, K, tile);
+  const RmsParams& p = ps[w];
+  const int i = static_cast<int>(tile - tile0[w]) * RMS_TILE + threadIdx.x;
+  if (i >= p.n_frames) return;
+  p.rms[i] = rms_frame(p.wave, p.base, p.n_samples, p.frame_length, p.hop, p.f_begin + i);
 }
 
 }  // namespace some
@@ -127,30 +154,72 @@ extern "C" int some_slicer_rms(const float* wave, long long n_samples, int frame
   return check_launch("some_slicer_rms");
 }
 
-extern "C" int some_slicer_rms_window(const float* wave, long long base, long long held, long long n_samples, int frame_length,
-                                      int hop, float* rms, long long f_begin, long long f_end, cudaStream_t stream) {
-  SOME_REQUIRE(wave && rms, "some_slicer_rms_window: null pointer");
-  SOME_REQUIRE(base >= 0 && held >= 0 && n_samples >= -1 && frame_length >= 1 && hop >= 1 && f_begin >= 0 && f_end >= f_begin &&
-                   f_end - f_begin < (1ll << 31),
-               "some_slicer_rms_window: bad sizes");
-  if (f_end == f_begin) return 0;
-  const long long half = frame_length / 2;
-  const bool final = n_samples >= 0;
+namespace {
+// The kernel arguments of one frame window, with the checks of some_slicer_rms_window: the buffer must hold every sample
+// inside the recording the frames read.
+int rms_window_params(const some_rms_window& w, const char* what, RmsParams& p) {
+  SOME_REQUIRE(w.wave && w.rms, "%s: null pointer", what);
+  SOME_REQUIRE(w.base >= 0 && w.held >= 0 && w.n_samples >= -1 && w.frame_length >= 1 && w.hop >= 1 && w.f_begin >= 0 &&
+                   w.f_end >= w.f_begin && w.f_end - w.f_begin < (1ll << 31),
+               "%s: bad sizes", what);
+  p = RmsParams{w.wave, w.base, 0, w.rms, w.f_begin, w.frame_length, w.hop, static_cast<int>(w.f_end - w.f_begin), 0};
+  if (w.f_end == w.f_begin) return 0;
+  const long long half = w.frame_length / 2;
+  const bool final = w.n_samples >= 0;
   if (final) {
-    const long long padded = n_samples + 2 * half;
-    SOME_REQUIRE(padded >= frame_length && f_end <= 1 + (padded - frame_length) / hop,
-                 "some_slicer_rms_window: frame %lld is past the last frame of %lld samples", f_end - 1, n_samples);
+    const long long padded = w.n_samples + 2 * half;
+    SOME_REQUIRE(padded >= w.frame_length && w.f_end <= 1 + (padded - w.frame_length) / w.hop,
+                 "%s: frame %lld is past the last frame of %lld samples", what, w.f_end - 1, w.n_samples);
   }
   // the samples the frames read that lie inside the recording: the buffer must hold them
-  const long long lo = std::max(0ll, f_begin * hop - half);
-  const long long hi = (f_end - 1) * hop - half + frame_length;
-  const long long hi_in = final ? std::min(hi, n_samples) : hi;
-  SOME_REQUIRE(lo >= base && hi_in <= base + held,
-               "some_slicer_rms_window: frames [%lld, %lld) read samples [%lld, %lld), the buffer holds [%lld, %lld)%s", f_begin,
-               f_end, lo, hi_in, base, base + held, final ? "" : " (the recording's length is not known yet)");
-  slicer_rms_kernel<<<static_cast<unsigned>((f_end - f_begin + 127) / 128), 128, 0, stream>>>(
-      wave, base, final ? n_samples : base + held, frame_length, hop, rms, f_begin, static_cast<int>(f_end - f_begin));
+  const long long lo = std::max(0ll, w.f_begin * w.hop - half);
+  const long long hi = (w.f_end - 1) * w.hop - half + w.frame_length;
+  const long long hi_in = final ? std::min(hi, w.n_samples) : hi;
+  SOME_REQUIRE(lo >= w.base && hi_in <= w.base + w.held,
+               "%s: frames [%lld, %lld) read samples [%lld, %lld), the buffer holds [%lld, %lld)%s", what, w.f_begin, w.f_end, lo,
+               hi_in, w.base, w.base + w.held, final ? "" : " (the recording's length is not known yet)");
+  p.n_samples = final ? w.n_samples : w.base + w.held;
+  return 0;
+}
+}  // namespace
+
+extern "C" int some_slicer_rms_window(const float* wave, long long base, long long held, long long n_samples, int frame_length,
+                                      int hop, float* rms, long long f_begin, long long f_end, cudaStream_t stream) {
+  RmsParams p;
+  if (rms_window_params({wave, base, held, n_samples, frame_length, hop, rms, f_begin, f_end}, "some_slicer_rms_window", p))
+    return -1;
+  if (p.n_frames == 0) return 0;
+  slicer_rms_kernel<<<static_cast<unsigned>((p.n_frames + 127) / 128), 128, 0, stream>>>(
+      p.wave, p.base, p.n_samples, p.frame_length, p.hop, p.rms, p.f_begin, p.n_frames);
   return check_launch("some_slicer_rms_window");
+}
+
+extern "C" long long some_slicer_rms_windows_bytes(int K) { return K < 0 ? -1 : static_cast<long long>(windows_bytes<RmsParams>(K)); }
+
+extern "C" int some_slicer_rms_windows_pack(const some_rms_window* w, int K, void* desc) {
+  SOME_REQUIRE(desc && K >= 0 && (K == 0 || w), "some_slicer_rms_windows_pack: bad arguments");
+  char what[64];
+  RmsParams* ps = windows_params<RmsParams>(desc, K);
+  long long* tile0 = windows_tile0(desc);
+  for (int i = 0; i < K; ++i) {
+    snprintf(what, sizeof(what), "some_slicer_rms_windows_pack: window %d", i);
+    if (rms_window_params(w[i], what, ps[i])) return -1;
+    tile0[i + 1] = (ps[i].n_frames + RMS_TILE - 1) / RMS_TILE;
+  }
+  windows_index(desc, K, 0);
+  SOME_REQUIRE(windows_tile0(desc)[K] < (1ll << 31), "some_slicer_rms_windows_pack: grid too large");
+  return 0;
+}
+
+extern "C" int some_slicer_rms_windows(const void* desc, const void* desc_d, cudaStream_t stream) {
+  SOME_REQUIRE(desc && desc_d && reinterpret_cast<uintptr_t>(desc_d) % 16 == 0, "some_slicer_rms_windows: bad arguments");
+  const WindowsHeader& h = *static_cast<const WindowsHeader*>(desc);
+  if (h.tiles == 0) return 0;
+  const int K = static_cast<int>(h.K);
+  void* d = const_cast<void*>(desc_d);
+  slicer_rms_windows_kernel<<<static_cast<unsigned>(h.tiles), RMS_TILE, 0, stream>>>(windows_params<RmsParams>(d, K),
+                                                                                     windows_tile0(d), K);
+  return check_launch("some_slicer_rms_windows");
 }
 
 // ---------------------------------------------------------------------------------------------------- slicer decisions

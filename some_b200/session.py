@@ -122,6 +122,23 @@ class Session:
         """some_stream_open: a recording pushed while it arrives (see Stream)."""
         return Stream(self, sample_rate, params)
 
+    def push_many(self, items: Sequence[Tuple['Stream', np.ndarray]], finish: Optional[Sequence[bool]] = None):
+        """some_stream_push_many: pushes samples to many streams of this session in one step, and finishes those with a true
+        entry in `finish`.  Returns one (offsets, ranges, notes) per item, what Stream.push (then Stream.finish) would return;
+        each stream's results go through its own Notes."""
+        k = len(items)
+        xs = [np.ascontiguousarray(x, dtype=np.float32) for _, x in items]
+        streams = (C.c_void_p * max(k, 1))(*[st.handle for st, _ in items])
+        ptrs = (C.c_void_p * max(k, 1))(*[x.ctypes.data for x in xs])
+        lens = np.array([x.shape[0] for x in xs] or [0], dtype=np.int64)
+        outs = (C.c_void_p * max(k, 1))(*[st.notes.handle for st, _ in items])
+        fin = None if finish is None else np.array([bool(f) for f in finish] or [0], dtype=np.int32)
+        if fin is not None and len(finish) != k:
+            raise ValueError(f'push_many: {k} items, {len(finish)} finish flags')
+        _lib.check(self.lib.some_stream_push_many(streams, ptrs, lens.ctypes.data, None if fin is None else fin.ctypes.data, k,
+                                                  outs), 'some_stream_push_many')
+        return [st._results() for st, _ in items]
+
 
 class Stream:
     """some_stream_*: push samples as they arrive; push() and finish() return the chunks that became final, in the shape
