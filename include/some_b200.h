@@ -18,6 +18,7 @@
 #ifndef SOME_B200_H_
 #define SOME_B200_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -385,6 +386,73 @@ int some_flac_scan(const uint8_t* data, long long n_bytes, const some_flac_strea
 int some_flac_decode(const uint8_t* data, const some_flac_stream* streams, const some_flac_frame* frames, const int32_t* chain,
                      const int64_t* scratch_off, const int64_t* out_off, int n_chain, int32_t* scratch, float* out, int mono,
                      int* status, cudaStream_t stream);
+/* some_flac_chain (host, no CUDA call): the frames a sequential decoder walks, from the candidate list of some_flac_scan
+ * (frames[0 .. n_frames), in byte order, downloaded to the host).  Recording r starts its walk at recs[r].audio_start; each
+ * next frame starts where the current one ends and carries the next frame number (fixed blocking) or sample number (variable
+ * blocking); the walk stops after recs[r].length samples (STREAMINFO; 0 = not stated: at recs[r].end).  Byte offsets in the
+ * messages are counted from recs[r].base (the first byte of the recording's file in `data`).  Writes the chained indices of
+ * recording r to chain[first[r] .. first[r + 1]) (first: [n_recs + 1]; capacity n_frames always suffices) and its decoded
+ * length to lengths[r].  Refused, with *failed = r and a message that names no file, when a header is missing where a frame
+ * must start, a chained frame's status is not SOME_FLAC_OK, a frame or sample number leaves a gap or overlaps or the blocking
+ * strategy changes, a frame decodes past the STREAMINFO length, or the recording ends early. */
+typedef struct {
+  int64_t base, audio_start, end, length;
+} some_flac_range;
+int some_flac_chain(const some_flac_frame* frames, int n_frames, const some_flac_range* recs, int n_recs, int32_t* chain,
+                    int capacity, int64_t* first, int64_t* lengths, int* failed);
+
+/* ---- Container metadata on the host (csrc/audio_host.cu, no CUDA call): what some_b200.audio.load accepts, but for one
+ * kind of file: integer PCM in 5-8 byte containers, which scipy reads as int64 and audio.decode_wav scales by 2^-63, is
+ * refused here (and with it 1-8 bit PCM in containers wider than one byte, which scipy misreads).
+ * some_audio_info  RIFF/WAVE as scipy.io.wavfile.read walks it (fmt tag 1: PCM in 1, 2, 3 or 4 byte containers; tag 3: float32
+ *                  or float64; tag 0xFFFE with a PCM or float subformat; any number of channels; other chunks skipped with
+ *                  their pad byte; a data chunk cut short by the end of the file yields the whole frames present), or fLaC,
+ *                  optionally behind an ID3v2 tag, with the metadata-block rules of audio.parse_flac (up to 24 bits per
+ *                  sample).  Refused with audio.decode_wav's / audio.parse_flac's reason (scipy's text for the WAV walk)
+ *                  and the byte offset: other containers (Ogg, MP3, AIFF, RIFX, RF64, CAF, AU) by name, truncated or
+ *                  missing chunks, unsupported tags or sample sizes, a bad STREAMINFO. */
+enum { SOME_AUDIO_WAV = 1, SOME_AUDIO_FLAC = 2 };
+enum { SOME_PCM_U8 = 1, SOME_PCM_S16 = 2, SOME_PCM_S24 = 3, SOME_PCM_S32 = 4, SOME_PCM_F32 = 5, SOME_PCM_F64 = 6 };
+typedef struct {
+  int container;                 /* SOME_AUDIO_* */
+  int rate, channels, bits;      /* bits: the fmt chunk's bits per sample / STREAMINFO's */
+  int kind;                      /* WAV: SOME_PCM_* (the sample container); FLAC: 0 */
+  int min_blocksize, max_blocksize;   /* FLAC STREAMINFO; WAV: 0 */
+  int reserved;
+  long long frames;              /* samples per channel (FLAC: STREAMINFO's, 0 = not stated) */
+  long long data_offset;         /* WAV: first sample byte; FLAC: first frame byte (after the metadata blocks) */
+  long long data_bytes;          /* WAV: frames * channels * sample bytes; FLAC: to the end of the data */
+} some_audio_meta;
+int some_audio_info(const void* data, long long n_bytes, some_audio_meta* out);
+
+/* ---- K-pcm: the samples of RIFF/WAVE data chunks as audio.decode_wav hands them to librosa.load, many recordings in one
+ * launch.  u8 -> (x - 128) / 128, s16 / s24 / s32 -> x / 2^(bits - 1) (s32 rounded to float32 first, as numpy's astype),
+ * f32 as is, f64 rounded to nearest float32.  Samples may start at any byte.  mono != 0: out[i] = np.mean's float32 order over
+ * librosa's (channels, n) view (channels added one after another below 8, numpy's 8-way pairwise sum from 8 to 128 channels,
+ * then / channels; the FLAC emitter uses the same function); mono == 0: interleaved out[i * channels + c].
+ * Packed and launched in two steps like some_slicer_rms_windows: some_pcm_decode_pack checks every item (the message names
+ * it; mono needs channels <= 128) and writes the descriptors to host memory of some_pcm_decode_bytes(K) bytes; some_pcm_decode
+ * launches from the host copy `desc` and its device copy `desc_d` (16-byte aligned). */
+typedef struct {
+  const uint8_t* data;           /* device: the first byte of the first sample */
+  long long frames;              /* samples per channel */
+  int channels, kind, mono, reserved;
+  float* out;                    /* device: frames floats (mono) or frames * channels */
+} some_pcm_item;
+long long some_pcm_decode_bytes(int K);
+int some_pcm_decode_pack(const some_pcm_item* items, int K, void* desc);
+int some_pcm_decode(const void* desc, const void* desc_d, cudaStream_t stream);
+
+/* ---- MIDI bytes (host, no CUDA call): the Standard MIDI File some_b200.midi.build_midi_file(offsets, segments,
+ * tempo).to_bytes() writes, with note_dur seconds = (double)note_dur * timestep.  Chunk c holds notes
+ * [sum counts[0 .. c), + counts[c]).  Ticks follow infer_utils.build_midi_file: offsets * tempo * 8 rounded half to even,
+ * each chunk's note ends from np.round of the float64 cumulative duration times tempo * 8, notes clipped at the next chunk's
+ * tick, rests and empty notes skipped.  *size = the bytes of the file; they are written only when capacity >= *size (buf may
+ * be NULL with capacity 0, to ask for the size).  Refused where Python raises (a note outside 0..127 after rounding, a negative
+ * delta time) and for a tempo whose round(60e6 / bpm) does not fit the 24 bits of set_tempo.
+ * some_notes_midi (below, with the session) does the same for a session's result. */
+int some_midi_write(int n_chunks, const double* offsets, const int32_t* counts, const float* note_midi, const int32_t* note_dur,
+                    const uint8_t* note_rest, double timestep, double tempo, uint8_t* buf, size_t capacity, size_t* size);
 
 /* ---- some_forward: the whole trunk Gmidi_conform.forward (Gconform.py:119-140) + head activation
  * (Gmidi_conform.py:30-40) as one call that enqueues the launch sequence above on `stream`.
@@ -613,6 +681,34 @@ int some_notes_destroy(some_notes* n);
 int some_notes_clips(const some_notes* n); /* number of clips / chunks (< 0: error) */
 int some_notes_get(const some_notes* n, int clip, int* count, const float** note_midi, const int32_t** note_dur,
                    const uint8_t** note_rest, int64_t* begin, int64_t* end); /* any output pointer may be NULL */
+/* some_midi_write over a result: chunk offsets begin / sample_rate seconds, as infer.py passes them to build_midi_file. */
+int some_notes_midi(const some_notes* n, int sample_rate, double timestep, double tempo, uint8_t* buf, size_t capacity,
+                    size_t* size);
+
+/* ---- Encoded files in, notes out: librosa.load(file, sr=None, mono=True) of WAV and FLAC files on the GPU, then the slicer
+ * and the model.  For item i, out[i] receives what some_session_transcribe_sliced(s, y, n, rate, params, out[i]) gives for
+ * y, rate = audio.load(file, sr=None, mono=True): the same chunk ranges (at the model's rate) and bit-identical notes.
+ * Results do not depend on the other items of the call.
+ *   One GPU step for all items: every item's audio bytes go up in one pinned copy; one some_flac_scan over the FLAC items,
+ * one download of its candidates and some_flac_chain on the host; one some_flac_decode and one some_pcm_decode into a
+ * native-rate buffer (items at the model's rate are decoded straight into the model-rate buffer); one
+ * some_resample_kaiser_windows launch for every item at another rate; one some_slicer_rms_windows launch, one download and
+ * one synchronise; the slicer on the host per item; one batch through the model for the chunks of all items.
+ *   Device memory held during the call (grow-only, kept by the session): the items' audio bytes, 4 bytes per FLAC sample and
+ * channel (the decoder's int32 scratch), 4 bytes per native-rate sample of the items at another rate, 4 bytes per model-rate
+ * sample of all items, plus the model's activations for the chunks; the caller bounds it by choosing `count`.  The same bytes
+ * are staged in pinned host memory.
+ *   Refused before any GPU work, with the index i in the message and no out[i] touched: NULL arrays or count < 0; a NULL or
+ * empty item; two entries sharing one some_notes; anything some_audio_info refuses; mono down-mix of more than 128 channels; a
+ * rate pair the resampler does not support; a recording too short to resample.  A corrupt FLAC stream is refused after the
+ * scan with its index and some_flac_chain's message, and no out[i] is written.  After a device error the session stays
+ * usable.  The call takes the session's mutex once; count == 0 does nothing.  params NULL: Slicer(sr, max_sil_kept=1000). */
+typedef struct {
+  const void* data;
+  long long n_bytes;
+} some_encoded;
+int some_session_transcribe_encoded(some_session* s, const some_encoded* items, int count, const some_slicer_params* params,
+                                    some_notes* const* out);
 /* The slicer's decisions on the HOST (no CUDA call): some_slicer_derive fills the frame counts for a sample rate (params NULL:
  * the session's defaults); some_slicer_ranges turns the RMS list of a recording of n_samples samples (some_slicer_rms) into the
  * [begin, end) sample ranges of its chunks, ranges[2 k], ranges[2 k + 1] (the cuts of Slicer.slice, utils/slicer2.py:82-145).

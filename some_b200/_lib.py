@@ -148,6 +148,28 @@ class RmsWindow(C.Structure):
                 ('f_end', C.c_longlong)]
 
 
+class FlacRange(C.Structure):
+    _fields_ = [('base', C.c_int64), ('audio_start', C.c_int64), ('end', C.c_int64), ('length', C.c_int64)]
+
+
+class AudioMeta(C.Structure):
+    _fields_ = [('container', C.c_int), ('rate', C.c_int), ('channels', C.c_int), ('bits', C.c_int), ('kind', C.c_int),
+                ('min_blocksize', C.c_int), ('max_blocksize', C.c_int), ('reserved', C.c_int), ('frames', C.c_longlong),
+                ('data_offset', C.c_longlong), ('data_bytes', C.c_longlong)]
+
+
+class PcmItem(C.Structure):
+    _fields_ = [('data', _vp), ('frames', C.c_longlong), ('channels', C.c_int), ('kind', C.c_int), ('mono', C.c_int),
+                ('reserved', C.c_int), ('out', _vp)]
+
+
+class Encoded(C.Structure):
+    _fields_ = [('data', _vp), ('n_bytes', C.c_longlong)]
+
+
+AUDIO_WAV, AUDIO_FLAC = 1, 2
+PCM_U8, PCM_S16, PCM_S24, PCM_S32, PCM_F32, PCM_F64 = range(1, 7)
+
 EXPORTS = {
     # name: (restype, argtypes)
     'some_version': (C.c_int, []),
@@ -187,6 +209,15 @@ EXPORTS = {
     'some_flac_scan_workspace_bytes': (C.c_uint64, [C.c_longlong]),
     'some_flac_scan': (C.c_int, [_vp, C.c_longlong, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp]),
     'some_flac_decode': (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp, C.c_int, _vp, _vp]),
+    'some_flac_chain': (C.c_int, [_vp, C.c_int, C.POINTER(FlacRange), C.c_int, _vp, C.c_int, _vp, _vp, C.POINTER(C.c_int)]),
+    'some_audio_info': (C.c_int, [_vp, C.c_longlong, C.POINTER(AudioMeta)]),
+    'some_pcm_decode_bytes': (C.c_longlong, [C.c_int]),
+    'some_pcm_decode_pack': (C.c_int, [C.POINTER(PcmItem), C.c_int, _vp]),
+    'some_pcm_decode': (C.c_int, [_vp, _vp, _vp]),
+    'some_midi_write': (C.c_int, [C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_double, C.c_double, _vp, C.c_size_t,
+                                  C.POINTER(C.c_size_t)]),
+    'some_notes_midi': (C.c_int, [_vp, C.c_int, C.c_double, C.c_double, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    'some_session_transcribe_encoded': (C.c_int, [_vp, C.POINTER(Encoded), C.c_int, C.POINTER(SlicerParams), _vp]),
     'some_row_stats': (C.c_int, [C.POINTER(RowStatsArgs), _vp]),
     'some_col_means': (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, _vp]),
     'some_forward': (C.c_int, [C.POINTER(ModelC), C.POINTER(WorkspaceC), C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp,

@@ -251,9 +251,6 @@ _STREAM_DTYPE = np.dtype([('audio_start', '<i8'), ('end', '<i8'), ('channels', '
                           ('max_blocksize', '<i4'), ('reserved', '<i4')])                       # some_flac_stream
 _FRAME_DTYPE = np.dtype([('pos', '<i8'), ('number', '<i8'), ('end', '<i8'), ('stream', '<i4'), ('blocksize', '<i4'),
                          ('header_len', '<i2'), ('chan_code', 'u1'), ('variable', 'u1'), ('status', '<i4')])  # some_flac_frame
-_FLAC_REASONS = {1: 'truncated frame', 2: 'CRC-16 mismatch', 3: 'non-zero padding bits', 4: 'reserved subframe type',
-                 5: 'invalid wasted-bits count', 6: 'predictor order larger than the block',
-                 7: 'invalid LPC precision or shift', 8: 'reserved residual coding method', 9: 'invalid partition order'}
 
 
 class FlacBatch:
@@ -300,42 +297,29 @@ class FlacBatch:
         self._chain(fr, bases)
 
     def _chain(self, fr, bases):
-        """Walks every recording from its first audio byte: each next frame starts where the current one ends and carries
-        the next frame number (fixed blocking) or sample number (variable blocking)."""
-        pos, end, status = fr['pos'].tolist(), fr['end'].tolist(), fr['status'].tolist()
-        number, variable, bs = fr['number'].tolist(), fr['variable'].tolist(), fr['blocksize'].tolist()
-        n = len(pos)
-        self.chains: List[np.ndarray] = []
-        self.lengths: List[int] = []
-        i = 0
+        """Walks every recording from its first audio byte (some_flac_chain, the walk the session uses too): each next frame
+        starts where the current one ends and carries the next frame number (fixed blocking) or sample number (variable
+        blocking)."""
+        from . import _lib
+        n, k = len(fr), len(self.records)
+        frames = np.ascontiguousarray(fr)
+        recs = (_lib.FlacRange * max(k, 1))()
         for r, rec in enumerate(self.records):
-            base, p, stop, total = int(bases[r]), int(bases[r]) + rec.audio_offset, int(bases[r + 1]), rec.length
-            chain, got, strategy = [], 0, None
-            while not (total and got == total) and not (not total and p == stop):
-                if p >= stop:
-                    raise ValueError(f'{rec.name}: FLAC stream ends at byte offset {p - base} after {got} of {total} samples')
-                while i < n and pos[i] < p:
-                    i += 1
-                if i >= n or pos[i] != p:
-                    raise ValueError(f'{rec.name}: no valid FLAC frame header (sync, reserved code, CRC-8 or STREAMINFO '
-                                     f'mismatch) at byte offset {p - base}')
-                if status[i]:
-                    raise ValueError(f'{rec.name}: FLAC frame at byte offset {p - base}: '
-                                     f'{_FLAC_REASONS.get(status[i], status[i])} (at byte offset {end[i] - base})')
-                strategy = variable[i] if strategy is None else strategy
-                want = got if variable[i] else len(chain)
-                if variable[i] != strategy or number[i] != want:
-                    raise ValueError(f'{rec.name}: FLAC frame at byte offset {p - base}: {"sample" if variable[i] else "frame"} '
-                                     f'number {number[i]}, expected {want} (gap, overlap or changed blocking strategy)')
-                got += bs[i]
-                if total and got > total:
-                    raise ValueError(f'{rec.name}: FLAC frame at byte offset {p - base} decodes past the {total} samples '
-                                     f'STREAMINFO states')
-                chain.append(i)
-                p = end[i]
-            self.chains.append(np.asarray(chain, dtype=np.int32))
-            self.lengths.append(got)
-        self._bs = np.asarray(bs, dtype=np.int64)
+            recs[r] = _lib.FlacRange(int(bases[r]), int(bases[r]) + rec.audio_offset, int(bases[r + 1]), rec.length)
+        chain = np.zeros(max(n, 1), np.int32)
+        first = np.zeros(k + 1, np.int64)
+        lengths = np.zeros(max(k, 1), np.int64)
+        failed = C.c_int(-1)
+        lib = _lib.load()
+        if lib.some_flac_chain(frames.ctypes.data if n else None, n, recs, k, chain.ctypes.data, n, first.ctypes.data,
+                               lengths.ctypes.data, C.byref(failed)):
+            msg = lib.some_last_error().decode('utf8', 'replace')
+            if failed.value < 0:
+                raise _lib.SomeB200Error(f'some_flac_chain failed: {msg}')
+            raise ValueError(f'{self.records[failed.value].name}: {msg}')
+        self.chains: List[np.ndarray] = [chain[first[r]:first[r + 1]].copy() for r in range(k)]
+        self.lengths: List[int] = [int(x) for x in lengths[:k]]
+        self._bs = fr['blocksize'].astype(np.int64)
 
     def emit(self, out, starts: Dict[int, int], mono: bool = True):
         """Decodes recording r into out[starts[r] : + lengths[r]] (mono: np.mean's float32 order over the channels, i.e.

@@ -20,13 +20,15 @@
 //   decode one thread per frame: subframes (CONSTANT, VERBATIM, FIXED 0-4, LPC 1-32, wasted bits), prediction with 64-bit
 //          sums, stereo decorrelation, into the frame's own int32 scratch slot [channels][blocksize].
 //   emit   one CTA per frame: x * 2^-(bps-1) (libsndfile's scaling, exact in float32 for bps <= 24), interleaved [n, ch] or
-//          mono in numpy's order for np.mean over librosa's (channels, n) view of an [n, ch] array: channels added one
-//          after another for 2-7 channels, the pairwise tree ((c0+c1)+(c2+c3))+((c4+c5)+(c6+c7)) for 8, then / channels.
+//          mono in numpy's order for np.mean over librosa's (channels, n) view of an [n, ch] array (mono_mean, downmix.cuh,
+//          shared with the PCM decoder): channels added one after another for 2-7 channels, the pairwise tree
+//          ((c0+c1)+(c2+c3))+((c4+c5)+(c6+c7)) for 8, then / channels.
 //
 // Every bit read is bounds-checked against the recording's byte range: reading past it yields zeros and marks the frame
 // truncated, so a malformed candidate can return a status but never read outside its recording or write anywhere.
 #include <stddef.h>
 
+#include "downmix.cuh"
 #include "host_common.h"
 
 #include "../../include/some_b200.h"
@@ -445,14 +447,17 @@ __global__ void __launch_bounds__(FL_FRAME_THREADS) flac_parse_kernel(const uint
 __global__ void __launch_bounds__(FL_FRAME_THREADS) flac_decode_kernel(const uint8_t* data, const some_flac_stream* streams,
                                                                        const some_flac_frame* frames, const int32_t* chain,
                                                                        const int64_t* scratch_off, int n_chain,
-                                                                       int32_t* scratch, int* status) {
+                                                                       int32_t* scratch, int* status, int* failed) {
   __shared__ int coef[32 * FL_FRAME_THREADS];                      // [j][thread]: conflict-free
   const int k = blockIdx.x * FL_FRAME_THREADS + threadIdx.x;
   if (k >= n_chain) return;
   const some_flac_frame f = frames[chain[k]];
   long long end;
   const int rc = walk_frame<true>(data, streams[f.stream], f, nullptr, scratch + scratch_off[k], coef + threadIdx.x, &end);
-  if (rc != SOME_FLAC_OK) atomicCAS(status, 0, rc);                // a chained frame parsed OK: never expected
+  if (rc != SOME_FLAC_OK) {                                        // a chained frame parsed OK: never expected
+    atomicCAS(status, 0, rc);
+    if (failed) atomicMin(failed, k);
+  }
 }
 
 __global__ void __launch_bounds__(FL_EMIT_THREADS) flac_emit_kernel(const some_flac_stream* streams,
@@ -470,19 +475,7 @@ __global__ void __launch_bounds__(FL_EMIT_THREADS) flac_emit_kernel(const some_f
       for (int c = 0; c < ch; ++c) y[static_cast<long long>(i) * ch + c] = __fmul_rn(static_cast<float>(s[c * bs + i]), scale);
       continue;
     }
-    float v[8];
-#pragma unroll
-    for (int c = 0; c < 8; ++c) v[c] = c < ch ? __fmul_rn(static_cast<float>(s[c * bs + i]), scale) : 0.f;
-    float sum;
-    if (ch == 8) {
-      sum = __fadd_rn(__fadd_rn(__fadd_rn(v[0], v[1]), __fadd_rn(v[2], v[3])), __fadd_rn(__fadd_rn(v[4], v[5]), __fadd_rn(v[6], v[7])));
-    } else {
-      sum = v[0];
-#pragma unroll
-      for (int c = 1; c < 7; ++c)
-        if (c < ch) sum = __fadd_rn(sum, v[c]);
-    }
-    y[i] = ch == 1 ? sum : __fdiv_rn(sum, static_cast<float>(ch));
+    y[i] = mono_mean(ch, [&](int c) { return __fmul_rn(static_cast<float>(s[c * bs + i]), scale); });
   }
 }
 
@@ -516,15 +509,22 @@ extern "C" int some_flac_scan(const uint8_t* data, long long n_bytes, const some
   return check_launch("some_flac_scan");
 }
 
-extern "C" int some_flac_decode(const uint8_t* data, const some_flac_stream* streams, const some_flac_frame* frames,
-                                const int32_t* chain, const int64_t* scratch_off, const int64_t* out_off, int n_chain,
-                                int32_t* scratch, float* out, int mono, int* status, cudaStream_t stream) {
+int some::flac_decode_chain(const uint8_t* data, const some_flac_stream* streams, const some_flac_frame* frames,
+                            const int32_t* chain, const int64_t* scratch_off, const int64_t* out_off, int n_chain,
+                            int32_t* scratch, float* out, int mono, int* status, int* failed, cudaStream_t stream) {
   SOME_REQUIRE(data && streams && frames && chain && scratch_off && out_off && scratch && out && status,
                "some_flac_decode: null pointer");
   SOME_REQUIRE(n_chain >= 0, "some_flac_decode: %d frames", n_chain);
   if (n_chain == 0) return 0;
   flac_decode_kernel<<<(n_chain + FL_FRAME_THREADS - 1) / FL_FRAME_THREADS, FL_FRAME_THREADS, 0, stream>>>(
-      data, streams, frames, chain, scratch_off, n_chain, scratch, status);
+      data, streams, frames, chain, scratch_off, n_chain, scratch, status, failed);
   flac_emit_kernel<<<n_chain, FL_EMIT_THREADS, 0, stream>>>(streams, frames, chain, scratch_off, out_off, scratch, out, mono);
   return check_launch("some_flac_decode");
+}
+
+extern "C" int some_flac_decode(const uint8_t* data, const some_flac_stream* streams, const some_flac_frame* frames,
+                                const int32_t* chain, const int64_t* scratch_off, const int64_t* out_off, int n_chain,
+                                int32_t* scratch, float* out, int mono, int* status, cudaStream_t stream) {
+  return flac_decode_chain(data, streams, frames, chain, scratch_off, out_off, n_chain, scratch, out, mono, status, nullptr,
+                           stream);
 }

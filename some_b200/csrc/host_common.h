@@ -58,6 +58,12 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
     }                                \
   } while (0)
 
+// some_flac_decode, and with `failed` != NULL (a device int, INT_MAX on entry) also the lowest chain index k whose frame failed
+// to decode, so that a caller decoding many recordings can name the one that failed.
+int flac_decode_chain(const uint8_t* data, const some_flac_stream* streams, const some_flac_frame* frames, const int32_t* chain,
+                      const int64_t* scratch_off, const int64_t* out_off, int n_chain, int32_t* scratch, float* out, int mono,
+                      int* status, int* failed, cudaStream_t stream);
+
 // The number of RMS frames whose windows end within the first `fixed` samples (the streaming slicer and the stream).
 inline int64_t frames_within(const some_slicer_frames& f, int64_t fixed) {
   const int64_t reach = f.win_size - f.win_size / 2;          // frame k reads samples up to k hop - win / 2 + win - 1

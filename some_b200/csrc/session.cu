@@ -14,6 +14,7 @@
 // The whole file is read and validated before any CUDA call.
 #include "host_common.h"
 
+#include <limits.h>
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -280,6 +281,9 @@ struct some_session {
   // grow-only buffers
   DevBuf ws_block, scratch, wave_d, tab_d, cu_d, slab_d, native_d, meta_d, rms_d, step_d;
   PinBuf wave_h, tab_h, cu_h, slab_h, meta_h, rms_h, step_h;   // step: the samples and descriptors of a stream step
+  // transcribe_encoded: the files' audio bytes, the FLAC candidate list, scan workspace and int32 scratch
+  DevBuf enc_d, flac_frames_d, flac_ws_d, flac_scratch_d;
+  PinBuf enc_h, flac_frames_h;
   int ws_m = 0;
   some_workspace ws{};
   some_notes chunks;                      // the notes of a stream step's chunks, before they are split by stream
@@ -294,10 +298,12 @@ void destroy(some_session* s) {
     if (s->stream) cudaStreamSynchronize(s->stream);
     if (s->copy_stream) cudaStreamSynchronize(s->copy_stream);
     for (DevBuf* b : {&s->ws_block, &s->scratch, &s->wave_d, &s->tab_d, &s->cu_d, &s->slab_d, &s->native_d, &s->meta_d,
-                      &s->rms_d, &s->step_d})
+                      &s->rms_d, &s->step_d, &s->enc_d, &s->flac_frames_d, &s->flac_ws_d, &s->flac_scratch_d})
       b->release();
     for (auto& t : s->tables) t.second.d.release();
-    for (PinBuf* b : {&s->wave_h, &s->tab_h, &s->cu_h, &s->slab_h, &s->meta_h, &s->rms_h, &s->step_h}) b->release();
+    for (PinBuf* b : {&s->wave_h, &s->tab_h, &s->cu_h, &s->slab_h, &s->meta_h, &s->rms_h, &s->step_h, &s->enc_h,
+                      &s->flac_frames_h})
+      b->release();
     for (cudaEvent_t& e : s->ev)
       if (e) cudaEventDestroy(e);
     if (s->stream) cudaStreamDestroy(s->stream);
@@ -689,7 +695,43 @@ extern "C" int some_session_get_info(const some_session* s, some_session_info* i
 }
 
 namespace {
-int transcribe_sliced(some_session* s, const float* samples, int64_t n, int sample_rate, int64_t n_out,
+// What the slicer sees of a recording of n samples at sample_rate: its length at the model's rate (audio.resampled_length:
+// librosa.load's output length; resampy refuses a recording whose own output would be empty) and, unless the recording is
+// one chunk anyway (no longer than min_length hops, slicer2.py:79-80), the number of RMS frames to cut it by.
+struct SliceShape {
+  int64_t n_out = 0;
+  int frames = 0;       // 0: one chunk [0, n_out)
+};
+int slice_shape(int64_t n, int sample_rate, int sr, const some_slicer_frames& sl, const char* who, SliceShape* sh) {
+  int64_t n_out = n;
+  if (sample_rate != sr) {
+    SOME_REQUIRE(n * sr / sample_rate >= 1, "%s: Input signal length=%lld is too small to resample from %d->%d", who,
+                 static_cast<long long>(n), sample_rate, sr);
+    n_out = static_cast<int64_t>(ceil(static_cast<double>(n) * (static_cast<double>(sr) / sample_rate)));
+  }
+  sh->n_out = n_out;
+  sh->frames = 0;
+  if ((n_out + sl.hop_size - 1) / sl.hop_size > sl.min_length) {
+    const int64_t frames = 1 + (n_out + 2 * (sl.win_size / 2) - sl.win_size) / sl.hop_size;
+    SOME_REQUIRE(frames < (int64_t(1) << 31), "%s: recording too long", who);
+    sh->frames = static_cast<int>(frames);
+  }
+  return 0;
+}
+// The chunk ranges of a recording from its shape and, when it is cut, its sh.frames RMS values.
+int slice_ranges(const SliceShape& sh, const float* rms, const some_slicer_frames& sl, std::vector<int64_t>& ranges) {
+  if (sh.frames == 0) {
+    ranges = {0, sh.n_out};
+    return 0;
+  }
+  ranges.resize(2 * (static_cast<size_t>(sh.frames) + 2));
+  int count = 0;
+  if (some_slicer_ranges(rms, sh.frames, sh.n_out, &sl, ranges.data(), sh.frames + 2, &count)) return -1;
+  ranges.resize(2 * static_cast<size_t>(count));
+  return 0;
+}
+
+int transcribe_sliced(some_session* s, const float* samples, int64_t n, int sample_rate, const SliceShape& sh,
                       const some_slicer_frames& sl, some_notes* out);
 
 // After a failure partway through a call, copies and kernels may still be queued on the session's streams: wait for them, so
@@ -724,18 +766,12 @@ extern "C" int some_session_transcribe_sliced(some_session* s, const float* samp
   const int sr = s->info.sample_rate;
   some_slicer_frames sl;
   if (some_slicer_derive(sr, params, &sl)) return -1;
-  // audio.resampled_length: librosa.load's output length, and resampy's refusal of too-short inputs
-  int64_t n_out = n;
-  const double ratio = static_cast<double>(sr) / sample_rate;
-  if (sample_rate != sr) {
-    SOME_REQUIRE(static_cast<int64_t>(n) * sr / sample_rate >= 1,
-                 "some_session_transcribe_sliced: Input signal length=%lld is too small to resample from %d->%d", n, sample_rate, sr);
-    n_out = static_cast<int64_t>(ceil(static_cast<double>(n) * ratio));
-  }
+  SliceShape sh;
+  if (slice_shape(n, sample_rate, sr, sl, "some_session_transcribe_sliced", &sh)) return -1;
   std::lock_guard<std::mutex> lock(s->mu);
   DeviceScope scope(s->device);
   SOME_CUDA(scope.err, "cudaSetDevice");
-  return settle(s, transcribe_sliced(s, samples, n, sample_rate, n_out, sl, out));
+  return settle(s, transcribe_sliced(s, samples, n, sample_rate, sh, sl, out));
 }
 
 namespace {
@@ -760,10 +796,10 @@ const double* table_for(some_session* s, int sample_rate) {
   return static_cast<const double*>(t.d.p);
 }
 
-int transcribe_sliced(some_session* s, const float* samples, int64_t n, int sample_rate, int64_t n_out,
+int transcribe_sliced(some_session* s, const float* samples, int64_t n, int sample_rate, const SliceShape& sh,
                       const some_slicer_frames& sl, some_notes* out) {
   const int sr = s->info.sample_rate;
-  const double ratio = static_cast<double>(sr) / sample_rate;
+  const int64_t n_out = sh.n_out;
   // upload (through pinned memory) and, at another rate, resample into the wave buffer
   if (s->wave_h.ensure(4ull * n + 16, "the staged audio") || s->wave_d.ensure(4ull * n_out + 16, "the audio")) return -1;
   float* wave = static_cast<float*>(s->wave_d.p);
@@ -784,23 +820,16 @@ int transcribe_sliced(some_session* s, const float* samples, int64_t n, int samp
                              table, kKaiserTaps, s->stream))
       return -1;
   }
-  // the slicer: a recording no longer than min_length is one chunk (slicer2.py:79-80)
+  // the slicer
   std::vector<int64_t> ranges;
-  if ((n_out + sl.hop_size - 1) / sl.hop_size <= sl.min_length) {
-    ranges = {0, n_out};
-  } else {
-    const int64_t frames = 1 + (n_out + 2 * (sl.win_size / 2) - sl.win_size) / sl.hop_size;
-    SOME_REQUIRE(frames < (int64_t(1) << 31), "some_session_transcribe_sliced: recording too long");
-    const int nf = static_cast<int>(frames);
+  if (sh.frames) {
+    const int nf = sh.frames;
     if (s->rms_d.ensure(4ull * nf, "the RMS frames") || s->rms_h.ensure(4ull * nf, "the RMS frames")) return -1;
     if (some_slicer_rms(wave, n_out, sl.win_size, sl.hop_size, static_cast<float*>(s->rms_d.p), nf, s->stream)) return -1;
     SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * nf, cudaMemcpyDeviceToHost, s->stream), "RMS download");
     SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
-    ranges.resize(2 * (static_cast<size_t>(nf) + 2));
-    int count = 0;
-    if (some_slicer_ranges(static_cast<const float*>(s->rms_h.p), nf, n_out, &sl, ranges.data(), nf + 2, &count)) return -1;
-    ranges.resize(2 * static_cast<size_t>(count));
   }
+  if (slice_ranges(sh, static_cast<const float*>(s->rms_h.p), sl, ranges)) return -1;
   const int B = static_cast<int>(ranges.size() / 2);
   if (B == 0) {
     out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
@@ -1177,4 +1206,280 @@ extern "C" int some_stream_get_info(const some_stream* st, some_stream_info* inf
 extern "C" int some_stream_close(some_stream* st) {
   if (st) destroy(st);
   return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- encoded files
+namespace {
+struct EncItem {
+  const uint8_t* bytes = nullptr;
+  some_audio_meta m{};
+  int64_t n = 0;              // decoded samples at the file's rate (FLAC without a stated length: known after the chain)
+  SliceShape sh;
+  int64_t up = 0;             // the audio bytes' offset in the upload
+  int64_t noff = 0, woff = 0; // the native-rate and model-rate samples in the session's native buffer (equal at the model's rate)
+  int64_t rms0 = 0;
+  int c0 = 0, c1 = 0;         // its chunks in the batch
+};
+
+// Re-raises the last error with the item's index in front.
+int item_error(int i) {
+  const std::string m = some_last_error();
+  set_error("some_session_transcribe_encoded: item %d: %s", i, m.c_str());
+  return -1;
+}
+
+constexpr int64_t align4(int64_t n) { return (n + 3) & ~int64_t(3); }
+
+// The GPU step of some_session_transcribe_encoded (under the session's mutex); out[] is written only at the end.
+int transcribe_encoded(some_session* s, std::vector<EncItem>& its, const some_slicer_frames& sl, some_notes* const* out) {
+  const int sr = s->info.sample_rate;
+  const int count = static_cast<int>(its.size());
+  std::vector<int> flac, wav;
+  for (int i = 0; i < count; ++i) (its[i].m.container == SOME_AUDIO_FLAC ? flac : wav).push_back(i);
+  const int nf = static_cast<int>(flac.size());
+  // 1. one upload: the FLAC items' audio bytes first (the scan covers only them), the WAV data chunks, the FLAC descriptors
+  int64_t at = 0;
+  for (int i : flac) its[i].up = at, at += static_cast<int64_t>(align16(static_cast<size_t>(its[i].m.data_bytes)));
+  const int64_t flac_bytes = at;
+  for (int i : wav) its[i].up = at, at += static_cast<int64_t>(align16(static_cast<size_t>(its[i].m.data_bytes)));
+  const int64_t streams_off = at;
+  const int64_t up_bytes = at + static_cast<int64_t>(sizeof(some_flac_stream)) * nf;
+  if (s->enc_h.ensure(up_bytes + 16, "the encoded files") || s->enc_d.ensure(up_bytes + 16, "the encoded files")) return -1;
+  uint8_t* up_h = static_cast<uint8_t*>(s->enc_h.p);
+  uint8_t* up_d = static_cast<uint8_t*>(s->enc_d.p);
+  {
+    constexpr int64_t kPiece = int64_t(1) << 20;
+    std::vector<std::pair<int, int64_t>> pieces;
+    for (int i = 0; i < count; ++i)
+      for (int64_t a = 0; a < its[i].m.data_bytes; a += kPiece) pieces.push_back({i, a});
+    const int nt = static_cast<int>(std::min<int64_t>(s->pool->size(), static_cast<int64_t>(pieces.size())));
+    s->pool->run(nt, [&](int t) {
+      for (size_t j = t; j < pieces.size(); j += nt) {
+        const EncItem& it = its[pieces[j].first];
+        const int64_t a = pieces[j].second;
+        memcpy(up_h + it.up + a, it.bytes + it.m.data_offset + a, static_cast<size_t>(std::min<int64_t>(kPiece, it.m.data_bytes - a)));
+      }
+    });
+  }
+  some_flac_stream* st_h = reinterpret_cast<some_flac_stream*>(up_h + streams_off);
+  for (int k = 0; k < nf; ++k) {
+    const EncItem& it = its[flac[k]];
+    st_h[k] = some_flac_stream{it.up, it.up + it.m.data_bytes, it.m.channels, it.m.bits, it.m.max_blocksize, 0};
+  }
+  SOME_CUDA(cudaMemcpyAsync(up_d, up_h, static_cast<size_t>(up_bytes), cudaMemcpyHostToDevice, s->stream), "encoded upload");
+  const some_flac_stream* st_d = reinterpret_cast<const some_flac_stream*>(up_d + streams_off);
+
+  // 2. the FLAC frames: one scan, the candidates down, the chain on the host
+  std::vector<int32_t> chain;
+  std::vector<int64_t> first(nf + 1, 0), lengths(nf, 0);
+  const some_flac_frame* frames_h = nullptr;
+  if (nf) {
+    int64_t cap = 64;
+    for (int i : flac) {
+      const some_audio_meta& m = its[i].m;
+      cap += m.frames ? m.frames / std::max(m.min_blocksize, 1) + 2 : m.data_bytes / 16 + 2;
+    }
+    SOME_REQUIRE(cap < (int64_t(1) << 31), "some_session_transcribe_encoded: too many FLAC frames in one call");
+    const uint64_t ws_bytes = some_flac_scan_workspace_bytes(flac_bytes);
+    if (s->flac_ws_d.ensure(ws_bytes + 16, "the FLAC scan workspace")) return -1;
+    int* count_d = reinterpret_cast<int*>(static_cast<char*>(s->flac_ws_d.p) + ws_bytes);
+    int n_cand = 0;
+    for (;;) {
+      if (s->flac_frames_d.ensure(sizeof(some_flac_frame) * cap, "the FLAC frames") ||
+          s->flac_frames_h.ensure(sizeof(some_flac_frame) * cap, "the FLAC frames"))
+        return -1;
+      if (some_flac_scan(up_d, flac_bytes, st_d, nf, static_cast<some_flac_frame*>(s->flac_frames_d.p), static_cast<int>(cap),
+                         count_d, s->flac_ws_d.p, s->stream))
+        return -1;
+      SOME_CUDA(cudaMemcpyAsync(s->flac_frames_h.p, count_d, sizeof(int), cudaMemcpyDeviceToHost, s->stream), "count download");
+      SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+      n_cand = *static_cast<int*>(s->flac_frames_h.p);
+      if (n_cand <= cap) break;
+      cap = n_cand;
+    }
+    SOME_CUDA(cudaMemcpyAsync(s->flac_frames_h.p, s->flac_frames_d.p, sizeof(some_flac_frame) * n_cand, cudaMemcpyDeviceToHost,
+                              s->stream), "candidate download");
+    SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+    frames_h = static_cast<const some_flac_frame*>(s->flac_frames_h.p);
+    std::vector<some_flac_range> recs(nf);
+    for (int k = 0; k < nf; ++k) {
+      const EncItem& it = its[flac[k]];
+      recs[k] = some_flac_range{it.up - it.m.data_offset, it.up, it.up + it.m.data_bytes, it.m.frames};
+    }
+    chain.resize(std::max(n_cand, 1));
+    int failed = -1;
+    if (some_flac_chain(frames_h, n_cand, recs.data(), nf, chain.data(), n_cand, first.data(), lengths.data(), &failed))
+      return item_error(failed >= 0 ? flac[failed] : 0);
+    for (int k = 0; k < nf; ++k) {
+      EncItem& it = its[flac[k]];
+      it.n = lengths[k];
+      char who[96];
+      snprintf(who, sizeof(who), "some_session_transcribe_encoded: item %d", flac[k]);
+      if (slice_shape(it.n, it.m.rate, sr, sl, who, &it.sh)) return -1;   // the length was not stated: checked now
+    }
+  }
+
+  // 3. where every recording goes: native samples, then (at another rate) the model-rate samples
+  int64_t total = 0, frames_total = 0;
+  for (EncItem& it : its) {
+    it.noff = total;
+    total += align4(it.n);
+    if (it.m.rate != sr) it.woff = total, total += align4(it.sh.n_out);
+    else it.woff = it.noff;
+    it.rms0 = frames_total;
+    frames_total += it.sh.frames;
+  }
+  if (s->native_d.ensure(4ull * total + 16, "the decoded audio") ||
+      s->rms_d.ensure(4ull * frames_total + 16, "the RMS frames") || s->rms_h.ensure(4ull * frames_total + 16, "the RMS frames"))
+    return -1;
+  float* base = static_cast<float*>(s->native_d.p);
+  // descriptors: the PCM items, the chained FLAC frames (their scratch and output offsets), resampling and RMS windows
+  std::vector<some_pcm_item> pcm;
+  for (int i : wav) {
+    const EncItem& it = its[i];
+    pcm.push_back(some_pcm_item{up_d + it.up, it.n, it.m.channels, it.m.kind, 1, 0, base + it.noff});
+  }
+  const int n_chain = nf ? static_cast<int>(first[nf]) : 0;
+  std::vector<int64_t> scratch_off(n_chain), out_off(n_chain);
+  int64_t scratch_total = 0;
+  for (int k = 0; k < nf; ++k) {
+    const EncItem& it = its[flac[k]];
+    int64_t o = it.noff;
+    for (int64_t j = first[k]; j < first[k + 1]; ++j) {
+      const some_flac_frame& f = frames_h[chain[j]];
+      scratch_off[j] = scratch_total, out_off[j] = o;
+      scratch_total += static_cast<int64_t>(f.blocksize) * it.m.channels;
+      o += f.blocksize;
+    }
+  }
+  std::vector<some_resample_window> rs;
+  std::vector<some_rms_window> rm;
+  for (const EncItem& it : its) {
+    if (it.m.rate != sr) {
+      const double* table = table_for(s, it.m.rate);
+      if (!table) return -1;
+      rs.push_back({base + it.noff, 0, it.n, 1, base + it.woff, 0, 0, it.sh.n_out, it.m.rate, sr, table, kKaiserTaps});
+    }
+    if (it.sh.frames)
+      rm.push_back({base + it.woff, 0, it.sh.n_out, it.sh.n_out, sl.win_size, sl.hop_size, static_cast<float*>(s->rms_d.p) + it.rms0,
+                    0, it.sh.frames});
+  }
+  const int kp = static_cast<int>(pcm.size()), kr = static_cast<int>(rs.size()), km = static_cast<int>(rm.size());
+  const size_t pcm_off = 0;
+  const size_t rs_off = pcm_off + align16(static_cast<size_t>(some_pcm_decode_bytes(kp)));
+  const size_t rm_off = rs_off + align16(static_cast<size_t>(some_resample_windows_bytes(kr)));
+  const size_t chain_off = rm_off + align16(static_cast<size_t>(some_slicer_rms_windows_bytes(km)));
+  const size_t soff_off = chain_off + align16(4ull * n_chain);
+  const size_t ooff_off = soff_off + 8ull * n_chain;
+  const size_t status_off = ooff_off + 8ull * n_chain;
+  const size_t bytes = status_off + 16;
+  if (s->step_h.ensure(bytes, "the decode descriptors") || s->step_d.ensure(bytes, "the decode descriptors") ||
+      s->flac_scratch_d.ensure(4ull * scratch_total + 16, "the FLAC scratch"))
+    return -1;
+  char* dh = static_cast<char*>(s->step_h.p);
+  char* dd = static_cast<char*>(s->step_d.p);
+  if (some_pcm_decode_pack(pcm.data(), kp, dh + pcm_off) || some_resample_windows_pack(rs.data(), kr, dh + rs_off) ||
+      some_slicer_rms_windows_pack(rm.data(), km, dh + rm_off))
+    return -1;
+  if (n_chain) {
+    memcpy(dh + chain_off, chain.data(), 4ull * n_chain);
+    memcpy(dh + soff_off, scratch_off.data(), 8ull * n_chain);
+    memcpy(dh + ooff_off, out_off.data(), 8ull * n_chain);
+  }
+  memset(dh + status_off, 0, 16);
+  reinterpret_cast<int*>(dh + status_off)[1] = INT_MAX;      // the first chained frame that fails to decode, if one does
+  int* status_d = reinterpret_cast<int*>(dd + status_off);
+  SOME_CUDA(cudaMemcpyAsync(dd, dh, bytes, cudaMemcpyHostToDevice, s->stream), "descriptor upload");
+  // 4. decode, resample, RMS; one download and one synchronise
+  if (some_pcm_decode(dh + pcm_off, dd + pcm_off, s->stream)) return -1;
+  if (n_chain &&
+      flac_decode_chain(up_d, st_d, static_cast<const some_flac_frame*>(s->flac_frames_d.p),
+                        reinterpret_cast<const int32_t*>(dd + chain_off), reinterpret_cast<const int64_t*>(dd + soff_off),
+                        reinterpret_cast<const int64_t*>(dd + ooff_off), n_chain, static_cast<int32_t*>(s->flac_scratch_d.p), base, 1,
+                        status_d, status_d + 1, s->stream))
+    return -1;
+  if (some_resample_kaiser_windows(dh + rs_off, dd + rs_off, s->stream) || some_slicer_rms_windows(dh + rm_off, dd + rm_off, s->stream))
+    return -1;
+  if (frames_total)
+    SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames_total, cudaMemcpyDeviceToHost, s->stream), "RMS download");
+  int* status_h = reinterpret_cast<int*>(dh + status_off);
+  SOME_CUDA(cudaMemcpyAsync(status_h, status_d, 2 * sizeof(int), cudaMemcpyDeviceToHost, s->stream), "status download");
+  SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+  if (status_h[0] != 0) {                          // the frame's item: the recording whose chain holds chain index k
+    const int64_t k = status_h[1];
+    int r = 0;
+    while (r + 1 < nf && first[r + 1] <= k) ++r;
+    const EncItem& it = its[flac[r]];
+    set_error("some_session_transcribe_encoded: item %d: FLAC frame at byte offset %lld failed to decode (status %d)", flac[r],
+              static_cast<long long>(frames_h[chain[k]].pos - (it.up - it.m.data_offset)), status_h[0]);
+    return -1;
+  }
+  // 5. the slicer per item, then one batch over the chunks of all items
+  std::vector<int64_t> starts, lens, begin;
+  std::vector<int64_t> ranges;
+  for (EncItem& it : its) {
+    if (slice_ranges(it.sh, static_cast<const float*>(s->rms_h.p) + it.rms0, sl, ranges)) return -1;
+    it.c0 = static_cast<int>(starts.size());
+    for (size_t r = 0; r + 1 < ranges.size(); r += 2) {
+      begin.push_back(ranges[r]);
+      starts.push_back(it.woff + ranges[r]);
+      lens.push_back(std::max<int64_t>(0, ranges[r + 1] - ranges[r]));
+    }
+    it.c1 = static_cast<int>(starts.size());
+  }
+  const int B = static_cast<int>(starts.size());
+  if (B && run_batch(s, nullptr, base, starts.data(), lens.data(), B, &s->chunks)) return -1;
+  const some_notes& all = s->chunks;
+  for (int i = 0; i < count; ++i) {
+    some_notes* o = out[i];
+    clear(o);
+    for (int c = its[i].c0; c < its[i].c1; ++c) {
+      const int64_t a = all.first[c], b = all.first[c + 1];
+      o->midi.insert(o->midi.end(), all.midi.begin() + a, all.midi.begin() + b);
+      o->dur.insert(o->dur.end(), all.dur.begin() + a, all.dur.begin() + b);
+      o->rest.insert(o->rest.end(), all.rest.begin() + a, all.rest.begin() + b);
+      o->first.push_back(o->first.back() + (b - a));
+      o->range.push_back(begin[c]), o->range.push_back(begin[c] + lens[c]);
+    }
+  }
+  return 0;
+}
+}  // namespace
+
+extern "C" int some_session_transcribe_encoded(some_session* s, const some_encoded* items, int count,
+                                               const some_slicer_params* params, some_notes* const* out) {
+  SOME_REQUIRE(s != nullptr && items != nullptr && out != nullptr && count >= 0, "some_session_transcribe_encoded: bad arguments");
+  if (count == 0) return 0;
+  const int sr = s->info.sample_rate;
+  some_slicer_frames sl;
+  if (some_slicer_derive(sr, params, &sl)) return -1;
+  // every item is checked before any GPU work
+  std::vector<EncItem> its(count);
+  std::map<const void*, int> seen_notes;
+  for (int i = 0; i < count; ++i) {
+    SOME_REQUIRE(items[i].data != nullptr && items[i].n_bytes > 0, "some_session_transcribe_encoded: item %d is NULL or empty", i);
+    SOME_REQUIRE(out[i] != nullptr, "some_session_transcribe_encoded: item %d: NULL notes", i);
+    const auto shared = seen_notes.emplace(out[i], i);
+    SOME_REQUIRE(shared.second, "some_session_transcribe_encoded: item %d shares its some_notes with item %d", i,
+                 shared.first->second);
+    EncItem& it = its[i];
+    it.bytes = static_cast<const uint8_t*>(items[i].data);
+    if (some_audio_info(items[i].data, items[i].n_bytes, &it.m)) return item_error(i);
+    SOME_REQUIRE(it.m.container == SOME_AUDIO_FLAC || it.m.channels <= 128,
+                 "some_session_transcribe_encoded: item %d: a mono down-mix of %d channels (at most 128)", i, it.m.channels);
+    if (it.m.rate != sr) {                           // rate pairs the resampler does not support
+      long long t_end, x_first;
+      if (some_resample_window_plan(0, 0, 0, it.m.rate, sr, kKaiserTaps, &t_end, &x_first)) return item_error(i);
+    }
+    it.n = it.m.frames;
+    if (it.m.container == SOME_AUDIO_WAV || it.m.frames > 0) {
+      char who[96];
+      snprintf(who, sizeof(who), "some_session_transcribe_encoded: item %d", i);
+      if (slice_shape(it.n, it.m.rate, sr, sl, who, &it.sh)) return -1;
+    }
+  }
+  std::lock_guard<std::mutex> lock(s->mu);
+  DeviceScope scope(s->device);
+  SOME_CUDA(scope.err, "cudaSetDevice");
+  return settle(s, transcribe_encoded(s, its, sl, out));
 }

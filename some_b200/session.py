@@ -118,6 +118,35 @@ class Session:
                 notes.close()
         return [a / self.sample_rate for a, _ in ranges], ranges, res
 
+    def transcribe_encoded(self, items: Sequence, params: Optional[_lib.SlicerParams] = None):
+        """some_session_transcribe_encoded: WAV or FLAC files (bytes, or paths to read) -> one (chunk offsets in seconds, chunk
+        sample ranges, per-chunk notes) per item, what transcribe_sliced returns for audio.load(file, sr=None, mono=True).
+        The files are decoded, resampled, sliced and transcribed in one GPU step."""
+        datas = []
+        for it in items:
+            if isinstance(it, (bytes, bytearray, memoryview)):
+                datas.append(bytes(it))
+            else:
+                with open(os.fspath(it), 'rb') as f:
+                    datas.append(f.read())
+        k = len(datas)
+        bufs = [C.create_string_buffer(d, len(d)) if d else None for d in datas]
+        enc = (_lib.Encoded * max(k, 1))(*[_lib.Encoded(C.cast(b, C.c_void_p) if b is not None else None, len(d))
+                                           for b, d in zip(bufs, datas)])
+        notes = [Notes() for _ in range(k)]
+        try:
+            outs = (C.c_void_p * max(k, 1))(*[n.handle for n in notes])
+            _lib.check(self.lib.some_session_transcribe_encoded(self.handle, enc, k, C.byref(params) if params is not None else None,
+                                                                outs), 'some_session_transcribe_encoded')
+            res = []
+            for n in notes:
+                ranges, r = n.results(self.timestep)
+                res.append(([a / self.sample_rate for a, _ in ranges], ranges, r))
+            return res
+        finally:
+            for n in notes:
+                n.close()
+
     def stream(self, sample_rate: Optional[int] = None, params: Optional[_lib.SlicerParams] = None) -> 'Stream':
         """some_stream_open: a recording pushed while it arrives (see Stream)."""
         return Stream(self, sample_rate, params)
