@@ -1,9 +1,11 @@
 // Native inference session: a model file written by `python -m some_b200.export` in, notes out, with no Python or torch in
 // between.  Host code, and the copy kernel that scatters a stream step's upload; the work is done by the sm_90a kernels of
-// this library, enqueued in the order Engine.enqueue
-// (some_b200/engine.py) and Engine.infer_sliced use:
-//   [some_resample_kaiser] -> [some_slicer_rms + the slicer's decisions on the host] -> per pipeline chunk:
+// this library, enqueued in the order Engine.enqueue (some_b200/engine.py) and Engine.infer_sliced use:
+//   [some_resample_kaiser_windows] -> [some_slicer_rms_windows + the slicer's decisions on the host] -> per pipeline chunk:
 //   some_mel_logmel -> some_forward (stand-alone LayerNorms, sigmoid / softmax head) -> some_decode_notes.
+// The sliced and the encoded calls share that front end (Recordings: one resampling window per recording at another rate,
+// one RMS window per recording that is cut, one batch over the chunks of all recordings); a stream step launches the same
+// two kernels over the windows of its streams.
 //
 // The model file (little-endian; INTEGRATION.md "Deploying without Python" has the table):
 //   header     128 bytes: magic "SOMEB200", format version, ABI number, file size, directory offset, tensor count, the scalars
@@ -119,43 +121,38 @@ std::string shape_str(const std::vector<uint64_t>& s) {
   return r + "]";
 }
 
-// Grow-only device / pinned buffers.
-struct DevBuf {
+// A grow-only buffer of device memory, or of pinned host memory.  It frees itself, so the structs that own buffers need not
+// list them; it is move-only, so a buffer has one owner.
+template <bool kPinned>
+struct GrowBuf {
   void* p = nullptr;
   size_t cap = 0;
+  GrowBuf() = default;
+  GrowBuf(GrowBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr, o.cap = 0; }
+  GrowBuf& operator=(GrowBuf&& o) noexcept {
+    release();
+    p = o.p, cap = o.cap;
+    o.p = nullptr, o.cap = 0;
+    return *this;
+  }
+  ~GrowBuf() { release(); }
   int ensure(size_t bytes, const char* what) {
     if (bytes <= cap) return 0;
     const size_t want = std::max(bytes, cap + cap / 4);
-    if (p) cudaFree(p);
-    p = nullptr, cap = 0;
-    cudaError_t e = cudaMalloc(&p, want);
-    SOME_REQUIRE(e == cudaSuccess, "session: cudaMalloc(%zu) for %s: %s", want, what, cudaGetErrorString(e));
+    release();
+    cudaError_t e = kPinned ? cudaHostAlloc(&p, want, cudaHostAllocDefault) : cudaMalloc(&p, want);
+    SOME_REQUIRE(e == cudaSuccess, "session: %s(%zu) for %s: %s", kPinned ? "cudaHostAlloc" : "cudaMalloc", want, what,
+                 cudaGetErrorString(e));
     cap = want;
     return 0;
   }
   void release() {
-    if (p) cudaFree(p);
+    if (p) kPinned ? cudaFreeHost(p) : cudaFree(p);
     p = nullptr, cap = 0;
   }
 };
-struct PinBuf {
-  void* p = nullptr;
-  size_t cap = 0;
-  int ensure(size_t bytes, const char* what) {
-    if (bytes <= cap) return 0;
-    const size_t want = std::max(bytes, cap + cap / 4);
-    if (p) cudaFreeHost(p);
-    p = nullptr, cap = 0;
-    cudaError_t e = cudaHostAlloc(&p, want, cudaHostAllocDefault);
-    SOME_REQUIRE(e == cudaSuccess, "session: cudaHostAlloc(%zu) for %s: %s", want, what, cudaGetErrorString(e));
-    cap = want;
-    return 0;
-  }
-  void release() {
-    if (p) cudaFreeHost(p);
-    p = nullptr, cap = 0;
-  }
-};
+using DevBuf = GrowBuf<false>;
+using PinBuf = GrowBuf<true>;
 
 // Makes `dev` current for the scope of a call and restores the caller's device afterwards.
 struct DeviceScope {
@@ -278,39 +275,72 @@ struct some_session {
   std::map<double, Table> tables;
   cudaStream_t stream = nullptr, copy_stream = nullptr;
   cudaEvent_t ev[4] = {};
-  // grow-only buffers
-  DevBuf ws_block, scratch, wave_d, tab_d, cu_d, slab_d, native_d, meta_d, rms_d, step_d;
-  PinBuf wave_h, tab_h, cu_h, slab_h, meta_h, rms_h, step_h;   // step: the samples and descriptors of a stream step
+  // grow-only buffers; rec_d: recordings at their own rates and at the model's (the sliced and encoded calls)
+  DevBuf ws_block, scratch, wave_d, tab_d, cu_d, slab_d, rec_d, rms_d, step_d;
+  PinBuf wave_h, tab_h, cu_h, slab_h, rms_h, step_h;   // step: the samples and descriptors of a step's upload
   // transcribe_encoded: the files' audio bytes, the FLAC candidate list, scan workspace and int32 scratch
   DevBuf enc_d, flac_frames_d, flac_ws_d, flac_scratch_d;
   PinBuf enc_h, flac_frames_h;
   int ws_m = 0;
   some_workspace ws{};
-  some_notes chunks;                      // the notes of a stream step's chunks, before they are split by stream
+  some_notes chunks;                      // the notes of a step's chunks, before they are split by recording or stream
   std::unique_ptr<WorkerPool> pool;
 };
 
 namespace {
 
 void destroy(some_session* s) {
-  {
-    DeviceScope scope(s->device);
-    if (s->stream) cudaStreamSynchronize(s->stream);
-    if (s->copy_stream) cudaStreamSynchronize(s->copy_stream);
-    for (DevBuf* b : {&s->ws_block, &s->scratch, &s->wave_d, &s->tab_d, &s->cu_d, &s->slab_d, &s->native_d, &s->meta_d,
-                      &s->rms_d, &s->step_d, &s->enc_d, &s->flac_frames_d, &s->flac_ws_d, &s->flac_scratch_d})
-      b->release();
-    for (auto& t : s->tables) t.second.d.release();
-    for (PinBuf* b : {&s->wave_h, &s->tab_h, &s->cu_h, &s->slab_h, &s->meta_h, &s->rms_h, &s->step_h, &s->enc_h,
-                      &s->flac_frames_h})
-      b->release();
-    for (cudaEvent_t& e : s->ev)
-      if (e) cudaEventDestroy(e);
-    if (s->stream) cudaStreamDestroy(s->stream);
-    if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
-    if (s->weights) cudaFree(s->weights);
+  DeviceScope scope(s->device);
+  if (s->stream) cudaStreamSynchronize(s->stream);
+  if (s->copy_stream) cudaStreamSynchronize(s->copy_stream);
+  for (cudaEvent_t& e : s->ev)
+    if (e) cudaEventDestroy(e);
+  if (s->stream) cudaStreamDestroy(s->stream);
+  if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
+  if (s->weights) cudaFree(s->weights);
+  delete s;                               // its buffers free themselves, on the session's device
+}
+
+void clear(some_notes* out) {
+  out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
+}
+
+// Sets *out to chunks [c0, c1) of `all` (the notes of a step's batch); chunk c is samples [begin[c], begin[c] + lens[c]).
+void take_chunks(const some_notes& all, int c0, int c1, const int64_t* begin, const int64_t* lens, some_notes* out) {
+  clear(out);
+  for (int c = c0; c < c1; ++c) {
+    const int64_t a = all.first[c], b = all.first[c + 1];
+    out->midi.insert(out->midi.end(), all.midi.begin() + a, all.midi.begin() + b);
+    out->dur.insert(out->dur.end(), all.dur.begin() + a, all.dur.begin() + b);
+    out->rest.insert(out->rest.end(), all.rest.begin() + a, all.rest.begin() + b);
+    out->first.push_back(out->first.back() + (b - a));
+    out->range.push_back(begin[c]), out->range.push_back(begin[c] + lens[c]);
   }
-  delete s;
+}
+
+// A span of host memory to copy into pinned memory.
+struct HostSpan {
+  void* dst;
+  const void* src;
+  size_t bytes;
+};
+// Copies the spans on the session's threads: each span in pieces of up to `piece` bytes, dealt out in turn to one thread per
+// `piece` bytes in all (at most the pool's size).
+void copy_to_pinned(WorkerPool& pool, const std::vector<HostSpan>& spans, size_t piece) {
+  std::vector<std::pair<const HostSpan*, size_t>> pieces;
+  size_t total = 0;
+  for (const HostSpan& sp : spans) {
+    for (size_t a = 0; a < sp.bytes; a += piece) pieces.push_back({&sp, a});
+    total += sp.bytes;
+  }
+  const int nt = static_cast<int>(std::min<size_t>(pool.size(), (total + piece - 1) / piece));
+  pool.run(nt, [&](int t) {
+    for (size_t j = t; j < pieces.size(); j += nt) {
+      const HostSpan& sp = *pieces[j].first;
+      const size_t a = pieces[j].second;
+      memcpy(static_cast<char*>(sp.dst) + a, static_cast<const char*>(sp.src) + a, std::min(piece, sp.bytes - a));
+    }
+  });
 }
 
 // Engine._chunks: up to three pipeline chunks of whole clips, a small first one.
@@ -465,19 +495,15 @@ int run_batch(some_session* s, const float* const* host, const float* resident, 
   return 0;
 }
 
-// Uploads n floats of host memory to `dst` through the pinned staging buffer: in pieces, each copied into pinned memory by the
-// session's threads and then sent while the next piece is copied.
+// Uploads n floats of host memory to `dst` through the pinned staging buffer: in pieces of 16 MB, each copied into pinned
+// memory by the session's threads (256 KB per thread and turn) and then sent while the next piece is copied.
 int upload_staged(some_session* s, float* dst, const float* src, int64_t n) {
-  constexpr int64_t kPiece = int64_t(1) << 22;   // 16 MB
+  constexpr int64_t kPiece = int64_t(1) << 22;
+  if (s->wave_h.ensure(4ull * n + 16, "the staged audio")) return -1;
   float* pin = static_cast<float*>(s->wave_h.p);
   for (int64_t a = 0; a < n; a += kPiece) {
     const int64_t len = std::min(kPiece, n - a);
-    const int nt = static_cast<int>(std::min<int64_t>(s->pool->size(), (len + 65535) / 65536));
-    const int64_t per = (len + nt - 1) / nt;
-    s->pool->run(nt, [&](int t) {
-      const int64_t b = a + t * per, e = std::min(a + len, b + per);
-      if (e > b) memcpy(pin + b, src + b, 4ull * (e - b));
-    });
+    copy_to_pinned(*s->pool, {{pin + a, src + a, 4ull * len}}, size_t(1) << 18);
     SOME_CUDA(cudaMemcpyAsync(dst + a, pin + a, 4ull * len, cudaMemcpyHostToDevice, s->stream), "audio upload");
   }
   return 0;
@@ -731,50 +757,22 @@ int slice_ranges(const SliceShape& sh, const float* rms, const some_slicer_frame
   return 0;
 }
 
-int transcribe_sliced(some_session* s, const float* samples, int64_t n, int sample_rate, const SliceShape& sh,
-                      const some_slicer_frames& sl, some_notes* out);
-
-// After a failure partway through a call, copies and kernels may still be queued on the session's streams: wait for them, so
-// that the next call cannot rewrite staging or device buffers they still use.  (The error message of the failure is kept.)
-int settle(some_session* s, int rc) {
+// Runs a call's work under the session's mutex, with the session's device current.  After a failure partway through, copies
+// and kernels may still be queued on the session's streams: it waits for them, so that the next call cannot rewrite staging
+// or device buffers they still use.  (The error message of the failure is kept.)
+template <class F>
+int locked(some_session* s, F work) {
+  std::lock_guard<std::mutex> lock(s->mu);
+  DeviceScope scope(s->device);
+  SOME_CUDA(scope.err, "cudaSetDevice");
+  const int rc = work();
   if (rc != 0) {
     cudaStreamSynchronize(s->copy_stream);
     cudaStreamSynchronize(s->stream);
   }
   return rc;
 }
-}  // namespace
 
-extern "C" int some_session_transcribe(some_session* s, const float* const* clips, const int64_t* lens, int B, some_notes* out) {
-  SOME_REQUIRE(s != nullptr && out != nullptr && B >= 0 && (B == 0 || (clips != nullptr && lens != nullptr)),
-               "some_session_transcribe: bad arguments");
-  for (int i = 0; i < B; ++i) SOME_REQUIRE(lens[i] >= 0 && (lens[i] == 0 || clips[i] != nullptr), "some_session_transcribe: clip %d", i);
-  std::lock_guard<std::mutex> lock(s->mu);
-  if (B == 0) {
-    out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
-    return 0;
-  }
-  DeviceScope scope(s->device);
-  SOME_CUDA(scope.err, "cudaSetDevice");
-  return settle(s, run_batch(s, clips, nullptr, nullptr, lens, B, out));
-}
-
-extern "C" int some_session_transcribe_sliced(some_session* s, const float* samples, long long n, int sample_rate,
-                                              const some_slicer_params* params, some_notes* out) {
-  SOME_REQUIRE(s != nullptr && out != nullptr && n >= 0 && (n == 0 || samples != nullptr) && sample_rate > 0,
-               "some_session_transcribe_sliced: bad arguments");
-  const int sr = s->info.sample_rate;
-  some_slicer_frames sl;
-  if (some_slicer_derive(sr, params, &sl)) return -1;
-  SliceShape sh;
-  if (slice_shape(n, sample_rate, sr, sl, "some_session_transcribe_sliced", &sh)) return -1;
-  std::lock_guard<std::mutex> lock(s->mu);
-  DeviceScope scope(s->device);
-  SOME_CUDA(scope.err, "cudaSetDevice");
-  return settle(s, transcribe_sliced(s, samples, n, sample_rate, sh, sl, out));
-}
-
-namespace {
 // The resampling table for sample_rate -> the model's rate: uploaded on the session's stream (in front of the resampling
 // launches that read it) the first time its ratio is used, and kept.  Upsampling reads the table as it is; resampy scales it
 // by the ratio when downsampling (audio._device_table), so each downsampling ratio has its own copy.
@@ -796,50 +794,151 @@ const double* table_for(some_session* s, int sample_rate) {
   return static_cast<const double*>(t.d.p);
 }
 
-int transcribe_sliced(some_session* s, const float* samples, int64_t n, int sample_rate, const SliceShape& sh,
-                      const some_slicer_frames& sl, some_notes* out) {
-  const int sr = s->info.sample_rate;
-  const int64_t n_out = sh.n_out;
-  // upload (through pinned memory) and, at another rate, resample into the wave buffer
-  if (s->wave_h.ensure(4ull * n + 16, "the staged audio") || s->wave_d.ensure(4ull * n_out + 16, "the audio")) return -1;
-  float* wave = static_cast<float*>(s->wave_d.p);
-  if (sample_rate == sr) {
-    if (upload_staged(s, wave, samples, n)) return -1;
-  } else {
-    const double* table = table_for(s, sample_rate);
-    if (!table) return -1;
-    if (s->native_d.ensure(4ull * n + 16, "the native audio") || s->meta_h.ensure(32, "resampling tables") ||
-        s->meta_d.ensure(32, "resampling tables"))
-      return -1;
-    int64_t* meta = static_cast<int64_t*>(s->meta_h.p);
-    meta[0] = 0, meta[1] = n, meta[2] = 0;
-    const int64_t* md = static_cast<const int64_t*>(s->meta_d.p);
-    if (upload_staged(s, static_cast<float*>(s->native_d.p), samples, n)) return -1;
-    SOME_CUDA(cudaMemcpyAsync(s->meta_d.p, meta, 24, cudaMemcpyHostToDevice, s->stream), "table upload");
-    if (some_resample_kaiser(static_cast<const float*>(s->native_d.p), md, md + 1, wave, md + 2, 1, n_out, sample_rate, sr,
-                             table, kKaiserTaps, s->stream))
-      return -1;
+// The host-to-device copy of a step's samples and descriptors: regions of the session's pinned step_h, each 16-byte aligned,
+// filled once reserve() has made room for all of them, and sent to the same offsets of step_d in one copy.
+struct Upload {
+  some_session* s;
+  size_t bytes = 0;
+  size_t add(size_t n) {
+    const size_t off = bytes;
+    bytes += align16(n);
+    return off;
   }
-  // the slicer
-  std::vector<int64_t> ranges;
-  if (sh.frames) {
-    const int nf = sh.frames;
-    if (s->rms_d.ensure(4ull * nf, "the RMS frames") || s->rms_h.ensure(4ull * nf, "the RMS frames")) return -1;
-    if (some_slicer_rms(wave, n_out, sl.win_size, sl.hop_size, static_cast<float*>(s->rms_d.p), nf, s->stream)) return -1;
-    SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * nf, cudaMemcpyDeviceToHost, s->stream), "RMS download");
-    SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
-  }
-  if (slice_ranges(sh, static_cast<const float*>(s->rms_h.p), sl, ranges)) return -1;
-  const int B = static_cast<int>(ranges.size() / 2);
-  if (B == 0) {
-    out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
+  int reserve(const char* what) { return s->step_h.ensure(bytes, what) || s->step_d.ensure(bytes, what) ? -1 : 0; }
+  char* h(size_t off) const { return static_cast<char*>(s->step_h.p) + off; }
+  char* d(size_t off) const { return static_cast<char*>(s->step_d.p) + off; }
+  int send(const char* what) const {
+    if (bytes) SOME_CUDA(cudaMemcpyAsync(s->step_d.p, s->step_h.p, bytes, cudaMemcpyHostToDevice, s->stream), what);
     return 0;
   }
-  std::vector<int64_t> starts(B), lens(B);
-  for (int i = 0; i < B; ++i) starts[i] = ranges[2 * i], lens[i] = std::max<int64_t>(0, ranges[2 * i + 1] - ranges[2 * i]);
-  return run_batch(s, nullptr, wave, starts.data(), lens.data(), B, out);
+};
+
+constexpr int64_t align4(int64_t n) { return (n + 3) & ~int64_t(3); }
+
+// Recordings in the session's recording buffer, each at its own rate, made into chunks and notes together (the sliced and
+// the encoded calls; a caller writes the recordings there and may add its own regions to the step's upload and its own
+// launches and downloads in front of the synchronise):
+//   place   where each recording, its model-rate samples and its RMS frames go; one resampling window per recording at
+//           another rate and one RMS window per recording that is cut, packed into regions added to the upload after the
+//           caller's own, and the upload reserved (the caller fills its regions after this);
+//   launch  after the upload is sent and the recordings are written: one resampling launch, one RMS launch, the RMS download;
+//   finish  after the caller's synchronise: each recording's cuts, one batch over all chunks, each recording's notes.
+struct Recordings {
+  struct Item {
+    int rate;
+    int64_t n;                // samples at `rate`
+    SliceShape sh;
+    some_notes* out;
+    int64_t x = 0, y = 0;     // its samples at `rate` and at the model's rate in the buffer (the same at the model's rate)
+    int64_t rms0 = 0;         // its first RMS frame
+    int c0 = 0, c1 = 0;       // its chunks in the batch
+  };
+  std::vector<Item> items;
+  float* base = nullptr;      // the recording buffer
+  int64_t frames = 0;
+  int kr = 0, km = 0;
+  size_t rs_off = 0, rm_off = 0;
+
+  int place(some_session* s, const some_slicer_frames& sl, Upload& up) {
+    const int sr = s->info.sample_rate;
+    int64_t total = 0;
+    for (Item& it : items) {
+      it.x = it.y = total;
+      total += align4(it.n);
+      if (it.rate != sr) it.y = total, total += align4(it.sh.n_out);
+      it.rms0 = frames;
+      frames += it.sh.frames;
+    }
+    if (s->rec_d.ensure(4ull * total + 16, "the recordings") || s->rms_d.ensure(4ull * frames + 16, "the RMS frames") ||
+        s->rms_h.ensure(4ull * frames + 16, "the RMS frames"))
+      return -1;
+    base = static_cast<float*>(s->rec_d.p);
+    std::vector<some_resample_window> rs;
+    std::vector<some_rms_window> rm;
+    for (const Item& it : items) {
+      if (it.rate != sr) {
+        const double* table = table_for(s, it.rate);
+        if (!table) return -1;
+        rs.push_back({base + it.x, 0, it.n, 1, base + it.y, 0, 0, it.sh.n_out, it.rate, sr, table, kKaiserTaps});
+      }
+      if (it.sh.frames)
+        rm.push_back({base + it.y, 0, it.sh.n_out, it.sh.n_out, sl.win_size, sl.hop_size, static_cast<float*>(s->rms_d.p) + it.rms0,
+                      0, it.sh.frames});
+    }
+    kr = static_cast<int>(rs.size()), km = static_cast<int>(rm.size());
+    if (kr) rs_off = up.add(static_cast<size_t>(some_resample_windows_bytes(kr)));
+    if (km) rm_off = up.add(static_cast<size_t>(some_slicer_rms_windows_bytes(km)));
+    if (up.reserve("the step's upload") || (kr && some_resample_windows_pack(rs.data(), kr, up.h(rs_off))) ||
+        (km && some_slicer_rms_windows_pack(rm.data(), km, up.h(rm_off))))
+      return -1;
+    return 0;
+  }
+
+  int launch(some_session* s, const Upload& up) const {
+    if ((kr && some_resample_kaiser_windows(up.h(rs_off), up.d(rs_off), s->stream)) ||
+        (km && some_slicer_rms_windows(up.h(rm_off), up.d(rm_off), s->stream)))
+      return -1;
+    if (frames)
+      SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames, cudaMemcpyDeviceToHost, s->stream), "RMS download");
+    return 0;
+  }
+
+  int finish(some_session* s, const some_slicer_frames& sl) {
+    std::vector<int64_t> starts, lens, begin, ranges;
+    for (Item& it : items) {
+      if (slice_ranges(it.sh, static_cast<const float*>(s->rms_h.p) + it.rms0, sl, ranges)) return -1;
+      it.c0 = static_cast<int>(starts.size());
+      for (size_t r = 0; r + 1 < ranges.size(); r += 2) {
+        begin.push_back(ranges[r]);
+        starts.push_back(it.y + ranges[r]);
+        lens.push_back(std::max<int64_t>(0, ranges[r + 1] - ranges[r]));
+      }
+      it.c1 = static_cast<int>(starts.size());
+    }
+    const int B = static_cast<int>(starts.size());
+    if (B && run_batch(s, nullptr, base, starts.data(), lens.data(), B, &s->chunks)) return -1;
+    for (const Item& it : items) take_chunks(s->chunks, it.c0, it.c1, begin.data(), lens.data(), it.out);
+    return 0;
+  }
+};
+
+// One recording: uploaded through pinned memory into the recording buffer, then the one-recording case of Recordings, with
+// a synchronise before the batch only when the recording is cut.
+int transcribe_sliced(some_session* s, const float* samples, int64_t n, int sample_rate, const SliceShape& sh,
+                      const some_slicer_frames& sl, some_notes* out) {
+  Recordings rec;
+  rec.items.push_back({sample_rate, n, sh, out});
+  Upload up{s};
+  if (rec.place(s, sl, up) || upload_staged(s, rec.base + rec.items[0].x, samples, n) || up.send("descriptor upload") ||
+      rec.launch(s, up))
+    return -1;
+  if (sh.frames) SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+  return rec.finish(s, sl);
 }
 }  // namespace
+
+extern "C" int some_session_transcribe(some_session* s, const float* const* clips, const int64_t* lens, int B, some_notes* out) {
+  SOME_REQUIRE(s != nullptr && out != nullptr && B >= 0 && (B == 0 || (clips != nullptr && lens != nullptr)),
+               "some_session_transcribe: bad arguments");
+  for (int i = 0; i < B; ++i) SOME_REQUIRE(lens[i] >= 0 && (lens[i] == 0 || clips[i] != nullptr), "some_session_transcribe: clip %d", i);
+  if (B == 0) {
+    clear(out);
+    return 0;
+  }
+  return locked(s, [&] { return run_batch(s, clips, nullptr, nullptr, lens, B, out); });
+}
+
+extern "C" int some_session_transcribe_sliced(some_session* s, const float* samples, long long n, int sample_rate,
+                                              const some_slicer_params* params, some_notes* out) {
+  SOME_REQUIRE(s != nullptr && out != nullptr && n >= 0 && (n == 0 || samples != nullptr) && sample_rate > 0,
+               "some_session_transcribe_sliced: bad arguments");
+  const int sr = s->info.sample_rate;
+  some_slicer_frames sl;
+  if (some_slicer_derive(sr, params, &sl)) return -1;
+  SliceShape sh;
+  if (slice_shape(n, sample_rate, sr, sl, "some_session_transcribe_sliced", &sh)) return -1;
+  return locked(s, [&] { return transcribe_sliced(s, samples, n, sample_rate, sh, sl, out); });
+}
 
 // ---------------------------------------------------------------------------------------------------- streams
 namespace {
@@ -865,8 +964,7 @@ struct SampleWindow {
     if (bigger.ensure(4ull * std::max<int64_t>(2 * (len + n), 1 << 16), what)) return -1;
     if (len) SOME_CUDA(cudaMemcpyAsync(bigger.p, at(first), 4ull * len, cudaMemcpyDeviceToDevice, stream), "stream compaction");
     SOME_CUDA(cudaStreamSynchronize(stream), "synchronise");
-    buf.release();
-    buf = bigger;
+    buf = std::move(bigger);
     off = 0;
     return 0;
   }
@@ -904,16 +1002,9 @@ struct some_stream {
 
 namespace {
 void destroy(some_stream* st) {
-  {
-    DeviceScope scope(st->s->device);
-    for (DevBuf* b : {&st->native.buf, &st->wave.buf, &st->head_d}) b->release();
-  }
   some_slicer_stream_destroy(st->slicer);
-  delete st;
-}
-
-void clear(some_notes* out) {
-  out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
+  DeviceScope scope(st->s->device);
+  delete st;                              // its buffers free themselves, on the session's device
 }
 
 // One stream's part of a step: n new samples, whether the recording ends there, and where its chunks go.
@@ -1000,56 +1091,43 @@ int streams_step(some_session* s, std::vector<StepItem>& items) {
 
   // the upload: samples, then the scatter, resampling and RMS descriptors
   const int ks = static_cast<int>(sc.size()), kr = static_cast<int>(rs.size()), km = static_cast<int>(rm.size());
-  const size_t sc_off = 4ull * up_floats;
-  const size_t rs_off = sc_off + align16(windows_bytes<ScatterParams>(ks));
-  const size_t rm_off = rs_off + align16(static_cast<size_t>(some_resample_windows_bytes(kr)));
-  const size_t bytes = rm_off + align16(static_cast<size_t>(some_slicer_rms_windows_bytes(km)));
-  if (s->step_h.ensure(bytes, "the stream upload") || s->step_d.ensure(bytes, "the stream upload") ||
-      s->rms_d.ensure(4ull * frames + 16, "the RMS frames") || s->rms_h.ensure(4ull * frames + 16, "the RMS frames"))
+  Upload up{s};
+  const size_t smp_off = up.add(4ull * up_floats);
+  const size_t sc_off = up.add(windows_bytes<ScatterParams>(ks));
+  const size_t rs_off = up.add(static_cast<size_t>(some_resample_windows_bytes(kr)));
+  const size_t rm_off = up.add(static_cast<size_t>(some_slicer_rms_windows_bytes(km)));
+  if (up.reserve("the stream upload") || s->rms_d.ensure(4ull * frames + 16, "the RMS frames") ||
+      s->rms_h.ensure(4ull * frames + 16, "the RMS frames"))
     return -1;
-  char* up_h = static_cast<char*>(s->step_h.p);
-  char* up_d = static_cast<char*>(s->step_d.p);
+  std::vector<HostSpan> spans;
   {
-    ScatterParams* ps = windows_params<ScatterParams>(up_h + sc_off, ks);
-    long long* tile0 = windows_tile0(up_h + sc_off);
+    ScatterParams* ps = windows_params<ScatterParams>(up.h(sc_off), ks);
+    long long* tile0 = windows_tile0(up.h(sc_off));
     int j = 0;
     for (const StepItem& it : items)
       if (it.n) {
         ps[j] = sc[j];
-        ps[j].src = reinterpret_cast<const float*>(up_d) + it.up;
+        ps[j].src = reinterpret_cast<const float*>(up.d(smp_off)) + it.up;
         tile0[j + 1] = (it.n + kScatterTile - 1) / kScatterTile;
+        spans.push_back({reinterpret_cast<float*>(up.h(smp_off)) + it.up, it.samples, 4ull * it.n});
         ++j;
       }
-    windows_index(up_h + sc_off, ks, 0);
+    windows_index(up.h(sc_off), ks, 0);
   }
   for (int j = 0, at = 0; j < km; at += static_cast<int>(rm[j].f_end - rm[j].f_begin), ++j)   // in item order, as rms0
     rm[j].rms = static_cast<float*>(s->rms_d.p) + at;
-  if (some_resample_windows_pack(rs.data(), kr, up_h + rs_off) || some_slicer_rms_windows_pack(rm.data(), km, up_h + rm_off))
+  if (some_resample_windows_pack(rs.data(), kr, up.h(rs_off)) || some_slicer_rms_windows_pack(rm.data(), km, up.h(rm_off)))
     return -1;
-  {                                                // the samples, copied by the session's threads in pieces of up to 1 MB
-    constexpr int64_t kPiece = int64_t(1) << 18;
-    std::vector<std::pair<const StepItem*, int64_t>> pieces;
-    for (const StepItem& it : items)
-      for (int64_t a = 0; a < it.n; a += kPiece) pieces.push_back({&it, a});
-    const int nt = static_cast<int>(std::min<int64_t>(s->pool->size(), (up_floats + kPiece - 1) / kPiece));
-    float* dst = reinterpret_cast<float*>(up_h);
-    s->pool->run(nt, [&](int t) {
-      for (size_t j = t; j < pieces.size(); j += nt) {
-        const StepItem& it = *pieces[j].first;
-        const int64_t a = pieces[j].second;
-        memcpy(dst + it.up + a, it.samples + a, 4ull * std::min(kPiece, it.n - a));
-      }
-    });
-  }
-  SOME_CUDA(cudaMemcpyAsync(up_d, up_h, bytes, cudaMemcpyHostToDevice, s->stream), "stream upload");
+  copy_to_pinned(*s->pool, spans, size_t(1) << 20);          // the samples, in pieces of up to 1 MB
+  if (up.send("stream upload")) return -1;
   if (ks) {
-    const WindowsHeader& h = *reinterpret_cast<const WindowsHeader*>(up_h + sc_off);
+    const WindowsHeader& h = *reinterpret_cast<const WindowsHeader*>(up.h(sc_off));
     scatter_kernel<<<static_cast<unsigned>(h.tiles), kScatterThreads, 0, s->stream>>>(
-        windows_params<ScatterParams>(up_d + sc_off, ks), windows_tile0(up_d + sc_off), ks);
+        windows_params<ScatterParams>(up.d(sc_off), ks), windows_tile0(up.d(sc_off)), ks);
     if (check_launch("stream upload scatter")) return -1;
   }
-  if (some_resample_kaiser_windows(up_h + rs_off, up_d + rs_off, s->stream) ||
-      some_slicer_rms_windows(up_h + rm_off, up_d + rm_off, s->stream))
+  if (some_resample_kaiser_windows(up.h(rs_off), up.d(rs_off), s->stream) ||
+      some_slicer_rms_windows(up.h(rm_off), up.d(rm_off), s->stream))
     return -1;
   if (frames)
     SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames, cudaMemcpyDeviceToHost, s->stream), "RMS download");
@@ -1095,31 +1173,14 @@ int streams_step(some_session* s, std::vector<StepItem>& items) {
         SOME_CUDA(cudaMemcpyAsync(wave + starts[c], src[c], 4ull * lens[c], cudaMemcpyDeviceToDevice, s->stream), "chunk copy");
     if (run_batch(s, nullptr, wave, starts.data(), lens.data(), B, &s->chunks)) return -1;
   }
-  // each stream's notes, with its chunks' ranges
-  const some_notes& all = s->chunks;
-  for (const StepItem& it : items) {
-    some_notes* out = it.out;
-    clear(out);
-    for (int c = it.c0; c < it.c1; ++c) {
-      const int64_t a = all.first[c], b = all.first[c + 1];
-      out->midi.insert(out->midi.end(), all.midi.begin() + a, all.midi.begin() + b);
-      out->dur.insert(out->dur.end(), all.dur.begin() + a, all.dur.begin() + b);
-      out->rest.insert(out->rest.end(), all.rest.begin() + a, all.rest.begin() + b);
-      out->first.push_back(out->first.back() + (b - a));
-      out->range.push_back(begin[c]), out->range.push_back(begin[c] + lens[c]);
-    }
-  }
+  for (const StepItem& it : items) take_chunks(s->chunks, it.c0, it.c1, begin.data(), lens.data(), it.out);
   return 0;
 }
 
 // A step of one stream (some_stream_push, some_stream_finish).
 int stream_call(some_stream* st, const float* samples, int64_t n, bool final, some_notes* out) {
-  some_session* s = st->s;
-  DeviceScope scope(s->device);
-  SOME_CUDA(scope.err, "cudaSetDevice");
   std::vector<StepItem> items{StepItem{st, samples, n, final, out}};
-  std::lock_guard<std::mutex> lock(s->mu);
-  return settle(s, streams_step(s, items));
+  return locked(st->s, [&] { return streams_step(st->s, items); });
 }
 }  // namespace
 
@@ -1191,10 +1252,7 @@ extern "C" int some_stream_push_many(some_stream* const* streams, const float* c
     if (final) streams[i]->finished = true;
     items.push_back(StepItem{streams[i], samples[i], n[i], final, out[i]});
   }
-  DeviceScope scope(s->device);
-  SOME_CUDA(scope.err, "cudaSetDevice");
-  std::lock_guard<std::mutex> lock(s->mu);
-  return settle(s, streams_step(s, items));
+  return locked(s, [&] { return streams_step(s, items); });
 }
 
 extern "C" int some_stream_get_info(const some_stream* st, some_stream_info* info) {
@@ -1216,9 +1274,6 @@ struct EncItem {
   int64_t n = 0;              // decoded samples at the file's rate (FLAC without a stated length: known after the chain)
   SliceShape sh;
   int64_t up = 0;             // the audio bytes' offset in the upload
-  int64_t noff = 0, woff = 0; // the native-rate and model-rate samples in the session's native buffer (equal at the model's rate)
-  int64_t rms0 = 0;
-  int c0 = 0, c1 = 0;         // its chunks in the batch
 };
 
 // Re-raises the last error with the item's index in front.
@@ -1227,8 +1282,6 @@ int item_error(int i) {
   set_error("some_session_transcribe_encoded: item %d: %s", i, m.c_str());
   return -1;
 }
-
-constexpr int64_t align4(int64_t n) { return (n + 3) & ~int64_t(3); }
 
 // The GPU step of some_session_transcribe_encoded (under the session's mutex); out[] is written only at the end.
 int transcribe_encoded(some_session* s, std::vector<EncItem>& its, const some_slicer_frames& sl, some_notes* const* out) {
@@ -1247,20 +1300,9 @@ int transcribe_encoded(some_session* s, std::vector<EncItem>& its, const some_sl
   if (s->enc_h.ensure(up_bytes + 16, "the encoded files") || s->enc_d.ensure(up_bytes + 16, "the encoded files")) return -1;
   uint8_t* up_h = static_cast<uint8_t*>(s->enc_h.p);
   uint8_t* up_d = static_cast<uint8_t*>(s->enc_d.p);
-  {
-    constexpr int64_t kPiece = int64_t(1) << 20;
-    std::vector<std::pair<int, int64_t>> pieces;
-    for (int i = 0; i < count; ++i)
-      for (int64_t a = 0; a < its[i].m.data_bytes; a += kPiece) pieces.push_back({i, a});
-    const int nt = static_cast<int>(std::min<int64_t>(s->pool->size(), static_cast<int64_t>(pieces.size())));
-    s->pool->run(nt, [&](int t) {
-      for (size_t j = t; j < pieces.size(); j += nt) {
-        const EncItem& it = its[pieces[j].first];
-        const int64_t a = pieces[j].second;
-        memcpy(up_h + it.up + a, it.bytes + it.m.data_offset + a, static_cast<size_t>(std::min<int64_t>(kPiece, it.m.data_bytes - a)));
-      }
-    });
-  }
+  std::vector<HostSpan> spans;
+  for (const EncItem& it : its) spans.push_back({up_h + it.up, it.bytes + it.m.data_offset, static_cast<size_t>(it.m.data_bytes)});
+  copy_to_pinned(*s->pool, spans, size_t(1) << 20);          // in pieces of up to 1 MB
   some_flac_stream* st_h = reinterpret_cast<some_flac_stream*>(up_h + streams_off);
   for (int k = 0; k < nf; ++k) {
     const EncItem& it = its[flac[k]];
@@ -1319,90 +1361,50 @@ int transcribe_encoded(some_session* s, std::vector<EncItem>& its, const some_sl
     }
   }
 
-  // 3. where every recording goes: native samples, then (at another rate) the model-rate samples
-  int64_t total = 0, frames_total = 0;
-  for (EncItem& it : its) {
-    it.noff = total;
-    total += align4(it.n);
-    if (it.m.rate != sr) it.woff = total, total += align4(it.sh.n_out);
-    else it.woff = it.noff;
-    it.rms0 = frames_total;
-    frames_total += it.sh.frames;
-  }
-  if (s->native_d.ensure(4ull * total + 16, "the decoded audio") ||
-      s->rms_d.ensure(4ull * frames_total + 16, "the RMS frames") || s->rms_h.ensure(4ull * frames_total + 16, "the RMS frames"))
-    return -1;
-  float* base = static_cast<float*>(s->native_d.p);
-  // descriptors: the PCM items, the chained FLAC frames (their scratch and output offsets), resampling and RMS windows
+  // 3. the recordings' places, and one descriptor upload: the PCM items, the chained FLAC frames (their scratch and output
+  // offsets) and the status word, then the resampling and RMS windows
+  Recordings rec;
+  for (int i = 0; i < count; ++i) rec.items.push_back({its[i].m.rate, its[i].n, its[i].sh, out[i]});
+  const int kp = static_cast<int>(wav.size());
+  const int n_chain = nf ? static_cast<int>(first[nf]) : 0;
+  Upload up{s};
+  const size_t pcm_off = up.add(static_cast<size_t>(some_pcm_decode_bytes(kp)));
+  const size_t chain_off = up.add(4ull * n_chain), soff_off = up.add(8ull * n_chain), ooff_off = up.add(8ull * n_chain);
+  const size_t status_off = up.add(2 * sizeof(int));
+  if (rec.place(s, sl, up)) return -1;
   std::vector<some_pcm_item> pcm;
   for (int i : wav) {
     const EncItem& it = its[i];
-    pcm.push_back(some_pcm_item{up_d + it.up, it.n, it.m.channels, it.m.kind, 1, 0, base + it.noff});
+    pcm.push_back(some_pcm_item{up_d + it.up, it.n, it.m.channels, it.m.kind, 1, 0, rec.base + rec.items[i].x});
   }
-  const int n_chain = nf ? static_cast<int>(first[nf]) : 0;
-  std::vector<int64_t> scratch_off(n_chain), out_off(n_chain);
+  int64_t* scratch_off = reinterpret_cast<int64_t*>(up.h(soff_off));
+  int64_t* out_off = reinterpret_cast<int64_t*>(up.h(ooff_off));
   int64_t scratch_total = 0;
   for (int k = 0; k < nf; ++k) {
-    const EncItem& it = its[flac[k]];
-    int64_t o = it.noff;
+    int64_t o = rec.items[flac[k]].x;
     for (int64_t j = first[k]; j < first[k + 1]; ++j) {
       const some_flac_frame& f = frames_h[chain[j]];
       scratch_off[j] = scratch_total, out_off[j] = o;
-      scratch_total += static_cast<int64_t>(f.blocksize) * it.m.channels;
+      scratch_total += static_cast<int64_t>(f.blocksize) * its[flac[k]].m.channels;
       o += f.blocksize;
     }
   }
-  std::vector<some_resample_window> rs;
-  std::vector<some_rms_window> rm;
-  for (const EncItem& it : its) {
-    if (it.m.rate != sr) {
-      const double* table = table_for(s, it.m.rate);
-      if (!table) return -1;
-      rs.push_back({base + it.noff, 0, it.n, 1, base + it.woff, 0, 0, it.sh.n_out, it.m.rate, sr, table, kKaiserTaps});
-    }
-    if (it.sh.frames)
-      rm.push_back({base + it.woff, 0, it.sh.n_out, it.sh.n_out, sl.win_size, sl.hop_size, static_cast<float*>(s->rms_d.p) + it.rms0,
-                    0, it.sh.frames});
-  }
-  const int kp = static_cast<int>(pcm.size()), kr = static_cast<int>(rs.size()), km = static_cast<int>(rm.size());
-  const size_t pcm_off = 0;
-  const size_t rs_off = pcm_off + align16(static_cast<size_t>(some_pcm_decode_bytes(kp)));
-  const size_t rm_off = rs_off + align16(static_cast<size_t>(some_resample_windows_bytes(kr)));
-  const size_t chain_off = rm_off + align16(static_cast<size_t>(some_slicer_rms_windows_bytes(km)));
-  const size_t soff_off = chain_off + align16(4ull * n_chain);
-  const size_t ooff_off = soff_off + 8ull * n_chain;
-  const size_t status_off = ooff_off + 8ull * n_chain;
-  const size_t bytes = status_off + 16;
-  if (s->step_h.ensure(bytes, "the decode descriptors") || s->step_d.ensure(bytes, "the decode descriptors") ||
-      s->flac_scratch_d.ensure(4ull * scratch_total + 16, "the FLAC scratch"))
+  if (s->flac_scratch_d.ensure(4ull * scratch_total + 16, "the FLAC scratch") || some_pcm_decode_pack(pcm.data(), kp, up.h(pcm_off)))
     return -1;
-  char* dh = static_cast<char*>(s->step_h.p);
-  char* dd = static_cast<char*>(s->step_d.p);
-  if (some_pcm_decode_pack(pcm.data(), kp, dh + pcm_off) || some_resample_windows_pack(rs.data(), kr, dh + rs_off) ||
-      some_slicer_rms_windows_pack(rm.data(), km, dh + rm_off))
-    return -1;
-  if (n_chain) {
-    memcpy(dh + chain_off, chain.data(), 4ull * n_chain);
-    memcpy(dh + soff_off, scratch_off.data(), 8ull * n_chain);
-    memcpy(dh + ooff_off, out_off.data(), 8ull * n_chain);
-  }
-  memset(dh + status_off, 0, 16);
-  reinterpret_cast<int*>(dh + status_off)[1] = INT_MAX;      // the first chained frame that fails to decode, if one does
-  int* status_d = reinterpret_cast<int*>(dd + status_off);
-  SOME_CUDA(cudaMemcpyAsync(dd, dh, bytes, cudaMemcpyHostToDevice, s->stream), "descriptor upload");
+  if (n_chain) memcpy(up.h(chain_off), chain.data(), 4ull * n_chain);
+  int* status_h = reinterpret_cast<int*>(up.h(status_off));
+  int* status_d = reinterpret_cast<int*>(up.d(status_off));
+  status_h[0] = 0, status_h[1] = INT_MAX;                    // the first chained frame that fails to decode, if one does
+  if (up.send("descriptor upload")) return -1;
   // 4. decode, resample, RMS; one download and one synchronise
-  if (some_pcm_decode(dh + pcm_off, dd + pcm_off, s->stream)) return -1;
+  if (some_pcm_decode(up.h(pcm_off), up.d(pcm_off), s->stream)) return -1;
   if (n_chain &&
       flac_decode_chain(up_d, st_d, static_cast<const some_flac_frame*>(s->flac_frames_d.p),
-                        reinterpret_cast<const int32_t*>(dd + chain_off), reinterpret_cast<const int64_t*>(dd + soff_off),
-                        reinterpret_cast<const int64_t*>(dd + ooff_off), n_chain, static_cast<int32_t*>(s->flac_scratch_d.p), base, 1,
-                        status_d, status_d + 1, s->stream))
+                        reinterpret_cast<const int32_t*>(up.d(chain_off)), reinterpret_cast<const int64_t*>(up.d(soff_off)),
+                        reinterpret_cast<const int64_t*>(up.d(ooff_off)), n_chain, static_cast<int32_t*>(s->flac_scratch_d.p),
+                        rec.base, 1, status_d, status_d + 1, s->stream))
     return -1;
-  if (some_resample_kaiser_windows(dh + rs_off, dd + rs_off, s->stream) || some_slicer_rms_windows(dh + rm_off, dd + rm_off, s->stream))
-    return -1;
-  if (frames_total)
-    SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames_total, cudaMemcpyDeviceToHost, s->stream), "RMS download");
-  int* status_h = reinterpret_cast<int*>(dh + status_off);
+  if (rec.launch(s, up)) return -1;
   SOME_CUDA(cudaMemcpyAsync(status_h, status_d, 2 * sizeof(int), cudaMemcpyDeviceToHost, s->stream), "status download");
   SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
   if (status_h[0] != 0) {                          // the frame's item: the recording whose chain holds chain index k
@@ -1415,34 +1417,7 @@ int transcribe_encoded(some_session* s, std::vector<EncItem>& its, const some_sl
     return -1;
   }
   // 5. the slicer per item, then one batch over the chunks of all items
-  std::vector<int64_t> starts, lens, begin;
-  std::vector<int64_t> ranges;
-  for (EncItem& it : its) {
-    if (slice_ranges(it.sh, static_cast<const float*>(s->rms_h.p) + it.rms0, sl, ranges)) return -1;
-    it.c0 = static_cast<int>(starts.size());
-    for (size_t r = 0; r + 1 < ranges.size(); r += 2) {
-      begin.push_back(ranges[r]);
-      starts.push_back(it.woff + ranges[r]);
-      lens.push_back(std::max<int64_t>(0, ranges[r + 1] - ranges[r]));
-    }
-    it.c1 = static_cast<int>(starts.size());
-  }
-  const int B = static_cast<int>(starts.size());
-  if (B && run_batch(s, nullptr, base, starts.data(), lens.data(), B, &s->chunks)) return -1;
-  const some_notes& all = s->chunks;
-  for (int i = 0; i < count; ++i) {
-    some_notes* o = out[i];
-    clear(o);
-    for (int c = its[i].c0; c < its[i].c1; ++c) {
-      const int64_t a = all.first[c], b = all.first[c + 1];
-      o->midi.insert(o->midi.end(), all.midi.begin() + a, all.midi.begin() + b);
-      o->dur.insert(o->dur.end(), all.dur.begin() + a, all.dur.begin() + b);
-      o->rest.insert(o->rest.end(), all.rest.begin() + a, all.rest.begin() + b);
-      o->first.push_back(o->first.back() + (b - a));
-      o->range.push_back(begin[c]), o->range.push_back(begin[c] + lens[c]);
-    }
-  }
-  return 0;
+  return rec.finish(s, sl);
 }
 }  // namespace
 
@@ -1478,8 +1453,5 @@ extern "C" int some_session_transcribe_encoded(some_session* s, const some_encod
       if (slice_shape(it.n, it.m.rate, sr, sl, who, &it.sh)) return -1;
     }
   }
-  std::lock_guard<std::mutex> lock(s->mu);
-  DeviceScope scope(s->device);
-  SOME_CUDA(scope.err, "cudaSetDevice");
-  return settle(s, transcribe_encoded(s, its, sl, out));
+  return locked(s, [&] { return transcribe_encoded(s, its, sl, out); });
 }

@@ -81,6 +81,11 @@ def test_sliced_equals_infer_sliced(model):
     offsets, ranges, got = sess.transcribe_sliced(short)
     assert ranges == [(0, len(short))]
     assert_same_notes(got, ins.infer([short]))
+    empty = np.zeros(0, np.float32)                           # one chunk of no samples
+    offsets, ranges, got = sess.transcribe_sliced(empty)
+    want_off, want = ins.model.infer_sliced(empty, slicer, quantized=ins.quantized)
+    assert offsets == list(want_off) and ranges == [(0, 0)]
+    assert_same_notes(got, want)
 
 
 @pytest.mark.parametrize('rate', [48000, 22050])
