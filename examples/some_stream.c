@@ -2,15 +2,19 @@
  * Python.
  *
  *   some_stream MODEL RATE [DEVICE] < pcm
+ *   some_stream MODEL - [DEVICE] < file.wav or file.flac
  *
- * Reads raw mono little-endian float32 samples at RATE Hz from stdin in blocks of 100 ms, pushes each block to a
- * some_stream and prints the notes of every chunk as soon as it is delivered, one line per note:
+ * With RATE, reads raw mono little-endian float32 samples at RATE Hz from stdin in blocks of 100 ms and pushes each block to a
+ * some_stream.  With `-`, reads a WAV or FLAC byte stream from stdin in 64 KB reads and pushes each read to an encoded stream
+ * (some_stream_open_encoded: the rate comes from the header; decoded and down-mixed on the GPU as
+ * some_session_transcribe_encoded does).  Prints the notes of every chunk as soon as it is delivered, one line per note:
  *
  *   <chunk offset in seconds> <note_midi> <duration in seconds> <rest 0/1>
  *
  * the same lines examples/some_transcribe prints for the whole recording.  Live from a microphone:
  *
- *   arecord -f FLOAT_LE -c1 -r 44100 | some_stream model.somemodel 44100 */
+ *   arecord -f FLOAT_LE -c1 -r 44100 | some_stream model.somemodel 44100
+ *   arecord -f S16_LE -c2 -r 48000 -t wav | some_stream model.somemodel - */
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -34,10 +38,52 @@ static void print_chunks(const some_notes* notes, const some_session_info* info)
   fflush(stdout);
 }
 
+/* `-`: the bytes of a WAV or FLAC file from stdin, 64 KB per push. */
+static int run_encoded(some_session* s, const some_session_info* info) {
+  static unsigned char buf[1 << 16];
+  some_stream* st = NULL;
+  some_notes* notes = NULL;
+  int rc = 1;
+  if (some_notes_create(&notes) != 0 || some_stream_open_encoded(s, NULL, &st) != 0) goto fail;
+  for (;;) {
+    const size_t got = fread(buf, 1, sizeof(buf), stdin);
+    if (got == 0) break;
+    if (some_stream_push_bytes(st, buf, (long long)got, notes) != 0) goto fail;
+    print_chunks(notes, info);
+  }
+  if (ferror(stdin)) {
+    fprintf(stderr, "some_stream: read error\n");
+    goto done;
+  }
+  if (some_stream_finish(st, notes) != 0) goto fail;
+  print_chunks(notes, info);
+  rc = 0;
+  goto done;
+fail:
+  fprintf(stderr, "some_stream: %s\n", some_last_error());
+done:
+  some_stream_close(st);
+  some_notes_destroy(notes);
+  return rc;
+}
+
 int main(int argc, char** argv) {
-  if (argc < 3 || atoi(argv[2]) <= 0) {
-    fprintf(stderr, "usage: %s MODEL RATE [DEVICE] < mono float32 little-endian PCM\n", argv[0]);
+  const int encoded = argc >= 3 && strcmp(argv[2], "-") == 0;
+  if (argc < 3 || (!encoded && atoi(argv[2]) <= 0)) {
+    fprintf(stderr, "usage: %s MODEL RATE [DEVICE] < mono float32 little-endian PCM\n"
+                    "       %s MODEL - [DEVICE] < WAV or FLAC bytes\n", argv[0], argv[0]);
     return 2;
+  }
+  if (encoded) {
+    some_session* s = NULL;
+    some_session_info info;
+    int rc = 1;
+    if (some_session_open(argv[1], argc > 3 ? atoi(argv[3]) : 0, &s) != 0 || some_session_get_info(s, &info) != 0)
+      fprintf(stderr, "some_stream: %s\n", some_last_error());
+    else
+      rc = run_encoded(s, &info);
+    some_session_close(s);
+    return rc;
   }
   const int rate = atoi(argv[2]);
   const size_t block = (size_t)(rate / 10 > 0 ? rate / 10 : 1);

@@ -400,6 +400,21 @@ typedef struct {
 } some_flac_range;
 int some_flac_chain(const some_flac_frame* frames, int n_frames, const some_flac_range* recs, int n_recs, int32_t* chain,
                     int capacity, int64_t* first, int64_t* lengths, int* failed);
+/* some_flac_chain_resume (host, no CUDA call): the same walk for one recording whose bytes arrive in pieces, continued over
+ * the candidates of one window at a time.  `walk` keeps what the walk needs between windows: pos (the file offset where the
+ * next frame must start; set it to the first frame byte, with the rest zero and strategy -1, before the first window), the
+ * samples and frames chained so far, the blocking strategy and whether the walk is done.  The window holds the file's bytes
+ * from walk->pos on: file offset x is x + base in the candidates' coordinates, and the window ends at `stop`.  Writes the
+ * indices of the frames it chains to chain[0 .. *n_chained).  final != 0: the window runs to the end of the file, and every
+ * check of some_flac_chain applies with its message (offsets from the file's first byte).  Before that, the walk stops
+ * without error at a frame that is SOME_FLAC_TRUNCATED (the window ends inside it) or where fewer than 16 bytes (the
+ * longest frame header) follow and no header was found; the next window starts at walk->pos. */
+typedef struct {
+  int64_t pos, got, count;
+  int32_t strategy, done;
+} some_flac_walk;
+int some_flac_chain_resume(const some_flac_frame* frames, int n_frames, int64_t base, int64_t stop, int64_t length, int final,
+                           some_flac_walk* walk, int32_t* chain, int capacity, int* n_chained);
 
 /* ---- Container metadata on the host (csrc/audio_host.cu, no CUDA call): what some_b200.audio.load accepts, but for one
  * kind of file: integer PCM in 5-8 byte containers, which scipy reads as int64 and audio.decode_wav scales by 2^-63, is
@@ -424,6 +439,22 @@ typedef struct {
   long long data_bytes;          /* WAV: frames * channels * sample bytes; FLAC: to the end of the data */
 } some_audio_meta;
 int some_audio_info(const void* data, long long n_bytes, some_audio_meta* out);
+/* some_audio_walk: the walk of some_audio_info fed in pieces; some_audio_info is the case where all bytes come in one feed with
+ * end != 0.  A feed costs time in proportion to its own bytes, and the walker holds no skipped bytes (ID3 tags, metadata
+ * blocks other than STREAMINFO, WAV chunks other than fmt and data) and no audio: *held (may be NULL) stays within 48 bytes.
+ * After each feed: -1 with some_audio_info's message and offset for the same bytes (or for the whole file) once the refusal
+ * is certain; else 0 and *known = 1 once the metadata is in *meta (WAV: from the data chunk's header, with its stated size;
+ * FLAC: after the last metadata block; final after the end), and the audio bytes of this feed are the file offsets
+ * [*audio_begin, *audio_end): WAV sample bytes within the data chunk's stated size, FLAC everything after the metadata.  The
+ * rules that depend on where the file ends (a data chunk cut short keeps its whole frames, a partial 24-bit sample or
+ * multi-channel frame is refused, "Unexpected end of file", chunks after the data chunk) apply at the feed with end != 0.
+ *   stream != 0: a second WAV data chunk, or a fmt chunk after the data chunk, is refused when its header is reached; without
+ * it (and in some_audio_info) the last data chunk is read with the last fmt chunk, as scipy reads them. */
+typedef struct some_audio_walk some_audio_walk;
+int some_audio_walk_create(int stream, some_audio_walk** out);
+int some_audio_walk_feed(some_audio_walk* w, const void* data, long long n_bytes, int end, int* known, some_audio_meta* meta,
+                         long long* audio_begin, long long* audio_end, long long* held);
+int some_audio_walk_destroy(some_audio_walk* w);
 
 /* ---- K-pcm: the samples of RIFF/WAVE data chunks as audio.decode_wav hands them to librosa.load, many recordings in one
  * launch.  u8 -> (x - 128) / 128, s16 / s24 / s32 -> x / 2^(bits - 1) (s32 rounded to float32 first, as numpy's astype),
@@ -792,6 +823,44 @@ int some_stream_close(some_stream* st);
  * single pushes on other streams; one stream is used by one thread at a time. */
 int some_stream_push_many(some_stream* const* streams, const float* const* samples, const long long* n, const int* finish,
                           int count, some_notes* const* out);
+/* Encoded streams: a WAV or FLAC file pushed as its bytes arrive (a recorder or encoder writing to a pipe, an upload), decoded
+ * and down-mixed on the GPU exactly as some_session_transcribe_encoded decodes the whole file.  The rate comes from the header.
+ *   For a file that some_session_transcribe_encoded accepts, pushed in order and split in any way (single bytes, any sizes, all
+ * at once), the chunks of all pushes and the finish, concatenated, equal some_session_transcribe_encoded on the whole file:
+ * the same ranges and bit-identical notes.  Each chunk comes in the push where some_stream_push would deliver it if that push
+ * carried the samples decoded in it: a FLAC sample is decoded once its whole frame has arrived and its CRC-16 is checked, a
+ * WAV sample once its whole sample frame has arrived.  A header whose sizes are placeholders (as recorders writing to a pipe
+ * leave them) reads to the end of the bytes, as some_session_transcribe_encoded reads such a file.  One difference: a WAV file
+ * with a second data chunk, or with a fmt chunk after its data chunk, is refused when that chunk's header arrives (a stream
+ * cannot take back the samples of the first data chunk nor change the format they were decoded in; the whole-file call reads
+ * the last of each, as scipy does).
+ *   some_stream_finish, some_stream_get_info and some_stream_close serve both kinds of stream; `received` counts samples
+ * decoded at the file's rate.  some_stream_push and some_stream_push_many refuse encoded streams; some_stream_push_bytes* refuse
+ * PCM streams.  some_stream_get_meta: the file's metadata once the header is complete (zero before: container 0), the bytes
+ * pushed and the bytes the stream holds on the host.
+ *   Refusals come at the push that makes them certain, or at the finish, with the message some_session_transcribe_encoded
+ * gives for the file, prefixed by the function's name (and in the many-call by "stream i"): anything some_audio_info refuses,
+ * a corrupt FLAC stream (some_flac_chain's message; byte offsets from the file's first byte), a frame that fails to decode,
+ * and, at the push that completes the header, a rate pair the resampler does not support, a mono down-mix of more than 128
+ * channels or FLAC above 24 bits.  Chunks delivered before stay delivered; after such a refusal only some_stream_get_info,
+ * some_stream_get_meta and some_stream_close remain defined on the stream, and the session stays usable.  A content refusal
+ * returns SOME_STREAM_REFUSED (< 0, distinct from other errors) with the first refusal's message: in the many-call the other
+ * streams have completed their step and their out[i] hold their chunks (a refused stream's out[i] holds none), so a caller
+ * reads every out[i] after it, as after success.  Any other error (< 0, not SOME_STREAM_REFUSED) leaves every out[i]
+ * untouched: argument errors (those of some_stream_push_many, and a PCM stream or a refused one) change no stream; after a
+ * device error only some_stream_get_info, some_stream_get_meta and some_stream_close remain defined on the call's streams.
+ *   Each step: the walk of each stream's bytes on the host; one pinned upload of the FLAC windows (the bytes from each stream's
+ * first frame not decoded yet) and the whole WAV sample frames; with FLAC streams, one some_flac_scan, one download of the
+ * candidates, one synchronise and each stream's chain (some_flac_chain_resume); then one some_pcm_decode and one FLAC decode
+ * into the region some_stream_push_many's step scatters, and that step.  On top of a PCM stream's memory, an encoded stream
+ * holds on the host the bytes of at most one incomplete FLAC frame or WAV sample frame, plus the push in progress, and nothing
+ * of skipped metadata; on the device the session keeps the decoder scratch of one step. */
+enum { SOME_STREAM_REFUSED = -3 };
+int some_stream_open_encoded(some_session* s, const some_slicer_params* params, some_stream** out);
+int some_stream_push_bytes(some_stream* st, const void* data, long long n_bytes, some_notes* out);
+int some_stream_push_bytes_many(some_stream* const* streams, const void* const* data, const long long* n_bytes, const int* finish,
+                                int count, some_notes* const* out);
+int some_stream_get_meta(const some_stream* st, some_audio_meta* meta, long long* bytes_received, long long* bytes_held);
 
 #ifdef __cplusplus
 }

@@ -152,6 +152,10 @@ class FlacRange(C.Structure):
     _fields_ = [('base', C.c_int64), ('audio_start', C.c_int64), ('end', C.c_int64), ('length', C.c_int64)]
 
 
+class FlacWalk(C.Structure):
+    _fields_ = [('pos', C.c_int64), ('got', C.c_int64), ('count', C.c_int64), ('strategy', C.c_int32), ('done', C.c_int32)]
+
+
 class AudioMeta(C.Structure):
     _fields_ = [('container', C.c_int), ('rate', C.c_int), ('channels', C.c_int), ('bits', C.c_int), ('kind', C.c_int),
                 ('min_blocksize', C.c_int), ('max_blocksize', C.c_int), ('reserved', C.c_int), ('frames', C.c_longlong),
@@ -210,7 +214,13 @@ EXPORTS = {
     'some_flac_scan': (C.c_int, [_vp, C.c_longlong, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp]),
     'some_flac_decode': (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp, C.c_int, _vp, _vp]),
     'some_flac_chain': (C.c_int, [_vp, C.c_int, C.POINTER(FlacRange), C.c_int, _vp, C.c_int, _vp, _vp, C.POINTER(C.c_int)]),
+    'some_flac_chain_resume': (C.c_int, [_vp, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.POINTER(FlacWalk), _vp, C.c_int,
+                                         C.POINTER(C.c_int)]),
     'some_audio_info': (C.c_int, [_vp, C.c_longlong, C.POINTER(AudioMeta)]),
+    'some_audio_walk_create': (C.c_int, [C.c_int, C.POINTER(_vp)]),
+    'some_audio_walk_feed': (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.POINTER(C.c_int), C.POINTER(AudioMeta),
+                                       C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]),
+    'some_audio_walk_destroy': (C.c_int, [_vp]),
     'some_pcm_decode_bytes': (C.c_longlong, [C.c_int]),
     'some_pcm_decode_pack': (C.c_int, [C.POINTER(PcmItem), C.c_int, _vp]),
     'some_pcm_decode': (C.c_int, [_vp, _vp, _vp]),
@@ -255,6 +265,10 @@ EXPORTS = {
     'some_stream_get_info': (C.c_int, [_vp, C.POINTER(StreamInfo)]),
     'some_stream_close': (C.c_int, [_vp]),
     'some_stream_push_many': (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, _vp]),
+    'some_stream_open_encoded': (C.c_int, [_vp, C.POINTER(SlicerParams), C.POINTER(_vp)]),
+    'some_stream_push_bytes': (C.c_int, [_vp, _vp, C.c_longlong, _vp]),
+    'some_stream_push_bytes_many': (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, _vp]),
+    'some_stream_get_meta': (C.c_int, [_vp, C.POINTER(AudioMeta), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]),
 }
 
 _lib = None
@@ -262,6 +276,18 @@ _lib = None
 
 class SomeB200Error(RuntimeError):
     pass
+
+
+STREAM_REFUSED = -3       # SOME_STREAM_REFUSED: a stream was refused on its content; the call's other streams completed
+
+
+class StreamRefused(SomeB200Error):
+    """An encoded stream was refused on its content.  `results` holds what every item of the call returned (the refused
+    stream's entry holds no chunks): the other streams completed their step, and their chunks are there."""
+
+    def __init__(self, message: str, results):
+        super().__init__(message)
+        self.results = results
 
 
 def load():

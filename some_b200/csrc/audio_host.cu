@@ -7,6 +7,7 @@
 // with audio.parse_flac's metadata-block rules.  Its refusals carry the Python reason and a byte offset.
 // some_flac_chain is the one copy of the walk FlacBatch used to do in Python; both the Python and the session's paths call it.
 // some_midi_write is some_b200.midi.build_midi_file(...).to_bytes(), tick for tick.
+#include <limits.h>
 #include <math.h>
 #include <string.h>
 
@@ -14,6 +15,7 @@
 #include <string>
 #include <vector>
 
+#include "audio_walk.h"
 #include "host_common.h"
 
 #include "../../include/some_b200.h"
@@ -30,51 +32,6 @@ long long id3_size(const uint8_t* d, long long n) {
   if (n < 10 || memcmp(d, "ID3", 3) != 0) return 0;
   const long long size = (d[6] & 0x7F) << 21 | (d[7] & 0x7F) << 14 | (d[8] & 0x7F) << 7 | (d[9] & 0x7F);
   return 10 + size + ((d[5] & 0x10) ? 10 : 0);
-}
-
-// audio.parse_flac
-int flac_info(const uint8_t* d, long long n, long long off, some_audio_meta* m) {
-  long long p = off + 4;
-  bool first = true;
-  int min_bs = 0, max_bs = 0, rate = 0, channels = 0, bps = 0;
-  long long length = 0;
-  for (;;) {
-    SOME_REQUIRE(p + 4 <= n, "FLAC metadata block header truncated at byte offset %lld", p);
-    const int last = d[p] >> 7, kind = d[p] & 0x7F;
-    const long long size = (static_cast<long long>(d[p + 1]) << 16) | (d[p + 2] << 8) | d[p + 3];
-    SOME_REQUIRE(!(first && (kind != 0 || size != 34)),
-                 "FLAC stream does not start with a 34-byte STREAMINFO block (type %d, %lld bytes at byte offset %lld)", kind,
-                 size, p);
-    SOME_REQUIRE(first || (kind != 0 && kind != 127), "%s FLAC metadata block at byte offset %lld",
-                 kind == 0 ? "second STREAMINFO" : "invalid", p);
-    SOME_REQUIRE(p + 4 + size <= n, "FLAC metadata block truncated at byte offset %lld", p);
-    if (first) {
-      const uint8_t* b = d + p + 4;
-      min_bs = (b[0] << 8) | b[1];
-      max_bs = (b[2] << 8) | b[3];
-      rate = (b[10] << 12) | (b[11] << 4) | (b[12] >> 4);
-      channels = ((b[12] >> 1) & 7) + 1;
-      bps = (((b[12] & 1) << 4) | (b[13] >> 4)) + 1;
-      length = (static_cast<long long>(b[13] & 15) << 32) | (static_cast<long long>(b[14]) << 24) | (b[15] << 16) |
-               (b[16] << 8) | b[17];
-      first = false;
-    }
-    p += 4 + size;
-    if (last) break;
-  }
-  SOME_REQUIRE(bps <= 24,
-               "FLAC stream of %d bits per sample (at byte offset %lld); only up to 24 bits are decoded (libsndfile's float "
-               "scaling is exact up to 24 bits)",
-               bps, off + 8);
-  SOME_REQUIRE(rate != 0 && max_bs != 0, "invalid FLAC STREAMINFO (sample rate %d, max block size %d) at byte offset %lld", rate,
-               max_bs, off + 8);
-  m->container = SOME_AUDIO_FLAC;
-  m->rate = rate, m->channels = channels, m->bits = bps, m->kind = 0;
-  m->min_blocksize = min_bs, m->max_blocksize = max_bs;
-  m->frames = length;
-  m->data_offset = p;
-  m->data_bytes = n - p;
-  return 0;
 }
 
 // The container named in audio.decode_wav's refusal of a file that is not RIFF/WAVE.
@@ -94,113 +51,6 @@ std::string not_wave_kind(const uint8_t* d, long long n) {
   char hex[4];
   for (long long i = 0; i < h; ++i) snprintf(hex, sizeof(hex), " %02x", d[i]), s += hex;
   return s;
-}
-
-// scipy.io.wavfile.read's walk over a RIFF/WAVE file (little-endian RIFF only: audio.decode_wav refuses the rest first).
-// `pos` follows the file position scipy's reads and seeks leave, so the chunk loop ends where scipy's does.
-int wav_info(const uint8_t* d, long long n, some_audio_meta* m) {
-  const long long file_size = static_cast<long long>(le32(d + 4)) + 8;
-  long long pos = 12;
-  bool have_fmt = false, have_data = false;
-  int tag = 0, channels = 0, rate = 0, block_align = 0, bits = 0;
-  int d_kind = 0, d_channels = 0, d_bits = 0;
-  long long d_frames = 0, d_offset = 0, d_bytes = 0;
-  while (pos < file_size) {
-    const long long p = pos;
-    if (p >= n) {
-      SOME_REQUIRE(have_data, "RIFF/WAVE: Unexpected end of file. (at byte offset %lld)", p);
-      break;
-    }
-    if (n - p < 4) {
-      SOME_REQUIRE(have_fmt && have_data, "RIFF/WAVE: Incomplete chunk ID (at byte offset %lld)", p);
-      break;                                                     // scipy warns and stops at the end of the file
-    }
-    const uint8_t* id = d + p;
-    const bool is_fmt = memcmp(id, "fmt ", 4) == 0, is_data = memcmp(id, "data", 4) == 0;
-    if (!is_fmt && !is_data) {                                   // fact, LIST, JUNK, Fake and unknown chunks: skipped
-      if (n - p == 4) {
-        pos = n;
-        continue;
-      }
-      SOME_REQUIRE(n - p >= 8, "RIFF/WAVE: '%.4s' chunk size truncated at byte offset %lld", id, p);
-      const long long size = le32(d + p + 4);
-      pos = p + 8 + size + (size & 1);
-      continue;
-    }
-    SOME_REQUIRE(n - p >= 8, "RIFF/WAVE: '%.4s' chunk size truncated at byte offset %lld", id, p);
-    const long long size = le32(d + p + 4);
-    if (is_fmt) {
-      SOME_REQUIRE(size >= 16, "RIFF/WAVE: Binary structure of wave file is not compliant (fmt chunk of %lld bytes at byte offset "
-                   "%lld)", size, p);
-      SOME_REQUIRE(n - p >= 24, "RIFF/WAVE: fmt chunk truncated at byte offset %lld", p);
-      const uint8_t* b = d + p + 8;
-      tag = le16(b), channels = le16(b + 2), rate = static_cast<int>(le32(b + 4)), block_align = le16(b + 12);
-      bits = le16(b + 14);
-      const uint32_t byte_rate = le32(b + 8);
-      if (tag == 0xFFFE && size >= 18) {
-        SOME_REQUIRE(n - p >= 26, "RIFF/WAVE: fmt chunk truncated at byte offset %lld", p);
-        const int ext = le16(b + 16);
-        SOME_REQUIRE(ext >= 22, "RIFF/WAVE: Binary structure of wave file is not compliant (extension of %d bytes at byte "
-                     "offset %lld)", ext, p);
-        static const uint8_t tail[12] = {0x00, 0x00, 0x10, 0x00, 0x80, 0x00, 0x00, 0xAA, 0x00, 0x38, 0x9B, 0x71};
-        if (n - p >= 8 + 18 + 22 && memcmp(b + 18 + 6 + 4, tail, 12) == 0) tag = static_cast<int>(le32(b + 18 + 6));
-      }
-      SOME_REQUIRE(tag == 1 || tag == 3, "RIFF/WAVE: Unknown wave file format: %#06x. Supported formats: PCM, IEEE_FLOAT (fmt chunk "
-                   "at byte offset %lld)", tag, p);
-      pos = std::min(p + 8 + size, n) + (size & 1);
-      SOME_REQUIRE(tag != 1 || byte_rate == static_cast<uint32_t>(rate) * static_cast<uint32_t>(block_align),
-                   "RIFF/WAVE: WAV header is invalid: nAvgBytesPerSec must equal product of nSamplesPerSec and nBlockAlign, but "
-                   "file has nSamplesPerSec = %d, nBlockAlign = %d, and nAvgBytesPerSec = %u (fmt chunk at byte offset %lld)",
-                   rate, block_align, byte_rate, p);
-      have_fmt = true;
-      continue;
-    }
-    // data
-    SOME_REQUIRE(have_fmt, "RIFF/WAVE: No fmt chunk before data (data chunk at byte offset %lld)", p);
-    SOME_REQUIRE(channels > 0 && block_align / channels > 0,
-                 "RIFF/WAVE: %d channels in blocks of %d bytes (data chunk at byte offset %lld)", channels, block_align, p);
-    const int bps = block_align / channels;                     // scipy's container size
-    int kind = 0, isz = bps;
-    if (tag == 1) {
-      SOME_REQUIRE(bits <= 64, "RIFF/WAVE: Unsupported bit depth: the WAV file has %d-bit integer data. (data chunk at byte "
-                   "offset %lld)", bits, p);
-      if (bits >= 1 && bits <= 8) kind = bps == 1 ? SOME_PCM_U8 : 0, isz = 1;
-      else kind = bps == 2 ? SOME_PCM_S16 : bps == 3 ? SOME_PCM_S24 : bps == 4 ? SOME_PCM_S32 : 0;
-      SOME_REQUIRE(kind, "RIFF/WAVE: %d-bit PCM in %d-byte containers is not read (u8, s16, s24 and s32 are; data chunk at "
-                   "byte offset %lld)", bits, bps, p);
-    } else {
-      SOME_REQUIRE(bits == 32 || bits == 64, "RIFF/WAVE: Unsupported bit depth: the WAV file has %d-bit floating-point data. "
-                   "(data chunk at byte offset %lld)", bits, p);
-      kind = bps == 4 ? SOME_PCM_F32 : bps == 8 ? SOME_PCM_F64 : 0;
-      SOME_REQUIRE(kind, "RIFF/WAVE: %d-bit float in %d-byte containers (data chunk at byte offset %lld)", bits, bps, p);
-    }
-    const long long avail = n - (p + 8);
-    long long samples, consumed;
-    if (kind == SOME_PCM_S24) {                                  // read as raw bytes, then regrouped by three
-      consumed = std::min(size, avail);
-      SOME_REQUIRE(consumed % 3 == 0, "RIFF/WAVE: %lld bytes of 24-bit samples are not a whole number of samples (data chunk at "
-                   "byte offset %lld)", consumed, p);
-      samples = consumed / 3;
-    } else {
-      const long long want = size / bps;                        // items of isz bytes (u8: one byte each)
-      samples = std::min(want, avail / isz);
-      consumed = std::min(want * isz, avail);
-    }
-    SOME_REQUIRE(channels == 1 || samples % channels == 0,
-                 "RIFF/WAVE: %lld samples do not fill whole frames of %d channels (data chunk at byte offset %lld)", samples,
-                 channels, p);
-    have_data = true;
-    d_kind = kind, d_channels = channels, d_bits = bits;
-    d_frames = samples / channels, d_offset = p + 8, d_bytes = samples * isz;
-    pos = p + 8 + consumed + (size & 1);
-  }
-  SOME_REQUIRE(have_fmt, "RIFF/WAVE: no fmt chunk");
-  SOME_REQUIRE(have_data, "RIFF/WAVE: no data chunk");
-  m->container = SOME_AUDIO_WAV;
-  m->rate = rate, m->channels = d_channels, m->bits = d_bits, m->kind = d_kind;
-  m->min_blocksize = 0, m->max_blocksize = 0;
-  m->frames = d_frames, m->data_offset = d_offset, m->data_bytes = d_bytes;
-  return 0;
 }
 
 const char* flac_reason(int status, char* buf, size_t cap) {
@@ -230,19 +80,331 @@ void put_varlen(std::vector<uint8_t>& o, uint64_t v) {
 
 }  // namespace
 
+// ---------------------------------------------------------------------------------------------------- the container walk
+// The feed loop: the bytes [received_, e) arrive; r is the first of them not consumed yet.  Outside the audio, the step at
+// pos_ runs on the bytes [pos_, r) held in buf_ (bpos_ == pos_ when it runs) and either advances pos_, asks for more bytes
+// (need_ from pos_) or refuses.  Bytes below pos_ that were never held are skipped as they arrive.
+int AudioWalk::feed(const uint8_t* data, long long n, bool end, int* known, long long* audio_begin, long long* audio_end) {
+  SOME_REQUIRE(!failed_, "the walk was refused before");
+  held_audio_.clear();
+  const long long r0 = received_, e = received_ + n;
+  long long r = r0, ab = -1, ae = -1;
+  auto align = [&] {                     // buf_ starts at pos_ again
+    if (pos_ <= bpos_) return;
+    const size_t drop = static_cast<size_t>(std::min<long long>(pos_ - bpos_, static_cast<long long>(buf_.size())));
+    buf_.erase(buf_.begin(), buf_.begin() + drop);
+    bpos_ = pos_;
+  };
+  auto fail = [&] {
+    failed_ = true;
+    return -1;
+  };
+  for (;;) {
+    if (phase_ == kDone) {
+      r = e;
+      break;
+    }
+    if (phase_ == kWavData || phase_ == kFlacAudio) {
+      const long long stop = phase_ == kWavData ? d_end_ : LLONG_MAX, hi = std::min(stop, e);
+      if (hi > pos_) {
+        if (r > pos_)                    // audio bytes a step had looked ahead at
+          held_audio_.insert(held_audio_.end(), buf_.begin(), buf_.begin() + (std::min(r, hi) - pos_));
+        if (ab < 0) ab = pos_;
+        ae = hi;
+        pos_ = hi;
+        align();
+        r = std::max(r, hi);
+      }
+      if (phase_ == kFlacAudio) {
+        m_.data_bytes = e - m_.data_offset;
+        if (end) phase_ = kDone;
+        if (!end) break;
+        continue;
+      }
+      if (pos_ < stop && !end) break;
+      if (data_done(pos_ < stop ? e - d_begin_ : d_end_ - d_begin_)) return fail();
+      align();
+      continue;
+    }
+    if (pos_ > r) r = std::min(pos_, e);   // skipped bytes
+    const bool at_end = end && r == e;
+    if (pos_ > r && !at_end) break;
+    const int st = step(at_end, r);
+    if (st == kFailed) return fail();
+    if (st == kMore) {
+      if (r == e) break;                 // (at the end a step never asks for more)
+      const long long take = std::min(e, pos_ + need_) - r;
+      buf_.insert(buf_.end(), data + (r - r0), data + (r - r0) + take);
+      r += take;
+      continue;
+    }
+    align();
+  }
+  received_ = e;
+  *known = known_ ? 1 : 0;
+  *audio_begin = ab < 0 ? 0 : ab;
+  *audio_end = ab < 0 ? 0 : ae;
+  return 0;
+}
+
+// One structure at p = pos_: `n` is the end of the bytes that have arrived; q holds the bytes [p, n) (none when p > n, at the
+// end only).  Before the end, a rule that would read bytes past p + k or depend on where the file ends waits for k bytes.
+int AudioWalk::step(bool at_end, long long n) {
+  const long long p = pos_, avail = n - p;
+  const uint8_t* q = buf_.data();
+#define SOME_WAIT(k)                \
+  if (!at_end && avail < (k)) {     \
+    need_ = (k);                    \
+    return kMore;                   \
+  }
+  switch (phase_) {
+    case kStart: {
+      SOME_WAIT(12);
+      head_len_ = std::min<long long>(avail, 12);
+      memcpy(head_, q, static_cast<size_t>(head_len_));
+      pos_ = id3_size(q, avail);
+      phase_ = kMagic;
+      return kAdvanced;
+    }
+    case kMagic: {
+      SOME_WAIT(4);
+      if (avail >= 4 && memcmp(q, "fLaC", 4) == 0) {
+        flac_off_ = p;
+        pos_ = p + 4;
+        phase_ = kFlacBlock;
+        return kAdvanced;
+      }
+      SOME_REQUIRE(head_len_ >= 12 && memcmp(head_, "RIFF", 4) == 0 && memcmp(head_ + 8, "WAVE", 4) == 0,
+                   "not a RIFF/WAVE file (%s); some_b200.audio reads WAV files only", not_wave_kind(head_, head_len_).c_str());
+      file_size_ = static_cast<long long>(le32(head_ + 4)) + 8;
+      pos_ = 12;
+      phase_ = kWavChunk;
+      return kAdvanced;
+    }
+    // audio.parse_flac
+    case kFlacBlock:
+    case kFlacEnd: {
+      if (skipped_ >= 0) {                 // the skipped block ends at p
+        SOME_REQUIRE(n >= p, "FLAC metadata block truncated at byte offset %lld", skipped_);
+        skipped_ = -1;
+      }
+      if (phase_ == kFlacEnd) {
+        SOME_REQUIRE(bps_ <= 24,
+                     "FLAC stream of %d bits per sample (at byte offset %lld); only up to 24 bits are decoded (libsndfile's "
+                     "float scaling is exact up to 24 bits)",
+                     bps_, flac_off_ + 8);
+        SOME_REQUIRE(rate_ != 0 && max_bs_ != 0, "invalid FLAC STREAMINFO (sample rate %d, max block size %d) at byte offset %lld",
+                     rate_, max_bs_, flac_off_ + 8);
+        m_.container = SOME_AUDIO_FLAC;
+        m_.rate = rate_, m_.channels = channels_, m_.bits = bps_, m_.kind = 0;
+        m_.min_blocksize = min_bs_, m_.max_blocksize = max_bs_;
+        m_.frames = length_;
+        m_.data_offset = p;
+        m_.data_bytes = 0;
+        known_ = true;
+        phase_ = kFlacAudio;
+        return kAdvanced;
+      }
+      SOME_WAIT(4);
+      SOME_REQUIRE(avail >= 4, "FLAC metadata block header truncated at byte offset %lld", p);
+      const int last = q[0] >> 7, kind = q[0] & 0x7F;
+      const long long size = (static_cast<long long>(q[1]) << 16) | (q[2] << 8) | q[3];
+      SOME_REQUIRE(!(first_ && (kind != 0 || size != 34)),
+                   "FLAC stream does not start with a 34-byte STREAMINFO block (type %d, %lld bytes at byte offset %lld)", kind,
+                   size, p);
+      SOME_REQUIRE(first_ || (kind != 0 && kind != 127), "%s FLAC metadata block at byte offset %lld",
+                   kind == 0 ? "second STREAMINFO" : "invalid", p);
+      if (first_) {
+        SOME_WAIT(4 + size);
+        SOME_REQUIRE(avail >= 4 + size, "FLAC metadata block truncated at byte offset %lld", p);
+        const uint8_t* b = q + 4;
+        min_bs_ = (b[0] << 8) | b[1];
+        max_bs_ = (b[2] << 8) | b[3];
+        rate_ = (b[10] << 12) | (b[11] << 4) | (b[12] >> 4);
+        channels_ = ((b[12] >> 1) & 7) + 1;
+        bps_ = (((b[12] & 1) << 4) | (b[13] >> 4)) + 1;
+        length_ = (static_cast<long long>(b[13] & 15) << 32) | (static_cast<long long>(b[14]) << 24) | (b[15] << 16) |
+                  (b[16] << 8) | b[17];
+        first_ = false;
+      } else {
+        skipped_ = p;                      // its body is skipped, not held
+      }
+      pos_ = p + 4 + size;
+      if (last) phase_ = kFlacEnd;
+      return kAdvanced;
+    }
+    // scipy.io.wavfile.read's walk over a RIFF/WAVE file (little-endian RIFF only: audio.decode_wav refuses the rest first).
+    // pos_ follows the file position scipy's reads and seeks leave, so the chunk loop ends where scipy's does.
+    case kWavChunk: {
+      if (fmt_end_ >= 0) {                 // a fmt chunk cut short by the end of the file: scipy's position is the end
+        if (at_end && n < fmt_end_) pos_ = n + fmt_pad_;
+        fmt_end_ = -1;
+        if (pos_ != p) return kAdvanced;
+      }
+      if (p >= file_size_) return wav_done();
+      SOME_WAIT(8);
+      if (avail <= 0) {
+        SOME_REQUIRE(have_data_, "RIFF/WAVE: Unexpected end of file. (at byte offset %lld)", p);
+        return wav_done();
+      }
+      if (avail < 4) {
+        SOME_REQUIRE(have_fmt_ && have_data_, "RIFF/WAVE: Incomplete chunk ID (at byte offset %lld)", p);
+        return wav_done();                 // scipy warns and stops at the end of the file
+      }
+      const bool is_fmt = memcmp(q, "fmt ", 4) == 0, is_data = memcmp(q, "data", 4) == 0;
+      if (!is_fmt && !is_data) {           // fact, LIST, JUNK, Fake and unknown chunks: skipped
+        if (avail == 4) {
+          pos_ = n;
+          return kAdvanced;
+        }
+        SOME_REQUIRE(avail >= 8, "RIFF/WAVE: '%.4s' chunk size truncated at byte offset %lld", q, p);
+        const long long size = le32(q + 4);
+        pos_ = p + 8 + size + (size & 1);
+        return kAdvanced;
+      }
+      SOME_REQUIRE(avail >= 8, "RIFF/WAVE: '%.4s' chunk size truncated at byte offset %lld", q, p);
+      const long long size = le32(q + 4);
+      if (is_fmt) {
+        SOME_REQUIRE(!(stream_ && d_begin_), "RIFF/WAVE: a fmt chunk after the data chunk at byte offset %lld; an encoded stream "
+                     "takes its format from the fmt chunk before its data (a whole file is read with its last, as scipy reads it)",
+                     p);
+        SOME_REQUIRE(size >= 16, "RIFF/WAVE: Binary structure of wave file is not compliant (fmt chunk of %lld bytes at byte "
+                     "offset %lld)", size, p);
+        SOME_WAIT(24);
+        SOME_REQUIRE(avail >= 24, "RIFF/WAVE: fmt chunk truncated at byte offset %lld", p);
+        const uint8_t* b = q + 8;
+        int tag = le16(b);
+        channels_ = le16(b + 2), rate_ = static_cast<int>(le32(b + 4)), block_align_ = le16(b + 12), bits_ = le16(b + 14);
+        const uint32_t byte_rate = le32(b + 8);
+        if (tag == 0xFFFE && size >= 18) {
+          SOME_WAIT(26);
+          SOME_REQUIRE(avail >= 26, "RIFF/WAVE: fmt chunk truncated at byte offset %lld", p);
+          const int ext = le16(b + 16);
+          SOME_REQUIRE(ext >= 22, "RIFF/WAVE: Binary structure of wave file is not compliant (extension of %d bytes at byte "
+                       "offset %lld)", ext, p);
+          static const uint8_t tail[12] = {0x00, 0x00, 0x10, 0x00, 0x80, 0x00, 0x00, 0xAA, 0x00, 0x38, 0x9B, 0x71};
+          SOME_WAIT(8 + 18 + 22);
+          if (avail >= 8 + 18 + 22 && memcmp(b + 18 + 6 + 4, tail, 12) == 0) tag = static_cast<int>(le32(b + 18 + 6));
+        }
+        tag_ = tag;
+        SOME_REQUIRE(tag == 1 || tag == 3, "RIFF/WAVE: Unknown wave file format: %#06x. Supported formats: PCM, IEEE_FLOAT (fmt "
+                     "chunk at byte offset %lld)", tag, p);
+        SOME_REQUIRE(tag != 1 || byte_rate == static_cast<uint32_t>(rate_) * static_cast<uint32_t>(block_align_),
+                     "RIFF/WAVE: WAV header is invalid: nAvgBytesPerSec must equal product of nSamplesPerSec and nBlockAlign, "
+                     "but file has nSamplesPerSec = %d, nBlockAlign = %d, and nAvgBytesPerSec = %u (fmt chunk at byte offset "
+                     "%lld)", rate_, block_align_, byte_rate, p);
+        fmt_end_ = p + 8 + size, fmt_pad_ = size & 1;
+        pos_ = fmt_end_ + fmt_pad_;
+        have_fmt_ = true;
+        return kAdvanced;
+      }
+      // data
+      SOME_REQUIRE(!(stream_ && d_begin_), "RIFF/WAVE: a second data chunk at byte offset %lld; an encoded stream reads one data "
+                   "chunk (a whole file is read to its last, as scipy reads it)", p);
+      SOME_REQUIRE(have_fmt_, "RIFF/WAVE: No fmt chunk before data (data chunk at byte offset %lld)", p);
+      SOME_REQUIRE(channels_ > 0 && block_align_ / channels_ > 0,
+                   "RIFF/WAVE: %d channels in blocks of %d bytes (data chunk at byte offset %lld)", channels_, block_align_, p);
+      const int bps = block_align_ / channels_;   // scipy's container size
+      int kind = 0, isz = bps;
+      if (tag_ == 1) {
+        SOME_REQUIRE(bits_ <= 64, "RIFF/WAVE: Unsupported bit depth: the WAV file has %d-bit integer data. (data chunk at byte "
+                     "offset %lld)", bits_, p);
+        if (bits_ >= 1 && bits_ <= 8) kind = bps == 1 ? SOME_PCM_U8 : 0, isz = 1;
+        else kind = bps == 2 ? SOME_PCM_S16 : bps == 3 ? SOME_PCM_S24 : bps == 4 ? SOME_PCM_S32 : 0;
+        SOME_REQUIRE(kind, "RIFF/WAVE: %d-bit PCM in %d-byte containers is not read (u8, s16, s24 and s32 are; data chunk at "
+                     "byte offset %lld)", bits_, bps, p);
+      } else {
+        SOME_REQUIRE(bits_ == 32 || bits_ == 64, "RIFF/WAVE: Unsupported bit depth: the WAV file has %d-bit floating-point data. "
+                     "(data chunk at byte offset %lld)", bits_, p);
+        kind = bps == 4 ? SOME_PCM_F32 : bps == 8 ? SOME_PCM_F64 : 0;
+        SOME_REQUIRE(kind, "RIFF/WAVE: %d-bit float in %d-byte containers (data chunk at byte offset %lld)", bits_, bps, p);
+      }
+      d_kind_ = kind, d_channels_ = channels_, d_bits_ = bits_, d_isz_ = isz, d_bps_ = bps, d_size_ = size;
+      d_begin_ = p + 8;
+      d_end_ = d_begin_ + (kind == SOME_PCM_S24 ? size : size / bps * isz);   // whole items of the stated size
+      m_.container = SOME_AUDIO_WAV;
+      m_.rate = rate_, m_.channels = channels_, m_.bits = bits_, m_.kind = kind;
+      m_.min_blocksize = 0, m_.max_blocksize = 0;
+      m_.frames = (d_end_ - d_begin_) / isz / channels_, m_.data_offset = d_begin_, m_.data_bytes = d_end_ - d_begin_;
+      known_ = true;
+      pos_ = d_begin_;
+      phase_ = kWavData;
+      return kAdvanced;
+    }
+    default:
+      return kAdvanced;
+  }
+#undef SOME_WAIT
+}
+
+// The data chunk ends: all its stated bytes arrived, or the file ended `avail` bytes into it.
+int AudioWalk::data_done(long long avail) {
+  const long long p = d_begin_ - 8;
+  long long samples, consumed;
+  if (d_kind_ == SOME_PCM_S24) {         // read as raw bytes, then regrouped by three
+    consumed = std::min(d_size_, avail);
+    SOME_REQUIRE(consumed % 3 == 0, "RIFF/WAVE: %lld bytes of 24-bit samples are not a whole number of samples (data chunk at "
+                 "byte offset %lld)", consumed, p);
+    samples = consumed / 3;
+  } else {
+    const long long want = d_size_ / d_bps_;            // items of isz bytes (u8: one byte each)
+    samples = std::min(want, avail / d_isz_);
+    consumed = std::min(want * d_isz_, avail);
+  }
+  SOME_REQUIRE(d_channels_ == 1 || samples % d_channels_ == 0,
+               "RIFF/WAVE: %lld samples do not fill whole frames of %d channels (data chunk at byte offset %lld)", samples,
+               d_channels_, p);
+  have_data_ = true;
+  d_frames_ = samples / d_channels_, d_offset_ = d_begin_, d_bytes_ = samples * d_isz_;
+  m_.frames = d_frames_, m_.data_bytes = d_bytes_;
+  pos_ = d_begin_ + consumed + (d_size_ & 1);
+  phase_ = kWavChunk;
+  return 0;
+}
+
+// The chunk loop ends.
+int AudioWalk::wav_done() {
+  SOME_REQUIRE(have_fmt_, "RIFF/WAVE: no fmt chunk");
+  SOME_REQUIRE(have_data_, "RIFF/WAVE: no data chunk");
+  m_.container = SOME_AUDIO_WAV;
+  m_.rate = rate_, m_.channels = d_channels_, m_.bits = d_bits_, m_.kind = d_kind_;
+  m_.min_blocksize = 0, m_.max_blocksize = 0;
+  m_.frames = d_frames_, m_.data_offset = d_offset_, m_.data_bytes = d_bytes_;
+  known_ = true;
+  phase_ = kDone;
+  return kAdvanced;
+}
+
 extern "C" int some_audio_info(const void* data, long long n_bytes, some_audio_meta* out) {
   SOME_REQUIRE(out != nullptr && n_bytes >= 0 && (data != nullptr || n_bytes == 0), "some_audio_info: bad arguments");
-  const uint8_t* d = static_cast<const uint8_t*>(data);
-  some_audio_meta m{};
-  const long long off = id3_size(d, n_bytes);
-  if (off + 4 <= n_bytes && memcmp(d + off, "fLaC", 4) == 0) {
-    if (flac_info(d, n_bytes, off, &m)) return -1;
-  } else {
-    SOME_REQUIRE(n_bytes >= 12 && memcmp(d, "RIFF", 4) == 0 && memcmp(d + 8, "WAVE", 4) == 0,
-                 "not a RIFF/WAVE file (%s); some_b200.audio reads WAV files only", not_wave_kind(d, n_bytes).c_str());
-    if (wav_info(d, n_bytes, &m)) return -1;
-  }
-  *out = m;
+  AudioWalk w(false);
+  int known;
+  long long a, b;
+  if (w.feed(static_cast<const uint8_t*>(data), n_bytes, true, &known, &a, &b)) return -1;
+  *out = w.meta();
+  return 0;
+}
+
+struct some_audio_walk {
+  AudioWalk w;
+  explicit some_audio_walk(bool stream) : w(stream) {}
+};
+extern "C" int some_audio_walk_create(int stream, some_audio_walk** out) {
+  SOME_REQUIRE(out != nullptr, "some_audio_walk_create: null pointer");
+  *out = new some_audio_walk(stream != 0);
+  return 0;
+}
+extern "C" int some_audio_walk_feed(some_audio_walk* w, const void* data, long long n_bytes, int end, int* known,
+                                    some_audio_meta* meta, long long* audio_begin, long long* audio_end, long long* held) {
+  SOME_REQUIRE(w != nullptr && known && meta && audio_begin && audio_end && n_bytes >= 0 && (data != nullptr || n_bytes == 0),
+               "some_audio_walk_feed: bad arguments");
+  if (w->w.feed(static_cast<const uint8_t*>(data), n_bytes, end != 0, known, audio_begin, audio_end)) return -1;
+  *meta = w->w.meta();
+  if (held) *held = w->w.held();
+  return 0;
+}
+extern "C" int some_audio_walk_destroy(some_audio_walk* w) {
+  delete w;
   return 0;
 }
 
@@ -254,55 +416,72 @@ extern "C" int some_flac_chain(const some_flac_frame* frames, int n_frames, cons
   if (failed) *failed = -1;
   int i = 0, k = 0;
   first[0] = 0;
-  char buf[16];
   for (int r = 0; r < n_recs; ++r) {
-    const long long base = recs[r].base, stop = recs[r].end, total = recs[r].length;
-    long long p = recs[r].audio_start, got = 0, count = 0;
-    int strategy = -1;
-    auto fail = [&]() {
+    FlacWalk w;
+    w.pos = recs[r].audio_start - recs[r].base;
+    if (flac_walk(frames, n_frames, &i, recs[r].base, recs[r].end, recs[r].length, true, &w, chain, capacity, &k)) {
       if (failed) *failed = r;
       return -1;
-    };
-    while (!(total && got == total) && !(!total && p == stop)) {
-      if (p >= stop) {
-        set_error("FLAC stream ends at byte offset %lld after %lld of %lld samples", p - base, got, total);
-        return fail();
-      }
-      while (i < n_frames && frames[i].pos < p) ++i;
-      if (i >= n_frames || frames[i].pos != p) {
-        set_error("no valid FLAC frame header (sync, reserved code, CRC-8 or STREAMINFO mismatch) at byte offset %lld", p - base);
-        return fail();
-      }
-      const some_flac_frame& f = frames[i];
-      if (f.status) {
-        set_error("FLAC frame at byte offset %lld: %s (at byte offset %lld)", p - base, flac_reason(f.status, buf, sizeof(buf)),
-                  static_cast<long long>(f.end) - base);
-        return fail();
-      }
-      if (strategy < 0) strategy = f.variable;
-      const long long want = f.variable ? got : count;
-      if (f.variable != strategy || f.number != want) {
-        set_error("FLAC frame at byte offset %lld: %s number %lld, expected %lld (gap, overlap or changed blocking strategy)",
-                  p - base, f.variable ? "sample" : "frame", static_cast<long long>(f.number), want);
-        return fail();
-      }
-      got += f.blocksize;
-      if (total && got > total) {
-        set_error("FLAC frame at byte offset %lld decodes past the %lld samples STREAMINFO states", p - base, total);
-        return fail();
-      }
-      if (k >= capacity) {
-        set_error("some_flac_chain: more than %d chained frames", capacity);
-        return fail();
-      }
-      chain[k++] = i;
-      ++count;
-      p = f.end;
     }
     first[r + 1] = k;
-    lengths[r] = got;
+    lengths[r] = w.got;
   }
   return 0;
+}
+
+int some::flac_walk(const some_flac_frame* frames, int n_frames, int* i, long long base, long long stop, long long total,
+                    bool final, FlacWalk* w, int32_t* chain, int capacity, int* k) {
+  char buf[16];
+  long long p = base + w->pos;
+  for (;;) {
+    if ((total && w->got == total) || (!total && p == stop && final)) {
+      w->done = true;
+      break;
+    }
+    if (p >= stop) {
+      if (!final) break;
+      SOME_REQUIRE(false, "FLAC stream ends at byte offset %lld after %lld of %lld samples", p - base, w->got, total);
+    }
+    while (*i < n_frames && frames[*i].pos < p) ++*i;
+    if (*i >= n_frames || frames[*i].pos != p) {
+      if (!final && stop - p < 16) break;        // the header may not have arrived yet
+      SOME_REQUIRE(false, "no valid FLAC frame header (sync, reserved code, CRC-8 or STREAMINFO mismatch) at byte offset %lld",
+                   p - base);
+    }
+    const some_flac_frame& f = frames[*i];
+    if (f.status) {
+      if (!final && f.status == SOME_FLAC_TRUNCATED) break;   // its window ends inside it
+      SOME_REQUIRE(false, "FLAC frame at byte offset %lld: %s (at byte offset %lld)", p - base,
+                   flac_reason(f.status, buf, sizeof(buf)), static_cast<long long>(f.end) - base);
+    }
+    if (w->strategy < 0) w->strategy = f.variable;
+    const long long want = f.variable ? w->got : w->count;
+    SOME_REQUIRE(f.variable == w->strategy && f.number == want,
+                 "FLAC frame at byte offset %lld: %s number %lld, expected %lld (gap, overlap or changed blocking strategy)",
+                 p - base, f.variable ? "sample" : "frame", static_cast<long long>(f.number), want);
+    SOME_REQUIRE(!total || w->got + f.blocksize <= total,
+                 "FLAC frame at byte offset %lld decodes past the %lld samples STREAMINFO states", p - base, total);
+    SOME_REQUIRE(*k < capacity, "some_flac_chain: more than %d chained frames", capacity);
+    w->got += f.blocksize;
+    chain[(*k)++] = *i;
+    ++w->count;
+    p = f.end;
+    w->pos = p - base;
+  }
+  return 0;
+}
+
+extern "C" int some_flac_chain_resume(const some_flac_frame* frames, int n_frames, int64_t base, int64_t stop, int64_t length,
+                                      int final, some_flac_walk* walk, int32_t* chain, int capacity, int* n_chained) {
+  SOME_REQUIRE((frames || n_frames == 0) && walk && n_chained && (chain || capacity == 0) && n_frames >= 0 && capacity >= 0,
+               "some_flac_chain_resume: bad arguments");
+  FlacWalk w;
+  w.pos = walk->pos, w.got = walk->got, w.count = walk->count, w.strategy = walk->strategy, w.done = walk->done != 0;
+  int i = 0;
+  *n_chained = 0;
+  const int rc = w.done ? 0 : flac_walk(frames, n_frames, &i, base, stop, length, final != 0, &w, chain, capacity, n_chained);
+  walk->pos = w.pos, walk->got = w.got, walk->count = w.count, walk->strategy = w.strategy, walk->done = w.done;
+  return rc;
 }
 
 extern "C" int some_midi_write(int n_chunks, const double* offsets, const int32_t* counts, const float* note_midi,

@@ -32,6 +32,7 @@
 #include <vector>
 
 #include "../../include/some_b200.h"
+#include "audio_walk.h"
 
 using namespace some;
 
@@ -998,6 +999,13 @@ struct some_stream {
   int64_t head_len = 0;
   int64_t received = 0, fixed = 0, frames = 0;   // frames: RMS frames computed so far
   bool finished = false;
+  // an encoded stream (some_stream_open_encoded; rate 0 until its header is complete): the container walk, the audio bytes
+  // not decoded yet (file offsets [pend_pos, pend_pos + size): an incomplete FLAC frame or WAV sample frame) and the chain
+  std::unique_ptr<AudioWalk> walk;
+  bool failed = false;                    // refused on its content
+  std::vector<uint8_t> pending;
+  long long pend_pos = 0;
+  FlacWalk fw;
 };
 
 namespace {
@@ -1017,6 +1025,77 @@ struct StepItem {
   int64_t up = 0;               // where its samples lie in the upload (floats)
   int64_t rms0 = 0, nf = 0;     // its new RMS frames in the session's RMS buffer
   int c0 = 0, c1 = 0;           // its chunks in the step's batch
+  bool dropped = false;         // its samples failed to decode: no slicer decisions, no chunks
+};
+
+// The decode stage in front of an encoded step (samples == NULL in its items): the samples are decoded on the device into
+// the upload's sample region, which the step's scatter reads.  Its descriptors go into the step's upload:
+//   add     the regions of the PCM descriptors, the chained FLAC frames (their scratch and output offsets) and the status;
+//   fill    after the step has placed each item's samples: the descriptors, with those places;
+//   launch  after the upload is sent, in front of the scatter: one some_pcm_decode, one FLAC decode, the status download;
+//   check   after the synchronise: the item whose frame failed to decode, if one did, is dropped.
+struct StepDecode {
+  const uint8_t* bytes_d = nullptr;              // the bytes upload
+  const some_flac_stream* streams_d = nullptr;   // its FLAC windows
+  const some_flac_frame* frames_h = nullptr;     // the candidates, on the host and on the device
+  const some_flac_frame* frames_d = nullptr;
+  std::vector<some_pcm_item> pcm;                // out: an offset in the item's samples until fill()
+  std::vector<int> pcm_of, flac_of;              // the step item of each PCM entry and of each FLAC window
+  std::vector<int64_t> first{0};                 // FLAC window r's frames: chain[first[r] .. first[r + 1])
+  std::vector<int32_t> chain;
+  std::vector<int> channels;
+  std::vector<long long> base;                   // FLAC window r: file offset x lies at x + base[r] in the bytes upload
+  int failed_item = -1;                          // check(): the dropped item, and where its frame lies
+  long long failed_pos = 0;
+  int failed_status = 0;
+  size_t pcm_off = 0, chain_off = 0, soff_off = 0, ooff_off = 0, status_off = 0;
+
+  void add(Upload& up) {
+    const size_t n = chain.size();
+    pcm_off = up.add(static_cast<size_t>(some_pcm_decode_bytes(static_cast<int>(pcm.size()))));
+    chain_off = up.add(4 * n), soff_off = up.add(8 * n), ooff_off = up.add(8 * n), status_off = up.add(2 * sizeof(int));
+  }
+  int fill(some_session* s, const Upload& up, float* samples_d, const std::vector<StepItem>& items) {
+    for (size_t j = 0; j < pcm.size(); ++j) pcm[j].out = samples_d + items[pcm_of[j]].up;
+    int64_t* soff = reinterpret_cast<int64_t*>(up.h(soff_off));
+    int64_t* ooff = reinterpret_cast<int64_t*>(up.h(ooff_off));
+    int64_t scratch = 0;
+    for (size_t r = 0; r < flac_of.size(); ++r) {
+      int64_t o = items[flac_of[r]].up;
+      for (int64_t j = first[r]; j < first[r + 1]; ++j) {
+        const int bs = frames_h[chain[j]].blocksize;
+        soff[j] = scratch, ooff[j] = o;
+        scratch += static_cast<int64_t>(bs) * channels[r], o += bs;
+      }
+    }
+    if (s->flac_scratch_d.ensure(4ull * scratch + 16, "the FLAC scratch") ||
+        some_pcm_decode_pack(pcm.data(), static_cast<int>(pcm.size()), up.h(pcm_off)))
+      return -1;
+    if (!chain.empty()) memcpy(up.h(chain_off), chain.data(), 4 * chain.size());
+    int* status = reinterpret_cast<int*>(up.h(status_off));
+    status[0] = 0, status[1] = INT_MAX;
+    return 0;
+  }
+  int launch(some_session* s, const Upload& up, float* samples_d) const {
+    if (some_pcm_decode(up.h(pcm_off), up.d(pcm_off), s->stream)) return -1;
+    if (chain.empty()) return 0;
+    int* status_d = reinterpret_cast<int*>(up.d(status_off));
+    if (flac_decode_chain(bytes_d, streams_d, frames_d, reinterpret_cast<const int32_t*>(up.d(chain_off)),
+                          reinterpret_cast<const int64_t*>(up.d(soff_off)), reinterpret_cast<const int64_t*>(up.d(ooff_off)),
+                          static_cast<int>(chain.size()), static_cast<int32_t*>(s->flac_scratch_d.p), samples_d, 1, status_d,
+                          status_d + 1, s->stream))
+      return -1;
+    SOME_CUDA(cudaMemcpyAsync(up.h(status_off), status_d, 2 * sizeof(int), cudaMemcpyDeviceToHost, s->stream), "status download");
+    return 0;
+  }
+  void check(const Upload& up, std::vector<StepItem>& items) {
+    const int* status = reinterpret_cast<const int*>(up.h(status_off));
+    if (chain.empty() || status[0] == 0) return;
+    size_t r = 0;
+    while (r + 1 < flac_of.size() && first[r + 1] <= status[1]) ++r;
+    failed_item = flac_of[r], failed_pos = frames_h[chain[status[1]]].pos - base[r], failed_status = status[0];
+    items[failed_item].dropped = true;
+  }
 };
 
 // One step of any number of streams of one session, under the session's mutex.  Each stream does what a push of its samples
@@ -1028,7 +1107,7 @@ struct StepItem {
 //      synchronise;
 //   3. the slicer's decisions for each stream;
 //   4. every chunk that became final, in any stream, copied next to each other and transcribed as one batch.
-int streams_step(some_session* s, std::vector<StepItem>& items) {
+int streams_step(some_session* s, std::vector<StepItem>& items, StepDecode* dec = nullptr) {
   const int sr = s->info.sample_rate;
   std::vector<some_resample_window> rs;
   std::vector<some_rms_window> rm;
@@ -1096,6 +1175,7 @@ int streams_step(some_session* s, std::vector<StepItem>& items) {
   const size_t sc_off = up.add(windows_bytes<ScatterParams>(ks));
   const size_t rs_off = up.add(static_cast<size_t>(some_resample_windows_bytes(kr)));
   const size_t rm_off = up.add(static_cast<size_t>(some_slicer_rms_windows_bytes(km)));
+  if (dec) dec->add(up);
   if (up.reserve("the stream upload") || s->rms_d.ensure(4ull * frames + 16, "the RMS frames") ||
       s->rms_h.ensure(4ull * frames + 16, "the RMS frames"))
     return -1;
@@ -1109,7 +1189,7 @@ int streams_step(some_session* s, std::vector<StepItem>& items) {
         ps[j] = sc[j];
         ps[j].src = reinterpret_cast<const float*>(up.d(smp_off)) + it.up;
         tile0[j + 1] = (it.n + kScatterTile - 1) / kScatterTile;
-        spans.push_back({reinterpret_cast<float*>(up.h(smp_off)) + it.up, it.samples, 4ull * it.n});
+        if (it.samples) spans.push_back({reinterpret_cast<float*>(up.h(smp_off)) + it.up, it.samples, 4ull * it.n});
         ++j;
       }
     windows_index(up.h(sc_off), ks, 0);
@@ -1118,8 +1198,10 @@ int streams_step(some_session* s, std::vector<StepItem>& items) {
     rm[j].rms = static_cast<float*>(s->rms_d.p) + at;
   if (some_resample_windows_pack(rs.data(), kr, up.h(rs_off)) || some_slicer_rms_windows_pack(rm.data(), km, up.h(rm_off)))
     return -1;
+  float* samples_d = reinterpret_cast<float*>(up.d(smp_off));
+  if (dec && dec->fill(s, up, samples_d, items)) return -1;
   copy_to_pinned(*s->pool, spans, size_t(1) << 20);          // the samples, in pieces of up to 1 MB
-  if (up.send("stream upload")) return -1;
+  if (up.send("stream upload") || (dec && dec->launch(s, up, samples_d))) return -1;
   if (ks) {
     const WindowsHeader& h = *reinterpret_cast<const WindowsHeader*>(up.h(sc_off));
     scatter_kernel<<<static_cast<unsigned>(h.tiles), kScatterThreads, 0, s->stream>>>(
@@ -1132,12 +1214,15 @@ int streams_step(some_session* s, std::vector<StepItem>& items) {
   if (frames)
     SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames, cudaMemcpyDeviceToHost, s->stream), "RMS download");
   SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");   // also frees the upload buffer for the next step
+  if (dec) dec->check(up, items);
 
   // the slicer's decisions, and where each chunk that became final lies
   std::vector<const float*> src;
   std::vector<int64_t> begin, lens;
   for (StepItem& it : items) {
     some_stream* st = it.st;
+    it.c0 = it.c1 = static_cast<int>(begin.size());
+    if (it.dropped) continue;
     st->frames += it.nf;
     const float* rms = static_cast<const float*>(s->rms_h.p) + it.rms0;
     const int64_t* ranges = nullptr;
@@ -1182,6 +1267,216 @@ int stream_call(some_stream* st, const float* samples, int64_t n, bool final, so
   std::vector<StepItem> items{StepItem{st, samples, n, final, out}};
   return locked(st->s, [&] { return streams_step(st->s, items); });
 }
+
+// One encoded stream's part of a step: its new bytes, whether the file ends there, and where its chunks go.
+struct ByteItem {
+  some_stream* st;
+  const uint8_t* data;
+  long long n;
+  bool final;
+  some_notes* out;
+  int index;                    // in a many-call (-1: a single call)
+  bool live = true;             // false once refused
+  int64_t up = 0, win = 0;      // its window in the bytes upload: the pending bytes that go up
+  int64_t samples = 0;          // the samples it decodes in this step
+  int fi = -1;                  // FLAC: its window in the step's decode
+};
+
+// A step of encoded streams (some_stream_push_bytes*, some_stream_finish), under the session's mutex:
+//   1. on the host, each stream's walk consumes its bytes; their audio joins the stream's pending bytes;
+//   2. one pinned upload of the FLAC windows (the pending bytes from each stream's first unchained frame) and the whole WAV
+//      sample frames;
+//   3. with FLAC streams: one some_flac_scan over all windows, one download of the candidates, one synchronise, then each
+//      stream's resumable chain;
+//   4. streams_step with the decode stage in front: one some_pcm_decode and one FLAC decode, mono, into the region its scatter
+//      reads.
+// A stream refused on its content (its walk, its chain, a decode failure, a rate or channel count the session cannot take)
+// leaves the step; the others go on, and the call then fails with the first refusal.
+int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
+  const int sr = s->info.sample_rate;
+  std::string refusal;
+  auto refuse = [&](ByteItem& b) {
+    b.st->failed = true, b.live = false;
+    if (!refusal.empty()) return;
+    char pre[128];
+    if (b.index < 0) snprintf(pre, sizeof(pre), "%s: ", who);
+    else snprintf(pre, sizeof(pre), "%s: stream %d: ", who, b.index);
+    refusal = std::string(pre) + some_last_error();
+  };
+  auto too_short = [&](ByteItem& b) {    // resampy's refusal, at the end of a file at another rate
+    const some_stream* st = b.st;
+    if (!b.final || !st->resample || (st->received + b.samples) * sr / st->rate >= 1) return false;
+    set_error("Input signal length=%lld is too small to resample from %d->%d", static_cast<long long>(st->received + b.samples),
+              st->rate, sr);
+    refuse(b);
+    return true;
+  };
+  // 1. the walks
+  for (ByteItem& b : bs) {
+    some_stream* st = b.st;
+    int known;
+    long long a0, a1;
+    if (st->walk->feed(b.data, b.n, b.final, &known, &a0, &a1)) {
+      refuse(b);
+      continue;
+    }
+    if (!known) continue;
+    const some_audio_meta& m = st->walk->meta();
+    if (st->rate == 0) {                 // this push completes the header
+      if (m.container == SOME_AUDIO_WAV && m.channels > 128) {
+        set_error("a mono down-mix of %d channels (at most 128)", m.channels);
+        refuse(b);
+        continue;
+      }
+      long long t_end, x_first;
+      if (m.rate != sr && some_resample_window_plan(0, 0, 0, m.rate, sr, kKaiserTaps, &t_end, &x_first)) {
+        refuse(b);
+        continue;
+      }
+      st->rate = m.rate, st->resample = m.rate != sr;
+      st->pend_pos = st->fw.pos = m.data_offset;
+    }
+    if (a1 > a0 && !st->fw.done) {       // its audio bytes join the pending ones
+      const std::vector<uint8_t>& held = st->walk->held_audio();
+      st->pending.insert(st->pending.end(), held.begin(), held.end());
+      const long long from = a0 + static_cast<long long>(held.size()), r0 = st->walk->received() - b.n;
+      if (a1 > from) st->pending.insert(st->pending.end(), b.data + (from - r0), b.data + (a1 - r0));
+    }
+  }
+  // 2. the bytes upload: the FLAC windows first (the scan covers only them), the WAV frames, the FLAC window descriptors
+  std::vector<ByteItem*> flac, wav;
+  for (ByteItem& b : bs)
+    if (b.live && b.st->rate) (b.st->walk->meta().container == SOME_AUDIO_FLAC ? flac : wav).push_back(&b);
+  int64_t at = 0;
+  for (ByteItem* b : flac) b->up = at, b->win = static_cast<int64_t>(b->st->pending.size()), at += align16(b->win);
+  const int64_t flac_bytes = at;
+  for (ByteItem* b : wav) {
+    const some_audio_meta& m = b->st->walk->meta();
+    static const int kBytes[7] = {0, 1, 2, 3, 4, 4, 8};
+    const int64_t frame = static_cast<int64_t>(m.channels) * kBytes[m.kind];
+    b->samples = static_cast<int64_t>(b->st->pending.size()) / frame;
+    b->win = b->samples * frame;
+    if (too_short(*b)) continue;
+    b->up = at, at += align16(b->win);
+  }
+  const int nf = static_cast<int>(flac.size());
+  const int64_t streams_off = at, up_bytes = at + static_cast<int64_t>(sizeof(some_flac_stream)) * nf;
+  if (s->enc_h.ensure(up_bytes + 16, "the encoded streams") || s->enc_d.ensure(up_bytes + 16, "the encoded streams")) return -1;
+  uint8_t* up_h = static_cast<uint8_t*>(s->enc_h.p);
+  const uint8_t* up_d = static_cast<const uint8_t*>(s->enc_d.p);
+  std::vector<HostSpan> spans;
+  for (ByteItem* b : flac) spans.push_back({up_h + b->up, b->st->pending.data(), static_cast<size_t>(b->win)});
+  for (ByteItem* b : wav)
+    if (b->live) spans.push_back({up_h + b->up, b->st->pending.data(), static_cast<size_t>(b->win)});
+  copy_to_pinned(*s->pool, spans, size_t(1) << 20);
+  some_flac_stream* win_h = reinterpret_cast<some_flac_stream*>(up_h + streams_off);
+  for (int r = 0; r < nf; ++r) {
+    const some_audio_meta& m = flac[r]->st->walk->meta();
+    win_h[r] = some_flac_stream{flac[r]->up, flac[r]->up + flac[r]->win, m.channels, m.bits, m.max_blocksize, 0};
+  }
+  if (up_bytes) SOME_CUDA(cudaMemcpyAsync(s->enc_d.p, up_h, static_cast<size_t>(up_bytes), cudaMemcpyHostToDevice, s->stream),
+                          "encoded upload");
+  StepDecode dec;
+  dec.bytes_d = up_d, dec.streams_d = reinterpret_cast<const some_flac_stream*>(up_d + streams_off);
+  // 3. the FLAC frames: one scan, the candidates down (again, larger, only if the estimate was short), the chains on the host
+  if (nf) {
+    int64_t cap = 64;
+    for (ByteItem* b : flac) cap += b->win / 64 + 8;
+    const uint64_t ws_bytes = some_flac_scan_workspace_bytes(flac_bytes);
+    if (s->flac_ws_d.ensure(ws_bytes + 16, "the FLAC scan workspace")) return -1;
+    int* count_d = reinterpret_cast<int*>(static_cast<char*>(s->flac_ws_d.p) + ws_bytes);
+    int n_cand = 0;
+    for (;;) {
+      SOME_REQUIRE(cap < (int64_t(1) << 31), "%s: too many FLAC frame candidates in one step", who);
+      if (s->flac_frames_d.ensure(sizeof(some_flac_frame) * cap, "the FLAC frames") ||
+          s->flac_frames_h.ensure(sizeof(some_flac_frame) * cap + 16, "the FLAC frames"))
+        return -1;
+      char* fh = static_cast<char*>(s->flac_frames_h.p);
+      if (some_flac_scan(up_d, flac_bytes, dec.streams_d, nf, static_cast<some_flac_frame*>(s->flac_frames_d.p),
+                         static_cast<int>(cap), count_d, s->flac_ws_d.p, s->stream))
+        return -1;
+      SOME_CUDA(cudaMemcpyAsync(fh, count_d, sizeof(int), cudaMemcpyDeviceToHost, s->stream), "count download");
+      SOME_CUDA(cudaMemcpyAsync(fh + 16, s->flac_frames_d.p, sizeof(some_flac_frame) * cap, cudaMemcpyDeviceToHost, s->stream),
+                "candidate download");
+      SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+      n_cand = *reinterpret_cast<const int*>(fh);
+      if (n_cand <= cap) break;
+      cap = n_cand;
+    }
+    dec.frames_h = reinterpret_cast<const some_flac_frame*>(static_cast<char*>(s->flac_frames_h.p) + 16);
+    dec.frames_d = static_cast<const some_flac_frame*>(s->flac_frames_d.p);
+    dec.chain.resize(std::max(n_cand, 1));
+    int i = 0, k = 0;
+    for (ByteItem* b : flac) {
+      some_stream* st = b->st;
+      const some_audio_meta& m = st->walk->meta();
+      const int k0 = k;
+      const long long base = b->up - st->pend_pos;
+      if (flac_walk(dec.frames_h, n_cand, &i, base, b->up + b->win, m.frames, b->final, &st->fw, dec.chain.data(), n_cand, &k)) {
+        k = k0;
+        refuse(*b);
+        continue;
+      }
+      for (int j = k0; j < k; ++j) b->samples += dec.frames_h[dec.chain[j]].blocksize;
+      // the bytes before the next frame are decoded (or, once the walk is done, past the recording)
+      const long long keep = st->fw.done ? st->pend_pos + static_cast<long long>(st->pending.size()) : st->fw.pos;
+      st->pending.erase(st->pending.begin(), st->pending.begin() + (keep - st->pend_pos));
+      st->pend_pos = keep;
+      if (too_short(*b)) {
+        k = k0;
+        continue;
+      }
+      if (k > k0) {
+        b->fi = static_cast<int>(dec.flac_of.size());
+        dec.flac_of.push_back(-1);       // its step item, below
+        dec.first.push_back(k);
+        dec.channels.push_back(m.channels);
+        dec.base.push_back(base);
+      }
+    }
+    dec.chain.resize(k);
+  }
+  for (ByteItem* b : wav) {
+    if (!b->live) continue;
+    b->st->pending.erase(b->st->pending.begin(), b->st->pending.begin() + b->win);
+    b->st->pend_pos += b->win;
+  }
+  // 4. the step: every stream whose header is complete, with its decoded samples
+  std::vector<StepItem> items;
+  std::vector<ByteItem*> of;
+  for (ByteItem& b : bs) {
+    clear(b.out);
+    if (!b.live || !b.st->rate) continue;
+    some_stream* st = b.st;
+    const int j = static_cast<int>(items.size());
+    if (b.fi >= 0) {
+      dec.flac_of[b.fi] = j;
+    } else if (b.samples && st->walk->meta().container == SOME_AUDIO_WAV) {
+      const some_audio_meta& m = st->walk->meta();
+      dec.pcm.push_back(some_pcm_item{up_d + b.up, b.samples, m.channels, m.kind, 1, 0, nullptr});
+      dec.pcm_of.push_back(j);
+    }
+    items.push_back(StepItem{st, nullptr, b.samples, b.final, b.out});
+    of.push_back(&b);
+  }
+  if (!items.empty() && streams_step(s, items, &dec)) return -1;
+  if (dec.failed_item >= 0) {
+    set_error("FLAC frame at byte offset %lld failed to decode (status %d)", dec.failed_pos, dec.failed_status);
+    refuse(*of[dec.failed_item]);
+  }
+  if (!refusal.empty()) {
+    set_error("%s", refusal.c_str());
+    return SOME_STREAM_REFUSED;
+  }
+  return 0;
+}
+
+// A step of one encoded stream (some_stream_push_bytes, some_stream_finish).
+int bytes_call(some_stream* st, const void* data, long long n, bool final, some_notes* out, const char* who) {
+  if (final) st->finished = true;
+  std::vector<ByteItem> bs{ByteItem{st, static_cast<const uint8_t*>(data), n, final, out, -1}};
+  return locked(st->s, [&] { return bytes_step(st->s, bs, who); });
+}
 }  // namespace
 
 extern "C" int some_stream_open(some_session* s, int sample_rate, const some_slicer_params* params, some_stream** out) {
@@ -1204,13 +1499,16 @@ extern "C" int some_stream_open(some_session* s, int sample_rate, const some_sli
 
 extern "C" int some_stream_push(some_stream* st, const float* samples, long long n, some_notes* out) {
   SOME_REQUIRE(st != nullptr && out != nullptr && n >= 0 && (n == 0 || samples != nullptr), "some_stream_push: bad arguments");
+  SOME_REQUIRE(!st->walk, "some_stream_push: an encoded stream takes bytes (some_stream_push_bytes)");
   SOME_REQUIRE(!st->finished, "some_stream_push: the stream has finished");
   return stream_call(st, samples, n, false, out);
 }
 
 extern "C" int some_stream_finish(some_stream* st, some_notes* out) {
   SOME_REQUIRE(st != nullptr && out != nullptr, "some_stream_finish: bad arguments");
+  SOME_REQUIRE(!st->failed, "some_stream_finish: the stream was refused");
   SOME_REQUIRE(!st->finished, "some_stream_finish: the stream has finished");
+  if (st->walk) return bytes_call(st, nullptr, 0, true, out, "some_stream_finish");
   const int sr = st->s->info.sample_rate;
   SOME_REQUIRE(!st->resample || st->received * sr / st->rate >= 1,
                "some_stream_finish: Input signal length=%lld is too small to resample from %d->%d", (long long)st->received,
@@ -1231,6 +1529,7 @@ extern "C" int some_stream_push_many(some_stream* const* streams, const float* c
     const some_stream* st = streams[i];
     SOME_REQUIRE(st != nullptr, "some_stream_push_many: stream %d is NULL", i);
     SOME_REQUIRE(st->s == s, "some_stream_push_many: stream %d belongs to another session than stream 0", i);
+    SOME_REQUIRE(!st->walk, "some_stream_push_many: stream %d is an encoded stream (some_stream_push_bytes_many)", i);
     const auto dup = seen.emplace(st, i);
     SOME_REQUIRE(dup.second, "some_stream_push_many: stream %d appears twice (also at %d)", i, dup.first->second);
     SOME_REQUIRE(!st->finished, "some_stream_push_many: stream %d has finished", i);
@@ -1263,6 +1562,74 @@ extern "C" int some_stream_get_info(const some_stream* st, some_stream_info* inf
 
 extern "C" int some_stream_close(some_stream* st) {
   if (st) destroy(st);
+  return 0;
+}
+
+extern "C" int some_stream_open_encoded(some_session* s, const some_slicer_params* params, some_stream** out) {
+  SOME_REQUIRE(s != nullptr && out != nullptr, "some_stream_open_encoded: bad arguments");
+  *out = nullptr;
+  some_slicer_frames sl;
+  if (some_slicer_derive(s->info.sample_rate, params, &sl)) return -1;
+  some_slicer_stream* slicer;
+  if (some_slicer_stream_create(&sl, &slicer)) return -1;
+  some_stream* st = new some_stream();
+  st->s = s, st->slicer = slicer, st->f = sl;
+  st->walk.reset(new AudioWalk(true));
+  *out = st;
+  return 0;
+}
+
+extern "C" int some_stream_push_bytes(some_stream* st, const void* data, long long n_bytes, some_notes* out) {
+  SOME_REQUIRE(st != nullptr && out != nullptr && n_bytes >= 0 && (n_bytes == 0 || data != nullptr),
+               "some_stream_push_bytes: bad arguments");
+  SOME_REQUIRE(st->walk, "some_stream_push_bytes: a PCM stream takes samples (some_stream_push)");
+  SOME_REQUIRE(!st->failed, "some_stream_push_bytes: the stream was refused");
+  SOME_REQUIRE(!st->finished, "some_stream_push_bytes: the stream has finished");
+  return bytes_call(st, data, n_bytes, false, out, "some_stream_push_bytes");
+}
+
+extern "C" int some_stream_push_bytes_many(some_stream* const* streams, const void* const* data, const long long* n_bytes,
+                                           const int* finish, int count, some_notes* const* out) {
+  SOME_REQUIRE(streams != nullptr && data != nullptr && n_bytes != nullptr && out != nullptr && count >= 0,
+               "some_stream_push_bytes_many: bad arguments");
+  if (count == 0) return 0;
+  // every argument is checked before any stream changes
+  some_session* s = streams[0] ? streams[0]->s : nullptr;
+  std::map<const void*, int> seen, seen_notes;
+  for (int i = 0; i < count; ++i) {
+    const some_stream* st = streams[i];
+    SOME_REQUIRE(st != nullptr, "some_stream_push_bytes_many: stream %d is NULL", i);
+    SOME_REQUIRE(st->s == s, "some_stream_push_bytes_many: stream %d belongs to another session than stream 0", i);
+    SOME_REQUIRE(st->walk, "some_stream_push_bytes_many: stream %d is a PCM stream (some_stream_push_many)", i);
+    const auto dup = seen.emplace(st, i);
+    SOME_REQUIRE(dup.second, "some_stream_push_bytes_many: stream %d appears twice (also at %d)", i, dup.first->second);
+    SOME_REQUIRE(!st->failed, "some_stream_push_bytes_many: stream %d was refused", i);
+    SOME_REQUIRE(!st->finished, "some_stream_push_bytes_many: stream %d has finished", i);
+    SOME_REQUIRE(n_bytes[i] >= 0 && (n_bytes[i] == 0 || data[i] != nullptr),
+                 "some_stream_push_bytes_many: stream %d: %lld bytes at %p", i, n_bytes[i], data[i]);
+    SOME_REQUIRE(out[i] != nullptr, "some_stream_push_bytes_many: stream %d: NULL notes", i);
+    const auto shared = seen_notes.emplace(out[i], i);
+    SOME_REQUIRE(shared.second, "some_stream_push_bytes_many: stream %d shares its some_notes with stream %d", i,
+                 shared.first->second);
+  }
+  std::vector<ByteItem> bs;
+  bs.reserve(count);
+  for (int i = 0; i < count; ++i) {
+    const bool final = finish && finish[i];
+    if (final) streams[i]->finished = true;
+    bs.push_back(ByteItem{streams[i], static_cast<const uint8_t*>(data[i]), n_bytes[i], final, out[i], i});
+  }
+  return locked(s, [&] { return bytes_step(s, bs, "some_stream_push_bytes_many"); });
+}
+
+extern "C" int some_stream_get_meta(const some_stream* st, some_audio_meta* meta, long long* bytes_received,
+                                    long long* bytes_held) {
+  SOME_REQUIRE(st != nullptr && meta != nullptr, "some_stream_get_meta: null pointer");
+  SOME_REQUIRE(st->walk, "some_stream_get_meta: a PCM stream has no container");
+  if (st->rate) *meta = st->walk->meta();
+  else *meta = some_audio_meta{};
+  if (bytes_received) *bytes_received = st->walk->received();
+  if (bytes_held) *bytes_held = static_cast<long long>(st->pending.size()) + st->walk->held_header();   // held_audio: in pending
   return 0;
 }
 

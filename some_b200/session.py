@@ -151,6 +151,31 @@ class Session:
         """some_stream_open: a recording pushed while it arrives (see Stream)."""
         return Stream(self, sample_rate, params)
 
+    def stream_encoded(self, params: Optional[_lib.SlicerParams] = None) -> 'EncodedStream':
+        """some_stream_open_encoded: a WAV or FLAC file pushed as its bytes arrive (see EncodedStream)."""
+        return EncodedStream(self, params)
+
+    def push_bytes_many(self, items: Sequence[Tuple['EncodedStream', bytes]], finish: Optional[Sequence[bool]] = None):
+        """some_stream_push_bytes_many: push_many for encoded streams, with bytes in place of samples.  When a stream is refused
+        on its content, the others still complete their step: the StreamRefused raised carries every item's results."""
+        k = len(items)
+        datas = [bytes(b) for _, b in items]
+        bufs = [C.create_string_buffer(d, len(d)) if d else None for d in datas]
+        streams = (C.c_void_p * max(k, 1))(*[st.handle for st, _ in items])
+        ptrs = (C.c_void_p * max(k, 1))(*[C.cast(b, C.c_void_p) if b is not None else None for b in bufs])
+        lens = np.array([len(d) for d in datas] or [0], dtype=np.int64)
+        outs = (C.c_void_p * max(k, 1))(*[st.notes.handle for st, _ in items])
+        fin = None if finish is None else np.array([bool(f) for f in finish] or [0], dtype=np.int32)
+        if fin is not None and len(finish) != k:
+            raise ValueError(f'push_bytes_many: {k} items, {len(finish)} finish flags')
+        rc = self.lib.some_stream_push_bytes_many(streams, ptrs, lens.ctypes.data, None if fin is None else fin.ctypes.data, k,
+                                                  outs)
+        if rc == _lib.STREAM_REFUSED:          # the other streams' chunks are in their Notes: hand them over with the refusal
+            msg = self.lib.some_last_error().decode('utf8', 'replace')
+            raise _lib.StreamRefused(f'some_stream_push_bytes_many failed ({rc}): {msg}', [st._results() for st, _ in items])
+        _lib.check(rc, 'some_stream_push_bytes_many')
+        return [st._results() for st, _ in items]
+
     def push_many(self, items: Sequence[Tuple['Stream', np.ndarray]], finish: Optional[Sequence[bool]] = None):
         """some_stream_push_many: pushes samples to many streams of this session in one step, and finishes those with a true
         entry in `finish`.  Returns one (offsets, ranges, notes) per item, what Stream.push (then Stream.finish) would return;
@@ -219,3 +244,31 @@ class Stream:
 
     def __del__(self):
         self.close()
+
+
+class EncodedStream(Stream):
+    """some_stream_open_encoded: push(bytes) takes the next bytes of a WAV or FLAC file; push() and finish() return the chunks
+    that became final, as Stream does.  Concatenated they equal Session.transcribe_encoded on the whole file."""
+
+    def __init__(self, session: Session, params: Optional[_lib.SlicerParams] = None):
+        self.lib, self.session = session.lib, session
+        h = C.c_void_p()
+        _lib.check(self.lib.some_stream_open_encoded(session.handle, C.byref(params) if params is not None else None,
+                                                     C.byref(h)), 'some_stream_open_encoded')
+        self.handle = h
+        self.notes = Notes()
+        session._streams.add(self)
+
+    def push(self, data: bytes):
+        d = bytes(data)
+        _lib.check(self.lib.some_stream_push_bytes(self.handle, d, len(d), self.notes.handle), 'some_stream_push_bytes')
+        return self._results()
+
+    def meta(self) -> Dict[str, int]:
+        """some_stream_get_meta: the file's metadata (container 0 until the header is complete), the bytes pushed and the
+        bytes held on the host."""
+        m, got, held = _lib.AudioMeta(), C.c_longlong(), C.c_longlong()
+        _lib.check(self.lib.some_stream_get_meta(self.handle, C.byref(m), C.byref(got), C.byref(held)), 'some_stream_get_meta')
+        out = {name: getattr(m, name) for name, _ in _lib.AudioMeta._fields_ if name != 'reserved'}
+        out.update(bytes_received=got.value, bytes_held=held.value)
+        return out
