@@ -5,7 +5,8 @@
 //   some_mel_logmel -> some_forward (stand-alone LayerNorms, sigmoid / softmax head) -> some_decode_notes.
 // The sliced and the encoded calls share that front end (Recordings: one resampling window per recording at another rate,
 // one RMS window per recording that is cut, one batch over the chunks of all recordings); a stream step launches the same
-// two kernels over the windows of its streams.
+// two kernels over the windows of its streams.  The encoded files call and the encoded stream step share the stage in front
+// of it (Decode: one upload of the audio bytes, one FLAC scan, one PCM and one FLAC decode).
 //
 // The model file (little-endian; INTEGRATION.md "Deploying without Python" has the table):
 //   header     128 bytes: magic "SOMEB200", format version, ABI number, file size, directory offset, tensor count, the scalars
@@ -279,7 +280,7 @@ struct some_session {
   // grow-only buffers; rec_d: recordings at their own rates and at the model's (the sliced and encoded calls)
   DevBuf ws_block, scratch, wave_d, tab_d, cu_d, slab_d, rec_d, rms_d, step_d;
   PinBuf wave_h, tab_h, cu_h, slab_h, rms_h, step_h;   // step: the samples and descriptors of a step's upload
-  // transcribe_encoded: the files' audio bytes, the FLAC candidate list, scan workspace and int32 scratch
+  // the encoded calls' Decode: the audio bytes, the FLAC candidate list, scan workspace and int32 scratch
   DevBuf enc_d, flac_frames_d, flac_ws_d, flac_scratch_d;
   PinBuf enc_h, flac_frames_h;
   int ws_m = 0;
@@ -1028,40 +1029,124 @@ struct StepItem {
   bool dropped = false;         // its samples failed to decode: no slicer decisions, no chunks
 };
 
-// The decode stage in front of an encoded step (samples == NULL in its items): the samples are decoded on the device into
-// the upload's sample region, which the step's scatter reads.  Its descriptors go into the step's upload:
-//   add     the regions of the PCM descriptors, the chained FLAC frames (their scratch and output offsets) and the status;
-//   fill    after the step has placed each item's samples: the descriptors, with those places;
-//   launch  after the upload is sent, in front of the scatter: one some_pcm_decode, one FLAC decode, the status download;
-//   check   after the synchronise: the item whose frame failed to decode, if one did, is dropped.
-struct StepDecode {
+// Accepts a container's format for a session at rate `sr`, or refuses it (the message has no prefix): a WAV file's mono
+// down-mix takes at most 128 channels, and the resampler must support the rate pair.
+int check_format(const some_audio_meta& m, int sr) {
+  SOME_REQUIRE(m.container == SOME_AUDIO_FLAC || m.channels <= 128, "a mono down-mix of %d channels (at most 128)", m.channels);
+  long long t_end, x_first;
+  if (m.rate != sr && some_resample_window_plan(0, 0, 0, m.rate, sr, kKaiserTaps, &t_end, &x_first)) return -1;
+  return 0;
+}
+// One window of a call's audio bytes (a file's data chunk, a stream's pending bytes), with its container's metadata.
+struct ByteWindow {
+  const some_audio_meta* m;
+  const uint8_t* src;
+  int64_t bytes;
+  int64_t* at;                                   // out: its offset in the bytes upload
+};
+
+// The encoded-input stage of the encoded calls (some_session_transcribe_encoded and the encoded stream step): the audio bytes
+// go up, FLAC frames are found on the device and chained on the host by the caller, and the samples are decoded, mono, into
+// the caller's buffer.
+//   upload  the windows, FLAC first (the scan covers only them), each 16-byte aligned, then one some_flac_stream per FLAC
+//           window: copied into pinned memory in pieces of up to 1 MB and sent in one copy;
+//   scan    with FLAC windows: one some_flac_scan and the candidates down, again with room for all if the estimate was short;
+//   add     the regions of the PCM descriptors, the chained FLAC frames (their scratch and output offsets) and the status
+//           word in the caller's descriptor upload;
+//   fill    after the caller has placed each item's samples: the descriptors, with those places;
+//   launch  after the descriptor upload is sent: one some_pcm_decode, one FLAC decode, the status download;
+//   check   after the synchronise: the item whose frame failed to decode, if one did, with the error set.
+struct Decode {
   const uint8_t* bytes_d = nullptr;              // the bytes upload
-  const some_flac_stream* streams_d = nullptr;   // its FLAC windows
+  int64_t flac_bytes = 0;                        // its FLAC windows: [0, flac_bytes), described by streams_d[0 .. nf)
+  int nf = 0;
+  const some_flac_stream* streams_d = nullptr;
   const some_flac_frame* frames_h = nullptr;     // the candidates, on the host and on the device
   const some_flac_frame* frames_d = nullptr;
-  std::vector<some_pcm_item> pcm;                // out: an offset in the item's samples until fill()
-  std::vector<int> pcm_of, flac_of;              // the step item of each PCM entry and of each FLAC window
+  int n_cand = 0;
+  std::vector<some_pcm_item> pcm;                // out: set by fill()
+  std::vector<int> pcm_of, flac_of;              // the caller's item of each PCM entry and of each FLAC window
   std::vector<int64_t> first{0};                 // FLAC window r's frames: chain[first[r] .. first[r + 1])
   std::vector<int32_t> chain;
   std::vector<int> channels;
   std::vector<long long> base;                   // FLAC window r: file offset x lies at x + base[r] in the bytes upload
-  int failed_item = -1;                          // check(): the dropped item, and where its frame lies
-  long long failed_pos = 0;
-  int failed_status = 0;
+  float* out = nullptr;                          // fill(): the FLAC windows' output base
   size_t pcm_off = 0, chain_off = 0, soff_off = 0, ooff_off = 0, status_off = 0;
 
+  int upload(some_session* s, const std::vector<ByteWindow>& ws, const char* what) {
+    int64_t at = 0;
+    auto place = [&](bool flac) {
+      for (const ByteWindow& w : ws)
+        if ((w.m->container == SOME_AUDIO_FLAC) == flac) *w.at = at, at += align16(w.bytes), nf += flac;
+    };
+    place(true);
+    flac_bytes = at;
+    place(false);
+    const int64_t up_bytes = at + static_cast<int64_t>(sizeof(some_flac_stream)) * nf;
+    if (s->enc_h.ensure(up_bytes + 16, what) || s->enc_d.ensure(up_bytes + 16, what)) return -1;
+    uint8_t* up_h = static_cast<uint8_t*>(s->enc_h.p);
+    std::vector<HostSpan> spans;
+    some_flac_stream* st_h = reinterpret_cast<some_flac_stream*>(up_h + at);
+    for (const ByteWindow& w : ws) {
+      spans.push_back({up_h + *w.at, w.src, static_cast<size_t>(w.bytes)});
+      if (w.m->container == SOME_AUDIO_FLAC)
+        *st_h++ = some_flac_stream{*w.at, *w.at + w.bytes, w.m->channels, w.m->bits, w.m->max_blocksize, 0};
+    }
+    copy_to_pinned(*s->pool, spans, size_t(1) << 20);
+    bytes_d = static_cast<const uint8_t*>(s->enc_d.p);
+    streams_d = reinterpret_cast<const some_flac_stream*>(bytes_d + at);
+    if (up_bytes) SOME_CUDA(cudaMemcpyAsync(s->enc_d.p, up_h, static_cast<size_t>(up_bytes), cudaMemcpyHostToDevice, s->stream),
+                            "encoded upload");
+    return 0;
+  }
+  // `cap`: the caller's estimate of the candidates.  with_count: all `cap` come down with the count, in one synchronise;
+  // otherwise the count comes down first, then exactly that many.
+  int scan(some_session* s, int64_t cap, bool with_count) {
+    const uint64_t ws_bytes = some_flac_scan_workspace_bytes(flac_bytes);
+    if (s->flac_ws_d.ensure(ws_bytes + 16, "the FLAC scan workspace")) return -1;
+    int* count_d = reinterpret_cast<int*>(static_cast<char*>(s->flac_ws_d.p) + ws_bytes);
+    char* fh;                                    // the count, then the candidates at fh + 16
+    for (;;) {
+      if (s->flac_frames_d.ensure(sizeof(some_flac_frame) * cap, "the FLAC frames") ||
+          s->flac_frames_h.ensure(sizeof(some_flac_frame) * cap + 16, "the FLAC frames"))
+        return -1;
+      fh = static_cast<char*>(s->flac_frames_h.p);
+      if (some_flac_scan(bytes_d, flac_bytes, streams_d, nf, static_cast<some_flac_frame*>(s->flac_frames_d.p),
+                         static_cast<int>(cap), count_d, s->flac_ws_d.p, s->stream))
+        return -1;
+      SOME_CUDA(cudaMemcpyAsync(fh, count_d, sizeof(int), cudaMemcpyDeviceToHost, s->stream), "count download");
+      if (with_count)
+        SOME_CUDA(cudaMemcpyAsync(fh + 16, s->flac_frames_d.p, sizeof(some_flac_frame) * cap, cudaMemcpyDeviceToHost,
+                                  s->stream), "candidate download");
+      SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+      n_cand = *reinterpret_cast<const int*>(fh);
+      if (n_cand <= cap) break;
+      cap = n_cand;
+    }
+    if (!with_count) {
+      SOME_CUDA(cudaMemcpyAsync(fh + 16, s->flac_frames_d.p, sizeof(some_flac_frame) * n_cand, cudaMemcpyDeviceToHost,
+                                s->stream), "candidate download");
+      SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+    }
+    frames_h = reinterpret_cast<const some_flac_frame*>(fh + 16);
+    frames_d = static_cast<const some_flac_frame*>(s->flac_frames_d.p);
+    return 0;
+  }
   void add(Upload& up) {
     const size_t n = chain.size();
     pcm_off = up.add(static_cast<size_t>(some_pcm_decode_bytes(static_cast<int>(pcm.size()))));
     chain_off = up.add(4 * n), soff_off = up.add(8 * n), ooff_off = up.add(8 * n), status_off = up.add(2 * sizeof(int));
   }
-  int fill(some_session* s, const Upload& up, float* samples_d, const std::vector<StepItem>& items) {
-    for (size_t j = 0; j < pcm.size(); ++j) pcm[j].out = samples_d + items[pcm_of[j]].up;
+  // item i's samples go to dst + at(i)
+  template <class At>
+  int fill(some_session* s, const Upload& up, float* dst, At at) {
+    out = dst;
+    for (size_t j = 0; j < pcm.size(); ++j) pcm[j].out = dst + at(pcm_of[j]);
     int64_t* soff = reinterpret_cast<int64_t*>(up.h(soff_off));
     int64_t* ooff = reinterpret_cast<int64_t*>(up.h(ooff_off));
     int64_t scratch = 0;
     for (size_t r = 0; r < flac_of.size(); ++r) {
-      int64_t o = items[flac_of[r]].up;
+      int64_t o = at(flac_of[r]);
       for (int64_t j = first[r]; j < first[r + 1]; ++j) {
         const int bs = frames_h[chain[j]].blocksize;
         soff[j] = scratch, ooff[j] = o;
@@ -1073,28 +1158,30 @@ struct StepDecode {
       return -1;
     if (!chain.empty()) memcpy(up.h(chain_off), chain.data(), 4 * chain.size());
     int* status = reinterpret_cast<int*>(up.h(status_off));
-    status[0] = 0, status[1] = INT_MAX;
+    status[0] = 0, status[1] = INT_MAX;          // the first chained frame that fails to decode, if one does
     return 0;
   }
-  int launch(some_session* s, const Upload& up, float* samples_d) const {
+  int launch(some_session* s, const Upload& up) const {
     if (some_pcm_decode(up.h(pcm_off), up.d(pcm_off), s->stream)) return -1;
     if (chain.empty()) return 0;
     int* status_d = reinterpret_cast<int*>(up.d(status_off));
     if (flac_decode_chain(bytes_d, streams_d, frames_d, reinterpret_cast<const int32_t*>(up.d(chain_off)),
                           reinterpret_cast<const int64_t*>(up.d(soff_off)), reinterpret_cast<const int64_t*>(up.d(ooff_off)),
-                          static_cast<int>(chain.size()), static_cast<int32_t*>(s->flac_scratch_d.p), samples_d, 1, status_d,
+                          static_cast<int>(chain.size()), static_cast<int32_t*>(s->flac_scratch_d.p), out, 1, status_d,
                           status_d + 1, s->stream))
       return -1;
     SOME_CUDA(cudaMemcpyAsync(up.h(status_off), status_d, 2 * sizeof(int), cudaMemcpyDeviceToHost, s->stream), "status download");
     return 0;
   }
-  void check(const Upload& up, std::vector<StepItem>& items) {
+  // The caller's item whose frame failed to decode, with the error set (the frame's byte offset in its file), or -1.
+  int check(const Upload& up) const {
     const int* status = reinterpret_cast<const int*>(up.h(status_off));
-    if (chain.empty() || status[0] == 0) return;
+    if (chain.empty() || status[0] == 0) return -1;
     size_t r = 0;
     while (r + 1 < flac_of.size() && first[r + 1] <= status[1]) ++r;
-    failed_item = flac_of[r], failed_pos = frames_h[chain[status[1]]].pos - base[r], failed_status = status[0];
-    items[failed_item].dropped = true;
+    set_error("FLAC frame at byte offset %lld failed to decode (status %d)",
+              static_cast<long long>(frames_h[chain[status[1]]].pos - base[r]), status[0]);
+    return flac_of[r];
   }
 };
 
@@ -1107,7 +1194,7 @@ struct StepDecode {
 //      synchronise;
 //   3. the slicer's decisions for each stream;
 //   4. every chunk that became final, in any stream, copied next to each other and transcribed as one batch.
-int streams_step(some_session* s, std::vector<StepItem>& items, StepDecode* dec = nullptr) {
+int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nullptr) {
   const int sr = s->info.sample_rate;
   std::vector<some_resample_window> rs;
   std::vector<some_rms_window> rm;
@@ -1199,9 +1286,9 @@ int streams_step(some_session* s, std::vector<StepItem>& items, StepDecode* dec 
   if (some_resample_windows_pack(rs.data(), kr, up.h(rs_off)) || some_slicer_rms_windows_pack(rm.data(), km, up.h(rm_off)))
     return -1;
   float* samples_d = reinterpret_cast<float*>(up.d(smp_off));
-  if (dec && dec->fill(s, up, samples_d, items)) return -1;
+  if (dec && dec->fill(s, up, samples_d, [&](int j) { return items[j].up; })) return -1;
   copy_to_pinned(*s->pool, spans, size_t(1) << 20);          // the samples, in pieces of up to 1 MB
-  if (up.send("stream upload") || (dec && dec->launch(s, up, samples_d))) return -1;
+  if (up.send("stream upload") || (dec && dec->launch(s, up))) return -1;
   if (ks) {
     const WindowsHeader& h = *reinterpret_cast<const WindowsHeader*>(up.h(sc_off));
     scatter_kernel<<<static_cast<unsigned>(h.tiles), kScatterThreads, 0, s->stream>>>(
@@ -1214,7 +1301,10 @@ int streams_step(some_session* s, std::vector<StepItem>& items, StepDecode* dec 
   if (frames)
     SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames, cudaMemcpyDeviceToHost, s->stream), "RMS download");
   SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");   // also frees the upload buffer for the next step
-  if (dec) dec->check(up, items);
+  if (dec) {
+    const int j = dec->check(up);
+    if (j >= 0) items[j].dropped = true;
+  }
 
   // the slicer's decisions, and where each chunk that became final lies
   std::vector<const float*> src;
@@ -1284,12 +1374,12 @@ struct ByteItem {
 
 // A step of encoded streams (some_stream_push_bytes*, some_stream_finish), under the session's mutex:
 //   1. on the host, each stream's walk consumes its bytes; their audio joins the stream's pending bytes;
-//   2. one pinned upload of the FLAC windows (the pending bytes from each stream's first unchained frame) and the whole WAV
-//      sample frames;
-//   3. with FLAC streams: one some_flac_scan over all windows, one download of the candidates, one synchronise, then each
-//      stream's resumable chain;
-//   4. streams_step with the decode stage in front: one some_pcm_decode and one FLAC decode, mono, into the region its scatter
-//      reads.
+//   2. the encoded-input stage (Decode) uploads the FLAC windows (the pending bytes from each stream's first unchained
+//      frame) and the whole WAV sample frames;
+//   3. with FLAC streams: its scan, with the candidates down in the same synchronise as the count, then each stream's
+//      resumable chain;
+//   4. streams_step with the stage's decodes in front: one some_pcm_decode and one FLAC decode, mono, into the region its
+//      scatter reads.
 // A stream refused on its content (its walk, its chain, a decode failure, a rate or channel count the session cannot take)
 // leaves the step; the others go on, and the call then fails with the first refusal.
 int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
@@ -1323,13 +1413,7 @@ int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
     if (!known) continue;
     const some_audio_meta& m = st->walk->meta();
     if (st->rate == 0) {                 // this push completes the header
-      if (m.container == SOME_AUDIO_WAV && m.channels > 128) {
-        set_error("a mono down-mix of %d channels (at most 128)", m.channels);
-        refuse(b);
-        continue;
-      }
-      long long t_end, x_first;
-      if (m.rate != sr && some_resample_window_plan(0, 0, 0, m.rate, sr, kKaiserTaps, &t_end, &x_first)) {
+      if (check_format(m, sr)) {
         refuse(b);
         continue;
       }
@@ -1343,91 +1427,56 @@ int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
       if (a1 > from) st->pending.insert(st->pending.end(), b.data + (from - r0), b.data + (a1 - r0));
     }
   }
-  // 2. the bytes upload: the FLAC windows first (the scan covers only them), the WAV frames, the FLAC window descriptors
-  std::vector<ByteItem*> flac, wav;
-  for (ByteItem& b : bs)
-    if (b.live && b.st->rate) (b.st->walk->meta().container == SOME_AUDIO_FLAC ? flac : wav).push_back(&b);
-  int64_t at = 0;
-  for (ByteItem* b : flac) b->up = at, b->win = static_cast<int64_t>(b->st->pending.size()), at += align16(b->win);
-  const int64_t flac_bytes = at;
-  for (ByteItem* b : wav) {
-    const some_audio_meta& m = b->st->walk->meta();
-    static const int kBytes[7] = {0, 1, 2, 3, 4, 4, 8};
-    const int64_t frame = static_cast<int64_t>(m.channels) * kBytes[m.kind];
-    b->samples = static_cast<int64_t>(b->st->pending.size()) / frame;
-    b->win = b->samples * frame;
-    if (too_short(*b)) continue;
-    b->up = at, at += align16(b->win);
-  }
-  const int nf = static_cast<int>(flac.size());
-  const int64_t streams_off = at, up_bytes = at + static_cast<int64_t>(sizeof(some_flac_stream)) * nf;
-  if (s->enc_h.ensure(up_bytes + 16, "the encoded streams") || s->enc_d.ensure(up_bytes + 16, "the encoded streams")) return -1;
-  uint8_t* up_h = static_cast<uint8_t*>(s->enc_h.p);
-  const uint8_t* up_d = static_cast<const uint8_t*>(s->enc_d.p);
-  std::vector<HostSpan> spans;
-  for (ByteItem* b : flac) spans.push_back({up_h + b->up, b->st->pending.data(), static_cast<size_t>(b->win)});
-  for (ByteItem* b : wav)
-    if (b->live) spans.push_back({up_h + b->up, b->st->pending.data(), static_cast<size_t>(b->win)});
-  copy_to_pinned(*s->pool, spans, size_t(1) << 20);
-  some_flac_stream* win_h = reinterpret_cast<some_flac_stream*>(up_h + streams_off);
-  for (int r = 0; r < nf; ++r) {
-    const some_audio_meta& m = flac[r]->st->walk->meta();
-    win_h[r] = some_flac_stream{flac[r]->up, flac[r]->up + flac[r]->win, m.channels, m.bits, m.max_blocksize, 0};
-  }
-  if (up_bytes) SOME_CUDA(cudaMemcpyAsync(s->enc_d.p, up_h, static_cast<size_t>(up_bytes), cudaMemcpyHostToDevice, s->stream),
-                          "encoded upload");
-  StepDecode dec;
-  dec.bytes_d = up_d, dec.streams_d = reinterpret_cast<const some_flac_stream*>(up_d + streams_off);
-  // 3. the FLAC frames: one scan, the candidates down (again, larger, only if the estimate was short), the chains on the host
-  if (nf) {
-    int64_t cap = 64;
-    for (ByteItem* b : flac) cap += b->win / 64 + 8;
-    const uint64_t ws_bytes = some_flac_scan_workspace_bytes(flac_bytes);
-    if (s->flac_ws_d.ensure(ws_bytes + 16, "the FLAC scan workspace")) return -1;
-    int* count_d = reinterpret_cast<int*>(static_cast<char*>(s->flac_ws_d.p) + ws_bytes);
-    int n_cand = 0;
-    for (;;) {
-      SOME_REQUIRE(cap < (int64_t(1) << 31), "%s: too many FLAC frame candidates in one step", who);
-      if (s->flac_frames_d.ensure(sizeof(some_flac_frame) * cap, "the FLAC frames") ||
-          s->flac_frames_h.ensure(sizeof(some_flac_frame) * cap + 16, "the FLAC frames"))
-        return -1;
-      char* fh = static_cast<char*>(s->flac_frames_h.p);
-      if (some_flac_scan(up_d, flac_bytes, dec.streams_d, nf, static_cast<some_flac_frame*>(s->flac_frames_d.p),
-                         static_cast<int>(cap), count_d, s->flac_ws_d.p, s->stream))
-        return -1;
-      SOME_CUDA(cudaMemcpyAsync(fh, count_d, sizeof(int), cudaMemcpyDeviceToHost, s->stream), "count download");
-      SOME_CUDA(cudaMemcpyAsync(fh + 16, s->flac_frames_d.p, sizeof(some_flac_frame) * cap, cudaMemcpyDeviceToHost, s->stream),
-                "candidate download");
-      SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
-      n_cand = *reinterpret_cast<const int*>(fh);
-      if (n_cand <= cap) break;
-      cap = n_cand;
+  // 2. the bytes upload: each stream's pending FLAC window (from its first unchained frame) or its whole WAV sample frames
+  auto flac = [](const ByteItem& b) { return b.live && b.st->rate && b.st->walk->meta().container == SOME_AUDIO_FLAC; };
+  std::vector<ByteWindow> ws;
+  for (ByteItem& b : bs) {
+    if (!b.live || !b.st->rate) continue;
+    const some_audio_meta& m = b.st->walk->meta();
+    b.win = static_cast<int64_t>(b.st->pending.size());
+    if (m.container == SOME_AUDIO_WAV) {
+      static const int kBytes[7] = {0, 1, 2, 3, 4, 4, 8};
+      const int64_t frame = static_cast<int64_t>(m.channels) * kBytes[m.kind];
+      b.samples = b.win / frame;
+      b.win = b.samples * frame;
+      if (too_short(b)) continue;
     }
-    dec.frames_h = reinterpret_cast<const some_flac_frame*>(static_cast<char*>(s->flac_frames_h.p) + 16);
-    dec.frames_d = static_cast<const some_flac_frame*>(s->flac_frames_d.p);
+    ws.push_back({&m, b.st->pending.data(), b.win, &b.up});
+  }
+  Decode dec;
+  if (dec.upload(s, ws, "the encoded streams")) return -1;
+  // 3. the FLAC frames: one scan, the candidates down with the count, the chains on the host
+  if (dec.nf) {
+    int64_t cap = 64;
+    for (const ByteItem& b : bs)
+      if (flac(b)) cap += b.win / 64 + 8;
+    SOME_REQUIRE(cap < (int64_t(1) << 31), "%s: too many FLAC frame candidates in one step", who);
+    if (dec.scan(s, cap, true)) return -1;
+    const int n_cand = dec.n_cand;
     dec.chain.resize(std::max(n_cand, 1));
     int i = 0, k = 0;
-    for (ByteItem* b : flac) {
-      some_stream* st = b->st;
+    for (ByteItem& b : bs) {
+      if (!flac(b)) continue;
+      some_stream* st = b.st;
       const some_audio_meta& m = st->walk->meta();
       const int k0 = k;
-      const long long base = b->up - st->pend_pos;
-      if (flac_walk(dec.frames_h, n_cand, &i, base, b->up + b->win, m.frames, b->final, &st->fw, dec.chain.data(), n_cand, &k)) {
+      const long long base = b.up - st->pend_pos;
+      if (flac_walk(dec.frames_h, n_cand, &i, base, b.up + b.win, m.frames, b.final, &st->fw, dec.chain.data(), n_cand, &k)) {
         k = k0;
-        refuse(*b);
+        refuse(b);
         continue;
       }
-      for (int j = k0; j < k; ++j) b->samples += dec.frames_h[dec.chain[j]].blocksize;
+      for (int j = k0; j < k; ++j) b.samples += dec.frames_h[dec.chain[j]].blocksize;
       // the bytes before the next frame are decoded (or, once the walk is done, past the recording)
       const long long keep = st->fw.done ? st->pend_pos + static_cast<long long>(st->pending.size()) : st->fw.pos;
       st->pending.erase(st->pending.begin(), st->pending.begin() + (keep - st->pend_pos));
       st->pend_pos = keep;
-      if (too_short(*b)) {
+      if (too_short(b)) {
         k = k0;
         continue;
       }
       if (k > k0) {
-        b->fi = static_cast<int>(dec.flac_of.size());
+        b.fi = static_cast<int>(dec.flac_of.size());
         dec.flac_of.push_back(-1);       // its step item, below
         dec.first.push_back(k);
         dec.channels.push_back(m.channels);
@@ -1436,10 +1485,10 @@ int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
     }
     dec.chain.resize(k);
   }
-  for (ByteItem* b : wav) {
-    if (!b->live) continue;
-    b->st->pending.erase(b->st->pending.begin(), b->st->pending.begin() + b->win);
-    b->st->pend_pos += b->win;
+  for (ByteItem& b : bs) {               // the WAV windows went up whole
+    if (!b.live || !b.st->rate || b.st->walk->meta().container != SOME_AUDIO_WAV) continue;
+    b.st->pending.erase(b.st->pending.begin(), b.st->pending.begin() + b.win);
+    b.st->pend_pos += b.win;
   }
   // 4. the step: every stream whose header is complete, with its decoded samples
   std::vector<StepItem> items;
@@ -1453,17 +1502,15 @@ int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
       dec.flac_of[b.fi] = j;
     } else if (b.samples && st->walk->meta().container == SOME_AUDIO_WAV) {
       const some_audio_meta& m = st->walk->meta();
-      dec.pcm.push_back(some_pcm_item{up_d + b.up, b.samples, m.channels, m.kind, 1, 0, nullptr});
+      dec.pcm.push_back(some_pcm_item{dec.bytes_d + b.up, b.samples, m.channels, m.kind, 1, 0, nullptr});
       dec.pcm_of.push_back(j);
     }
     items.push_back(StepItem{st, nullptr, b.samples, b.final, b.out});
     of.push_back(&b);
   }
   if (!items.empty() && streams_step(s, items, &dec)) return -1;
-  if (dec.failed_item >= 0) {
-    set_error("FLAC frame at byte offset %lld failed to decode (status %d)", dec.failed_pos, dec.failed_status);
-    refuse(*of[dec.failed_item]);
-  }
+  for (size_t j = 0; j < items.size(); ++j)
+    if (items[j].dropped) refuse(*of[j]);      // its frame failed to decode
   if (!refusal.empty()) {
     set_error("%s", refusal.c_str());
     return SOME_STREAM_REFUSED;
@@ -1476,6 +1523,36 @@ int bytes_call(some_stream* st, const void* data, long long n, bool final, some_
   if (final) st->finished = true;
   std::vector<ByteItem> bs{ByteItem{st, static_cast<const uint8_t*>(data), n, final, out, -1}};
   return locked(st->s, [&] { return bytes_step(st->s, bs, who); });
+}
+
+// The arguments of a many-call `who` (streams of one kind, encoded or PCM; n[i] bytes or samples at data[i]), every one
+// checked before any stream changes.
+template <class T>
+int check_many(some_stream* const* streams, const T* const* data, const long long* n, const int* finish, int count,
+               some_notes* const* out, bool encoded, const char* who) {
+  some_session* s = streams[0] ? streams[0]->s : nullptr;
+  std::map<const void*, int> seen, seen_notes;
+  for (int i = 0; i < count; ++i) {
+    const some_stream* st = streams[i];
+    SOME_REQUIRE(st != nullptr, "%s: stream %d is NULL", who, i);
+    SOME_REQUIRE(st->s == s, "%s: stream %d belongs to another session than stream 0", who, i);
+    SOME_REQUIRE(!st->walk == !encoded, "%s: stream %d is %s", who, i,
+                 encoded ? "a PCM stream (some_stream_push_many)" : "an encoded stream (some_stream_push_bytes_many)");
+    const auto dup = seen.emplace(st, i);
+    SOME_REQUIRE(dup.second, "%s: stream %d appears twice (also at %d)", who, i, dup.first->second);
+    SOME_REQUIRE(!st->failed, "%s: stream %d was refused", who, i);     // only an encoded stream is refused
+    SOME_REQUIRE(!st->finished, "%s: stream %d has finished", who, i);
+    SOME_REQUIRE(n[i] >= 0 && (n[i] == 0 || data[i] != nullptr), "%s: stream %d: %lld %s at %p", who, i, n[i],
+                 encoded ? "bytes" : "samples", static_cast<const void*>(data[i]));
+    SOME_REQUIRE(out[i] != nullptr, "%s: stream %d: NULL notes", who, i);
+    const auto shared = seen_notes.emplace(out[i], i);
+    SOME_REQUIRE(shared.second, "%s: stream %d shares its some_notes with stream %d", who, i, shared.first->second);
+    const int sr = s->info.sample_rate;                                 // a PCM stream's end at another rate
+    SOME_REQUIRE(encoded || !(finish && finish[i]) || !st->resample || (st->received + n[i]) * sr / st->rate >= 1,
+                 "%s: stream %d: Input signal length=%lld is too small to resample from %d->%d", who, i,
+                 (long long)(st->received + n[i]), st->rate, sr);
+  }
+  return 0;
 }
 }  // namespace
 
@@ -1522,28 +1599,8 @@ extern "C" int some_stream_push_many(some_stream* const* streams, const float* c
   SOME_REQUIRE(streams != nullptr && samples != nullptr && n != nullptr && out != nullptr && count >= 0,
                "some_stream_push_many: bad arguments");
   if (count == 0) return 0;
-  // every argument is checked before any stream changes
-  some_session* s = streams[0] ? streams[0]->s : nullptr;
-  std::map<const void*, int> seen, seen_notes;
-  for (int i = 0; i < count; ++i) {
-    const some_stream* st = streams[i];
-    SOME_REQUIRE(st != nullptr, "some_stream_push_many: stream %d is NULL", i);
-    SOME_REQUIRE(st->s == s, "some_stream_push_many: stream %d belongs to another session than stream 0", i);
-    SOME_REQUIRE(!st->walk, "some_stream_push_many: stream %d is an encoded stream (some_stream_push_bytes_many)", i);
-    const auto dup = seen.emplace(st, i);
-    SOME_REQUIRE(dup.second, "some_stream_push_many: stream %d appears twice (also at %d)", i, dup.first->second);
-    SOME_REQUIRE(!st->finished, "some_stream_push_many: stream %d has finished", i);
-    SOME_REQUIRE(n[i] >= 0 && (n[i] == 0 || samples[i] != nullptr), "some_stream_push_many: stream %d: %lld samples at %p", i,
-                 n[i], static_cast<const void*>(samples[i]));
-    SOME_REQUIRE(out[i] != nullptr, "some_stream_push_many: stream %d: NULL notes", i);
-    const auto shared = seen_notes.emplace(out[i], i);
-    SOME_REQUIRE(shared.second, "some_stream_push_many: stream %d shares its some_notes with stream %d", i,
-                 shared.first->second);
-    const int sr = s->info.sample_rate;
-    SOME_REQUIRE(!(finish && finish[i]) || !st->resample || (st->received + n[i]) * sr / st->rate >= 1,
-                 "some_stream_push_many: stream %d: Input signal length=%lld is too small to resample from %d->%d", i,
-                 (long long)(st->received + n[i]), st->rate, sr);
-  }
+  if (check_many(streams, samples, n, finish, count, out, false, "some_stream_push_many")) return -1;
+  some_session* s = streams[0]->s;
   std::vector<StepItem> items;
   items.reserve(count);
   for (int i = 0; i < count; ++i) {
@@ -1593,25 +1650,8 @@ extern "C" int some_stream_push_bytes_many(some_stream* const* streams, const vo
   SOME_REQUIRE(streams != nullptr && data != nullptr && n_bytes != nullptr && out != nullptr && count >= 0,
                "some_stream_push_bytes_many: bad arguments");
   if (count == 0) return 0;
-  // every argument is checked before any stream changes
-  some_session* s = streams[0] ? streams[0]->s : nullptr;
-  std::map<const void*, int> seen, seen_notes;
-  for (int i = 0; i < count; ++i) {
-    const some_stream* st = streams[i];
-    SOME_REQUIRE(st != nullptr, "some_stream_push_bytes_many: stream %d is NULL", i);
-    SOME_REQUIRE(st->s == s, "some_stream_push_bytes_many: stream %d belongs to another session than stream 0", i);
-    SOME_REQUIRE(st->walk, "some_stream_push_bytes_many: stream %d is a PCM stream (some_stream_push_many)", i);
-    const auto dup = seen.emplace(st, i);
-    SOME_REQUIRE(dup.second, "some_stream_push_bytes_many: stream %d appears twice (also at %d)", i, dup.first->second);
-    SOME_REQUIRE(!st->failed, "some_stream_push_bytes_many: stream %d was refused", i);
-    SOME_REQUIRE(!st->finished, "some_stream_push_bytes_many: stream %d has finished", i);
-    SOME_REQUIRE(n_bytes[i] >= 0 && (n_bytes[i] == 0 || data[i] != nullptr),
-                 "some_stream_push_bytes_many: stream %d: %lld bytes at %p", i, n_bytes[i], data[i]);
-    SOME_REQUIRE(out[i] != nullptr, "some_stream_push_bytes_many: stream %d: NULL notes", i);
-    const auto shared = seen_notes.emplace(out[i], i);
-    SOME_REQUIRE(shared.second, "some_stream_push_bytes_many: stream %d shares its some_notes with stream %d", i,
-                 shared.first->second);
-  }
+  if (check_many(streams, data, n_bytes, finish, count, out, true, "some_stream_push_bytes_many")) return -1;
+  some_session* s = streams[0]->s;
   std::vector<ByteItem> bs;
   bs.reserve(count);
   for (int i = 0; i < count; ++i) {
@@ -1650,140 +1690,65 @@ int item_error(int i) {
   return -1;
 }
 
-// The GPU step of some_session_transcribe_encoded (under the session's mutex); out[] is written only at the end.
+// The GPU step of some_session_transcribe_encoded (under the session's mutex); out[] is written only at the end.  Each
+// file's data chunk goes through Decode (with FLAC files: the count, then the candidates down, and some_flac_chain) into
+// the recording buffer, whose Recordings are resampled, cut and transcribed after one synchronise.
 int transcribe_encoded(some_session* s, std::vector<EncItem>& its, const some_slicer_frames& sl, some_notes* const* out) {
   const int sr = s->info.sample_rate;
   const int count = static_cast<int>(its.size());
-  std::vector<int> flac, wav;
-  for (int i = 0; i < count; ++i) (its[i].m.container == SOME_AUDIO_FLAC ? flac : wav).push_back(i);
-  const int nf = static_cast<int>(flac.size());
-  // 1. one upload: the FLAC items' audio bytes first (the scan covers only them), the WAV data chunks, the FLAC descriptors
-  int64_t at = 0;
-  for (int i : flac) its[i].up = at, at += static_cast<int64_t>(align16(static_cast<size_t>(its[i].m.data_bytes)));
-  const int64_t flac_bytes = at;
-  for (int i : wav) its[i].up = at, at += static_cast<int64_t>(align16(static_cast<size_t>(its[i].m.data_bytes)));
-  const int64_t streams_off = at;
-  const int64_t up_bytes = at + static_cast<int64_t>(sizeof(some_flac_stream)) * nf;
-  if (s->enc_h.ensure(up_bytes + 16, "the encoded files") || s->enc_d.ensure(up_bytes + 16, "the encoded files")) return -1;
-  uint8_t* up_h = static_cast<uint8_t*>(s->enc_h.p);
-  uint8_t* up_d = static_cast<uint8_t*>(s->enc_d.p);
-  std::vector<HostSpan> spans;
-  for (const EncItem& it : its) spans.push_back({up_h + it.up, it.bytes + it.m.data_offset, static_cast<size_t>(it.m.data_bytes)});
-  copy_to_pinned(*s->pool, spans, size_t(1) << 20);          // in pieces of up to 1 MB
-  some_flac_stream* st_h = reinterpret_cast<some_flac_stream*>(up_h + streams_off);
-  for (int k = 0; k < nf; ++k) {
-    const EncItem& it = its[flac[k]];
-    st_h[k] = some_flac_stream{it.up, it.up + it.m.data_bytes, it.m.channels, it.m.bits, it.m.max_blocksize, 0};
+  std::vector<ByteWindow> ws;
+  for (EncItem& it : its) ws.push_back({&it.m, it.bytes + it.m.data_offset, it.m.data_bytes, &it.up});
+  Decode dec;
+  if (dec.upload(s, ws, "the encoded files")) return -1;
+  for (int i = 0; i < count; ++i) {
+    const EncItem& it = its[i];
+    if (it.m.container == SOME_AUDIO_FLAC) {
+      dec.flac_of.push_back(i);
+    } else {
+      dec.pcm.push_back(some_pcm_item{dec.bytes_d + it.up, it.n, it.m.channels, it.m.kind, 1, 0, nullptr});
+      dec.pcm_of.push_back(i);
+    }
   }
-  SOME_CUDA(cudaMemcpyAsync(up_d, up_h, static_cast<size_t>(up_bytes), cudaMemcpyHostToDevice, s->stream), "encoded upload");
-  const some_flac_stream* st_d = reinterpret_cast<const some_flac_stream*>(up_d + streams_off);
-
-  // 2. the FLAC frames: one scan, the candidates down, the chain on the host
-  std::vector<int32_t> chain;
-  std::vector<int64_t> first(nf + 1, 0), lengths(nf, 0);
-  const some_flac_frame* frames_h = nullptr;
+  const int nf = dec.nf;
   if (nf) {
     int64_t cap = 64;
-    for (int i : flac) {
-      const some_audio_meta& m = its[i].m;
-      cap += m.frames ? m.frames / std::max(m.min_blocksize, 1) + 2 : m.data_bytes / 16 + 2;
+    std::vector<some_flac_range> recs;
+    for (int i : dec.flac_of) {
+      const EncItem& it = its[i];
+      cap += it.m.frames ? it.m.frames / std::max(it.m.min_blocksize, 1) + 2 : it.m.data_bytes / 16 + 2;
+      recs.push_back(some_flac_range{it.up - it.m.data_offset, it.up, it.up + it.m.data_bytes, it.m.frames});
+      dec.channels.push_back(it.m.channels);
+      dec.base.push_back(it.up - it.m.data_offset);
     }
     SOME_REQUIRE(cap < (int64_t(1) << 31), "some_session_transcribe_encoded: too many FLAC frames in one call");
-    const uint64_t ws_bytes = some_flac_scan_workspace_bytes(flac_bytes);
-    if (s->flac_ws_d.ensure(ws_bytes + 16, "the FLAC scan workspace")) return -1;
-    int* count_d = reinterpret_cast<int*>(static_cast<char*>(s->flac_ws_d.p) + ws_bytes);
-    int n_cand = 0;
-    for (;;) {
-      if (s->flac_frames_d.ensure(sizeof(some_flac_frame) * cap, "the FLAC frames") ||
-          s->flac_frames_h.ensure(sizeof(some_flac_frame) * cap, "the FLAC frames"))
-        return -1;
-      if (some_flac_scan(up_d, flac_bytes, st_d, nf, static_cast<some_flac_frame*>(s->flac_frames_d.p), static_cast<int>(cap),
-                         count_d, s->flac_ws_d.p, s->stream))
-        return -1;
-      SOME_CUDA(cudaMemcpyAsync(s->flac_frames_h.p, count_d, sizeof(int), cudaMemcpyDeviceToHost, s->stream), "count download");
-      SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
-      n_cand = *static_cast<int*>(s->flac_frames_h.p);
-      if (n_cand <= cap) break;
-      cap = n_cand;
-    }
-    SOME_CUDA(cudaMemcpyAsync(s->flac_frames_h.p, s->flac_frames_d.p, sizeof(some_flac_frame) * n_cand, cudaMemcpyDeviceToHost,
-                              s->stream), "candidate download");
-    SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
-    frames_h = static_cast<const some_flac_frame*>(s->flac_frames_h.p);
-    std::vector<some_flac_range> recs(nf);
-    for (int k = 0; k < nf; ++k) {
-      const EncItem& it = its[flac[k]];
-      recs[k] = some_flac_range{it.up - it.m.data_offset, it.up, it.up + it.m.data_bytes, it.m.frames};
-    }
-    chain.resize(std::max(n_cand, 1));
+    if (dec.scan(s, cap, false)) return -1;
+    std::vector<int64_t> lengths(nf, 0);
+    dec.first.assign(nf + 1, 0);
+    dec.chain.resize(std::max(dec.n_cand, 1));
     int failed = -1;
-    if (some_flac_chain(frames_h, n_cand, recs.data(), nf, chain.data(), n_cand, first.data(), lengths.data(), &failed))
-      return item_error(failed >= 0 ? flac[failed] : 0);
+    if (some_flac_chain(dec.frames_h, dec.n_cand, recs.data(), nf, dec.chain.data(), dec.n_cand, dec.first.data(),
+                        lengths.data(), &failed))
+      return item_error(failed >= 0 ? dec.flac_of[failed] : 0);
+    dec.chain.resize(dec.first[nf]);
     for (int k = 0; k < nf; ++k) {
-      EncItem& it = its[flac[k]];
+      EncItem& it = its[dec.flac_of[k]];
       it.n = lengths[k];
       char who[96];
-      snprintf(who, sizeof(who), "some_session_transcribe_encoded: item %d", flac[k]);
+      snprintf(who, sizeof(who), "some_session_transcribe_encoded: item %d", dec.flac_of[k]);
       if (slice_shape(it.n, it.m.rate, sr, sl, who, &it.sh)) return -1;   // the length was not stated: checked now
     }
   }
 
-  // 3. the recordings' places, and one descriptor upload: the PCM items, the chained FLAC frames (their scratch and output
-  // offsets) and the status word, then the resampling and RMS windows
   Recordings rec;
   for (int i = 0; i < count; ++i) rec.items.push_back({its[i].m.rate, its[i].n, its[i].sh, out[i]});
-  const int kp = static_cast<int>(wav.size());
-  const int n_chain = nf ? static_cast<int>(first[nf]) : 0;
   Upload up{s};
-  const size_t pcm_off = up.add(static_cast<size_t>(some_pcm_decode_bytes(kp)));
-  const size_t chain_off = up.add(4ull * n_chain), soff_off = up.add(8ull * n_chain), ooff_off = up.add(8ull * n_chain);
-  const size_t status_off = up.add(2 * sizeof(int));
-  if (rec.place(s, sl, up)) return -1;
-  std::vector<some_pcm_item> pcm;
-  for (int i : wav) {
-    const EncItem& it = its[i];
-    pcm.push_back(some_pcm_item{up_d + it.up, it.n, it.m.channels, it.m.kind, 1, 0, rec.base + rec.items[i].x});
-  }
-  int64_t* scratch_off = reinterpret_cast<int64_t*>(up.h(soff_off));
-  int64_t* out_off = reinterpret_cast<int64_t*>(up.h(ooff_off));
-  int64_t scratch_total = 0;
-  for (int k = 0; k < nf; ++k) {
-    int64_t o = rec.items[flac[k]].x;
-    for (int64_t j = first[k]; j < first[k + 1]; ++j) {
-      const some_flac_frame& f = frames_h[chain[j]];
-      scratch_off[j] = scratch_total, out_off[j] = o;
-      scratch_total += static_cast<int64_t>(f.blocksize) * its[flac[k]].m.channels;
-      o += f.blocksize;
-    }
-  }
-  if (s->flac_scratch_d.ensure(4ull * scratch_total + 16, "the FLAC scratch") || some_pcm_decode_pack(pcm.data(), kp, up.h(pcm_off)))
+  dec.add(up);
+  if (rec.place(s, sl, up) || dec.fill(s, up, rec.base, [&](int i) { return rec.items[i].x; }) ||
+      up.send("descriptor upload") || dec.launch(s, up) || rec.launch(s, up))
     return -1;
-  if (n_chain) memcpy(up.h(chain_off), chain.data(), 4ull * n_chain);
-  int* status_h = reinterpret_cast<int*>(up.h(status_off));
-  int* status_d = reinterpret_cast<int*>(up.d(status_off));
-  status_h[0] = 0, status_h[1] = INT_MAX;                    // the first chained frame that fails to decode, if one does
-  if (up.send("descriptor upload")) return -1;
-  // 4. decode, resample, RMS; one download and one synchronise
-  if (some_pcm_decode(up.h(pcm_off), up.d(pcm_off), s->stream)) return -1;
-  if (n_chain &&
-      flac_decode_chain(up_d, st_d, static_cast<const some_flac_frame*>(s->flac_frames_d.p),
-                        reinterpret_cast<const int32_t*>(up.d(chain_off)), reinterpret_cast<const int64_t*>(up.d(soff_off)),
-                        reinterpret_cast<const int64_t*>(up.d(ooff_off)), n_chain, static_cast<int32_t*>(s->flac_scratch_d.p),
-                        rec.base, 1, status_d, status_d + 1, s->stream))
-    return -1;
-  if (rec.launch(s, up)) return -1;
-  SOME_CUDA(cudaMemcpyAsync(status_h, status_d, 2 * sizeof(int), cudaMemcpyDeviceToHost, s->stream), "status download");
   SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
-  if (status_h[0] != 0) {                          // the frame's item: the recording whose chain holds chain index k
-    const int64_t k = status_h[1];
-    int r = 0;
-    while (r + 1 < nf && first[r + 1] <= k) ++r;
-    const EncItem& it = its[flac[r]];
-    set_error("some_session_transcribe_encoded: item %d: FLAC frame at byte offset %lld failed to decode (status %d)", flac[r],
-              static_cast<long long>(frames_h[chain[k]].pos - (it.up - it.m.data_offset)), status_h[0]);
-    return -1;
-  }
-  // 5. the slicer per item, then one batch over the chunks of all items
+  const int failed = dec.check(up);
+  if (failed >= 0) return item_error(failed);
   return rec.finish(s, sl);
 }
 }  // namespace
@@ -1806,13 +1771,7 @@ extern "C" int some_session_transcribe_encoded(some_session* s, const some_encod
                  shared.first->second);
     EncItem& it = its[i];
     it.bytes = static_cast<const uint8_t*>(items[i].data);
-    if (some_audio_info(items[i].data, items[i].n_bytes, &it.m)) return item_error(i);
-    SOME_REQUIRE(it.m.container == SOME_AUDIO_FLAC || it.m.channels <= 128,
-                 "some_session_transcribe_encoded: item %d: a mono down-mix of %d channels (at most 128)", i, it.m.channels);
-    if (it.m.rate != sr) {                           // rate pairs the resampler does not support
-      long long t_end, x_first;
-      if (some_resample_window_plan(0, 0, 0, it.m.rate, sr, kKaiserTaps, &t_end, &x_first)) return item_error(i);
-    }
+    if (some_audio_info(items[i].data, items[i].n_bytes, &it.m) || check_format(it.m, sr)) return item_error(i);
     it.n = it.m.frames;
     if (it.m.container == SOME_AUDIO_WAV || it.m.frames > 0) {
       char who[96];
