@@ -126,8 +126,10 @@ class Engine:
         SiLU outputs, i.e. by the weights, and white noise calibrates equally well; with folded LayerNorms the operand is the
         normalised row itself and a voice-like signal matters: residual -7e-5 vs -1.5e-4) runs through the sequencer, which
         records the column means of every GEMM's effective operand (some_forward, `calib`), and each layer's bias absorbs
-        (W_master - bf16(W)) . mean.  After it the mean error of `bounds` is within +-1e-4 (clip dependent, +-3e-5 on most
-        clips) and zero-mean rounding noise remains.  (A second, head-level calibration against the library's own fp32 path
+        (W_master - bf16(W)) . mean.  Measured on an H100 over eight 30 s clips (tests/test_gpu_calibration.py), the mean
+        error of `bounds` per clip, 2e-4 to 3.4e-4 in magnitude without it (4e-5 for one model's folded sequence), is
+        3e-5 to 1.4e-4 on average with it and never above 2.1e-4, depending on the model and the launch sequence; the
+        rest is zero-mean rounding noise.  (A second, head-level calibration against the library's own fp32 path
         was tried and removed: what is left after this step depends on the input, not on the weights.)"""
         reg = getattr(self.w, 'rounding', None)
         if reg is None:
