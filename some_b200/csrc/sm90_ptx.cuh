@@ -267,7 +267,11 @@ __device__ __forceinline__ float tanh_approx(float x) {
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// sigmoid / SiLU through one MUFU.TANH (rel. error ~2^-11: below bf16 output resolution).
+// sigmoid / SiLU through one MUFU.TANH.  tanh.approx.f32 is within 2^-10.987 of tanh relative to tanh, so the error is
+// small against the INPUT, not the output: at most 0.5 |tanh(x/2)| 2^-10.987 (sigmoid_fast) and |x/2| |tanh(x/2)| 2^-10.987
+// (silu_fast) absolute.  For negative x the outputs shrink faster than that error: below x = -8.6 both are off by more
+// than one bf16 ulp of the exact output (measured on an H100), and where tanh(x/2) rounds to -1 they return exactly 0
+// (tests/test_gpu_gemm_epilogues.py::test_activations_across_the_range).
 __device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(0.5f, tanh_approx(0.5f * x), 0.5f); }
 __device__ __forceinline__ float silu_fast(float x) {
   float h = 0.5f * x;
