@@ -30,6 +30,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/some_b200.h"
@@ -63,57 +64,68 @@ const char* dtype_name(uint32_t dt) {
   return dt == DT_F32 ? "f32" : dt == DT_BF16 ? "bf16" : dt == DT_I32 ? "i32" : dt == DT_F64 ? "f64" : "?";
 }
 
+// A tensor of the model file and the device pointer field it sets: at byte `field` of some_block_weights `block`, or of
+// some_model when block < 0 (field < 0: the tensor is read by name).  A table row of count n > 1 is an array field, its
+// tensors name.0 .. name.{n-1}; rows of one count next to each other go index-major (ln_g.0, ln_b.0, ln_g.1, ...).
 struct Spec {
   std::string name;
   uint32_t dtype;
   std::vector<uint64_t> shape;
+  ptrdiff_t field = -1;
+  int count = 1, block = -1;
 };
 
-// The tensors a file of this geometry must hold (some_b200/export.py: tensor_specs writes the same list).
+// A pointer field's offset and its count, from the field itself: 1, or the length of an array of pointers.
+template <class F>
+constexpr int pointer_count() {
+  static_assert(std::is_pointer<typename std::remove_extent<F>::type>::value, "a tensor binds a pointer field");
+  return static_cast<int>(sizeof(F) / sizeof(void*));
+}
+#define FIELD(S, f) static_cast<ptrdiff_t>(offsetof(S, f)), pointer_count<decltype(S::f)>()
+#define BLOCK_FIELD(f) FIELD(some_block_weights, f)
+#define MODEL_FIELD(f) FIELD(some_model, f)
+constexpr uint64_t kDim = SOME_DIM, kFfn = 4 * SOME_DIM;
+// The tensors of one block, under "blk<j>." (some_b200/weights.py: BLOCK_TENSORS).
+const Spec kBlockRows[] = {
+    {"ln_g", DT_F32, {kDim}, BLOCK_FIELD(ln_g)}, {"ln_b", DT_F32, {kDim}, BLOCK_FIELD(ln_b)},
+    {"ffn_w1", DT_BF16, {kFfn, kDim}, BLOCK_FIELD(ffn_w1)}, {"ffn_b1", DT_F32, {kFfn}, BLOCK_FIELD(ffn_b1)},
+    {"ffn_w2", DT_BF16, {kDim, kFfn}, BLOCK_FIELD(ffn_w2)}, {"ffn_b2", DT_F32, {kDim}, BLOCK_FIELD(ffn_b2)},
+    {"w_qkv", DT_BF16, {3 * kDim, kDim}, BLOCK_FIELD(w_qkv)},
+    {"w_out", DT_BF16, {kDim, kDim}, BLOCK_FIELD(w_out)}, {"b_out", DT_F32, {kDim}, BLOCK_FIELD(b_out)},
+    {"w_pw1", DT_BF16, {2 * kDim, kDim}, BLOCK_FIELD(w_pw1)}, {"b_pw1", DT_F32, {2 * kDim}, BLOCK_FIELD(b_pw1)},
+    {"w_dw", DT_F32, {SOME_CONV_K, kDim}, BLOCK_FIELD(w_dw)}, {"b_dw", DT_F32, {kDim}, BLOCK_FIELD(b_dw)},
+    {"w_pw2", DT_BF16, {kDim, kDim}, BLOCK_FIELD(w_pw2)}, {"b_pw2", DT_F32, {kDim}, BLOCK_FIELD(b_pw2)}};
+const Spec kInputRows[] = {{"w_in", DT_BF16, {kDim, SOME_N_MELS}, MODEL_FIELD(w_in)}, {"b_in", DT_F32, {kDim}, MODEL_FIELD(b_in)}};
+const Spec kGluRows[] = {{"w", DT_BF16, {2 * kDim, kDim}}, {"b", DT_F32, {2 * kDim}}};     // under "glu<j>."
+
+template <size_t n>
+void add_rows(std::vector<Spec>& v, const std::string& prefix, int block, const Spec (&rows)[n]) {
+  for (size_t i = 0, end; i < n; i = end) {
+    for (end = i; end < n && rows[end].count == rows[i].count;) ++end;
+    for (int k = 0; k < rows[i].count; ++k)
+      for (size_t r = i; r < end; ++r) {
+        Spec s = rows[r];
+        if (s.count > 1) s.name += "." + std::to_string(k), s.field += k * static_cast<ptrdiff_t>(sizeof(void*));
+        s.name = prefix + s.name, s.count = 1, s.block = block;
+        v.push_back(s);
+      }
+  }
+}
+
+// The tensors a file of this geometry must hold, in file order (some_b200/export.py: tensor_specs writes the same list).
 std::vector<Spec> expected_tensors(int lay, int outdim) {
-  const uint64_t D = SOME_DIM, F = 4 * SOME_DIM;
+  const Spec head[] = {
+      {"w_head", DT_BF16, {static_cast<uint64_t>(outdim), kDim}, MODEL_FIELD(w_head)},
+      {"b_head", DT_F32, {static_cast<uint64_t>((outdim + 31) / 32 * 32)}, MODEL_FIELD(b_head)},
+      {"w_cut", DT_F32, {kDim}, MODEL_FIELD(w_cut)}, {"b_cut", DT_F32, {1}},
+      {"mel_start", DT_I32, {SOME_N_MELS}}, {"mel_count", DT_I32, {SOME_N_MELS}},
+      {"mel_weights", DT_F32, {SOME_N_MELS, SOME_MEL_MAXW}}, {"twiddle", DT_F32, {SOME_MEL_TW, 2}},
+      {"window", DT_F32, {SOME_N_FFT}}, {"kaiser_best", DT_F64, {kKaiserTaps}}};
   std::vector<Spec> v;
-  for (int s = 0; s < 2; ++s) {
-    v.push_back({"w_in." + std::to_string(s), DT_BF16, {D, SOME_N_MELS}});
-    v.push_back({"b_in." + std::to_string(s), DT_F32, {D}});
-  }
-  for (int j = 0; j < 2 * (lay + 1); ++j) {
-    const std::string p = "blk" + std::to_string(j) + ".";
-    for (int k = 0; k < 5; ++k) {
-      v.push_back({p + "ln_g." + std::to_string(k), DT_F32, {D}});
-      v.push_back({p + "ln_b." + std::to_string(k), DT_F32, {D}});
-    }
-    for (int k = 0; k < 2; ++k) {
-      const std::string q = "." + std::to_string(k);
-      v.push_back({p + "ffn_w1" + q, DT_BF16, {F, D}});
-      v.push_back({p + "ffn_b1" + q, DT_F32, {F}});
-      v.push_back({p + "ffn_w2" + q, DT_BF16, {D, F}});
-      v.push_back({p + "ffn_b2" + q, DT_F32, {D}});
-    }
-    v.push_back({p + "w_qkv", DT_BF16, {3 * D, D}});
-    v.push_back({p + "w_out", DT_BF16, {D, D}});
-    v.push_back({p + "b_out", DT_F32, {D}});
-    v.push_back({p + "w_pw1", DT_BF16, {2 * D, D}});
-    v.push_back({p + "b_pw1", DT_F32, {2 * D}});
-    v.push_back({p + "w_dw", DT_F32, {SOME_CONV_K, D}});
-    v.push_back({p + "b_dw", DT_F32, {D}});
-    v.push_back({p + "w_pw2", DT_BF16, {D, D}});
-    v.push_back({p + "b_pw2", DT_F32, {D}});
-  }
-  for (int j = 0; j < 2 * lay; ++j) {
-    v.push_back({"glu" + std::to_string(j) + ".w", DT_BF16, {2 * D, D}});
-    v.push_back({"glu" + std::to_string(j) + ".b", DT_F32, {2 * D}});
-  }
-  v.push_back({"w_head", DT_BF16, {static_cast<uint64_t>(outdim), D}});
-  v.push_back({"b_head", DT_F32, {static_cast<uint64_t>((outdim + 31) / 32 * 32)}});
-  v.push_back({"w_cut", DT_F32, {D}});
-  v.push_back({"b_cut", DT_F32, {1}});
-  v.push_back({"mel_start", DT_I32, {SOME_N_MELS}});
-  v.push_back({"mel_count", DT_I32, {SOME_N_MELS}});
-  v.push_back({"mel_weights", DT_F32, {SOME_N_MELS, SOME_MEL_MAXW}});
-  v.push_back({"twiddle", DT_F32, {SOME_MEL_TW, 2}});
-  v.push_back({"window", DT_F32, {SOME_N_FFT}});
-  v.push_back({"kaiser_best", DT_F64, {kKaiserTaps}});
+  add_rows(v, "", -1, kInputRows);
+  for (int j = 0; j < 2 * (lay + 1); ++j) add_rows(v, "blk" + std::to_string(j) + ".", j, kBlockRows);
+  for (int j = 0; j < 2 * lay; ++j) add_rows(v, "glu" + std::to_string(j) + ".", -1, kGluRows);
+  add_rows(v, "", -1, head);
   return v;
 }
 
@@ -660,35 +672,24 @@ extern "C" int some_session_open(const char* path, int device, some_session** ou
   }
   uint8_t* base = static_cast<uint8_t*>(s->weights);
   auto dp = [&](const std::string& name) -> const void* { return base + (dir.at(name).off - data_off); };
-  auto bf = [&](const std::string& n) { return static_cast<const uint16_t*>(dp(n)); };
   auto fl = [&](const std::string& n) { return static_cast<const float*>(dp(n)); };
-  s->blocks.resize(2 * (lay + 1));
-  for (int j = 0; j < 2 * (lay + 1); ++j) {
-    const std::string p = "blk" + std::to_string(j) + ".";
-    some_block_weights& b = s->blocks[j];
-    memset(&b, 0, sizeof(b));
-    for (int k = 0; k < 5; ++k) b.ln_g[k] = fl(p + "ln_g." + std::to_string(k)), b.ln_b[k] = fl(p + "ln_b." + std::to_string(k));
-    for (int k = 0; k < 2; ++k) {
-      const std::string q = "." + std::to_string(k);
-      b.ffn_w1[k] = bf(p + "ffn_w1" + q), b.ffn_b1[k] = fl(p + "ffn_b1" + q);
-      b.ffn_w2[k] = bf(p + "ffn_w2" + q), b.ffn_b2[k] = fl(p + "ffn_b2" + q);
-    }
-    b.w_qkv = bf(p + "w_qkv"), b.w_out = bf(p + "w_out"), b.b_out = fl(p + "b_out");
-    b.w_pw1 = bf(p + "w_pw1"), b.b_pw1 = fl(p + "b_pw1"), b.w_dw = fl(p + "w_dw"), b.b_dw = fl(p + "b_dw");
-    b.w_pw2 = bf(p + "w_pw2"), b.b_pw2 = fl(p + "b_pw2");
+  some_model& m = s->model;
+  s->blocks.resize(2 * (lay + 1));            // value-initialised: the LayerNorm-folded fields stay null
+  for (const Spec& sp : specs) {
+    if (sp.field < 0) continue;
+    const void* p = dp(sp.name);
+    void* target = sp.block < 0 ? static_cast<void*>(&m) : static_cast<void*>(&s->blocks[sp.block]);
+    memcpy(static_cast<uint8_t*>(target) + sp.field, &p, sizeof(p));
   }
   for (int j = 0; j < 2 * lay; ++j) {
-    s->glu_w.push_back(bf("glu" + std::to_string(j) + ".w"));
+    s->glu_w.push_back(static_cast<const uint16_t*>(dp("glu" + std::to_string(j) + ".w")));
     s->glu_b.push_back(fl("glu" + std::to_string(j) + ".b"));
   }
   if (lay == 0) s->glu_w.push_back(nullptr), s->glu_b.push_back(nullptr);
-  some_model& m = s->model;
   m.lay = lay, m.outdim = outdim;
-  for (int k = 0; k < 2; ++k) m.w_in[k] = bf("w_in." + std::to_string(k)), m.b_in[k] = fl("b_in." + std::to_string(k));
   m.blocks = s->blocks.data();
   m.glu_w = s->glu_w.data();
   m.glu_b = s->glu_b.data();
-  m.w_head = bf("w_head"), m.b_head = fl("b_head"), m.w_cut = fl("w_cut");
   const Entry& bc = dir.at("b_cut");
   m.b_cut = rd<float>(f + bc.off);               // a host scalar of some_model
   m.ln_fold = 0;                                  // the default stand-alone LayerNorm sequence

@@ -30,31 +30,17 @@ ALIGN = 256
 DTYPES = {np.dtype('<f4'): 1, np.dtype('<u2'): 2, np.dtype('<i4'): 3, np.dtype('<f8'): 4}   # u2 = raw bfloat16
 KAISER_TAPS = 32769
 DIM, FFN, N_MELS, CONV_K, MEL_MAXW, MEL_TW, N_FFT, HOP = 512, 2048, 80, 31, 24, 1396, 2048, 512
+# the tables of the front end, after the model's tensors (weights.model_tensors)
+FRONT_END = [('mel_start', np.dtype('<i4'), (N_MELS,)), ('mel_count', np.dtype('<i4'), (N_MELS,)),
+             ('mel_weights', np.dtype('<f4'), (N_MELS, MEL_MAXW)), ('twiddle', np.dtype('<f4'), (MEL_TW, 2)),
+             ('window', np.dtype('<f4'), (N_FFT,)), ('kaiser_best', np.dtype('<f8'), (KAISER_TAPS,))]
 
 
 def tensor_specs(lay: int, outdim: int) -> List[Tuple[str, np.dtype, Tuple[int, ...]]]:
     """The tensors of a model file, in file order: (name, dtype, shape).  ``some_session_open`` expects exactly these."""
-    f32, bf, i32, f64 = np.dtype('<f4'), np.dtype('<u2'), np.dtype('<i4'), np.dtype('<f8')
-    v = []
-    for s in range(2):
-        v += [(f'w_in.{s}', bf, (DIM, N_MELS)), (f'b_in.{s}', f32, (DIM,))]
-    for j in range(2 * (lay + 1)):                   # block i of stream s is entry 2 i + s (some_model.blocks)
-        p = f'blk{j}.'
-        for k in range(5):
-            v += [(f'{p}ln_g.{k}', f32, (DIM,)), (f'{p}ln_b.{k}', f32, (DIM,))]
-        for k in range(2):
-            v += [(f'{p}ffn_w1.{k}', bf, (FFN, DIM)), (f'{p}ffn_b1.{k}', f32, (FFN,)),
-                  (f'{p}ffn_w2.{k}', bf, (DIM, FFN)), (f'{p}ffn_b2.{k}', f32, (DIM,))]
-        v += [(p + 'w_qkv', bf, (3 * DIM, DIM)), (p + 'w_out', bf, (DIM, DIM)), (p + 'b_out', f32, (DIM,)),
-              (p + 'w_pw1', bf, (2 * DIM, DIM)), (p + 'b_pw1', f32, (2 * DIM,)), (p + 'w_dw', f32, (CONV_K, DIM)),
-              (p + 'b_dw', f32, (DIM,)), (p + 'w_pw2', bf, (DIM, DIM)), (p + 'b_pw2', f32, (DIM,))]
-    for j in range(2 * lay):                         # 2 i + 0 = glu1 (fed by midi), 2 i + 1 = glu2
-        v += [(f'glu{j}.w', bf, (2 * DIM, DIM)), (f'glu{j}.b', f32, (2 * DIM,))]
-    v += [('w_head', bf, (outdim, DIM)), ('b_head', f32, ((outdim + 31) // 32 * 32,)), ('w_cut', f32, (DIM,)),
-          ('b_cut', f32, (1,)),
-          ('mel_start', i32, (N_MELS,)), ('mel_count', i32, (N_MELS,)), ('mel_weights', f32, (N_MELS, MEL_MAXW)),
-          ('twiddle', f32, (MEL_TW, 2)), ('window', f32, (N_FFT,)), ('kaiser_best', f64, (KAISER_TAPS,))]
-    return v
+    from .weights import model_tensors
+    dims = {'outdim': outdim, 'outdim32': (outdim + 31) // 32 * 32}
+    return [(t.key, t.dtype, tuple(dims.get(d, d) for d in t.shape)) for t in model_tensors(lay)] + FRONT_END
 
 
 def write_model_file(path, scalars: dict, tensors: Dict[str, np.ndarray]) -> List[dict]:
@@ -104,30 +90,16 @@ def engine_tensors(engine) -> Dict[str, np.ndarray]:
     import torch
 
     from .audio import kaiser_best_table
+    from .weights import model_tensors, packed_tensor
 
     def host(t):
+        if isinstance(t, float):                    # b_cut, a host scalar of the engine
+            return np.array([t], dtype='<f4')
         t = t.detach().contiguous().cpu()
         return t.view(torch.uint16).numpy() if t.dtype == torch.bfloat16 else t.numpy()
 
-    w, out = engine.w, {}
-    for s in range(2):
-        out[f'w_in.{s}'], out[f'b_in.{s}'] = host(w.w_in[s]), host(w.b_in[s])
-    for i, pair in enumerate(w.blocks):
-        for s, bw in enumerate(pair):
-            p = f'blk{2 * i + s}.'
-            for k in range(5):
-                out[f'{p}ln_g.{k}'], out[f'{p}ln_b.{k}'] = host(bw.ln_g[k]), host(bw.ln_b[k])
-            for k in range(2):
-                f = bw.ffn[k]
-                out[f'{p}ffn_w1.{k}'], out[f'{p}ffn_b1.{k}'] = host(f['w1']), host(f['b1'])
-                out[f'{p}ffn_w2.{k}'], out[f'{p}ffn_b2.{k}'] = host(f['w2']), host(f['b2'])
-            for k in ('w_qkv', 'w_out', 'b_out', 'w_pw1', 'b_pw1', 'w_dw', 'b_dw', 'w_pw2', 'b_pw2'):
-                out[p + k] = host(getattr(bw, k))
-    for i in range(w.lay):
-        for s in range(2):
-            out[f'glu{2 * i + s}.w'], out[f'glu{2 * i + s}.b'] = host(w.glu_w[i][s]), host(w.glu_b[i][s])
-    out['w_head'], out['b_head'], out['w_cut'] = host(w.w_head), host(w.b_head), host(w.w_cut)
-    out['b_cut'] = np.array([w.b_cut], dtype='<f4')
+    w = engine.w
+    out = {t.key: host(packed_tensor(w, t)) for t in model_tensors(w.lay)}
     for k in ('mel_start', 'mel_count', 'mel_weights', 'twiddle', 'window'):
         out[k] = host(engine.mel[k])
     out['kaiser_best'] = np.asarray(kaiser_best_table(), dtype='<f8')

@@ -15,13 +15,16 @@
 """
 from __future__ import annotations
 
+import itertools
+from collections import namedtuple
+from types import SimpleNamespace
 from typing import Dict, List
 
 import numpy as np
 import torch
 
 from . import _lib
-from .config import DIM
+from .config import DIM, FFN_DIM
 
 BN_EPS = 1e-5
 
@@ -121,33 +124,44 @@ class RoundingRegistry:
         self.entries[w.data_ptr()] = (m, ww, bias)
 
 
+def checkpoint_block(sd, p: str) -> SimpleNamespace:
+    """The checkpoint tensors of one conform_blocke under BlockWeights' names: to_q | to_kv concatenated, 1x1 convolutions
+    squeezed to [N, K], BatchNorm folded into the depthwise taps in float64, taps transposed to [K][C].  Neither rounded nor
+    GLU-packed: the fp32 validation path runs them as they are, BlockWeights packs them."""
+    d = lambda n: sd[f'{p}.{n}'].double()
+    scale = d('conv.norm.weight') / torch.sqrt(d('conv.norm.running_var') + BN_EPS)
+    return SimpleNamespace(
+        ln_g=[sd[f'{p}.norm{i}.weight'] for i in range(1, 6)], ln_b=[sd[f'{p}.norm{i}.bias'] for i in range(1, 6)],
+        ffn=[dict(w1=sd[f'{p}.{f}.ln1.weight'], b1=sd[f'{p}.{f}.ln1.bias'], w2=sd[f'{p}.{f}.ln2.weight'],
+                  b2=sd[f'{p}.{f}.ln2.bias']) for f in ('ffn1', 'ffn2')],
+        w_qkv=torch.cat([sd[f'{p}.att.to_q.weight'], sd[f'{p}.att.to_kv.weight']], dim=0),
+        w_out=sd[f'{p}.att.to_out.0.weight'], b_out=sd[f'{p}.att.to_out.0.bias'],
+        w_pw1=sd[f'{p}.conv.pointwise_conv1.weight'][:, :, 0], b_pw1=sd[f'{p}.conv.pointwise_conv1.bias'],
+        w_dw=(d('conv.depthwise_conv.weight')[:, 0, :] * scale[:, None]).t(),
+        b_dw=(d('conv.depthwise_conv.bias') - d('conv.norm.running_mean')) * scale + d('conv.norm.bias'),
+        w_pw2=sd[f'{p}.conv.pointwise_conv2.weight'][:, :, 0], b_pw2=sd[f'{p}.conv.pointwise_conv2.bias'])
+
+
 class BlockWeights:
     """Device tensors of one conform_blocke (Gconform.py:37-63)."""
 
     def __init__(self, sd, p: str, device, reg: 'RoundingRegistry'):
         f32 = lambda t: t.to(device=device, dtype=torch.float32).contiguous()
-
-        def bf(t, bias=None):
-            return reg.round(t, bias)
-
-        self.ln_g = [f32(sd[f'{p}.norm{i}.weight']) for i in range(1, 6)]
-        self.ln_b = [f32(sd[f'{p}.norm{i}.bias']) for i in range(1, 6)]
+        bf = reg.round
+        c = checkpoint_block(sd, p)
+        self.ln_g, self.ln_b = [f32(t) for t in c.ln_g], [f32(t) for t in c.ln_b]
         self.ffn = []
-        for name in ('ffn1', 'ffn2'):
-            b1, b2 = f32(sd[f'{p}.{name}.ln1.bias']), f32(sd[f'{p}.{name}.ln2.bias'])
-            self.ffn.append(dict(w1=bf(sd[f'{p}.{name}.ln1.weight'], b1), b1=b1, w2=bf(sd[f'{p}.{name}.ln2.weight'], b2), b2=b2))
-        self.w_qkv = bf(torch.cat([sd[f'{p}.att.to_q.weight'], sd[f'{p}.att.to_kv.weight']], dim=0))   # no bias to correct
-        self.b_out = f32(sd[f'{p}.att.to_out.0.bias'])
-        self.w_out = bf(sd[f'{p}.att.to_out.0.weight'], self.b_out)
-        self.b_pw1 = f32(glu_pack_rows(sd[f'{p}.conv.pointwise_conv1.bias']))
-        self.w_pw1 = bf(glu_pack_rows(sd[f'{p}.conv.pointwise_conv1.weight'][:, :, 0]), self.b_pw1)
-        scale = sd[f'{p}.conv.norm.weight'].double() / torch.sqrt(sd[f'{p}.conv.norm.running_var'].double() + BN_EPS)
-        dw = sd[f'{p}.conv.depthwise_conv.weight'][:, 0, :].double()            # [C, K]
-        self.w_dw = f32((dw * scale[:, None]).t())                              # [K, C]
-        self.b_dw = f32((sd[f'{p}.conv.depthwise_conv.bias'].double() - sd[f'{p}.conv.norm.running_mean'].double())
-                        * scale + sd[f'{p}.conv.norm.bias'].double())
-        self.b_pw2 = f32(sd[f'{p}.conv.pointwise_conv2.bias'])
-        self.w_pw2 = bf(sd[f'{p}.conv.pointwise_conv2.weight'][:, :, 0], self.b_pw2)
+        for f in c.ffn:
+            b1, b2 = f32(f['b1']), f32(f['b2'])
+            self.ffn.append(dict(w1=bf(f['w1'], b1), b1=b1, w2=bf(f['w2'], b2), b2=b2))
+        self.w_qkv = bf(c.w_qkv)                        # no bias to correct
+        self.b_out = f32(c.b_out)
+        self.w_out = bf(c.w_out, self.b_out)
+        self.b_pw1 = f32(glu_pack_rows(c.b_pw1))
+        self.w_pw1 = bf(glu_pack_rows(c.w_pw1), self.b_pw1)
+        self.w_dw, self.b_dw = f32(c.w_dw), f32(c.b_dw)
+        self.b_pw2 = f32(c.b_pw2)
+        self.w_pw2 = bf(c.w_pw2, self.b_pw2)
 
         # ---- LayerNorm-folded consumers: (norm index, weight [N, 512], bias or None) -> (W' bf16, s f32, b' f32)
         def fold(i, w, b, pack=lambda t: t):
@@ -158,126 +172,136 @@ class BlockWeights:
             s_col = wf.double().sum(dim=1)                           # sums of the ROUNDED operand the tensor core sees
             return wf, f32(s_col), bias
 
-        self.ffn_fold = [fold(1, sd[f'{p}.ffn1.ln1.weight'], sd[f'{p}.ffn1.ln1.bias']),
-                         fold(4, sd[f'{p}.ffn2.ln1.weight'], sd[f'{p}.ffn2.ln1.bias'])]
-        self.qkv_fold = fold(2, torch.cat([sd[f'{p}.att.to_q.weight'], sd[f'{p}.att.to_kv.weight']], dim=0), None)
-        self.pw1_fold = fold(3, sd[f'{p}.conv.pointwise_conv1.weight'][:, :, 0], sd[f'{p}.conv.pointwise_conv1.bias'],
-                             pack=glu_pack_rows)
+        self.ffn_fold = [fold(i, f['w1'], f['b1']) for i, f in zip((1, 4), c.ffn)]
+        self.qkv_fold = fold(2, c.w_qkv, None)
+        self.pw1_fold = fold(3, c.w_pw1, c.b_pw1, pack=glu_pack_rows)
 
 
 class ModelWeights:
     """All device tensors of Gmidi_conform (Gconform.py:92-140); index 0 = midi stream (att1), 1 = bound (att2)."""
 
     def __init__(self, sd, config: dict, device):
-        args = config['midi_extractor_args']
-        self.lay = args['lay']
-        self.outdim = config['midi_num_bins']
+        c = checkpoint_model(sd, config)
+        self.lay, self.outdim = c.lay, c.outdim
         self.rounding = reg = RoundingRegistry(device)      # dropped by Engine.calibrate()
         bf = reg.round
         f32 = lambda t: t.to(device=device, dtype=torch.float32).contiguous()
-        self.b_in = [f32(sd['model.inln.bias']), f32(sd['model.inln1.bias'])]
-        self.w_in = [bf(sd['model.inln.weight'], self.b_in[0]), bf(sd['model.inln1.weight'], self.b_in[1])]
-        self.blocks: List[List[BlockWeights]] = []      # [lay + 1][2]
-        self.glu_w, self.glu_b = [], []                 # [lay][2]: index 0 = glu1 (fed by midi), 1 = glu2 (fed by bound)
-        for i in range(self.lay):
-            p = f'model.cf_lay.{i}'
-            self.blocks.append([BlockWeights(sd, p + '.att1', device, reg), BlockWeights(sd, p + '.att2', device, reg)])
-            self.glu_b.append([f32(glu_pack_rows(sd[p + '.glu1.0.bias'])), f32(glu_pack_rows(sd[p + '.glu2.0.bias']))])
-            self.glu_w.append([bf(glu_pack_rows(sd[p + '.glu1.0.weight']), self.glu_b[-1][0]),
-                               bf(glu_pack_rows(sd[p + '.glu2.0.weight']), self.glu_b[-1][1])])
-        self.blocks.append([BlockWeights(sd, 'model.att1', device, reg), BlockWeights(sd, 'model.att2', device, reg)])
-        self.b_head = f32(_pad32(sd['model.outln.bias']))
-        self.w_head = bf(sd['model.outln.weight'], self.b_head)          # [outdim, 512]
-        self.w_cut = f32(sd['model.cutheard.weight'][0])                 # [512]
-        self.b_cut = float(sd['model.cutheard.bias'][0])
+        self.b_in = [f32(t) for t in c.b_in]
+        self.w_in = [bf(t, b) for t, b in zip(c.w_in, self.b_in)]
+        self.blocks: List[List[BlockWeights]] = [[BlockWeights(sd, p, device, reg) for p in ps] for ps in c.prefixes]
+        # [lay][2]: index 0 = glu1 (fed by midi), 1 = glu2 (fed by bound)
+        self.glu_b = [[f32(glu_pack_rows(t)) for t in pair] for pair in c.glu_b]
+        self.glu_w = [[bf(glu_pack_rows(t), b) for t, b in zip(ws, bs)] for ws, bs in zip(c.glu_w, self.glu_b)]
+        self.b_head = f32(_pad32(c.b_head))
+        self.w_head = bf(c.w_head, self.b_head)                          # [outdim, 512]
+        self.w_cut, self.b_cut = f32(c.w_cut), c.b_cut                   # [512], a float
         assert self.w_in[0].shape == (DIM, config['units_dim'])
+
+
+# --------------------------------------------------------------------------- the packed model's tensors
+BF16, F32 = np.dtype('<u2'), np.dtype('<f4')       # as the model file stores them: bf16 as its raw bits
+# The model file's tensors of a block, keys under 'blk{j}.': (some_block_weights field, count, dtype, shape).  BlockWeights
+# holds ffn_w1 .. ffn_b2 as ffn[k]['w1'] .., every other field under its own name.
+BLOCK_TENSORS = [
+    ('ln_g', 5, F32, (DIM,)), ('ln_b', 5, F32, (DIM,)),
+    ('ffn_w1', 2, BF16, (FFN_DIM, DIM)), ('ffn_b1', 2, F32, (FFN_DIM,)),
+    ('ffn_w2', 2, BF16, (DIM, FFN_DIM)), ('ffn_b2', 2, F32, (DIM,)),
+    ('w_qkv', 1, BF16, (3 * DIM, DIM)), ('w_out', 1, BF16, (DIM, DIM)), ('b_out', 1, F32, (DIM,)),
+    ('w_pw1', 1, BF16, (2 * DIM, DIM)), ('b_pw1', 1, F32, (2 * DIM,)),
+    ('w_dw', 1, F32, (_lib.CONV_K, DIM)), ('b_dw', 1, F32, (DIM,)),
+    ('w_pw2', 1, BF16, (DIM, DIM)), ('b_pw2', 1, F32, (DIM,))]
+# The LayerNorm-folded consumers (some_model.ln_fold), packed at load time, never written to a model file: the BlockWeights
+# triples (W', s, b'), their count and their some_block_weights fields.
+FOLDED_TENSORS = [('ffn_fold', 2, ('ffn_w1f', 'ffn_s1', 'ffn_b1f')), ('qkv_fold', 1, ('w_qkvf', 's_qkv', 'b_qkvf')),
+                  ('pw1_fold', 1, ('w_pw1f', 's_pw1', 'b_pw1f'))]
+# The model-level tensors before and after the blocks; 'outdim' / 'outdim32': the head width, and it padded to 32 lanes.
+INPUT_TENSORS = [('w_in', 2, BF16, (DIM, _lib.N_MELS)), ('b_in', 2, F32, (DIM,))]
+HEAD_TENSORS = [('w_head', 1, BF16, ('outdim', DIM)), ('b_head', 1, F32, ('outdim32',)), ('w_cut', 1, F32, (DIM,)),
+                ('b_cut', 1, F32, (1,))]
+# Tensor: key None for the folded ones, block None for the model level; index: into an array field.
+Tensor = namedtuple('Tensor', 'key block field index dtype shape')
+
+
+def model_tensors(lay: int, folded: bool = False) -> List[Tensor]:
+    """Every tensor of a packed model with `lay` conformer layers in the model file's order, then the folded ones if
+    `folded`.  An array field's tensors go index-major with the rows of its count (ln_g.0, ln_b.0, ln_g.1, ...).  Block i of
+    stream s is entry j = 2 i + s of some_model.blocks; GLU mix j = 2 i + 0 is glu1 (fed by midi), 2 i + 1 glu2."""
+    def rows(table, prefix='', block=None):
+        for count, group in itertools.groupby(table, key=lambda r: r[1]):
+            group = list(group)
+            yield from (Tensor(prefix + (f'{f}.{k}' if count > 1 else f), block, f, k if count > 1 else None, dt, shape)
+                        for k in range(count) for f, _, dt, shape in group)
+
+    out = [*rows(INPUT_TENSORS), *(t for j in range(2 * (lay + 1)) for t in rows(BLOCK_TENSORS, f'blk{j}.', j))]
+    out += [Tensor(f'glu{j}.{x}', None, f'glu_{x}', j, dt, shape) for j in range(2 * lay)
+            for x, dt, shape in (('w', BF16, (2 * DIM, DIM)), ('b', F32, (2 * DIM,)))]
+    out += rows(HEAD_TENSORS)
+    return out + [Tensor(None, j, f, k if count > 1 else None, None, None) for j in range(2 * (lay + 1)) if folded
+                  for _, count, fields in FOLDED_TENSORS for k in range(count) for f in fields]
+
+
+def packed_tensor(w, t: Tensor):
+    """Tensor t in w: a ModelWeights, or the checkpoint_model it was packed from (b_cut: a float)."""
+    obj = w if t.block is None else w.blocks[t.block // 2][t.block % 2]
+    if t.field.startswith('glu_'):
+        return getattr(obj, t.field)[t.index // 2][t.index % 2]
+    name, pos = next(((n, fs.index(t.field)) for n, _, fs in FOLDED_TENSORS if t.field in fs),
+                     ('ffn', t.field[4:]) if t.field.startswith('ffn_') else (t.field, None))
+    v = getattr(obj, name) if t.index is None else getattr(obj, name)[t.index]
+    return v if pos is None else v[pos]
+
+
+def _c_model(model_t, block_t, w, folded: bool, upload=lambda t: t):
+    """A model_t (ModelC / ModelF32C) pointing to the tensors of w (ModelWeights or checkpoint_model), each passed through
+    upload.  Returns (struct, keepalive): the struct only holds raw pointers, `keepalive` owns the arrays."""
+    import ctypes as C
+    blocks = (block_t * (2 * (w.lay + 1)))()
+    glu_w, glu_b = (C.c_void_p * max(2 * w.lay, 1))(), (C.c_void_p * max(2 * w.lay, 1))()
+    m = model_t(lay=w.lay, outdim=w.outdim, blocks=C.cast(blocks, C.POINTER(block_t)),
+                glu_w=C.cast(glu_w, C.POINTER(C.c_void_p)), glu_b=C.cast(glu_b, C.POINTER(C.c_void_p)))
+    for t in model_tensors(w.lay, folded):
+        s, v = m if t.block is None else blocks[t.block], packed_tensor(w, t)
+        if not hasattr(type(s), t.field):
+            raise AttributeError(f'{type(s).__name__} has no field {t.field!r}')
+        v = v if isinstance(v, float) else upload(v).data_ptr()
+        if t.index is None:
+            setattr(s, t.field, v)
+        else:
+            getattr(s, t.field)[t.index] = v
+    return m, (blocks, glu_w, glu_b)
 
 
 def build_c_model(w: ModelWeights, ln_fold: bool = True):
     """ctypes mirror (include/some_b200.h: some_model) of the packed weights for the native launch sequencer
     some_forward.  Returns (ModelC, keepalive): the struct only holds raw pointers, `keepalive` owns the arrays."""
-    import ctypes as C
-    nblk = (w.lay + 1) * 2
-    blocks = (_lib.BlockWeightsC * nblk)()
-    for i, pair in enumerate(w.blocks):
-        for s, bw in enumerate(pair):
-            b = blocks[2 * i + s]
-            for k in range(5):
-                b.ln_g[k], b.ln_b[k] = bw.ln_g[k].data_ptr(), bw.ln_b[k].data_ptr()
-            for k in range(2):
-                f = bw.ffn[k]
-                b.ffn_w1[k], b.ffn_b1[k] = f['w1'].data_ptr(), f['b1'].data_ptr()
-                b.ffn_w2[k], b.ffn_b2[k] = f['w2'].data_ptr(), f['b2'].data_ptr()
-            b.w_qkv, b.w_out, b.b_out = bw.w_qkv.data_ptr(), bw.w_out.data_ptr(), bw.b_out.data_ptr()
-            b.w_pw1, b.b_pw1 = bw.w_pw1.data_ptr(), bw.b_pw1.data_ptr()
-            b.w_dw, b.b_dw = bw.w_dw.data_ptr(), bw.b_dw.data_ptr()
-            b.w_pw2, b.b_pw2 = bw.w_pw2.data_ptr(), bw.b_pw2.data_ptr()
-            for k in range(2):
-                b.ffn_w1f[k], b.ffn_s1[k], b.ffn_b1f[k] = (t.data_ptr() for t in bw.ffn_fold[k])
-            b.w_qkvf, b.s_qkv, b.b_qkvf = (t.data_ptr() for t in bw.qkv_fold)
-            b.w_pw1f, b.s_pw1, b.b_pw1f = (t.data_ptr() for t in bw.pw1_fold)
-    n_glu = max(w.lay * 2, 1)
-    glu_w = (C.c_void_p * n_glu)()
-    glu_b = (C.c_void_p * n_glu)()
-    for i in range(w.lay):
-        for s in range(2):
-            glu_w[2 * i + s] = w.glu_w[i][s].data_ptr()
-            glu_b[2 * i + s] = w.glu_b[i][s].data_ptr()
-    m = _lib.ModelC()
-    m.lay, m.outdim = w.lay, w.outdim
-    for s in range(2):
-        m.w_in[s], m.b_in[s] = w.w_in[s].data_ptr(), w.b_in[s].data_ptr()
-    m.blocks = C.cast(blocks, C.POINTER(_lib.BlockWeightsC))
-    m.glu_w = C.cast(glu_w, C.POINTER(C.c_void_p))
-    m.glu_b = C.cast(glu_b, C.POINTER(C.c_void_p))
-    m.w_head, m.b_head, m.w_cut, m.b_cut = w.w_head.data_ptr(), w.b_head.data_ptr(), w.w_cut.data_ptr(), w.b_cut
+    m, keep = _c_model(_lib.ModelC, _lib.BlockWeightsC, w, folded=True)
     m.ln_fold = int(bool(ln_fold))
-    return m, (blocks, glu_w, glu_b)
+    return m, keep
+
+
+def checkpoint_model(sd, config: dict) -> SimpleNamespace:
+    """The model-level checkpoint tensors under ModelWeights' names, unpacked like checkpoint_block, and the checkpoint
+    prefixes of the blocks ([lay + 1][2], as ModelWeights.blocks)."""
+    lay = config['midi_extractor_args']['lay']
+    glu = lambda kind: [[sd[f'model.cf_lay.{i}.glu{s}.0.{kind}'] for s in (1, 2)] for i in range(lay)]
+    return SimpleNamespace(
+        lay=lay, outdim=config['midi_num_bins'], w_in=[sd['model.inln.weight'], sd['model.inln1.weight']],
+        b_in=[sd['model.inln.bias'], sd['model.inln1.bias']], glu_w=glu('weight'), glu_b=glu('bias'),
+        prefixes=[[f'model.cf_lay.{i}.att1', f'model.cf_lay.{i}.att2'] for i in range(lay)] + [['model.att1', 'model.att2']],
+        w_head=sd['model.outln.weight'], b_head=sd['model.outln.bias'], w_cut=sd['model.cutheard.weight'][0],
+        b_cut=float(sd['model.cutheard.bias'][0]))
 
 
 def build_f32_model(sd, config: dict, device):
-    """fp32 weights of the validation path (some_forward_f32, csrc/accurate.cu): the checkpoint's own tensors in nn.Linear
-    layout, to_q | to_kv concatenated, BatchNorm folded into the depthwise taps (in double), nothing rounded or packed.
-    Returns (ModelF32C, keepalive)."""
-    import ctypes as C
-    f32 = lambda t: t.to(device=device, dtype=torch.float32).contiguous()
+    """fp32 weights of the validation path (some_forward_f32, csrc/accurate.cu): checkpoint_model and checkpoint_block,
+    nothing rounded or packed.  Returns (ModelF32C, keepalive)."""
     keep = []
 
-    def ptr(t):
-        t = f32(t)
-        keep.append(t)
-        return t.data_ptr()
+    def upload(t):
+        keep.append(t.to(device=device, dtype=torch.float32).contiguous())
+        return keep[-1]
 
-    lay, outdim = config['midi_extractor_args']['lay'], config['midi_num_bins']
-    prefixes = [f'model.cf_lay.{i}.att{s}' for i in range(lay) for s in (1, 2)] + ['model.att1', 'model.att2']
-    blocks = (_lib.BlockWeightsF32C * len(prefixes))()
-    for b, p in zip(blocks, prefixes):
-        for k in range(5):
-            b.ln_g[k], b.ln_b[k] = ptr(sd[f'{p}.norm{k + 1}.weight']), ptr(sd[f'{p}.norm{k + 1}.bias'])
-        for k, name in enumerate(('ffn1', 'ffn2')):
-            b.ffn_w1[k], b.ffn_b1[k] = ptr(sd[f'{p}.{name}.ln1.weight']), ptr(sd[f'{p}.{name}.ln1.bias'])
-            b.ffn_w2[k], b.ffn_b2[k] = ptr(sd[f'{p}.{name}.ln2.weight']), ptr(sd[f'{p}.{name}.ln2.bias'])
-        b.w_qkv = ptr(torch.cat([sd[f'{p}.att.to_q.weight'], sd[f'{p}.att.to_kv.weight']], dim=0))
-        b.w_out, b.b_out = ptr(sd[f'{p}.att.to_out.0.weight']), ptr(sd[f'{p}.att.to_out.0.bias'])
-        b.w_pw1, b.b_pw1 = ptr(sd[f'{p}.conv.pointwise_conv1.weight'][:, :, 0]), ptr(sd[f'{p}.conv.pointwise_conv1.bias'])
-        scale = sd[f'{p}.conv.norm.weight'].double() / torch.sqrt(sd[f'{p}.conv.norm.running_var'].double() + BN_EPS)
-        dw = sd[f'{p}.conv.depthwise_conv.weight'][:, 0, :].double()
-        b.w_dw = ptr((dw * scale[:, None]).t())
-        b.b_dw = ptr((sd[f'{p}.conv.depthwise_conv.bias'].double() - sd[f'{p}.conv.norm.running_mean'].double()) * scale
-                     + sd[f'{p}.conv.norm.bias'].double())
-        b.w_pw2, b.b_pw2 = ptr(sd[f'{p}.conv.pointwise_conv2.weight'][:, :, 0]), ptr(sd[f'{p}.conv.pointwise_conv2.bias'])
-    n_glu = max(2 * lay, 1)
-    glu_w, glu_b = (C.c_void_p * n_glu)(), (C.c_void_p * n_glu)()
-    for i in range(lay):
-        for s in range(2):
-            glu_w[2 * i + s] = ptr(sd[f'model.cf_lay.{i}.glu{s + 1}.0.weight'])
-            glu_b[2 * i + s] = ptr(sd[f'model.cf_lay.{i}.glu{s + 1}.0.bias'])
-    m = _lib.ModelF32C()
-    m.lay, m.outdim = lay, outdim
-    m.w_in[0], m.w_in[1] = ptr(sd['model.inln.weight']), ptr(sd['model.inln1.weight'])
-    m.b_in[0], m.b_in[1] = ptr(sd['model.inln.bias']), ptr(sd['model.inln1.bias'])
-    m.blocks = C.cast(blocks, C.POINTER(_lib.BlockWeightsF32C))
-    m.glu_w, m.glu_b = C.cast(glu_w, C.POINTER(C.c_void_p)), C.cast(glu_b, C.POINTER(C.c_void_p))
-    m.w_head, m.b_head = ptr(sd['model.outln.weight']), ptr(sd['model.outln.bias'])
-    m.w_cut, m.b_cut = ptr(sd['model.cutheard.weight'][0]), float(sd['model.cutheard.bias'][0])
-    return m, (keep, blocks, glu_w, glu_b)
+    ck = checkpoint_model(sd, config)
+    ck.blocks = [[checkpoint_block(sd, p) for p in ps] for ps in ck.prefixes]
+    m, arrays = _c_model(_lib.ModelF32C, _lib.BlockWeightsF32C, ck, False, upload)
+    return m, (keep, *arrays)
