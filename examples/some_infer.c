@@ -1,4 +1,4 @@
-/* some_infer: infer.py in C.  Transcribes a WAV or FLAC file with a model file written by `python -m some_b200.export` and
+/* some_infer: infer.py in C.  Transcribes a WAV, FLAC or AIFF file with a model file written by `python -m some_b200.export` and
  * saves the notes as a MIDI file, without Python.
  *
  *   some_infer MODEL AUDIO [--midi PATH] [--tempo BPM] [--device N]

@@ -2,11 +2,11 @@
  * Python.
  *
  *   some_stream MODEL RATE [DEVICE] < pcm
- *   some_stream MODEL - [DEVICE] < file.wav or file.flac
+ *   some_stream MODEL - [DEVICE] < file.wav, file.flac or file.aif
  *
  * With RATE, reads raw mono little-endian float32 samples at RATE Hz from stdin in blocks of 100 ms and pushes each block to a
- * some_stream.  With `-`, reads a WAV or FLAC byte stream from stdin in 64 KB reads and pushes each read to an encoded stream
- * (some_stream_open_encoded: the rate comes from the header; decoded and down-mixed on the GPU as
+ * some_stream.  With `-`, reads a WAV, FLAC or AIFF byte stream from stdin in 64 KB reads and pushes each read to an encoded
+ * stream (some_stream_open_encoded: the rate comes from the header; decoded and down-mixed on the GPU as
  * some_session_transcribe_encoded does).  Prints the notes of every chunk as soon as it is delivered, one line per note:
  *
  *   <chunk offset in seconds> <note_midi> <duration in seconds> <rest 0/1>
@@ -38,7 +38,7 @@ static void print_chunks(const some_notes* notes, const some_session_info* info)
   fflush(stdout);
 }
 
-/* `-`: the bytes of a WAV or FLAC file from stdin, 64 KB per push. */
+/* `-`: the bytes of a WAV, FLAC or AIFF file from stdin, 64 KB per push. */
 static int run_encoded(some_session* s, const some_session_info* info) {
   static unsigned char buf[1 << 16];
   some_stream* st = NULL;
@@ -71,7 +71,7 @@ int main(int argc, char** argv) {
   const int encoded = argc >= 3 && strcmp(argv[2], "-") == 0;
   if (argc < 3 || (!encoded && atoi(argv[2]) <= 0)) {
     fprintf(stderr, "usage: %s MODEL RATE [DEVICE] < mono float32 little-endian PCM\n"
-                    "       %s MODEL - [DEVICE] < WAV or FLAC bytes\n", argv[0], argv[0]);
+                    "       %s MODEL - [DEVICE] < WAV, FLAC or AIFF bytes\n", argv[0], argv[0]);
     return 2;
   }
   if (encoded) {

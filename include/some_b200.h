@@ -423,31 +423,43 @@ int some_flac_chain_resume(const some_flac_frame* frames, int n_frames, int64_t 
  *                  or float64; tag 0xFFFE with a PCM or float subformat; any number of channels; other chunks skipped with
  *                  their pad byte; a data chunk cut short by the end of the file yields the whole frames present), or fLaC,
  *                  optionally behind an ID3v2 tag, with the metadata-block rules of audio.parse_flac (up to 24 bits per
- *                  sample).  Refused with audio.decode_wav's / audio.parse_flac's reason (scipy's text for the WAV walk)
- *                  and the byte offset: other containers (Ogg, MP3, AIFF, RIFX, RF64, CAF, AU) by name, truncated or
- *                  missing chunks, unsupported tags or sample sizes, a bad STREAMINFO. */
-enum { SOME_AUDIO_WAV = 1, SOME_AUDIO_FLAC = 2 };
-enum { SOME_PCM_U8 = 1, SOME_PCM_S16 = 2, SOME_PCM_S24 = 3, SOME_PCM_S32 = 4, SOME_PCM_F32 = 5, SOME_PCM_F64 = 6 };
+ *                  sample), or FORM/AIFF and FORM/AIFC as libsndfile reads them (COMM before SSND, other chunks skipped
+ *                  with their pad byte, the walk bounded by the FORM size and ending with the SSND chunk; the rate is the
+ *                  integer part of COMM's 80-bit extended value; the frames are the whole frames of the SSND bytes within
+ *                  its stated size and the file; integer PCM of 1-32 bits big-endian or `sowt`, `raw ` 8-bit unsigned,
+ *                  `fl32` / `fl64` big-endian float, `ulaw` / `alaw` G.711).  Refused with audio.decode_wav's /
+ *                  audio.parse_flac's reason (scipy's text for the WAV walk; "AIFF/IFF: ..." for AIFF) and the byte offset:
+ *                  other containers (Ogg, MP3, RIFX, RF64, CAF, AU) by name, truncated or missing chunks, unsupported tags,
+ *                  compression types or sample sizes, a bad STREAMINFO, an AIFF rate outside [1, 2^31). */
+enum { SOME_AUDIO_WAV = 1, SOME_AUDIO_FLAC = 2, SOME_AUDIO_AIFF = 3 };
+/* Sample containers: little-endian U8 .. F64 (WAV, AIFF-C `sowt` and `raw `), and for AIFF: S8 (1-8 bit signed), the
+ * big-endian S16BE .. F64BE and G.711 ULAW / ALAW (one byte per sample). */
+enum { SOME_PCM_U8 = 1, SOME_PCM_S16 = 2, SOME_PCM_S24 = 3, SOME_PCM_S32 = 4, SOME_PCM_F32 = 5, SOME_PCM_F64 = 6,
+       SOME_PCM_S8 = 7, SOME_PCM_S16BE = 8, SOME_PCM_S24BE = 9, SOME_PCM_S32BE = 10, SOME_PCM_F32BE = 11, SOME_PCM_F64BE = 12,
+       SOME_PCM_ULAW = 13, SOME_PCM_ALAW = 14 };
 typedef struct {
   int container;                 /* SOME_AUDIO_* */
-  int rate, channels, bits;      /* bits: the fmt chunk's bits per sample / STREAMINFO's */
-  int kind;                      /* WAV: SOME_PCM_* (the sample container); FLAC: 0 */
-  int min_blocksize, max_blocksize;   /* FLAC STREAMINFO; WAV: 0 */
+  int rate, channels, bits;      /* bits: the fmt chunk's bits per sample / STREAMINFO's / COMM's sampleSize */
+  int kind;                      /* WAV, AIFF: SOME_PCM_* (the sample container); FLAC: 0 */
+  int min_blocksize, max_blocksize;   /* FLAC STREAMINFO; WAV, AIFF: 0 */
   int reserved;
   long long frames;              /* samples per channel (FLAC: STREAMINFO's, 0 = not stated) */
-  long long data_offset;         /* WAV: first sample byte; FLAC: first frame byte (after the metadata blocks) */
-  long long data_bytes;          /* WAV: frames * channels * sample bytes; FLAC: to the end of the data */
+  long long data_offset;         /* WAV, AIFF: first sample byte; FLAC: first frame byte (after the metadata blocks) */
+  long long data_bytes;          /* WAV, AIFF: frames * channels * sample bytes; FLAC: to the end of the data */
 } some_audio_meta;
 int some_audio_info(const void* data, long long n_bytes, some_audio_meta* out);
 /* some_audio_walk: the walk of some_audio_info fed in pieces; some_audio_info is the case where all bytes come in one feed with
  * end != 0.  A feed costs time in proportion to its own bytes, and the walker holds no skipped bytes (ID3 tags, metadata
- * blocks other than STREAMINFO, WAV chunks other than fmt and data) and no audio: *held (may be NULL) stays within 48 bytes.
+ * blocks other than STREAMINFO, WAV and AIFF chunks other than fmt, data, COMM and SSND, the AIFF-C compression name) and no
+ * audio: *held (may be NULL) stays within 48 bytes.
  * After each feed: -1 with some_audio_info's message and offset for the same bytes (or for the whole file) once the refusal
- * is certain; else 0 and *known = 1 once the metadata is in *meta (WAV: from the data chunk's header, with its stated size;
- * FLAC: after the last metadata block; final after the end), and the audio bytes of this feed are the file offsets
- * [*audio_begin, *audio_end): WAV sample bytes within the data chunk's stated size, FLAC everything after the metadata.  The
- * rules that depend on where the file ends (a data chunk cut short keeps its whole frames, a partial 24-bit sample or
- * multi-channel frame is refused, "Unexpected end of file", chunks after the data chunk) apply at the feed with end != 0.
+ * is certain; else 0 and *known = 1 once the metadata is in *meta (WAV, AIFF: from the data / SSND chunk's header, with its
+ * stated size; FLAC: after the last metadata block; final after the end), and the audio bytes of this feed are the file
+ * offsets [*audio_begin, *audio_end): WAV / AIFF sample bytes of the whole frames within the data / SSND chunk's stated size,
+ * FLAC everything after the metadata.  The rules that depend on where the file ends (a data or SSND chunk cut short keeps its
+ * whole frames, a partial 24-bit sample or multi-channel WAV frame is refused, "Unexpected end of file", chunks after the
+ * data chunk) apply at the feed with end != 0.  AIFF reads the same in both modes: its COMM chunk must come before SSND (an
+ * SSND chunk before COMM is refused when its header is reached) and nothing after the SSND chunk is read.
  *   stream != 0: a second WAV data chunk, or a fmt chunk after the data chunk, is refused when its header is reached; without
  * it (and in some_audio_info) the last data chunk is read with the last fmt chunk, as scipy reads them. */
 typedef struct some_audio_walk some_audio_walk;
@@ -456,9 +468,11 @@ int some_audio_walk_feed(some_audio_walk* w, const void* data, long long n_bytes
                          long long* audio_begin, long long* audio_end, long long* held);
 int some_audio_walk_destroy(some_audio_walk* w);
 
-/* ---- K-pcm: the samples of RIFF/WAVE data chunks as audio.decode_wav hands them to librosa.load, many recordings in one
- * launch.  u8 -> (x - 128) / 128, s16 / s24 / s32 -> x / 2^(bits - 1) (s32 rounded to float32 first, as numpy's astype),
- * f32 as is, f64 rounded to nearest float32.  Samples may start at any byte.  mono != 0: out[i] = np.mean's float32 order over
+/* ---- K-pcm: the samples of RIFF/WAVE data chunks and AIFF / AIFF-C SSND chunks as libsndfile hands them to librosa.load,
+ * many recordings in one launch.  u8 -> (x - 128) / 128, s8 / s16 / s24 / s32 (either byte order) -> x / 2^(bits - 1) of
+ * the container (s32 rounded to float32 first, as numpy's astype), f32 as is, f64 rounded to nearest float32 (either byte
+ * order), G.711 u-law / A-law -> the 16-bit value of the standard expansion / 32768.  Samples may start at any byte.  Each
+ * kind's container is 1 (u8, s8, u-law, A-law), 2, 3, 4 (s32, f32) or 8 bytes.  mono != 0: out[i] = np.mean's float32 order over
  * librosa's (channels, n) view (channels added one after another below 8, numpy's 8-way pairwise sum from 8 to 128 channels,
  * then / channels; the FLAC emitter uses the same function); mono == 0: interleaved out[i * channels + c].
  * Packed and launched in two steps like some_slicer_rms_windows: some_pcm_decode_pack checks every item (the message names
@@ -716,8 +730,8 @@ int some_notes_get(const some_notes* n, int clip, int* count, const float** note
 int some_notes_midi(const some_notes* n, int sample_rate, double timestep, double tempo, uint8_t* buf, size_t capacity,
                     size_t* size);
 
-/* ---- Encoded files in, notes out: librosa.load(file, sr=None, mono=True) of WAV and FLAC files on the GPU, then the slicer
- * and the model.  For item i, out[i] receives what some_session_transcribe_sliced(s, y, n, rate, params, out[i]) gives for
+/* ---- Encoded files in, notes out: librosa.load(file, sr=None, mono=True) of WAV, FLAC and AIFF files on the GPU, then the
+ * slicer and the model.  For item i, out[i] receives what some_session_transcribe_sliced(s, y, n, rate, params, out[i]) gives for
  * y, rate = audio.load(file, sr=None, mono=True): the same chunk ranges (at the model's rate) and bit-identical notes.
  * Results do not depend on the other items of the call.
  *   One GPU step for all items: every item's audio bytes go up in one pinned copy; one some_flac_scan over the FLAC items,
@@ -823,13 +837,14 @@ int some_stream_close(some_stream* st);
  * single pushes on other streams; one stream is used by one thread at a time. */
 int some_stream_push_many(some_stream* const* streams, const float* const* samples, const long long* n, const int* finish,
                           int count, some_notes* const* out);
-/* Encoded streams: a WAV or FLAC file pushed as its bytes arrive (a recorder or encoder writing to a pipe, an upload), decoded
- * and down-mixed on the GPU exactly as some_session_transcribe_encoded decodes the whole file.  The rate comes from the header.
+/* Encoded streams: a WAV, FLAC or AIFF file pushed as its bytes arrive (a recorder or encoder writing to a pipe, an upload),
+ * decoded and down-mixed on the GPU exactly as some_session_transcribe_encoded decodes the whole file.  The rate comes from the
+ * header.
  *   For a file that some_session_transcribe_encoded accepts, pushed in order and split in any way (single bytes, any sizes, all
  * at once), the chunks of all pushes and the finish, concatenated, equal some_session_transcribe_encoded on the whole file:
  * the same ranges and bit-identical notes.  Each chunk comes in the push where some_stream_push would deliver it if that push
  * carried the samples decoded in it: a FLAC sample is decoded once its whole frame has arrived and its CRC-16 is checked, a
- * WAV sample once its whole sample frame has arrived.  A header whose sizes are placeholders (as recorders writing to a pipe
+ * WAV or AIFF sample once its whole sample frame has arrived.  A header whose sizes are placeholders (as recorders writing to a pipe
  * leave them) reads to the end of the bytes, as some_session_transcribe_encoded reads such a file.  One difference: a WAV file
  * with a second data chunk, or with a fmt chunk after its data chunk, is refused when that chunk's header arrives (a stream
  * cannot take back the samples of the first data chunk nor change the format they were decoded in; the whole-file call reads

@@ -171,8 +171,11 @@ class Encoded(C.Structure):
     _fields_ = [('data', _vp), ('n_bytes', C.c_longlong)]
 
 
-AUDIO_WAV, AUDIO_FLAC = 1, 2
+AUDIO_WAV, AUDIO_FLAC, AUDIO_AIFF = 1, 2, 3
 PCM_U8, PCM_S16, PCM_S24, PCM_S32, PCM_F32, PCM_F64 = range(1, 7)
+PCM_S8, PCM_S16BE, PCM_S24BE, PCM_S32BE, PCM_F32BE, PCM_F64BE, PCM_ULAW, PCM_ALAW = range(7, 15)
+PCM_BYTES = {PCM_U8: 1, PCM_S16: 2, PCM_S24: 3, PCM_S32: 4, PCM_F32: 4, PCM_F64: 8, PCM_S8: 1, PCM_S16BE: 2, PCM_S24BE: 3,
+             PCM_S32BE: 4, PCM_F32BE: 4, PCM_F64BE: 8, PCM_ULAW: 1, PCM_ALAW: 1}     # the bytes of one sample
 
 EXPORTS = {
     # name: (restype, argtypes)

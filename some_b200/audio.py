@@ -8,13 +8,17 @@
 - ``read_encoded`` / ``EncodedAudio`` / ``FlacBatch`` / ``decode_flac``: FLAC files (libsndfile reads them through libFLAC)
   decoded on the GPU (csrc/flac.cu): the file's bytes and its STREAMINFO are read on the host, the frames are found,
   checked and decoded on the device, many recordings in one set of launches, straight to mono if wanted.
-- ``load``: librosa.load for RIFF/WAVE files (PCM 8/16/24/32-bit, float32/64, WAVE_FORMAT_EXTENSIBLE) and for FLAC files
-  (``fLaC``, optionally behind an ID3v2 tag; up to 24 bits per sample), chosen by the file's content.  Other containers
-  (Ogg, MP3, AIFF, ...) raise: librosa decodes those through libsndfile / audioread, which this module does not restate.
+- ``decode_aiff``: AIFF and AIFF-C files as libsndfile reads them, decoded on the GPU: the container is walked on the host
+  (some_audio_info, csrc/audio_host.cu), the SSND bytes go up and one some_pcm_decode (csrc/pcm.cu) scales them (integer
+  PCM of 1-32 bits in either byte order, 8-bit unsigned, big-endian float32 / float64, G.711 u-law and A-law).
+- ``load``: librosa.load for RIFF/WAVE files (PCM 8/16/24/32-bit, float32/64, WAVE_FORMAT_EXTENSIBLE), for FLAC files
+  (``fLaC``, optionally behind an ID3v2 tag; up to 24 bits per sample) and for AIFF / AIFF-C files (``FORM``), chosen by
+  the file's content.  Other containers (Ogg, MP3, ...) raise: librosa decodes those through libsndfile / audioread,
+  which this module does not restate.
 - ``load_native``: the decoded recording at its own rate, for batch.batch_infer_dataset's device-resident resampling.
 
-The arithmetic is restated in oracle/resample.py and oracle/flac.py (test infrastructure), which document what was
-restated and what could not be compared with the libraries themselves.
+The arithmetic is restated in oracle/resample.py, oracle/flac.py and oracle/aiff.py (test infrastructure), which document
+what was restated and what could not be compared with the libraries themselves.
 """
 from __future__ import annotations
 
@@ -228,9 +232,11 @@ def parse_flac(data: bytes, name: str = '<bytes>') -> EncodedAudio:
 
 
 def _sniff(path) -> str:
-    """'flac' for 'fLaC' (optionally behind an ID3v2 tag), else 'other'."""
+    """'aiff' for 'FORM', 'flac' for 'fLaC' (optionally behind an ID3v2 tag), else 'other'."""
     with open(path, 'rb') as f:
         head = f.read(10)
+        if head[:4] == b'FORM':
+            return 'aiff'
         off = _id3_size(head)
         if off:
             f.seek(off)
@@ -382,17 +388,75 @@ def decode_flac(path) -> Tuple[np.ndarray, int]:
     return (y.cpu().numpy() if y.ndim == 1 else y.t().contiguous().cpu().numpy()), rec.rate
 
 
+# ---------------------------------------------------------------------------------------------- AIFF (device)
+def audio_info(data: bytes, name: str = '<bytes>'):
+    """some_audio_info on a file's bytes (host): its _lib.AudioMeta, or ValueError naming the file, the container and the
+    byte offset."""
+    from . import _lib
+    lib = _lib.load()
+    m = _lib.AudioMeta()
+    if lib.some_audio_info(data, len(data), C.byref(m)):
+        raise ValueError(f'{name}: {lib.some_last_error().decode("utf8", "replace")}')
+    return m
+
+
+def _pcm_device(data: bytes, m, mono: bool):
+    """The samples some_audio_info found in ``data`` (a WAV data or AIFF SSND chunk), decoded by one some_pcm_decode on the
+    current stream: a CUDA float32 tensor, [n] (mono or one channel) or [channels, n]."""
+    import torch
+    from . import _lib
+    lib = _lib.load()
+    dev = torch.device('cuda', torch.cuda.current_device())
+    n, ch = int(m.frames), (1 if mono else int(m.channels))
+    raw = np.frombuffer(data, np.uint8, count=int(m.data_bytes), offset=int(m.data_offset))
+    src = torch.from_numpy(raw.copy()).to(dev)
+    y = torch.empty(max(n * ch, 1), dtype=torch.float32, device=dev)
+    item = _lib.PcmItem(src.data_ptr(), n, int(m.channels), int(m.kind), int(mono), 0, y.data_ptr())
+    desc = np.zeros(int(lib.some_pcm_decode_bytes(1)), np.uint8)
+    _lib.check(lib.some_pcm_decode_pack(C.byref(item), 1, desc.ctypes.data), 'some_pcm_decode_pack')
+    desc_d = torch.from_numpy(desc).to(dev)
+    _lib.check(lib.some_pcm_decode(desc.ctypes.data, desc_d.data_ptr(),
+                                   C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), 'some_pcm_decode')
+    y = y[:n * ch]
+    return y if ch == 1 else y.view(n, ch).t().contiguous()
+
+
+def _read_aiff(path):
+    """(file bytes, meta) of an AIFF / AIFF-C file; ValueError for anything else."""
+    from . import _lib
+    with open(path, 'rb') as f:
+        data = f.read()
+    m = audio_info(data, str(path))
+    if m.container != _lib.AUDIO_AIFF:
+        raise ValueError(f'{path}: not an AIFF or AIFF-C file')
+    return data, m
+
+
+def decode_aiff(path) -> Tuple[np.ndarray, int]:
+    """(samples, native rate) of an AIFF / AIFF-C file as libsndfile hands them to librosa.load, decoded on the GPU: float32
+    [n] (one channel) or [n, channels]."""
+    data, m = _read_aiff(path)
+    y = _pcm_device(data, m, mono=False)
+    return (y.cpu().numpy() if y.ndim == 1 else y.t().contiguous().cpu().numpy()), int(m.rate)
+
+
 # ---------------------------------------------------------------------------------------------- librosa.load
 def load(path, sr=22050, mono: bool = True):
-    """librosa.load(path, sr=sr, mono=mono) (librosa 0.9, res_type='kaiser_best') for RIFF/WAVE and FLAC files: (y, rate).
-    ``sr=None`` keeps the native rate; otherwise the decoded (and down-mixed) samples are resampled on the GPU.  FLAC files
-    are decoded and down-mixed on the GPU too."""
-    if _sniff(path) == 'flac':
-        rec = read_encoded(path)
-        y, _ = _flac_device(rec, mono)
-        if sr is not None and as_rate(sr) != rec.rate:
-            return resample(y, rec.rate, as_rate(sr)).cpu().numpy(), as_rate(sr)
-        return y.cpu().numpy(), rec.rate
+    """librosa.load(path, sr=sr, mono=mono) (librosa 0.9, res_type='kaiser_best') for RIFF/WAVE, FLAC and AIFF files:
+    (y, rate).  ``sr=None`` keeps the native rate; otherwise the decoded (and down-mixed) samples are resampled on the GPU.
+    FLAC and AIFF files are decoded and down-mixed on the GPU too."""
+    kind = _sniff(path)
+    if kind in ('flac', 'aiff'):
+        if kind == 'flac':
+            rec = read_encoded(path)
+            y, _ = _flac_device(rec, mono)
+            native = rec.rate
+        else:
+            data, m = _read_aiff(path)
+            y, native = _pcm_device(data, m, mono), int(m.rate)
+        if sr is not None and as_rate(sr) != native:
+            return resample(y, native, as_rate(sr)).cpu().numpy(), as_rate(sr)
+        return y.cpu().numpy(), native
     x, native = decode_wav(path)
     y = x.T                                                  # librosa's (channels, n)
     if mono:

@@ -3,8 +3,9 @@
 //
 // some_audio_info restates what some_b200.audio.load accepts, except integer PCM in 5-8 byte containers (scipy: int64,
 // x / 2^63) and 1-8 bit PCM in wider containers, which it refuses: RIFF/WAVE exactly as scipy.io.wavfile.read walks it (the
-// chunk loop bounded by the RIFF size, the pad byte of odd chunks, a data chunk cut short by the end of the file), and FLAC
-// with audio.parse_flac's metadata-block rules.  Its refusals carry the Python reason and a byte offset.
+// chunk loop bounded by the RIFF size, the pad byte of odd chunks, a data chunk cut short by the end of the file), FLAC
+// with audio.parse_flac's metadata-block rules, and AIFF / AIFF-C as libsndfile reads them (oracle/aiff.py restates the
+// walk in numpy).  Its refusals carry the Python reason and a byte offset.
 // some_flac_chain is the one copy of the walk FlacBatch used to do in Python; both the Python and the session's paths call it.
 // some_midi_write is some_b200.midi.build_midi_file(...).to_bytes(), tick for tick.
 #include <limits.h>
@@ -26,6 +27,43 @@ namespace {
 
 uint32_t le32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | (static_cast<uint32_t>(p[3]) << 24); }
 uint16_t le16(const uint8_t* p) { return static_cast<uint16_t>(p[0] | (p[1] << 8)); }
+uint32_t be32(const uint8_t* p) { return (static_cast<uint32_t>(p[0]) << 24) | (p[1] << 16) | (p[2] << 8) | p[3]; }
+int16_t be16(const uint8_t* p) { return static_cast<int16_t>((p[0] << 8) | p[1]); }
+
+// A chunk id or compression type for a message: printable ASCII as is, other bytes as \xNN.
+std::string fourcc(const uint8_t* p) {
+  std::string s;
+  char hex[8];
+  for (int i = 0; i < 4; ++i) {
+    if (p[i] >= 0x20 && p[i] < 0x7F && p[i] != '\\') s += static_cast<char>(p[i]);
+    else snprintf(hex, sizeof(hex), "\\x%02x", p[i]), s += hex;
+  }
+  return s;
+}
+
+// The integer part of an 80-bit IEEE extended value (sign, 15-bit exponent, 64-bit mantissa with its explicit integer bit),
+// which is how libsndfile's aiff.c turns COMM's sampleRate into an int; -1 when it is not finite, below 1 or at least 2^31.
+// *value: the value as a double, for the message.
+long long extended_int(const uint8_t* b, double* value) {
+  const int sign = b[0] >> 7, e = ((b[0] & 0x7F) << 8 | b[1]) - 16383;
+  uint64_t mant = 0;
+  for (int i = 2; i < 10; ++i) mant = mant << 8 | b[i];
+  if (e == 0x7FFF - 16383) {
+    *value = mant << 1 ? NAN : (sign ? -INFINITY : INFINITY);
+    return -1;
+  }
+  *value = (sign ? -1.0 : 1.0) * ldexp(static_cast<double>(mant), e - 63);
+  if (sign || e < 0) return -1;                            // negative, or below 1
+  uint64_t ip;
+  if (e <= 63) {
+    ip = mant >> (63 - e);
+  } else {                                                 // an unnormalised mantissa may still give a small value
+    const int sh = e - 63;
+    if (sh >= 31 || mant >= (uint64_t(1) << (31 - sh))) return -1;
+    ip = mant << sh;
+  }
+  return ip >= 1 && ip < (uint64_t(1) << 31) ? static_cast<long long>(ip) : -1;
+}
 
 // audio._id3_size: 10 + the syncsafe size (+ 10 with a footer), 0 without a tag.
 long long id3_size(const uint8_t* d, long long n) {
@@ -104,8 +142,8 @@ int AudioWalk::feed(const uint8_t* data, long long n, bool end, int* known, long
       r = e;
       break;
     }
-    if (phase_ == kWavData || phase_ == kFlacAudio) {
-      const long long stop = phase_ == kWavData ? d_end_ : LLONG_MAX, hi = std::min(stop, e);
+    if (phase_ == kPcmData || phase_ == kFlacAudio) {
+      const long long stop = phase_ == kPcmData ? d_end_ : LLONG_MAX, hi = std::min(stop, e);
       if (hi > pos_) {
         if (r > pos_)                    // audio bytes a step had looked ahead at
           held_audio_.insert(held_audio_.end(), buf_.begin(), buf_.begin() + (std::min(r, hi) - pos_));
@@ -172,6 +210,16 @@ int AudioWalk::step(bool at_end, long long n) {
         flac_off_ = p;
         pos_ = p + 4;
         phase_ = kFlacBlock;
+        return kAdvanced;
+      }
+      if (head_len_ >= 4 && memcmp(head_, "FORM", 4) == 0) {
+        SOME_REQUIRE(head_len_ >= 12, "AIFF/IFF: FORM header truncated at byte offset 0");
+        aifc_ = memcmp(head_ + 8, "AIFC", 4) == 0;
+        SOME_REQUIRE(aifc_ || memcmp(head_ + 8, "AIFF", 4) == 0, "AIFF/IFF: form type '%s' is neither AIFF nor AIFC (at byte "
+                     "offset 8); AIFF and AIFF-C files are read", fourcc(head_ + 8).c_str());
+        form_end_ = static_cast<long long>(be32(head_ + 4)) + 8;
+        pos_ = 12;
+        phase_ = kAiffChunk;
         return kAdvanced;
       }
       SOME_REQUIRE(head_len_ >= 12 && memcmp(head_, "RIFF", 4) == 0 && memcmp(head_ + 8, "WAVE", 4) == 0,
@@ -328,17 +376,111 @@ int AudioWalk::step(bool at_end, long long n) {
       m_.frames = (d_end_ - d_begin_) / isz / channels_, m_.data_offset = d_begin_, m_.data_bytes = d_end_ - d_begin_;
       known_ = true;
       pos_ = d_begin_;
-      phase_ = kWavData;
+      phase_ = kPcmData;
       return kAdvanced;
     }
+    case kAiffChunk:
+      return aiff_chunk(at_end, p, avail, q);
     default:
       return kAdvanced;
   }
-#undef SOME_WAIT
 }
 
-// The data chunk ends: all its stated bytes arrived, or the file ended `avail` bytes into it.
+// libsndfile's walk over a FORM/AIFF or FORM/AIFC file (aiff.c), as oracle/aiff.py restates it: big-endian chunks padded to
+// an even length, within the FORM size; COMM gives the format, SSND the samples, and every other chunk is skipped unread.
+// The walk ends at the SSND chunk, so both modes read the same: COMM must come before it, and a later COMM or SSND is never
+// seen.  The frames are the whole frames of the SSND bytes within its stated size and the file (COMM's numSampleFrames is
+// not used), libsndfile's count for a file cut short or written with placeholder sizes.
+int AudioWalk::aiff_chunk(bool at_end, long long p, long long avail, const uint8_t* q) {
+  auto walk_end = [&] {
+    set_error("AIFF/IFF: no %s chunk before byte offset %lld", have_comm_ ? "SSND" : "COMM", p);
+    return kFailed;
+  };
+  if (p + 8 > form_end_) return walk_end();     // no chunk header left within the FORM size
+  SOME_WAIT(8);
+  if (avail < 8) return walk_end();              // the file ends
+  const long long size = be32(q + 4);
+  if (memcmp(q, "COMM", 4) == 0) {
+    const int need = aifc_ ? 22 : 18;            // AIFF-C: the compression type; its pascal-string name is not read
+    SOME_REQUIRE(size >= need, "AIFF/IFF: COMM chunk of %lld bytes at byte offset %lld (%s needs %d)", size, p,
+                 aifc_ ? "AIFF-C" : "AIFF", need);
+    SOME_WAIT(8 + need);
+    SOME_REQUIRE(avail >= 8 + need, "AIFF/IFF: COMM chunk truncated at byte offset %lld", p);
+    const uint8_t* b = q + 8;
+    const int channels = be16(b), bits = be16(b + 6);
+    SOME_REQUIRE(channels >= 1, "AIFF/IFF: %d channels (COMM chunk at byte offset %lld)", channels, p);
+    static const uint8_t none[4] = {'N', 'O', 'N', 'E'};
+    const uint8_t* ct = aifc_ ? b + 18 : none;
+    auto is = [&](const char* a, const char* b2) { return memcmp(ct, a, 4) == 0 || (b2 && memcmp(ct, b2, 4) == 0); };
+    const std::string name = fourcc(ct);
+    int kind = 0;
+    bool known_type = true;
+    if (is("NONE", "twos") || is("sowt", nullptr)) {
+      const bool le = is("sowt", nullptr);
+      if (bits >= 1 && bits <= 8) kind = SOME_PCM_S8;
+      else if (bits >= 9 && bits <= 16) kind = le ? SOME_PCM_S16 : SOME_PCM_S16BE;
+      else if (bits >= 17 && bits <= 24) kind = le ? SOME_PCM_S24 : SOME_PCM_S24BE;
+      else if (bits >= 25 && bits <= 32) kind = le ? SOME_PCM_S32 : SOME_PCM_S32BE;
+    } else if (is("raw ", nullptr)) {
+      kind = bits == 8 ? SOME_PCM_U8 : 0;
+    } else if (is("fl32", "FL32")) {
+      kind = bits == 32 ? SOME_PCM_F32BE : 0;
+    } else if (is("fl64", "FL64")) {
+      kind = bits == 64 ? SOME_PCM_F64BE : 0;
+    } else if (is("ulaw", "ULAW")) {
+      kind = SOME_PCM_ULAW;
+    } else if (is("alaw", "ALAW")) {
+      kind = SOME_PCM_ALAW;
+    } else {
+      known_type = false;
+    }
+    SOME_REQUIRE(known_type, "AIFF/IFF: AIFF-C compression type '%s' is not read (COMM chunk at byte offset %lld); NONE, "
+                 "twos, sowt, raw , fl32, fl64, ulaw and alaw are", name.c_str(), p);
+    SOME_REQUIRE(kind, "AIFF/IFF: sampleSize %d is not read with compression type '%s' (COMM chunk at byte offset %lld)", bits,
+                 name.c_str(), p);
+    double value;
+    const long long rate = extended_int(b + 8, &value);
+    SOME_REQUIRE(rate > 0, "AIFF/IFF: sample rate %g is outside [1, 2^31) (COMM chunk at byte offset %lld)", value, p);
+    channels_ = channels, bits_ = bits, rate_ = static_cast<int>(rate);
+    d_kind_ = kind, d_isz_ = pcm_sample_bytes(kind);
+    have_comm_ = true;
+    pos_ = p + 8 + size + (size & 1);
+    return kAdvanced;
+  }
+  if (memcmp(q, "SSND", 4) != 0) {               // FVER, MARK, INST, COMT, NAME, ANNO, ID3, APPL, ...: skipped
+    pos_ = p + 8 + size + (size & 1);
+    return kAdvanced;
+  }
+  SOME_REQUIRE(have_comm_, "AIFF/IFF: SSND chunk before the COMM chunk at byte offset %lld; the COMM chunk must come first", p);
+  SOME_WAIT(16);
+  SOME_REQUIRE(avail >= 16, "AIFF/IFF: SSND chunk header truncated at byte offset %lld", p);
+  const long long offset = be32(q + 8);          // the blockSize at q + 12 is not used
+  SOME_REQUIRE(size >= 8 && offset <= size - 8, "AIFF/IFF: SSND offset %lld past its chunk of %lld bytes at byte offset %lld",
+               offset, size, p);
+  const long long frame = static_cast<long long>(channels_) * d_isz_;
+  d_begin_ = p + 16 + offset;
+  d_end_ = d_begin_ + (size - 8 - offset) / frame * frame;   // the whole frames of the stated size
+  m_.container = SOME_AUDIO_AIFF;
+  m_.rate = rate_, m_.channels = channels_, m_.bits = bits_, m_.kind = d_kind_;
+  m_.min_blocksize = 0, m_.max_blocksize = 0;
+  m_.frames = (d_end_ - d_begin_) / frame, m_.data_offset = d_begin_, m_.data_bytes = d_end_ - d_begin_;
+  known_ = true;
+  pos_ = d_begin_;
+  phase_ = kPcmData;
+  return kAdvanced;
+}
+#undef SOME_WAIT
+
+// The data (SSND) chunk ends: all its stated bytes arrived, or the file ended `avail` bytes into it (AIFF: avail < 0 when the
+// SSND offset points past the end).  AIFF keeps the whole frames and reads nothing after them.
 int AudioWalk::data_done(long long avail) {
+  if (m_.container == SOME_AUDIO_AIFF) {
+    const long long frame = static_cast<long long>(channels_) * d_isz_;
+    m_.frames = std::min(d_end_ - d_begin_, std::max(avail, 0ll)) / frame;
+    m_.data_bytes = m_.frames * frame;
+    phase_ = kDone;
+    return 0;
+  }
   const long long p = d_begin_ - 8;
   long long samples, consumed;
   if (d_kind_ == SOME_PCM_S24) {         // read as raw bytes, then regrouped by three

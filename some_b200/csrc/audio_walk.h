@@ -10,9 +10,9 @@
 
 namespace some {
 
-// RIFF/WAVE or FLAC metadata, fed in pieces.  Each feed costs time in proportion to its own bytes: the walker holds only the
+// RIFF/WAVE, AIFF / AIFF-C or FLAC metadata, fed in pieces.  Each feed costs time in proportion to its own bytes: the walker holds only the
 // bytes of the structure it is reading (at most 48), never those of skipped chunks, tags or metadata blocks, and never the
-// audio.  The rules that depend on where the file ends (a data chunk cut short, "Unexpected end of file", ...) apply when
+// audio.  AIFF is read the same way in both modes: COMM must come before SSND, and the walk ends with the SSND chunk.  The rules that depend on where the file ends (a data chunk cut short, "Unexpected end of file", ...) apply when
 // the end is signalled, so a refusal comes with some_audio_info's message and offset as soon as it is certain.
 //   stream: a second WAV data chunk, or a fmt chunk after the data chunk, is refused when its header is reached (a stream
 // cannot take back the samples of the first data chunk, nor change the format they were decoded in); otherwise the last data
@@ -21,9 +21,9 @@ class AudioWalk {
  public:
   explicit AudioWalk(bool stream) : stream_(stream) {}
   // Feeds the next n bytes (end: they are the file's last).  Returns -1 with the refusal, else 0 and *known (whether meta()
-  // holds the stream's metadata: WAV once the data chunk's header is read, FLAC after the last metadata block; final after
-  // the end).  The audio bytes of this feed are the file offsets [*audio_begin, *audio_end) (empty when equal): WAV sample
-  // bytes within the data chunk's stated size, FLAC everything after the metadata.  The first held_audio().size() of them
+  // holds the stream's metadata: WAV / AIFF once the data / SSND chunk's header is read, FLAC after the last metadata block;
+  // final after the end).  The audio bytes of this feed are the file offsets [*audio_begin, *audio_end) (empty when equal):
+  // WAV / AIFF sample bytes within the data / SSND chunk's stated size, FLAC everything after the metadata.  The first held_audio().size() of them
   // are in held_audio() (bytes a header rule had looked ahead at), until the next feed; the rest are in `data`.
   int feed(const uint8_t* data, long long n, bool end, int* known, long long* audio_begin, long long* audio_end);
   const some_audio_meta& meta() const { return m_; }
@@ -35,11 +35,12 @@ class AudioWalk {
   long long held_header() const { return static_cast<long long>(buf_.size()); }
 
  private:
-  enum Phase { kStart, kMagic, kFlacBlock, kFlacEnd, kFlacAudio, kWavChunk, kWavData, kDone };
+  enum Phase { kStart, kMagic, kFlacBlock, kFlacEnd, kFlacAudio, kWavChunk, kAiffChunk, kPcmData, kDone };   // kPcmData: a WAV data or AIFF SSND chunk
   enum { kAdvanced = 0, kMore = 1, kFailed = -1 };
   int step(bool at_end, long long n);
   int data_done(long long avail);
   int wav_done();
+  int aiff_chunk(bool at_end, long long p, long long avail, const uint8_t* q);
 
   const bool stream_;
   Phase phase_ = kStart;
@@ -61,6 +62,10 @@ class AudioWalk {
   int tag_ = 0, block_align_ = 0, bits_ = 0;
   int d_kind_ = 0, d_channels_ = 0, d_bits_ = 0, d_isz_ = 0, d_bps_ = 0;
   long long d_size_ = 0, d_begin_ = 0, d_end_ = 0, d_frames_ = 0, d_offset_ = 0, d_bytes_ = 0;
+  // AIFF: the end of the FORM chunk (it bounds the walk), whether the form type is AIFC and COMM has been read (its format
+  // is in channels_, rate_, bits_ and d_kind_ / d_isz_)
+  long long form_end_ = 0;
+  bool aifc_ = false, have_comm_ = false;
 };
 
 // One recording's frame chain, resumable: where the next frame must start (a file offset), the samples and frames chained so

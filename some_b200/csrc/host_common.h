@@ -64,6 +64,18 @@ int flac_decode_chain(const uint8_t* data, const some_flac_stream* streams, cons
                       const int64_t* scratch_off, const int64_t* out_off, int n_chain, int32_t* scratch, float* out, int mono,
                       int* status, int* failed, cudaStream_t stream);
 
+// The bytes of one sample of a SOME_PCM_* kind (0: not a kind).
+inline int pcm_sample_bytes(int kind) {
+  switch (kind) {
+    case SOME_PCM_U8: case SOME_PCM_S8: case SOME_PCM_ULAW: case SOME_PCM_ALAW: return 1;
+    case SOME_PCM_S16: case SOME_PCM_S16BE: return 2;
+    case SOME_PCM_S24: case SOME_PCM_S24BE: return 3;
+    case SOME_PCM_S32: case SOME_PCM_S32BE: case SOME_PCM_F32: case SOME_PCM_F32BE: return 4;
+    case SOME_PCM_F64: case SOME_PCM_F64BE: return 8;
+    default: return 0;
+  }
+}
+
 // The number of RMS frames whose windows end within the first `fixed` samples (the streaming slicer and the stream).
 inline int64_t frames_within(const some_slicer_frames& f, int64_t fixed) {
   const int64_t reach = f.win_size - f.win_size / 2;          // frame k reads samples up to k hop - win / 2 + win - 1

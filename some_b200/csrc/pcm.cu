@@ -1,12 +1,15 @@
-// K-pcm: the samples of RIFF/WAVE data chunks as audio.decode_wav hands them to librosa.load (libsndfile's scaling, read
-// through scipy.io.wavfile), many recordings in one launch, from their bytes on the device.
-//   u8 -> (x - 128) / 128; s16 / s24 / s32 -> x / 2^(bits - 1) (s32 is rounded to float32 first, as numpy's astype does; the
-//   division by a power of two is exact); f32 as is; f64 rounded to nearest float32.
+// K-pcm: the samples of RIFF/WAVE data chunks and AIFF / AIFF-C SSND chunks as libsndfile hands them to librosa.load (for
+// WAV read through scipy.io.wavfile, as audio.decode_wav does), many recordings in one launch, from their bytes on the device.
+//   u8 -> (x - 128) / 128; s8 / s16 / s24 / s32, little- or big-endian -> x / 2^(8 bytes - 1) (s32 is rounded to float32
+//   first, as numpy's astype does; the division by a power of two is exact); f32 as is; f64 rounded to nearest float32;
+//   G.711 u-law / A-law -> libsndfile's 16-bit expansion / 32768, computed with the standard bit arithmetic (a table in
+//   constant memory would serialise the lanes' different indices).
 // Samples may start at any byte: every sample is assembled from its bytes, so 24-bit and unaligned float samples need no
 // alignment.  Mono output is np.mean's float32 order over the channels (mono_mean, downmix.cuh, shared with the FLAC
 // emitter); otherwise the output is interleaved [n, channels].
 // Work split: each CTA writes a fixed tile of PCM_TILE output frames of one recording and finds its recording from the tiles'
-// prefix sums (window_of), as some_resample_kaiser_windows does; the descriptors travel in the caller's upload.
+// prefix sums (window_of), as some_resample_kaiser_windows does; the descriptors travel in the caller's upload.  The kind is
+// the same for every lane of a recording, so the switch in pcm_sample does not diverge.
 #include <stddef.h>
 
 #include "downmix.cuh"
@@ -24,38 +27,52 @@ struct PcmParams {
   const uint8_t* data;
   float* out;
   long long frames;
-  int channels, kind, mono, isz;
+  int channels, kind, mono, isz, be;   // be: the samples are big-endian
 };
 
-__device__ __forceinline__ float pcm_sample(const uint8_t* __restrict__ p, int kind) {
+// G.711 expansions to 16-bit values (ITU-T G.711; the bit arithmetic of Sun's g711.c, whose values libsndfile tabulates).
+__device__ __forceinline__ int ulaw_value(uint32_t code) {
+  const uint32_t u = ~code & 0xFF;
+  const int t = static_cast<int>(((u & 0x0F) << 3) + 0x84) << ((u >> 4) & 7);
+  return (u & 0x80) ? 0x84 - t : t - 0x84;
+}
+__device__ __forceinline__ int alaw_value(uint32_t code) {
+  const uint32_t a = code ^ 0x55;
+  const int seg = (a >> 4) & 7, m = static_cast<int>(a & 0x0F) << 4;
+  const int t = seg == 0 ? m + 8 : (m + 0x108) << (seg - 1);
+  return (a & 0x80) ? t : -t;
+}
+
+// One sample: its isz bytes at p as an unsigned integer in the kind's byte order (be: big-endian), then the kind's value.
+__device__ __forceinline__ float pcm_sample(const uint8_t* __restrict__ p, int kind, int isz, bool be) {
+  unsigned long long u = 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+    if (i < isz) u |= static_cast<unsigned long long>(__ldg(p + i)) << (8 * (be ? isz - 1 - i : i));
+  const uint32_t w = static_cast<uint32_t>(u);
   switch (kind) {
     case SOME_PCM_U8:
-      return __fmul_rn(__fsub_rn(static_cast<float>(__ldg(p)), 128.f), 0.0078125f);
-    case SOME_PCM_S16: {
-      const int16_t v = static_cast<int16_t>(__ldg(p) | (__ldg(p + 1) << 8));
-      return __fmul_rn(static_cast<float>(v), 3.0517578125e-05f);                     // 2^-15
-    }
-    case SOME_PCM_S24: {                                                               // left-justified in int32, as scipy
-      const int32_t v = static_cast<int32_t>((static_cast<uint32_t>(__ldg(p)) << 8) | (static_cast<uint32_t>(__ldg(p + 1)) << 16) |
-                                             (static_cast<uint32_t>(__ldg(p + 2)) << 24));
-      return __fmul_rn(__int2float_rn(v), 4.656612873077393e-10f);                    // 2^-31
-    }
-    case SOME_PCM_S32: {
-      const int32_t v = static_cast<int32_t>(static_cast<uint32_t>(__ldg(p)) | (static_cast<uint32_t>(__ldg(p + 1)) << 8) |
-                                             (static_cast<uint32_t>(__ldg(p + 2)) << 16) | (static_cast<uint32_t>(__ldg(p + 3)) << 24));
-      return __fmul_rn(__int2float_rn(v), 4.656612873077393e-10f);
-    }
-    case SOME_PCM_F32: {
-      const uint32_t u = static_cast<uint32_t>(__ldg(p)) | (static_cast<uint32_t>(__ldg(p + 1)) << 8) |
-                         (static_cast<uint32_t>(__ldg(p + 2)) << 16) | (static_cast<uint32_t>(__ldg(p + 3)) << 24);
-      return __uint_as_float(u);
-    }
-    default: {                                                                         // SOME_PCM_F64
-      unsigned long long u = 0;
-#pragma unroll
-      for (int k = 0; k < 8; ++k) u |= static_cast<unsigned long long>(__ldg(p + k)) << (8 * k);
+      return __fmul_rn(__fsub_rn(static_cast<float>(w), 128.f), 0.0078125f);
+    case SOME_PCM_S8:
+      return __fmul_rn(static_cast<float>(static_cast<int8_t>(w)), 0.0078125f);          // 2^-7
+    case SOME_PCM_S16:
+    case SOME_PCM_S16BE:
+      return __fmul_rn(static_cast<float>(static_cast<int16_t>(w)), 3.0517578125e-05f);  // 2^-15
+    case SOME_PCM_S24:                                                                 // left-justified in int32, as scipy
+    case SOME_PCM_S24BE:
+      return __fmul_rn(__int2float_rn(static_cast<int32_t>(w << 8)), 4.656612873077393e-10f);   // 2^-31
+    case SOME_PCM_S32:
+    case SOME_PCM_S32BE:
+      return __fmul_rn(__int2float_rn(static_cast<int32_t>(w)), 4.656612873077393e-10f);
+    case SOME_PCM_F32:
+    case SOME_PCM_F32BE:
+      return __uint_as_float(w);
+    case SOME_PCM_ULAW:
+      return __fmul_rn(static_cast<float>(ulaw_value(w)), 3.0517578125e-05f);
+    case SOME_PCM_ALAW:
+      return __fmul_rn(static_cast<float>(alaw_value(w)), 3.0517578125e-05f);
+    default:                                                                           // SOME_PCM_F64, SOME_PCM_F64BE
       return __double2float_rn(__longlong_as_double(static_cast<long long>(u)));
-    }
   }
 }
 
@@ -70,16 +87,11 @@ __global__ void __launch_bounds__(PCM_THREADS) pcm_decode_kernel(const PcmParams
   for (long long f = f0 + threadIdx.x; f < f1; f += PCM_THREADS) {
     const uint8_t* row = p.data + f * ch * p.isz;
     if (p.mono) {
-      p.out[f] = mono_mean(ch, [&](int c) { return pcm_sample(row + static_cast<long long>(c) * p.isz, p.kind); });
+      p.out[f] = mono_mean(ch, [&](int c) { return pcm_sample(row + static_cast<long long>(c) * p.isz, p.kind, p.isz, p.be); });
     } else {
-      for (int c = 0; c < ch; ++c) p.out[f * ch + c] = pcm_sample(row + static_cast<long long>(c) * p.isz, p.kind);
+      for (int c = 0; c < ch; ++c) p.out[f * ch + c] = pcm_sample(row + static_cast<long long>(c) * p.isz, p.kind, p.isz, p.be);
     }
   }
-}
-
-int sample_bytes(int kind) {
-  return kind == SOME_PCM_U8 ? 1 : kind == SOME_PCM_S16 ? 2 : kind == SOME_PCM_S24 ? 3 : kind == SOME_PCM_F64 ? 8
-         : (kind == SOME_PCM_S32 || kind == SOME_PCM_F32) ? 4 : 0;
 }
 
 }  // namespace
@@ -95,7 +107,7 @@ extern "C" int some_pcm_decode_pack(const some_pcm_item* items, int K, void* des
   long long* tile0 = windows_tile0(desc);
   for (int i = 0; i < K; ++i) {
     const some_pcm_item& it = items[i];
-    const int isz = sample_bytes(it.kind);
+    const int isz = pcm_sample_bytes(it.kind);
     SOME_REQUIRE(isz > 0, "some_pcm_decode_pack: item %d: unknown sample kind %d", i, it.kind);
     SOME_REQUIRE(it.frames >= 0 && it.channels >= 1, "some_pcm_decode_pack: item %d: %lld frames of %d channels", i, it.frames,
                  it.channels);
@@ -103,7 +115,9 @@ extern "C" int some_pcm_decode_pack(const some_pcm_item* items, int K, void* des
                  "some_pcm_decode_pack: item %d: a mono down-mix of %d channels (numpy's order is restated up to %d)", i,
                  it.channels, kMonoMaxChannels);
     SOME_REQUIRE(it.frames == 0 || (it.data && it.out), "some_pcm_decode_pack: item %d: null pointer", i);
-    ps[i] = PcmParams{it.data, it.out, it.frames, it.channels, it.kind, it.mono ? 1 : 0, isz};
+    const bool be = it.kind == SOME_PCM_S16BE || it.kind == SOME_PCM_S24BE || it.kind == SOME_PCM_S32BE ||
+                    it.kind == SOME_PCM_F32BE || it.kind == SOME_PCM_F64BE;
+    ps[i] = PcmParams{it.data, it.out, it.frames, it.channels, it.kind, it.mono ? 1 : 0, isz, be ? 1 : 0};
     tile0[i + 1] = (it.frames + PCM_TILE - 1) / PCM_TILE;
   }
   windows_index(desc, K, 0);

@@ -1002,7 +1002,7 @@ struct some_stream {
   int64_t received = 0, fixed = 0, frames = 0;   // frames: RMS frames computed so far
   bool finished = false;
   // an encoded stream (some_stream_open_encoded; rate 0 until its header is complete): the container walk, the audio bytes
-  // not decoded yet (file offsets [pend_pos, pend_pos + size): an incomplete FLAC frame or WAV sample frame) and the chain
+  // not decoded yet (file offsets [pend_pos, pend_pos + size): an incomplete FLAC frame or WAV or AIFF sample frame) and the chain
   std::unique_ptr<AudioWalk> walk;
   bool failed = false;                    // refused on its content
   std::vector<uint8_t> pending;
@@ -1030,10 +1030,14 @@ struct StepItem {
   bool dropped = false;         // its samples failed to decode: no slicer decisions, no chunks
 };
 
-// Accepts a container's format for a session at rate `sr`, or refuses it (the message has no prefix): a WAV file's mono
+// Whether a container's samples are PCM that some_pcm_decode reads (WAV, AIFF) rather than FLAC frames: the one place the
+// encoded calls tell the two paths apart.
+bool pcm_container(const some_audio_meta& m) { return m.container != SOME_AUDIO_FLAC; }
+
+// Accepts a container's format for a session at rate `sr`, or refuses it (the message has no prefix): a PCM file's mono
 // down-mix takes at most 128 channels, and the resampler must support the rate pair.
 int check_format(const some_audio_meta& m, int sr) {
-  SOME_REQUIRE(m.container == SOME_AUDIO_FLAC || m.channels <= 128, "a mono down-mix of %d channels (at most 128)", m.channels);
+  SOME_REQUIRE(!pcm_container(m) || m.channels <= 128, "a mono down-mix of %d channels (at most 128)", m.channels);
   long long t_end, x_first;
   if (m.rate != sr && some_resample_window_plan(0, 0, 0, m.rate, sr, kKaiserTaps, &t_end, &x_first)) return -1;
   return 0;
@@ -1078,7 +1082,7 @@ struct Decode {
     int64_t at = 0;
     auto place = [&](bool flac) {
       for (const ByteWindow& w : ws)
-        if ((w.m->container == SOME_AUDIO_FLAC) == flac) *w.at = at, at += align16(w.bytes), nf += flac;
+        if (!pcm_container(*w.m) == flac) *w.at = at, at += align16(w.bytes), nf += flac;
     };
     place(true);
     flac_bytes = at;
@@ -1090,7 +1094,7 @@ struct Decode {
     some_flac_stream* st_h = reinterpret_cast<some_flac_stream*>(up_h + at);
     for (const ByteWindow& w : ws) {
       spans.push_back({up_h + *w.at, w.src, static_cast<size_t>(w.bytes)});
-      if (w.m->container == SOME_AUDIO_FLAC)
+      if (!pcm_container(*w.m))
         *st_h++ = some_flac_stream{*w.at, *w.at + w.bytes, w.m->channels, w.m->bits, w.m->max_blocksize, 0};
     }
     copy_to_pinned(*s->pool, spans, size_t(1) << 20);
@@ -1376,7 +1380,7 @@ struct ByteItem {
 // A step of encoded streams (some_stream_push_bytes*, some_stream_finish), under the session's mutex:
 //   1. on the host, each stream's walk consumes its bytes; their audio joins the stream's pending bytes;
 //   2. the encoded-input stage (Decode) uploads the FLAC windows (the pending bytes from each stream's first unchained
-//      frame) and the whole WAV sample frames;
+//      frame) and the whole WAV or AIFF sample frames;
 //   3. with FLAC streams: its scan, with the candidates down in the same synchronise as the count, then each stream's
 //      resumable chain;
 //   4. streams_step with the stage's decodes in front: one some_pcm_decode and one FLAC decode, mono, into the region its
@@ -1428,16 +1432,15 @@ int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
       if (a1 > from) st->pending.insert(st->pending.end(), b.data + (from - r0), b.data + (a1 - r0));
     }
   }
-  // 2. the bytes upload: each stream's pending FLAC window (from its first unchained frame) or its whole WAV sample frames
-  auto flac = [](const ByteItem& b) { return b.live && b.st->rate && b.st->walk->meta().container == SOME_AUDIO_FLAC; };
+  // 2. the bytes upload: each stream's pending FLAC window (from its first unchained frame) or its whole PCM sample frames
+  auto flac = [](const ByteItem& b) { return b.live && b.st->rate && !pcm_container(b.st->walk->meta()); };
   std::vector<ByteWindow> ws;
   for (ByteItem& b : bs) {
     if (!b.live || !b.st->rate) continue;
     const some_audio_meta& m = b.st->walk->meta();
     b.win = static_cast<int64_t>(b.st->pending.size());
-    if (m.container == SOME_AUDIO_WAV) {
-      static const int kBytes[7] = {0, 1, 2, 3, 4, 4, 8};
-      const int64_t frame = static_cast<int64_t>(m.channels) * kBytes[m.kind];
+    if (pcm_container(m)) {
+      const int64_t frame = static_cast<int64_t>(m.channels) * pcm_sample_bytes(m.kind);
       b.samples = b.win / frame;
       b.win = b.samples * frame;
       if (too_short(b)) continue;
@@ -1486,8 +1489,8 @@ int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
     }
     dec.chain.resize(k);
   }
-  for (ByteItem& b : bs) {               // the WAV windows went up whole
-    if (!b.live || !b.st->rate || b.st->walk->meta().container != SOME_AUDIO_WAV) continue;
+  for (ByteItem& b : bs) {               // the PCM windows went up whole
+    if (!b.live || !b.st->rate || !pcm_container(b.st->walk->meta())) continue;
     b.st->pending.erase(b.st->pending.begin(), b.st->pending.begin() + b.win);
     b.st->pend_pos += b.win;
   }
@@ -1501,7 +1504,7 @@ int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
     const int j = static_cast<int>(items.size());
     if (b.fi >= 0) {
       dec.flac_of[b.fi] = j;
-    } else if (b.samples && st->walk->meta().container == SOME_AUDIO_WAV) {
+    } else if (b.samples && pcm_container(st->walk->meta())) {
       const some_audio_meta& m = st->walk->meta();
       dec.pcm.push_back(some_pcm_item{dec.bytes_d + b.up, b.samples, m.channels, m.kind, 1, 0, nullptr});
       dec.pcm_of.push_back(j);
@@ -1703,7 +1706,7 @@ int transcribe_encoded(some_session* s, std::vector<EncItem>& its, const some_sl
   if (dec.upload(s, ws, "the encoded files")) return -1;
   for (int i = 0; i < count; ++i) {
     const EncItem& it = its[i];
-    if (it.m.container == SOME_AUDIO_FLAC) {
+    if (!pcm_container(it.m)) {
       dec.flac_of.push_back(i);
     } else {
       dec.pcm.push_back(some_pcm_item{dec.bytes_d + it.up, it.n, it.m.channels, it.m.kind, 1, 0, nullptr});
@@ -1774,7 +1777,7 @@ extern "C" int some_session_transcribe_encoded(some_session* s, const some_encod
     it.bytes = static_cast<const uint8_t*>(items[i].data);
     if (some_audio_info(items[i].data, items[i].n_bytes, &it.m) || check_format(it.m, sr)) return item_error(i);
     it.n = it.m.frames;
-    if (it.m.container == SOME_AUDIO_WAV || it.m.frames > 0) {
+    if (pcm_container(it.m) || it.m.frames > 0) {
       char who[96];
       snprintf(who, sizeof(who), "some_session_transcribe_encoded: item %d", i);
       if (slice_shape(it.n, it.m.rate, sr, sl, who, &it.sh)) return -1;

@@ -119,7 +119,7 @@ class Session:
         return [a / self.sample_rate for a, _ in ranges], ranges, res
 
     def transcribe_encoded(self, items: Sequence, params: Optional[_lib.SlicerParams] = None):
-        """some_session_transcribe_encoded: WAV or FLAC files (bytes, or paths to read) -> one (chunk offsets in seconds, chunk
+        """some_session_transcribe_encoded: WAV, FLAC or AIFF files (bytes, or paths to read) -> one (chunk offsets in seconds, chunk
         sample ranges, per-chunk notes) per item, what transcribe_sliced returns for audio.load(file, sr=None, mono=True).
         The files are decoded, resampled, sliced and transcribed in one GPU step."""
         datas = []
@@ -152,7 +152,7 @@ class Session:
         return Stream(self, sample_rate, params)
 
     def stream_encoded(self, params: Optional[_lib.SlicerParams] = None) -> 'EncodedStream':
-        """some_stream_open_encoded: a WAV or FLAC file pushed as its bytes arrive (see EncodedStream)."""
+        """some_stream_open_encoded: a WAV, FLAC or AIFF file pushed as its bytes arrive (see EncodedStream)."""
         return EncodedStream(self, params)
 
     def push_bytes_many(self, items: Sequence[Tuple['EncodedStream', bytes]], finish: Optional[Sequence[bool]] = None):
@@ -247,7 +247,7 @@ class Stream:
 
 
 class EncodedStream(Stream):
-    """some_stream_open_encoded: push(bytes) takes the next bytes of a WAV or FLAC file; push() and finish() return the chunks
+    """some_stream_open_encoded: push(bytes) takes the next bytes of a WAV, FLAC or AIFF file; push() and finish() return the chunks
     that became final, as Stream does.  Concatenated they equal Session.transcribe_encoded on the whole file."""
 
     def __init__(self, session: Session, params: Optional[_lib.SlicerParams] = None):
