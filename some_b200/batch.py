@@ -2,9 +2,10 @@
 
 The reference transcribes a DiffSinger dataset strictly one file at a time (batch_infer.py:164-176: librosa.load -> Slicer ->
 infer on that file's chunks, a handful of 5-15 s clips per launch sequence).  Here the chunks of MANY recordings form one
-var-len batch: every recording is uploaded once into one device buffer, the slicer's RMS lists of all of them come back in one
-copy (csrc/slicer.cu), the cuts are decided on the host, and ONE mel -> trunk -> decode pass runs over all chunks where they lie
-(Engine.enqueue(resident=...)); audio files are read by a thread pool while the GPU works on the previous group.
+var-len batch: every recording is uploaded once into one device buffer (``stage_recordings``), then
+``Engine.transcribe_resident`` -- the same step ``Engine.infer_sliced`` ends in -- brings the slicer's RMS lists of all of them
+back in one copy, decides the cuts on the host and runs ONE mel -> trunk -> decode pass over all chunks where they lie; audio
+files are read by a thread pool while the GPU works on the previous group.
 
 Everything after the notes is host string / rounding work and is restated so that ``transcriptions.csv`` comes out BYTE-identical
 to batch_infer.py for the same notes (pinned by tests/golden/host_rows.npz, produced by the unmodified reference):
@@ -28,6 +29,7 @@ sharps, ``unicode=False``) and ``librosa.load(path, sr=audio_sample_rate, mono=T
 from __future__ import annotations
 
 import concurrent.futures
+import contextlib
 import pathlib
 import re
 from csv import DictReader, DictWriter
@@ -36,7 +38,7 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import audio
-from .slicer import Slicer, cut_ranges
+from .slicer import Slicer
 
 _NOTE_NAMES = ('C', 'C#', 'D', 'D#', 'E', 'F', 'F#', 'G', 'G#', 'A', 'A#', 'B')
 
@@ -196,7 +198,7 @@ def stage_recordings(eng, target_sr: int, waveforms: Sequence, rates: Optional[S
     ``target_sr``, as transcribe_recordings describes: recordings at another rate are resampled on the device, FLAC records
     decoded there.  Call on the engine's device.  Returns (wave_d, bases int64 [n + 1], lens, flac_status): recording i is
     wave_d[bases[i] : bases[i] + lens[i]]; the FLAC status words are checked with audio._check_status once the stream has
-    passed them."""
+    passed them, as ``staged`` does."""
     import torch
     enc = {i: w for i, w in enumerate(waveforms) if isinstance(w, audio.EncodedAudio)}
     waves = [None if i in enc else np.ascontiguousarray(w, dtype=np.float32) for i, w in enumerate(waveforms)]
@@ -242,13 +244,30 @@ def stage_recordings(eng, target_sr: int, waveforms: Sequence, rates: Optional[S
     return wave_d, bases, lens, flac_status
 
 
+@contextlib.contextmanager
+def staged(infer_ins, waveforms: Sequence, rates: Optional[Sequence[Optional[int]]]):
+    """``stage_recordings`` for a plugin instance at its ``audio_sample_rate``, yielding (wave_d, bases, lens).  The block
+    runs under the instance's lock (if it has one: concurrent callers share one engine and its buffers) on the engine's
+    device.  When the block ends normally, its work on the stream has passed the FLAC decode, whose status words are then
+    checked (audio._check_status)."""
+    import torch
+    eng = infer_ins.model
+    lock = getattr(infer_ins, '_lock', None)
+    with (lock if lock is not None else contextlib.nullcontext()), torch.cuda.device(eng.device):
+        wave_d, bases, lens, flac_status = stage_recordings(eng, int(infer_ins.config['audio_sample_rate']), waveforms, rates)
+        yield wave_d, bases, lens
+        for st in flac_status:
+            audio._check_status(st)
+
+
 def transcribe_recordings(infer_ins, waveforms: Sequence, slicer: Optional[Slicer] = None,
                           rates: Optional[Sequence[Optional[int]]] = None):
     """[(chunk offsets in seconds, per-chunk notes)] for several mono recordings, as ONE var-len batch.
 
     Equivalent to ``[ (offsets, infer_ins.infer(chunks)) for chunks in (Slicer.slice(w) for w in waveforms) ]``
-    (batch_infer.py:50-54) but every recording is uploaded once, all RMS lists come back in one copy, and a single
-    mel -> trunk -> decode pass covers every chunk of every recording.
+    (batch_infer.py:50-54) but every recording is uploaded once (``stage_recordings``), and ``Engine.transcribe_resident``
+    brings all RMS lists back in one copy and covers every chunk of every recording with a single mel -> trunk -> decode
+    pass.
 
     ``rates``: each recording's native sample rate (default: all at ``audio_sample_rate``).  A recording at another rate is
     uploaded as it is and resampled on the device, grouped by rate, straight into the batch's wave buffer, exactly as
@@ -259,35 +278,9 @@ def transcribe_recordings(infer_ins, waveforms: Sequence, slicer: Optional[Slice
     come from the records (a ``rates`` entry for one must be None or equal it); the bytes of all of them are uploaded into
     one buffer and decoded on the device, straight to mono at their native rate (audio.FlacBatch), into the wave buffer or
     the resampler's input."""
-    import torch
-    eng = infer_ins.model
-    target_sr = int(infer_ins.config['audio_sample_rate'])
-    slicer = slicer or Slicer(sr=target_sr, max_sil_kept=1000)                                 # batch_infer.py:52
-    quantized = bool(getattr(infer_ins, 'quantized', False))
-    lock = getattr(infer_ins, '_lock', None)
-    if lock is not None:
-        lock.acquire()
-    try:
-        with torch.cuda.device(eng.device):
-            wave_d, bases, lens, flac_status = stage_recordings(eng, target_sr, waveforms, rates)
-            per_rec = cut_ranges(slicer, lens, lambda need: eng.rms_frames_many(
-                [wave_d[bases[i]:bases[i] + lens[i]] for i in need], slicer.win_size, slicer.hop_size))
-            flat = [(int(bases[i]) + a, int(bases[i]) + b) for i, rs in enumerate(per_rec) for a, b in rs]
-            results: List[Dict[str, np.ndarray]] = []
-            if flat:
-                slab, cu, layout, _ = eng.enqueue(None, quantized, resident=(wave_d, flat))
-                host = slab.cpu().numpy()                                                    # one D2H + sync
-                results = eng.unpack_slab(host, cu, layout)
-            for st in flac_status:                                                           # already complete
-                audio._check_status(st)
-    finally:
-        if lock is not None:
-            lock.release()
-    out, k = [], 0
-    for rs in per_rec:
-        out.append(([a / slicer.sr for a, _ in rs], results[k:k + len(rs)]))
-        k += len(rs)
-    return out
+    slicer = slicer or Slicer(sr=int(infer_ins.config['audio_sample_rate']), max_sil_kept=1000)   # batch_infer.py:52
+    with staged(infer_ins, waveforms, rates) as (wave_d, bases, lens):
+        return infer_ins.model.transcribe_resident(wave_d, bases, lens, slicer, bool(getattr(infer_ins, 'quantized', False)))
 
 
 def load_wav(path, sr: int) -> np.ndarray:

@@ -23,7 +23,7 @@ import torch
 
 from . import _lib
 from .config import DIM, FFN_DIM, check_supported
-from .slicer import cut_ranges
+from .slicer import cut_ranges, one_chunk, rms_lists
 from .weights import ModelWeights, build_c_model, mel_tables
 
 HOP = 512
@@ -425,12 +425,12 @@ class Engine:
         decode kernel to the collective without a staging copy.
 
         Contract: the engine owns ONE set of staging / slab buffers.  A second enqueue() may only be issued after the consumer
-        of the previous one has synchronised (or waited on the stream): infer(), infer_sliced(), dist.infer_sharded() and the
-        dataset driver all do.  The call itself first makes the copy stream wait for everything enqueued so far.
+        of the previous one has synchronised (or waited on the stream): infer(), transcribe_resident(), dist.infer_sharded()
+        and the evaluator all do.  The call itself first makes the copy stream wait for everything enqueued so far.
 
         ``resident = (wave_d, ranges)``: the audio is already on the device (f32 tensor) and the clips are the sample ranges
-        ``[(begin, end), ...]`` inside it (``waveforms`` is ignored): no staging, no audio H2D — the slicer path
-        (infer_sliced) cuts the recording where it lies.
+        ``[(begin, end), ...]`` inside it (``waveforms`` is ignored): no staging, no audio H2D — transcribe_resident runs the
+        slicer's chunks of recordings where they lie, the evaluator whole recordings.
 
         ``logits_hook``: optional ``hook(ws, c0, c1, mc, cu_d)``, enqueued for every pipeline chunk (clips c0..c1, mc frames,
         chunk-relative cu_frames cu_d) between the trunk and the decode.  With a hook the trunk writes the raw logits
@@ -556,58 +556,48 @@ class Engine:
         self._h2d_done = ev if layout else None
         return out_d[:nbytes_total], cu, layout, extra
 
-    def rms_frames_many(self, waves_d: Sequence[torch.Tensor], frame_length: int, hop: int) -> List[np.ndarray]:
-        """Short-time RMS lists of device-resident f32 recordings (some_slicer_rms), bit-identical to the reference's get_rms
-        (utils/slicer2.py:5-38): one launch each into ONE buffer, one D2H copy and sync for all.  The slicer's decisions are
-        taken on the host from these copies."""
-        counts = [1 + (int(w.numel()) + 2 * (frame_length // 2) - frame_length) // hop for w in waves_d]
-        if not counts:
-            return []
-        cuts = np.zeros(len(counts) + 1, dtype=np.int64)
-        np.cumsum(counts, out=cuts[1:])
-        rms_d = torch.empty(int(cuts[-1]), dtype=torch.float32, device=self.device)
-        for w, a, n in zip(waves_d, cuts, counts):
-            _lib.check(self.lib.some_slicer_rms(w.data_ptr(), int(w.numel()), frame_length, hop, rms_d[a:].data_ptr(), n,
-                                                self._stream), 'some_slicer_rms')
-            self.launches += 1
-        host = rms_d.cpu().numpy()
-        return [host[a:b] for a, b in zip(cuts[:-1], cuts[1:])]
+    def transcribe_resident(self, wave_d: torch.Tensor, bases: Sequence[int], lens: Sequence[int], slicer,
+                            quantized: bool = False) -> List[tuple]:
+        """Recordings already on the device (recording i = ``wave_d[bases[i] : bases[i] + lens[i]]``) -> per recording
+        (chunk offsets in seconds, per-chunk notes), as ``Slicer.slice`` then ``infer`` on the chunks would give.  The RMS
+        lists of the recordings that may be cut come back in one copy (slicer.rms_lists), the slicer's decisions are taken on
+        the host, and the chunks of all recordings run where they lie as one var-len batch whose notes land in the pinned
+        landing buffer with one synchronise.  Call on the engine's device."""
+        per_rec = cut_ranges(slicer, lens, lambda need: rms_lists(
+            [wave_d[bases[i]:bases[i] + lens[i]] for i in need], slicer.win_size, slicer.hop_size))
+        flat = [(int(bases[i]) + a, int(bases[i]) + b) for i, rs in enumerate(per_rec) for a, b in rs]
+        results: List[Dict[str, np.ndarray]] = []
+        if flat:
+            slab, cu, layout, _ = self.enqueue(None, quantized, resident=(wave_d, flat))
+            out_h = self._stage['out_h'][:slab.numel()]
+            out_h.copy_(slab, non_blocking=True)
+            torch.cuda.current_stream(self.device).synchronize()
+            results = self.unpack_slab(out_h.numpy(), cu, layout)
+        out, k = [], 0
+        for rs in per_rec:
+            out.append(([a / slicer.sr for a, _ in rs], results[k:k + len(rs)]))
+            k += len(rs)
+        return out
 
     def infer_sliced(self, waveform: np.ndarray, slicer, quantized: bool = False):
         """One long mono recording -> (chunk offsets in seconds, per-chunk notes): the flow of infer.py:38-41 /
-        batch_infer.py:50-54 (Slicer.slice, then infer on the chunks) with the recording uploaded ONCE.  The RMS frames are
-        computed on the device, the slicer's decisions are taken on the host from the copied RMS list (15 k floats for 5 min),
-        and the chunks are then processed where they lie in device memory as one var-len batch."""
+        batch_infer.py:50-54 (Slicer.slice, then infer on the chunks) with the recording uploaded ONCE and cut and run on the
+        device by ``transcribe_resident``.  A recording the slicer leaves whole (slicer.one_chunk, also the empty one) is not
+        uploaded here but goes to ``infer``, whose small batches replay as CUDA graphs."""
         samples = np.ascontiguousarray(waveform, dtype=np.float32)
         assert samples.ndim == 1, 'infer_sliced expects a mono waveform (infer.py loads with mono=True)'
         n = int(samples.shape[0])
-        dev = self.device
-        with torch.cuda.device(dev):
-            uploaded = []
-
-            def rms_of(_):                      # only for a recording long enough to be cut
-                src = torch.from_numpy(samples)
-                if not src.is_pinned():
-                    st = self._staging(n, 1, 1 + n // HOP)
-                    st['wave_h'][:n].copy_(src)
-                    src = st['wave_h'][:n]
-                wave_d = torch.empty(n, dtype=torch.float32, device=dev)
-                wave_d.copy_(src, non_blocking=True)
-                uploaded.append(wave_d)
-                return self.rms_frames_many(uploaded, slicer.win_size, slicer.hop_size)
-
-            [ranges] = cut_ranges(slicer, [n], rms_of)
-            if not uploaded:                    # one chunk, the whole recording
-                return [0], self.infer([samples], quantized)
-            if not ranges:
-                return [], []
-            slab, cu, layout, _ = self.enqueue(None, quantized, resident=(uploaded[0], ranges))
-            self._staging(0, len(ranges), int(cu[-1]))
-            out_h = self._stage['out_h']
-            out_h[:slab.numel()].copy_(slab, non_blocking=True)
-            torch.cuda.current_stream(dev).synchronize()
-            results = self.unpack_slab(out_h[:slab.numel()].numpy(), cu, layout)
-        offsets = [begin / slicer.sr for begin, _ in ranges]
+        if one_chunk(slicer, n):
+            return [0], self.infer([samples], quantized)
+        with torch.cuda.device(self.device):
+            src = torch.from_numpy(samples)
+            if not src.is_pinned():
+                st = self._staging(n, 1, 1 + n // HOP)
+                st['wave_h'][:n].copy_(src)
+                src = st['wave_h'][:n]
+            wave_d = torch.empty(n, dtype=torch.float32, device=self.device)
+            wave_d.copy_(src, non_blocking=True)
+            [(offsets, results)] = self.transcribe_resident(wave_d, [0], [n], slicer, quantized)
         return offsets, results
 
     def unpack_slab(self, host: np.ndarray, cu: np.ndarray, layout, extra=None) -> List[Dict[str, np.ndarray]]:

@@ -34,7 +34,7 @@ from typing import Callable, Dict, List, Optional, Sequence, Union
 import numpy as np
 
 from . import _lib, audio
-from .batch import load_groups, midi_to_note, note_to_midi, stage_recordings
+from .batch import load_groups, midi_to_note, note_to_midi, staged
 
 HOP = 512
 
@@ -269,48 +269,37 @@ def evaluate_recordings(infer_ins, waveforms: Sequence, labels: Sequence[Dict[st
     import torch
     eng = infer_ins.model
     quantized = bool(getattr(infer_ins, 'quantized', False))
-    target_sr = int(infer_ins.config['audio_sample_rate'])
     if precision not in ('bf16', 'fp32'):
         raise ValueError(f"precision must be 'bf16' or 'fp32', got {precision!r}")
-    lock = getattr(infer_ins, '_lock', None)
-    if lock is not None:
-        lock.acquire()
-    try:
-        with torch.cuda.device(eng.device):
-            wave_d, bases, lens, flac_status = stage_recordings(eng, target_sr, waveforms, rates)
-            frames = [1 + n // HOP for n in lens]
-            for lab, t, it in zip(labels, frames, range(len(labels))):
-                if lab['unit2note'].shape[0] != t:
-                    raise ValueError(f'recording {it}: labels for {lab["unit2note"].shape[0]} frames, audio has {t}')
-            lab = _Labels(labels, eng.device)
-            ranges = [(int(b), int(b) + n) for b, n in zip(bases, lens)]
-            if precision == 'bf16':
-                def hook(ws, c0, c1, mc, cu_d):
-                    eval_clips(eng, ws.probs, ws.bounds, cu_d, lab, c0, c1, int(cu[c0]), mc, quantized,
-                               _lib.EVAL_HEAD_TC, probs=ws.probs)
-                cu = np.zeros(len(ranges) + 1, dtype=np.int64)
-                np.cumsum(frames, out=cu[1:])
-                slab, cu_e, layout, _ = eng.enqueue(None, quantized, resident=(wave_d, ranges), logits_hook=hook)
-                notes = eng.unpack_slab(slab.cpu().numpy(), cu_e, layout)
-            else:
-                notes = []
-                for i, ((b0, _), n, t) in enumerate(zip(ranges, lens, frames)):
-                    start = torch.zeros(1, dtype=torch.int64, device=eng.device)
-                    length = torch.full((1,), n, dtype=torch.int64, device=eng.device)
+    with staged(infer_ins, waveforms, rates) as (wave_d, bases, lens):
+        frames = [1 + n // HOP for n in lens]
+        for lab, t, it in zip(labels, frames, range(len(labels))):
+            if lab['unit2note'].shape[0] != t:
+                raise ValueError(f'recording {it}: labels for {lab["unit2note"].shape[0]} frames, audio has {t}')
+        lab = _Labels(labels, eng.device)
+        ranges = [(int(b), int(b) + n) for b, n in zip(bases, lens)]
+        if precision == 'bf16':
+            def hook(ws, c0, c1, mc, cu_d):
+                eval_clips(eng, ws.probs, ws.bounds, cu_d, lab, c0, c1, int(cu[c0]), mc, quantized,
+                           _lib.EVAL_HEAD_TC, probs=ws.probs)
+            cu = np.zeros(len(ranges) + 1, dtype=np.int64)
+            np.cumsum(frames, out=cu[1:])
+            slab, cu_e, layout, _ = eng.enqueue(None, quantized, resident=(wave_d, ranges), logits_hook=hook)
+            notes = eng.unpack_slab(slab.cpu().numpy(), cu_e, layout)
+        else:
+            notes = []
+            for i, ((b0, _), n, t) in enumerate(zip(ranges, lens, frames)):
+                start = torch.zeros(1, dtype=torch.int64, device=eng.device)
+                length = torch.full((1,), n, dtype=torch.int64, device=eng.device)
 
-                    def hook(tt, cu_d, i=i, t=t):
-                        eval_clips(eng, tt['probs'], tt['bounds'], cu_d, lab, i, i + 1, int(sum(frames[:i])), t, quantized,
-                                   _lib.EVAL_HEAD_F32, probs=tt['probs'])
-                    _, ws, k = eng.accurate_clip(wave_d[b0:] if n else wave_d, start, length, t, quantized, logits_hook=hook)
-                    notes.append({'note_midi': ws.note_midi[:k].cpu().numpy(),
-                                  'note_dur': ws.note_dur[:k].cpu().numpy().astype(np.int64) * eng.timestep,
-                                  'note_rest': ws.note_rest[:k].cpu().numpy().astype(bool)})
-            midi_sum, bound_sum, correct = lab.midi_loss.cpu().numpy(), lab.bound_loss.cpu().numpy(), lab.correct.cpu().numpy()
-            for st in flac_status:
-                audio._check_status(st)
-    finally:
-        if lock is not None:
-            lock.release()
+                def hook(tt, cu_d, i=i, t=t):
+                    eval_clips(eng, tt['probs'], tt['bounds'], cu_d, lab, i, i + 1, int(sum(frames[:i])), t, quantized,
+                               _lib.EVAL_HEAD_F32, probs=tt['probs'])
+                _, ws, k = eng.accurate_clip(wave_d[b0:] if n else wave_d, start, length, t, quantized, logits_hook=hook)
+                notes.append({'note_midi': ws.note_midi[:k].cpu().numpy(),
+                              'note_dur': ws.note_dur[:k].cpu().numpy().astype(np.int64) * eng.timestep,
+                              'note_rest': ws.note_rest[:k].cpu().numpy().astype(bool)})
+        midi_sum, bound_sum, correct = lab.midi_loss.cpu().numpy(), lab.bound_loss.cpu().numpy(), lab.correct.cpu().numpy()
     return [(float(ms), float(bs), int(c), t, nt) for ms, bs, c, t, nt in zip(midi_sum, bound_sum, correct, frames, notes)]
 
 

@@ -3,14 +3,15 @@
 The reference computes the short-time RMS with numpy (slicer2.py:5-38: ~53 M multiply-adds and a 200 MB temporary for a
 5-minute recording) and then walks the RMS list frame by frame in Python (:84-127).  Here
 
-* the RMS frames come from ``some_slicer_rms`` (csrc/slicer.cu): the recording is uploaded once — it has to go to the GPU
-  for the mel front end anyway — and the kernel reproduces numpy's float32 pairwise summation bit for bit, so every
-  threshold comparison and argmin sees the reference's numbers;
+* the RMS frames come from ``some_slicer_rms`` (csrc/slicer.cu), launched by ``rms_lists`` on recordings that are already
+  on the device — they have to go to the GPU for the mel front end anyway — and the kernel reproduces numpy's float32
+  pairwise summation bit for bit, so every threshold comparison and argmin sees the reference's numbers;
 * the cuts are decided by the native slicer next to that kernel (``some_slicer_ranges``, csrc/slicer.cu), on the host with no
   CUDA call: per SILENT RUN instead of per frame, since the reference's loop only acts on the first voiced frame after a run
   of frames with ``rms < threshold``.  The native session, streaming and the C ABI use the same code, so the cut rules exist
   once;
-* ``Engine.infer_sliced`` then processes the chunks where they lie in device memory (no second upload).
+* ``Engine.transcribe_resident`` cuts recordings with ``cut_ranges`` over ``rms_lists`` and runs the chunks where they lie in
+  device memory (no second upload); ``Engine.infer_sliced`` and ``batch.transcribe_recordings`` upload into it.
 
 ``Slicer`` keeps the reference's constructor, derived attributes and ``slice()`` return value (list of
 ``{'offset': seconds, 'waveform': view}``), so ``infer.py``-style callers can use it unchanged.  There is no CPU path:
@@ -54,14 +55,41 @@ def slicer_ranges(rms: np.ndarray, num_samples: int, frames: _lib.SlicerFrames) 
     return [(int(out[2 * k]), int(out[2 * k + 1])) for k in range(count.value)]
 
 
+def rms_lists(waves_d: Sequence, frame_length: int, hop: int) -> List[np.ndarray]:
+    """Short-time RMS lists of device-resident float32 recordings, bit-identical to the reference's get_rms
+    (slicer2.py:5-38): one ``some_slicer_rms`` launch each into one buffer on the current stream, then one device-to-host
+    copy and sync for all of them."""
+    import torch
+    counts = [1 + (int(w.numel()) + 2 * (frame_length // 2) - frame_length) // hop for w in waves_d]
+    if not counts:
+        return []
+    lib = _lib.load()
+    dev = waves_d[0].device
+    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    cuts = np.zeros(len(counts) + 1, dtype=np.int64)
+    np.cumsum(counts, out=cuts[1:])
+    rms_d = torch.empty(int(cuts[-1]), dtype=torch.float32, device=dev)
+    for w, a, n in zip(waves_d, cuts, counts):
+        _lib.check(lib.some_slicer_rms(w.data_ptr(), int(w.numel()), frame_length, hop, rms_d[a:].data_ptr(), n, stream),
+                   'some_slicer_rms')
+    host = rms_d.cpu().numpy()
+    return [host[a:b] for a, b in zip(cuts[:-1], cuts[1:])]
+
+
+def one_chunk(slicer, num_samples: int) -> bool:
+    """Whether ``slicer`` leaves a recording of ``num_samples`` samples whole without looking at its RMS: no more than
+    min_length hops (slicer2.py:79-80)."""
+    return (num_samples + slicer.hop_size - 1) // slicer.hop_size <= slicer.min_length
+
+
 def cut_ranges(slicer, lengths: Sequence[int],
                rms_of: Callable[[List[int]], Sequence[np.ndarray]]) -> List[List[Tuple[int, int]]]:
     """[begin, end) sample ranges of the chunks of recordings of the given lengths, cut by ``slicer``: any object with the
-    reference Slicer's attributes (threshold, hop_size, win_size, min_length, min_interval, max_sil_kept).  A recording of no
-    more than min_length hops is one chunk (slicer2.py:79-80); ``rms_of(indices)`` returns the RMS lists of the others, in
-    that order, and is called once, only if there is one, so that short recordings make no device call."""
+    reference Slicer's attributes (threshold, hop_size, win_size, min_length, min_interval, max_sil_kept).  A recording
+    that is ``one_chunk`` stays whole; ``rms_of(indices)`` returns the RMS lists of the others, in that order, and is called
+    once, only if there is one, so that short recordings make no device call."""
     out = [[(0, int(n))] for n in lengths]
-    need = [i for i, n in enumerate(lengths) if (n + slicer.hop_size - 1) // slicer.hop_size > slicer.min_length]
+    need = [i for i, n in enumerate(lengths) if not one_chunk(slicer, n)]
     if need:
         frames = _lib.SlicerFrames(np.float32(slicer.threshold), slicer.hop_size, slicer.win_size, slicer.min_length,
                                    slicer.min_interval, slicer.max_sil_kept)
@@ -143,19 +171,12 @@ class Slicer:
     def rms(self, samples: np.ndarray) -> np.ndarray:
         """RMS list of a mono float32 waveform, computed on the GPU (bit-identical to get_rms, slicer2.py:5-38)."""
         import torch
-        lib = _lib.load()
         if not torch.cuda.is_available():
             raise _lib.SomeB200Error('some_b200.slicer needs a CUDA device (no CPU path)')
         dev = torch.device(self.device if self.device is not None else 'cuda')
         with torch.cuda.device(dev):
             x = torch.from_numpy(np.ascontiguousarray(samples, dtype=np.float32)).to(dev)
-            n = int(x.numel())
-            n_frames = 1 + (n + 2 * (self.win_size // 2) - self.win_size) // self.hop_size
-            out = torch.empty(n_frames, dtype=torch.float32, device=dev)
-            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(lib.some_slicer_rms(x.data_ptr(), n, self.win_size, self.hop_size, out.data_ptr(), n_frames, stream),
-                       'some_slicer_rms')
-            return out.cpu().numpy()
+            return rms_lists([x], self.win_size, self.hop_size)[0]
 
     # ------------------------------------------------------------------ reference API
     def ranges(self, waveform: np.ndarray) -> List[Tuple[int, int]]:
