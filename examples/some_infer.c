@@ -1,7 +1,7 @@
 /* some_infer: infer.py in C.  Transcribes a WAV, FLAC or AIFF file with a model file written by `python -m some_b200.export` and
  * saves the notes as a MIDI file, without Python.
  *
- *   some_infer MODEL AUDIO [--midi PATH] [--tempo BPM] [--device N]
+ *   some_infer MODEL AUDIO [--midi PATH] [--tempo BPM] [--device N[,N...]]
  *
  * The file is decoded on the GPU (librosa.load(AUDIO, sr=None, mono=True)), resampled to the model's rate, cut by the silence
  * slicer of infer.py and transcribed by some_session_transcribe_encoded; the MIDI bytes are those of
@@ -13,6 +13,20 @@
 #include <string.h>
 
 #include "some_b200.h"
+
+/* Parses a device list: one index, or several separated by commas ("0,1"; "0,0" runs two replicas on one GPU).  Returns the
+ * count (at most 64), or 0 when the list is malformed. */
+static int parse_devices(const char* list, int* devices) {
+  int n = 0;
+  for (const char* p = list;; ++p) {
+    char* end;
+    const long v = strtol(p, &end, 10);
+    if (end == p || *p == '-' || *p == '+' || v > 1000000 || n == 64 || (*end != ',' && *end != '\0')) return 0;
+    devices[n++] = (int)v;
+    if (*end == '\0') return n;
+    p = end;
+  }
+}
 
 /* pathlib.PurePath(path).with_suffix('.mid'): the suffix of the last component (a leading dot does not start one). */
 static char* with_mid_suffix(const char* path) {
@@ -76,17 +90,17 @@ int main(int argc, char** argv) {
   const char* audio = NULL;
   const char* midi = NULL;
   double tempo = 120.0;
-  int device = 0, positional = 0;
+  int devices[64] = {0}, n_devices = 1, positional = 0;
   for (int i = 1; i < argc; ++i) {
     if (!strcmp(argv[i], "--midi") && i + 1 < argc) midi = argv[++i];
     else if (!strcmp(argv[i], "--tempo") && i + 1 < argc) tempo = atof(argv[++i]);
-    else if (!strcmp(argv[i], "--device") && i + 1 < argc) device = atoi(argv[++i]);
+    else if (!strcmp(argv[i], "--device") && i + 1 < argc) n_devices = parse_devices(argv[++i], devices);
     else if (positional == 0) model = argv[i], ++positional;
     else if (positional == 1) audio = argv[i], ++positional;
     else positional = 3;
   }
-  if (!model || !audio || positional != 2) {
-    fprintf(stderr, "usage: %s MODEL AUDIO [--midi PATH] [--tempo BPM] [--device N]\n", argv[0]);
+  if (!model || !audio || positional != 2 || n_devices == 0) {
+    fprintf(stderr, "usage: %s MODEL AUDIO [--midi PATH] [--tempo BPM] [--device N[,N...]]\n", argv[0]);
     return 2;
   }
   long long n_bytes = 0;
@@ -101,7 +115,7 @@ int main(int argc, char** argv) {
   int rc = 1;
   const some_encoded item = {bytes, n_bytes};
   size_t size = 0;
-  if (!path || some_session_open(model, device, &s) != 0 || some_session_get_info(s, &info) != 0 ||
+  if (!path || some_session_open_devices(model, devices, n_devices, &s) != 0 || some_session_get_info(s, &info) != 0 ||
       some_notes_create(&notes) != 0 || some_session_transcribe_encoded(s, &item, 1, NULL, &notes) != 0 ||
       some_notes_midi(notes, info.sample_rate, info.timestep, tempo, NULL, 0, &size) != 0 || !(buf = malloc(size)) ||
       some_notes_midi(notes, info.sample_rate, info.timestep, tempo, buf, size, &size) != 0) {

@@ -1,8 +1,8 @@
 /* some_stream: transcribe a recording while it arrives, with a model file written by `python -m some_b200.export`, without
  * Python.
  *
- *   some_stream MODEL RATE [DEVICE] < pcm
- *   some_stream MODEL - [DEVICE] < file.wav, file.flac or file.aif
+ *   some_stream MODEL RATE [DEVICES] < pcm
+ *   some_stream MODEL - [DEVICES] < file.wav, file.flac or file.aif
  *
  * With RATE, reads raw mono little-endian float32 samples at RATE Hz from stdin in blocks of 100 ms and pushes each block to a
  * some_stream.  With `-`, reads a WAV, FLAC or AIFF byte stream from stdin in 64 KB reads and pushes each read to an encoded
@@ -21,6 +21,20 @@
 #include <string.h>
 
 #include "some_b200.h"
+
+/* Parses a device list: one index, or several separated by commas ("0,1"; "0,0" runs two replicas on one GPU).  Returns the
+ * count (at most 64), or 0 when the list is malformed. */
+static int parse_devices(const char* list, int* devices) {
+  int n = 0;
+  for (const char* p = list;; ++p) {
+    char* end;
+    const long v = strtol(p, &end, 10);
+    if (end == p || *p == '-' || *p == '+' || v > 1000000 || n == 64 || (*end != ',' && *end != '\0')) return 0;
+    devices[n++] = (int)v;
+    if (*end == '\0') return n;
+    p = end;
+  }
+}
 
 static void print_chunks(const some_notes* notes, const some_session_info* info) {
   const int chunks = some_notes_clips(notes);
@@ -70,15 +84,21 @@ done:
 int main(int argc, char** argv) {
   const int encoded = argc >= 3 && strcmp(argv[2], "-") == 0;
   if (argc < 3 || (!encoded && atoi(argv[2]) <= 0)) {
-    fprintf(stderr, "usage: %s MODEL RATE [DEVICE] < mono float32 little-endian PCM\n"
-                    "       %s MODEL - [DEVICE] < WAV, FLAC or AIFF bytes\n", argv[0], argv[0]);
+    fprintf(stderr, "usage: %s MODEL RATE [DEVICES] < mono float32 little-endian PCM\n"
+                    "       %s MODEL - [DEVICES] < WAV, FLAC or AIFF bytes\n", argv[0], argv[0]);
+    return 2;
+  }
+  int devices[64] = {0};
+  const int n_devices = argc > 3 ? parse_devices(argv[3], devices) : 1;
+  if (n_devices == 0) {
+    fprintf(stderr, "some_stream: bad device list '%s' (device indices separated by commas)\n", argv[3]);
     return 2;
   }
   if (encoded) {
     some_session* s = NULL;
     some_session_info info;
     int rc = 1;
-    if (some_session_open(argv[1], argc > 3 ? atoi(argv[3]) : 0, &s) != 0 || some_session_get_info(s, &info) != 0)
+    if (some_session_open_devices(argv[1], devices, n_devices, &s) != 0 || some_session_get_info(s, &info) != 0)
       fprintf(stderr, "some_stream: %s\n", some_last_error());
     else
       rc = run_encoded(s, &info);
@@ -95,7 +115,7 @@ int main(int argc, char** argv) {
   some_session_info info;
   int rc = 1;
   if (!raw || !samples) goto done;
-  if (some_session_open(argv[1], argc > 3 ? atoi(argv[3]) : 0, &s) != 0 || some_session_get_info(s, &info) != 0 ||
+  if (some_session_open_devices(argv[1], devices, n_devices, &s) != 0 || some_session_get_info(s, &info) != 0 ||
       some_notes_create(&notes) != 0 || some_stream_open(s, rate, NULL, &st) != 0) {
     fprintf(stderr, "some_stream: %s\n", some_last_error());
     goto done;

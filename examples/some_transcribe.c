@@ -1,6 +1,6 @@
 /* some_transcribe: transcribe a WAV file with a model file written by `python -m some_b200.export`, without Python.
  *
- *   some_transcribe MODEL WAV [DEVICE]
+ *   some_transcribe MODEL WAV [DEVICES]
  *
  * Reads a mono RIFF/WAVE file (16-bit PCM, scaled x / 32768 as libsndfile hands it to librosa.load, or 32-bit float) at any
  * rate, runs some_session_transcribe_sliced (resampling to the model's rate on the GPU when needed, then the silence slicer of
@@ -8,7 +8,8 @@
  *
  *   <chunk offset in seconds> <note_midi> <duration in seconds> <rest 0/1>
  *
- * with the duration computed as (double)dur * timestep, the float64 product of me_infer.py:95. */
+ * with the duration computed as (double)dur * timestep, the float64 product of me_infer.py:95.  DEVICES is a device index (default
+ * 0) or a comma-separated list of them: a replica of the model on each, with the same output. */
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -18,6 +19,20 @@
 
 static uint32_t le32(const unsigned char* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
 static uint16_t le16(const unsigned char* p) { return (uint16_t)(p[0] | (p[1] << 8)); }
+
+/* Parses a device list: one index, or several separated by commas ("0,1"; "0,0" runs two replicas on one GPU).  Returns the
+ * count (at most 64), or 0 when the list is malformed. */
+static int parse_devices(const char* list, int* devices) {
+  int n = 0;
+  for (const char* p = list;; ++p) {
+    char* end;
+    const long v = strtol(p, &end, 10);
+    if (end == p || *p == '-' || *p == '+' || v > 1000000 || n == 64 || (*end != ',' && *end != '\0')) return 0;
+    devices[n++] = (int)v;
+    if (*end == '\0') return n;
+    p = end;
+  }
+}
 
 /* Returns the samples (malloc'ed) or NULL with a message on stderr. */
 static float* read_wav(const char* path, long long* n_out, int* rate_out) {
@@ -92,7 +107,13 @@ done:
 
 int main(int argc, char** argv) {
   if (argc < 3) {
-    fprintf(stderr, "usage: %s MODEL WAV [DEVICE]\n", argv[0]);
+    fprintf(stderr, "usage: %s MODEL WAV [DEVICES]\n", argv[0]);
+    return 2;
+  }
+  int devices[64] = {0};
+  const int n_devices = argc > 3 ? parse_devices(argv[3], devices) : 1;
+  if (n_devices == 0) {
+    fprintf(stderr, "some_transcribe: bad device list '%s' (device indices separated by commas)\n", argv[3]);
     return 2;
   }
   long long n = 0;
@@ -103,7 +124,7 @@ int main(int argc, char** argv) {
   some_notes* notes = NULL;
   some_session_info info;
   int rc = 1;
-  if (some_session_open(argv[1], argc > 3 ? atoi(argv[3]) : 0, &s) != 0 || some_session_get_info(s, &info) != 0 ||
+  if (some_session_open_devices(argv[1], devices, n_devices, &s) != 0 || some_session_get_info(s, &info) != 0 ||
       some_notes_create(&notes) != 0 || some_session_transcribe_sliced(s, samples, n, rate, NULL, notes) != 0) {
     fprintf(stderr, "some_transcribe: %s\n", some_last_error());
     goto done;

@@ -716,6 +716,32 @@ typedef struct {
 } some_slicer_frames;
 
 int some_session_open(const char* path, int device, some_session** out);
+/* ---- One session on several devices: a replica of the model on each listed device, the chunks of every call spread over them.
+ * For every call, a session opened on devices [d0, d1, ...] returns exactly what a session on [d0] returns: the same clips and
+ * chunks in the same order, the same ranges and bit-identical notes (a chunk's notes do not depend on the rest of its batch).
+ * The front end (byte upload, FLAC scan and decode, PCM decode, resampling, RMS windows, the slicer, the stream buffers) runs
+ * on d0 as in a one-device session; the chunks of the call are then assigned with some_shard_clips, replica 0 runs its share
+ * on the calling thread and each other replica its share on a thread of its own (created at open, joined at close), with the
+ * caller's some_set_pdl setting.  Chunks on d0's device go to replica r with cudaMemcpyPeerAsync (peer access is used when
+ * the application has enabled it, not required); host clips of some_session_transcribe are staged straight to their replica.
+ *   Each replica holds its own copy of the weights (104 MB for two_head, 235 MB for midi_conformer) and the workspace of its
+ * share.  A device may be listed twice: two replicas on one GPU.
+ *   some_session_open_devices checks, in this order: the arguments (devices not NULL, 1 <= n <= 64, every entry >= 0), the
+ * model file exactly as some_session_open does, before any CUDA call, then every listed device (it exists and is sm_90)
+ * before anything is allocated; a refused device is named by its index in the list.  some_session_open(path, d, out) is the
+ * n == 1 case.  A device error on any replica fails the call with a message naming the device; every replica's streams are
+ * waited for and the session stays usable.  some_session_close waits for every replica and frees each one's memory on its own
+ * device. */
+int some_session_open_devices(const char* path, const int* devices, int n, some_session** out);
+/* The session's devices in replica order: *n = their count, the first min(capacity, *n) written to devices. */
+int some_session_get_devices(const some_session* s, int* devices, int capacity, int* n);
+/* For each replica, the chunks and frames (1 + samples / 512 each) it ran in the session's last completed call: *n = the
+ * replica count, the first min(capacity, *n) written. */
+int some_session_get_load(const some_session* s, int64_t* chunks, int64_t* frames, int capacity, int* n);
+/* Host only, no CUDA call: owner[i] = the replica of clip i of n.  Longest processing time first: clips in order of
+ * (-cost, index), cost = T * (103.31e6 + 16384 * T) with T = 1 + lens[i] / 512, each to the least loaded replica (ties: the
+ * lowest).  The sessions above and some_b200.dist.shard_clips assign clips with it. */
+int some_shard_clips(const int64_t* lens, int n, int replicas, int32_t* owner);
 int some_session_close(some_session* s);
 int some_session_get_info(const some_session* s, some_session_info* info);
 int some_session_transcribe(some_session* s, const float* const* clips, const int64_t* lens, int B, some_notes* out);

@@ -245,6 +245,10 @@ EXPORTS = {
     'some_profiler_read': (C.c_int, [_vp, C.c_int, C.POINTER(ProfileRecord)]),
     'some_session_open': (C.c_int, [C.c_char_p, C.c_int, C.POINTER(_vp)]),
     'some_session_close': (C.c_int, [_vp]),
+    'some_session_open_devices': (C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.c_int, C.POINTER(_vp)]),
+    'some_session_get_devices': (C.c_int, [_vp, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]),
+    'some_session_get_load': (C.c_int, [_vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int, C.POINTER(C.c_int)]),
+    'some_shard_clips': (C.c_int, [_vp, C.c_int, C.c_int, _vp]),
     'some_session_get_info': (C.c_int, [_vp, C.POINTER(SessionInfo)]),
     'some_session_transcribe': (C.c_int, [_vp, _vp, _vp, C.c_int, _vp]),
     'some_session_transcribe_sliced': (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.POINTER(SlicerParams), _vp]),

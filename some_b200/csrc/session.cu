@@ -6,7 +6,9 @@
 // The sliced and the encoded calls share that front end (Recordings: one resampling window per recording at another rate,
 // one RMS window per recording that is cut, one batch over the chunks of all recordings); a stream step launches the same
 // two kernels over the windows of its streams.  The encoded files call and the encoded stream step share the stage in front
-// of it (Decode: one upload of the audio bytes, one FLAC scan, one PCM and one FLAC decode).
+// of it (Decode: one upload of the audio bytes, one FLAC scan, one PCM and one FLAC decode).  A session opened on several
+// devices holds one replica of the model per device: the front end runs on replica 0, and run_chunks spreads the chunks of
+// each call over the replicas, each on its own thread, and gathers their notes in chunk order.
 //
 // The model file (little-endian; INTEGRATION.md "Deploying without Python" has the table):
 //   header     128 bytes: magic "SOMEB200", format version, ABI number, file size, directory offset, tensor count, the scalars
@@ -267,11 +269,11 @@ struct some_notes {
   std::vector<uint8_t> rest;
 };
 
-struct some_session {
-  std::mutex mu;
+namespace {
+// One copy of the model on one device, and what it needs to run a batch of chunks there: a session holds one replica per
+// device it was opened on (a device listed twice holds two).  Replica 0 also runs the front end of every call.
+struct Replica {
   int device = 0;
-  some_session_info info{};
-  float vmin = 0.f, vmax = 0.f, deviation = 1.f, threshold = 0.1f;
   void* weights = nullptr;
   std::vector<some_block_weights> blocks;
   std::vector<const uint16_t*> glu_w;
@@ -279,6 +281,23 @@ struct some_session {
   some_model model{};
   const int32_t *mel_start = nullptr, *mel_count = nullptr;
   const float *mel_weights = nullptr, *twiddle = nullptr, *window = nullptr;
+  cudaStream_t stream = nullptr, copy_stream = nullptr;
+  cudaEvent_t ev[4] = {};
+  // grow-only buffers of its batches; wave: the staged clips, or the chunks copied from replica 0's device
+  DevBuf ws_block, scratch, wave_d, tab_d, cu_d, slab_d;
+  PinBuf wave_h, tab_h, cu_h, slab_h;
+  int ws_m = 0;
+  some_workspace ws{};
+  std::unique_ptr<WorkerPool> pool;       // its staging lanes (WorkerPool::run is not re-entrant)
+  some_notes part;                        // with several replicas: the notes of its share of a call
+  int64_t chunks = 0, frames = 0;         // its share of the call in progress
+};
+}  // namespace
+
+struct some_session {
+  mutable std::mutex mu;
+  some_session_info info{};
+  float vmin = 0.f, vmax = 0.f, deviation = 1.f, threshold = 0.1f;
   std::vector<double> kaiser;             // host copy of the float64 table (scaled per rate pair on upload)
   // the device tables by downsampling ratio (1.0: the unscaled table every upsampling pair shares), each kept with the host
   // copy its upload reads
@@ -287,32 +306,45 @@ struct some_session {
     std::vector<double> h;
   };
   std::map<double, Table> tables;
-  cudaStream_t stream = nullptr, copy_stream = nullptr;
-  cudaEvent_t ev[4] = {};
-  // grow-only buffers; rec_d: recordings at their own rates and at the model's (the sliced and encoded calls)
-  DevBuf ws_block, scratch, wave_d, tab_d, cu_d, slab_d, rec_d, rms_d, step_d;
-  PinBuf wave_h, tab_h, cu_h, slab_h, rms_h, step_h;   // step: the samples and descriptors of a step's upload
+  // replica 0's device, stream and staging lanes, which the front end (uploads, decode, resampling, RMS) runs on
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  WorkerPool* pool = nullptr;
+  // grow-only buffers on replica 0's device; rec_d: recordings at their own rates and at the model's (the sliced and
+  // encoded calls)
+  DevBuf rec_d, rms_d, step_d;
+  PinBuf rms_h, step_h;                   // step: the samples and descriptors of a step's upload
   // the encoded calls' Decode: the audio bytes, the FLAC candidate list, scan workspace and int32 scratch
   DevBuf enc_d, flac_frames_d, flac_ws_d, flac_scratch_d;
   PinBuf enc_h, flac_frames_h;
-  int ws_m = 0;
-  some_workspace ws{};
   some_notes chunks;                      // the notes of a step's chunks, before they are split by recording or stream
-  std::unique_ptr<WorkerPool> pool;
+  std::vector<std::unique_ptr<Replica>> reps;
+  // with several replicas: lane r runs replica r's share of a call (lane 0 on the calling thread), and `fed` is recorded on
+  // replica 0's stream once the front end has written the chunks the others copy
+  std::unique_ptr<WorkerPool> lanes;
+  cudaEvent_t fed = nullptr;
+  std::vector<std::pair<int64_t, int64_t>> load;   // each replica's chunks and frames in the last completed call
 };
 
 namespace {
 
 void destroy(some_session* s) {
+  s->lanes.reset();                       // joins the replicas' threads
+  for (std::unique_ptr<Replica>& r : s->reps) {
+    if (!r) continue;
+    DeviceScope scope(r->device);
+    if (r->stream) cudaStreamSynchronize(r->stream);
+    if (r->copy_stream) cudaStreamSynchronize(r->copy_stream);
+    for (cudaEvent_t& e : r->ev)
+      if (e) cudaEventDestroy(e);
+    if (r->stream) cudaStreamDestroy(r->stream);
+    if (r->copy_stream) cudaStreamDestroy(r->copy_stream);
+    if (r->weights) cudaFree(r->weights);
+    r.reset();                            // its buffers free themselves, on its device
+  }
   DeviceScope scope(s->device);
-  if (s->stream) cudaStreamSynchronize(s->stream);
-  if (s->copy_stream) cudaStreamSynchronize(s->copy_stream);
-  for (cudaEvent_t& e : s->ev)
-    if (e) cudaEventDestroy(e);
-  if (s->stream) cudaStreamDestroy(s->stream);
-  if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
-  if (s->weights) cudaFree(s->weights);
-  delete s;                               // its buffers free themselves, on the session's device
+  if (s->fed) cudaEventDestroy(s->fed);
+  delete s;                               // its buffers free themselves, on replica 0's device
 }
 
 void clear(some_notes* out) {
@@ -380,10 +412,11 @@ std::vector<std::pair<int, int>> split_chunks(const std::vector<int32_t>& cu) {
   return out;
 }
 
-// One var-len batch through mel -> trunk -> decode, pipelined like Engine.enqueue.  Host clips (`host` != NULL: clip i is
-// host[i][0 .. lens[i])) are staged through pinned memory and copied on the copy stream while the previous chunk's kernels
-// run; resident clips (`resident` != NULL) are the sample ranges [starts[i], starts[i] + lens[i]) of that device buffer.
-int run_batch(some_session* s, const float* const* host, const float* resident, const int64_t* res_starts,
+// One var-len batch through mel -> trunk -> decode on replica r, pipelined like Engine.enqueue.  Host clips (`host` != NULL:
+// clip i is host[i][0 .. lens[i])) are staged through pinned memory and copied on the copy stream while the previous chunk's
+// kernels run; resident clips (`resident` != NULL) are the sample ranges [starts[i], starts[i] + lens[i]) of that buffer on
+// r's device, written by work on r's streams or awaited by its copy stream.
+int run_batch(const some_session* s, Replica& r, const float* const* host, const float* resident, const int64_t* res_starts,
               const int64_t* lens, int B, some_notes* out) {
   std::vector<int32_t> cu(B + 1, 0);
   std::vector<int64_t> starts(B, 0);
@@ -411,34 +444,34 @@ int run_batch(some_session* s, const float* const* host, const float* resident, 
     max_mc = std::max(max_mc, mc);
   }
   // buffers
-  if (max_mc > s->ws_m) {
+  if (max_mc > r.ws_m) {
     const uint64_t bytes = some_workspace_bytes(max_mc, s->info.outdim, 0);
-    if (s->ws_block.ensure(bytes, "the workspace")) return -1;
-    if (some_workspace_carve(s->ws_block.p, s->ws_block.cap, max_mc, s->info.outdim, 0, &s->ws)) return -1;
-    if (s->scratch.ensure(some_decode_scratch_bytes(max_mc), "the decode scratch")) return -1;
-    s->ws_m = max_mc;
+    if (r.ws_block.ensure(bytes, "the workspace")) return -1;
+    if (some_workspace_carve(r.ws_block.p, r.ws_block.cap, max_mc, s->info.outdim, 0, &r.ws)) return -1;
+    if (r.scratch.ensure(some_decode_scratch_bytes(max_mc), "the decode scratch")) return -1;
+    r.ws_m = max_mc;
   }
-  if (s->tab_h.ensure(16ull * B + 16, "tables") || s->tab_d.ensure(16ull * B + 16, "tables") ||
-      s->cu_h.ensure(4ull * (B + layout.size()) + 4, "cu_frames") || s->cu_d.ensure(4ull * (B + layout.size()) + 4, "cu_frames") ||
-      s->slab_h.ensure(slab_bytes + 16, "the note slab") || s->slab_d.ensure(slab_bytes + 16, "the note slab"))
+  if (r.tab_h.ensure(16ull * B + 16, "tables") || r.tab_d.ensure(16ull * B + 16, "tables") ||
+      r.cu_h.ensure(4ull * (B + layout.size()) + 4, "cu_frames") || r.cu_d.ensure(4ull * (B + layout.size()) + 4, "cu_frames") ||
+      r.slab_h.ensure(slab_bytes + 16, "the note slab") || r.slab_d.ensure(slab_bytes + 16, "the note slab"))
     return -1;
-  if (host && (s->wave_h.ensure(4ull * total + 16, "the staged audio") || s->wave_d.ensure(4ull * total + 16, "the audio")))
+  if (host && (r.wave_h.ensure(4ull * total + 16, "the staged audio") || r.wave_d.ensure(4ull * total + 16, "the audio")))
     return -1;
-  float* wave_h = static_cast<float*>(s->wave_h.p);
-  const float* wave = host ? static_cast<const float*>(s->wave_d.p) : resident;
-  int64_t* tab_h = static_cast<int64_t*>(s->tab_h.p);
-  int64_t* tab_d = static_cast<int64_t*>(s->tab_d.p);
-  int32_t* cu_h = static_cast<int32_t*>(s->cu_h.p);
-  int32_t* cu_d = static_cast<int32_t*>(s->cu_d.p);
-  uint8_t* slab = static_cast<uint8_t*>(s->slab_d.p);
+  float* wave_h = static_cast<float*>(r.wave_h.p);
+  const float* wave = host ? static_cast<const float*>(r.wave_d.p) : resident;
+  int64_t* tab_h = static_cast<int64_t*>(r.tab_h.p);
+  int64_t* tab_d = static_cast<int64_t*>(r.tab_d.p);
+  int32_t* cu_h = static_cast<int32_t*>(r.cu_h.p);
+  int32_t* cu_d = static_cast<int32_t*>(r.cu_d.p);
+  uint8_t* slab = static_cast<uint8_t*>(r.slab_d.p);
   const int head = s->info.quantized ? SOME_EPI_SOFTMAX_F32 : SOME_EPI_SIGMOID_F32;
 
   for (size_t ci = 0; ci < layout.size(); ++ci) {
     const Chunk& ch = layout[ci];
     const int64_t lo = starts[ch.c0];
     if (host) {                                  // stage this chunk's clips; the GPU is still busy with the previous chunk
-      const int nt = std::min(s->pool->size(), ch.bc);
-      s->pool->run(nt, [&](int t) {
+      const int nt = std::min(r.pool->size(), ch.bc);
+      r.pool->run(nt, [&](int t) {
         for (int i = ch.c0 + t; i < ch.c1; i += nt)
           if (lens[i]) memcpy(wave_h + starts[i], host[i], 4ull * lens[i]);
       });
@@ -454,40 +487,40 @@ int run_batch(some_session* s, const float* const* host, const float* resident, 
     for (int i = 0; i <= ch.bc; ++i) cuc[i] = cu[ch.c0 + i] - cu[ch.c0];
     const int64_t hi = host ? starts[ch.c1 - 1] + ((lens[ch.c1 - 1] + 3) & ~int64_t(3)) : lo;
     if (hi > lo)
-      SOME_CUDA(cudaMemcpyAsync(static_cast<float*>(s->wave_d.p) + lo, wave_h + lo, 4ull * (hi - lo), cudaMemcpyHostToDevice,
-                                s->copy_stream), "audio upload");
-    SOME_CUDA(cudaMemcpyAsync(tab_d + 2 * ch.c0, tab, 16ull * ch.bc, cudaMemcpyHostToDevice, s->copy_stream), "table upload");
-    SOME_CUDA(cudaMemcpyAsync(cu_d + ch.c0 + ci, cuc, 4ull * (ch.bc + 1), cudaMemcpyHostToDevice, s->copy_stream),
+      SOME_CUDA(cudaMemcpyAsync(static_cast<float*>(r.wave_d.p) + lo, wave_h + lo, 4ull * (hi - lo), cudaMemcpyHostToDevice,
+                                r.copy_stream), "audio upload");
+    SOME_CUDA(cudaMemcpyAsync(tab_d + 2 * ch.c0, tab, 16ull * ch.bc, cudaMemcpyHostToDevice, r.copy_stream), "table upload");
+    SOME_CUDA(cudaMemcpyAsync(cu_d + ch.c0 + ci, cuc, 4ull * (ch.bc + 1), cudaMemcpyHostToDevice, r.copy_stream),
               "cu_frames upload");
-    SOME_CUDA(cudaEventRecord(s->ev[ci], s->copy_stream), "event record");
-    SOME_CUDA(cudaStreamWaitEvent(s->stream, s->ev[ci], 0), "stream wait");
+    SOME_CUDA(cudaEventRecord(r.ev[ci], r.copy_stream), "event record");
+    SOME_CUDA(cudaStreamWaitEvent(r.stream, r.ev[ci], 0), "stream wait");
 
     const int32_t* cud = cu_d + ch.c0 + ci;
     uint8_t* o = slab + ch.off;
-    if (some_mel_logmel(wave + lo, tab_d + 2 * ch.c0, tab_d + 2 * ch.c0 + ch.bc, cud, ch.bc, max_frames, s->mel_start,
-                        s->mel_count, s->mel_weights, s->twiddle, s->window, nullptr, const_cast<uint16_t*>(s->ws.units), 1e-5f,
-                        s->stream))
+    if (some_mel_logmel(wave + lo, tab_d + 2 * ch.c0, tab_d + 2 * ch.c0 + ch.bc, cud, ch.bc, max_frames, r.mel_start,
+                        r.mel_count, r.mel_weights, r.twiddle, r.window, nullptr, const_cast<uint16_t*>(r.ws.units), 1e-5f,
+                        r.stream))
       return -1;
-    if (some_forward(&s->model, &s->ws, ch.mc, ch.bc, cud, max_frames, head, nullptr, nullptr, s->stream)) return -1;
+    if (some_forward(&r.model, &r.ws, ch.mc, ch.bc, cud, max_frames, head, nullptr, nullptr, r.stream)) return -1;
     some_decode_args d{};
-    d.probs = s->ws.probs, d.bounds = s->ws.bounds, d.cu_frames = cud;
+    d.probs = r.ws.probs, d.bounds = r.ws.bounds, d.cu_frames = cud;
     d.B = ch.bc, d.M = ch.mc, d.N = s->info.outdim, d.quantized = s->info.quantized;
     d.vmin = s->vmin, d.vmax = s->vmax, d.deviation = s->deviation, d.threshold = s->threshold;
     d.note_count = reinterpret_cast<int32_t*>(o);
     d.note_dur = reinterpret_cast<int32_t*>(o + 4ull * ch.bc);
     d.note_midi = reinterpret_cast<float*>(o + 4ull * ch.bc + 4ull * ch.mc);
     d.note_rest = o + 4ull * ch.bc + 8ull * ch.mc;
-    d.scratch = s->scratch.p;
-    if (some_decode_notes(&d, s->stream)) return -1;
+    d.scratch = r.scratch.p;
+    if (some_decode_notes(&d, r.stream)) return -1;
   }
-  if (slab_bytes) SOME_CUDA(cudaMemcpyAsync(s->slab_h.p, slab, slab_bytes, cudaMemcpyDeviceToHost, s->stream), "note download");
-  SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+  if (slab_bytes) SOME_CUDA(cudaMemcpyAsync(r.slab_h.p, slab, slab_bytes, cudaMemcpyDeviceToHost, r.stream), "note download");
+  SOME_CUDA(cudaStreamSynchronize(r.stream), "synchronise");
 
   // unpack: the notes of clip b start at its first frame's row of the chunk slab
   out->first.assign(1, 0);
   out->range.clear();
   out->midi.clear(), out->dur.clear(), out->rest.clear();
-  const uint8_t* h = static_cast<const uint8_t*>(s->slab_h.p);
+  const uint8_t* h = static_cast<const uint8_t*>(r.slab_h.p);
   for (const Chunk& ch : layout) {
     const uint8_t* o = h + ch.off;
     for (int b = 0; b < ch.bc; ++b) {
@@ -509,12 +542,93 @@ int run_batch(some_session* s, const float* const* host, const float* resident, 
   return 0;
 }
 
+// The chunks of a call, on every replica of the session.  With one replica this is run_batch.  With several, some_shard_clips
+// assigns the chunks; replica 0 runs its share on the calling thread and replica r its share on lane r, each with the
+// caller's some_set_pdl setting and each through run_batch; the notes come back in chunk order, as one batch gives them (a
+// chunk's notes do not depend on the rest of its batch).  Resident chunks lie in a buffer on replica 0's device, written on
+// its stream: replica r > 0 waits on its copy stream for `fed`, recorded there after the front end, and copies its share,
+// packed at 16-byte aligned starts, into its own audio buffer (a peer copy, or a device-to-device copy when both replicas are
+// on one device).  Host clips are staged straight to the replica that runs them.
+int run_chunks(some_session* s, const float* const* host, const float* resident, const int64_t* starts, const int64_t* lens,
+               int B, some_notes* out) {
+  const int R = static_cast<int>(s->reps.size());
+  if (R == 1) {
+    Replica& r = *s->reps[0];
+    r.chunks = B;
+    for (int c = 0; c < B; ++c) r.frames += 1 + lens[c] / SOME_HOP;
+    return run_batch(s, r, host, resident, starts, lens, B, out);
+  }
+  std::vector<int32_t> owner(B);
+  if (some_shard_clips(lens, B, R, owner.data())) return -1;
+  std::vector<std::vector<int>> share(R);
+  for (int c = 0; c < B; ++c) share[owner[c]].push_back(c);
+  if (resident) SOME_CUDA(cudaEventRecord(s->fed, s->stream), "event record");
+  const int pdl = pdl_enabled() ? 1 : 0;
+  std::vector<int> rc(R, 0);
+  std::vector<std::string> err(R);
+  s->lanes->run(R, [&](int ri) {
+    Replica& r = *s->reps[ri];
+    const std::vector<int>& mine = share[ri];
+    clear(&r.part);
+    const int b = static_cast<int>(mine.size());
+    if (b == 0) return;
+    std::vector<const float*> clips;
+    std::vector<int64_t> at, len;
+    int64_t total = 0;
+    for (int c : mine) {
+      len.push_back(lens[c]);
+      r.frames += 1 + lens[c] / SOME_HOP;
+      if (host) clips.push_back(host[c]);
+      else if (ri == 0) at.push_back(starts[c]);
+      else at.push_back(total), total += (lens[c] + 3) & ~int64_t(3);
+    }
+    r.chunks = b;
+    auto work = [&]() -> int {
+      if (!resident || ri == 0) return run_batch(s, r, host ? clips.data() : nullptr, resident, at.data(), len.data(), b, &r.part);
+      if (r.wave_d.ensure(4ull * total + 16, "the audio")) return -1;
+      float* wave = static_cast<float*>(r.wave_d.p);
+      SOME_CUDA(cudaStreamWaitEvent(r.copy_stream, s->fed, 0), "stream wait");
+      for (int k = 0; k < b; ++k)
+        if (len[k])
+          SOME_CUDA(cudaMemcpyPeerAsync(wave + at[k], r.device, resident + starts[mine[k]], s->device, 4ull * len[k],
+                                        r.copy_stream), "chunk copy");
+      return run_batch(s, r, nullptr, wave, at.data(), len.data(), b, &r.part);
+    };
+    if (ri == 0) {
+      rc[ri] = work();
+    } else {
+      some_set_pdl(pdl);
+      DeviceScope scope(r.device);
+      if (scope.err != cudaSuccess) set_error("cudaSetDevice: %s", cudaGetErrorString(scope.err)), rc[ri] = -1;
+      else rc[ri] = work();
+    }
+    if (rc[ri]) err[ri] = some_last_error();
+  });
+  for (int ri = 0; ri < R; ++ri)
+    SOME_REQUIRE(rc[ri] == 0, "device %d (replica %d): %s", s->reps[ri]->device, ri, err[ri].c_str());
+  clear(out);
+  std::vector<int> next(R, 0);
+  for (int c = 0; c < B; ++c) {
+    const some_notes& p = s->reps[owner[c]]->part;
+    const int k = next[owner[c]]++;
+    const int64_t a = p.first[k], e = p.first[k + 1];
+    out->midi.insert(out->midi.end(), p.midi.begin() + a, p.midi.begin() + e);
+    out->dur.insert(out->dur.end(), p.dur.begin() + a, p.dur.begin() + e);
+    out->rest.insert(out->rest.end(), p.rest.begin() + a, p.rest.begin() + e);
+    out->first.push_back(out->first.back() + (e - a));
+    out->range.push_back(host ? 0 : starts[c]);
+    out->range.push_back(host ? lens[c] : starts[c] + lens[c]);
+  }
+  return 0;
+}
+
 // Uploads n floats of host memory to `dst` through the pinned staging buffer: in pieces of 16 MB, each copied into pinned
 // memory by the session's threads (256 KB per thread and turn) and then sent while the next piece is copied.
 int upload_staged(some_session* s, float* dst, const float* src, int64_t n) {
   constexpr int64_t kPiece = int64_t(1) << 22;
-  if (s->wave_h.ensure(4ull * n + 16, "the staged audio")) return -1;
-  float* pin = static_cast<float*>(s->wave_h.p);
+  PinBuf& staging = s->reps[0]->wave_h;
+  if (staging.ensure(4ull * n + 16, "the staged audio")) return -1;
+  float* pin = static_cast<float*>(staging.p);
   for (int64_t a = 0; a < n; a += kPiece) {
     const int64_t len = std::min(kPiece, n - a);
     copy_to_pinned(*s->pool, {{pin + a, src + a, 4ull * len}}, size_t(1) << 18);
@@ -555,9 +669,39 @@ extern "C" int some_notes_get(const some_notes* n, int clip, int* count, const f
 }
 
 // ---------------------------------------------------------------------------------------------------- session
-extern "C" int some_session_open(const char* path, int device, some_session** out) {
-  SOME_REQUIRE(path != nullptr && out != nullptr, "some_session_open: null pointer");
-  *out = nullptr;
+namespace {
+constexpr int kMaxReplicas = 64;
+
+// Points a replica's model and mel tables into its copy of the weights; dp(name) is a tensor's device address there.
+template <class Dp>
+void bind_weights(Replica& r, const std::vector<Spec>& specs, int lay, int outdim, Dp dp) {
+  auto fl = [&](const std::string& n) { return static_cast<const float*>(dp(n)); };
+  some_model& m = r.model;
+  r.blocks.resize(2 * (lay + 1));            // value-initialised: the LayerNorm-folded fields stay null
+  for (const Spec& sp : specs) {
+    if (sp.field < 0) continue;
+    const void* p = dp(sp.name);
+    void* target = sp.block < 0 ? static_cast<void*>(&m) : static_cast<void*>(&r.blocks[sp.block]);
+    memcpy(static_cast<uint8_t*>(target) + sp.field, &p, sizeof(p));
+  }
+  for (int j = 0; j < 2 * lay; ++j) {
+    r.glu_w.push_back(static_cast<const uint16_t*>(dp("glu" + std::to_string(j) + ".w")));
+    r.glu_b.push_back(fl("glu" + std::to_string(j) + ".b"));
+  }
+  if (lay == 0) r.glu_w.push_back(nullptr), r.glu_b.push_back(nullptr);
+  m.lay = lay, m.outdim = outdim;
+  m.blocks = r.blocks.data();
+  m.glu_w = r.glu_w.data();
+  m.glu_b = r.glu_b.data();
+  m.ln_fold = 0;                                  // the default stand-alone LayerNorm sequence
+  r.mel_start = static_cast<const int32_t*>(dp("mel_start"));
+  r.mel_count = static_cast<const int32_t*>(dp("mel_count"));
+  r.mel_weights = fl("mel_weights"), r.twiddle = fl("twiddle"), r.window = fl("window");
+}
+
+// some_session_open_devices, after its arguments are checked; `who` names the function in messages, and `listed` adds the
+// index of a refused device in the list.
+int open_session(const char* who, const char* path, const int* devices, int n, bool listed, some_session** out) {
   FILE* fp = fopen(path, "rb");
   SOME_REQUIRE(fp != nullptr, "%s: cannot open the model file", path);
   std::vector<uint8_t> file;
@@ -637,65 +781,71 @@ extern "C" int some_session_open(const char* path, int device, some_session** ou
   SOME_REQUIRE(dir.size() == specs.size(), "%s: %zu tensors, a model with lay %d / outdim %d has %zu", path, dir.size(), lay,
                outdim, specs.size());
 
-  // ---- the device (first CUDA call)
+  // ---- the devices (first CUDA call), every one checked before anything is allocated
   int n_dev = 0;
   cudaError_t e = cudaGetDeviceCount(&n_dev);
-  SOME_REQUIRE(e == cudaSuccess && device >= 0 && device < n_dev, "some_session_open: no CUDA device %d (%s)", device,
-               e == cudaSuccess ? "out of range" : cudaGetErrorString(e));
-  cudaDeviceProp prop;
-  SOME_CUDA(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties");
-  SOME_REQUIRE(prop.major == 9 && prop.minor == 0, "some_session_open: device %d (%s) is sm_%d%d; the kernels are built for sm_90a",
-               device, prop.name, prop.major, prop.minor);
+  for (int i = 0; i < n; ++i) {
+    const int device = devices[i];
+    char at[32] = "";
+    if (listed) snprintf(at, sizeof(at), "devices[%d]: ", i);
+    SOME_REQUIRE(e == cudaSuccess && device >= 0 && device < n_dev, "%s: %sno CUDA device %d (%s)", who, at, device,
+                 e == cudaSuccess ? "out of range" : cudaGetErrorString(e));
+    cudaDeviceProp prop;
+    SOME_CUDA(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties");
+    SOME_REQUIRE(prop.major == 9 && prop.minor == 0, "%s: %sdevice %d (%s) is sm_%d%d; the kernels are built for sm_90a", who,
+                 at, device, prop.name, prop.major, prop.minor);
+  }
   some_session* s = new some_session();
-  s->device = device;
-  DeviceScope scope(device);
+  s->device = devices[0];
   auto fail = [&](int rc) {
     destroy(s);
     return rc;
   };
-  if (scope.err != cudaSuccess) {
-    set_error("some_session_open: cudaSetDevice(%d): %s", device, cudaGetErrorString(scope.err));
-    return fail(-2);
+  const unsigned hw = std::thread::hardware_concurrency();
+  const int lanes = static_cast<int>(std::min(8u, std::max(2u, hw / 2)));
+  for (int i = 0; i < n; ++i) {
+    const int device = devices[i];
+    char at[32] = "";
+    if (listed) snprintf(at, sizeof(at), "devices[%d]: ", i);
+    s->reps.emplace_back(new Replica());
+    Replica& r = *s->reps.back();
+    r.device = device;
+    DeviceScope scope(device);
+    if (scope.err != cudaSuccess) {
+      set_error("%s: %scudaSetDevice(%d): %s", who, at, device, cudaGetErrorString(scope.err));
+      return fail(-2);
+    }
+    e = cudaStreamCreateWithFlags(&r.stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&r.copy_stream, cudaStreamNonBlocking);
+    for (cudaEvent_t& ev : r.ev)
+      if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+    // the weights go up on the replica's own (non-blocking) stream, which every later kernel of the replica runs on; the wait
+    // also keeps the host copy of the file alive until the copy has read it
+    if (e == cudaSuccess) e = cudaMalloc(&r.weights, std::max<uint64_t>(size - data_off, 1));
+    if (e == cudaSuccess) e = cudaMemcpyAsync(r.weights, f + data_off, size - data_off, cudaMemcpyHostToDevice, r.stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(r.stream);
+    if (e != cudaSuccess) {
+      set_error("%s: %suploading %s: %s", who, at, path, cudaGetErrorString(e));
+      return fail(-2);
+    }
+    bind_weights(r, specs, lay, outdim, [&](const std::string& name) -> const void* {
+      return static_cast<uint8_t*>(r.weights) + (dir.at(name).off - data_off);
+    });
+    r.model.b_cut = rd<float>(f + dir.at("b_cut").off);   // a host scalar of some_model
+    r.pool.reset(new WorkerPool(lanes));
   }
-  e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s->copy_stream, cudaStreamNonBlocking);
-  for (cudaEvent_t& ev : s->ev)
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-  // the weights go up on the session's own (non-blocking) stream, which every later kernel of the session runs on; the wait
-  // also keeps the host copy of the file alive until the copy has read it
-  if (e == cudaSuccess) e = cudaMalloc(&s->weights, std::max<uint64_t>(size - data_off, 1));
-  if (e == cudaSuccess) e = cudaMemcpyAsync(s->weights, f + data_off, size - data_off, cudaMemcpyHostToDevice, s->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
-  if (e != cudaSuccess) {
-    set_error("some_session_open: uploading %s: %s", path, cudaGetErrorString(e));
-    return fail(-2);
+  s->stream = s->reps[0]->stream;
+  s->pool = s->reps[0]->pool.get();
+  s->load.assign(n, {0, 0});
+  if (n > 1) {
+    DeviceScope scope(s->device);
+    e = cudaEventCreateWithFlags(&s->fed, cudaEventDisableTiming);
+    if (e != cudaSuccess) {
+      set_error("%s: cudaEventCreate: %s", who, cudaGetErrorString(e));
+      return fail(-2);
+    }
+    s->lanes.reset(new WorkerPool(n));
   }
-  uint8_t* base = static_cast<uint8_t*>(s->weights);
-  auto dp = [&](const std::string& name) -> const void* { return base + (dir.at(name).off - data_off); };
-  auto fl = [&](const std::string& n) { return static_cast<const float*>(dp(n)); };
-  some_model& m = s->model;
-  s->blocks.resize(2 * (lay + 1));            // value-initialised: the LayerNorm-folded fields stay null
-  for (const Spec& sp : specs) {
-    if (sp.field < 0) continue;
-    const void* p = dp(sp.name);
-    void* target = sp.block < 0 ? static_cast<void*>(&m) : static_cast<void*>(&s->blocks[sp.block]);
-    memcpy(static_cast<uint8_t*>(target) + sp.field, &p, sizeof(p));
-  }
-  for (int j = 0; j < 2 * lay; ++j) {
-    s->glu_w.push_back(static_cast<const uint16_t*>(dp("glu" + std::to_string(j) + ".w")));
-    s->glu_b.push_back(fl("glu" + std::to_string(j) + ".b"));
-  }
-  if (lay == 0) s->glu_w.push_back(nullptr), s->glu_b.push_back(nullptr);
-  m.lay = lay, m.outdim = outdim;
-  m.blocks = s->blocks.data();
-  m.glu_w = s->glu_w.data();
-  m.glu_b = s->glu_b.data();
-  const Entry& bc = dir.at("b_cut");
-  m.b_cut = rd<float>(f + bc.off);               // a host scalar of some_model
-  m.ln_fold = 0;                                  // the default stand-alone LayerNorm sequence
-  s->mel_start = static_cast<const int32_t*>(dp("mel_start"));
-  s->mel_count = static_cast<const int32_t*>(dp("mel_count"));
-  s->mel_weights = fl("mel_weights"), s->twiddle = fl("twiddle"), s->window = fl("window");
   const Entry& kt = dir.at("kaiser_best");
   s->kaiser.resize(kKaiserTaps);
   memcpy(s->kaiser.data(), f + kt.off, kt.bytes);
@@ -706,9 +856,65 @@ extern "C" int some_session_open(const char* path, int device, some_session** ou
   s->info.bias_corrected = bias_corrected;
   s->info.timestep = static_cast<double>(hop) / static_cast<double>(sr);    // base_infer.py:20
   s->vmin = rd<float>(f + 60), s->vmax = rd<float>(f + 64), s->deviation = rd<float>(f + 68), s->threshold = rd<float>(f + 72);
-  const unsigned hw = std::thread::hardware_concurrency();
-  s->pool.reset(new WorkerPool(static_cast<int>(std::min(8u, std::max(2u, hw / 2)))));
   *out = s;
+  return 0;
+}
+}  // namespace
+
+extern "C" int some_session_open(const char* path, int device, some_session** out) {
+  SOME_REQUIRE(path != nullptr && out != nullptr, "some_session_open: null pointer");
+  *out = nullptr;
+  return open_session("some_session_open", path, &device, 1, false, out);
+}
+
+extern "C" int some_session_open_devices(const char* path, const int* devices, int n, some_session** out) {
+  const char* who = "some_session_open_devices";
+  SOME_REQUIRE(path != nullptr && out != nullptr, "%s: null pointer", who);
+  *out = nullptr;
+  SOME_REQUIRE(devices != nullptr, "%s: the device list is NULL", who);
+  SOME_REQUIRE(n >= 1 && n <= kMaxReplicas, "%s: %d devices (1 to %d)", who, n, kMaxReplicas);
+  for (int i = 0; i < n; ++i) SOME_REQUIRE(devices[i] >= 0, "%s: devices[%d] is %d", who, i, devices[i]);
+  return open_session(who, path, devices, n, true, out);
+}
+
+extern "C" int some_session_get_devices(const some_session* s, int* devices, int capacity, int* n) {
+  SOME_REQUIRE(s != nullptr && n != nullptr && capacity >= 0 && (capacity == 0 || devices != nullptr),
+               "some_session_get_devices: bad arguments");
+  *n = static_cast<int>(s->reps.size());
+  for (int i = 0; i < std::min(capacity, *n); ++i) devices[i] = s->reps[i]->device;
+  return 0;
+}
+
+extern "C" int some_session_get_load(const some_session* s, int64_t* chunks, int64_t* frames, int capacity, int* n) {
+  SOME_REQUIRE(s != nullptr && n != nullptr && capacity >= 0 && (capacity == 0 || (chunks != nullptr && frames != nullptr)),
+               "some_session_get_load: bad arguments");
+  std::lock_guard<std::mutex> lock(s->mu);
+  *n = static_cast<int>(s->load.size());
+  for (int i = 0; i < std::min(capacity, *n); ++i) chunks[i] = s->load[i].first, frames[i] = s->load[i].second;
+  return 0;
+}
+
+extern "C" int some_shard_clips(const int64_t* lens, int n, int replicas, int32_t* owner) {
+  SOME_REQUIRE(n >= 0 && replicas >= 1 && (n == 0 || (lens != nullptr && owner != nullptr)), "some_shard_clips: bad arguments");
+  // clip_cost of some_b200/dist.py: T frames cost T * (dense + attention * T); 16384 * T is exact, so no rounding depends on
+  // how the compiler contracts the expression
+  std::vector<double> cost(n);
+  for (int i = 0; i < n; ++i) {
+    SOME_REQUIRE(lens[i] >= 0, "some_shard_clips: clip %d has a negative length", i);
+    const double t = static_cast<double>(1 + lens[i] / SOME_HOP);
+    cost[i] = t * (103.31e6 + 16384.0 * t);
+  }
+  std::vector<int> order(n);
+  for (int i = 0; i < n; ++i) order[i] = i;
+  std::sort(order.begin(), order.end(), [&](int a, int b) { return cost[a] != cost[b] ? cost[a] > cost[b] : a < b; });
+  std::vector<double> load(replicas, 0.0);
+  for (int i : order) {                   // longest first, to the least loaded replica (ties: the lowest)
+    int best = 0;
+    for (int r = 1; r < replicas; ++r)
+      if (load[r] < load[best]) best = r;
+    owner[i] = best;
+    load[best] += cost[i];
+  }
   return 0;
 }
 
@@ -763,15 +969,22 @@ int slice_ranges(const SliceShape& sh, const float* rms, const some_slicer_frame
 // Runs a call's work under the session's mutex, with the session's device current.  After a failure partway through, copies
 // and kernels may still be queued on the session's streams: it waits for them, so that the next call cannot rewrite staging
 // or device buffers they still use.  (The error message of the failure is kept.)
+// With several replicas, every replica's streams are waited for.  A call that completes records each replica's share of it.
 template <class F>
 int locked(some_session* s, F work) {
   std::lock_guard<std::mutex> lock(s->mu);
   DeviceScope scope(s->device);
   SOME_CUDA(scope.err, "cudaSetDevice");
+  for (std::unique_ptr<Replica>& r : s->reps) r->chunks = r->frames = 0;
   const int rc = work();
-  if (rc != 0) {
-    cudaStreamSynchronize(s->copy_stream);
-    cudaStreamSynchronize(s->stream);
+  for (size_t i = 0; i < s->reps.size(); ++i) {
+    Replica& r = *s->reps[i];
+    if (rc != 0) {
+      cudaStreamSynchronize(r.copy_stream);
+      cudaStreamSynchronize(r.stream);
+    } else {
+      s->load[i] = {r.chunks, r.frames};
+    }
   }
   return rc;
 }
@@ -899,7 +1112,7 @@ struct Recordings {
       it.c1 = static_cast<int>(starts.size());
     }
     const int B = static_cast<int>(starts.size());
-    if (B && run_batch(s, nullptr, base, starts.data(), lens.data(), B, &s->chunks)) return -1;
+    if (B && run_chunks(s, nullptr, base, starts.data(), lens.data(), B, &s->chunks)) return -1;
     for (const Item& it : items) take_chunks(s->chunks, it.c0, it.c1, begin.data(), lens.data(), it.out);
     return 0;
   }
@@ -928,7 +1141,7 @@ extern "C" int some_session_transcribe(some_session* s, const float* const* clip
     clear(out);
     return 0;
   }
-  return locked(s, [&] { return run_batch(s, clips, nullptr, nullptr, lens, B, out); });
+  return locked(s, [&] { return run_chunks(s, clips, nullptr, nullptr, lens, B, out); });
 }
 
 extern "C" int some_session_transcribe_sliced(some_session* s, const float* samples, long long n, int sample_rate,
@@ -1346,12 +1559,13 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
     std::vector<int64_t> starts(B);
     int64_t total = 0;
     for (int c = 0; c < B; ++c) starts[c] = total, total += (lens[c] + 3) & ~int64_t(3);
-    if (s->wave_d.ensure(4ull * total + 16, "the audio")) return -1;
-    float* wave = static_cast<float*>(s->wave_d.p);
+    DevBuf& chunks_d = s->reps[0]->wave_d;
+    if (chunks_d.ensure(4ull * total + 16, "the audio")) return -1;
+    float* wave = static_cast<float*>(chunks_d.p);
     for (int c = 0; c < B; ++c)
       if (lens[c])
         SOME_CUDA(cudaMemcpyAsync(wave + starts[c], src[c], 4ull * lens[c], cudaMemcpyDeviceToDevice, s->stream), "chunk copy");
-    if (run_batch(s, nullptr, wave, starts.data(), lens.data(), B, &s->chunks)) return -1;
+    if (run_chunks(s, nullptr, wave, starts.data(), lens.data(), B, &s->chunks)) return -1;
   }
   for (const StepItem& it : items) take_chunks(s->chunks, it.c0, it.c1, begin.data(), lens.data(), it.out);
   return 0;

@@ -14,12 +14,13 @@ from __future__ import annotations
 
 import collections.abc
 import functools
-import heapq
 from typing import Dict, List, Sequence
 
 import numpy as np
 import torch
 import torch.distributed as dist
+
+from .session import shard_clips as shard_owner
 
 HOP = 512
 # per-frame cost model (SURVEY.md §8d): 103.31 MFLOP dense + 2 * 8 blocks * 2 * T * 512 FLOP attention
@@ -33,15 +34,12 @@ def clip_cost(num_samples: int) -> float:
 
 @functools.lru_cache(maxsize=64)
 def _shard_clips(lengths: tuple, world: int):
-    cost = [clip_cost(n) for n in lengths]
-    order = sorted(range(len(lengths)), key=lambda i: (-cost[i], i))
-    heap = [(0.0, r) for r in range(world)]          # (load, rank): ties go to the lowest rank, as a linear scan would
+    # LPT over clip_cost, in order of (-cost, index), each clip to the least loaded rank (ties: the lowest): some_shard_clips,
+    # the rule a multi-device native session assigns its chunks by
     shards: List[List[int]] = [[] for _ in range(world)]
-    for i in order:
-        load, r = heapq.heappop(heap)
+    for i, r in enumerate(shard_owner(lengths, world)):
         shards[r].append(i)
-        heapq.heappush(heap, (load + cost[i], r))
-    return tuple(tuple(sorted(s)) for s in shards)
+    return tuple(tuple(s) for s in shards)
 
 
 def shard_clips(lengths: Sequence[int], world: int) -> List[List[int]]:

@@ -10,7 +10,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import weakref
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -59,15 +59,33 @@ class Notes:
         return ranges, out
 
 
+def shard_clips(lengths: Sequence[int], replicas: int) -> List[int]:
+    """some_shard_clips: the replica (or rank) of every clip, by the longest-processing-time rule a multi-device session and
+    some_b200.dist use."""
+    lib = _lib.load()
+    lens = np.ascontiguousarray(np.asarray(lengths, dtype=np.int64).reshape(-1))
+    owner = np.zeros(max(lens.shape[0], 1), dtype=np.int32)
+    _lib.check(lib.some_shard_clips(lens.ctypes.data, int(lens.shape[0]), int(replicas), owner.ctypes.data), 'some_shard_clips')
+    return owner[:lens.shape[0]].tolist()
+
+
 class Session:
-    """some_session_open(path, device) ... some_session_close."""
+    """some_session_open(path, device) ... some_session_close.  `device` is one device index, or a sequence of them
+    (some_session_open_devices): a replica of the model on each, with the chunks of every call spread over them and the same
+    results as a session on the first."""
 
     handle = None
 
-    def __init__(self, path, device: int = 0):
+    def __init__(self, path, device: Union[int, Sequence[int]] = 0):
         self.lib = _lib.load()
         h = C.c_void_p()
-        _lib.check(self.lib.some_session_open(os.fsencode(os.fspath(path)), int(device), C.byref(h)), 'some_session_open')
+        if isinstance(device, (int, np.integer)):
+            _lib.check(self.lib.some_session_open(os.fsencode(os.fspath(path)), int(device), C.byref(h)), 'some_session_open')
+        else:
+            devs = [int(d) for d in device]
+            arr = (C.c_int * max(len(devs), 1))(*devs)
+            _lib.check(self.lib.some_session_open_devices(os.fsencode(os.fspath(path)), arr, len(devs), C.byref(h)),
+                       'some_session_open_devices')
         self.handle = h
         self._streams = weakref.WeakSet()      # closed before the session: a stream uses the session's device state
         info = _lib.SessionInfo()
@@ -85,6 +103,23 @@ class Session:
 
     def __del__(self):
         self.close()
+
+    @property
+    def devices(self) -> List[int]:
+        """some_session_get_devices: the device of every replica, in order."""
+        n = C.c_int()
+        _lib.check(self.lib.some_session_get_devices(self.handle, None, 0, C.byref(n)), 'some_session_get_devices')
+        arr = (C.c_int * max(n.value, 1))()
+        _lib.check(self.lib.some_session_get_devices(self.handle, arr, n.value, C.byref(n)), 'some_session_get_devices')
+        return list(arr[:n.value])
+
+    def load(self) -> List[Tuple[int, int]]:
+        """some_session_get_load: (chunks, frames) each replica ran in the session's last completed call."""
+        n = C.c_int()
+        _lib.check(self.lib.some_session_get_load(self.handle, None, None, 0, C.byref(n)), 'some_session_get_load')
+        chunks, frames = (C.c_int64 * max(n.value, 1))(), (C.c_int64 * max(n.value, 1))()
+        _lib.check(self.lib.some_session_get_load(self.handle, chunks, frames, n.value, C.byref(n)), 'some_session_get_load')
+        return list(zip(chunks[:n.value], frames[:n.value]))
 
     def transcribe(self, waveforms: Sequence[np.ndarray], notes: Optional[Notes] = None) -> List[Dict[str, np.ndarray]]:
         """some_session_transcribe: mono float32 clips at the model's rate -> one dict per clip, in input order."""
