@@ -683,7 +683,8 @@ int some_forward_f32(const some_model_f32* model, const some_workspace_f32* ws, 
  * (Engine.calibrate), into one self-contained model file (format: INTEGRATION.md "Deploying without Python"); a session opens
  * that file and transcribes recordings with the kernels above, enqueued in the order of some_b200/engine.py, so its notes are
  * bit-identical to plugin.infer() / Engine.infer_sliced.  Host memory in, host memory out; the session owns its streams and
- * buffers, and calls on one session are serialised on a mutex (several threads may share it, each with its own result).
+ * buffers.  Several threads may share a session, each with its own result: calls that queue while a step runs are run
+ * together as one GPU step (see "Calls from several threads" below).
  *
  * some_session_open       reads and validates the whole file before any CUDA call (magic, format version, ABI, directory
  *                         bounds, every tensor present with the shape implied by lay / outdim, file size); refuses a device
@@ -735,9 +736,39 @@ int some_session_open(const char* path, int device, some_session** out);
 int some_session_open_devices(const char* path, const int* devices, int n, some_session** out);
 /* The session's devices in replica order: *n = their count, the first min(capacity, *n) written to devices. */
 int some_session_get_devices(const some_session* s, int* devices, int capacity, int* n);
-/* For each replica, the chunks and frames (1 + samples / 512 each) it ran in the session's last completed call: *n = the
- * replica count, the first min(capacity, *n) written. */
+/* For each replica, the chunks and frames (1 + samples / 512 each) it ran in the session's last completed step (with one
+ * calling thread: its last completed call): *n = the replica count, the first min(capacity, *n) written. */
 int some_session_get_load(const some_session* s, int64_t* chunks, int64_t* frames, int capacity, int* n);
+/* ---- Calls from several threads.  Every call that reaches the GPU (every session and stream call below, after the checks it
+ * makes before any GPU work) becomes a request in a first-in, first-out queue of the session.  If no step is running, the
+ * calling thread runs the next step itself: the oldest request and every later queued request that may join it, in arrival
+ * order, as one GPU step; it hands each request its result, and repeats while its own request has not run.  Meanwhile the
+ * other callers wait for their own request.  There is no waiting window: a lone caller, or a single-threaded host, runs the
+ * same steps as before, and calls merge only when they queue behind a running step.
+ *   Which requests may share a step: clip calls (some_session_transcribe) with clip calls; sliced and encoded calls together
+ * (one recordings step: their recordings decoded, resampled, cut and transcribed as one); PCM stream calls together (push,
+ * finish, push_many: one stream step); encoded stream calls together (push_bytes*, finish of an encoded stream).  Calls of
+ * different kinds run as consecutive steps.  Never in one step: two requests that touch the same some_stream or the same
+ * some_notes (the later one waits for a later step, so each stream's calls apply in arrival order), or requests whose threads
+ * have different some_set_pdl settings (the step runs with its requests' setting).  A request joins only while the step's
+ * model-rate samples stay within max(the oldest request's own, SOME_SESSION_STEP_SAMPLES), so a merged step holds no more
+ * device memory than its largest request alone or a step of that size.  The samples are known before any GPU work: clips,
+ * the sliced and encoded recordings at the model's rate, a PCM stream push's samples at the model's rate, and an encoded
+ * stream push's bytes.  An encoded call with a FLAC file that states no length (STREAMINFO total 0) takes no joiners and joins
+ * no step.  A request that cannot join stays the oldest, and the next step is built around it.
+ *   Results: a step of several requests gives each request exactly what it gives alone (a chunk's notes do not depend on the
+ * rest of its batch).  An encoded call refused after the scan (a corrupt FLAC file) fails alone with the message and item
+ * index it gives alone and no out[i] written, and a refused encoded stream fails only its own call; the other requests of the
+ * step run on.  Each caller's some_last_error() is set on its own thread.  A device error fails every request of its step
+ * with the device's message, and the session stays usable. */
+#define SOME_SESSION_STEP_SAMPLES 84672000LL /* 64 recordings x 30 s at 44.1 kHz: about 4.5 GB of activations */
+typedef struct {
+  int64_t calls;     /* requests queued since open */
+  int64_t steps;     /* steps run since open */
+  int64_t max_calls; /* the most requests one step has held */
+  int64_t queued;    /* requests waiting at this moment (not counting those of a step in progress) */
+} some_session_stats;
+int some_session_get_stats(const some_session* s, some_session_stats* stats);
 /* Host only, no CUDA call: owner[i] = the replica of clip i of n.  Longest processing time first: clips in order of
  * (-cost, index), cost = T * (103.31e6 + 16384 * T) with T = 1 + lens[i] / 512, each to the least loaded replica (ties: the
  * lowest).  The sessions above and some_b200.dist.shard_clips assign clips with it. */
@@ -773,7 +804,8 @@ int some_notes_midi(const some_notes* n, int sample_rate, double timestep, doubl
  * empty item; two entries sharing one some_notes; anything some_audio_info refuses; mono down-mix of more than 128 channels; a
  * rate pair the resampler does not support; a recording too short to resample.  A corrupt FLAC stream is refused after the
  * scan with its index and some_flac_chain's message, and no out[i] is written.  After a device error the session stays
- * usable.  The call takes the session's mutex once; count == 0 does nothing.  params NULL: Slicer(sr, max_sil_kept=1000). */
+ * usable.  The call is one request (see "Calls from several threads"); count == 0 does nothing.  params NULL: Slicer(sr,
+ * max_sil_kept=1000). */
 typedef struct {
   const void* data;
   long long n_bytes;
@@ -831,8 +863,8 @@ int some_slicer_stream_destroy(some_slicer_stream* st);
  * chunk plus 2 max_sil_kept frames and the RMS window (during a long leading silence: the first and the last max_sil_kept
  * frames and the RMS window), plus the push in progress, however long the recording or its silences; until more than
  * min_length hops are fixed (the recording may still prove to be one chunk) it holds everything so far.
- *   Any number of streams may share a session, from different threads: each GPU step takes the session's mutex.  One stream
- * is used by one thread at a time.  sample_rate: any integer rate (params NULL: Slicer(sr, max_sil_kept=1000)).  At finish, a
+ *   Any number of streams may share a session, from different threads: pushes that queue behind a running step are run as
+ * one step (see "Calls from several threads").  One stream is used by one thread at a time.  sample_rate: any integer rate (params NULL: Slicer(sr, max_sil_kept=1000)).  At finish, a
  * recording too short to resample is refused as resampy refuses it; an empty stream finishes like transcribe_sliced on zero
  * samples.  No push after finish.  Close a session's streams before the session: a stream uses its session's device, streams
  * and buffers. */
@@ -859,8 +891,8 @@ int some_stream_close(some_stream* st);
  * two entries share one some_notes; a resampling stream is to finish with too few input samples to resample.  count == 0
  * does nothing.  A failure after that (a device error) is reported like one of some_stream_push; the session stays usable,
  * but on every stream of the failed call only some_stream_get_info and some_stream_close remain defined.
- *   The call takes the session's mutex once.  Threads may call it on disjoint sets of streams of one session, mixed with
- * single pushes on other streams; one stream is used by one thread at a time. */
+ *   The call is one request (see "Calls from several threads").  Threads may call it on disjoint sets of streams of one
+ * session, mixed with single pushes on other streams; one stream is used by one thread at a time. */
 int some_stream_push_many(some_stream* const* streams, const float* const* samples, const long long* n, const int* finish,
                           int count, some_notes* const* out);
 /* Encoded streams: a WAV, FLAC or AIFF file pushed as its bytes arrive (a recorder or encoder writing to a pipe, an upload),

@@ -122,6 +122,10 @@ class SessionInfo(C.Structure):
                 ('bias_corrected', C.c_int), ('timestep', C.c_double)]
 
 
+class SessionStats(C.Structure):
+    _fields_ = [('calls', C.c_int64), ('steps', C.c_int64), ('max_calls', C.c_int64), ('queued', C.c_int64)]
+
+
 class SlicerParams(C.Structure):
     _fields_ = [('threshold_db', C.c_double), ('min_length_ms', C.c_double), ('min_interval_ms', C.c_double),
                 ('hop_size_ms', C.c_double), ('max_sil_kept_ms', C.c_double)]
@@ -248,6 +252,7 @@ EXPORTS = {
     'some_session_open_devices': (C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.c_int, C.POINTER(_vp)]),
     'some_session_get_devices': (C.c_int, [_vp, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]),
     'some_session_get_load': (C.c_int, [_vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int, C.POINTER(C.c_int)]),
+    'some_session_get_stats': (C.c_int, [_vp, C.POINTER(SessionStats)]),
     'some_shard_clips': (C.c_int, [_vp, C.c_int, C.c_int, _vp]),
     'some_session_get_info': (C.c_int, [_vp, C.POINTER(SessionInfo)]),
     'some_session_transcribe': (C.c_int, [_vp, _vp, _vp, C.c_int, _vp]),

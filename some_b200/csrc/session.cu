@@ -8,7 +8,9 @@
 // two kernels over the windows of its streams.  The encoded files call and the encoded stream step share the stage in front
 // of it (Decode: one upload of the audio bytes, one FLAC scan, one PCM and one FLAC decode).  A session opened on several
 // devices holds one replica of the model per device: the front end runs on replica 0, and run_chunks spreads the chunks of
-// each call over the replicas, each on its own thread, and gathers their notes in chunk order.
+// each call over the replicas, each on its own thread, and gathers their notes in chunk order.  Every call is a request in
+// the session's queue (submit, at the end): calls of one kind that queue while a step runs share the next step, whose back
+// end (run_chunks, Recordings, streams_step, bytes_step) takes the items of all of them.
 //
 // The model file (little-endian; INTEGRATION.md "Deploying without Python" has the table):
 //   header     128 bytes: magic "SOMEB200", format version, ABI number, file size, directory offset, tensor count, the scalars
@@ -26,10 +28,12 @@
 
 #include <algorithm>
 #include <condition_variable>
+#include <deque>
 #include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
+#include <set>
 #include <string>
 #include <thread>
 #include <type_traits>
@@ -197,7 +201,7 @@ struct Chunk {
 
 // A fixed set of worker threads for the host copies (staging of clips and recordings into pinned memory), kept for the
 // session's lifetime like Engine._pool, so that no call creates threads.  run(n, fn) runs fn(0 .. n-1), lane 0 on the calling
-// thread, and returns when every lane has finished; calls are serialised by the session's mutex.
+// thread, and returns when every lane has finished; one step of the session runs at a time.
 class WorkerPool {
  public:
   explicit WorkerPool(int n) : size_(std::max(1, n)) {
@@ -270,6 +274,7 @@ struct some_notes {
 };
 
 namespace {
+struct Request;
 // One copy of the model on one device, and what it needs to run a batch of chunks there: a session holds one replica per
 // device it was opened on (a device listed twice holds two).  Replica 0 also runs the front end of every call.
 struct Replica {
@@ -295,7 +300,13 @@ struct Replica {
 }  // namespace
 
 struct some_session {
+  // the calls waiting for a step (oldest first), whether a thread is running one, and the totals of some_session_get_stats,
+  // all under mu; a caller waits on `done` until its own call has run
   mutable std::mutex mu;
+  std::condition_variable done;
+  std::deque<Request*> queue;
+  bool running = false;
+  some_session_stats stats{};
   some_session_info info{};
   float vmin = 0.f, vmax = 0.f, deviation = 1.f, threshold = 0.1f;
   std::vector<double> kaiser;             // host copy of the float64 table (scaled per rate pair on upload)
@@ -323,7 +334,7 @@ struct some_session {
   // replica 0's stream once the front end has written the chunks the others copy
   std::unique_ptr<WorkerPool> lanes;
   cudaEvent_t fed = nullptr;
-  std::vector<std::pair<int64_t, int64_t>> load;   // each replica's chunks and frames in the last completed call
+  std::vector<std::pair<int64_t, int64_t>> load;   // each replica's chunks and frames in the last completed step
 };
 
 namespace {
@@ -622,17 +633,28 @@ int run_chunks(some_session* s, const float* const* host, const float* resident,
   return 0;
 }
 
-// Uploads n floats of host memory to `dst` through the pinned staging buffer: in pieces of 16 MB, each copied into pinned
-// memory by the session's threads (256 KB per thread and turn) and then sent while the next piece is copied.
-int upload_staged(some_session* s, float* dst, const float* src, int64_t n) {
+// Host floats to upload: n floats at src go to dst.
+struct Staged {
+  float* dst;
+  const float* src;
+  int64_t n;
+};
+// Uploads host recordings through the pinned staging buffer, each at its own place there: in pieces of 16 MB, each copied
+// into pinned memory by the session's threads (256 KB per thread and turn) and then sent while the next piece is copied.
+int upload_staged(some_session* s, const std::vector<Staged>& recs) {
   constexpr int64_t kPiece = int64_t(1) << 22;
+  int64_t total = 0;
+  for (const Staged& r : recs) total += (r.n + 3) & ~int64_t(3);
   PinBuf& staging = s->reps[0]->wave_h;
-  if (staging.ensure(4ull * n + 16, "the staged audio")) return -1;
+  if (staging.ensure(4ull * total + 16, "the staged audio")) return -1;
   float* pin = static_cast<float*>(staging.p);
-  for (int64_t a = 0; a < n; a += kPiece) {
-    const int64_t len = std::min(kPiece, n - a);
-    copy_to_pinned(*s->pool, {{pin + a, src + a, 4ull * len}}, size_t(1) << 18);
-    SOME_CUDA(cudaMemcpyAsync(dst + a, pin + a, 4ull * len, cudaMemcpyHostToDevice, s->stream), "audio upload");
+  for (const Staged& r : recs) {
+    for (int64_t a = 0; a < r.n; a += kPiece) {
+      const int64_t len = std::min(kPiece, r.n - a);
+      copy_to_pinned(*s->pool, {{pin + a, r.src + a, 4ull * len}}, size_t(1) << 18);
+      SOME_CUDA(cudaMemcpyAsync(r.dst + a, pin + a, 4ull * len, cudaMemcpyHostToDevice, s->stream), "audio upload");
+    }
+    pin += (r.n + 3) & ~int64_t(3);
   }
   return 0;
 }
@@ -894,6 +916,14 @@ extern "C" int some_session_get_load(const some_session* s, int64_t* chunks, int
   return 0;
 }
 
+extern "C" int some_session_get_stats(const some_session* s, some_session_stats* stats) {
+  SOME_REQUIRE(s != nullptr && stats != nullptr, "some_session_get_stats: null pointer");
+  std::lock_guard<std::mutex> lock(s->mu);
+  *stats = s->stats;
+  stats->queued = static_cast<int64_t>(s->queue.size());
+  return 0;
+}
+
 extern "C" int some_shard_clips(const int64_t* lens, int n, int replicas, int32_t* owner) {
   SOME_REQUIRE(n >= 0 && replicas >= 1 && (n == 0 || (lens != nullptr && owner != nullptr)), "some_shard_clips: bad arguments");
   // clip_cost of some_b200/dist.py: T frames cost T * (dense + attention * T); 16384 * T is exact, so no rounding depends on
@@ -966,28 +996,45 @@ int slice_ranges(const SliceShape& sh, const float* rms, const some_slicer_frame
   return 0;
 }
 
-// Runs a call's work under the session's mutex, with the session's device current.  After a failure partway through, copies
-// and kernels may still be queued on the session's streams: it waits for them, so that the next call cannot rewrite staging
-// or device buffers they still use.  (The error message of the failure is kept.)
-// With several replicas, every replica's streams are waited for.  A call that completes records each replica's share of it.
-template <class F>
-int locked(some_session* s, F work) {
-  std::lock_guard<std::mutex> lock(s->mu);
-  DeviceScope scope(s->device);
-  SOME_CUDA(scope.err, "cudaSetDevice");
-  for (std::unique_ptr<Replica>& r : s->reps) r->chunks = r->frames = 0;
-  const int rc = work();
-  for (size_t i = 0; i < s->reps.size(); ++i) {
-    Replica& r = *s->reps[i];
-    if (rc != 0) {
-      cudaStreamSynchronize(r.copy_stream);
-      cudaStreamSynchronize(r.stream);
-    } else {
-      s->load[i] = {r.chunks, r.frames};
-    }
+// A recording of a sliced or an encoded call: host floats (`host`, the sliced call) or a file's bytes (the encoded call).
+struct RecItem {
+  const float* host = nullptr;
+  const uint8_t* bytes = nullptr;
+  some_audio_meta m{};        // of the file; the sliced call sets only its rate
+  int64_t n = 0;              // samples at its rate (FLAC without a stated length: known after the chain)
+  SliceShape sh;
+  some_notes* out = nullptr;
+  int64_t up = 0;             // the audio bytes' offset in the upload
+};
+struct StepItem;
+struct ByteItem;
+
+// One public call, queued for a step (see submit): what it asks for, what it touches and, once its step has run, its result.
+struct Request {
+  enum Kind { CLIPS, RECORDINGS, STREAMS, BYTES } kind;
+  int pdl = 0;                            // the caller's some_set_pdl setting
+  int64_t samples = 0;                    // the model-rate samples it adds to a step (streams: see some_session_stats)
+  bool sized = true;                      // false: its size is not known before the GPU work (it takes no joiners)
+  std::vector<const void*> touches;       // its streams and its some_notes
+  // the work, by kind: CLIPS
+  const float* const* clips = nullptr;
+  const int64_t* lens = nullptr;
+  int B = 0;
+  some_notes* out = nullptr;
+  // RECORDINGS (the sliced call: one host item) with the slicer's frames, STREAMS, BYTES
+  std::vector<RecItem>* recs = nullptr;
+  some_slicer_frames sl{};
+  std::vector<StepItem>* items = nullptr;
+  std::vector<ByteItem>* bytes = nullptr;
+  // the result
+  int rc = 0;
+  std::string err;
+  bool done = false;
+  void fail(int code, const std::string& message) {
+    if (rc == 0) rc = code, err = message;
   }
-  return rc;
-}
+};
+int submit(some_session* s, Request& rq);
 
 // The resampling table for sample_rate -> the model's rate: uploaded on the session's stream (in front of the resampling
 // launches that read it) the first time its ratio is used, and kept.  Upsampling reads the table as it is; resampy scales it
@@ -1031,19 +1078,21 @@ struct Upload {
 
 constexpr int64_t align4(int64_t n) { return (n + 3) & ~int64_t(3); }
 
-// Recordings in the session's recording buffer, each at its own rate, made into chunks and notes together (the sliced and
-// the encoded calls; a caller writes the recordings there and may add its own regions to the step's upload and its own
-// launches and downloads in front of the synchronise):
+// Recordings in the session's recording buffer, each at its own rate and with its own slicer frames, made into chunks and
+// notes together (the sliced and the encoded calls of a step; the step writes the recordings there and may add its own regions
+// to the upload and its own launches and downloads in front of the synchronise):
 //   place   where each recording, its model-rate samples and its RMS frames go; one resampling window per recording at
 //           another rate and one RMS window per recording that is cut, packed into regions added to the upload after the
 //           caller's own, and the upload reserved (the caller fills its regions after this);
 //   launch  after the upload is sent and the recordings are written: one resampling launch, one RMS launch, the RMS download;
-//   finish  after the caller's synchronise: each recording's cuts, one batch over all chunks, each recording's notes.
+//   finish  after the caller's synchronise: each recording's cuts, one batch over all chunks, each recording's notes (a
+//           recording whose `out` has been set to NULL since place, its call refused, is left out).
 struct Recordings {
   struct Item {
     int rate;
     int64_t n;                // samples at `rate`
     SliceShape sh;
+    const some_slicer_frames* sl;
     some_notes* out;
     int64_t x = 0, y = 0;     // its samples at `rate` and at the model's rate in the buffer (the same at the model's rate)
     int64_t rms0 = 0;         // its first RMS frame
@@ -1055,7 +1104,7 @@ struct Recordings {
   int kr = 0, km = 0;
   size_t rs_off = 0, rm_off = 0;
 
-  int place(some_session* s, const some_slicer_frames& sl, Upload& up) {
+  int place(some_session* s, Upload& up) {
     const int sr = s->info.sample_rate;
     int64_t total = 0;
     for (Item& it : items) {
@@ -1078,8 +1127,8 @@ struct Recordings {
         rs.push_back({base + it.x, 0, it.n, 1, base + it.y, 0, 0, it.sh.n_out, it.rate, sr, table, kKaiserTaps});
       }
       if (it.sh.frames)
-        rm.push_back({base + it.y, 0, it.sh.n_out, it.sh.n_out, sl.win_size, sl.hop_size, static_cast<float*>(s->rms_d.p) + it.rms0,
-                      0, it.sh.frames});
+        rm.push_back({base + it.y, 0, it.sh.n_out, it.sh.n_out, it.sl->win_size, it.sl->hop_size,
+                      static_cast<float*>(s->rms_d.p) + it.rms0, 0, it.sh.frames});
     }
     kr = static_cast<int>(rs.size()), km = static_cast<int>(rm.size());
     if (kr) rs_off = up.add(static_cast<size_t>(some_resample_windows_bytes(kr)));
@@ -1099,10 +1148,11 @@ struct Recordings {
     return 0;
   }
 
-  int finish(some_session* s, const some_slicer_frames& sl) {
+  int finish(some_session* s) {
     std::vector<int64_t> starts, lens, begin, ranges;
     for (Item& it : items) {
-      if (slice_ranges(it.sh, static_cast<const float*>(s->rms_h.p) + it.rms0, sl, ranges)) return -1;
+      if (!it.out) continue;
+      if (slice_ranges(it.sh, static_cast<const float*>(s->rms_h.p) + it.rms0, *it.sl, ranges)) return -1;
       it.c0 = static_cast<int>(starts.size());
       for (size_t r = 0; r + 1 < ranges.size(); r += 2) {
         begin.push_back(ranges[r]);
@@ -1113,24 +1163,12 @@ struct Recordings {
     }
     const int B = static_cast<int>(starts.size());
     if (B && run_chunks(s, nullptr, base, starts.data(), lens.data(), B, &s->chunks)) return -1;
-    for (const Item& it : items) take_chunks(s->chunks, it.c0, it.c1, begin.data(), lens.data(), it.out);
+    for (const Item& it : items)
+      if (it.out) take_chunks(s->chunks, it.c0, it.c1, begin.data(), lens.data(), it.out);
     return 0;
   }
 };
 
-// One recording: uploaded through pinned memory into the recording buffer, then the one-recording case of Recordings, with
-// a synchronise before the batch only when the recording is cut.
-int transcribe_sliced(some_session* s, const float* samples, int64_t n, int sample_rate, const SliceShape& sh,
-                      const some_slicer_frames& sl, some_notes* out) {
-  Recordings rec;
-  rec.items.push_back({sample_rate, n, sh, out});
-  Upload up{s};
-  if (rec.place(s, sl, up) || upload_staged(s, rec.base + rec.items[0].x, samples, n) || up.send("descriptor upload") ||
-      rec.launch(s, up))
-    return -1;
-  if (sh.frames) SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
-  return rec.finish(s, sl);
-}
 }  // namespace
 
 extern "C" int some_session_transcribe(some_session* s, const float* const* clips, const int64_t* lens, int B, some_notes* out) {
@@ -1141,7 +1179,11 @@ extern "C" int some_session_transcribe(some_session* s, const float* const* clip
     clear(out);
     return 0;
   }
-  return locked(s, [&] { return run_chunks(s, clips, nullptr, nullptr, lens, B, out); });
+  Request rq{Request::CLIPS};
+  rq.clips = clips, rq.lens = lens, rq.B = B, rq.out = out;
+  for (int i = 0; i < B; ++i) rq.samples += lens[i];
+  rq.touches = {out};
+  return submit(s, rq);
 }
 
 extern "C" int some_session_transcribe_sliced(some_session* s, const float* samples, long long n, int sample_rate,
@@ -1151,9 +1193,13 @@ extern "C" int some_session_transcribe_sliced(some_session* s, const float* samp
   const int sr = s->info.sample_rate;
   some_slicer_frames sl;
   if (some_slicer_derive(sr, params, &sl)) return -1;
-  SliceShape sh;
-  if (slice_shape(n, sample_rate, sr, sl, "some_session_transcribe_sliced", &sh)) return -1;
-  return locked(s, [&] { return transcribe_sliced(s, samples, n, sample_rate, sh, sl, out); });
+  std::vector<RecItem> recs(1);
+  RecItem& it = recs[0];
+  if (slice_shape(n, sample_rate, sr, sl, "some_session_transcribe_sliced", &it.sh)) return -1;
+  it.host = samples, it.m.rate = sample_rate, it.n = n, it.out = out;
+  Request rq{Request::RECORDINGS};
+  rq.recs = &recs, rq.sl = sl, rq.samples = it.sh.n_out, rq.touches = {out};
+  return submit(s, rq);
 }
 
 // ---------------------------------------------------------------------------------------------------- streams
@@ -1241,6 +1287,7 @@ struct StepItem {
   int64_t rms0 = 0, nf = 0;     // its new RMS frames in the session's RMS buffer
   int c0 = 0, c1 = 0;           // its chunks in the step's batch
   bool dropped = false;         // its samples failed to decode: no slicer decisions, no chunks
+  std::string why;              // and the decoder's message
 };
 
 // Whether a container's samples are PCM that some_pcm_decode reads (WAV, AIFF) rather than FLAC frames: the one place the
@@ -1273,7 +1320,7 @@ struct ByteWindow {
 //           word in the caller's descriptor upload;
 //   fill    after the caller has placed each item's samples: the descriptors, with those places;
 //   launch  after the descriptor upload is sent: one some_pcm_decode, one FLAC decode, the status download;
-//   check   after the synchronise: the item whose frame failed to decode, if one did, with the error set.
+//   check   after the synchronise: every item whose frame failed to decode, each with its message.
 struct Decode {
   const uint8_t* bytes_d = nullptr;              // the bytes upload
   int64_t flac_bytes = 0;                        // its FLAC windows: [0, flac_bytes), described by streams_d[0 .. nf)
@@ -1391,19 +1438,39 @@ struct Decode {
     SOME_CUDA(cudaMemcpyAsync(up.h(status_off), status_d, 2 * sizeof(int), cudaMemcpyDeviceToHost, s->stream), "status download");
     return 0;
   }
-  // The caller's item whose frame failed to decode, with the error set (the frame's byte offset in its file), or -1.
-  int check(const Upload& up) const {
-    const int* status = reinterpret_cast<const int*>(up.h(status_off));
-    if (chain.empty() || status[0] == 0) return -1;
-    size_t r = 0;
-    while (r + 1 < flac_of.size() && first[r + 1] <= status[1]) ++r;
-    set_error("FLAC frame at byte offset %lld failed to decode (status %d)",
-              static_cast<long long>(frames_h[chain[status[1]]].pos - base[r]), status[0]);
-    return flac_of[r];
+  // The caller's items whose frame failed to decode, each with the message of its first such frame (the frame's byte offset
+  // in its file), in window order.  The status word names the first failing frame of a launch, so after each failure the
+  // frames of the later windows are decoded again, with a fresh status word, until none fails (into the same places, with
+  // the same values: only the status is new).
+  int check(some_session* s, const Upload& up, std::vector<std::pair<int, std::string>>& failed) const {
+    int* status = reinterpret_cast<int*>(up.h(status_off));
+    int* status_d = reinterpret_cast<int*>(up.d(status_off));
+    int64_t k = 0;                               // the launch checked covers chain[k ..)
+    while (!chain.empty() && status[0] != 0) {
+      const int64_t j = k + status[1];
+      size_t r = 0;
+      while (r + 1 < flac_of.size() && first[r + 1] <= j) ++r;
+      char msg[160];
+      snprintf(msg, sizeof(msg), "FLAC frame at byte offset %lld failed to decode (status %d)",
+               static_cast<long long>(frames_h[chain[j]].pos - base[r]), status[0]);
+      failed.push_back({flac_of[r], msg});
+      k = first[r + 1];
+      if (k >= static_cast<int64_t>(chain.size())) break;
+      status[0] = 0, status[1] = INT_MAX;
+      SOME_CUDA(cudaMemcpyAsync(status_d, status, 2 * sizeof(int), cudaMemcpyHostToDevice, s->stream), "status upload");
+      if (flac_decode_chain(bytes_d, streams_d, frames_d, reinterpret_cast<const int32_t*>(up.d(chain_off)) + k,
+                            reinterpret_cast<const int64_t*>(up.d(soff_off)) + k, reinterpret_cast<const int64_t*>(up.d(ooff_off)) + k,
+                            static_cast<int>(chain.size() - k), static_cast<int32_t*>(s->flac_scratch_d.p), out, 1, status_d,
+                            status_d + 1, s->stream))
+        return -1;
+      SOME_CUDA(cudaMemcpyAsync(status, status_d, 2 * sizeof(int), cudaMemcpyDeviceToHost, s->stream), "status download");
+      SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+    }
+    return 0;
   }
 };
 
-// One step of any number of streams of one session, under the session's mutex.  Each stream does what a push of its samples
+// One step of any number of streams of one session (one step runs at a time).  Each stream does what a push of its samples
 // (and a finish, when `final`) does alone, but the GPU work is made once for all of them:
 //   1. per stream on the host: what to keep, the samples set apart during a leading silence, the window plans and room in the
 //      stream's buffers;
@@ -1520,8 +1587,9 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
     SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames, cudaMemcpyDeviceToHost, s->stream), "RMS download");
   SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");   // also frees the upload buffer for the next step
   if (dec) {
-    const int j = dec->check(up);
-    if (j >= 0) items[j].dropped = true;
+    std::vector<std::pair<int, std::string>> failed;
+    if (dec->check(s, up, failed)) return -1;
+    for (const auto& f : failed) items[f.first].dropped = true, items[f.first].why = f.second;
   }
 
   // the slicer's decisions, and where each chunk that became final lies
@@ -1571,10 +1639,16 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
   return 0;
 }
 
-// A step of one stream (some_stream_push, some_stream_finish).
-int stream_call(some_stream* st, const float* samples, int64_t n, bool final, some_notes* out) {
-  std::vector<StepItem> items{StepItem{st, samples, n, final, out}};
-  return locked(st->s, [&] { return streams_step(st->s, items); });
+// Queues PCM stream items as one call (some_stream_push, some_stream_finish, some_stream_push_many).
+int stream_call(some_session* s, std::vector<StepItem>& items) {
+  Request rq{Request::STREAMS};
+  rq.items = &items;
+  for (const StepItem& it : items) {
+    const some_stream* st = it.st;
+    rq.samples += st->resample ? (it.n * s->info.sample_rate + st->rate - 1) / st->rate : it.n;
+    rq.touches.push_back(st), rq.touches.push_back(it.out);
+  }
+  return submit(s, rq);
 }
 
 // One encoded stream's part of a step: its new bytes, whether the file ends there, and where its chunks go.
@@ -1585,13 +1659,15 @@ struct ByteItem {
   bool final;
   some_notes* out;
   int index;                    // in a many-call (-1: a single call)
+  const char* who;              // the call, for its messages
+  std::string* refusal;         // its call's first refusal
   bool live = true;             // false once refused
   int64_t up = 0, win = 0;      // its window in the bytes upload: the pending bytes that go up
   int64_t samples = 0;          // the samples it decodes in this step
   int fi = -1;                  // FLAC: its window in the step's decode
 };
 
-// A step of encoded streams (some_stream_push_bytes*, some_stream_finish), under the session's mutex:
+// A step of encoded streams (some_stream_push_bytes*, some_stream_finish):
 //   1. on the host, each stream's walk consumes its bytes; their audio joins the stream's pending bytes;
 //   2. the encoded-input stage (Decode) uploads the FLAC windows (the pending bytes from each stream's first unchained
 //      frame) and the whole WAV or AIFF sample frames;
@@ -1600,17 +1676,16 @@ struct ByteItem {
 //   4. streams_step with the stage's decodes in front: one some_pcm_decode and one FLAC decode, mono, into the region its
 //      scatter reads.
 // A stream refused on its content (its walk, its chain, a decode failure, a rate or channel count the session cannot take)
-// leaves the step; the others go on, and the call then fails with the first refusal.
-int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
+// leaves the step; the others go on, and each call with a refused stream then fails with its first refusal.
+int bytes_step(some_session* s, std::vector<ByteItem>& bs) {
   const int sr = s->info.sample_rate;
-  std::string refusal;
   auto refuse = [&](ByteItem& b) {
     b.st->failed = true, b.live = false;
-    if (!refusal.empty()) return;
+    if (!b.refusal->empty()) return;
     char pre[128];
-    if (b.index < 0) snprintf(pre, sizeof(pre), "%s: ", who);
-    else snprintf(pre, sizeof(pre), "%s: stream %d: ", who, b.index);
-    refusal = std::string(pre) + some_last_error();
+    if (b.index < 0) snprintf(pre, sizeof(pre), "%s: ", b.who);
+    else snprintf(pre, sizeof(pre), "%s: stream %d: ", b.who, b.index);
+    *b.refusal = std::string(pre) + some_last_error();
   };
   auto too_short = [&](ByteItem& b) {    // resampy's refusal, at the end of a file at another rate
     const some_stream* st = b.st;
@@ -1668,7 +1743,7 @@ int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
     int64_t cap = 64;
     for (const ByteItem& b : bs)
       if (flac(b)) cap += b.win / 64 + 8;
-    SOME_REQUIRE(cap < (int64_t(1) << 31), "%s: too many FLAC frame candidates in one step", who);
+    SOME_REQUIRE(cap < (int64_t(1) << 31), "%s: too many FLAC frame candidates in one step", bs[0].who);
     if (dec.scan(s, cap, true)) return -1;
     const int n_cand = dec.n_cand;
     dec.chain.resize(std::max(n_cand, 1));
@@ -1728,19 +1803,22 @@ int bytes_step(some_session* s, std::vector<ByteItem>& bs, const char* who) {
   }
   if (!items.empty() && streams_step(s, items, &dec)) return -1;
   for (size_t j = 0; j < items.size(); ++j)
-    if (items[j].dropped) refuse(*of[j]);      // its frame failed to decode
-  if (!refusal.empty()) {
-    set_error("%s", refusal.c_str());
-    return SOME_STREAM_REFUSED;
-  }
+    if (items[j].dropped) set_error("%s", items[j].why.c_str()), refuse(*of[j]);   // its frame failed to decode
   return 0;
 }
 
+// Queues encoded stream items as one call (some_stream_push_bytes*, some_stream_finish).
+int bytes_call(some_session* s, std::vector<ByteItem>& bs) {
+  Request rq{Request::BYTES};
+  rq.bytes = &bs;
+  for (const ByteItem& b : bs) rq.samples += b.n, rq.touches.push_back(b.st), rq.touches.push_back(b.out);
+  return submit(s, rq);
+}
 // A step of one encoded stream (some_stream_push_bytes, some_stream_finish).
 int bytes_call(some_stream* st, const void* data, long long n, bool final, some_notes* out, const char* who) {
   if (final) st->finished = true;
-  std::vector<ByteItem> bs{ByteItem{st, static_cast<const uint8_t*>(data), n, final, out, -1}};
-  return locked(st->s, [&] { return bytes_step(st->s, bs, who); });
+  std::vector<ByteItem> bs{ByteItem{st, static_cast<const uint8_t*>(data), n, final, out, -1, who}};
+  return bytes_call(st->s, bs);
 }
 
 // The arguments of a many-call `who` (streams of one kind, encoded or PCM; n[i] bytes or samples at data[i]), every one
@@ -1796,7 +1874,8 @@ extern "C" int some_stream_push(some_stream* st, const float* samples, long long
   SOME_REQUIRE(st != nullptr && out != nullptr && n >= 0 && (n == 0 || samples != nullptr), "some_stream_push: bad arguments");
   SOME_REQUIRE(!st->walk, "some_stream_push: an encoded stream takes bytes (some_stream_push_bytes)");
   SOME_REQUIRE(!st->finished, "some_stream_push: the stream has finished");
-  return stream_call(st, samples, n, false, out);
+  std::vector<StepItem> items{StepItem{st, samples, n, false, out}};
+  return stream_call(st->s, items);
 }
 
 extern "C" int some_stream_finish(some_stream* st, some_notes* out) {
@@ -1809,7 +1888,8 @@ extern "C" int some_stream_finish(some_stream* st, some_notes* out) {
                "some_stream_finish: Input signal length=%lld is too small to resample from %d->%d", (long long)st->received,
                st->rate, sr);
   st->finished = true;
-  return stream_call(st, nullptr, 0, true, out);
+  std::vector<StepItem> items{StepItem{st, nullptr, 0, true, out}};
+  return stream_call(st->s, items);
 }
 
 extern "C" int some_stream_push_many(some_stream* const* streams, const float* const* samples, const long long* n,
@@ -1826,7 +1906,7 @@ extern "C" int some_stream_push_many(some_stream* const* streams, const float* c
     if (final) streams[i]->finished = true;
     items.push_back(StepItem{streams[i], samples[i], n[i], final, out[i]});
   }
-  return locked(s, [&] { return streams_step(s, items); });
+  return stream_call(s, items);
 }
 
 extern "C" int some_stream_get_info(const some_stream* st, some_stream_info* info) {
@@ -1875,9 +1955,10 @@ extern "C" int some_stream_push_bytes_many(some_stream* const* streams, const vo
   for (int i = 0; i < count; ++i) {
     const bool final = finish && finish[i];
     if (final) streams[i]->finished = true;
-    bs.push_back(ByteItem{streams[i], static_cast<const uint8_t*>(data[i]), n_bytes[i], final, out[i], i});
+    bs.push_back(ByteItem{streams[i], static_cast<const uint8_t*>(data[i]), n_bytes[i], final, out[i], i,
+                          "some_stream_push_bytes_many"});
   }
-  return locked(s, [&] { return bytes_step(s, bs, "some_stream_push_bytes_many"); });
+  return bytes_call(s, bs);
 }
 
 extern "C" int some_stream_get_meta(const some_stream* st, some_audio_meta* meta, long long* bytes_received,
@@ -1893,81 +1974,120 @@ extern "C" int some_stream_get_meta(const some_stream* st, some_audio_meta* meta
 
 // ---------------------------------------------------------------------------------------------------- encoded files
 namespace {
-struct EncItem {
-  const uint8_t* bytes = nullptr;
-  some_audio_meta m{};
-  int64_t n = 0;              // decoded samples at the file's rate (FLAC without a stated length: known after the chain)
-  SliceShape sh;
-  int64_t up = 0;             // the audio bytes' offset in the upload
-};
-
-// Re-raises the last error with the item's index in front.
-int item_error(int i) {
-  const std::string m = some_last_error();
-  set_error("some_session_transcribe_encoded: item %d: %s", i, m.c_str());
-  return -1;
+// Item i's message with its index in front.
+std::string item_message(int i, const std::string& m) {
+  return "some_session_transcribe_encoded: item " + std::to_string(i) + ": " + m;
 }
 
-// The GPU step of some_session_transcribe_encoded (under the session's mutex); out[] is written only at the end.  Each
-// file's data chunk goes through Decode (with FLAC files: the count, then the candidates down, and some_flac_chain) into
-// the recording buffer, whose Recordings are resampled, cut and transcribed after one synchronise.
-int transcribe_encoded(some_session* s, std::vector<EncItem>& its, const some_slicer_frames& sl, some_notes* const* out) {
+// The GPU step of sliced and encoded calls (Recordings).  The encoded files' data chunks go through one Decode (with FLAC
+// files: the count, then the candidates down, and some_flac_chain per file) and the sliced calls' recordings through the
+// pinned staging buffer, into the recording buffer, whose Recordings are resampled, cut and transcribed after one synchronise
+// (in a step of sliced calls only, when a recording is cut).  An encoded call whose file is refused after the scan (its chain,
+// its length, its decode) fails with what it gives alone and leaves the step; its out[] are not written.
+int recordings_step(some_session* s, const std::vector<Request*>& g) {
   const int sr = s->info.sample_rate;
-  const int count = static_cast<int>(its.size());
+  struct Ref {
+    Request* rq;
+    int i;
+  };
+  std::vector<Ref> refs;                  // every recording of the step, in call order
+  for (Request* rq : g)
+    for (int i = 0; i < static_cast<int>(rq->recs->size()); ++i) refs.push_back({rq, i});
+  auto item = [&](const Ref& f) -> RecItem& { return (*f.rq->recs)[f.i]; };
   std::vector<ByteWindow> ws;
-  for (EncItem& it : its) ws.push_back({&it.m, it.bytes + it.m.data_offset, it.m.data_bytes, &it.up});
-  Decode dec;
-  if (dec.upload(s, ws, "the encoded files")) return -1;
-  for (int i = 0; i < count; ++i) {
-    const EncItem& it = its[i];
-    if (!pcm_container(it.m)) {
-      dec.flac_of.push_back(i);
-    } else {
-      dec.pcm.push_back(some_pcm_item{dec.bytes_d + it.up, it.n, it.m.channels, it.m.kind, 1, 0, nullptr});
-      dec.pcm_of.push_back(i);
-    }
+  std::vector<int> flac;                  // the refs of the FLAC files, in upload order
+  for (int k = 0; k < static_cast<int>(refs.size()); ++k) {
+    RecItem& it = item(refs[k]);
+    if (it.host) continue;
+    ws.push_back({&it.m, it.bytes + it.m.data_offset, it.m.data_bytes, &it.up});
+    if (!pcm_container(it.m)) flac.push_back(k);
   }
-  const int nf = dec.nf;
-  if (nf) {
+  const bool encoded = !ws.empty();
+  Decode dec;
+  if (encoded && dec.upload(s, ws, "the encoded files")) return -1;
+  std::vector<std::vector<int32_t>> chains(flac.size());
+  if (dec.nf) {
     int64_t cap = 64;
-    std::vector<some_flac_range> recs;
-    for (int i : dec.flac_of) {
-      const EncItem& it = its[i];
+    for (int k : flac) {
+      const RecItem& it = item(refs[k]);
       cap += it.m.frames ? it.m.frames / std::max(it.m.min_blocksize, 1) + 2 : it.m.data_bytes / 16 + 2;
-      recs.push_back(some_flac_range{it.up - it.m.data_offset, it.up, it.up + it.m.data_bytes, it.m.frames});
-      dec.channels.push_back(it.m.channels);
-      dec.base.push_back(it.up - it.m.data_offset);
     }
     SOME_REQUIRE(cap < (int64_t(1) << 31), "some_session_transcribe_encoded: too many FLAC frames in one call");
     if (dec.scan(s, cap, false)) return -1;
-    std::vector<int64_t> lengths(nf, 0);
-    dec.first.assign(nf + 1, 0);
-    dec.chain.resize(std::max(dec.n_cand, 1));
-    int failed = -1;
-    if (some_flac_chain(dec.frames_h, dec.n_cand, recs.data(), nf, dec.chain.data(), dec.n_cand, dec.first.data(),
-                        lengths.data(), &failed))
-      return item_error(failed >= 0 ? dec.flac_of[failed] : 0);
-    dec.chain.resize(dec.first[nf]);
-    for (int k = 0; k < nf; ++k) {
-      EncItem& it = its[dec.flac_of[k]];
-      it.n = lengths[k];
-      char who[96];
-      snprintf(who, sizeof(who), "some_session_transcribe_encoded: item %d", dec.flac_of[k]);
-      if (slice_shape(it.n, it.m.rate, sr, sl, who, &it.sh)) return -1;   // the length was not stated: checked now
+    for (size_t r = 0; r < flac.size(); ++r) {   // every file's chain first, then the lengths, as in one call
+      const Ref& f = refs[flac[r]];
+      RecItem& it = item(f);
+      if (f.rq->rc) continue;
+      const some_flac_range rec{it.up - it.m.data_offset, it.up, it.up + it.m.data_bytes, it.m.frames};
+      chains[r].resize(std::max(dec.n_cand, 1));
+      int64_t first[2], length = 0;
+      if (some_flac_chain(dec.frames_h, dec.n_cand, &rec, 1, chains[r].data(), dec.n_cand, first, &length, nullptr)) {
+        f.rq->fail(-1, item_message(f.i, some_last_error()));
+        continue;
+      }
+      chains[r].resize(first[1]);
+      it.n = length;
+    }
+    for (size_t r = 0; r < flac.size(); ++r) {
+      const Ref& f = refs[flac[r]];
+      RecItem& it = item(f);
+      if (f.rq->rc) continue;
+      const std::string who = "some_session_transcribe_encoded: item " + std::to_string(f.i);
+      if (slice_shape(it.n, it.m.rate, sr, f.rq->sl, who.c_str(), &it.sh)) f.rq->fail(-1, some_last_error());
     }
   }
-
+  // the recordings of the calls still in the step
   Recordings rec;
-  for (int i = 0; i < count; ++i) rec.items.push_back({its[i].m.rate, its[i].n, its[i].sh, out[i]});
+  std::vector<int> rec_of(refs.size(), -1), ref_of;
+  for (int k = 0; k < static_cast<int>(refs.size()); ++k) {
+    const Ref& f = refs[k];
+    const RecItem& it = item(f);
+    if (f.rq->rc) continue;
+    const int j = static_cast<int>(rec.items.size());
+    rec_of[k] = j, ref_of.push_back(k);
+    rec.items.push_back({it.m.rate, it.n, it.sh, &f.rq->sl, it.out});
+    if (!it.host && pcm_container(it.m)) {
+      dec.pcm.push_back(some_pcm_item{dec.bytes_d + it.up, it.n, it.m.channels, it.m.kind, 1, 0, nullptr});
+      dec.pcm_of.push_back(j);
+    }
+  }
+  if (rec.items.empty()) return 0;
+  for (size_t r = 0; r < flac.size(); ++r) {
+    const int j = rec_of[flac[r]];
+    if (j < 0) continue;
+    const RecItem& it = item(refs[flac[r]]);
+    dec.chain.insert(dec.chain.end(), chains[r].begin(), chains[r].end());
+    dec.flac_of.push_back(j);
+    dec.first.push_back(static_cast<int64_t>(dec.chain.size()));
+    dec.channels.push_back(it.m.channels);
+    dec.base.push_back(it.up - it.m.data_offset);
+  }
   Upload up{s};
-  dec.add(up);
-  if (rec.place(s, sl, up) || dec.fill(s, up, rec.base, [&](int i) { return rec.items[i].x; }) ||
-      up.send("descriptor upload") || dec.launch(s, up) || rec.launch(s, up))
+  if (encoded) dec.add(up);
+  if (rec.place(s, up)) return -1;
+  std::vector<Staged> staged;
+  bool cut = false;
+  for (size_t j = 0; j < rec.items.size(); ++j) {
+    const RecItem& it = item(refs[ref_of[j]]);
+    if (it.host) staged.push_back({rec.base + rec.items[j].x, it.host, it.n});
+    cut |= rec.items[j].sh.frames > 0;
+  }
+  if ((!staged.empty() && upload_staged(s, staged)) ||
+      (encoded && dec.fill(s, up, rec.base, [&](int j) { return rec.items[j].x; })) || up.send("descriptor upload") ||
+      (encoded && dec.launch(s, up)) || rec.launch(s, up))
     return -1;
-  SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
-  const int failed = dec.check(up);
-  if (failed >= 0) return item_error(failed);
-  return rec.finish(s, sl);
+  if (encoded || cut) SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+  if (encoded) {
+    std::vector<std::pair<int, std::string>> failed;
+    if (dec.check(s, up, failed)) return -1;
+    for (const auto& fl : failed) {
+      const Ref& f = refs[ref_of[fl.first]];
+      f.rq->fail(-1, item_message(f.i, fl.second));
+    }
+    for (size_t j = 0; j < rec.items.size(); ++j)
+      if (refs[ref_of[j]].rq->rc) rec.items[j].out = nullptr;
+  }
+  return rec.finish(s);
 }
 }  // namespace
 
@@ -1979,7 +2099,9 @@ extern "C" int some_session_transcribe_encoded(some_session* s, const some_encod
   some_slicer_frames sl;
   if (some_slicer_derive(sr, params, &sl)) return -1;
   // every item is checked before any GPU work
-  std::vector<EncItem> its(count);
+  std::vector<RecItem> its(count);
+  Request rq{Request::RECORDINGS};
+  rq.recs = &its, rq.sl = sl;
   std::map<const void*, int> seen_notes;
   for (int i = 0; i < count; ++i) {
     SOME_REQUIRE(items[i].data != nullptr && items[i].n_bytes > 0, "some_session_transcribe_encoded: item %d is NULL or empty", i);
@@ -1987,15 +2109,147 @@ extern "C" int some_session_transcribe_encoded(some_session* s, const some_encod
     const auto shared = seen_notes.emplace(out[i], i);
     SOME_REQUIRE(shared.second, "some_session_transcribe_encoded: item %d shares its some_notes with item %d", i,
                  shared.first->second);
-    EncItem& it = its[i];
+    RecItem& it = its[i];
     it.bytes = static_cast<const uint8_t*>(items[i].data);
-    if (some_audio_info(items[i].data, items[i].n_bytes, &it.m) || check_format(it.m, sr)) return item_error(i);
+    it.out = out[i];
+    if (some_audio_info(items[i].data, items[i].n_bytes, &it.m) || check_format(it.m, sr)) {
+      set_error("%s", item_message(i, some_last_error()).c_str());
+      return -1;
+    }
     it.n = it.m.frames;
     if (pcm_container(it.m) || it.m.frames > 0) {
-      char who[96];
-      snprintf(who, sizeof(who), "some_session_transcribe_encoded: item %d", i);
-      if (slice_shape(it.n, it.m.rate, sr, sl, who, &it.sh)) return -1;
+      const std::string who = "some_session_transcribe_encoded: item " + std::to_string(i);
+      if (slice_shape(it.n, it.m.rate, sr, sl, who.c_str(), &it.sh)) return -1;
+      rq.samples += it.sh.n_out;
+    } else {
+      rq.sized = false;                   // a FLAC file without a stated length: known only after its chain
+    }
+    rq.touches.push_back(out[i]);
+  }
+  return submit(s, rq);
+}
+
+// ---------------------------------------------------------------------------------------------------- the scheduler
+namespace {
+constexpr int64_t kStepSamples = SOME_SESSION_STEP_SAMPLES;
+
+// A step of clip calls: their clips in one run_chunks, then split per call.
+int clips_step(some_session* s, const std::vector<Request*>& g) {
+  std::vector<const float*> clips;
+  std::vector<int64_t> lens;
+  for (const Request* rq : g) clips.insert(clips.end(), rq->clips, rq->clips + rq->B), lens.insert(lens.end(), rq->lens, rq->lens + rq->B);
+  const int B = static_cast<int>(lens.size());
+  if (run_chunks(s, clips.data(), nullptr, nullptr, lens.data(), B, &s->chunks)) return -1;
+  const std::vector<int64_t> begin(B, 0);
+  int c = 0;
+  for (const Request* rq : g) take_chunks(s->chunks, c, c + rq->B, begin.data(), lens.data(), rq->out), c += rq->B;
+  return 0;
+}
+
+// A step of PCM stream calls, or of encoded stream calls: their items in one streams_step or bytes_step.
+int streams_calls_step(some_session* s, const std::vector<Request*>& g) {
+  std::vector<StepItem> items;
+  for (const Request* rq : g) items.insert(items.end(), rq->items->begin(), rq->items->end());
+  return streams_step(s, items);
+}
+int bytes_calls_step(some_session* s, const std::vector<Request*>& g) {
+  std::vector<std::string> refusals(g.size());
+  std::vector<ByteItem> bs;
+  for (size_t k = 0; k < g.size(); ++k)
+    for (ByteItem b : *g[k]->bytes) b.refusal = &refusals[k], bs.push_back(b);
+  if (bytes_step(s, bs)) return -1;
+  for (size_t k = 0; k < g.size(); ++k)
+    if (!refusals[k].empty()) g[k]->fail(SOME_STREAM_REFUSED, refusals[k]);
+  return 0;
+}
+
+// Runs one step on the calling thread, with the session's device current and the calls' some_set_pdl setting.  After a
+// failure partway through, copies and kernels may still be queued on the session's streams: it waits for them, on every
+// replica, so that the next step cannot rewrite staging or device buffers they still use; every call of the step then fails
+// with the failure's message.  Returns the step's result.
+int run_step(some_session* s, const std::vector<Request*>& g) {
+  const int pdl = some_set_pdl(g[0]->pdl);
+  int rc = -1;
+  {
+    DeviceScope scope(s->device);
+    if (scope.err != cudaSuccess) {
+      set_error("session: cudaSetDevice: %s", cudaGetErrorString(scope.err));
+    } else {
+      for (std::unique_ptr<Replica>& r : s->reps) r->chunks = r->frames = 0;
+      switch (g[0]->kind) {
+        case Request::CLIPS: rc = clips_step(s, g); break;
+        case Request::RECORDINGS: rc = recordings_step(s, g); break;
+        case Request::STREAMS: rc = streams_calls_step(s, g); break;
+        case Request::BYTES: rc = bytes_calls_step(s, g); break;
+      }
+    }
+    if (rc != 0) {
+      const std::string msg = some_last_error();
+      for (Request* rq : g) rq->fail(-1, msg);
+      for (std::unique_ptr<Replica>& r : s->reps) {
+        cudaStreamSynchronize(r->copy_stream);
+        cudaStreamSynchronize(r->stream);
+      }
     }
   }
-  return locked(s, [&] { return transcribe_encoded(s, its, sl, out); });
+  some_set_pdl(pdl);
+  return rc;
 }
+
+// The next step, under the session's mutex: the oldest queued call and every later call that may join it, in arrival order
+// (include/some_b200.h, "Calls from several threads").  A call that cannot join keeps its place, and no later call that
+// touches one of its streams or some_notes joins past it.
+std::vector<Request*> take_step(some_session* s) {
+  Request* first = s->queue.front();
+  s->queue.pop_front();
+  std::vector<Request*> g{first};
+  if (!first->sized) return g;
+  const int64_t bound = std::max(first->samples, kStepSamples);
+  int64_t total = first->samples;
+  std::set<const void*> held(first->touches.begin(), first->touches.end());
+  for (auto it = s->queue.begin(); it != s->queue.end();) {
+    Request* r = *it;
+    bool clash = false;
+    for (const void* p : r->touches) clash = clash || held.count(p) > 0;
+    held.insert(r->touches.begin(), r->touches.end());
+    if (clash || r->kind != first->kind || r->pdl != first->pdl || !r->sized || total + r->samples > bound) {
+      ++it;
+      continue;
+    }
+    g.push_back(r), total += r->samples;
+    it = s->queue.erase(it);
+  }
+  return g;
+}
+
+// Queues a call and returns its result, by flat combining: while its call has not run and no step is running, the calling
+// thread takes the next step (take_step) and runs it for every call in it; otherwise it waits.  Its own call's message, if
+// it failed, becomes its thread's some_last_error().
+int submit(some_session* s, Request& rq) {
+  rq.pdl = pdl_enabled() ? 1 : 0;
+  std::unique_lock<std::mutex> lock(s->mu);
+  s->queue.push_back(&rq);
+  ++s->stats.calls;
+  while (!rq.done) {
+    if (s->running) {
+      s->done.wait(lock);
+      continue;
+    }
+    const std::vector<Request*> g = take_step(s);
+    s->running = true;
+    ++s->stats.steps;
+    s->stats.max_calls = std::max<int64_t>(s->stats.max_calls, static_cast<int64_t>(g.size()));
+    lock.unlock();
+    const int rc = run_step(s, g);
+    lock.lock();
+    if (rc == 0)
+      for (size_t i = 0; i < s->reps.size(); ++i) s->load[i] = {s->reps[i]->chunks, s->reps[i]->frames};
+    for (Request* r : g) r->done = true;
+    s->running = false;
+    s->done.notify_all();
+  }
+  lock.unlock();
+  if (rq.rc) set_error("%s", rq.err.c_str());
+  return rq.rc;
+}
+}  // namespace

@@ -114,12 +114,20 @@ class Session:
         return list(arr[:n.value])
 
     def load(self) -> List[Tuple[int, int]]:
-        """some_session_get_load: (chunks, frames) each replica ran in the session's last completed call."""
+        """some_session_get_load: (chunks, frames) each replica ran in the session's last completed step."""
         n = C.c_int()
         _lib.check(self.lib.some_session_get_load(self.handle, None, None, 0, C.byref(n)), 'some_session_get_load')
         chunks, frames = (C.c_int64 * max(n.value, 1))(), (C.c_int64 * max(n.value, 1))()
         _lib.check(self.lib.some_session_get_load(self.handle, chunks, frames, n.value, C.byref(n)), 'some_session_get_load')
         return list(zip(chunks[:n.value], frames[:n.value]))
+
+    def stats(self) -> Dict[str, int]:
+        """some_session_get_stats: totals since open (``calls``, ``steps``, ``max_calls``: the most calls one step held) and
+        the calls ``queued`` at this moment.  The library is loaded with ctypes.CDLL, which releases the GIL around every
+        call, so Python threads that share a session queue together and their calls can share a step."""
+        st = _lib.SessionStats()
+        _lib.check(self.lib.some_session_get_stats(self.handle, C.byref(st)), 'some_session_get_stats')
+        return {name: getattr(st, name) for name, _ in _lib.SessionStats._fields_}
 
     def transcribe(self, waveforms: Sequence[np.ndarray], notes: Optional[Notes] = None) -> List[Dict[str, np.ndarray]]:
         """some_session_transcribe: mono float32 clips at the model's rate -> one dict per clip, in input order."""
