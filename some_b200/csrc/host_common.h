@@ -82,6 +82,13 @@ inline int64_t frames_within(const some_slicer_frames& f, int64_t fixed) {
   return fixed < reach ? 0 : (fixed - reach) / f.hop_size + 1;
 }
 
+// The RMS frames slicer2 cuts a whole recording of n samples by (librosa's centred frames), or 0 when the recording is one
+// chunk anyway: no longer than min_length hops (slicer2.py:79-80).
+inline int64_t frames_whole(const some_slicer_frames& f, int64_t n) {
+  if ((n + f.hop_size - 1) / f.hop_size <= f.min_length) return 0;
+  return 1 + (n + 2 * (f.win_size / 2) - f.win_size) / f.hop_size;
+}
+
 // Packed descriptors of a many-window launch (some_resample_windows_pack, some_slicer_rms_windows_pack and the stream's
 // upload): a header, the windows' first tiles (K + 1 prefix sums: the grid lays the windows' tiles end to end) and the K
 // kernel parameter blocks P, each part 16-byte aligned.  The host copy sizes the launch; the kernel reads a device copy of

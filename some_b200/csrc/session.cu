@@ -5,10 +5,11 @@
 //   some_mel_logmel -> some_forward (stand-alone LayerNorms, sigmoid / softmax head) -> some_decode_notes.
 // The sliced and the encoded calls share that front end (Recordings: one resampling window per recording at another rate,
 // one RMS window per recording that is cut, one batch over the chunks of all recordings); a stream step launches the same
-// two kernels over the windows of its streams.  The encoded files call and the encoded stream step share the stage in front
-// of it (Decode: one upload of the audio bytes, one FLAC scan, one PCM and one FLAC decode).  A session opened on several
-// devices holds one replica of the model per device: the front end runs on replica 0, and run_chunks spreads the chunks of
-// each call over the replicas, each on its own thread, and gathers their notes in chunk order.  Every call is a request in
+// two kernels over the windows of its streams (both through StepWindows).  The encoded files call and the encoded stream
+// step share the stage in front of it (Decode: one upload of the audio bytes, one FLAC scan, one PCM and one FLAC decode).
+// A session holds one replica of the model per device it was opened on: the front end runs on replica 0, run_chunks spreads
+// the chunks of each step over the replicas, each on its own thread (replica 0, the only one of a one-device session, on the
+// calling thread), and take_chunks reads each caller's notes from the replica that ran each chunk.  Every call is a request in
 // the session's queue (submit, at the end): calls of one kind that queue while a step runs share the next step, whose back
 // end (run_chunks, Recordings, streams_step, bytes_step) takes the items of all of them.
 //
@@ -193,6 +194,9 @@ struct DeviceScope {
     SOME_REQUIRE(e_ == cudaSuccess, "session: %s: %s", what, cudaGetErrorString(e_));   \
   } while (0)
 
+// n floats rounded up to a 16-byte multiple: where the next clip or recording of a buffer starts.
+constexpr int64_t align4(int64_t n) { return (n + 3) & ~int64_t(3); }
+
 struct Chunk {
   int c0, c1;
   uint64_t off;
@@ -294,8 +298,8 @@ struct Replica {
   int ws_m = 0;
   some_workspace ws{};
   std::unique_ptr<WorkerPool> pool;       // its staging lanes (WorkerPool::run is not re-entrant)
-  some_notes part;                        // with several replicas: the notes of its share of a call
-  int64_t chunks = 0, frames = 0;         // its share of the call in progress
+  some_notes part;                        // the notes of its share of the step's chunks, in its order (no ranges)
+  int64_t chunks = 0, frames = 0;         // its share of the step in progress
 };
 }  // namespace
 
@@ -328,12 +332,12 @@ struct some_session {
   // the encoded calls' Decode: the audio bytes, the FLAC candidate list, scan workspace and int32 scratch
   DevBuf enc_d, flac_frames_d, flac_ws_d, flac_scratch_d;
   PinBuf enc_h, flac_frames_h;
-  some_notes chunks;                      // the notes of a step's chunks, before they are split by recording or stream
   std::vector<std::unique_ptr<Replica>> reps;
-  // with several replicas: lane r runs replica r's share of a call (lane 0 on the calling thread), and `fed` is recorded on
-  // replica 0's stream once the front end has written the chunks the others copy
+  // lane r runs replica r's share of a step (lane 0 on the calling thread, the only lane of a one-device session); with
+  // several replicas, `fed` is recorded on replica 0's stream once the front end has written the chunks the others copy
   std::unique_ptr<WorkerPool> lanes;
   cudaEvent_t fed = nullptr;
+  std::vector<std::pair<int, int>> held;  // chunk c of the step: the replica that ran it, and its clip in that replica's part
   std::vector<std::pair<int64_t, int64_t>> load;   // each replica's chunks and frames in the last completed step
 };
 
@@ -362,17 +366,22 @@ void clear(some_notes* out) {
   out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
 }
 
-// Sets *out to chunks [c0, c1) of `all` (the notes of a step's batch); chunk c is samples [begin[c], begin[c] + lens[c]).
-void take_chunks(const some_notes& all, int c0, int c1, const int64_t* begin, const int64_t* lens, some_notes* out) {
+// Appends the notes of clip k of `from` to *out, as its next clip of sample range [b, e).
+void append_clip(const some_notes& from, int k, int64_t b, int64_t e, some_notes* out) {
+  const int64_t n0 = from.first[k], n1 = from.first[k + 1];
+  out->midi.insert(out->midi.end(), from.midi.begin() + n0, from.midi.begin() + n1);
+  out->dur.insert(out->dur.end(), from.dur.begin() + n0, from.dur.begin() + n1);
+  out->rest.insert(out->rest.end(), from.rest.begin() + n0, from.rest.begin() + n1);
+  out->first.push_back(out->first.back() + (n1 - n0));
+  out->range.push_back(b), out->range.push_back(e);
+}
+
+// Sets *out to chunks [c0, c1) of the step's last run_chunks, each read from the replica that ran it; chunk c is samples
+// [begin[c], begin[c] + lens[c]).
+void take_chunks(const some_session* s, int c0, int c1, const int64_t* begin, const int64_t* lens, some_notes* out) {
   clear(out);
-  for (int c = c0; c < c1; ++c) {
-    const int64_t a = all.first[c], b = all.first[c + 1];
-    out->midi.insert(out->midi.end(), all.midi.begin() + a, all.midi.begin() + b);
-    out->dur.insert(out->dur.end(), all.dur.begin() + a, all.dur.begin() + b);
-    out->rest.insert(out->rest.end(), all.rest.begin() + a, all.rest.begin() + b);
-    out->first.push_back(out->first.back() + (b - a));
-    out->range.push_back(begin[c]), out->range.push_back(begin[c] + lens[c]);
-  }
+  for (int c = c0; c < c1; ++c)
+    append_clip(s->reps[s->held[c].first]->part, s->held[c].second, begin[c], begin[c] + lens[c], out);
 }
 
 // A span of host memory to copy into pinned memory.
@@ -426,9 +435,9 @@ std::vector<std::pair<int, int>> split_chunks(const std::vector<int32_t>& cu) {
 // One var-len batch through mel -> trunk -> decode on replica r, pipelined like Engine.enqueue.  Host clips (`host` != NULL:
 // clip i is host[i][0 .. lens[i])) are staged through pinned memory and copied on the copy stream while the previous chunk's
 // kernels run; resident clips (`resident` != NULL) are the sample ranges [starts[i], starts[i] + lens[i]) of that buffer on
-// r's device, written by work on r's streams or awaited by its copy stream.
+// r's device, written by work on r's streams or awaited by its copy stream.  The notes of clip i go to clip i of r.part.
 int run_batch(const some_session* s, Replica& r, const float* const* host, const float* resident, const int64_t* res_starts,
-              const int64_t* lens, int B, some_notes* out) {
+              const int64_t* lens, int B) {
   std::vector<int32_t> cu(B + 1, 0);
   std::vector<int64_t> starts(B, 0);
   int64_t total = 0;
@@ -439,7 +448,7 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
     cu[i + 1] = static_cast<int32_t>(cu[i] + frames);
     if (host) {
       starts[i] = total;
-      total += (lens[i] + 3) & ~int64_t(3);     // 16-byte aligned clip starts, as Engine.tables
+      total += align4(lens[i]);                 // 16-byte aligned clip starts, as Engine.tables
     } else {
       starts[i] = res_starts[i];
     }
@@ -496,7 +505,7 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
     }
     int32_t* cuc = cu_h + ch.c0 + ci;            // chunk ci owns entries [c0 + ci, c1 + ci]
     for (int i = 0; i <= ch.bc; ++i) cuc[i] = cu[ch.c0 + i] - cu[ch.c0];
-    const int64_t hi = host ? starts[ch.c1 - 1] + ((lens[ch.c1 - 1] + 3) & ~int64_t(3)) : lo;
+    const int64_t hi = host ? starts[ch.c1 - 1] + align4(lens[ch.c1 - 1]) : lo;
     if (hi > lo)
       SOME_CUDA(cudaMemcpyAsync(static_cast<float*>(r.wave_d.p) + lo, wave_h + lo, 4ull * (hi - lo), cudaMemcpyHostToDevice,
                                 r.copy_stream), "audio upload");
@@ -528,9 +537,8 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
   SOME_CUDA(cudaStreamSynchronize(r.stream), "synchronise");
 
   // unpack: the notes of clip b start at its first frame's row of the chunk slab
-  out->first.assign(1, 0);
-  out->range.clear();
-  out->midi.clear(), out->dur.clear(), out->rest.clear();
+  some_notes* out = &r.part;
+  clear(out);
   const uint8_t* h = static_cast<const uint8_t*>(r.slab_h.p);
   for (const Chunk& ch : layout) {
     const uint8_t* o = h + ch.off;
@@ -546,41 +554,37 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
         out->rest.push_back(o[4ull * ch.bc + 8ull * ch.mc + r]);
       }
       out->first.push_back(out->first.back() + n);
-      out->range.push_back(host ? 0 : starts[ch.c0 + b]);
-      out->range.push_back(host ? lens[ch.c0 + b] : starts[ch.c0 + b] + lens[ch.c0 + b]);
     }
   }
   return 0;
 }
 
-// The chunks of a call, on every replica of the session.  With one replica this is run_batch.  With several, some_shard_clips
-// assigns the chunks; replica 0 runs its share on the calling thread and replica r its share on lane r, each with the
-// caller's some_set_pdl setting and each through run_batch; the notes come back in chunk order, as one batch gives them (a
-// chunk's notes do not depend on the rest of its batch).  Resident chunks lie in a buffer on replica 0's device, written on
-// its stream: replica r > 0 waits on its copy stream for `fed`, recorded there after the front end, and copies its share,
-// packed at 16-byte aligned starts, into its own audio buffer (a peer copy, or a device-to-device copy when both replicas are
-// on one device).  Host clips are staged straight to the replica that runs them.
+// The chunks of a step, on every replica of the session: some_shard_clips assigns them (one replica runs all of them);
+// replica 0 runs its share on the calling thread and replica r > 0 its share on lane r, with the caller's some_set_pdl
+// setting, each through run_batch into its own part, and s->held records which replica ran each chunk and where its notes
+// lie there, for take_chunks (a chunk's notes do not depend on the rest of its batch).  Resident chunks lie in a buffer on
+// replica 0's device, written on its stream: replica r > 0 waits on its copy stream for `fed`, recorded there after the
+// front end, and copies its share, packed at 16-byte aligned starts, into its own audio buffer (a peer copy, or a
+// device-to-device copy when both replicas are on one device).  Host clips are staged straight to the replica that runs them.
 int run_chunks(some_session* s, const float* const* host, const float* resident, const int64_t* starts, const int64_t* lens,
-               int B, some_notes* out) {
+               int B) {
   const int R = static_cast<int>(s->reps.size());
-  if (R == 1) {
-    Replica& r = *s->reps[0];
-    r.chunks = B;
-    for (int c = 0; c < B; ++c) r.frames += 1 + lens[c] / SOME_HOP;
-    return run_batch(s, r, host, resident, starts, lens, B, out);
-  }
-  std::vector<int32_t> owner(B);
-  if (some_shard_clips(lens, B, R, owner.data())) return -1;
+  std::vector<int32_t> owner(B, 0);
+  if (R > 1 && some_shard_clips(lens, B, R, owner.data())) return -1;
   std::vector<std::vector<int>> share(R);
-  for (int c = 0; c < B; ++c) share[owner[c]].push_back(c);
-  if (resident) SOME_CUDA(cudaEventRecord(s->fed, s->stream), "event record");
+  s->held.resize(B);
+  for (int c = 0; c < B; ++c) {
+    s->held[c] = {owner[c], static_cast<int>(share[owner[c]].size())};
+    share[owner[c]].push_back(c);
+  }
+  if (resident && std::any_of(share.begin() + 1, share.end(), [](const std::vector<int>& v) { return !v.empty(); }))
+    SOME_CUDA(cudaEventRecord(s->fed, s->stream), "event record");
   const int pdl = pdl_enabled() ? 1 : 0;
   std::vector<int> rc(R, 0);
   std::vector<std::string> err(R);
   s->lanes->run(R, [&](int ri) {
     Replica& r = *s->reps[ri];
     const std::vector<int>& mine = share[ri];
-    clear(&r.part);
     const int b = static_cast<int>(mine.size());
     if (b == 0) return;
     std::vector<const float*> clips;
@@ -591,11 +595,11 @@ int run_chunks(some_session* s, const float* const* host, const float* resident,
       r.frames += 1 + lens[c] / SOME_HOP;
       if (host) clips.push_back(host[c]);
       else if (ri == 0) at.push_back(starts[c]);
-      else at.push_back(total), total += (lens[c] + 3) & ~int64_t(3);
+      else at.push_back(total), total += align4(lens[c]);
     }
     r.chunks = b;
     auto work = [&]() -> int {
-      if (!resident || ri == 0) return run_batch(s, r, host ? clips.data() : nullptr, resident, at.data(), len.data(), b, &r.part);
+      if (!resident || ri == 0) return run_batch(s, r, host ? clips.data() : nullptr, resident, at.data(), len.data(), b);
       if (r.wave_d.ensure(4ull * total + 16, "the audio")) return -1;
       float* wave = static_cast<float*>(r.wave_d.p);
       SOME_CUDA(cudaStreamWaitEvent(r.copy_stream, s->fed, 0), "stream wait");
@@ -603,7 +607,7 @@ int run_chunks(some_session* s, const float* const* host, const float* resident,
         if (len[k])
           SOME_CUDA(cudaMemcpyPeerAsync(wave + at[k], r.device, resident + starts[mine[k]], s->device, 4ull * len[k],
                                         r.copy_stream), "chunk copy");
-      return run_batch(s, r, nullptr, wave, at.data(), len.data(), b, &r.part);
+      return run_batch(s, r, nullptr, wave, at.data(), len.data(), b);
     };
     if (ri == 0) {
       rc[ri] = work();
@@ -616,20 +620,10 @@ int run_chunks(some_session* s, const float* const* host, const float* resident,
     if (rc[ri]) err[ri] = some_last_error();
   });
   for (int ri = 0; ri < R; ++ri)
-    SOME_REQUIRE(rc[ri] == 0, "device %d (replica %d): %s", s->reps[ri]->device, ri, err[ri].c_str());
-  clear(out);
-  std::vector<int> next(R, 0);
-  for (int c = 0; c < B; ++c) {
-    const some_notes& p = s->reps[owner[c]]->part;
-    const int k = next[owner[c]]++;
-    const int64_t a = p.first[k], e = p.first[k + 1];
-    out->midi.insert(out->midi.end(), p.midi.begin() + a, p.midi.begin() + e);
-    out->dur.insert(out->dur.end(), p.dur.begin() + a, p.dur.begin() + e);
-    out->rest.insert(out->rest.end(), p.rest.begin() + a, p.rest.begin() + e);
-    out->first.push_back(out->first.back() + (e - a));
-    out->range.push_back(host ? 0 : starts[c]);
-    out->range.push_back(host ? lens[c] : starts[c] + lens[c]);
-  }
+    if (rc[ri]) {
+      if (R > 1) set_error("device %d (replica %d): %s", s->reps[ri]->device, ri, err[ri].c_str());   // one replica: as is
+      return -1;
+    }
   return 0;
 }
 
@@ -644,7 +638,7 @@ struct Staged {
 int upload_staged(some_session* s, const std::vector<Staged>& recs) {
   constexpr int64_t kPiece = int64_t(1) << 22;
   int64_t total = 0;
-  for (const Staged& r : recs) total += (r.n + 3) & ~int64_t(3);
+  for (const Staged& r : recs) total += align4(r.n);
   PinBuf& staging = s->reps[0]->wave_h;
   if (staging.ensure(4ull * total + 16, "the staged audio")) return -1;
   float* pin = static_cast<float*>(staging.p);
@@ -654,7 +648,7 @@ int upload_staged(some_session* s, const std::vector<Staged>& recs) {
       copy_to_pinned(*s->pool, {{pin + a, r.src + a, 4ull * len}}, size_t(1) << 18);
       SOME_CUDA(cudaMemcpyAsync(r.dst + a, pin + a, 4ull * len, cudaMemcpyHostToDevice, s->stream), "audio upload");
     }
-    pin += (r.n + 3) & ~int64_t(3);
+    pin += align4(r.n);
   }
   return 0;
 }
@@ -859,6 +853,7 @@ int open_session(const char* who, const char* path, const int* devices, int n, b
   s->stream = s->reps[0]->stream;
   s->pool = s->reps[0]->pool.get();
   s->load.assign(n, {0, 0});
+  s->lanes.reset(new WorkerPool(n));      // one replica: no thread, its lane runs on the calling thread
   if (n > 1) {
     DeviceScope scope(s->device);
     e = cudaEventCreateWithFlags(&s->fed, cudaEventDisableTiming);
@@ -866,7 +861,6 @@ int open_session(const char* who, const char* path, const int* devices, int n, b
       set_error("%s: cudaEventCreate: %s", who, cudaGetErrorString(e));
       return fail(-2);
     }
-    s->lanes.reset(new WorkerPool(n));
   }
   const Entry& kt = dir.at("kaiser_best");
   s->kaiser.resize(kKaiserTaps);
@@ -960,27 +954,24 @@ extern "C" int some_session_get_info(const some_session* s, some_session_info* i
 }
 
 namespace {
+// resampy's refusal: a recording of n samples at `rate` whose output at the model's rate sr would be empty.
+bool too_short_to_resample(int64_t n, int rate, int sr) { return rate != sr && n * sr / rate < 1; }
+
 // What the slicer sees of a recording of n samples at sample_rate: its length at the model's rate (audio.resampled_length:
 // librosa.load's output length; resampy refuses a recording whose own output would be empty) and, unless the recording is
-// one chunk anyway (no longer than min_length hops, slicer2.py:79-80), the number of RMS frames to cut it by.
+// one chunk anyway, the number of RMS frames to cut it by.
 struct SliceShape {
   int64_t n_out = 0;
   int frames = 0;       // 0: one chunk [0, n_out)
 };
 int slice_shape(int64_t n, int sample_rate, int sr, const some_slicer_frames& sl, const char* who, SliceShape* sh) {
-  int64_t n_out = n;
-  if (sample_rate != sr) {
-    SOME_REQUIRE(n * sr / sample_rate >= 1, "%s: Input signal length=%lld is too small to resample from %d->%d", who,
-                 static_cast<long long>(n), sample_rate, sr);
-    n_out = static_cast<int64_t>(ceil(static_cast<double>(n) * (static_cast<double>(sr) / sample_rate)));
-  }
-  sh->n_out = n_out;
-  sh->frames = 0;
-  if ((n_out + sl.hop_size - 1) / sl.hop_size > sl.min_length) {
-    const int64_t frames = 1 + (n_out + 2 * (sl.win_size / 2) - sl.win_size) / sl.hop_size;
-    SOME_REQUIRE(frames < (int64_t(1) << 31), "%s: recording too long", who);
-    sh->frames = static_cast<int>(frames);
-  }
+  SOME_REQUIRE(!too_short_to_resample(n, sample_rate, sr), "%s: Input signal length=%lld is too small to resample from %d->%d",
+               who, static_cast<long long>(n), sample_rate, sr);
+  sh->n_out = n;
+  if (sample_rate != sr) sh->n_out = static_cast<int64_t>(ceil(static_cast<double>(n) * (static_cast<double>(sr) / sample_rate)));
+  const int64_t frames = frames_whole(sl, sh->n_out);
+  SOME_REQUIRE(frames < (int64_t(1) << 31), "%s: recording too long", who);
+  sh->frames = static_cast<int>(frames);
   return 0;
 }
 // The chunk ranges of a recording from its shape and, when it is cut, its sh.frames RMS values.
@@ -1076,15 +1067,56 @@ struct Upload {
   }
 };
 
-constexpr int64_t align4(int64_t n) { return (n + 3) & ~int64_t(3); }
+// The resampling and RMS windows of a step, launched together on the session's stream:
+//   rms     adds an RMS window and returns where its first frame lies in the session's RMS buffers (after the frames of the
+//           windows added before it);
+//   place   after every other region of the step's upload is added: a descriptor region for each kind that has windows (so
+//           a step without any uploads nothing for them), the upload reserved, the RMS buffers sized and the descriptors packed;
+//   launch  after the upload is sent and the samples are written: one resampling launch, one RMS launch, the RMS download.
+struct StepWindows {
+  std::vector<some_resample_window> rs;
+  std::vector<some_rms_window> rm;
+  int64_t frames = 0;
+  size_t rs_off = 0, rm_off = 0;
+
+  int64_t rms(const some_rms_window& w) {
+    const int64_t at = frames;
+    rm.push_back(w);
+    frames += w.f_end - w.f_begin;
+    return at;
+  }
+
+  int place(some_session* s, Upload& up, const char* what) {
+    const int kr = static_cast<int>(rs.size()), km = static_cast<int>(rm.size());
+    if (kr) rs_off = up.add(static_cast<size_t>(some_resample_windows_bytes(kr)));
+    if (km) rm_off = up.add(static_cast<size_t>(some_slicer_rms_windows_bytes(km)));
+    if (up.reserve(what) || s->rms_d.ensure(4ull * frames + 16, "the RMS frames") ||
+        s->rms_h.ensure(4ull * frames + 16, "the RMS frames"))
+      return -1;
+    float* at = static_cast<float*>(s->rms_d.p);
+    for (some_rms_window& w : rm) w.rms = at, at += w.f_end - w.f_begin;
+    if ((kr && some_resample_windows_pack(rs.data(), kr, up.h(rs_off))) ||
+        (km && some_slicer_rms_windows_pack(rm.data(), km, up.h(rm_off))))
+      return -1;
+    return 0;
+  }
+
+  int launch(some_session* s, const Upload& up) const {
+    if ((!rs.empty() && some_resample_kaiser_windows(up.h(rs_off), up.d(rs_off), s->stream)) ||
+        (!rm.empty() && some_slicer_rms_windows(up.h(rm_off), up.d(rm_off), s->stream)))
+      return -1;
+    if (frames)
+      SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames, cudaMemcpyDeviceToHost, s->stream), "RMS download");
+    return 0;
+  }
+};
 
 // Recordings in the session's recording buffer, each at its own rate and with its own slicer frames, made into chunks and
 // notes together (the sliced and the encoded calls of a step; the step writes the recordings there and may add its own regions
 // to the upload and its own launches and downloads in front of the synchronise):
-//   place   where each recording, its model-rate samples and its RMS frames go; one resampling window per recording at
-//           another rate and one RMS window per recording that is cut, packed into regions added to the upload after the
-//           caller's own, and the upload reserved (the caller fills its regions after this);
-//   launch  after the upload is sent and the recordings are written: one resampling launch, one RMS launch, the RMS download;
+//   place   where each recording and its model-rate samples go; one resampling window per recording at another rate and one
+//           RMS window per recording that is cut, placed in the upload after the caller's own regions (the caller fills its
+//           regions after this, and launches the windows once the upload is sent and the recordings are written);
 //   finish  after the caller's synchronise: each recording's cuts, one batch over all chunks, each recording's notes (a
 //           recording whose `out` has been set to NULL since place, its call refused, is left out).
 struct Recordings {
@@ -1100,9 +1132,7 @@ struct Recordings {
   };
   std::vector<Item> items;
   float* base = nullptr;      // the recording buffer
-  int64_t frames = 0;
-  int kr = 0, km = 0;
-  size_t rs_off = 0, rm_off = 0;
+  StepWindows win;
 
   int place(some_session* s, Upload& up) {
     const int sr = s->info.sample_rate;
@@ -1111,41 +1141,19 @@ struct Recordings {
       it.x = it.y = total;
       total += align4(it.n);
       if (it.rate != sr) it.y = total, total += align4(it.sh.n_out);
-      it.rms0 = frames;
-      frames += it.sh.frames;
     }
-    if (s->rec_d.ensure(4ull * total + 16, "the recordings") || s->rms_d.ensure(4ull * frames + 16, "the RMS frames") ||
-        s->rms_h.ensure(4ull * frames + 16, "the RMS frames"))
-      return -1;
+    if (s->rec_d.ensure(4ull * total + 16, "the recordings")) return -1;
     base = static_cast<float*>(s->rec_d.p);
-    std::vector<some_resample_window> rs;
-    std::vector<some_rms_window> rm;
-    for (const Item& it : items) {
+    for (Item& it : items) {
       if (it.rate != sr) {
         const double* table = table_for(s, it.rate);
         if (!table) return -1;
-        rs.push_back({base + it.x, 0, it.n, 1, base + it.y, 0, 0, it.sh.n_out, it.rate, sr, table, kKaiserTaps});
+        win.rs.push_back({base + it.x, 0, it.n, 1, base + it.y, 0, 0, it.sh.n_out, it.rate, sr, table, kKaiserTaps});
       }
       if (it.sh.frames)
-        rm.push_back({base + it.y, 0, it.sh.n_out, it.sh.n_out, it.sl->win_size, it.sl->hop_size,
-                      static_cast<float*>(s->rms_d.p) + it.rms0, 0, it.sh.frames});
+        it.rms0 = win.rms({base + it.y, 0, it.sh.n_out, it.sh.n_out, it.sl->win_size, it.sl->hop_size, nullptr, 0, it.sh.frames});
     }
-    kr = static_cast<int>(rs.size()), km = static_cast<int>(rm.size());
-    if (kr) rs_off = up.add(static_cast<size_t>(some_resample_windows_bytes(kr)));
-    if (km) rm_off = up.add(static_cast<size_t>(some_slicer_rms_windows_bytes(km)));
-    if (up.reserve("the step's upload") || (kr && some_resample_windows_pack(rs.data(), kr, up.h(rs_off))) ||
-        (km && some_slicer_rms_windows_pack(rm.data(), km, up.h(rm_off))))
-      return -1;
-    return 0;
-  }
-
-  int launch(some_session* s, const Upload& up) const {
-    if ((kr && some_resample_kaiser_windows(up.h(rs_off), up.d(rs_off), s->stream)) ||
-        (km && some_slicer_rms_windows(up.h(rm_off), up.d(rm_off), s->stream)))
-      return -1;
-    if (frames)
-      SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames, cudaMemcpyDeviceToHost, s->stream), "RMS download");
-    return 0;
+    return win.place(s, up, "the step's upload");
   }
 
   int finish(some_session* s) {
@@ -1162,9 +1170,9 @@ struct Recordings {
       it.c1 = static_cast<int>(starts.size());
     }
     const int B = static_cast<int>(starts.size());
-    if (B && run_chunks(s, nullptr, base, starts.data(), lens.data(), B, &s->chunks)) return -1;
+    if (B && run_chunks(s, nullptr, base, starts.data(), lens.data(), B)) return -1;
     for (const Item& it : items)
-      if (it.out) take_chunks(s->chunks, it.c0, it.c1, begin.data(), lens.data(), it.out);
+      if (it.out) take_chunks(s, it.c0, it.c1, begin.data(), lens.data(), it.out);
     return 0;
   }
 };
@@ -1294,13 +1302,18 @@ struct StepItem {
 // encoded calls tell the two paths apart.
 bool pcm_container(const some_audio_meta& m) { return m.container != SOME_AUDIO_FLAC; }
 
+// Accepts audio at `rate` for a session at rate `sr`, or refuses a rate pair the resampler does not support (with
+// some_resample_window_plan's message).
+int check_rates(int rate, int sr) {
+  long long t_end, x_first;
+  return rate != sr && some_resample_window_plan(0, 0, 0, rate, sr, kKaiserTaps, &t_end, &x_first) ? -1 : 0;
+}
+
 // Accepts a container's format for a session at rate `sr`, or refuses it (the message has no prefix): a PCM file's mono
 // down-mix takes at most 128 channels, and the resampler must support the rate pair.
 int check_format(const some_audio_meta& m, int sr) {
   SOME_REQUIRE(!pcm_container(m) || m.channels <= 128, "a mono down-mix of %d channels (at most 128)", m.channels);
-  long long t_end, x_first;
-  if (m.rate != sr && some_resample_window_plan(0, 0, 0, m.rate, sr, kKaiserTaps, &t_end, &x_first)) return -1;
-  return 0;
+  return check_rates(m.rate, sr);
 }
 // One window of a call's audio bytes (a file's data chunk, a stream's pending bytes), with its container's metadata.
 struct ByteWindow {
@@ -1481,10 +1494,9 @@ struct Decode {
 //   4. every chunk that became final, in any stream, copied next to each other and transcribed as one batch.
 int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nullptr) {
   const int sr = s->info.sample_rate;
-  std::vector<some_resample_window> rs;
-  std::vector<some_rms_window> rm;
+  StepWindows win;
   std::vector<ScatterParams> sc;
-  int64_t up_floats = 0, frames = 0;
+  int64_t up_floats = 0;
   for (StepItem& it : items) {
     some_stream* st = it.st;
     const some_slicer_frames& f = st->f;
@@ -1514,8 +1526,8 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
       st->native.len += it.n, st->received += it.n;
       if (some_resample_window_plan(st->received, it.final, st->fixed, st->rate, sr, kKaiserTaps, &t_end, &x_first)) return -1;
       if (st->wave.reserve(s->stream, keep, t_end - st->fixed, "the stream's audio")) return -1;
-      rs.push_back({st->native.at(st->native.first), st->native.first, st->received, it.final, st->wave.at(st->wave.first),
-                    st->wave.first, st->fixed, t_end, st->rate, sr, table, kKaiserTaps});
+      win.rs.push_back({st->native.at(st->native.first), st->native.first, st->received, it.final, st->wave.at(st->wave.first),
+                        st->wave.first, st->fixed, t_end, st->rate, sr, table, kKaiserTaps});
       st->wave.len += t_end - st->fixed, st->fixed = t_end;
     } else {
       if (st->wave.reserve(s->stream, keep, it.n, "the stream's audio")) return -1;
@@ -1524,33 +1536,25 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
     }
     if (it.n) {
       it.up = up_floats;
-      up_floats += (it.n + 3) & ~int64_t(3);         // 16-byte aligned
+      up_floats += align4(it.n);
       sc.push_back({nullptr, dst, it.n});
     }
     // the RMS frames the fixed samples complete (at the end: all of them, unless the recording is one chunk anyway)
-    const int64_t hop = f.hop_size;
-    int64_t f_end = frames_within(f, st->fixed);
-    if (it.final && (st->fixed + hop - 1) / hop > f.min_length) f_end = 1 + (st->fixed + 2 * (f.win_size / 2) - f.win_size) / hop;
+    int64_t f_end = it.final ? frames_whole(f, st->fixed) : 0;
+    if (f_end == 0) f_end = frames_within(f, st->fixed);
     it.nf = std::max<int64_t>(0, f_end - st->frames);
-    it.rms0 = frames;
-    if (it.nf) {
-      rm.push_back({st->wave.at(st->wave.first), st->wave.first, st->wave.len, it.final ? st->fixed : -1, f.win_size,
-                    f.hop_size, nullptr, st->frames, st->frames + it.nf});
-      frames += it.nf;
-    }
+    if (it.nf)
+      it.rms0 = win.rms({st->wave.at(st->wave.first), st->wave.first, st->wave.len, it.final ? st->fixed : -1, f.win_size,
+                         f.hop_size, nullptr, st->frames, st->frames + it.nf});
   }
 
-  // the upload: samples, then the scatter, resampling and RMS descriptors
-  const int ks = static_cast<int>(sc.size()), kr = static_cast<int>(rs.size()), km = static_cast<int>(rm.size());
+  // the upload: samples, then the scatter, the decode's and the windows' descriptors
+  const int ks = static_cast<int>(sc.size());
   Upload up{s};
   const size_t smp_off = up.add(4ull * up_floats);
   const size_t sc_off = up.add(windows_bytes<ScatterParams>(ks));
-  const size_t rs_off = up.add(static_cast<size_t>(some_resample_windows_bytes(kr)));
-  const size_t rm_off = up.add(static_cast<size_t>(some_slicer_rms_windows_bytes(km)));
   if (dec) dec->add(up);
-  if (up.reserve("the stream upload") || s->rms_d.ensure(4ull * frames + 16, "the RMS frames") ||
-      s->rms_h.ensure(4ull * frames + 16, "the RMS frames"))
-    return -1;
+  if (win.place(s, up, "the stream upload")) return -1;
   std::vector<HostSpan> spans;
   {
     ScatterParams* ps = windows_params<ScatterParams>(up.h(sc_off), ks);
@@ -1566,10 +1570,6 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
       }
     windows_index(up.h(sc_off), ks, 0);
   }
-  for (int j = 0, at = 0; j < km; at += static_cast<int>(rm[j].f_end - rm[j].f_begin), ++j)   // in item order, as rms0
-    rm[j].rms = static_cast<float*>(s->rms_d.p) + at;
-  if (some_resample_windows_pack(rs.data(), kr, up.h(rs_off)) || some_slicer_rms_windows_pack(rm.data(), km, up.h(rm_off)))
-    return -1;
   float* samples_d = reinterpret_cast<float*>(up.d(smp_off));
   if (dec && dec->fill(s, up, samples_d, [&](int j) { return items[j].up; })) return -1;
   copy_to_pinned(*s->pool, spans, size_t(1) << 20);          // the samples, in pieces of up to 1 MB
@@ -1580,11 +1580,7 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
         windows_params<ScatterParams>(up.d(sc_off), ks), windows_tile0(up.d(sc_off)), ks);
     if (check_launch("stream upload scatter")) return -1;
   }
-  if (some_resample_kaiser_windows(up.h(rs_off), up.d(rs_off), s->stream) ||
-      some_slicer_rms_windows(up.h(rm_off), up.d(rm_off), s->stream))
-    return -1;
-  if (frames)
-    SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames, cudaMemcpyDeviceToHost, s->stream), "RMS download");
+  if (win.launch(s, up)) return -1;
   SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");   // also frees the upload buffer for the next step
   if (dec) {
     std::vector<std::pair<int, std::string>> failed;
@@ -1626,16 +1622,16 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
   if (B) {                                          // the chunks side by side in the audio buffer, then one batch
     std::vector<int64_t> starts(B);
     int64_t total = 0;
-    for (int c = 0; c < B; ++c) starts[c] = total, total += (lens[c] + 3) & ~int64_t(3);
+    for (int c = 0; c < B; ++c) starts[c] = total, total += align4(lens[c]);
     DevBuf& chunks_d = s->reps[0]->wave_d;
     if (chunks_d.ensure(4ull * total + 16, "the audio")) return -1;
     float* wave = static_cast<float*>(chunks_d.p);
     for (int c = 0; c < B; ++c)
       if (lens[c])
         SOME_CUDA(cudaMemcpyAsync(wave + starts[c], src[c], 4ull * lens[c], cudaMemcpyDeviceToDevice, s->stream), "chunk copy");
-    if (run_chunks(s, nullptr, wave, starts.data(), lens.data(), B, &s->chunks)) return -1;
+    if (run_chunks(s, nullptr, wave, starts.data(), lens.data(), B)) return -1;
   }
-  for (const StepItem& it : items) take_chunks(s->chunks, it.c0, it.c1, begin.data(), lens.data(), it.out);
+  for (const StepItem& it : items) take_chunks(s, it.c0, it.c1, begin.data(), lens.data(), it.out);
   return 0;
 }
 
@@ -1689,7 +1685,7 @@ int bytes_step(some_session* s, std::vector<ByteItem>& bs) {
   };
   auto too_short = [&](ByteItem& b) {    // resampy's refusal, at the end of a file at another rate
     const some_stream* st = b.st;
-    if (!b.final || !st->resample || (st->received + b.samples) * sr / st->rate >= 1) return false;
+    if (!b.final || !too_short_to_resample(st->received + b.samples, st->rate, sr)) return false;
     set_error("Input signal length=%lld is too small to resample from %d->%d", static_cast<long long>(st->received + b.samples),
               st->rate, sr);
     refuse(b);
@@ -1844,7 +1840,7 @@ int check_many(some_stream* const* streams, const T* const* data, const long lon
     const auto shared = seen_notes.emplace(out[i], i);
     SOME_REQUIRE(shared.second, "%s: stream %d shares its some_notes with stream %d", who, i, shared.first->second);
     const int sr = s->info.sample_rate;                                 // a PCM stream's end at another rate
-    SOME_REQUIRE(encoded || !(finish && finish[i]) || !st->resample || (st->received + n[i]) * sr / st->rate >= 1,
+    SOME_REQUIRE(encoded || !(finish && finish[i]) || !too_short_to_resample(st->received + n[i], st->rate, sr),
                  "%s: stream %d: Input signal length=%lld is too small to resample from %d->%d", who, i,
                  (long long)(st->received + n[i]), st->rate, sr);
   }
@@ -1857,10 +1853,7 @@ extern "C" int some_stream_open(some_session* s, int sample_rate, const some_sli
   *out = nullptr;
   some_slicer_frames sl;
   if (some_slicer_derive(s->info.sample_rate, params, &sl)) return -1;
-  if (sample_rate != s->info.sample_rate) {          // refuses rate pairs the resampler does not support, before any push
-    long long t_end, x_first;
-    if (some_resample_window_plan(0, 0, 0, sample_rate, s->info.sample_rate, kKaiserTaps, &t_end, &x_first)) return -1;
-  }
+  if (check_rates(sample_rate, s->info.sample_rate)) return -1;     // before any push
   some_slicer_stream* slicer;
   if (some_slicer_stream_create(&sl, &slicer)) return -1;
   some_stream* st = new some_stream();
@@ -1884,7 +1877,7 @@ extern "C" int some_stream_finish(some_stream* st, some_notes* out) {
   SOME_REQUIRE(!st->finished, "some_stream_finish: the stream has finished");
   if (st->walk) return bytes_call(st, nullptr, 0, true, out, "some_stream_finish");
   const int sr = st->s->info.sample_rate;
-  SOME_REQUIRE(!st->resample || st->received * sr / st->rate >= 1,
+  SOME_REQUIRE(!too_short_to_resample(st->received, st->rate, sr),
                "some_stream_finish: Input signal length=%lld is too small to resample from %d->%d", (long long)st->received,
                st->rate, sr);
   st->finished = true;
@@ -2066,17 +2059,15 @@ int recordings_step(some_session* s, const std::vector<Request*>& g) {
   if (encoded) dec.add(up);
   if (rec.place(s, up)) return -1;
   std::vector<Staged> staged;
-  bool cut = false;
   for (size_t j = 0; j < rec.items.size(); ++j) {
     const RecItem& it = item(refs[ref_of[j]]);
     if (it.host) staged.push_back({rec.base + rec.items[j].x, it.host, it.n});
-    cut |= rec.items[j].sh.frames > 0;
   }
   if ((!staged.empty() && upload_staged(s, staged)) ||
       (encoded && dec.fill(s, up, rec.base, [&](int j) { return rec.items[j].x; })) || up.send("descriptor upload") ||
-      (encoded && dec.launch(s, up)) || rec.launch(s, up))
+      (encoded && dec.launch(s, up)) || rec.win.launch(s, up))
     return -1;
-  if (encoded || cut) SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
+  if (encoded || rec.win.frames) SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");   // with a recording to cut
   if (encoded) {
     std::vector<std::pair<int, std::string>> failed;
     if (dec.check(s, up, failed)) return -1;
@@ -2139,10 +2130,10 @@ int clips_step(some_session* s, const std::vector<Request*>& g) {
   std::vector<int64_t> lens;
   for (const Request* rq : g) clips.insert(clips.end(), rq->clips, rq->clips + rq->B), lens.insert(lens.end(), rq->lens, rq->lens + rq->B);
   const int B = static_cast<int>(lens.size());
-  if (run_chunks(s, clips.data(), nullptr, nullptr, lens.data(), B, &s->chunks)) return -1;
+  if (run_chunks(s, clips.data(), nullptr, nullptr, lens.data(), B)) return -1;
   const std::vector<int64_t> begin(B, 0);
   int c = 0;
-  for (const Request* rq : g) take_chunks(s->chunks, c, c + rq->B, begin.data(), lens.data(), rq->out), c += rq->B;
+  for (const Request* rq : g) take_chunks(s, c, c + rq->B, begin.data(), lens.data(), rq->out), c += rq->B;
   return 0;
 }
 

@@ -486,13 +486,12 @@ int slicer_finish(some_slicer_stream* st, const float* rms, int64_t n, int64_t n
   st->fixed = n_samples;
   st->finished = true;
   if (st->core.feed(rms, n, st->queued)) return -1;
-  const int64_t hop = st->f.hop_size;
-  if ((n_samples + hop - 1) / hop <= st->f.min_length) {   // one chunk (slicer2.py:79-80)
+  const int64_t total = frames_whole(st->f, n_samples);
+  if (total == 0) {                                       // one chunk
     st->queued.clear();
     st->out = {0, n_samples};
     return 0;
   }
-  const int64_t total = 1 + (n_samples + 2 * (st->f.win_size / 2) - st->f.win_size) / hop;
   SOME_REQUIRE(st->core.known() == total, "some_slicer_stream_finish: %lld of the %lld frames of %lld samples were fed",
                (long long)st->core.known(), (long long)total, (long long)n_samples);
   if (st->core.finish(st->queued)) return -1;

@@ -96,6 +96,7 @@ def test_transcribe(pair):
     clips += [np.zeros(0, np.float32), synth.synth_waveform(77, num_samples=2047), synth.synth_waveform(78, num_samples=513)]
     for batch in (clips, clips[:1], clips[-1:], clips[-3:-2], [clips[3]] * 5):
         want = transcribe(first, batch)
+        assert_split(first, [len(c) for c in batch])
         got = transcribe(many, batch)
         assert got[0] == want[0]
         assert_same_notes(got[1], want[1])
