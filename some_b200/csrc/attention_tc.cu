@@ -66,6 +66,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmq0, const __grid_const
   const int grp = blockIdx.z;
   const CUtensorMap* tmq = grp == 0 ? &tmq0 : &tmq1;
   const CUtensorMap* tmkv = grp == 0 ? &tmkv0 : &tmkv1;
+  __nv_bfloat16* out = grp == 0 ? p.out[0] : p.out[1];   // no dynamic index into the parameter space (a local copy)
   const int n_tiles = (T + TC_BN - 1) / TC_BN;
 
   if (threadIdx.x == 0) {
@@ -185,7 +186,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmq0, const __grid_const
     const float inv = 1.0f / lt;
     const int qrow = q0 + r + 8 * h;
     if (qrow < T) {
-      __nv_bfloat16* dst = p.out[grp] + (size_t)(row_begin + qrow) * SOME_DIM + head * 64 + 2 * q;
+      __nv_bfloat16* dst = out + (size_t)(row_begin + qrow) * SOME_DIM + head * 64 + 2 * q;
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj)
         *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);

@@ -14,6 +14,8 @@
 //   5. mel[m] = sum over the filter's contiguous bin range (<= 24 bins), log(max(., clamp)); lane m, m + 32, m + 64.
 // No CTA barrier after the table load; a CTA is just MEL_WARPS independent warps sharing the 19 KB of tables.
 // Algorithmic traffic: 512 x 4 B in + 80 x 4 B out per frame (2368 B); ~60 kFLOP per frame keep it issue-bound.
+// On an H100 80GB HBM3 (700 W) one 64 x 30 s batch takes 0.61 ms (bench_rowwise.py); while c[] of the DFTs sat in local
+// memory (a 336-byte stack frame and spills, see dif_butterflies) it took 3.67 ms.
 #include "host_common.h"
 #include "sm90_ptx.cuh"
 
@@ -21,7 +23,7 @@
 
 namespace some {
 
-constexpr int MEL_WARPS = 4;                   // warps per CTA
+constexpr int MEL_WARPS = 8;                   // warps per CTA
 constexpr int MEL_FPW = 8;                     // consecutive frames per warp (75 % of a frame's samples are L1 hits)
 constexpr int MEL_FPB = MEL_WARPS * MEL_FPW;   // frames per CTA
 constexpr int MEL_MAXW = SOME_MEL_MAXW;
@@ -45,30 +47,49 @@ __device__ constexpr float kS32[16] = {0.0f,          -0.19509032f, -0.38268343f
                                        -0.92387953f,  -0.98078528f, -1.0f,        -0.98078528f, -0.92387953f, -0.83146961f,
                                        -0.70710678f,  -0.55557023f, -0.38268343f, -0.19509032f};
 
-// In-place 32-point radix-2 DIF DFT, fully unrolled (all indices and twiddles are compile-time): c[i] ends up holding
-// X[bitrev5(i)].
-__device__ __forceinline__ void dft32(cpx (&c)[32]) {
-#pragma unroll
-  for (int s = 0; s < 5; ++s) {
-    const int half = 16 >> s;
-#pragma unroll
-    for (int g = 0; g < 32; g += 2 * half) {
-#pragma unroll
-      for (int j = 0; j < half; ++j) {
-        const cpx a = c[g + j], b = c[g + j + half];
-        c[g + j] = cadd(a, b);
-        const cpx d = csub(a, b);
-        const int t = j * (16 / half);   // W_(2 half)^j = W_32^t
-        if (t == 0) {
-          c[g + j + half] = d;
-        } else if (t == 8) {             // -i
-          c[g + j + half] = {d.y, -d.x};
-        } else {
-          c[g + j + half] = cmul(d, kC32[t], kS32[t]);
-        }
-      }
+// Twiddle multiply of a DFT butterfly, W_32^t with T = t known at compile time, its rounding spelled out so that it does
+// not depend on how the compiler contracts the products (that changes with whether the twiddle is a constant or a load):
+// re = fma(x, wr, -(y wi)), im = fma(y, wr, x wi).  For W_32^12 in the span-4 stage, where wr = wi, the product x wr is
+// the one that is rounded: re = fma(y, -wi, x wr).  These are the roundings of the earlier form of this kernel, kept so
+// that its outputs stay the same bits.
+template <int HALF, int T>
+__device__ __forceinline__ cpx twiddle(cpx d) {
+  const float wr = kC32[T], wi = kS32[T];
+  if (HALF == 4 && T == 12) return {__fmaf_rn(d.y, -wi, __fmul_rn(d.x, wr)), __fmaf_rn(d.y, wr, __fmul_rn(d.x, wi))};
+  return {__fmaf_rn(d.x, wr, -__fmul_rn(d.y, wi)), __fmaf_rn(d.y, wr, __fmul_rn(d.x, wi))};
+}
+// One radix-2 DIF stage of butterflies HALF apart.  HALF and j are template arguments, so every register index and twiddle
+// is a compile-time constant: with the stage span derived from an unrolled outer loop instead, the compiler unrolled the
+// inner loop by 4 before the outer one, indexed c[] at run time and put it in local memory.
+template <int HALF, int J = 0>
+__device__ __forceinline__ void dif_butterflies(cpx (&c)[32], int g) {
+  if constexpr (J < HALF) {
+    const cpx a = c[g + J], b = c[g + J + HALF];
+    c[g + J] = cadd(a, b);
+    const cpx d = csub(a, b);
+    constexpr int t = J * (16 / HALF);   // W_(2 HALF)^J = W_32^t
+    if constexpr (t == 0) {
+      c[g + J + HALF] = d;
+    } else if constexpr (t == 8) {       // -i
+      c[g + J + HALF] = {d.y, -d.x};
+    } else {
+      c[g + J + HALF] = twiddle<HALF, t>(d);
     }
+    dif_butterflies<HALF, J + 1>(c, g);
   }
+}
+template <int HALF>
+__device__ __forceinline__ void dif_stage(cpx (&c)[32]) {
+#pragma unroll
+  for (int g = 0; g < 32; g += 2 * HALF) dif_butterflies<HALF>(c, g);
+}
+// In-place 32-point radix-2 DIF DFT, fully unrolled: c[i] ends up holding X[bitrev5(i)].
+__device__ __forceinline__ void dft32(cpx (&c)[32]) {
+  dif_stage<16>(c);
+  dif_stage<8>(c);
+  dif_stage<4>(c);
+  dif_stage<2>(c);
+  dif_stage<1>(c);
 }
 __device__ __forceinline__ constexpr int bitrev5(int i) {
   return ((i & 1) << 4) | ((i & 2) << 2) | (i & 4) | ((i & 8) >> 2) | ((i & 16) >> 4);
@@ -76,9 +97,19 @@ __device__ __forceinline__ constexpr int bitrev5(int i) {
 // warp-private 32 x 32 complex tile, element (row, col) with the column XOR-swizzled by the row: a lane writing its 32
 // values down a column and a lane reading its 32 values along a row are both conflict-free (8-byte accesses, half-warps)
 __device__ __forceinline__ int tsw(int row, int col) { return row * 32 + (col ^ row); }
+// The lane index, read afresh where it is called: the 64 swizzled tile addresses of steps 2 and 3 are then formed in each
+// frame next to their use instead of being hoisted out of the frame loop, where they held ~40 registers for the whole
+// kernel and pushed it into spills at the register budget of 3 CTAs per SM.
+__device__ __forceinline__ int lane_now() {
+  int l;
+  asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));
+  return l;
+}
 
+// 2 CTAs x 8 warps per SM: at most 128 registers per thread (no stack frame, no spills) and 2 x 92 KB of shared
+// memory, which needs the maximum shared-memory carveout (set at the first launch, checked with the occupancy calculator).
 #ifndef MEL_MIN_CTAS
-#define MEL_MIN_CTAS 3   // 168 registers, 12 warps / SM: 0.70 ms per 64 x 30 s batch; 4 (128 registers, spills) measured 0.79 ms
+#define MEL_MIN_CTAS 2
 #endif
 __global__ void __launch_bounds__(MEL_WARPS * 32, MEL_MIN_CTAS)
 mel_kernel(const float* __restrict__ wave, const int64_t* __restrict__ clip_start, const int64_t* __restrict__ clip_len,
@@ -154,24 +185,25 @@ mel_kernel(const float* __restrict__ wave, const int64_t* __restrict__ clip_star
 #pragma unroll
     for (int n1 = 0; n1 < 32; ++n1) {
       const float2 wv = *reinterpret_cast<const float2*>(s_win + 64 * n1 + 2 * lane);
-      c[n1].x *= wv.x;
-      c[n1].y *= wv.y;
+      c[n1].x = __fmul_rn(c[n1].x, wv.x);   // a rounded product: not fused into the first butterfly's add
+      c[n1].y = __fmul_rn(c[n1].y, wv.y);
     }
     dft32(c);
     // ---- 2. twiddle W_1024^(n2 k1) and transpose: register i holds k1 = bitrev5(i)
     __syncwarp();   // the previous frame's mel pass has finished reading the tile
+    const int ln = lane_now();
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int k1 = bitrev5(i);
-      const float2 w = s_tw[k1 * 32 + lane];
+      const float2 w = s_tw[k1 * 32 + ln];
       const cpx v = cmul(c[i], w.x, w.y);
-      tile_z[tsw(k1, lane)] = make_float2(v.x, v.y);
+      tile_z[tsw(k1, ln)] = make_float2(v.x, v.y);
     }
     __syncwarp();
     // ---- 3. second DFT (over n2, lane = k1)
 #pragma unroll
     for (int n2 = 0; n2 < 32; ++n2) {
-      const float2 v = tile_z[tsw(lane, n2)];
+      const float2 v = tile_z[tsw(ln, n2)];
       c[n2] = {v.x, v.y};
     }
     dft32(c);
@@ -211,10 +243,13 @@ mel_kernel(const float* __restrict__ wave, const int64_t* __restrict__ clip_star
       if (m < SOME_N_MELS) {
         // all MEL_MAXW taps, unrolled: the weights beyond the filter's width are zero (the bin index is clamped so that the
         // zero always multiplies a finite magnitude); ascending bins, one fma chain = the order of the round-1 kernel
+        // (st is made opaque per frame so that the 24 clamped bin addresses are formed here, not kept for the whole loop)
+        int st = m_st[i];
+        asm volatile("" : "+r"(st));
         float acc = 0.f;
 #pragma unroll
         for (int j = 0; j < MEL_MAXW; ++j)
-          acc = fmaf(s_mw[j * MEL_WSTRIDE + m], mag[min(m_st[i] + j, SOME_MEL_BINS - 1)], acc);
+          acc = fmaf(s_mw[j * MEL_WSTRIDE + m], mag[min(st + j, SOME_MEL_BINS - 1)], acc);
         const float v = logf(fmaxf(acc, clamp));
         const size_t o = static_cast<size_t>(row_begin + f) * SOME_N_MELS + m;
         if (out_f32 != nullptr) out_f32[o] = v;
@@ -322,6 +357,12 @@ extern "C" int some_mel_logmel(const float* wave, const int64_t* clip_start, con
   if (!configured[dev_]) {
     cudaError_t e = cudaFuncSetAttribute(mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MEL_SMEM);
     SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(mel): %s", cudaGetErrorString(e));
+    e = cudaFuncSetAttribute(mel_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(mel carveout): %s", cudaGetErrorString(e));
+    int ctas = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, mel_kernel, MEL_WARPS * 32, MEL_SMEM);
+    SOME_REQUIRE(e == cudaSuccess && ctas >= MEL_MIN_CTAS, "some_mel_logmel: %d CTAs per SM, the kernel is built for %d (%s)",
+                 ctas, MEL_MIN_CTAS, cudaGetErrorString(e));
     configured[dev_] = true;
   }
   const int tiles_per_clip = (max_frames + MEL_FPB - 1) / MEL_FPB;

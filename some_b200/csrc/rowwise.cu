@@ -65,15 +65,15 @@ __device__ __forceinline__ void ln_row(const float* __restrict__ xr, const float
   ln_load(xr, lane, v);
   ln_normalise(v, gamma, beta, lane, y);
 }
-__device__ __forceinline__ void ln_store(const LnParams& p, int grp, int row, int lane, const float (&y)[16]) {
-  if (p.out_f32[grp] != nullptr) {
-    float* o = p.out_f32[grp] + (size_t)row * D;
+__device__ __forceinline__ void ln_store(float* out_f32, __nv_bfloat16* out_bf16, int row, int lane, const float (&y)[16]) {
+  if (out_f32 != nullptr) {
+    float* o = out_f32 + (size_t)row * D;
 #pragma unroll
     for (int i = 0; i < 4; ++i)
       *reinterpret_cast<float4*>(o + 128 * i + 4 * lane) = make_float4(y[4 * i], y[4 * i + 1], y[4 * i + 2], y[4 * i + 3]);
   }
-  if (p.out_bf16[grp] != nullptr) {
-    __nv_bfloat16* o = p.out_bf16[grp] + (size_t)row * D;
+  if (out_bf16 != nullptr) {
+    __nv_bfloat16* o = out_bf16 + (size_t)row * D;
 #pragma unroll
     for (int i = 0; i < 4; ++i)
       *reinterpret_cast<uint2*>(o + 128 * i + 4 * lane) =
@@ -83,9 +83,16 @@ __device__ __forceinline__ void ln_store(const LnParams& p, int grp, int row, in
 
 // Each warp streams LN_RPW rows per pass with all their loads issued up front (128 B per lane in flight): the kernel is a
 // pure HBM stream and memory-level parallelism is what sets its bandwidth.
+// The group's pointers are selected with a conditional, not by indexing p.x[grp] with the runtime grp: a dynamic index into
+// the parameter space makes every thread copy the whole struct to local memory first (as in gemm.cu).
 constexpr int LN_RPW = 2;
-__global__ void __launch_bounds__(256) layernorm_kernel(const LnParams p) {
-  const int grp = blockIdx.y;
+__global__ void __launch_bounds__(256, 4) layernorm_kernel(const LnParams p) {   // 4 CTAs = 32 warps per SM
+  const bool g1 = blockIdx.y != 0;
+  const float* __restrict__ x = g1 ? p.x[1] : p.x[0];
+  const float* __restrict__ gamma = g1 ? p.gamma[1] : p.gamma[0];
+  const float* __restrict__ beta = g1 ? p.beta[1] : p.beta[0];
+  float* out_f32 = g1 ? p.out_f32[1] : p.out_f32[0];
+  __nv_bfloat16* out_bf16 = g1 ? p.out_bf16[1] : p.out_bf16[0];
   const int lane = threadIdx.x & 31;
   const int row0 = (blockIdx.x * 8 + (threadIdx.x >> 5)) * LN_RPW;
   griddep_launch();   // programmatic dependent launch (host_common.h)
@@ -94,13 +101,13 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const LnParams p) {
   float v[LN_RPW][16];
 #pragma unroll
   for (int r = 0; r < LN_RPW; ++r)
-    if (row0 + r < p.M) ln_load(p.x[grp] + (size_t)(row0 + r) * D, lane, v[r]);
+    if (row0 + r < p.M) ln_load(x + (size_t)(row0 + r) * D, lane, v[r]);
 #pragma unroll
   for (int r = 0; r < LN_RPW; ++r) {
     if (row0 + r < p.M) {
       float y[16];
-      ln_normalise(v[r], p.gamma[grp], p.beta[grp], lane, y);
-      ln_store(p, grp, row0 + r, lane, y);
+      ln_normalise(v[r], gamma, beta, lane, y);
+      ln_store(out_f32, out_bf16, row0 + r, lane, y);
     }
   }
 }
@@ -115,14 +122,17 @@ struct RowStatsParams {
   int M;
 };
 __global__ void __launch_bounds__(256) row_stats_kernel(const RowStatsParams p) {
-  const int grp = blockIdx.y;
+  const bool g1 = blockIdx.y != 0;   // pointer select without a dynamic parameter index (see layernorm_kernel)
+  const float* __restrict__ x = g1 ? p.x[1] : p.x[0];
+  __nv_bfloat16* out_bf16 = g1 ? p.out_bf16[1] : p.out_bf16[0];
+  float* stats = g1 ? p.stats[1] : p.stats[0];
   const int lane = threadIdx.x & 31;
   const int row0 = (blockIdx.x * 8 + (threadIdx.x >> 5)) * LN_RPW;
   if (row0 >= p.M) return;
   float v[LN_RPW][16];
 #pragma unroll
   for (int r = 0; r < LN_RPW; ++r)
-    if (row0 + r < p.M) ln_load(p.x[grp] + (size_t)(row0 + r) * D, lane, v[r]);
+    if (row0 + r < p.M) ln_load(x + (size_t)(row0 + r) * D, lane, v[r]);
 #pragma unroll
   for (int r = 0; r < LN_RPW; ++r) {
     if (row0 + r < p.M) {
@@ -134,13 +144,13 @@ __global__ void __launch_bounds__(256) row_stats_kernel(const RowStatsParams p) 
       }
       s = warp_sum(s);
       q = warp_sum(q);
-      __nv_bfloat16* o = p.out_bf16[grp] + (size_t)(row0 + r) * D;
+      __nv_bfloat16* o = out_bf16 + (size_t)(row0 + r) * D;
 #pragma unroll
       for (int i = 0; i < 4; ++i)
         *reinterpret_cast<uint2*>(o + 128 * i + 4 * lane) =
             make_uint2(pack_bf16x2(v[r][4 * i], v[r][4 * i + 1]), pack_bf16x2(v[r][4 * i + 2], v[r][4 * i + 3]));
       if (lane == 0)
-        reinterpret_cast<float2*>(p.stats[grp])[(size_t)(row0 + r) * SOME_LN_SLOTS] = make_float2(s, q);
+        reinterpret_cast<float2*>(stats)[(size_t)(row0 + r) * SOME_LN_SLOTS] = make_float2(s, q);
     }
   }
 }
@@ -230,10 +240,12 @@ struct DwParams {
 
 __global__ void __launch_bounds__(256) dwconv_kernel(const DwParams p) {
   __shared__ __align__(16) __nv_bfloat16 tile[2][DW_ROWS * DW_C];
-  const int grp = blockIdx.z;
+  const bool g1 = blockIdx.z != 0;   // pointer select without a dynamic parameter index (see layernorm_kernel)
   const int c0 = blockIdx.y * DW_C;
-  const __nv_bfloat16* __restrict__ x = p.x[grp];
-  __nv_bfloat16* __restrict__ out = p.out[grp];
+  const __nv_bfloat16* __restrict__ x = g1 ? p.x[1] : p.x[0];
+  __nv_bfloat16* __restrict__ out = g1 ? p.out[1] : p.out[0];
+  const float* __restrict__ wg = g1 ? p.w[1] : p.w[0];
+  const float* __restrict__ bg = g1 ? p.b[1] : p.b[0];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int c = c0 + 2 * lane;
 
@@ -262,8 +274,8 @@ __global__ void __launch_bounds__(256) dwconv_kernel(const DwParams p) {
   // fp32 pairs: {a[c], a[c+1]} += {w[c], w[c+1]} * {x[c], x[c+1]}
   uint64_t w[SOME_CONV_K];
 #pragma unroll
-  for (int k = 0; k < SOME_CONV_K; ++k) w[k] = __ldg(reinterpret_cast<const unsigned long long*>(p.w[grp] + k * D + c));
-  const uint64_t bb = __ldg(reinterpret_cast<const unsigned long long*>(p.b[grp] + c));
+  for (int k = 0; k < SOME_CONV_K; ++k) w[k] = __ldg(reinterpret_cast<const unsigned long long*>(wg + k * D + c));
+  const uint64_t bb = __ldg(reinterpret_cast<const unsigned long long*>(bg + c));
   griddep_launch();   // programmatic dependent launch: the taps (weights) are loaded, activations only after the wait
   griddep_wait();
 
