@@ -1,8 +1,8 @@
 /* some_stream: transcribe a recording while it arrives, with a model file written by `python -m some_b200.export`, without
  * Python.
  *
- *   some_stream MODEL RATE [DEVICES] < pcm
- *   some_stream MODEL - [DEVICES] < file.wav, file.flac or file.aif
+ *   some_stream [--peek MS] MODEL RATE [DEVICES] < pcm
+ *   some_stream [--peek MS] MODEL - [DEVICES] < file.wav, file.flac or file.aif
  *
  * With RATE, reads raw mono little-endian float32 samples at RATE Hz from stdin in blocks of 100 ms and pushes each block to a
  * some_stream.  With `-`, reads a WAV, FLAC or AIFF byte stream from stdin in 64 KB reads and pushes each read to an encoded
@@ -11,7 +11,13 @@
  *
  *   <chunk offset in seconds> <note_midi> <duration in seconds> <rest 0/1>
  *
- * the same lines examples/some_transcribe prints for the whole recording.  Live from a microphone:
+ * the same lines examples/some_transcribe prints for the whole recording.  With --peek MS, after each push that completes
+ * another MS milliseconds of audio (at most one peek per push), it also prints the provisional notes of the part of the
+ * recording no chunk has covered yet (some_stream_peek), in the same format with "~ " in front:
+ *
+ *   ~ <region offset in seconds> <note_midi> <duration in seconds> <rest 0/1>
+ *
+ * A later peek or the delivered chunk replaces them.  Live from a microphone:
  *
  *   arecord -f FLOAT_LE -c1 -r 44100 | some_stream model.somemodel 44100
  *   arecord -f S16_LE -c2 -r 48000 -t wav | some_stream model.somemodel - */
@@ -36,7 +42,7 @@ static int parse_devices(const char* list, int* devices) {
   }
 }
 
-static void print_chunks(const some_notes* notes, const some_session_info* info) {
+static void print_chunks(const some_notes* notes, const some_session_info* info, const char* prefix) {
   const int chunks = some_notes_clips(notes);
   for (int c = 0; c < chunks; ++c) {
     int count = 0;
@@ -47,13 +53,28 @@ static void print_chunks(const some_notes* notes, const some_session_info* info)
     some_notes_get(notes, c, &count, &midi, &dur, &rest, &begin, &end);
     const double offset = (double)begin / info->sample_rate;
     for (int k = 0; k < count; ++k)
-      printf("%.17g %.9g %.17g %d\n", offset, midi[k], (double)dur[k] * info->timestep, rest[k] ? 1 : 0);
+      printf("%s%.17g %.9g %.17g %d\n", prefix, offset, midi[k], (double)dur[k] * info->timestep, rest[k] ? 1 : 0);
   }
   fflush(stdout);
 }
 
+/* --peek MS: peeks and prints once `received` samples at `rate` reach the next multiple of MS milliseconds (peek_ms 0: never). */
+typedef struct {
+  int peek_ms;
+  long long next_ms;
+  some_notes* notes;
+} peeker;
+
+static int maybe_peek(peeker* p, some_stream* st, long long received, int rate, const some_session_info* info) {
+  if (p->peek_ms <= 0 || rate <= 0 || received * 1000 < p->next_ms * rate) return 0;
+  if (some_stream_peek(st, p->notes) != 0) return -1;
+  print_chunks(p->notes, info, "~ ");
+  p->next_ms = (received * 1000 / rate / p->peek_ms + 1) * p->peek_ms;
+  return 0;
+}
+
 /* `-`: the bytes of a WAV, FLAC or AIFF file from stdin, 64 KB per push. */
-static int run_encoded(some_session* s, const some_session_info* info) {
+static int run_encoded(some_session* s, const some_session_info* info, peeker* pk) {
   static unsigned char buf[1 << 16];
   some_stream* st = NULL;
   some_notes* notes = NULL;
@@ -63,14 +84,19 @@ static int run_encoded(some_session* s, const some_session_info* info) {
     const size_t got = fread(buf, 1, sizeof(buf), stdin);
     if (got == 0) break;
     if (some_stream_push_bytes(st, buf, (long long)got, notes) != 0) goto fail;
-    print_chunks(notes, info);
+    print_chunks(notes, info, "");
+    some_stream_info si;
+    some_audio_meta m;
+    if (some_stream_get_info(st, &si) != 0 || some_stream_get_meta(st, &m, NULL, NULL) != 0 ||
+        maybe_peek(pk, st, si.received, m.rate, info) != 0)
+      goto fail;
   }
   if (ferror(stdin)) {
     fprintf(stderr, "some_stream: read error\n");
     goto done;
   }
   if (some_stream_finish(st, notes) != 0) goto fail;
-  print_chunks(notes, info);
+  print_chunks(notes, info, "");
   rc = 0;
   goto done;
 fail:
@@ -82,10 +108,21 @@ done:
 }
 
 int main(int argc, char** argv) {
+  peeker pk = {0, 0, NULL};
+  if (argc >= 3 && strcmp(argv[1], "--peek") == 0) {
+    pk.peek_ms = atoi(argv[2]);
+    if (pk.peek_ms <= 0) {
+      fprintf(stderr, "some_stream: --peek takes a positive number of milliseconds, not '%s'\n", argv[2]);
+      return 2;
+    }
+    pk.next_ms = pk.peek_ms;
+    argv[2] = argv[0];
+    argc -= 2, argv += 2;
+  }
   const int encoded = argc >= 3 && strcmp(argv[2], "-") == 0;
   if (argc < 3 || (!encoded && atoi(argv[2]) <= 0)) {
-    fprintf(stderr, "usage: %s MODEL RATE [DEVICES] < mono float32 little-endian PCM\n"
-                    "       %s MODEL - [DEVICES] < WAV, FLAC or AIFF bytes\n", argv[0], argv[0]);
+    fprintf(stderr, "usage: %s [--peek MS] MODEL RATE [DEVICES] < mono float32 little-endian PCM\n"
+                    "       %s [--peek MS] MODEL - [DEVICES] < WAV, FLAC or AIFF bytes\n", argv[0], argv[0]);
     return 2;
   }
   int devices[64] = {0};
@@ -98,10 +135,12 @@ int main(int argc, char** argv) {
     some_session* s = NULL;
     some_session_info info;
     int rc = 1;
-    if (some_session_open_devices(argv[1], devices, n_devices, &s) != 0 || some_session_get_info(s, &info) != 0)
+    if (some_session_open_devices(argv[1], devices, n_devices, &s) != 0 || some_session_get_info(s, &info) != 0 ||
+        (pk.peek_ms && some_notes_create(&pk.notes) != 0))
       fprintf(stderr, "some_stream: %s\n", some_last_error());
     else
-      rc = run_encoded(s, &info);
+      rc = run_encoded(s, &info, &pk);
+    some_notes_destroy(pk.notes);
     some_session_close(s);
     return rc;
   }
@@ -116,11 +155,13 @@ int main(int argc, char** argv) {
   int rc = 1;
   if (!raw || !samples) goto done;
   if (some_session_open_devices(argv[1], devices, n_devices, &s) != 0 || some_session_get_info(s, &info) != 0 ||
-      some_notes_create(&notes) != 0 || some_stream_open(s, rate, NULL, &st) != 0) {
+      some_notes_create(&notes) != 0 || some_stream_open(s, rate, NULL, &st) != 0 ||
+      (pk.peek_ms && some_notes_create(&pk.notes) != 0)) {
     fprintf(stderr, "some_stream: %s\n", some_last_error());
     goto done;
   }
   size_t have = 0;                       /* bytes of the current block read so far */
+  long long pushed = 0;
   for (;;) {
     const size_t got = fread(raw + have, 1, 4 * block - have, stdin);
     have += got;
@@ -138,7 +179,12 @@ int main(int argc, char** argv) {
         fprintf(stderr, "some_stream: %s\n", some_last_error());
         goto done;
       }
-      print_chunks(notes, &info);
+      print_chunks(notes, &info, "");
+      pushed += (long long)n;
+      if (maybe_peek(&pk, st, pushed, rate, &info) != 0) {
+        fprintf(stderr, "some_stream: %s\n", some_last_error());
+        goto done;
+      }
     }
     if (eof) break;
   }
@@ -150,11 +196,12 @@ int main(int argc, char** argv) {
     fprintf(stderr, "some_stream: %s\n", some_last_error());
     goto done;
   }
-  print_chunks(notes, &info);
+  print_chunks(notes, &info, "");
   rc = 0;
 done:
   some_stream_close(st);
   some_notes_destroy(notes);
+  some_notes_destroy(pk.notes);
   some_session_close(s);
   free(raw);
   free(samples);

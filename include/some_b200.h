@@ -747,14 +747,15 @@ int some_session_get_load(const some_session* s, int64_t* chunks, int64_t* frame
  * same steps as before, and calls merge only when they queue behind a running step.
  *   Which requests may share a step: clip calls (some_session_transcribe) with clip calls; sliced and encoded calls together
  * (one recordings step: their recordings decoded, resampled, cut and transcribed as one); PCM stream calls together (push,
- * finish, push_many: one stream step); encoded stream calls together (push_bytes*, finish of an encoded stream).  Calls of
+ * finish, push_many: one stream step); encoded stream calls together (push_bytes*, finish of an encoded stream); peeks
+ * together (some_stream_peek*: one batch of open regions).  Calls of
  * different kinds run as consecutive steps.  Never in one step: two requests that touch the same some_stream or the same
  * some_notes (the later one waits for a later step, so each stream's calls apply in arrival order), or requests whose threads
  * have different some_set_pdl settings (the step runs with its requests' setting).  A request joins only while the step's
  * model-rate samples stay within max(the oldest request's own, SOME_SESSION_STEP_SAMPLES), so a merged step holds no more
  * device memory than its largest request alone or a step of that size.  The samples are known before any GPU work: clips,
  * the sliced and encoded recordings at the model's rate, a PCM stream push's samples at the model's rate, and an encoded
- * stream push's bytes.  An encoded call with a FLAC file that states no length (STREAMINFO total 0) takes no joiners and joins
+ * stream push's bytes, and a peek's open regions.  An encoded call with a FLAC file that states no length (STREAMINFO total 0) takes no joiners and joins
  * no step.  A request that cannot join stays the oldest, and the next step is built around it.
  *   Results: a step of several requests gives each request exactly what it gives alone (a chunk's notes do not depend on the
  * rest of its batch).  An encoded call refused after the scan (a corrupt FLAC file) fails alone with the message and item
@@ -934,6 +935,31 @@ int some_stream_push_bytes(some_stream* st, const void* data, long long n_bytes,
 int some_stream_push_bytes_many(some_stream* const* streams, const void* const* data, const long long* n_bytes, const int* finish,
                                 int count, some_notes* const* out);
 int some_stream_get_meta(const some_stream* st, some_audio_meta* meta, long long* bytes_received, long long* bytes_held);
+/* Provisional notes: the part of a stream the slicer has not closed yet, transcribed on demand, without waiting for the
+ * chunk to be delivered.  A stream's open region is [a, b) in model-rate samples: a = the first sample of a range not returned
+ * yet (some_slicer_stream_keep_from's *sample: 0 until more than min_length hops are fixed), b = `fixed` of
+ * some_stream_get_info.  If b > a, `out` receives one clip with begin = a, end = b and the notes some_session_transcribe gives
+ * for samples [a, b) of the recording at the model's rate (for a stream at another rate: of audio.resample of the whole input;
+ * for an encoded stream: of the decoded file), bit for bit; if b == a, zero clips and no GPU work.  A peek changes nothing in
+ * the stream: the chunks of all pushes and the finish are the same with or without peeks.  It works on PCM and encoded
+ * streams alike; an encoded stream's samples are decoded already, so a peek decodes nothing.
+ *   For each stream, a never decreases from one peek to the next, is never before the end of a chunk already delivered, and
+ * every chunk delivered later begins at or after it, with one exception (some_slicer_stream_keep_from's head): a recording
+ * that ends inside a leading silence longer than max_sil_kept frames is one chunk [0, e) with e <= max_sil_kept hops, which
+ * begins before the a of the peeks made during that silence.
+ *   Cost: the trunk runs over the whole open region at every peek, so the work grows with the region's length times the peek
+ * rate; the caller chooses the rate, and the region spans the chunk in progress and any silence after it.  Each call is one step: the
+ * regions of all its streams are copied, on the device, next to each other and transcribed as one batch (spread over the
+ * replicas of a multi-device session like the chunks of any call), with one synchronise.
+ *   some_stream_peek_many peeks `count` streams of one session in one call; out[i] receives stream i's clip.  Refused, with
+ * the index i in the message and no stream or out[i] changed, when: an array is NULL or count < 0; a stream is NULL, belongs
+ * to another session than stream 0, appears twice, has finished or was refused on its content; two entries share one
+ * some_notes.  count == 0 does nothing.  A device error fails the call like any other; since a peek changes no stream state,
+ * the session and its streams stay usable after it, and every out[i] is left untouched.
+ *   Each call is one request (see "Calls from several threads"): peeks share a step with other peeks, never with a call that
+ * touches the same stream or some_notes, and run after every earlier call on their streams. */
+int some_stream_peek(some_stream* st, some_notes* out);
+int some_stream_peek_many(some_stream* const* streams, int count, some_notes* const* out);
 
 #ifdef __cplusplus
 }

@@ -281,6 +281,8 @@ EXPORTS = {
     'some_stream_push_bytes': (C.c_int, [_vp, _vp, C.c_longlong, _vp]),
     'some_stream_push_bytes_many': (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, _vp]),
     'some_stream_get_meta': (C.c_int, [_vp, C.POINTER(AudioMeta), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]),
+    'some_stream_peek': (C.c_int, [_vp, _vp]),
+    'some_stream_peek_many': (C.c_int, [_vp, C.c_int, _vp]),
 }
 
 _lib = None

@@ -11,7 +11,7 @@
 // the chunks of each step over the replicas, each on its own thread (replica 0, the only one of a one-device session, on the
 // calling thread), and take_chunks reads each caller's notes from the replica that ran each chunk.  Every call is a request in
 // the session's queue (submit, at the end): calls of one kind that queue while a step runs share the next step, whose back
-// end (run_chunks, Recordings, streams_step, bytes_step) takes the items of all of them.
+// end (run_chunks, Recordings, streams_step, bytes_step, peeks_step) takes the items of all of them.
 //
 // The model file (little-endian; INTEGRATION.md "Deploying without Python" has the table):
 //   header     128 bytes: magic "SOMEB200", format version, ABI number, file size, directory offset, tensor count, the scalars
@@ -999,10 +999,11 @@ struct RecItem {
 };
 struct StepItem;
 struct ByteItem;
+struct PeekItem;
 
 // One public call, queued for a step (see submit): what it asks for, what it touches and, once its step has run, its result.
 struct Request {
-  enum Kind { CLIPS, RECORDINGS, STREAMS, BYTES } kind;
+  enum Kind { CLIPS, RECORDINGS, STREAMS, BYTES, PEEKS } kind;
   int pdl = 0;                            // the caller's some_set_pdl setting
   int64_t samples = 0;                    // the model-rate samples it adds to a step (streams: see some_session_stats)
   bool sized = true;                      // false: its size is not known before the GPU work (it takes no joiners)
@@ -1012,11 +1013,12 @@ struct Request {
   const int64_t* lens = nullptr;
   int B = 0;
   some_notes* out = nullptr;
-  // RECORDINGS (the sliced call: one host item) with the slicer's frames, STREAMS, BYTES
+  // RECORDINGS (the sliced call: one host item) with the slicer's frames, STREAMS, BYTES, PEEKS
   std::vector<RecItem>* recs = nullptr;
   some_slicer_frames sl{};
   std::vector<StepItem>* items = nullptr;
   std::vector<ByteItem>* bytes = nullptr;
+  std::vector<PeekItem>* peeks = nullptr;
   // the result
   int rc = 0;
   std::string err;
@@ -1483,6 +1485,23 @@ struct Decode {
   }
 };
 
+// Device-resident ranges of the session's streams (src[c]: lens[c] samples on replica 0's device), copied next to each other
+// into replica 0's audio buffer on the session's stream and transcribed as one batch.
+int run_resident(some_session* s, const std::vector<const float*>& src, const std::vector<int64_t>& lens) {
+  const int B = static_cast<int>(lens.size());
+  if (B == 0) return 0;
+  std::vector<int64_t> starts(B);
+  int64_t total = 0;
+  for (int c = 0; c < B; ++c) starts[c] = total, total += align4(lens[c]);
+  DevBuf& chunks_d = s->reps[0]->wave_d;
+  if (chunks_d.ensure(4ull * total + 16, "the audio")) return -1;
+  float* wave = static_cast<float*>(chunks_d.p);
+  for (int c = 0; c < B; ++c)
+    if (lens[c])
+      SOME_CUDA(cudaMemcpyAsync(wave + starts[c], src[c], 4ull * lens[c], cudaMemcpyDeviceToDevice, s->stream), "chunk copy");
+  return run_chunks(s, nullptr, wave, starts.data(), lens.data(), B);
+}
+
 // One step of any number of streams of one session (one step runs at a time).  Each stream does what a push of its samples
 // (and a finish, when `final`) does alone, but the GPU work is made once for all of them:
 //   1. per stream on the host: what to keep, the samples set apart during a leading silence, the window plans and room in the
@@ -1618,20 +1637,48 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
     }
     it.c1 = static_cast<int>(begin.size());
   }
-  const int B = static_cast<int>(begin.size());
-  if (B) {                                          // the chunks side by side in the audio buffer, then one batch
-    std::vector<int64_t> starts(B);
-    int64_t total = 0;
-    for (int c = 0; c < B; ++c) starts[c] = total, total += align4(lens[c]);
-    DevBuf& chunks_d = s->reps[0]->wave_d;
-    if (chunks_d.ensure(4ull * total + 16, "the audio")) return -1;
-    float* wave = static_cast<float*>(chunks_d.p);
-    for (int c = 0; c < B; ++c)
-      if (lens[c])
-        SOME_CUDA(cudaMemcpyAsync(wave + starts[c], src[c], 4ull * lens[c], cudaMemcpyDeviceToDevice, s->stream), "chunk copy");
-    if (run_chunks(s, nullptr, wave, starts.data(), lens.data(), B)) return -1;
-  }
+  if (run_resident(s, src, lens)) return -1;
   for (const StepItem& it : items) take_chunks(s, it.c0, it.c1, begin.data(), lens.data(), it.out);
+  return 0;
+}
+
+// The open region of a stream, [*a, *b) in model-rate samples: from the first sample a range not returned yet may begin at
+// (its slicer's keep_from) to the last fixed sample.  It lies in the stream's device buffer (the buffer keeps everything from
+// keep_from on, and keep_from never goes back).
+int open_region(const some_stream* st, int64_t* a, int64_t* b) {
+  long long from;
+  if (some_slicer_stream_keep_from(st->slicer, &from, nullptr, nullptr)) return -1;
+  *a = from, *b = st->fixed;
+  return 0;
+}
+
+// One stream's part of a peek step: its open region, and where its notes go.
+struct PeekItem {
+  some_stream* st;
+  some_notes* out;
+  int64_t a = 0, b = 0;
+  int c0 = 0, c1 = 0;           // its clip in the step's batch (none when the region is empty)
+};
+
+// A step of peeks (some_stream_peek*): the open regions of all its streams, copied from the streams' device buffers (run_resident)
+// and transcribed as one batch; no stream changes.
+int peeks_step(some_session* s, const std::vector<Request*>& g) {
+  std::vector<const float*> src;
+  std::vector<int64_t> begin, lens;
+  for (Request* rq : g)
+    for (PeekItem& p : *rq->peeks) {
+      const some_stream* st = p.st;
+      p.c0 = p.c1 = static_cast<int>(begin.size());
+      if (p.b <= p.a) continue;
+      SOME_REQUIRE(p.a >= st->wave.first && p.b <= st->wave.first + st->wave.len,
+                   "stream: open region [%lld, %lld) is not resident ([%lld, %lld))", (long long)p.a, (long long)p.b,
+                   (long long)st->wave.first, (long long)(st->wave.first + st->wave.len));
+      src.push_back(st->wave.at(p.a)), begin.push_back(p.a), lens.push_back(p.b - p.a);
+      p.c1 = p.c0 + 1;
+    }
+  if (run_resident(s, src, lens)) return -1;
+  for (Request* rq : g)
+    for (const PeekItem& p : *rq->peeks) take_chunks(s, p.c0, p.c1, begin.data(), lens.data(), p.out);
   return 0;
 }
 
@@ -1965,6 +2012,51 @@ extern "C" int some_stream_get_meta(const some_stream* st, some_audio_meta* meta
   return 0;
 }
 
+namespace {
+// Queues peeks of streams of one session as one call, each with its open region, whose model-rate samples size the request.
+int peek_call(some_stream* const* streams, int count, some_notes* const* out) {
+  std::vector<PeekItem> peeks;
+  Request rq{Request::PEEKS};
+  for (int i = 0; i < count; ++i) {
+    PeekItem p{streams[i], out[i]};
+    if (open_region(p.st, &p.a, &p.b)) return -1;
+    rq.samples += std::max<int64_t>(0, p.b - p.a);
+    rq.touches.push_back(p.st), rq.touches.push_back(p.out);
+    peeks.push_back(p);
+  }
+  rq.peeks = &peeks;
+  return submit(streams[0]->s, rq);
+}
+}  // namespace
+
+extern "C" int some_stream_peek(some_stream* st, some_notes* out) {
+  SOME_REQUIRE(st != nullptr && out != nullptr, "some_stream_peek: bad arguments");
+  SOME_REQUIRE(!st->failed, "some_stream_peek: the stream was refused");
+  SOME_REQUIRE(!st->finished, "some_stream_peek: the stream has finished");
+  return peek_call(&st, 1, &out);
+}
+
+extern "C" int some_stream_peek_many(some_stream* const* streams, int count, some_notes* const* out) {
+  const char* who = "some_stream_peek_many";
+  SOME_REQUIRE(streams != nullptr && out != nullptr && count >= 0, "%s: bad arguments", who);
+  if (count == 0) return 0;
+  const some_session* s = streams[0] ? streams[0]->s : nullptr;
+  std::map<const void*, int> seen, seen_notes;
+  for (int i = 0; i < count; ++i) {
+    const some_stream* st = streams[i];
+    SOME_REQUIRE(st != nullptr, "%s: stream %d is NULL", who, i);
+    SOME_REQUIRE(st->s == s, "%s: stream %d belongs to another session than stream 0", who, i);
+    const auto dup = seen.emplace(st, i);
+    SOME_REQUIRE(dup.second, "%s: stream %d appears twice (also at %d)", who, i, dup.first->second);
+    SOME_REQUIRE(!st->failed, "%s: stream %d was refused", who, i);
+    SOME_REQUIRE(!st->finished, "%s: stream %d has finished", who, i);
+    SOME_REQUIRE(out[i] != nullptr, "%s: stream %d: NULL notes", who, i);
+    const auto shared = seen_notes.emplace(out[i], i);
+    SOME_REQUIRE(shared.second, "%s: stream %d shares its some_notes with stream %d", who, i, shared.first->second);
+  }
+  return peek_call(streams, count, out);
+}
+
 // ---------------------------------------------------------------------------------------------------- encoded files
 namespace {
 // Item i's message with its index in front.
@@ -2172,6 +2264,7 @@ int run_step(some_session* s, const std::vector<Request*>& g) {
         case Request::RECORDINGS: rc = recordings_step(s, g); break;
         case Request::STREAMS: rc = streams_calls_step(s, g); break;
         case Request::BYTES: rc = bytes_calls_step(s, g); break;
+        case Request::PEEKS: rc = peeks_step(s, g); break;
       }
     }
     if (rc != 0) {

@@ -236,6 +236,15 @@ class Session:
                                                   outs), 'some_stream_push_many')
         return [st._results() for st, _ in items]
 
+    def peek_many(self, streams: Sequence['Stream']):
+        """some_stream_peek_many: the provisional notes of many streams of this session (PCM or encoded) in one step.  Returns
+        one (offsets, ranges, notes) per stream, what Stream.peek returns."""
+        k = len(streams)
+        handles = (C.c_void_p * max(k, 1))(*[st.handle for st in streams])
+        outs = (C.c_void_p * max(k, 1))(*[st._peek_notes().handle for st in streams])
+        _lib.check(self.lib.some_stream_peek_many(handles, k, outs), 'some_stream_peek_many')
+        return [st._results(st.peeked) for st in streams]
+
 
 class Stream:
     """some_stream_*: push samples as they arrive; push() and finish() return the chunks that became final, in the shape
@@ -244,6 +253,7 @@ class Stream:
 
     handle = None
     notes = None
+    peeked = None
 
     def __init__(self, session: Session, sample_rate: Optional[int] = None, params: Optional[_lib.SlicerParams] = None):
         self.lib, self.session = session.lib, session
@@ -254,9 +264,22 @@ class Stream:
         self.notes = Notes()
         session._streams.add(self)
 
-    def _results(self):
-        ranges, res = self.notes.results(self.session.timestep)
+    def _results(self, notes: Optional[Notes] = None):
+        ranges, res = (notes or self.notes).results(self.session.timestep)
         return [a / self.session.sample_rate for a, _ in ranges], ranges, res
+
+    def _peek_notes(self) -> Notes:
+        if self.peeked is None:
+            self.peeked = Notes()
+        return self.peeked
+
+    def peek(self):
+        """some_stream_peek: the provisional notes of the part of the recording the slicer has not closed yet, from the first
+        sample no delivered chunk covers to the last fixed sample: zero or one clip, in the shape push() returns, with what
+        transcribe() gives for those samples.  The stream does not change, and the results of the last push stay as they were
+        (a peek has its own Notes)."""
+        _lib.check(self.lib.some_stream_peek(self.handle, self._peek_notes().handle), 'some_stream_peek')
+        return self._results(self.peeked)
 
     def push(self, samples: np.ndarray):
         x = np.ascontiguousarray(samples, dtype=np.float32)
@@ -278,6 +301,8 @@ class Stream:
             self.handle = None
         if self.notes is not None:
             self.notes.close()
+        if self.peeked is not None:
+            self.peeked.close()
 
     def __enter__(self):
         return self
