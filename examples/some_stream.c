@@ -1,8 +1,8 @@
 /* some_stream: transcribe a recording while it arrives, with a model file written by `python -m some_b200.export`, without
  * Python.
  *
- *   some_stream [--peek MS] MODEL RATE [DEVICES] < pcm
- *   some_stream [--peek MS] MODEL - [DEVICES] < file.wav, file.flac or file.aif
+ *   some_stream [--peek MS] [--frames] MODEL RATE [DEVICES] < pcm
+ *   some_stream [--peek MS] [--frames] MODEL - [DEVICES] < file.wav, file.flac or file.aif
  *
  * With RATE, reads raw mono little-endian float32 samples at RATE Hz from stdin in blocks of 100 ms and pushes each block to a
  * some_stream.  With `-`, reads a WAV, FLAC or AIFF byte stream from stdin in 64 KB reads and pushes each read to an encoded
@@ -17,7 +17,12 @@
  *
  *   ~ <region offset in seconds> <note_midi> <duration in seconds> <rest 0/1>
  *
- * A later peek or the delivered chunk replaces them.  Live from a microphone:
+ * A later peek or the delivered chunk replaces them.  With --frames, each chunk's (and each peeked region's) note lines are
+ * followed by one line per frame of it, from its frame curves (some_notes_get_frames), with "~ " in front for a peek:
+ *
+ *   f <frame time in seconds> <midi> <rest 0/1> <boundary probability> <1-based note index>
+ *
+ * frame t of a chunk is centred at its first sample + t * hop.  Live from a microphone:
  *
  *   arecord -f FLOAT_LE -c1 -r 44100 | some_stream model.somemodel 44100
  *   arecord -f S16_LE -c2 -r 48000 -t wav | some_stream model.somemodel - */
@@ -42,6 +47,8 @@ static int parse_devices(const char* list, int* devices) {
   }
 }
 
+static int print_frames = 0;             /* --frames */
+
 static void print_chunks(const some_notes* notes, const some_session_info* info, const char* prefix) {
   const int chunks = some_notes_clips(notes);
   for (int c = 0; c < chunks; ++c) {
@@ -54,6 +61,15 @@ static void print_chunks(const some_notes* notes, const some_session_info* info,
     const double offset = (double)begin / info->sample_rate;
     for (int k = 0; k < count; ++k)
       printf("%s%.17g %.9g %.17g %d\n", prefix, offset, midi[k], (double)dur[k] * info->timestep, rest[k] ? 1 : 0);
+    if (!print_frames) continue;
+    int frames = 0;
+    const float *fm, *fb;
+    const uint8_t* fr;
+    const int32_t* fn;
+    if (some_notes_get_frames(notes, c, &frames, &fm, &fr, &fb, &fn) != 0) continue;
+    for (int t = 0; t < frames; ++t)
+      printf("%sf %.17g %.9g %d %.9g %d\n", prefix, (double)(begin + (int64_t)t * info->hop) / info->sample_rate, fm[t],
+             fr[t] ? 1 : 0, fb[t], fn[t]);
   }
   fflush(stdout);
 }
@@ -79,7 +95,9 @@ static int run_encoded(some_session* s, const some_session_info* info, peeker* p
   some_stream* st = NULL;
   some_notes* notes = NULL;
   int rc = 1;
-  if (some_notes_create(&notes) != 0 || some_stream_open_encoded(s, NULL, &st) != 0) goto fail;
+  if (some_notes_create(&notes) != 0 || some_notes_set_frames(notes, print_frames) != 0 ||
+      some_stream_open_encoded(s, NULL, &st) != 0)
+    goto fail;
   for (;;) {
     const size_t got = fread(buf, 1, sizeof(buf), stdin);
     if (got == 0) break;
@@ -109,20 +127,28 @@ done:
 
 int main(int argc, char** argv) {
   peeker pk = {0, 0, NULL};
-  if (argc >= 3 && strcmp(argv[1], "--peek") == 0) {
-    pk.peek_ms = atoi(argv[2]);
-    if (pk.peek_ms <= 0) {
-      fprintf(stderr, "some_stream: --peek takes a positive number of milliseconds, not '%s'\n", argv[2]);
-      return 2;
+  for (;;) {
+    if (argc >= 3 && strcmp(argv[1], "--peek") == 0) {
+      pk.peek_ms = atoi(argv[2]);
+      if (pk.peek_ms <= 0) {
+        fprintf(stderr, "some_stream: --peek takes a positive number of milliseconds, not '%s'\n", argv[2]);
+        return 2;
+      }
+      pk.next_ms = pk.peek_ms;
+      argv[2] = argv[0];
+      argc -= 2, argv += 2;
+    } else if (argc >= 2 && strcmp(argv[1], "--frames") == 0) {
+      print_frames = 1;
+      argv[1] = argv[0];
+      argc -= 1, argv += 1;
+    } else {
+      break;
     }
-    pk.next_ms = pk.peek_ms;
-    argv[2] = argv[0];
-    argc -= 2, argv += 2;
   }
   const int encoded = argc >= 3 && strcmp(argv[2], "-") == 0;
   if (argc < 3 || (!encoded && atoi(argv[2]) <= 0)) {
-    fprintf(stderr, "usage: %s [--peek MS] MODEL RATE [DEVICES] < mono float32 little-endian PCM\n"
-                    "       %s [--peek MS] MODEL - [DEVICES] < WAV, FLAC or AIFF bytes\n", argv[0], argv[0]);
+    fprintf(stderr, "usage: %s [--peek MS] [--frames] MODEL RATE [DEVICES] < mono float32 little-endian PCM\n"
+                    "       %s [--peek MS] [--frames] MODEL - [DEVICES] < WAV, FLAC or AIFF bytes\n", argv[0], argv[0]);
     return 2;
   }
   int devices[64] = {0};
@@ -136,7 +162,7 @@ int main(int argc, char** argv) {
     some_session_info info;
     int rc = 1;
     if (some_session_open_devices(argv[1], devices, n_devices, &s) != 0 || some_session_get_info(s, &info) != 0 ||
-        (pk.peek_ms && some_notes_create(&pk.notes) != 0))
+        (pk.peek_ms && (some_notes_create(&pk.notes) != 0 || some_notes_set_frames(pk.notes, print_frames) != 0)))
       fprintf(stderr, "some_stream: %s\n", some_last_error());
     else
       rc = run_encoded(s, &info, &pk);
@@ -155,8 +181,9 @@ int main(int argc, char** argv) {
   int rc = 1;
   if (!raw || !samples) goto done;
   if (some_session_open_devices(argv[1], devices, n_devices, &s) != 0 || some_session_get_info(s, &info) != 0 ||
-      some_notes_create(&notes) != 0 || some_stream_open(s, rate, NULL, &st) != 0 ||
-      (pk.peek_ms && some_notes_create(&pk.notes) != 0)) {
+      some_notes_create(&notes) != 0 || some_notes_set_frames(notes, print_frames) != 0 ||
+      some_stream_open(s, rate, NULL, &st) != 0 ||
+      (pk.peek_ms && (some_notes_create(&pk.notes) != 0 || some_notes_set_frames(pk.notes, print_frames) != 0))) {
     fprintf(stderr, "some_stream: %s\n", some_last_error());
     goto done;
   }

@@ -192,7 +192,9 @@ int some_bound_head(const float* x, const float* gamma, const float* beta, const
  *   outputs are packed per clip at offset cu_frames[b] (a clip never has more notes than frames):
  *     note_midi f32 [M], note_dur i32 [M] (frames; seconds = dur * hop / sr on the host, me_infer.py:95),
  *     note_rest u8 [M], note_count i32 [B]
- *   optional debug outputs (may be NULL): frame2item i32 [M], values f32 [M], rest u8 [M]
+ *   optional per-frame outputs (may be NULL: then they live in the scratch): frame2item i32 [M] (1-based note index of each
+ *     frame within its clip, infer_utils.py:27-39), values f32 [M] (phase A's pitch value), rest u8 [M] (phase A's rest
+ *     flag); the notes are the same with or without them.  The session's frame curves (some_notes_get_frames) are these.
  * Integer outputs match the CPU reference exactly for identical inputs: the boundary cumsum is accumulated
  * sequentially in double and rounded per prefix like ATen's CPU cumsum; per-note sums run in frame order. */
 typedef struct {
@@ -784,6 +786,27 @@ int some_notes_destroy(some_notes* n);
 int some_notes_clips(const some_notes* n); /* number of clips / chunks (< 0: error) */
 int some_notes_get(const some_notes* n, int clip, int* count, const float** note_midi, const int32_t** note_dur,
                    const uint8_t** note_rest, int64_t* begin, int64_t* end); /* any output pointer may be NULL */
+/* Frame curves: what lies under and between the notes, for pitch-line displays.  Off by default.  While
+ * some_notes_set_frames(n, 1) is in effect, every call that fills `n` (transcribe, sliced, encoded, stream push / finish /
+ * push_many / push_bytes*, peek*) also fills one curve set per clip or chunk, in the order of the notes; set it before the
+ * call, not while a call on `n` runs.  For clip `clip` of T frames (T = 1 + len / hop, len: its samples at the model's rate,
+ * the rows the model ran), some_notes_get_frames gives:
+ *   midi        f32 [T]  the pitch value of each frame: continuous models, the gaussian-blurred decode of the probabilities
+ *                        (decode_gaussian_blurred_probs, utils/infer_utils.py:9-24); quantized models, clip(argmax, 0, 127)
+ *                        (me_quant_infer.py:28-31)
+ *   rest        u8 [T]   1 where the frame is a rest: max probability < rest_threshold, or argmax == 128 (quantized)
+ *   bound       f32 [T]  the boundary probability the model wrote for the frame (sigmoid of its cut head)
+ *   note_index  i32 [T]  the 1-based note the frame belongs to (decode_bounds_to_alignment, infer_utils.py:27-39); the notes
+ *                        of some_notes_get are exactly the runs of equal note_index, in order
+ * Frame t of a clip is centred at sample begin + t * hop of the clip's range (begin from some_notes_get): the mel frames are
+ * taken after 1024 + 1024 zero samples of padding with a centre-free STFT (spec.py:48-60).  The notes are bit-identical with
+ * frames on or off.  Cost: 13 bytes per frame more in the step's one download, plus one device copy of the bounds per
+ * pipeline chunk; a step copies that much more only when one of its results asks for curves.  The pointers stay valid until
+ * the next call that fills `n`; any output pointer may be NULL.  Refused: a NULL `n`, a clip out of range, and notes that
+ * were last filled with frames off. */
+int some_notes_set_frames(some_notes* n, int on);
+int some_notes_get_frames(const some_notes* n, int clip, int* frames, const float** midi, const uint8_t** rest,
+                          const float** bound, const int32_t** note_index);
 /* some_midi_write over a result: chunk offsets begin / sample_rate seconds, as infer.py passes them to build_midi_file. */
 int some_notes_midi(const some_notes* n, int sample_rate, double timestep, double tempo, uint8_t* buf, size_t capacity,
                     size_t* size);

@@ -262,6 +262,9 @@ EXPORTS = {
     'some_notes_clips': (C.c_int, [_vp]),
     'some_notes_get': (C.c_int, [_vp, C.c_int, C.POINTER(C.c_int), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp),
                                  C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    'some_notes_set_frames': (C.c_int, [_vp, C.c_int]),
+    'some_notes_get_frames': (C.c_int, [_vp, C.c_int, C.POINTER(C.c_int), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp),
+                                        C.POINTER(_vp)]),
     'some_slicer_derive': (C.c_int, [C.c_int, C.POINTER(SlicerParams), C.POINTER(SlicerFrames)]),
     'some_slicer_ranges': (C.c_int, [_vp, C.c_int, C.c_longlong, C.POINTER(SlicerFrames), _vp, C.c_int,
                                      C.POINTER(C.c_int)]),

@@ -275,6 +275,12 @@ struct some_notes {
   std::vector<float> midi;
   std::vector<int32_t> dur;
   std::vector<uint8_t> rest;
+  // the frame curves (some_notes_set_frames): `frames` asks for them, `framed` says the last fill wrote them
+  bool frames = false, framed = false;
+  std::vector<int64_t> frame_first;   // [clips + 1] prefix sums of the frame counts
+  std::vector<float> f_midi, f_bound;
+  std::vector<uint8_t> f_rest;
+  std::vector<int32_t> f_note;
 };
 
 namespace {
@@ -339,6 +345,7 @@ struct some_session {
   cudaEvent_t fed = nullptr;
   std::vector<std::pair<int, int>> held;  // chunk c of the step: the replica that ran it, and its clip in that replica's part
   std::vector<std::pair<int64_t, int64_t>> load;   // each replica's chunks and frames in the last completed step
+  bool frames = false;                    // the step in progress decodes frame curves (a result of it asks for them)
 };
 
 namespace {
@@ -362,22 +369,38 @@ void destroy(some_session* s) {
   delete s;                               // its buffers free themselves, on replica 0's device
 }
 
+// Empties *out for its next fill, which writes frame curves if it asks for them.
 void clear(some_notes* out) {
   out->first.assign(1, 0), out->range.clear(), out->midi.clear(), out->dur.clear(), out->rest.clear();
+  out->framed = out->frames;
+  out->frame_first.assign(1, 0), out->f_midi.clear(), out->f_bound.clear(), out->f_rest.clear(), out->f_note.clear();
 }
 
-// Appends the notes of clip k of `from` to *out, as its next clip of sample range [b, e).
+template <class T>
+void append_range(std::vector<T>& to, const std::vector<T>& from, int64_t a, int64_t b) {
+  to.insert(to.end(), from.begin() + a, from.begin() + b);
+}
+
+// Appends the notes of clip k of `from` to *out, as its next clip of sample range [b, e), and its frame curves when *out
+// takes them (`from` then holds them: a step decodes curves when any of its results asks for them).
 void append_clip(const some_notes& from, int k, int64_t b, int64_t e, some_notes* out) {
   const int64_t n0 = from.first[k], n1 = from.first[k + 1];
-  out->midi.insert(out->midi.end(), from.midi.begin() + n0, from.midi.begin() + n1);
-  out->dur.insert(out->dur.end(), from.dur.begin() + n0, from.dur.begin() + n1);
-  out->rest.insert(out->rest.end(), from.rest.begin() + n0, from.rest.begin() + n1);
+  append_range(out->midi, from.midi, n0, n1);
+  append_range(out->dur, from.dur, n0, n1);
+  append_range(out->rest, from.rest, n0, n1);
   out->first.push_back(out->first.back() + (n1 - n0));
   out->range.push_back(b), out->range.push_back(e);
+  if (!out->framed) return;
+  const int64_t f0 = from.frame_first[k], f1 = from.frame_first[k + 1];
+  append_range(out->f_midi, from.f_midi, f0, f1);
+  append_range(out->f_bound, from.f_bound, f0, f1);
+  append_range(out->f_rest, from.f_rest, f0, f1);
+  append_range(out->f_note, from.f_note, f0, f1);
+  out->frame_first.push_back(out->frame_first.back() + (f1 - f0));
 }
 
-// Sets *out to chunks [c0, c1) of the step's last run_chunks, each read from the replica that ran it; chunk c is samples
-// [begin[c], begin[c] + lens[c]).
+// Sets *out to chunks [c0, c1) of the step's last run_chunks, each read from the replica that ran it, with their frame curves
+// when *out asks for them; chunk c is samples [begin[c], begin[c] + lens[c]).
 void take_chunks(const some_session* s, int c0, int c1, const int64_t* begin, const int64_t* lens, some_notes* out) {
   clear(out);
   for (int c = c0; c < c1; ++c)
@@ -436,6 +459,11 @@ std::vector<std::pair<int, int>> split_chunks(const std::vector<int32_t>& cu) {
 // clip i is host[i][0 .. lens[i])) are staged through pinned memory and copied on the copy stream while the previous chunk's
 // kernels run; resident clips (`resident` != NULL) are the sample ranges [starts[i], starts[i] + lens[i]) of that buffer on
 // r's device, written by work on r's streams or awaited by its copy stream.  The notes of clip i go to clip i of r.part.
+//   Each pipeline chunk's results come down in one slab, one copy for the whole batch.  Per chunk of bc clips and mc frames:
+// note counts i32 [bc] | durations i32 [mc] | MIDI f32 [mc] | rests u8 [mc], padded to 16 bytes.  When the step decodes
+// frame curves (s->frames), the chunk's region goes on with its curves, padded to 16 bytes: the decode's per-frame values
+// f32 [mc], the bounds f32 [mc] (a device copy of the trunk's output, so the slab still comes down in one copy), the frame ->
+// note index i32 [mc] and the rest flags u8 [mc], 13 bytes per frame.  A step without curves copies what it copied before.
 int run_batch(const some_session* s, Replica& r, const float* const* host, const float* resident, const int64_t* res_starts,
               const int64_t* lens, int B) {
   std::vector<int32_t> cu(B + 1, 0);
@@ -457,10 +485,12 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
   std::vector<Chunk> layout;
   uint64_t slab_bytes = 0;
   int max_mc = 1;
+  auto notes_bytes = [](const Chunk& ch) { return (4ull * ch.bc + 9ull * ch.mc + 15) & ~uint64_t(15); };
   for (const auto& sp : spans) {
     const int bc = sp.second - sp.first, mc = cu[sp.second] - cu[sp.first];
     layout.push_back({sp.first, sp.second, slab_bytes, bc, mc});
-    slab_bytes += (4ull * bc + 9ull * mc + 15) & ~uint64_t(15);
+    slab_bytes += notes_bytes(layout.back());
+    if (s->frames) slab_bytes += (13ull * mc + 15) & ~uint64_t(15);
     max_mc = std::max(max_mc, mc);
   }
   // buffers
@@ -531,13 +561,22 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
     d.note_midi = reinterpret_cast<float*>(o + 4ull * ch.bc + 4ull * ch.mc);
     d.note_rest = o + 4ull * ch.bc + 8ull * ch.mc;
     d.scratch = r.scratch.p;
+    uint8_t* f = o + notes_bytes(ch);
+    if (s->frames) {
+      d.dbg_values = reinterpret_cast<float*>(f);
+      d.dbg_frame2item = reinterpret_cast<int32_t*>(f + 8ull * ch.mc);
+      d.dbg_rest = f + 12ull * ch.mc;
+    }
     if (some_decode_notes(&d, r.stream)) return -1;
+    if (s->frames)
+      SOME_CUDA(cudaMemcpyAsync(f + 4ull * ch.mc, r.ws.bounds, 4ull * ch.mc, cudaMemcpyDeviceToDevice, r.stream), "bounds copy");
   }
   if (slab_bytes) SOME_CUDA(cudaMemcpyAsync(r.slab_h.p, slab, slab_bytes, cudaMemcpyDeviceToHost, r.stream), "note download");
   SOME_CUDA(cudaStreamSynchronize(r.stream), "synchronise");
 
-  // unpack: the notes of clip b start at its first frame's row of the chunk slab
+  // unpack: the notes of clip b start at its first frame's row of the chunk slab, and so do its curves
   some_notes* out = &r.part;
+  out->frames = s->frames;
   clear(out);
   const uint8_t* h = static_cast<const uint8_t*>(r.slab_h.p);
   for (const Chunk& ch : layout) {
@@ -545,8 +584,8 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
     for (int b = 0; b < ch.bc; ++b) {
       const int32_t n = rd<int32_t>(o + 4ull * b);
       const int64_t row = cu[ch.c0 + b] - cu[ch.c0];
-      SOME_REQUIRE(n >= 0 && row + n <= ch.mc, "session: decode returned %d notes for a clip of %d frames", n,
-                   cu[ch.c0 + b + 1] - cu[ch.c0 + b]);
+      const int32_t T = cu[ch.c0 + b + 1] - cu[ch.c0 + b];
+      SOME_REQUIRE(n >= 0 && row + n <= ch.mc, "session: decode returned %d notes for a clip of %d frames", n, T);
       for (int j = 0; j < n; ++j) {
         const uint64_t r = static_cast<uint64_t>(row + j);
         out->dur.push_back(rd<int32_t>(o + 4ull * ch.bc + 4 * r));
@@ -554,6 +593,19 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
         out->rest.push_back(o[4ull * ch.bc + 8ull * ch.mc + r]);
       }
       out->first.push_back(out->first.back() + n);
+      if (!s->frames) continue;
+      const uint8_t* f = o + notes_bytes(ch);
+      auto put = [&](auto& to, const uint8_t* at) {
+        using T_ = typename std::remove_reference<decltype(to)>::type::value_type;
+        const size_t k = to.size();
+        to.resize(k + T);
+        memcpy(to.data() + k, at + sizeof(T_) * row, sizeof(T_) * T);
+      };
+      put(out->f_midi, f);
+      put(out->f_bound, f + 4ull * ch.mc);
+      put(out->f_note, f + 8ull * ch.mc);
+      put(out->f_rest, f + 12ull * ch.mc);
+      out->frame_first.push_back(out->frame_first.back() + T);
     }
   }
   return 0;
@@ -681,6 +733,24 @@ extern "C" int some_notes_get(const some_notes* n, int clip, int* count, const f
   if (note_rest) *note_rest = n->rest.data() + a;
   if (begin) *begin = n->range[2 * clip];
   if (end) *end = n->range[2 * clip + 1];
+  return 0;
+}
+extern "C" int some_notes_set_frames(some_notes* n, int on) {
+  SOME_REQUIRE(n != nullptr, "some_notes_set_frames: null pointer");
+  n->frames = on != 0;
+  return 0;
+}
+extern "C" int some_notes_get_frames(const some_notes* n, int clip, int* frames, const float** midi, const uint8_t** rest,
+                                     const float** bound, const int32_t** note_index) {
+  SOME_REQUIRE(n != nullptr, "some_notes_get_frames: null pointer");
+  SOME_REQUIRE(clip >= 0 && clip + 1 < static_cast<int>(n->first.size()), "some_notes_get_frames: clip %d out of range", clip);
+  SOME_REQUIRE(n->framed, "some_notes_get_frames: the notes were filled with frames off (some_notes_set_frames)");
+  const int64_t a = n->frame_first[clip];
+  if (frames) *frames = static_cast<int>(n->frame_first[clip + 1] - a);
+  if (midi) *midi = n->f_midi.data() + a;
+  if (rest) *rest = n->f_rest.data() + a;
+  if (bound) *bound = n->f_bound.data() + a;
+  if (note_index) *note_index = n->f_note.data() + a;
   return 0;
 }
 
@@ -2246,6 +2316,20 @@ int bytes_calls_step(some_session* s, const std::vector<Request*>& g) {
   return 0;
 }
 
+// Whether a request fills a some_notes that asks for frame curves: its step then decodes curves for all its chunks, and
+// each result takes them only if it asks for them.
+bool wants_frames(const Request* rq) {
+  auto framed = [](const auto* v) { return std::any_of(v->begin(), v->end(), [](const auto& it) { return it.out->frames; }); };
+  switch (rq->kind) {
+    case Request::CLIPS: return rq->out->frames;
+    case Request::RECORDINGS: return framed(rq->recs);
+    case Request::STREAMS: return framed(rq->items);
+    case Request::BYTES: return framed(rq->bytes);
+    case Request::PEEKS: return framed(rq->peeks);
+  }
+  return false;
+}
+
 // Runs one step on the calling thread, with the session's device current and the calls' some_set_pdl setting.  After a
 // failure partway through, copies and kernels may still be queued on the session's streams: it waits for them, on every
 // replica, so that the next step cannot rewrite staging or device buffers they still use; every call of the step then fails
@@ -2253,6 +2337,7 @@ int bytes_calls_step(some_session* s, const std::vector<Request*>& g) {
 int run_step(some_session* s, const std::vector<Request*>& g) {
   const int pdl = some_set_pdl(g[0]->pdl);
   int rc = -1;
+  s->frames = std::any_of(g.begin(), g.end(), wants_frames);
   {
     DeviceScope scope(s->device);
     if (scope.err != cudaSuccess) {

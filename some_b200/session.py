@@ -4,13 +4,19 @@
 The slicer parameters of transcribe_sliced and stream are ``slicer_params(...)`` (defined in some_b200.slicer).
 
 Results have the plugin's shape: one dict per clip / chunk with ``note_midi`` f32, ``note_dur`` in seconds
-(``dur * timestep``, float64 as me_infer.py:95) and ``note_rest`` bool, plus ``note_frames`` (the durations in frames)."""
+(``dur * timestep``, float64 as me_infer.py:95) and ``note_rest`` bool, plus ``note_frames`` (the durations in frames).
+
+Every call takes ``frames=False``.  With ``frames=True`` it also returns the frame curves of every clip / chunk
+(some_notes_get_frames), one ``Curves`` tuple ``(midi f32, rest bool, bound f32, note_index i32)`` per clip, as one more
+element beside what it returns with frames off: ``transcribe`` returns ``(notes, curves)``, the calls that return
+``(offsets, ranges, notes)`` return ``(offsets, ranges, notes, curves)``.  Frame t of a clip is centred at sample
+``begin + t * hop``."""
 from __future__ import annotations
 
 import ctypes as C
 import os
 import weakref
-from typing import Dict, List, Optional, Sequence, Tuple, Union
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -20,16 +26,49 @@ from . import _lib
 from .slicer import SlicerStream, slicer_frames, slicer_params, slicer_ranges  # noqa: F401
 
 
+class Curves(NamedTuple):
+    """The frame curves of one clip (some_notes_get_frames), T = 1 + samples // hop entries each."""
+    midi: np.ndarray          # f32: the pitch value of each frame
+    rest: np.ndarray          # bool: the frame is a rest
+    bound: np.ndarray         # f32: the boundary probability
+    note_index: np.ndarray    # i32: the 1-based note of the frame
+
+
 class Notes:
     """A caller-owned result object (some_notes_create / some_notes_destroy)."""
 
     handle = None
+    _frames = False
 
     def __init__(self):
         self.lib = _lib.load()
         h = C.c_void_p()
         _lib.check(self.lib.some_notes_create(C.byref(h)), 'some_notes_create')
         self.handle = h
+
+    def set_frames(self, on: bool):
+        """some_notes_set_frames: whether the calls that fill this object also fill frame curves.  The native object starts
+        with frames off, and only a change is passed on, so a call with frames=False makes no extra native call."""
+        if bool(on) != self._frames:
+            _lib.check(self.lib.some_notes_set_frames(self.handle, int(bool(on))), 'some_notes_set_frames')
+            self._frames = bool(on)
+
+    def curves(self) -> List[Curves]:
+        """The frame curves of every clip, copied out of the native object (it must have been filled with frames on)."""
+        n = self.lib.some_notes_clips(self.handle)
+        if n < 0:
+            _lib.check(n, 'some_notes_clips')
+        out = []
+        t, pm, pr, pb, pn = C.c_int(), C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        def copy(p, dtype):              # a buffer copy: np.ctypeslib.as_array costs several times more per array
+            size = t.value * np.dtype(dtype).itemsize
+            return np.frombuffer((C.c_char * size).from_address(p.value), dtype).copy() if size else np.zeros(0, dtype)
+
+        for i in range(n):
+            _lib.check(self.lib.some_notes_get_frames(self.handle, i, C.byref(t), C.byref(pm), C.byref(pr), C.byref(pb),
+                                                      C.byref(pn)), 'some_notes_get_frames')
+            out.append(Curves(copy(pm, np.float32), copy(pr, np.uint8).view(bool), copy(pb, np.float32), copy(pn, np.int32)))
+        return out
 
     def close(self):
         if self.handle is not None:
@@ -129,39 +168,48 @@ class Session:
         _lib.check(self.lib.some_session_get_stats(self.handle, C.byref(st)), 'some_session_get_stats')
         return {name: getattr(st, name) for name, _ in _lib.SessionStats._fields_}
 
-    def transcribe(self, waveforms: Sequence[np.ndarray], notes: Optional[Notes] = None) -> List[Dict[str, np.ndarray]]:
-        """some_session_transcribe: mono float32 clips at the model's rate -> one dict per clip, in input order."""
+    def transcribe(self, waveforms: Sequence[np.ndarray], notes: Optional[Notes] = None, frames: bool = False):
+        """some_session_transcribe: mono float32 clips at the model's rate -> one dict per clip, in input order (frames=True:
+        and one Curves per clip)."""
         waves = [np.ascontiguousarray(w, dtype=np.float32) for w in waveforms]
         ptrs = (C.c_void_p * max(len(waves), 1))(*[w.ctypes.data for w in waves])
         lens = np.array([w.shape[0] for w in waves] or [0], dtype=np.int64)
         own = notes is None
         notes = notes or Notes()
         try:
+            notes.set_frames(frames)
             _lib.check(self.lib.some_session_transcribe(self.handle, ptrs, lens.ctypes.data, len(waves), notes.handle),
                        'some_session_transcribe')
-            return notes.results(self.timestep)[1]
+            res = notes.results(self.timestep)[1]
+            return (res, notes.curves()) if frames else res
         finally:
             if own:
                 notes.close()
 
     def transcribe_sliced(self, samples: np.ndarray, sample_rate: Optional[int] = None,
-                          params: Optional[_lib.SlicerParams] = None, notes: Optional[Notes] = None):
+                          params: Optional[_lib.SlicerParams] = None, notes: Optional[Notes] = None, frames: bool = False):
         """some_session_transcribe_sliced: one mono recording (any integer rate) -> (chunk offsets in seconds, chunk sample
         ranges, per-chunk notes), as Engine.infer_sliced returns offsets and notes."""
         x = np.ascontiguousarray(samples, dtype=np.float32)
         own = notes is None
         notes = notes or Notes()
         try:
+            notes.set_frames(frames)
             _lib.check(self.lib.some_session_transcribe_sliced(
                 self.handle, x.ctypes.data, int(x.shape[0]), int(sample_rate or self.sample_rate),
                 C.byref(params) if params is not None else None, notes.handle), 'some_session_transcribe_sliced')
-            ranges, res = notes.results(self.timestep)
+            return self._results(notes, frames)
         finally:
             if own:
                 notes.close()
-        return [a / self.sample_rate for a, _ in ranges], ranges, res
 
-    def transcribe_encoded(self, items: Sequence, params: Optional[_lib.SlicerParams] = None):
+    def _results(self, notes: Notes, frames: bool):
+        """(offsets in seconds, ranges, notes), and the curves when `frames`."""
+        ranges, res = notes.results(self.timestep)
+        offsets = [a / self.sample_rate for a, _ in ranges]
+        return (offsets, ranges, res, notes.curves()) if frames else (offsets, ranges, res)
+
+    def transcribe_encoded(self, items: Sequence, params: Optional[_lib.SlicerParams] = None, frames: bool = False):
         """some_session_transcribe_encoded: WAV, FLAC or AIFF files (bytes, or paths to read) -> one (chunk offsets in seconds, chunk
         sample ranges, per-chunk notes) per item, what transcribe_sliced returns for audio.load(file, sr=None, mono=True).
         The files are decoded, resampled, sliced and transcribed in one GPU step."""
@@ -178,14 +226,12 @@ class Session:
                                            for b, d in zip(bufs, datas)])
         notes = [Notes() for _ in range(k)]
         try:
+            for n in notes:
+                n.set_frames(frames)
             outs = (C.c_void_p * max(k, 1))(*[n.handle for n in notes])
             _lib.check(self.lib.some_session_transcribe_encoded(self.handle, enc, k, C.byref(params) if params is not None else None,
                                                                 outs), 'some_session_transcribe_encoded')
-            res = []
-            for n in notes:
-                ranges, r = n.results(self.timestep)
-                res.append(([a / self.sample_rate for a, _ in ranges], ranges, r))
-            return res
+            return [self._results(n, frames) for n in notes]
         finally:
             for n in notes:
                 n.close()
@@ -198,7 +244,8 @@ class Session:
         """some_stream_open_encoded: a WAV, FLAC or AIFF file pushed as its bytes arrive (see EncodedStream)."""
         return EncodedStream(self, params)
 
-    def push_bytes_many(self, items: Sequence[Tuple['EncodedStream', bytes]], finish: Optional[Sequence[bool]] = None):
+    def push_bytes_many(self, items: Sequence[Tuple['EncodedStream', bytes]], finish: Optional[Sequence[bool]] = None,
+                        frames: bool = False):
         """some_stream_push_bytes_many: push_many for encoded streams, with bytes in place of samples.  When a stream is refused
         on its content, the others still complete their step: the StreamRefused raised carries every item's results."""
         k = len(items)
@@ -211,15 +258,19 @@ class Session:
         fin = None if finish is None else np.array([bool(f) for f in finish] or [0], dtype=np.int32)
         if fin is not None and len(finish) != k:
             raise ValueError(f'push_bytes_many: {k} items, {len(finish)} finish flags')
+        for st, _ in items:
+            st.notes.set_frames(frames)
         rc = self.lib.some_stream_push_bytes_many(streams, ptrs, lens.ctypes.data, None if fin is None else fin.ctypes.data, k,
                                                   outs)
         if rc == _lib.STREAM_REFUSED:          # the other streams' chunks are in their Notes: hand them over with the refusal
             msg = self.lib.some_last_error().decode('utf8', 'replace')
-            raise _lib.StreamRefused(f'some_stream_push_bytes_many failed ({rc}): {msg}', [st._results() for st, _ in items])
+            raise _lib.StreamRefused(f'some_stream_push_bytes_many failed ({rc}): {msg}',
+                                     [st._results(frames=frames) for st, _ in items])
         _lib.check(rc, 'some_stream_push_bytes_many')
-        return [st._results() for st, _ in items]
+        return [st._results(frames=frames) for st, _ in items]
 
-    def push_many(self, items: Sequence[Tuple['Stream', np.ndarray]], finish: Optional[Sequence[bool]] = None):
+    def push_many(self, items: Sequence[Tuple['Stream', np.ndarray]], finish: Optional[Sequence[bool]] = None,
+                  frames: bool = False):
         """some_stream_push_many: pushes samples to many streams of this session in one step, and finishes those with a true
         entry in `finish`.  Returns one (offsets, ranges, notes) per item, what Stream.push (then Stream.finish) would return;
         each stream's results go through its own Notes."""
@@ -232,18 +283,20 @@ class Session:
         fin = None if finish is None else np.array([bool(f) for f in finish] or [0], dtype=np.int32)
         if fin is not None and len(finish) != k:
             raise ValueError(f'push_many: {k} items, {len(finish)} finish flags')
+        for st, _ in items:
+            st.notes.set_frames(frames)
         _lib.check(self.lib.some_stream_push_many(streams, ptrs, lens.ctypes.data, None if fin is None else fin.ctypes.data, k,
                                                   outs), 'some_stream_push_many')
-        return [st._results() for st, _ in items]
+        return [st._results(frames=frames) for st, _ in items]
 
-    def peek_many(self, streams: Sequence['Stream']):
+    def peek_many(self, streams: Sequence['Stream'], frames: bool = False):
         """some_stream_peek_many: the provisional notes of many streams of this session (PCM or encoded) in one step.  Returns
         one (offsets, ranges, notes) per stream, what Stream.peek returns."""
         k = len(streams)
         handles = (C.c_void_p * max(k, 1))(*[st.handle for st in streams])
-        outs = (C.c_void_p * max(k, 1))(*[st._peek_notes().handle for st in streams])
+        outs = (C.c_void_p * max(k, 1))(*[st._peek_notes(frames).handle for st in streams])
         _lib.check(self.lib.some_stream_peek_many(handles, k, outs), 'some_stream_peek_many')
-        return [st._results(st.peeked) for st in streams]
+        return [st._results(st.peeked, frames) for st in streams]
 
 
 class Stream:
@@ -264,31 +317,33 @@ class Stream:
         self.notes = Notes()
         session._streams.add(self)
 
-    def _results(self, notes: Optional[Notes] = None):
-        ranges, res = (notes or self.notes).results(self.session.timestep)
-        return [a / self.session.sample_rate for a, _ in ranges], ranges, res
+    def _results(self, notes: Optional[Notes] = None, frames: bool = False):
+        return self.session._results(notes or self.notes, frames)
 
-    def _peek_notes(self) -> Notes:
+    def _peek_notes(self, frames: bool = False) -> Notes:
         if self.peeked is None:
             self.peeked = Notes()
+        self.peeked.set_frames(frames)
         return self.peeked
 
-    def peek(self):
+    def peek(self, frames: bool = False):
         """some_stream_peek: the provisional notes of the part of the recording the slicer has not closed yet, from the first
         sample no delivered chunk covers to the last fixed sample: zero or one clip, in the shape push() returns, with what
         transcribe() gives for those samples.  The stream does not change, and the results of the last push stay as they were
         (a peek has its own Notes)."""
-        _lib.check(self.lib.some_stream_peek(self.handle, self._peek_notes().handle), 'some_stream_peek')
-        return self._results(self.peeked)
+        _lib.check(self.lib.some_stream_peek(self.handle, self._peek_notes(frames).handle), 'some_stream_peek')
+        return self._results(self.peeked, frames)
 
-    def push(self, samples: np.ndarray):
+    def push(self, samples: np.ndarray, frames: bool = False):
         x = np.ascontiguousarray(samples, dtype=np.float32)
+        self.notes.set_frames(frames)
         _lib.check(self.lib.some_stream_push(self.handle, x.ctypes.data, int(x.shape[0]), self.notes.handle), 'some_stream_push')
-        return self._results()
+        return self._results(frames=frames)
 
-    def finish(self):
+    def finish(self, frames: bool = False):
+        self.notes.set_frames(frames)
         _lib.check(self.lib.some_stream_finish(self.handle, self.notes.handle), 'some_stream_finish')
-        return self._results()
+        return self._results(frames=frames)
 
     def info(self) -> Dict[str, int]:
         i = _lib.StreamInfo()
@@ -327,10 +382,11 @@ class EncodedStream(Stream):
         self.notes = Notes()
         session._streams.add(self)
 
-    def push(self, data: bytes):
+    def push(self, data: bytes, frames: bool = False):
         d = bytes(data)
+        self.notes.set_frames(frames)
         _lib.check(self.lib.some_stream_push_bytes(self.handle, d, len(d), self.notes.handle), 'some_stream_push_bytes')
-        return self._results()
+        return self._results(frames=frames)
 
     def meta(self) -> Dict[str, int]:
         """some_stream_get_meta: the file's metadata (container 0 until the header is complete), the bytes pushed and the
