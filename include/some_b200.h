@@ -679,6 +679,18 @@ typedef struct {
 } some_workspace_f32;
 int some_forward_f32(const some_model_f32* model, const some_workspace_f32* ws, int M, int B, const int32_t* cu_frames,
                      int max_frames, int head, cudaStream_t stream);
+/* some_forward_f32_tiled: the same launch sequence and arguments, with register- and shared-memory-tiled fp32 GEMM, attention
+ * and depthwise-conv kernels that keep every output's operation order: every buffer of `ws` (x a h qkv g y probs bounds)
+ * holds the same bits as after some_forward_f32, at many times its speed: the fp32 precision of Engine.infer and of an
+ * fp32 session.  Every workspace buffer and GEMM operand must be 16-byte aligned, with K and row pitches multiples of 4
+ * floats (true for every buffer some_workspace_f32_carve hands out and every tensor of the model); otherwise the call fails
+ * with an error and launches nothing.  A clip's rows do not depend on the other clips of the launch. */
+int some_forward_f32_tiled(const some_model_f32* model, const some_workspace_f32* ws, int M, int B, const int32_t* cu_frames,
+                           int max_frames, int head, cudaStream_t stream);
+/* Size of, and carving of one 256-byte aligned device block into, an fp32 workspace for M rows: x a h qkv g y, units, probs,
+ * bounds in that order, each 256-byte aligned. */
+uint64_t some_workspace_f32_bytes(int M, int outdim);
+int some_workspace_f32_carve(void* device_block, uint64_t bytes, int M, int outdim, some_workspace_f32* ws);
 
 /* ---- Native inference session (csrc/session.cu): the export/deployment path of the reference (export.py + deployment/) for
  * hosts without Python.  `python -m some_b200.export --model CKPT` writes a checkpoint, its load-time bias correction applied
@@ -778,6 +790,12 @@ int some_session_get_stats(const some_session* s, some_session_stats* stats);
 int some_shard_clips(const int64_t* lens, int n, int replicas, int32_t* owner);
 int some_session_close(some_session* s);
 int some_session_get_info(const some_session* s, some_session_info* info);
+/* The precision of the model file the session opened, which every call runs at: SOME_PRECISION_BF16 (the product trunk,
+ * some_forward) or SOME_PRECISION_FP32 (a file written by `python -m some_b200.export --precision fp32`: the checkpoint's fp32
+ * tensors, log-mel as f32 and some_forward_f32_tiled, notes bit-identical to Engine.infer(..., precision='fp32')).  The model
+ * file records it in the header's int32 at byte 88, which bf16 files leave zero. */
+enum { SOME_PRECISION_BF16 = 0, SOME_PRECISION_FP32 = 1 };
+int some_session_get_precision(const some_session* s, int* precision);
 int some_session_transcribe(some_session* s, const float* const* clips, const int64_t* lens, int B, some_notes* out);
 int some_session_transcribe_sliced(some_session* s, const float* samples, long long n, int sample_rate,
                                    const some_slicer_params* params, some_notes* out);

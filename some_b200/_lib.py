@@ -241,6 +241,10 @@ EXPORTS = {
                                C.POINTER(CalibrationC), _vp]),
     'some_forward_f32': (C.c_int, [C.POINTER(ModelF32C), C.POINTER(WorkspaceF32C), C.c_int, C.c_int, _vp, C.c_int, C.c_int,
                                    _vp]),
+    'some_forward_f32_tiled': (C.c_int, [C.POINTER(ModelF32C), C.POINTER(WorkspaceF32C), C.c_int, C.c_int, _vp, C.c_int,
+                                         C.c_int, _vp]),
+    'some_workspace_f32_bytes': (C.c_uint64, [C.c_int, C.c_int]),
+    'some_workspace_f32_carve': (C.c_int, [_vp, C.c_uint64, C.c_int, C.c_int, C.POINTER(WorkspaceF32C)]),
     'some_workspace_bytes': (C.c_uint64, [C.c_int, C.c_int, C.c_int]),
     'some_workspace_carve': (C.c_int, [_vp, C.c_uint64, C.c_int, C.c_int, C.c_int, C.POINTER(WorkspaceC)]),
     'some_profiler_create': (C.c_int, [C.c_int, C.POINTER(_vp)]),
@@ -255,6 +259,7 @@ EXPORTS = {
     'some_session_get_stats': (C.c_int, [_vp, C.POINTER(SessionStats)]),
     'some_shard_clips': (C.c_int, [_vp, C.c_int, C.c_int, _vp]),
     'some_session_get_info': (C.c_int, [_vp, C.POINTER(SessionInfo)]),
+    'some_session_get_precision': (C.c_int, [_vp, C.POINTER(C.c_int)]),
     'some_session_transcribe': (C.c_int, [_vp, _vp, _vp, C.c_int, _vp]),
     'some_session_transcribe_sliced': (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.POINTER(SlicerParams), _vp]),
     'some_notes_create': (C.c_int, [C.POINTER(_vp)]),

@@ -280,7 +280,8 @@ def transcribe_recordings(infer_ins, waveforms: Sequence, slicer: Optional[Slice
     the resampler's input."""
     slicer = slicer or Slicer(sr=int(infer_ins.config['audio_sample_rate']), max_sil_kept=1000)   # batch_infer.py:52
     with staged(infer_ins, waveforms, rates) as (wave_d, bases, lens):
-        return infer_ins.model.transcribe_resident(wave_d, bases, lens, slicer, bool(getattr(infer_ins, 'quantized', False)))
+        return infer_ins.model.transcribe_resident(wave_d, bases, lens, slicer, bool(getattr(infer_ins, 'quantized', False)),
+                                                   getattr(infer_ins, 'precision', 'bf16'))
 
 
 def load_wav(path, sr: int) -> np.ndarray:

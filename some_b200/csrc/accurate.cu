@@ -12,6 +12,18 @@
 //   K-dwconv-f32 depthwise k = 31 + folded BatchNorm + SiLU   base_conv.py:66-68
 //   K-head-f32   sigmoid / softmax of the logits         Gmidi_conform.py:33-37
 // LayerNorm and the bound head reuse some_layernorm (fp32 output) / some_bound_head, which are fp32 already.
+//
+// some_forward_f32_tiled runs the same launch sequence with three kernels replaced by register- and shared-memory-tiled
+// ones that keep every output's arithmetic: the same fmaf chains in the same order, the same online-softmax steps and
+// shuffle trees, the same tap chain.  Every workspace buffer it writes is bit-identical to some_forward_f32's, at a large
+// multiple of its speed (BASELINE.md), so the fp32 trunk serves inference and scoring and the checker specifies it:
+//   K-sgemm-tiled   128 x 128 CTA tile, 256 threads x (8 x 8) outputs, k-major operand slices double-buffered in shared
+//                   memory; each output is fmaf(A[m][k], W[n][k], acc) for k = 0 .. K-1 ascending, then the checker's epilogue
+//   K-attn-tiled    one CTA per (clip, head, 64 queries), 8 warps x 8 queries; 32-key K / V tiles staged once per CTA
+//                   (cp.async, double-buffered); lane = key for the scores, lane = channel pair for P.V, as in the checker
+//   K-dwconv-tiled  32 rows x 128 channels per CTA with the 31-tap halo in shared memory, clips found by binary search
+// Where the checker's compiled code contracts or keeps a rounding (cuobjdump -sass), the tiled kernels spell it out
+// (__fmaf_rn / __fmul_rn / __fadd_rn), so their bits do not depend on what the optimiser does with the new loop structure.
 #include "host_common.h"
 
 #include <math.h>
@@ -158,6 +170,306 @@ __global__ void dwconv_f32_kernel(const float* __restrict__ x, const float* __re
   out[(size_t)row * D + c] = acc / (1.0f + expf(-acc));
 }
 
+// ---------------------------------------------------------------------------------------------- K-sgemm-tiled
+constexpr int TG_BM = 128, TG_BN = 128, TG_BK = 16, TG_LD = 128 + 4;   // k-major slices, rows padded to keep float4 reads
+
+template <int EPI>
+__global__ void __launch_bounds__(256)
+sgemm_tiled_kernel(const float* __restrict__ A, int lda, const float* __restrict__ W, const float* __restrict__ bias,
+                   float* C, int ldc, const float* resid, float alpha, int M, int N, int K) {   // resid may alias C
+  __shared__ __align__(16) float sA[2][TG_BK][TG_LD];
+  __shared__ __align__(16) float sW[2][TG_BK][TG_LD];
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const int m0 = blockIdx.y * TG_BM, n0 = blockIdx.x * TG_BN;
+  // loader: rows lr and lr + 64 of both operands, k = lk .. lk + 3 of the slice (zero outside M / N / K, as the checker pads)
+  const int lr = tid >> 2, lk = (tid & 3) * 4;
+  float4 ra[2], rw[2];
+  auto gload = [&](int k0) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = lr + 64 * h;
+      const bool kin = k0 + lk < K;
+      ra[h] = (m0 + r < M && kin) ? *reinterpret_cast<const float4*>(A + (size_t)(m0 + r) * lda + k0 + lk)
+                                  : make_float4(0.f, 0.f, 0.f, 0.f);
+      rw[h] = (n0 + r < N && kin) ? *reinterpret_cast<const float4*>(W + (size_t)(n0 + r) * K + k0 + lk)
+                                  : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  };
+  auto sstore = [&](int buf) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = lr + 64 * h;
+      sA[buf][lk + 0][r] = ra[h].x, sA[buf][lk + 1][r] = ra[h].y, sA[buf][lk + 2][r] = ra[h].z, sA[buf][lk + 3][r] = ra[h].w;
+      sW[buf][lk + 0][r] = rw[h].x, sW[buf][lk + 1][r] = rw[h].y, sW[buf][lk + 2][r] = rw[h].z, sW[buf][lk + 3][r] = rw[h].w;
+    }
+  };
+  // thread (ty, tx) owns rows {ty*4 + i, 64 + ty*4 + i} and columns {tx*4 + j, 64 + tx*4 + j}: conflict-free float4 reads
+  float acc[8][8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
+  gload(0);
+  sstore(0);
+  __syncthreads();
+  int buf = 0;
+  for (int k0 = 0; k0 < K; k0 += TG_BK) {
+    const bool more = k0 + TG_BK < K;
+    if (more) gload(k0 + TG_BK);
+#pragma unroll
+    for (int k = 0; k < TG_BK; ++k) {
+      const float4 a0 = *reinterpret_cast<const float4*>(&sA[buf][k][ty * 4]);
+      const float4 a1 = *reinterpret_cast<const float4*>(&sA[buf][k][64 + ty * 4]);
+      const float4 w0 = *reinterpret_cast<const float4*>(&sW[buf][k][tx * 4]);
+      const float4 w1 = *reinterpret_cast<const float4*>(&sW[buf][k][64 + tx * 4]);
+      const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+      const float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[i][j] = __fmaf_rn(a[i], w[j], acc[i][j]);
+    }
+    if (more) sstore(buf ^ 1);
+    __syncthreads();
+    buf ^= 1;
+  }
+  const bool vec = (ldc & 3) == 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int m = m0 + (i < 4 ? ty * 4 + i : 64 + ty * 4 + i - 4);
+    if (m >= M) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int nb = n0 + 64 * h + tx * 4;
+      float v[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int n = nb + j;
+        if (n >= N) continue;
+        // the checker's epilogue, expression for expression
+        v[j] = acc[i][4 * h + j] + (bias != nullptr ? bias[n] : 0.f);
+        if constexpr (EPI == F32_EPI_SILU) v[j] = v[j] / (1.0f + expf(-v[j]));
+        if constexpr (EPI == F32_EPI_RESID) v[j] = __fmaf_rn(alpha, v[j], resid[(size_t)m * ldc + n]);
+      }
+      float* dst = C + (size_t)m * ldc + nb;
+      if (vec && nb + 3 < N) {
+        *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+      } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (nb + j < N) dst[j] = v[j];
+      }
+    }
+  }
+}
+
+static int sgemm_tiled(int epi, const float* A, int lda, const float* W, const float* bias, float* C, int ldc,
+                       const float* resid, float alpha, int M, int N, int K, cudaStream_t st) {
+  SOME_REQUIRE(K % 4 == 0 && lda % 4 == 0 && (reinterpret_cast<uintptr_t>(A) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(W) & 15) == 0,
+               "some_forward_f32_tiled: GEMM operands must be 16-byte aligned with K and lda multiples of 4 (K=%d lda=%d)", K, lda);
+  const int gy = (M + TG_BM - 1) / TG_BM;
+  SOME_REQUIRE(gy <= 65535, "some_forward_f32_tiled: M=%d is too large for one launch", M);
+  dim3 grid((N + TG_BN - 1) / TG_BN, gy);
+  if (epi == F32_EPI_BIAS) sgemm_tiled_kernel<F32_EPI_BIAS><<<grid, 256, 0, st>>>(A, lda, W, bias, C, ldc, resid, alpha, M, N, K);
+  else if (epi == F32_EPI_SILU) sgemm_tiled_kernel<F32_EPI_SILU><<<grid, 256, 0, st>>>(A, lda, W, bias, C, ldc, resid, alpha, M, N, K);
+  else sgemm_tiled_kernel<F32_EPI_RESID><<<grid, 256, 0, st>>>(A, lda, W, bias, C, ldc, resid, alpha, M, N, K);
+  return check_launch("some_forward_f32_tiled(gemm)");
+}
+
+// ---------------------------------------------------------------------------------------------- K-attn-tiled
+constexpr int FA_WARPS = 8, FA_QPW = 8, FA_Q = FA_WARPS * FA_QPW, FA_KLD = 64 + 4;
+struct FaSmem {
+  float q[FA_Q][64];
+  float k[2][32][FA_KLD];        // key rows padded: lane = key reads its row as float4s without bank conflicts
+  float v[2][32][64];
+  float p[FA_WARPS][FA_QPW][32]; // each warp's probabilities of the current key block, read back as broadcasts
+};
+constexpr int FA_SMEM = sizeof(FaSmem);
+
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool valid) {   // zero-fills when !valid
+  const unsigned s = static_cast<unsigned>(__cvta_generic_to_shared(smem));
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(s), "l"(gmem), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait1() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
+
+__global__ void __launch_bounds__(FA_WARPS * 32)
+attention_f32_tiled_kernel(const float* __restrict__ qkv, float* __restrict__ out, const int32_t* __restrict__ cu) {
+  extern __shared__ __align__(16) unsigned char fa_raw[];
+  FaSmem& sm = *reinterpret_cast<FaSmem*>(fa_raw);
+  const int clip = blockIdx.z, head = blockIdx.y;
+  const int row0 = cu[clip], T = cu[clip + 1] - row0;
+  const int q0 = blockIdx.x * FA_Q;
+  if (q0 >= T) return;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const float* base = qkv + (size_t)row0 * 3 * D + head * 64;
+  for (int i = tid; i < FA_Q * 16; i += FA_WARPS * 32) {
+    const int r = i >> 4, c = (i & 15) * 4;
+    const bool ok = q0 + r < T;
+    cp_async16(&sm.q[r][c], base + (size_t)(ok ? q0 + r : 0) * 3 * D + c, ok);
+  }
+  auto load_kv = [&](int buf, int j0) {
+    for (int i = tid; i < 32 * 16; i += FA_WARPS * 32) {
+      const int r = i >> 4, c = (i & 15) * 4;
+      const bool ok = j0 + r < T;
+      const float* src = base + (size_t)(ok ? j0 + r : 0) * 3 * D + c;
+      cp_async16(&sm.k[buf][r][c], src + D, ok);
+      cp_async16(&sm.v[buf][r][c], src + 2 * D, ok);
+    }
+  };
+  load_kv(0, 0);
+  cp_async_commit();
+  float m[FA_QPW], l[FA_QPW], o0[FA_QPW], o1[FA_QPW];
+#pragma unroll
+  for (int qi = 0; qi < FA_QPW; ++qi) m[qi] = -INFINITY, l[qi] = 0.f, o0[qi] = 0.f, o1[qi] = 0.f;
+  const int nblk = (T + 31) / 32;
+  for (int blk = 0; blk < nblk; ++blk) {
+    const int buf = blk & 1, j0 = blk * 32, j = j0 + lane;
+    if (blk + 1 < nblk) load_kv(buf ^ 1, j0 + 32);
+    cp_async_commit();
+    cp_async_wait1();
+    __syncthreads();
+    // scores of key j for the warp's queries: one ascending fmaf chain over the 64 channels each
+    float s[FA_QPW];
+#pragma unroll
+    for (int qi = 0; qi < FA_QPW; ++qi) s[qi] = 0.f;
+#pragma unroll
+    for (int c = 0; c < 64; c += 4) {
+      const float4 kk = *reinterpret_cast<const float4*>(&sm.k[buf][lane][c]);
+#pragma unroll
+      for (int qi = 0; qi < FA_QPW; ++qi) {
+        const float4 qq = *reinterpret_cast<const float4*>(&sm.q[warp * FA_QPW + qi][c]);
+        s[qi] = __fmaf_rn(qq.x, kk.x, s[qi]);
+        s[qi] = __fmaf_rn(qq.y, kk.y, s[qi]);
+        s[qi] = __fmaf_rn(qq.z, kk.z, s[qi]);
+        s[qi] = __fmaf_rn(qq.w, kk.w, s[qi]);
+      }
+    }
+    // the checker's online-softmax step (lane = key j0 + lane)
+#pragma unroll
+    for (int qi = 0; qi < FA_QPW; ++qi) {
+      const float sc = j < T ? __fmul_rn(s[qi], 0.125f) : -INFINITY;
+      float mx = sc;
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+      const float m_new = fmaxf(m[qi], mx);
+      const float corr = expf(__fsub_rn(m[qi], m_new));
+      const float p = j < T ? expf(__fsub_rn(sc, m_new)) : 0.f;
+      float ps = p;
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) ps = __fadd_rn(ps, __shfl_xor_sync(0xffffffffu, ps, off));
+      l[qi] = __fmaf_rn(l[qi], corr, ps);   // contracted to one FFMA in the checker
+      o0[qi] = __fmul_rn(o0[qi], corr);
+      o1[qi] = __fmul_rn(o1[qi], corr);
+      sm.p[warp][qi][lane] = p;
+      m[qi] = m_new;
+    }
+    __syncwarp();
+    // o = fmaf(p_t, v_t, o) over the block's keys in ascending order; lane owns channels lane and lane + 32
+    const int nk = min(32, T - j0);
+    int t = 0;
+    for (; t + 4 <= nk; t += 4) {
+      float v0[4], v1[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) v0[u] = sm.v[buf][t + u][lane], v1[u] = sm.v[buf][t + u][lane + 32];
+#pragma unroll
+      for (int qi = 0; qi < FA_QPW; ++qi) {
+        const float4 pp = *reinterpret_cast<const float4*>(&sm.p[warp][qi][t]);
+        const float pv[4] = {pp.x, pp.y, pp.z, pp.w};
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          o0[qi] = __fmaf_rn(pv[u], v0[u], o0[qi]);
+          o1[qi] = __fmaf_rn(pv[u], v1[u], o1[qi]);
+        }
+      }
+    }
+    for (; t < nk; ++t) {
+      const float v0 = sm.v[buf][t][lane], v1 = sm.v[buf][t][lane + 32];
+#pragma unroll
+      for (int qi = 0; qi < FA_QPW; ++qi) {
+        const float pt = sm.p[warp][qi][t];
+        o0[qi] = __fmaf_rn(pt, v0, o0[qi]);
+        o1[qi] = __fmaf_rn(pt, v1, o1[qi]);
+      }
+    }
+    __syncthreads();   // every warp is done with this buffer before the next iteration refills it
+  }
+#pragma unroll
+  for (int qi = 0; qi < FA_QPW; ++qi) {
+    const int q = q0 + warp * FA_QPW + qi;
+    if (q >= T) continue;
+    float* dst = out + (size_t)(row0 + q) * D + head * 64;
+    dst[lane] = o0[qi] / l[qi];
+    dst[lane + 32] = o1[qi] / l[qi];
+  }
+}
+
+static int attention_f32_tiled(const float* qkv, float* out, const int32_t* cu, int B, int max_frames, cudaStream_t st) {
+  static bool configured[kMaxDevices] = {};   // function attributes are per device
+  const int dev_ = device_index();
+  if (!configured[dev_]) {
+    cudaError_t e = cudaFuncSetAttribute(attention_f32_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM);
+    SOME_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(attention_f32_tiled): %s", cudaGetErrorString(e));
+    configured[dev_] = true;
+  }
+  SOME_REQUIRE(B <= 65535, "some_forward_f32_tiled: %d clips in one launch, at most 65535", B);
+  dim3 grid((max_frames + FA_Q - 1) / FA_Q, SOME_HEADS, B);
+  attention_f32_tiled_kernel<<<grid, FA_WARPS * 32, FA_SMEM, st>>>(qkv, out, cu);
+  return check_launch("some_forward_f32_tiled(attention)");
+}
+
+// ---------------------------------------------------------------------------------------------- K-dwconv-tiled
+constexpr int DW_ROWS = 32, DW_CH = 128, DW_HALO = SOME_CONV_K / 2;
+
+__global__ void __launch_bounds__(256)
+dwconv_f32_tiled_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
+                        float* __restrict__ out, const int32_t* __restrict__ cu, int B, int M) {
+  __shared__ __align__(16) float sx[DW_ROWS + 2 * DW_HALO][DW_CH];
+  __shared__ int slo[DW_ROWS], shi[DW_ROWS];
+  const int tid = threadIdx.x, r0 = blockIdx.x * DW_ROWS, c0 = blockIdx.y * DW_CH;
+  for (int i = tid; i < (DW_ROWS + 2 * DW_HALO) * (DW_CH / 4); i += 256) {
+    const int rr = i / (DW_CH / 4), cq = (i % (DW_CH / 4)) * 4, g = r0 - DW_HALO + rr;
+    *reinterpret_cast<float4*>(&sx[rr][cq]) = (g >= 0 && g < M) ? *reinterpret_cast<const float4*>(x + (size_t)g * D + c0 + cq)
+                                                                : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  if (tid < DW_ROWS && r0 + tid < M) {   // clip of the row: the last clip whose first frame is <= row
+    const int row = r0 + tid;
+    int lo = 0, hi = B - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (cu[mid] <= row) lo = mid;
+      else hi = mid - 1;
+    }
+    slo[tid] = cu[lo], shi[tid] = cu[lo + 1];
+  }
+  __syncthreads();
+  const int c = tid % DW_CH, rbeg = (tid / DW_CH) * (DW_ROWS / 2);
+  float wk[SOME_CONV_K];
+#pragma unroll
+  for (int k = 0; k < SOME_CONV_K; ++k) wk[k] = w[k * D + c0 + c];
+  const float bias = b[c0 + c];
+  for (int rl = rbeg; rl < rbeg + DW_ROWS / 2; ++rl) {
+    const int row = r0 + rl;
+    if (row >= M) break;
+    const int lo = slo[rl], hi = shi[rl];
+    float acc = bias;
+#pragma unroll
+    for (int k = 0; k < SOME_CONV_K; ++k) {
+      const int r = row + k - DW_HALO;
+      if (r >= lo && r < hi) acc = __fmaf_rn(wk[k], sx[rl + k][c], acc);
+    }
+    out[(size_t)row * D + c0 + c] = acc / (1.0f + expf(-acc));
+  }
+}
+
+static int dwconv_f32_tiled(const float* x, const float* w, const float* b, float* out, const int32_t* cu, int B, int M,
+                            cudaStream_t st) {
+  dim3 grid((M + DW_ROWS - 1) / DW_ROWS, D / DW_CH);
+  dwconv_f32_tiled_kernel<<<grid, 256, 0, st>>>(x, w, b, out, cu, B, M);
+  return check_launch("some_forward_f32_tiled(dwconv)");
+}
+
 // ---------------------------------------------------------------------------------------------- K-head-f32
 __global__ void head_f32_kernel(float* __restrict__ y, int M, int N, int head) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -190,12 +502,32 @@ struct SeqF32 {
   int M, B, max_frames;
   const int32_t* cu;
   cudaStream_t st;
+  bool tiled;    // some_forward_f32_tiled: the tiled GEMM, attention and depthwise conv
   int rc = 0;
 
   void gemm(int epi, int s, const float* A, int lda, const float* W, const float* bias, float* C, int ldc, int N, int K,
             float alpha = 1.0f) {
     if (rc) return;
-    rc = sgemm(epi, A, lda, W, bias, C, ldc, epi == F32_EPI_RESID ? C : nullptr, alpha, M, N, K, st);
+    rc = (tiled ? sgemm_tiled : sgemm)(epi, A, lda, W, bias, C, ldc, epi == F32_EPI_RESID ? C : nullptr, alpha, M, N, K, st);
+  }
+  void attention(const float* qkv, float* out) {
+    if (rc) return;
+    if (tiled) {
+      rc = attention_f32_tiled(qkv, out, cu, B, max_frames, st);
+      return;
+    }
+    dim3 grid((max_frames + 7) / 8, SOME_HEADS, B);
+    attention_f32_kernel<<<grid, 256, 0, st>>>(qkv, out, cu, max_frames);
+    rc = check_launch("some_forward_f32(attention)");
+  }
+  void dwconv(const some_block_weights_f32& w, const float* g, float* out) {
+    if (rc) return;
+    if (tiled) {
+      rc = dwconv_f32_tiled(g, w.w_dw, w.b_dw, out, cu, B, M, st);
+      return;
+    }
+    dwconv_f32_kernel<<<dim3(M, D / 256), 256, 0, st>>>(g, w.w_dw, w.b_dw, out, cu, B);
+    rc = check_launch("some_forward_f32(dwconv)");
   }
   void ln(int s, const float* g, const float* b, float* out) {
     if (rc) return;
@@ -215,19 +547,12 @@ struct SeqF32 {
       if (f == 1) {
         ln(s, w.ln_g[1], w.ln_b[1], a);
         gemm(F32_EPI_BIAS, s, a, D, w.w_qkv, nullptr, qkv, 3 * D, 3 * D, D);
-        if (!rc) {
-          dim3 grid((max_frames + 7) / 8, SOME_HEADS, B);
-          attention_f32_kernel<<<grid, 256, 0, st>>>(qkv, a, cu, max_frames);
-          rc = check_launch("some_forward_f32(attention)");
-        }
+        attention(qkv, a);
         gemm(F32_EPI_RESID, s, a, D, w.w_out, w.b_out, x, D, D, D);
         ln(s, w.ln_g[2], w.ln_b[2], a);
         gemm(F32_EPI_BIAS, s, a, D, w.w_pw1, w.b_pw1, y, 2 * D, 2 * D, D);
         glu(y, g, nullptr);
-        if (!rc) {
-          dwconv_f32_kernel<<<dim3(M, D / 256), 256, 0, st>>>(g, w.w_dw, w.b_dw, a, cu, B);
-          rc = check_launch("some_forward_f32(dwconv)");
-        }
+        dwconv(w, g, a);
         gemm(F32_EPI_RESID, s, a, D, w.w_pw2, w.b_pw2, x, D, D, D);
       }
       ln(s, w.ln_g[f == 0 ? 0 : 3], w.ln_b[f == 0 ? 0 : 3], a);
@@ -238,15 +563,21 @@ struct SeqF32 {
   }
 };
 
-}  // namespace
-
-extern "C" int some_forward_f32(const some_model_f32* m, const some_workspace_f32* ws, int M, int B, const int32_t* cu_frames,
-                                int max_frames, int head, cudaStream_t stream) {
-  SOME_REQUIRE(m != nullptr && ws != nullptr && cu_frames != nullptr && m->blocks != nullptr, "some_forward_f32: null argument");
+int forward_f32(const char* who, bool tiled, const some_model_f32* m, const some_workspace_f32* ws, int M, int B,
+                const int32_t* cu_frames, int max_frames, int head, cudaStream_t stream) {
+  SOME_REQUIRE(m != nullptr && ws != nullptr && cu_frames != nullptr && m->blocks != nullptr, "%s: null argument", who);
   SOME_REQUIRE(head == SOME_EPI_SIGMOID_F32 || head == SOME_EPI_SOFTMAX_F32 || head == SOME_EPI_BIAS_F32,
-               "some_forward_f32: bad head %d", head);
+               "%s: bad head %d", who, head);
   if (M <= 0 || B <= 0) return 0;
-  SeqF32 s{m, ws, M, B, max_frames, cu_frames, stream};
+  if (tiled) {   // the tiled kernels move 16-byte vectors through every workspace buffer
+    bool aligned = (reinterpret_cast<uintptr_t>(ws->units) & 15) == 0 && (reinterpret_cast<uintptr_t>(ws->probs) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(ws->bounds) & 15) == 0;
+    for (int g = 0; g < 2; ++g)
+      for (const float* p : {ws->x[g], ws->a[g], ws->h[g], ws->qkv[g], ws->g[g], ws->y[g]})
+        aligned = aligned && (reinterpret_cast<uintptr_t>(p) & 15) == 0;
+    SOME_REQUIRE(aligned, "%s: every workspace buffer must be 16-byte aligned", who);
+  }
+  SeqF32 s{m, ws, M, B, max_frames, cu_frames, stream, tiled};
   for (int g = 0; g < 2; ++g) s.gemm(F32_EPI_BIAS, g, ws->units, SOME_N_MELS, m->w_in[g], m->b_in[g], ws->x[g], D, D, SOME_N_MELS);
   for (int i = 0; i < m->lay; ++i) {
     for (int g = 0; g < 2; ++g) s.block(g, m->blocks[2 * i + g], false);
@@ -268,4 +599,48 @@ extern "C" int some_forward_f32(const some_model_f32* m, const some_workspace_f3
   }
   if (!s.rc) s.rc = some_bound_head(ws->x[1], w1.ln_g[4], w1.ln_b[4], m->w_cut, m->b_cut, M, ws->bounds, stream);
   return s.rc;
+}
+
+uint64_t carve_f32(Carver& c, int M, int outdim, some_workspace_f32* ws) {
+  const uint64_t m = static_cast<uint64_t>(M > 0 ? M : 0);
+  some_workspace_f32 w{};
+  for (int s = 0; s < 2; ++s) w.x[s] = c.take<float>(m * D * 4);
+  for (int s = 0; s < 2; ++s) w.a[s] = c.take<float>(m * D * 4);
+  for (int s = 0; s < 2; ++s) w.h[s] = c.take<float>(m * FFN * 4);
+  for (int s = 0; s < 2; ++s) w.qkv[s] = c.take<float>(m * 3 * D * 4);
+  for (int s = 0; s < 2; ++s) w.g[s] = c.take<float>(m * D * 4);
+  for (int s = 0; s < 2; ++s) w.y[s] = c.take<float>(m * 2 * D * 4);
+  w.units = c.take<float>(m * SOME_N_MELS * 4);
+  w.probs = c.take<float>(m * static_cast<uint64_t>(outdim) * 4);
+  w.bounds = c.take<float>(m * 4);
+  if (ws != nullptr) *ws = w;
+  return c.off;
+}
+
+}  // namespace
+
+extern "C" int some_forward_f32(const some_model_f32* m, const some_workspace_f32* ws, int M, int B, const int32_t* cu_frames,
+                                int max_frames, int head, cudaStream_t stream) {
+  return forward_f32("some_forward_f32", false, m, ws, M, B, cu_frames, max_frames, head, stream);
+}
+
+extern "C" int some_forward_f32_tiled(const some_model_f32* m, const some_workspace_f32* ws, int M, int B,
+                                      const int32_t* cu_frames, int max_frames, int head, cudaStream_t stream) {
+  return forward_f32("some_forward_f32_tiled", true, m, ws, M, B, cu_frames, max_frames, head, stream);
+}
+
+extern "C" uint64_t some_workspace_f32_bytes(int M, int outdim) {
+  Carver c{nullptr};
+  return carve_f32(c, M, outdim, nullptr);
+}
+
+extern "C" int some_workspace_f32_carve(void* device_block, uint64_t bytes, int M, int outdim, some_workspace_f32* ws) {
+  SOME_REQUIRE(device_block != nullptr && ws != nullptr && M > 0 && outdim >= 1 && outdim <= 256,
+               "some_workspace_f32_carve: bad arguments");
+  SOME_REQUIRE((reinterpret_cast<uintptr_t>(device_block) & 255) == 0, "some_workspace_f32_carve: the block must be 256-byte aligned");
+  SOME_REQUIRE(bytes >= some_workspace_f32_bytes(M, outdim), "some_workspace_f32_carve: block of %llu bytes is too small for M=%d",
+               (unsigned long long)bytes, M);
+  Carver c{static_cast<uint8_t*>(device_block)};
+  carve_f32(c, M, outdim, ws);
+  return 0;
 }

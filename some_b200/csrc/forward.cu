@@ -307,17 +307,7 @@ extern "C" int some_profiler_read(some_profiler* p, int cap, some_profile_record
 
 // ---------------------------------------------------------------------------------------------------- workspace sizing
 namespace {
-struct Carver {
-  uint8_t* base;
-  uint64_t off = 0;
-  template <class T>
-  T* take(uint64_t bytes) {
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += (bytes + 255) & ~uint64_t(255);
-    return p;
-  }
-};
-uint64_t carve(Carver& c, int M, int outdim, int ln_fold, some_workspace* ws) {
+uint64_t carve(some::Carver& c, int M, int outdim, int ln_fold, some_workspace* ws) {
   const uint64_t m = static_cast<uint64_t>(M > 0 ? M : 0);
   some_workspace w{};
   for (int s = 0; s < 2; ++s) w.x[s] = c.take<float>(m * D * 4);
@@ -338,7 +328,7 @@ uint64_t carve(Carver& c, int M, int outdim, int ln_fold, some_workspace* ws) {
 }  // namespace
 
 extern "C" uint64_t some_workspace_bytes(int M, int outdim, int ln_fold) {
-  Carver c{nullptr};
+  some::Carver c{nullptr};
   return carve(c, M, outdim, ln_fold, nullptr);
 }
 extern "C" int some_workspace_carve(void* device_block, uint64_t bytes, int M, int outdim, int ln_fold, some_workspace* ws) {
@@ -346,7 +336,7 @@ extern "C" int some_workspace_carve(void* device_block, uint64_t bytes, int M, i
   SOME_REQUIRE((reinterpret_cast<uintptr_t>(device_block) & 255) == 0, "some_workspace_carve: the block must be 256-byte aligned");
   SOME_REQUIRE(bytes >= some_workspace_bytes(M, outdim, ln_fold), "some_workspace_carve: block of %llu bytes is too small for M=%d",
                (unsigned long long)bytes, M);
-  Carver c{static_cast<uint8_t*>(device_block)};
+  some::Carver c{static_cast<uint8_t*>(device_block)};
   carve(c, M, outdim, ln_fold, ws);
   return 0;
 }

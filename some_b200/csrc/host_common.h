@@ -50,6 +50,18 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
+// Workspace carving: consecutive 256-byte aligned buffers of one device block; with base == nullptr it only sizes them.
+struct Carver {
+  uint8_t* base;
+  uint64_t off = 0;
+  template <class T>
+  T* take(uint64_t bytes) {
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += (bytes + 255) & ~uint64_t(255);
+    return p;
+  }
+};
+
 #define SOME_REQUIRE(cond, ...)      \
   do {                               \
     if (!(cond)) {                   \

@@ -91,6 +91,8 @@ constexpr int pointer_count() {
 #define FIELD(S, f) static_cast<ptrdiff_t>(offsetof(S, f)), pointer_count<decltype(S::f)>()
 #define BLOCK_FIELD(f) FIELD(some_block_weights, f)
 #define MODEL_FIELD(f) FIELD(some_model, f)
+#define BLOCK_FIELD32(f) FIELD(some_block_weights_f32, f)
+#define MODEL_FIELD32(f) FIELD(some_model_f32, f)
 constexpr uint64_t kDim = SOME_DIM, kFfn = 4 * SOME_DIM;
 // The tensors of one block, under "blk<j>." (some_b200/weights.py: BLOCK_TENSORS).
 const Spec kBlockRows[] = {
@@ -104,6 +106,20 @@ const Spec kBlockRows[] = {
     {"w_pw2", DT_BF16, {kDim, kDim}, BLOCK_FIELD(w_pw2)}, {"b_pw2", DT_F32, {kDim}, BLOCK_FIELD(b_pw2)}};
 const Spec kInputRows[] = {{"w_in", DT_BF16, {kDim, SOME_N_MELS}, MODEL_FIELD(w_in)}, {"b_in", DT_F32, {kDim}, MODEL_FIELD(b_in)}};
 const Spec kGluRows[] = {{"w", DT_BF16, {2 * kDim, kDim}}, {"b", DT_F32, {2 * kDim}}};     // under "glu<j>."
+// The fp32 file's tensors (some_b200/weights.py: model_tensors_f32): the same names, order and shapes, every one f32 and bound
+// into some_model_f32 / some_block_weights_f32; b_head is not padded.
+const Spec kBlockRowsF32[] = {
+    {"ln_g", DT_F32, {kDim}, BLOCK_FIELD32(ln_g)}, {"ln_b", DT_F32, {kDim}, BLOCK_FIELD32(ln_b)},
+    {"ffn_w1", DT_F32, {kFfn, kDim}, BLOCK_FIELD32(ffn_w1)}, {"ffn_b1", DT_F32, {kFfn}, BLOCK_FIELD32(ffn_b1)},
+    {"ffn_w2", DT_F32, {kDim, kFfn}, BLOCK_FIELD32(ffn_w2)}, {"ffn_b2", DT_F32, {kDim}, BLOCK_FIELD32(ffn_b2)},
+    {"w_qkv", DT_F32, {3 * kDim, kDim}, BLOCK_FIELD32(w_qkv)},
+    {"w_out", DT_F32, {kDim, kDim}, BLOCK_FIELD32(w_out)}, {"b_out", DT_F32, {kDim}, BLOCK_FIELD32(b_out)},
+    {"w_pw1", DT_F32, {2 * kDim, kDim}, BLOCK_FIELD32(w_pw1)}, {"b_pw1", DT_F32, {2 * kDim}, BLOCK_FIELD32(b_pw1)},
+    {"w_dw", DT_F32, {SOME_CONV_K, kDim}, BLOCK_FIELD32(w_dw)}, {"b_dw", DT_F32, {kDim}, BLOCK_FIELD32(b_dw)},
+    {"w_pw2", DT_F32, {kDim, kDim}, BLOCK_FIELD32(w_pw2)}, {"b_pw2", DT_F32, {kDim}, BLOCK_FIELD32(b_pw2)}};
+const Spec kInputRowsF32[] = {{"w_in", DT_F32, {kDim, SOME_N_MELS}, MODEL_FIELD32(w_in)},
+                              {"b_in", DT_F32, {kDim}, MODEL_FIELD32(b_in)}};
+const Spec kGluRowsF32[] = {{"w", DT_F32, {2 * kDim, kDim}}, {"b", DT_F32, {2 * kDim}}};
 
 template <size_t n>
 void add_rows(std::vector<Spec>& v, const std::string& prefix, int block, const Spec (&rows)[n]) {
@@ -119,20 +135,33 @@ void add_rows(std::vector<Spec>& v, const std::string& prefix, int block, const 
   }
 }
 
-// The tensors a file of this geometry must hold, in file order (some_b200/export.py: tensor_specs writes the same list).
-std::vector<Spec> expected_tensors(int lay, int outdim) {
-  const Spec head[] = {
-      {"w_head", DT_BF16, {static_cast<uint64_t>(outdim), kDim}, MODEL_FIELD(w_head)},
-      {"b_head", DT_F32, {static_cast<uint64_t>((outdim + 31) / 32 * 32)}, MODEL_FIELD(b_head)},
-      {"w_cut", DT_F32, {kDim}, MODEL_FIELD(w_cut)}, {"b_cut", DT_F32, {1}},
+// The tensors a file of this geometry and precision must hold, in file order (some_b200/export.py: tensor_specs writes the
+// same list).
+std::vector<Spec> expected_tensors(int lay, int outdim, int precision) {
+  const bool f32 = precision == SOME_PRECISION_FP32;
+  const uint64_t n = static_cast<uint64_t>(outdim), n32 = static_cast<uint64_t>((outdim + 31) / 32 * 32);
+  const Spec front[] = {
       {"mel_start", DT_I32, {SOME_N_MELS}}, {"mel_count", DT_I32, {SOME_N_MELS}},
       {"mel_weights", DT_F32, {SOME_N_MELS, SOME_MEL_MAXW}}, {"twiddle", DT_F32, {SOME_MEL_TW, 2}},
       {"window", DT_F32, {SOME_N_FFT}}, {"kaiser_best", DT_F64, {kKaiserTaps}}};
+  const Spec head[] = {{"w_head", DT_BF16, {n, kDim}, MODEL_FIELD(w_head)}, {"b_head", DT_F32, {n32}, MODEL_FIELD(b_head)},
+                       {"w_cut", DT_F32, {kDim}, MODEL_FIELD(w_cut)}, {"b_cut", DT_F32, {1}}};
+  const Spec head32[] = {{"w_head", DT_F32, {n, kDim}, MODEL_FIELD32(w_head)}, {"b_head", DT_F32, {n}, MODEL_FIELD32(b_head)},
+                         {"w_cut", DT_F32, {kDim}, MODEL_FIELD32(w_cut)}, {"b_cut", DT_F32, {1}}};
   std::vector<Spec> v;
-  add_rows(v, "", -1, kInputRows);
-  for (int j = 0; j < 2 * (lay + 1); ++j) add_rows(v, "blk" + std::to_string(j) + ".", j, kBlockRows);
-  for (int j = 0; j < 2 * lay; ++j) add_rows(v, "glu" + std::to_string(j) + ".", -1, kGluRows);
-  add_rows(v, "", -1, head);
+  if (f32) add_rows(v, "", -1, kInputRowsF32);
+  else add_rows(v, "", -1, kInputRows);
+  for (int j = 0; j < 2 * (lay + 1); ++j) {
+    if (f32) add_rows(v, "blk" + std::to_string(j) + ".", j, kBlockRowsF32);
+    else add_rows(v, "blk" + std::to_string(j) + ".", j, kBlockRows);
+  }
+  for (int j = 0; j < 2 * lay; ++j) {
+    if (f32) add_rows(v, "glu" + std::to_string(j) + ".", -1, kGluRowsF32);
+    else add_rows(v, "glu" + std::to_string(j) + ".", -1, kGluRows);
+  }
+  if (f32) add_rows(v, "", -1, head32);
+  else add_rows(v, "", -1, head);
+  add_rows(v, "", -1, front);
   return v;
 }
 
@@ -294,6 +323,10 @@ struct Replica {
   std::vector<const uint16_t*> glu_w;
   std::vector<const float*> glu_b;
   some_model model{};
+  // an fp32 file's model (some_session_get_precision): bound instead of `model`, run by some_forward_f32_tiled
+  std::vector<some_block_weights_f32> blocks32;
+  std::vector<const float*> glu_w32;
+  some_model_f32 model32{};
   const int32_t *mel_start = nullptr, *mel_count = nullptr;
   const float *mel_weights = nullptr, *twiddle = nullptr, *window = nullptr;
   cudaStream_t stream = nullptr, copy_stream = nullptr;
@@ -303,6 +336,7 @@ struct Replica {
   PinBuf wave_h, tab_h, cu_h, slab_h;
   int ws_m = 0;
   some_workspace ws{};
+  some_workspace_f32 ws32{};
   std::unique_ptr<WorkerPool> pool;       // its staging lanes (WorkerPool::run is not re-entrant)
   some_notes part;                        // the notes of its share of the step's chunks, in its order (no ranges)
   int64_t chunks = 0, frames = 0;         // its share of the step in progress
@@ -318,6 +352,7 @@ struct some_session {
   bool running = false;
   some_session_stats stats{};
   some_session_info info{};
+  int precision = SOME_PRECISION_BF16;
   float vmin = 0.f, vmax = 0.f, deviation = 1.f, threshold = 0.1f;
   std::vector<double> kaiser;             // host copy of the float64 table (scaled per rate pair on upload)
   // the device tables by downsampling ratio (1.0: the unscaled table every upsampling pair shares), each kept with the host
@@ -494,10 +529,13 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
     max_mc = std::max(max_mc, mc);
   }
   // buffers
+  const bool f32 = s->precision == SOME_PRECISION_FP32;
   if (max_mc > r.ws_m) {
-    const uint64_t bytes = some_workspace_bytes(max_mc, s->info.outdim, 0);
+    const uint64_t bytes = f32 ? some_workspace_f32_bytes(max_mc, s->info.outdim) : some_workspace_bytes(max_mc, s->info.outdim, 0);
     if (r.ws_block.ensure(bytes, "the workspace")) return -1;
-    if (some_workspace_carve(r.ws_block.p, r.ws_block.cap, max_mc, s->info.outdim, 0, &r.ws)) return -1;
+    if (f32 ? some_workspace_f32_carve(r.ws_block.p, r.ws_block.cap, max_mc, s->info.outdim, &r.ws32)
+            : some_workspace_carve(r.ws_block.p, r.ws_block.cap, max_mc, s->info.outdim, 0, &r.ws))
+      return -1;
     if (r.scratch.ensure(some_decode_scratch_bytes(max_mc), "the decode scratch")) return -1;
     r.ws_m = max_mc;
   }
@@ -515,6 +553,8 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
   int32_t* cu_d = static_cast<int32_t*>(r.cu_d.p);
   uint8_t* slab = static_cast<uint8_t*>(r.slab_d.p);
   const int head = s->info.quantized ? SOME_EPI_SOFTMAX_F32 : SOME_EPI_SIGMOID_F32;
+  const float* probs = f32 ? r.ws32.probs : r.ws.probs;
+  const float* bounds = f32 ? r.ws32.bounds : r.ws.bounds;
 
   for (size_t ci = 0; ci < layout.size(); ++ci) {
     const Chunk& ch = layout[ci];
@@ -547,13 +587,16 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
 
     const int32_t* cud = cu_d + ch.c0 + ci;
     uint8_t* o = slab + ch.off;
+    // an fp32 session writes the mel as f32 and runs the fp32 trunk (Engine.enqueue(..., precision='fp32'))
     if (some_mel_logmel(wave + lo, tab_d + 2 * ch.c0, tab_d + 2 * ch.c0 + ch.bc, cud, ch.bc, max_frames, r.mel_start,
-                        r.mel_count, r.mel_weights, r.twiddle, r.window, nullptr, const_cast<uint16_t*>(r.ws.units), 1e-5f,
-                        r.stream))
+                        r.mel_count, r.mel_weights, r.twiddle, r.window, f32 ? const_cast<float*>(r.ws32.units) : nullptr,
+                        f32 ? nullptr : const_cast<uint16_t*>(r.ws.units), 1e-5f, r.stream))
       return -1;
-    if (some_forward(&r.model, &r.ws, ch.mc, ch.bc, cud, max_frames, head, nullptr, nullptr, r.stream)) return -1;
+    if (f32 ? some_forward_f32_tiled(&r.model32, &r.ws32, ch.mc, ch.bc, cud, max_frames, head, r.stream)
+            : some_forward(&r.model, &r.ws, ch.mc, ch.bc, cud, max_frames, head, nullptr, nullptr, r.stream))
+      return -1;
     some_decode_args d{};
-    d.probs = r.ws.probs, d.bounds = r.ws.bounds, d.cu_frames = cud;
+    d.probs = probs, d.bounds = bounds, d.cu_frames = cud;
     d.B = ch.bc, d.M = ch.mc, d.N = s->info.outdim, d.quantized = s->info.quantized;
     d.vmin = s->vmin, d.vmax = s->vmax, d.deviation = s->deviation, d.threshold = s->threshold;
     d.note_count = reinterpret_cast<int32_t*>(o);
@@ -569,7 +612,7 @@ int run_batch(const some_session* s, Replica& r, const float* const* host, const
     }
     if (some_decode_notes(&d, r.stream)) return -1;
     if (s->frames)
-      SOME_CUDA(cudaMemcpyAsync(f + 4ull * ch.mc, r.ws.bounds, 4ull * ch.mc, cudaMemcpyDeviceToDevice, r.stream), "bounds copy");
+      SOME_CUDA(cudaMemcpyAsync(f + 4ull * ch.mc, bounds, 4ull * ch.mc, cudaMemcpyDeviceToDevice, r.stream), "bounds copy");
   }
   if (slab_bytes) SOME_CUDA(cudaMemcpyAsync(r.slab_h.p, slab, slab_bytes, cudaMemcpyDeviceToHost, r.stream), "note download");
   SOME_CUDA(cudaStreamSynchronize(r.stream), "synchronise");
@@ -760,26 +803,37 @@ constexpr int kMaxReplicas = 64;
 
 // Points a replica's model and mel tables into its copy of the weights; dp(name) is a tensor's device address there.
 template <class Dp>
-void bind_weights(Replica& r, const std::vector<Spec>& specs, int lay, int outdim, Dp dp) {
+void bind_weights(Replica& r, const std::vector<Spec>& specs, int lay, int outdim, bool f32, Dp dp) {
   auto fl = [&](const std::string& n) { return static_cast<const float*>(dp(n)); };
   some_model& m = r.model;
-  r.blocks.resize(2 * (lay + 1));            // value-initialised: the LayerNorm-folded fields stay null
+  some_model_f32& m32 = r.model32;
+  if (f32) r.blocks32.resize(2 * (lay + 1));
+  else r.blocks.resize(2 * (lay + 1));       // value-initialised: the LayerNorm-folded fields stay null
   for (const Spec& sp : specs) {
     if (sp.field < 0) continue;
     const void* p = dp(sp.name);
-    void* target = sp.block < 0 ? static_cast<void*>(&m) : static_cast<void*>(&r.blocks[sp.block]);
+    void* target = f32 ? (sp.block < 0 ? static_cast<void*>(&m32) : static_cast<void*>(&r.blocks32[sp.block]))
+                       : (sp.block < 0 ? static_cast<void*>(&m) : static_cast<void*>(&r.blocks[sp.block]));
     memcpy(static_cast<uint8_t*>(target) + sp.field, &p, sizeof(p));
   }
   for (int j = 0; j < 2 * lay; ++j) {
-    r.glu_w.push_back(static_cast<const uint16_t*>(dp("glu" + std::to_string(j) + ".w")));
+    if (f32) r.glu_w32.push_back(fl("glu" + std::to_string(j) + ".w"));
+    else r.glu_w.push_back(static_cast<const uint16_t*>(dp("glu" + std::to_string(j) + ".w")));
     r.glu_b.push_back(fl("glu" + std::to_string(j) + ".b"));
   }
-  if (lay == 0) r.glu_w.push_back(nullptr), r.glu_b.push_back(nullptr);
-  m.lay = lay, m.outdim = outdim;
-  m.blocks = r.blocks.data();
-  m.glu_w = r.glu_w.data();
-  m.glu_b = r.glu_b.data();
-  m.ln_fold = 0;                                  // the default stand-alone LayerNorm sequence
+  if (lay == 0) r.glu_w.push_back(nullptr), r.glu_w32.push_back(nullptr), r.glu_b.push_back(nullptr);
+  if (f32) {
+    m32.lay = lay, m32.outdim = outdim;
+    m32.blocks = r.blocks32.data();
+    m32.glu_w = r.glu_w32.data();
+    m32.glu_b = r.glu_b.data();
+  } else {
+    m.lay = lay, m.outdim = outdim;
+    m.blocks = r.blocks.data();
+    m.glu_w = r.glu_w.data();
+    m.glu_b = r.glu_b.data();
+    m.ln_fold = 0;                                // the default stand-alone LayerNorm sequence
+  }
   r.mel_start = static_cast<const int32_t*>(dp("mel_start"));
   r.mel_count = static_cast<const int32_t*>(dp("mel_count"));
   r.mel_weights = fl("mel_weights"), r.twiddle = fl("twiddle"), r.window = fl("window");
@@ -813,6 +867,7 @@ int open_session(const char* who, const char* path, const int* devices, int n, b
   const int32_t lay = rd<int32_t>(f + 36), outdim = rd<int32_t>(f + 40), quantized = rd<int32_t>(f + 44);
   const int32_t sr = rd<int32_t>(f + 48), hop = rd<int32_t>(f + 52), win = rd<int32_t>(f + 56);
   const int32_t bias_corrected = rd<int32_t>(f + 76);
+  const int32_t precision = rd<int32_t>(f + 88);    // zero in bf16 files
   SOME_REQUIRE(dir_off >= kHeaderBytes && dir_off <= size && n_tensors <= (size - dir_off) / kEntryBytes,
                "%s: truncated directory (%u entries at byte %llu, file of %llu bytes)", path, n_tensors,
                (unsigned long long)dir_off, (unsigned long long)size);
@@ -824,6 +879,8 @@ int open_session(const char* who, const char* path, const int* devices, int n, b
                    hop == SOME_HOP && win == SOME_N_FFT,
                "%s: unsupported model scalars (lay %d, outdim %d, quantized %d, rate %d, hop %d, win %d)", path, lay, outdim,
                quantized, sr, hop, win);
+  SOME_REQUIRE(precision == SOME_PRECISION_BF16 || precision == SOME_PRECISION_FP32,
+               "%s: unknown precision %d in the header (0 = bf16, 1 = fp32)", path, precision);
   // ---- directory
   struct Entry {
     uint32_t dtype;
@@ -855,13 +912,14 @@ int open_session(const char* who, const char* path, const int* devices, int n, b
                  name, (unsigned long long)en.bytes, (unsigned long long)(elems * dtype_bytes(en.dtype)));
     SOME_REQUIRE(dir.emplace(name, en).second, "%s: tensor '%s' appears twice", path, name);
   }
-  const std::vector<Spec> specs = expected_tensors(lay, outdim);
+  const std::vector<Spec> specs = expected_tensors(lay, outdim, precision);
   for (const Spec& sp : specs) {
     auto it = dir.find(sp.name);
     SOME_REQUIRE(it != dir.end(), "%s: missing tensor '%s'", path, sp.name.c_str());
     SOME_REQUIRE(it->second.dtype == sp.dtype && it->second.shape == sp.shape,
-                 "%s: tensor '%s' is %s %s, a model with lay %d / outdim %d needs %s %s", path, sp.name.c_str(),
-                 dtype_name(it->second.dtype), shape_str(it->second.shape).c_str(), lay, outdim, dtype_name(sp.dtype),
+                 "%s: tensor '%s' is %s %s, a%s model with lay %d / outdim %d needs %s %s", path, sp.name.c_str(),
+                 dtype_name(it->second.dtype), shape_str(it->second.shape).c_str(),
+                 precision == SOME_PRECISION_FP32 ? "n fp32" : " bf16", lay, outdim, dtype_name(sp.dtype),
                  shape_str(sp.shape).c_str());
   }
   SOME_REQUIRE(dir.size() == specs.size(), "%s: %zu tensors, a model with lay %d / outdim %d has %zu", path, dir.size(), lay,
@@ -914,10 +972,10 @@ int open_session(const char* who, const char* path, const int* devices, int n, b
       set_error("%s: %suploading %s: %s", who, at, path, cudaGetErrorString(e));
       return fail(-2);
     }
-    bind_weights(r, specs, lay, outdim, [&](const std::string& name) -> const void* {
+    bind_weights(r, specs, lay, outdim, precision == SOME_PRECISION_FP32, [&](const std::string& name) -> const void* {
       return static_cast<uint8_t*>(r.weights) + (dir.at(name).off - data_off);
     });
-    r.model.b_cut = rd<float>(f + dir.at("b_cut").off);   // a host scalar of some_model
+    r.model.b_cut = r.model32.b_cut = rd<float>(f + dir.at("b_cut").off);   // a host scalar of the model
     r.pool.reset(new WorkerPool(lanes));
   }
   s->stream = s->reps[0]->stream;
@@ -940,6 +998,7 @@ int open_session(const char* who, const char* path, const int* devices, int n, b
   s->info.outdim = outdim;
   s->info.quantized = quantized;
   s->info.bias_corrected = bias_corrected;
+  s->precision = precision;
   s->info.timestep = static_cast<double>(hop) / static_cast<double>(sr);    // base_infer.py:20
   s->vmin = rd<float>(f + 60), s->vmax = rd<float>(f + 64), s->deviation = rd<float>(f + 68), s->threshold = rd<float>(f + 72);
   *out = s;
@@ -1020,6 +1079,12 @@ extern "C" int some_session_close(some_session* s) {
 extern "C" int some_session_get_info(const some_session* s, some_session_info* info) {
   SOME_REQUIRE(s != nullptr && info != nullptr, "some_session_get_info: null pointer");
   *info = s->info;
+  return 0;
+}
+
+extern "C" int some_session_get_precision(const some_session* s, int* precision) {
+  SOME_REQUIRE(s != nullptr && precision != nullptr, "some_session_get_precision: null pointer");
+  *precision = s->precision;
   return 0;
 }
 

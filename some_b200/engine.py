@@ -69,6 +69,38 @@ class _Workspace:
         c.units, c.probs, c.bounds = self.units.data_ptr(), self.probs.data_ptr(), self.bounds.data_ptr()
 
 
+class _WorkspaceF32:
+    """fp32 trunk buffers for up to m rows: one device block carved by some_workspace_f32_carve (the layout the native
+    session uses), torch views of the mel input and the probs / bounds outputs, and the decode's own notes and scratch."""
+
+    def __init__(self, m: int, outdim: int, device):
+        lib = _lib.load()
+        self.m = m
+        nbytes = int(lib.some_workspace_f32_bytes(m, outdim))
+        self.block = torch.empty(nbytes + 256, dtype=torch.uint8, device=device)
+        base = (self.block.data_ptr() + 255) & ~255
+        c = self.c = _lib.WorkspaceF32C()
+        _lib.check(lib.some_workspace_f32_carve(base, nbytes, m, outdim, C.byref(c)), 'some_workspace_f32_carve')
+
+        def view(ptr, *shape):
+            off = ptr - self.block.data_ptr()
+            return self.block[off:off + 4 * int(np.prod(shape))].view(torch.float32).view(*shape)
+        self.units, self.probs, self.bounds = view(c.units, m, 80), view(c.probs, m, outdim), view(c.bounds, m)
+        self.note_midi = torch.empty((m,), dtype=torch.float32, device=device)
+        self.note_dur = torch.empty((m,), dtype=torch.int32, device=device)
+        self.note_rest = torch.empty((m,), dtype=torch.uint8, device=device)
+        self.scratch = torch.empty((int(lib.some_decode_scratch_bytes(m)),), dtype=torch.uint8, device=device)
+
+
+PRECISIONS = ('bf16', 'fp32')
+
+
+def check_precision(precision: str) -> str:
+    if precision not in PRECISIONS:
+        raise ValueError(f"precision must be 'bf16' or 'fp32', got {precision!r}")
+    return precision
+
+
 class Engine:
     def __init__(self, config: dict, state_dict, device='cuda'):
         self.lib = _lib.load()
@@ -87,6 +119,7 @@ class Engine:
         self.outdim = config['midi_num_bins']
         self.timestep = config['hop_size'] / config['audio_sample_rate']
         self._ws: Optional[_Workspace] = None
+        self._ws32: Optional[_WorkspaceF32] = None
         self.launches = 0
         self._sum_t2 = 0.0
         # launches of one trunk pass: inln (+ row_stats) + (lay + 1) blocks x 11 (15 unfolded) + lay GLU mixes
@@ -240,6 +273,19 @@ class Engine:
             self._ws = _Workspace(max(m, 1), self.outdim, self.device)
         return self._ws
 
+    def workspace_f32(self, m: int) -> _WorkspaceF32:
+        if self._ws32 is None or self._ws32.m < m:
+            self._ws32 = None
+            self._ws32 = _WorkspaceF32(max(m, 1), self.outdim, self.device)
+        return self._ws32
+
+    def model_f32(self):
+        """The checkpoint's fp32 tensors (weights.build_f32_model) on this engine's device, uploaded on first use."""
+        if self._f32 is None:
+            from .weights import build_f32_model
+            self._f32 = build_f32_model(self._state_dict, self.config, self.device)
+        return self._f32[0]
+
     # ------------------------------------------------------------------ stages
     def run_mel(self, wave: torch.Tensor, clip_start: torch.Tensor, clip_len: torch.Tensor, cu_frames: torch.Tensor,
                 b: int, max_frames: int, out_f32: Optional[torch.Tensor], out_bf16: Optional[torch.Tensor]):
@@ -263,6 +309,18 @@ class Engine:
         _lib.check(self.lib.some_forward(C.byref(self._cmodel), C.byref(ws.c), m, b, cu_frames.data_ptr(), max_frames,
                                          epi, prof, None, self._stream), 'some_forward')
         self.launches += self.trunk_launches
+
+    def run_trunk_f32(self, ws: _WorkspaceF32, m: int, b: int, cu_frames: torch.Tensor, max_frames: int,
+                      head: str = 'sigmoid'):
+        """The fp32 trunk (some_forward_f32_tiled, csrc/accurate.cu): the bits of the fp32 checker at batch speed.  Reads
+        ws.units; writes ws.probs [m, outdim] and ws.bounds [m]."""
+        epi = {'sigmoid': _lib.EPI_SIGMOID_F32, 'softmax': _lib.EPI_SOFTMAX_F32, 'logits': _lib.EPI_BIAS_F32}[head]
+        _lib.check(self.lib.some_forward_f32_tiled(C.byref(self.model_f32()), C.byref(ws.c), m, b, cu_frames.data_ptr(),
+                                                   max_frames, epi, self._stream), 'some_forward_f32_tiled')
+        # 2 input GEMMs, 15 launches per block and stream, norm5 + 2 GEMMs + 2 GLUs per layer, final LN + head GEMM +
+        # bound head, and the activation kernel unless the raw logits are asked for
+        lay = self.w.lay
+        self.launches += 2 + 30 * (lay + 1) + 6 * lay + 3 + int(head != 'logits')
 
     def run_decode(self, ws: _Workspace, m: int, b: int, cu_frames: torch.Tensor, note_count: torch.Tensor,
                    quantized: bool, dbg: Optional[dict] = None, probs=None, bounds=None, out=None):
@@ -415,7 +473,8 @@ class Engine:
         return cu, layout, off
 
     def enqueue(self, waveforms: Sequence[np.ndarray], quantized: bool = False, return_intermediates: bool = False,
-                resident=None, out: Optional[torch.Tensor] = None, logits_hook: Optional[Callable] = None):
+                resident=None, out: Optional[torch.Tensor] = None, logits_hook: Optional[Callable] = None,
+                precision: str = 'bf16'):
         """Stages, copies and enqueues the whole batch WITHOUT synchronising.  Returns (device slab uint8 [nbytes], cu, layout,
         extra): the decoded notes land in the device slab (see slab_layout); the caller copies it to the host (infer) or
         hands it to the all-gather (dist.infer_sharded).
@@ -436,7 +495,12 @@ class Engine:
         chunk-relative cu_frames cu_d) between the trunk and the decode.  With a hook the trunk writes the raw logits
         (SOME_EPI_BIAS_F32) into ``ws.probs[:mc]`` and the hook must leave there the probabilities the decode reads
         (some_eval_clips does both in one pass: the evaluator, some_b200/evaluate.py).  Without one (the default) the trunk
-        applies the sigmoid / softmax head itself."""
+        applies the sigmoid / softmax head itself.
+
+        ``precision='fp32'``: the trunk runs in fp32 on the CUDA cores (some_forward_f32_tiled, bit-identical to the fp32
+        checker behind infer_accurate) on an fp32 workspace, the mel is written as f32, and no chunk is replayed as a CUDA
+        graph; staging, chunks, decode and the slab are the same."""
+        fp32 = check_precision(precision) == 'fp32'
         dev = self.device
         if resident is not None:
             wave_res, ranges = resident
@@ -484,7 +548,7 @@ class Engine:
             direct = [bool(lens[i]) and w.dtype == np.float32 and w.flags.c_contiguous and torch.from_numpy(w).is_pinned()
                       for i, w in enumerate(waveforms)]
 
-        ws = self.workspace(max(mc for *_, mc in layout))
+        ws = (self.workspace_f32 if fp32 else self.workspace)(max(mc for *_, mc in layout))
         extra = None
         cu_h, cu_dev = st['cu_h'], st['cu_d']
         for ci, (c0, c1, out_off, bc, mc) in enumerate(layout):
@@ -527,24 +591,28 @@ class Engine:
             note_dur = o[4 * bc:4 * bc + 4 * mc].view(torch.int32)
             note_midi = o[4 * bc + 4 * mc:4 * bc + 8 * mc].view(torch.float32)
             note_rest = o[4 * bc + 8 * mc:]
-            mel_f32 = torch.empty((mc, 80), dtype=torch.float32, device=dev) if return_intermediates else None
+            mel_f32 = torch.empty((mc, 80), dtype=torch.float32, device=dev) if return_intermediates and not fp32 else None
             pdl = self.pdl == 'all' or (self.pdl == 'small' and mc <= self.GRAPH_MAX_FRAMES)
+            head = 'logits' if logits_hook is not None else 'softmax' if quantized else 'sigmoid'
 
             def launch_chunk():
-                self.run_mel(wave_d[lo:], tab_dev[:bc], tab_dev[bc:2 * bc], cu_d, bc, max_frames, mel_f32, ws.units)
-                was = self.lib.some_set_pdl(1) if pdl else 0    # programmatic dependent launch of the trunk kernels
-                try:
-                    self.run_trunk(ws, mc, bc, cu_d, max_frames,
-                                   'logits' if logits_hook is not None else 'softmax' if quantized else 'sigmoid')
-                finally:
-                    if pdl:
-                        self.lib.some_set_pdl(was)
+                if fp32:
+                    self.run_mel(wave_d[lo:], tab_dev[:bc], tab_dev[bc:2 * bc], cu_d, bc, max_frames, ws.units[:mc], None)
+                    self.run_trunk_f32(ws, mc, bc, cu_d, max_frames, head)
+                else:
+                    self.run_mel(wave_d[lo:], tab_dev[:bc], tab_dev[bc:2 * bc], cu_d, bc, max_frames, mel_f32, ws.units)
+                    was = self.lib.some_set_pdl(1) if pdl else 0    # programmatic dependent launch of the trunk kernels
+                    try:
+                        self.run_trunk(ws, mc, bc, cu_d, max_frames, head)
+                    finally:
+                        if pdl:
+                            self.lib.some_set_pdl(was)
                 if logits_hook is not None:
                     logits_hook(ws, c0, c1, mc, cu_d)
                 self.run_decode(ws, mc, bc, cu_d, note_count, quantized, out=(note_midi, note_dur, note_rest))
 
             if (mc <= self.GRAPH_MAX_FRAMES and self.use_graphs and self.prof is None and not return_intermediates
-                    and logits_hook is None):
+                    and logits_hook is None and not fp32):
                 # small batches are launch-bound (~56 launches of a few microseconds each): replay them as ONE CUDA graph,
                 # keyed by everything the captured kernel arguments depend on
                 self._graphed((wave_d.data_ptr() + 4 * lo, tab_dev.data_ptr(), cu_d.data_ptr(), o.data_ptr(), ws.serial, bc, mc,
@@ -552,23 +620,24 @@ class Engine:
             else:
                 launch_chunk()
             if return_intermediates:
-                extra = (mel_f32, ws.probs[:mc], ws.bounds[:mc])
+                extra = (ws.units[:mc] if fp32 else mel_f32, ws.probs[:mc], ws.bounds[:mc])
         self._h2d_done = ev if layout else None
         return out_d[:nbytes_total], cu, layout, extra
 
     def transcribe_resident(self, wave_d: torch.Tensor, bases: Sequence[int], lens: Sequence[int], slicer,
-                            quantized: bool = False) -> List[tuple]:
+                            quantized: bool = False, precision: str = 'bf16') -> List[tuple]:
         """Recordings already on the device (recording i = ``wave_d[bases[i] : bases[i] + lens[i]]``) -> per recording
         (chunk offsets in seconds, per-chunk notes), as ``Slicer.slice`` then ``infer`` on the chunks would give.  The RMS
         lists of the recordings that may be cut come back in one copy (slicer.rms_lists), the slicer's decisions are taken on
         the host, and the chunks of all recordings run where they lie as one var-len batch whose notes land in the pinned
-        landing buffer with one synchronise.  Call on the engine's device."""
+        landing buffer with one synchronise.  ``precision`` as in enqueue().  Call on the engine's device."""
+        check_precision(precision)
         per_rec = cut_ranges(slicer, lens, lambda need: rms_lists(
             [wave_d[bases[i]:bases[i] + lens[i]] for i in need], slicer.win_size, slicer.hop_size))
         flat = [(int(bases[i]) + a, int(bases[i]) + b) for i, rs in enumerate(per_rec) for a, b in rs]
         results: List[Dict[str, np.ndarray]] = []
         if flat:
-            slab, cu, layout, _ = self.enqueue(None, quantized, resident=(wave_d, flat))
+            slab, cu, layout, _ = self.enqueue(None, quantized, resident=(wave_d, flat), precision=precision)
             out_h = self._stage['out_h'][:slab.numel()]
             out_h.copy_(slab, non_blocking=True)
             torch.cuda.current_stream(self.device).synchronize()
@@ -579,16 +648,17 @@ class Engine:
             k += len(rs)
         return out
 
-    def infer_sliced(self, waveform: np.ndarray, slicer, quantized: bool = False):
+    def infer_sliced(self, waveform: np.ndarray, slicer, quantized: bool = False, precision: str = 'bf16'):
         """One long mono recording -> (chunk offsets in seconds, per-chunk notes): the flow of infer.py:38-41 /
         batch_infer.py:50-54 (Slicer.slice, then infer on the chunks) with the recording uploaded ONCE and cut and run on the
         device by ``transcribe_resident``.  A recording the slicer leaves whole (slicer.one_chunk, also the empty one) is not
-        uploaded here but goes to ``infer``, whose small batches replay as CUDA graphs."""
+        uploaded here but goes to ``infer``, whose small batches replay as CUDA graphs.  ``precision`` as in infer()."""
+        check_precision(precision)
         samples = np.ascontiguousarray(waveform, dtype=np.float32)
         assert samples.ndim == 1, 'infer_sliced expects a mono waveform (infer.py loads with mono=True)'
         n = int(samples.shape[0])
         if one_chunk(slicer, n):
-            return [0], self.infer([samples], quantized)
+            return [0], self.infer([samples], quantized, precision=precision)
         with torch.cuda.device(self.device):
             src = torch.from_numpy(samples)
             if not src.is_pinned():
@@ -597,7 +667,7 @@ class Engine:
                 src = st['wave_h'][:n]
             wave_d = torch.empty(n, dtype=torch.float32, device=self.device)
             wave_d.copy_(src, non_blocking=True)
-            [(offsets, results)] = self.transcribe_resident(wave_d, [0], [n], slicer, quantized)
+            [(offsets, results)] = self.transcribe_resident(wave_d, [0], [n], slicer, quantized, precision)
         return offsets, results
 
     def unpack_slab(self, host: np.ndarray, cu: np.ndarray, layout, extra=None) -> List[Dict[str, np.ndarray]]:
@@ -612,18 +682,22 @@ class Engine:
         return results
 
     def infer(self, waveforms: Sequence[np.ndarray], quantized: bool = False,
-              return_intermediates: bool = False) -> List[Dict[str, np.ndarray]]:
+              return_intermediates: bool = False, precision: str = 'bf16') -> List[Dict[str, np.ndarray]]:
         """waveform-in -> notes-out for a list of clips: the batched equivalent of BaseInference.infer
         (base_infer.py:46-53).  Host buffers in, host buffers out.  The batch is cut into up to 3 chunks of whole clips
         (small first chunk); for each chunk the clips are staged into pinned memory by a small thread pool (memcpy releases
         the GIL), copied H2D on a copy stream, and the kernels of the chunk are enqueued behind an event — so staging and
         H2D of chunk c+1 overlap the kernels of chunk c.  The notes come back in ONE packed D2H copy
-        [counts | dur | midi | rest] per chunk slab; there is a single host synchronisation at the end."""
+        [counts | dur | midi | rest] per chunk slab; there is a single host synchronisation at the end.
+
+        ``precision='fp32'``: the trunk in fp32 (some_forward_f32_tiled): notes and probabilities bit-identical to
+        infer_accurate's, clip by clip, many clips per launch."""
+        check_precision(precision)
         if len(waveforms) == 0:
             return []
         dev = self.device
         with torch.cuda.device(dev):
-            slab, cu, layout, extra = self.enqueue(waveforms, quantized, return_intermediates)
+            slab, cu, layout, extra = self.enqueue(waveforms, quantized, return_intermediates, precision=precision)
             out_h = self._stage['out_h']
             out_h[:slab.numel()].copy_(slab, non_blocking=True)
             if extra is not None:
@@ -655,11 +729,8 @@ class Engine:
         decode, on the current device.  Returns (the fp32 tensors {units, probs, bounds, ...}, the workspace holding the notes
         at rows [0, n), n).  ``logits_hook(t, cu_d)``: as in enqueue(), run between the trunk (which then writes raw logits
         into t['probs']) and the decode."""
-        from .weights import build_f32_model
         dev = self.device
-        if self._f32 is None:
-            self._f32 = build_f32_model(self._state_dict, self.config, dev)
-        cmodel = self._f32[0]
+        cmodel = self.model_f32()
         head = _lib.EPI_BIAS_F32 if logits_hook is not None else _lib.EPI_SOFTMAX_F32 if quantized else _lib.EPI_SIGMOID_F32
         cu_d = torch.tensor([0, m], dtype=torch.int32, device=dev)
         f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)

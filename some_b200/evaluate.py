@@ -35,6 +35,7 @@ import numpy as np
 
 from . import _lib, audio
 from .batch import load_groups, midi_to_note, note_to_midi, staged
+from .engine import check_precision
 
 HOP = 512
 
@@ -262,15 +263,20 @@ def eval_clips(eng, logits, bounds, cu_frames, lab: _Labels, c0: int, c1: int, r
 
 
 def evaluate_recordings(infer_ins, waveforms: Sequence, labels: Sequence[Dict[str, np.ndarray]],
-                        rates: Optional[Sequence[Optional[int]]] = None, precision: str = 'bf16'):
+                        rates: Optional[Sequence[Optional[int]]] = None, precision: str = 'bf16', per_item: bool = False):
     """Evaluates whole recordings (no slicing: the task evaluates each item in one piece) against their label arrays
     (``item_labels`` for the recording's frame count).  ``waveforms`` / ``rates`` as in batch.transcribe_recordings.
-    Returns per recording (midi_loss sum, bound_loss sum, correct, frames, notes dict)."""
+    Returns per recording (midi_loss sum, bound_loss sum, correct, frames, notes dict).
+
+    All recordings run as one var-len batch through the trunk of ``precision``.  ``per_item=True`` (fp32 only) runs them
+    one at a time through the fp32 checker (Engine.accurate_clip, some_forward_f32) instead: the specification the batched
+    fp32 path gives the same numbers as."""
     import torch
     eng = infer_ins.model
     quantized = bool(getattr(infer_ins, 'quantized', False))
-    if precision not in ('bf16', 'fp32'):
-        raise ValueError(f"precision must be 'bf16' or 'fp32', got {precision!r}")
+    check_precision(precision)
+    if per_item and precision != 'fp32':
+        raise ValueError('per_item evaluation runs the fp32 checker: it needs precision=\'fp32\'')
     with staged(infer_ins, waveforms, rates) as (wave_d, bases, lens):
         frames = [1 + n // HOP for n in lens]
         for lab, t, it in zip(labels, frames, range(len(labels))):
@@ -278,15 +284,7 @@ def evaluate_recordings(infer_ins, waveforms: Sequence, labels: Sequence[Dict[st
                 raise ValueError(f'recording {it}: labels for {lab["unit2note"].shape[0]} frames, audio has {t}')
         lab = _Labels(labels, eng.device)
         ranges = [(int(b), int(b) + n) for b, n in zip(bases, lens)]
-        if precision == 'bf16':
-            def hook(ws, c0, c1, mc, cu_d):
-                eval_clips(eng, ws.probs, ws.bounds, cu_d, lab, c0, c1, int(cu[c0]), mc, quantized,
-                           _lib.EVAL_HEAD_TC, probs=ws.probs)
-            cu = np.zeros(len(ranges) + 1, dtype=np.int64)
-            np.cumsum(frames, out=cu[1:])
-            slab, cu_e, layout, _ = eng.enqueue(None, quantized, resident=(wave_d, ranges), logits_hook=hook)
-            notes = eng.unpack_slab(slab.cpu().numpy(), cu_e, layout)
-        else:
+        if per_item:
             notes = []
             for i, ((b0, _), n, t) in enumerate(zip(ranges, lens, frames)):
                 start = torch.zeros(1, dtype=torch.int64, device=eng.device)
@@ -299,13 +297,23 @@ def evaluate_recordings(infer_ins, waveforms: Sequence, labels: Sequence[Dict[st
                 notes.append({'note_midi': ws.note_midi[:k].cpu().numpy(),
                               'note_dur': ws.note_dur[:k].cpu().numpy().astype(np.int64) * eng.timestep,
                               'note_rest': ws.note_rest[:k].cpu().numpy().astype(bool)})
+        else:
+            head = _lib.EVAL_HEAD_TC if precision == 'bf16' else _lib.EVAL_HEAD_F32
+
+            def hook(ws, c0, c1, mc, cu_d):
+                eval_clips(eng, ws.probs, ws.bounds, cu_d, lab, c0, c1, int(cu[c0]), mc, quantized, head, probs=ws.probs)
+            cu = np.zeros(len(ranges) + 1, dtype=np.int64)
+            np.cumsum(frames, out=cu[1:])
+            slab, cu_e, layout, _ = eng.enqueue(None, quantized, resident=(wave_d, ranges), logits_hook=hook,
+                                                precision=precision)
+            notes = eng.unpack_slab(slab.cpu().numpy(), cu_e, layout)
         midi_sum, bound_sum, correct = lab.midi_loss.cpu().numpy(), lab.bound_loss.cpu().numpy(), lab.correct.cpu().numpy()
     return [(float(ms), float(bs), int(c), t, nt) for ms, bs, c, t, nt in zip(midi_sum, bound_sum, correct, frames, notes)]
 
 
 def evaluate_dataset(infer_ins, raw_data_dirs: Union[str, pathlib.Path, Sequence], config: dict, precision: str = 'bf16',
                      load_audio: Callable = audio.load_native, max_frames_per_batch: int = 400_000,
-                     workers: int = 4) -> EvalReport:
+                     workers: int = 4, per_item: bool = False) -> EvalReport:
     """The trainer's validation numbers for a checkpoint (``infer_ins``, a plugin inference instance) over one or more
     DiffSinger raw data directories (``transcriptions.csv``, ``wavs/{name}.wav`` + ``wavs/{name}.ds``).
 
@@ -313,9 +321,11 @@ def evaluate_dataset(infer_ins, raw_data_dirs: Union[str, pathlib.Path, Sequence
     ``max_frames_per_batch`` frames, as batch.batch_infer_dataset does; the default ``audio.load_native`` and
     ``audio.read_encoded`` (FLAC) give exactly librosa.load's samples, resampled / decoded on the device.
 
-    ``precision='bf16'``: the product trunk (some_forward, bf16 tensor cores) once per batch; ``'fp32'``: the fp32
-    validation trunk (some_forward_f32) one item at a time.  Either way some_eval_clips turns the logits into the losses,
-    the accuracy counts and the probabilities the predicted notes are decoded from."""
+    ``precision='bf16'``: the product trunk (some_forward, bf16 tensor cores) once per batch; ``'fp32'``: the fp32 trunk
+    (some_forward_f32_tiled) once per batch, whose logits are the fp32 checker's bit for bit, so every item's numbers are
+    those of the trainer's fp32 validation as the checker computes them (``per_item=True`` runs the checker itself, one item
+    at a time; see evaluate_recordings).  Either way some_eval_clips turns the logits into the losses, the accuracy counts
+    and the probabilities the predicted notes are decoded from."""
     if isinstance(raw_data_dirs, (str, pathlib.Path)):
         raw_data_dirs = [raw_data_dirs]
     quantized = bool(getattr(infer_ins, 'quantized', False))
@@ -330,7 +340,8 @@ def evaluate_dataset(infer_ins, raw_data_dirs: Union[str, pathlib.Path, Sequence
         waves = [w for _, w, _ in group]
         rates = [r for _, _, r in group]
         labels = [item_labels(it, 1 + _resampled_len(w, r, sr) // HOP, timestep, quantized) for it, w, r in group]
-        for (it, _, _), (ms, bs, c, t, nt) in zip(group, evaluate_recordings(infer_ins, waves, labels, rates, precision)):
+        for (it, _, _), (ms, bs, c, t, nt) in zip(group, evaluate_recordings(infer_ins, waves, labels, rates, precision,
+                                                                                       per_item)):
             midi = ms / t if quantized else ms / (t * n_bins)
             items.append(EvalItem(it['name'], t, midi, bs / t, c, t, nt['note_midi'], nt['note_dur'], nt['note_rest']))
     return EvalReport(items, summarize(items, config), precision)
@@ -361,7 +372,7 @@ def _main():
     @click.option('--model', required=True, metavar='CKPT_PATH', help='Path to the model checkpoint (*.ckpt)')
     @click.option('--dataset', 'datasets', required=True, multiple=True, metavar='DIR',
                   help='Raw data directory with transcriptions.csv and wavs/*.wav + *.ds (repeatable)')
-    @click.option('--fp32', is_flag=True, help='Use the fp32 validation trunk instead of the bf16 product path')
+    @click.option('--fp32', is_flag=True, help='Use the fp32 trunk instead of the bf16 product path')
     @click.option('--items-csv', required=False, metavar='PATH', help='Write the per-item table to this CSV file')
     def evaluate(model, datasets, fp32, items_csv):
         import yaml

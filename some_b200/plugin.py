@@ -21,7 +21,7 @@ import torch
 
 from . import _lib
 from .config import load_state_dict_strict
-from .engine import Engine, frames_of
+from .engine import Engine, check_precision, frames_of
 
 
 class BaseInference:
@@ -38,6 +38,9 @@ class BaseInference:
                 f"some_b200 plugin needs a CUDA (sm_90a) device, got device='{device}'. "
                 "It has no CPU path; use the reference implementation on CPU.")
         self.timestep = self.config['hop_size'] / self.config['audio_sample_rate']   # base_infer.py:20
+        # optional config key `infer_precision: fp32`: infer() (and batch.transcribe_recordings) run the fp32 trunk, whose
+        # notes are the fp32 checker's bit for bit; the default `bf16` is the tensor-core product path
+        self.precision = check_precision(self.config.get('infer_precision', 'bf16'))
         self._lock = threading.Lock()     # webui.py:104 runs up to 10 concurrent callers on one instance
         self.model: Engine = self.build_model()
 
@@ -137,7 +140,7 @@ class MIDIExtractionInference(BaseInference):
     def infer(self, waveforms: List[np.ndarray]) -> List[Dict[str, np.ndarray]]:
         """base_infer.py:46-53, batched: same order as the input, one dict per waveform."""
         with self._lock:
-            return self.model.infer(list(waveforms), quantized=self.quantized)
+            return self.model.infer(list(waveforms), quantized=self.quantized, precision=self.precision)
 
 
 class QuantizedMIDIExtractionInference(MIDIExtractionInference):

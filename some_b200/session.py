@@ -131,6 +131,9 @@ class Session:
         _lib.check(self.lib.some_session_get_info(h, C.byref(info)), 'some_session_get_info')
         self.sample_rate, self.hop, self.outdim = info.sample_rate, info.hop, info.outdim
         self.quantized, self.bias_corrected, self.timestep = bool(info.quantized), bool(info.bias_corrected), info.timestep
+        prec = C.c_int()
+        _lib.check(self.lib.some_session_get_precision(h, C.byref(prec)), 'some_session_get_precision')
+        self.precision = {0: 'bf16', 1: 'fp32'}[prec.value]    # of the model file: every call runs at it
 
     def close(self):
         """Closes the session and, first, every stream still open on it."""

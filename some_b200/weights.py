@@ -292,8 +292,22 @@ def checkpoint_model(sd, config: dict) -> SimpleNamespace:
         b_cut=float(sd['model.cutheard.bias'][0]))
 
 
+def checkpoint_f32(sd, config: dict) -> SimpleNamespace:
+    """checkpoint_model with its blocks: the fp32 model's tensors, readable by packed_tensor under model_tensors_f32."""
+    ck = checkpoint_model(sd, config)
+    ck.blocks = [[checkpoint_block(sd, p) for p in ps] for ps in ck.prefixes]
+    return ck
+
+
+def model_tensors_f32(lay: int) -> List[Tensor]:
+    """The tensors of the fp32 model (some_model_f32; an fp32 model file, some_b200/export.py): model_tensors' names, order
+    and fields, every one f32 (the checkpoint's own values, nothing rounded or packed), b_head unpadded.  The C mirror is
+    kBlockRowsF32 / expected_tensors in csrc/session.cu."""
+    return [t._replace(dtype=F32, shape=('outdim',) if t.field == 'b_head' else t.shape) for t in model_tensors(lay)]
+
+
 def build_f32_model(sd, config: dict, device):
-    """fp32 weights of the validation path (some_forward_f32, csrc/accurate.cu): checkpoint_model and checkpoint_block,
+    """fp32 weights of some_forward_f32 / some_forward_f32_tiled (csrc/accurate.cu): checkpoint_model and checkpoint_block,
     nothing rounded or packed.  Returns (ModelF32C, keepalive)."""
     keep = []
 
@@ -301,7 +315,5 @@ def build_f32_model(sd, config: dict, device):
         keep.append(t.to(device=device, dtype=torch.float32).contiguous())
         return keep[-1]
 
-    ck = checkpoint_model(sd, config)
-    ck.blocks = [[checkpoint_block(sd, p) for p in ps] for ps in ck.prefixes]
-    m, arrays = _c_model(_lib.ModelF32C, _lib.BlockWeightsF32C, ck, False, upload)
+    m, arrays = _c_model(_lib.ModelF32C, _lib.BlockWeightsF32C, checkpoint_f32(sd, config), False, upload)
     return m, (keep, *arrays)
