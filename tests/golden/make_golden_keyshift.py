@@ -1,6 +1,7 @@
 """Generates tests/golden/keyshift.npz by EXECUTING THE UNMODIFIED reference MelSpectrogram (modules/rmvpe/spec.py) on CPU
-through oracle/refshim.py for keyshift in {-5 .. +5} (the binarizer's augmentation range, preprocessing/me_binarizer.py:235-247),
-plus one speed != 1 and one center=False case.  Build container only; outputs are committed.
+through oracle/refshim.py for keyshift in {-5 .. +5}, plus one fractional shift, one speed != 1 and one center=False case.  The
+binarizer's pitch augmentation (preprocessing/me_binarizer.py:235-247) draws from key_shift_range, [-12, 12] in both shipped
+configs; make_golden_keyshift_wide.py covers the shifts beyond +-5.  Build container only; outputs are committed.
 
     python tests/golden/make_golden_keyshift.py
 """
