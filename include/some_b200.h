@@ -424,14 +424,15 @@ int some_flac_chain_resume(const some_flac_frame* frames, int n_frames, int64_t 
  * some_audio_info  RIFF/WAVE as scipy.io.wavfile.read walks it (fmt tag 1: PCM in 1, 2, 3 or 4 byte containers; tag 3: float32
  *                  or float64; tag 0xFFFE with a PCM or float subformat; any number of channels; other chunks skipped with
  *                  their pad byte; a data chunk cut short by the end of the file yields the whole frames present), or fLaC,
- *                  optionally behind an ID3v2 tag, with the metadata-block rules of audio.parse_flac (up to 24 bits per
+ *                  optionally behind an ID3v2 tag (the first block a 34-byte STREAMINFO, type 127 invalid; up to 24 bits per
  *                  sample), or FORM/AIFF and FORM/AIFC as libsndfile reads them (COMM before SSND, other chunks skipped
  *                  with their pad byte, the walk bounded by the FORM size and ending with the SSND chunk; the rate is the
  *                  integer part of COMM's 80-bit extended value; the frames are the whole frames of the SSND bytes within
  *                  its stated size and the file; integer PCM of 1-32 bits big-endian or `sowt`, `raw ` 8-bit unsigned,
- *                  `fl32` / `fl64` big-endian float, `ulaw` / `alaw` G.711).  Refused with audio.decode_wav's /
- *                  audio.parse_flac's reason (scipy's text for the WAV walk; "AIFF/IFF: ..." for AIFF) and the byte offset:
- *                  other containers (Ogg, MP3, RIFX, RF64, CAF, AU) by name, truncated or missing chunks, unsupported tags,
+ *                  `fl32` / `fl64` big-endian float, `ulaw` / `alaw` G.711).  Refused with a reason (audio.decode_wav's, i.e.
+ *                  scipy's, text for the WAV walk; one naming FLAC; "AIFF/IFF: ..." for AIFF) and the byte offset:
+ *                  other containers (Ogg, MP3, RIFX, RF64, CAF, AU) by name (after an ID3v2 tag also with the byte offset
+ *                  where the fLaC marker was looked for), truncated or missing chunks, unsupported tags,
  *                  compression types or sample sizes, a bad STREAMINFO, an AIFF rate outside [1, 2^31). */
 enum { SOME_AUDIO_WAV = 1, SOME_AUDIO_FLAC = 2, SOME_AUDIO_AIFF = 3 };
 /* Sample containers: little-endian U8 .. F64 (WAV, AIFF-C `sowt` and `raw `), and for AIFF: S8 (1-8 bit signed), the

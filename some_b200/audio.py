@@ -5,16 +5,19 @@
 - ``decode_wav`` / ``to_mono``: libsndfile's integer -> float32 scaling for RIFF/WAVE files and librosa.to_mono.
 - ``resample``: librosa.resample(res_type='kaiser_best') on the GPU (csrc/resample.cu, some_resample_kaiser), BIT-identical to
   resampy's float32 loop; numpy in -> numpy out, CUDA tensor in -> CUDA tensor out on the current stream.
-- ``read_encoded`` / ``EncodedAudio`` / ``FlacBatch`` / ``decode_flac``: FLAC files (libsndfile reads them through libFLAC)
-  decoded on the GPU (csrc/flac.cu): the file's bytes and its STREAMINFO are read on the host, the frames are found,
-  checked and decoded on the device, many recordings in one set of launches, straight to mono if wanted.
+- ``audio_info``: the native container walk (some_audio_info, csrc/audio_host.cu) on a file's bytes, the one reader of
+  FLAC and AIFF headers: container, rate, channels, sample kind, frames and where the audio starts.
+- ``read_encoded`` / ``parse_flac`` / ``EncodedAudio`` / ``FlacBatch`` / ``decode_flac``: FLAC files (libsndfile reads them
+  through libFLAC) decoded on the GPU (csrc/flac.cu): the file's bytes and its STREAMINFO (from ``audio_info``) are read on
+  the host, the frames are found, checked and decoded on the device, many recordings in one set of launches, straight to
+  mono if wanted.
 - ``decode_aiff``: AIFF and AIFF-C files as libsndfile reads them, decoded on the GPU: the container is walked on the host
-  (some_audio_info, csrc/audio_host.cu), the SSND bytes go up and one some_pcm_decode (csrc/pcm.cu) scales them (integer
-  PCM of 1-32 bits in either byte order, 8-bit unsigned, big-endian float32 / float64, G.711 u-law and A-law).
-- ``load``: librosa.load for RIFF/WAVE files (PCM 8/16/24/32-bit, float32/64, WAVE_FORMAT_EXTENSIBLE), for FLAC files
-  (``fLaC``, optionally behind an ID3v2 tag; up to 24 bits per sample) and for AIFF / AIFF-C files (``FORM``), chosen by
-  the file's content.  Other containers (Ogg, MP3, ...) raise: librosa decodes those through libsndfile / audioread,
-  which this module does not restate.
+  (``audio_info``), the SSND bytes go up and one some_pcm_decode (csrc/pcm.cu) scales them (integer PCM of 1-32 bits in
+  either byte order, 8-bit unsigned, big-endian float32 / float64, G.711 u-law and A-law).
+- ``load``: librosa.load for RIFF/WAVE files (PCM 8/16/24/32-bit, float32/64, WAVE_FORMAT_EXTENSIBLE; read by
+  ``decode_wav``), and, through ``audio_info``, for FLAC files (``fLaC``, optionally behind an ID3v2 tag; up to 24 bits
+  per sample) and AIFF / AIFF-C files (``FORM``), chosen by the file's content.  Other containers (Ogg, MP3, ...) raise:
+  librosa decodes those through libsndfile / audioread, which this module does not restate.
 - ``load_native``: the decoded recording at its own rate, for batch.batch_infer_dataset's device-resident resampling.
 
 The arithmetic is restated in oracle/resample.py, oracle/flac.py and oracle/aiff.py (test infrastructure), which document
@@ -25,6 +28,7 @@ from __future__ import annotations
 import ctypes as C
 import dataclasses
 import functools
+import re
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -171,7 +175,18 @@ def resample(y, orig_sr: int, target_sr: int):
     return dst.cpu().numpy() if is_np else dst
 
 
-# ---------------------------------------------------------------------------------------------- FLAC (host metadata)
+# ---------------------------------------------------------------------------------------------- container metadata (host)
+def audio_info(data: bytes, name: str = '<bytes>'):
+    """some_audio_info on a file's bytes (host): its _lib.AudioMeta, or ValueError naming the file, the container and the
+    byte offset."""
+    from . import _lib
+    lib = _lib.load()
+    m = _lib.AudioMeta()
+    if lib.some_audio_info(data, len(data), C.byref(m)):
+        raise ValueError(f'{name}: {lib.some_last_error().decode("utf8", "replace")}')
+    return m
+
+
 @dataclasses.dataclass(frozen=True, eq=False)
 class EncodedAudio:
     """A FLAC recording as read from disk, not yet decoded: the file's bytes and its STREAMINFO.  ``length`` is the
@@ -187,61 +202,34 @@ class EncodedAudio:
     max_blocksize: int
 
 
-def _id3_size(data: bytes) -> int:
-    """Length of an ID3v2 tag at the start of ``data`` (0 if none): 10 + its syncsafe size, + 10 with a footer (0x10)."""
-    if len(data) < 10 or data[:3] != b'ID3':
-        return 0
-    size = (data[6] & 0x7F) << 21 | (data[7] & 0x7F) << 14 | (data[8] & 0x7F) << 7 | (data[9] & 0x7F)
-    return 10 + size + (10 if data[5] & 0x10 else 0)
+# How the container walk's refusals of bytes it does not take for FLAC begin; its FLAC refusals name FLAC instead.
+_OTHER_CONTAINERS = ('not a RIFF/WAVE file', 'RIFF/WAVE: ', 'AIFF/IFF: ')
+
+
+def _flac_record(data: bytes, name: str, m) -> EncodedAudio:
+    """The record of FLAC bytes from the _lib.AudioMeta some_audio_info gave for them."""
+    return EncodedAudio(name=name, data=bytes(data), rate=m.rate, channels=m.channels, bps=m.bits, length=m.frames,
+                        audio_offset=m.data_offset, min_blocksize=m.min_blocksize, max_blocksize=m.max_blocksize)
 
 
 def parse_flac(data: bytes, name: str = '<bytes>') -> EncodedAudio:
-    """The metadata of a FLAC stream (host; raises ValueError naming FLAC and the byte offset on malformed input): the
-    first block must be a 34-byte STREAMINFO; PADDING, APPLICATION, SEEKTABLE, VORBIS_COMMENT, CUESHEET, PICTURE and unknown
-    blocks are skipped; type 127 is invalid.  Streams of more than 24 bits per sample are refused."""
-    off = _id3_size(data)
-    if data[off:off + 4] != b'fLaC':
+    """The metadata of a FLAC stream, read by the native container walk (``audio_info``).  Malformed metadata raises
+    ValueError naming the file, FLAC and the byte offset (the first block must be a 34-byte STREAMINFO, type 127 is
+    invalid, more than 24 bits per sample are refused); bytes of any other container raise 'not a FLAC stream' with the
+    byte offset where the fLaC marker was looked for (after any ID3v2 tag)."""
+    from . import _lib
+    off = 0
+    try:
+        m = audio_info(data, name)
+    except ValueError as e:
+        reason = str(e)[len(name) + 2:]
+        if not reason.startswith(_OTHER_CONTAINERS):
+            raise
+        at = re.search(r'no fLaC marker at byte offset (\d+)', reason)     # the walk names it after an ID3v2 tag
+        m, off = None, int(at.group(1)) if at else 0
+    if m is None or m.container != _lib.AUDIO_FLAC:
         raise ValueError(f'{name}: not a FLAC stream (no fLaC marker at byte offset {off})')
-    p, info, first = off + 4, None, True
-    while True:
-        if p + 4 > len(data):
-            raise ValueError(f'{name}: FLAC metadata block header truncated at byte offset {p}')
-        last, kind, size = data[p] >> 7, data[p] & 0x7F, int.from_bytes(data[p + 1:p + 4], 'big')
-        if first and (kind != 0 or size != 34):
-            raise ValueError(f'{name}: FLAC stream does not start with a 34-byte STREAMINFO block (type {kind}, {size} '
-                             f'bytes at byte offset {p})')
-        if not first and kind in (0, 127):
-            raise ValueError(f'{name}: {"second STREAMINFO" if kind == 0 else "invalid"} FLAC metadata block at byte offset {p}')
-        if p + 4 + size > len(data):
-            raise ValueError(f'{name}: FLAC metadata block truncated at byte offset {p}')
-        if first:
-            b = int.from_bytes(data[p + 4:p + 22], 'big')               # the 144 bits in front of the MD5
-            info = dict(min_blocksize=b >> 128, max_blocksize=(b >> 112) & 0xFFFF, rate=(b >> 44) & 0xFFFFF,
-                        channels=((b >> 41) & 7) + 1, bps=((b >> 36) & 31) + 1, length=b & ((1 << 36) - 1))
-            first = False
-        p += 4 + size
-        if last:
-            break
-    if info['bps'] > 24:
-        raise ValueError(f'{name}: FLAC stream of {info["bps"]} bits per sample (at byte offset {off + 8}); only up to 24 '
-                         f'bits are decoded (libsndfile\'s float scaling is exact up to 24 bits)')
-    if info['rate'] == 0 or info['max_blocksize'] == 0:
-        raise ValueError(f'{name}: invalid FLAC STREAMINFO (sample rate {info["rate"]}, max block size '
-                         f'{info["max_blocksize"]}) at byte offset {off + 8}')
-    return EncodedAudio(name=name, data=bytes(data), audio_offset=p, **info)
-
-
-def _sniff(path) -> str:
-    """'aiff' for 'FORM', 'flac' for 'fLaC' (optionally behind an ID3v2 tag), else 'other'."""
-    with open(path, 'rb') as f:
-        head = f.read(10)
-        if head[:4] == b'FORM':
-            return 'aiff'
-        off = _id3_size(head)
-        if off:
-            f.seek(off)
-            head = f.read(4)
-    return 'flac' if head[:4] == b'fLaC' else 'other'
+    return _flac_record(data, name, m)
 
 
 def read_encoded(path, sr=None) -> EncodedAudio:
@@ -389,17 +377,6 @@ def decode_flac(path) -> Tuple[np.ndarray, int]:
 
 
 # ---------------------------------------------------------------------------------------------- AIFF (device)
-def audio_info(data: bytes, name: str = '<bytes>'):
-    """some_audio_info on a file's bytes (host): its _lib.AudioMeta, or ValueError naming the file, the container and the
-    byte offset."""
-    from . import _lib
-    lib = _lib.load()
-    m = _lib.AudioMeta()
-    if lib.some_audio_info(data, len(data), C.byref(m)):
-        raise ValueError(f'{name}: {lib.some_last_error().decode("utf8", "replace")}')
-    return m
-
-
 def _pcm_device(data: bytes, m, mono: bool):
     """The samples some_audio_info found in ``data`` (a WAV data or AIFF SSND chunk), decoded by one some_pcm_decode on the
     current stream: a CUDA float32 tensor, [n] (mono or one channel) or [channels, n]."""
@@ -421,21 +398,15 @@ def _pcm_device(data: bytes, m, mono: bool):
     return y if ch == 1 else y.view(n, ch).t().contiguous()
 
 
-def _read_aiff(path):
-    """(file bytes, meta) of an AIFF / AIFF-C file; ValueError for anything else."""
+def decode_aiff(path) -> Tuple[np.ndarray, int]:
+    """(samples, native rate) of an AIFF / AIFF-C file as libsndfile hands them to librosa.load, decoded on the GPU: float32
+    [n] (one channel) or [n, channels]."""
     from . import _lib
     with open(path, 'rb') as f:
         data = f.read()
     m = audio_info(data, str(path))
     if m.container != _lib.AUDIO_AIFF:
         raise ValueError(f'{path}: not an AIFF or AIFF-C file')
-    return data, m
-
-
-def decode_aiff(path) -> Tuple[np.ndarray, int]:
-    """(samples, native rate) of an AIFF / AIFF-C file as libsndfile hands them to librosa.load, decoded on the GPU: float32
-    [n] (one channel) or [n, channels]."""
-    data, m = _read_aiff(path)
     y = _pcm_device(data, m, mono=False)
     return (y.cpu().numpy() if y.ndim == 1 else y.t().contiguous().cpu().numpy()), int(m.rate)
 
@@ -445,25 +416,27 @@ def load(path, sr=22050, mono: bool = True):
     """librosa.load(path, sr=sr, mono=mono) (librosa 0.9, res_type='kaiser_best') for RIFF/WAVE, FLAC and AIFF files:
     (y, rate).  ``sr=None`` keeps the native rate; otherwise the decoded (and down-mixed) samples are resampled on the GPU.
     FLAC and AIFF files are decoded and down-mixed on the GPU too."""
-    kind = _sniff(path)
-    if kind in ('flac', 'aiff'):
-        if kind == 'flac':
-            rec = read_encoded(path)
-            y, _ = _flac_device(rec, mono)
-            native = rec.rate
-        else:
-            data, m = _read_aiff(path)
-            y, native = _pcm_device(data, m, mono), int(m.rate)
+    from . import _lib
+    with open(path, 'rb') as f:
+        data = f.read(4)
+        if data != b'RIFF':                                  # scipy reads RIFF files itself
+            data += f.read()
+    if data == b'RIFF':
+        x, native = decode_wav(path)
+        y = x.T                                              # librosa's (channels, n)
+        if mono:
+            y = to_mono(y)
         if sr is not None and as_rate(sr) != native:
-            return resample(y, native, as_rate(sr)).cpu().numpy(), as_rate(sr)
-        return y.cpu().numpy(), native
-    x, native = decode_wav(path)
-    y = x.T                                                  # librosa's (channels, n)
-    if mono:
-        y = to_mono(y)
-    if sr is not None and as_rate(sr) != native:
-        return resample(np.ascontiguousarray(y), native, as_rate(sr)), as_rate(sr)
-    return y, native
+            return resample(np.ascontiguousarray(y), native, as_rate(sr)), as_rate(sr)
+        return y, native
+    m = audio_info(data, str(path))                          # FLAC or AIFF / AIFF-C; ValueError for anything else
+    if m.container == _lib.AUDIO_FLAC:
+        y, _ = _flac_device(_flac_record(data, str(path), m), mono)
+    else:
+        y = _pcm_device(data, m, mono)
+    if sr is not None and as_rate(sr) != m.rate:
+        return resample(y, m.rate, as_rate(sr)).cpu().numpy(), as_rate(sr)
+    return y.cpu().numpy(), m.rate
 
 
 def load_native(path, sr=None):

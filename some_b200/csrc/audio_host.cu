@@ -1,11 +1,11 @@
 // Host-only helpers of the encoded-file path (no CUDA call): container metadata (some_audio_info), the FLAC frame chain
 // (some_flac_chain) and Standard MIDI File bytes (some_midi_write, some_notes_midi).
 //
-// some_audio_info restates what some_b200.audio.load accepts, except integer PCM in 5-8 byte containers (scipy: int64,
-// x / 2^63) and 1-8 bit PCM in wider containers, which it refuses: RIFF/WAVE exactly as scipy.io.wavfile.read walks it (the
-// chunk loop bounded by the RIFF size, the pad byte of odd chunks, a data chunk cut short by the end of the file), FLAC
-// with audio.parse_flac's metadata-block rules, and AIFF / AIFF-C as libsndfile reads them (oracle/aiff.py restates the
-// walk in numpy).  Its refusals carry the Python reason and a byte offset.
+// some_audio_info reads what some_b200.audio.load accepts (load reads FLAC and AIFF headers through it), except integer
+// PCM in 5-8 byte containers (scipy: int64, x / 2^63) and 1-8 bit PCM in wider containers, which it refuses: RIFF/WAVE
+// exactly as scipy.io.wavfile.read walks it (the chunk loop bounded by the RIFF size, the pad byte of odd chunks, a data
+// chunk cut short by the end of the file), FLAC (oracle/flac.py restates its metadata rules), and AIFF / AIFF-C as
+// libsndfile reads them (oracle/aiff.py restates the walk in numpy).  Its refusals carry a reason and a byte offset.
 // some_flac_chain is the one copy of the walk FlacBatch used to do in Python; both the Python and the session's paths call it.
 // some_midi_write is some_b200.midi.build_midi_file(...).to_bytes(), tick for tick.
 #include <limits.h>
@@ -65,7 +65,7 @@ long long extended_int(const uint8_t* b, double* value) {
   return ip >= 1 && ip < (uint64_t(1) << 31) ? static_cast<long long>(ip) : -1;
 }
 
-// audio._id3_size: 10 + the syncsafe size (+ 10 with a footer), 0 without a tag.
+// The length of an ID3v2 tag: 10 + the syncsafe size (+ 10 with a footer), 0 without a tag.
 long long id3_size(const uint8_t* d, long long n) {
   if (n < 10 || memcmp(d, "ID3", 3) != 0) return 0;
   const long long size = (d[6] & 0x7F) << 21 | (d[7] & 0x7F) << 14 | (d[8] & 0x7F) << 7 | (d[9] & 0x7F);
@@ -222,14 +222,16 @@ int AudioWalk::step(bool at_end, long long n) {
         phase_ = kAiffChunk;
         return kAdvanced;
       }
+      // p > 0: an ID3v2 tag came first, which only a FLAC stream may have; say where its fLaC marker was looked for
       SOME_REQUIRE(head_len_ >= 12 && memcmp(head_, "RIFF", 4) == 0 && memcmp(head_ + 8, "WAVE", 4) == 0,
-                   "not a RIFF/WAVE file (%s); some_b200.audio reads WAV files only", not_wave_kind(head_, head_len_).c_str());
+                   "not a RIFF/WAVE file (%s%s); some_b200.audio reads WAV files only", not_wave_kind(head_, head_len_).c_str(),
+                   p > 0 ? ("; no fLaC marker at byte offset " + std::to_string(p)).c_str() : "");
       file_size_ = static_cast<long long>(le32(head_ + 4)) + 8;
       pos_ = 12;
       phase_ = kWavChunk;
       return kAdvanced;
     }
-    // audio.parse_flac
+    // FLAC metadata blocks (audio.parse_flac reads FLAC headers through this walk)
     case kFlacBlock:
     case kFlacEnd: {
       if (skipped_ >= 0) {                 // the skipped block ends at p

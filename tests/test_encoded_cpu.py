@@ -1,6 +1,7 @@
 """CPU tests of the host half of the encoded-file path (csrc/audio_host.cu; the library loads without a GPU):
-some_audio_info against audio.decode_wav / audio.parse_flac, some_flac_chain against the Python walk FlacBatch used to do
-(kept here as the comparison), and some_midi_write against midi.build_midi_file(...).to_bytes()."""
+some_audio_info against audio.decode_wav and oracle/flac.py, audio.parse_flac's refusals word for word, some_flac_chain
+against the Python walk FlacBatch used to do (kept here as the comparison), and some_midi_write against
+midi.build_midi_file(...).to_bytes()."""
 import ctypes as C
 import struct
 import warnings
@@ -8,6 +9,7 @@ import warnings
 import numpy as np
 import pytest
 
+from oracle import aiff as oa
 from oracle import flac as of
 from some_b200 import _lib, audio, midi
 
@@ -207,46 +209,60 @@ def test_wav_riff_size_bounds_the_walk(tmp_path):
 
 # ---------------------------------------------------------------------------------------------- FLAC metadata
 @pytest.mark.parametrize('name,x,kw', of.feature_cases(), ids=[c[0] for c in of.feature_cases()])
-def test_flac_info_equals_parse_flac(name, x, kw):
+def test_flac_info_equals_oracle(name, x, kw):
     data = of.encode(x, **kw)
-    rec = audio.parse_flac(data)
+    want = of.parse_metadata(data)
     m = info(data)
-    assert (m.container, m.rate, m.channels, m.bits, m.frames) == (_lib.AUDIO_FLAC, rec.rate, rec.channels, rec.bps, rec.length)
+    assert (m.container, m.rate, m.channels, m.bits, m.frames) == \
+        (_lib.AUDIO_FLAC, want['rate'], want['channels'], want['bps'], want['total'])
     assert (m.min_blocksize, m.max_blocksize, m.data_offset, m.data_bytes) == \
-        (rec.min_blocksize, rec.max_blocksize, rec.audio_offset, len(data) - rec.audio_offset)
+        (want['min_blocksize'], want['max_blocksize'], want['audio_offset'], len(data) - want['audio_offset'])
 
 
 def _flac_refusals():
     x = of.test_signal(1000, 1, 16, 1)
     good = of.encode(x, rate=44100, bps=16)
     si = good.index(b'fLaC') + 4
-    out = []
     b32 = bytearray(good)
     b32[si + 4 + 12] = (b32[si + 4 + 12] & 0xFE) | 1         # bps - 1 = 31 -> 32 bits (high bit of the 5-bit field)
     b32[si + 4 + 13] = (b32[si + 4 + 13] & 0x0F) | 0xF0
-    out.append((bytes(b32), 'bits per sample'))
     rate0 = bytearray(good)
     rate0[si + 4 + 10:si + 4 + 12] = b'\0\0'
     rate0[si + 4 + 12] &= 0x0F
-    out.append((bytes(rate0), 'invalid FLAC STREAMINFO'))
-    out.append((good[:si] + bytes([0x00, 0, 0, 34]) + good[si + 4:si + 38] + bytes([0x80, 0, 0, 34]) + good[si + 4:],
-                'second STREAMINFO'))
-    out.append((good[:si] + bytes([0x00, 0, 0, 34]) + good[si + 4:si + 38] + bytes([0xFF, 0, 0, 0]) + good[si + 38:],
-                'invalid FLAC metadata block'))
-    out.append((good[:si] + bytes([0x81, 0, 0, 34]) + good[si + 4:], 'does not start with a 34-byte STREAMINFO'))
-    out.append((good[:si + 20], 'metadata block truncated'))
-    out.append((good[:si + 2], 'block header truncated'))
-    out.append((of.id3_tag() + good[:si + 20], 'metadata block truncated'))
-    return out
+    not_flac = 'f: not a FLAC stream (no fLaC marker at byte offset 0)'
+    return [
+        ('bps_32', bytes(b32), "f: FLAC stream of 32 bits per sample (at byte offset 8); only up to 24 bits are decoded "
+                               "(libsndfile's float scaling is exact up to 24 bits)"),
+        ('rate_0', bytes(rate0), 'f: invalid FLAC STREAMINFO (sample rate 0, max block size 1000) at byte offset 8'),
+        ('second_streaminfo', good[:si] + bytes([0x00, 0, 0, 34]) + good[si + 4:si + 38] + bytes([0x80, 0, 0, 34]) +
+         good[si + 4:], 'f: second STREAMINFO FLAC metadata block at byte offset 42'),
+        ('block_127', good[:si] + bytes([0x00, 0, 0, 34]) + good[si + 4:si + 38] + bytes([0xFF, 0, 0, 0]) + good[si + 38:],
+         'f: invalid FLAC metadata block at byte offset 42'),
+        ('first_not_streaminfo', good[:si] + bytes([0x81, 0, 0, 34]) + good[si + 4:],
+         'f: FLAC stream does not start with a 34-byte STREAMINFO block (type 1, 34 bytes at byte offset 4)'),
+        ('block_truncated', good[:si + 20], 'f: FLAC metadata block truncated at byte offset 4'),
+        ('header_truncated', good[:si + 2], 'f: FLAC metadata block header truncated at byte offset 4'),
+        ('id3_block_truncated', of.id3_tag() + good[:si + 20], 'f: FLAC metadata block truncated at byte offset 28'),
+        # bytes the walk takes for, or refuses as, another container
+        ('no_marker', b'fLaX' + good[4:], not_flac),
+        ('id3_no_marker', of.id3_tag() + b'fLaX' + good[4:], 'f: not a FLAC stream (no fLaC marker at byte offset 24)'),
+        ('wav', wav_bytes('s16', 1, 10), not_flac),
+        ('bad_wav', _riff(_fmt(tag=6), chunk(b'data', bytes(8))), not_flac),
+        ('aiff', oa.aiff_bytes(bytes(20), 1, 16, 8000.0), not_flac),
+        ('bad_aiff', b'FORM\x00\x00\x00\x20' + b'8SVX' + bytes(40), not_flac),
+    ]
 
 
-@pytest.mark.parametrize('data,reason', _flac_refusals())
-def test_flac_refusals_equal_parse_flac(data, reason):
-    with pytest.raises(ValueError, match=reason) as py:
+FLAC_REFUSALS = _flac_refusals()
+
+
+@pytest.mark.parametrize('name,data,message', FLAC_REFUSALS, ids=[c[0] for c in FLAC_REFUSALS])
+def test_flac_refusal_messages(name, data, message):
+    """audio.parse_flac's refusals, word for word: the walk's FLAC reason and byte offset, or 'not a FLAC stream' and
+    where the marker was looked for."""
+    with pytest.raises(ValueError) as e:
         audio.parse_flac(data, 'f')
-    with pytest.raises(ValueError, match=reason) as c:
-        info(data)
-    assert str(py.value) == 'f: ' + str(c.value)
+    assert str(e.value) == message
 
 
 # ---------------------------------------------------------------------------------------------- the frame chain

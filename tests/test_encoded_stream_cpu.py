@@ -174,8 +174,9 @@ def test_flac_walk_equals_audio_info(name, x, kw):
 
 
 def test_flac_walk_refusals_and_large_skipped_blocks():
-    for data, _ in tc._flac_refusals():
-        check_walks(data)
+    for _, data, message in tc.FLAC_REFUSALS:
+        if 'not a FLAC stream' not in message:                  # the walk's own FLAC refusals
+            check_walks(data)
     x = of.test_signal(3000, 2, 16, 7)
     big = of.encode(x, rate=44100, bps=16, id3=of.id3_tag(bytes(300000)),
                     metadata=[('PICTURE', b'\xff\xf8\xc9\x08' * 250000), ('PADDING', bytes(5000))])

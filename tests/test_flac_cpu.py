@@ -5,6 +5,7 @@ import re
 
 import numpy as np
 import pytest
+import torch
 
 from oracle import flac as of
 from some_b200 import audio
@@ -170,9 +171,10 @@ def test_encoder_decoder_round_trip(case):
     y, info = of.decode(data, name)
     np.testing.assert_array_equal(y, x)
     assert (info['rate'], info['channels'], info['bps']) == (kw['rate'], x.shape[1], kw['bps'])
-    rec = audio.parse_flac(data, name)                      # the product's host parser agrees with the oracle's
-    assert (rec.rate, rec.channels, rec.bps, rec.audio_offset) == (info['rate'], info['channels'], info['bps'],
-                                                                   info['audio_offset'])
+    rec = audio.parse_flac(data, name)                      # the native container walk agrees with the oracle's metadata
+    assert (rec.rate, rec.channels, rec.bps, rec.length, rec.min_blocksize, rec.max_blocksize, rec.audio_offset) == \
+        (info['rate'], info['channels'], info['bps'], info['total'], info['min_blocksize'], info['max_blocksize'],
+         info['audio_offset'])
     assert rec.length == (0 if kw.get('total_samples') == 0 else len(x))
 
 
@@ -288,7 +290,7 @@ def test_trailing_bytes_after_the_stated_length_are_ignored():
 
 
 @pytest.mark.parametrize('footer', [False, True])
-def test_id3v2_tag_is_skipped(footer, tmp_path):
+def test_id3v2_tagged_flac_is_read_as_flac(footer, tmp_path, monkeypatch):
     x = of.test_signal(3000, 2, 16, 4)
     tag = of.id3_tag(b'TIT2\x00\x00\x00\x06\x00\x00\xff\xf8\xc9\x08', footer=footer)   # a sync pattern inside the tag
     data = of.encode(x, 44100, 16, id3=tag)
@@ -298,7 +300,15 @@ def test_id3v2_tag_is_skipped(footer, tmp_path):
     assert audio.parse_flac(data).audio_offset == info['audio_offset']
     p = tmp_path / 'tagged.flac'
     p.write_bytes(data)
-    assert audio._sniff(p) == 'flac'
+    taken = []                                                  # load() takes it for FLAC: the record goes to the device path
+
+    def flac_device(rec, mono):
+        taken.append(rec)
+        return torch.zeros(rec.length), None
+    monkeypatch.setattr(audio, '_flac_device', flac_device)
+    assert audio.load(p, sr=None)[1] == 44100
+    assert [(r.audio_offset, r.length, r.channels) for r in taken] == [(info['audio_offset'], len(x), 2)]
+    assert taken[0].data == data and taken[0].name == str(p)
     with pytest.raises(ValueError, match='not a RIFF/WAVE file'):  # decode_wav keeps refusing FLAC files
         audio.decode_wav(p)
     p.write_bytes(data[len(tag):])
