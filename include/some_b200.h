@@ -855,6 +855,66 @@ typedef struct {
 } some_encoded;
 int some_session_transcribe_encoded(some_session* s, const some_encoded* items, int count, const some_slicer_params* params,
                                     some_notes* const* out);
+
+/* ---- Labelling a DiffSinger dataset (csrc/label.cu, host only): batch_infer.py's note_seq / note_dur fields of
+ * transcriptions.csv, byte for byte as some_b200.batch.row_notes(ph_dur, ph_num, note_timeline(offsets, segments), round_midi)
+ * writes them (batch_infer.py:56-81, 84-135, 178-219): the notes on one timeline rounded to 6 decimals, each start clipped at
+ * the previous end; word spans from ph_dur / ph_num; note edges within 0.05 s of a word edge snapped to it; per word the
+ * touching notes and a rest for any uncovered remainder (round_midi: the note of largest overlap, or rest, for the whole
+ * word).  Python's arithmetic is kept where it decides a digit: round(x, 6) on the exact binary value, str(float) as
+ * CPython's shortest repr (5e-05, 2.0), CPython 3.12's compensated sum(), int(round(m - round(m), 2) * 100) cents.
+ * ph_dur / ph_num are the CSV fields: values separated by single spaces, ph_dur decimal numbers with an optional exponent,
+ * ph_num integers; any other form is refused.
+ *   some_label_write  chunk c holds notes [sum counts[0 .. c), + counts[c]) starting offsets[c] seconds into the recording;
+ *                     note seconds = (double)note_dur * timestep (frames, as me_infer.py:95).  *seq_size / *dur_size = the
+ *                     bytes of each field including its terminating NUL; a field is written only when its capacity holds it
+ *                     (buffers may be NULL with capacity 0, to ask for the sizes).
+ *   some_notes_label  the same over one result of the session (chunk offsets begin / sample_rate, as some_notes_midi). */
+int some_label_write(int n_chunks, const double* offsets, const int32_t* counts, const float* note_midi, const int32_t* note_dur,
+                     const uint8_t* note_rest, double timestep, const char* ph_dur, const char* ph_num, int round_midi, char* seq_buf,
+                     size_t seq_cap, size_t* seq_size, char* dur_buf, size_t dur_cap, size_t* dur_size);
+int some_notes_label(const some_notes* n, int sample_rate, double timestep, const char* ph_dur, const char* ph_num, int round_midi,
+                     char* seq_buf, size_t seq_cap, size_t* seq_size, char* dur_buf, size_t dur_cap, size_t* dur_size);
+/* some_session_label_dataset: the command of batch_infer.py:149-226 (`--dataset DIR [--csv PATH] [--round_midi]
+ * [--overwrite]`) as some_b200.batch.batch_infer_dataset runs it with load_audio=audio.load_native; the output file is
+ * byte-identical to it, whatever the frame budget and the session's devices.
+ *   Reads DIR/transcriptions.csv as csv.DictReader does (UTF-8; the excel dialect: quoted fields, doubled quotes, newlines
+ * inside quotes; blank lines skipped; short rows padded with absent fields).  Item `name` is read from DIR/wavs/{name}.wav,
+ * whatever format its bytes are (WAV, FLAC, AIFF).  A file that does not exist goes to on_missing(path, user) (may be NULL),
+ * in row order, before any GPU work (batch_infer.py prints "WARNING: audio file does not exist: '<path>'"; the library prints
+ * nothing), and its row keeps its fields.  The other rows go to some_session_transcribe_encoded in groups of at most
+ * params->max_frames frames (1 + samples / hop per item at the model's rate; an item above the budget goes alone; 0 or
+ * params NULL: SOME_SESSION_STEP_SAMPLES / hop), with the slicer params->slicer (NULL: Slicer(sr, max_sil_kept=1000)); a
+ * worker thread reads the files of the next group while a group's step runs.  Writes csv_path (NULL: DIR/transcriptions.csv)
+ * as csv.DictWriter does: the fieldnames name, ph_seq, ph_dur, ph_num, note_seq, note_dur, QUOTE_MINIMAL, \r\n line ends,
+ * UTF-8, empty for absent fields.  Paths in messages and on_missing are spelled as pathlib spells them.
+ *   Refused before any GPU work, with the output file untouched: an existing output without `overwrite` (the reference's
+ * FileExistsError text); a transcriptions.csv that cannot be read or is not UTF-8; when there are rows: a missing name, ph_dur
+ * or ph_num column, and columns outside the six fieldnames or rows longer than the header (DictWriter's "dict contains fields
+ * not in fieldnames: ..." text, fields in the header's order).  The reference truncates the output to its header line in that
+ * last case and raises; here the file is not touched.  A row with audio whose ph_dur / ph_num does not parse is refused, naming
+ * the item (the reference raises after transcribing it).  The session is used only when a row has audio (s may be NULL when
+ * none has).
+ *   A file the encoded step refuses (e.g. a corrupt FLAC stream) or that cannot be read stops the command with the session's
+ * message, naming the file; nothing is written.  report (may be NULL) receives the counts and times of a successful call. */
+typedef struct {
+  const some_slicer_params* slicer; /* NULL: Slicer(sr, max_sil_kept=1000) */
+  long long max_frames;             /* frame budget of one group; 0: SOME_SESSION_STEP_SAMPLES / hop */
+} some_label_params;
+typedef struct {
+  int64_t rows;          /* data rows of transcriptions.csv */
+  int64_t labelled;      /* rows whose audio was transcribed */
+  int64_t missing;       /* rows whose audio file does not exist */
+  int64_t groups;        /* some_session_transcribe_encoded calls */
+  int64_t chunks;        /* slicer chunks of all labelled items */
+  double audio_seconds;  /* of the labelled items (their frames / rate) */
+  double seconds;        /* wall time of the call */
+  double gpu_seconds;    /* of which inside some_session_transcribe_encoded; the rest is host work the steps did not hide */
+} some_label_report;
+typedef void (*some_label_missing_fn)(const char* path, void* user);
+int some_session_label_dataset(some_session* s, const char* dataset_dir, const char* csv_path, int round_midi, int overwrite,
+                               const some_label_params* params, some_label_missing_fn on_missing, void* user,
+                               some_label_report* report);
 /* The slicer's decisions on the HOST (no CUDA call): some_slicer_derive fills the frame counts for a sample rate (params NULL:
  * the session's defaults); some_slicer_ranges turns the RMS list of a recording of n_samples samples (some_slicer_rms) into the
  * [begin, end) sample ranges of its chunks, ranges[2 k], ranges[2 k + 1] (the cuts of Slicer.slice, utils/slicer2.py:82-145).

@@ -175,6 +175,18 @@ class Encoded(C.Structure):
     _fields_ = [('data', _vp), ('n_bytes', C.c_longlong)]
 
 
+class LabelParams(C.Structure):
+    _fields_ = [('slicer', C.POINTER(SlicerParams)), ('max_frames', C.c_longlong)]
+
+
+class LabelReport(C.Structure):
+    _fields_ = [('rows', C.c_int64), ('labelled', C.c_int64), ('missing', C.c_int64), ('groups', C.c_int64),
+                ('chunks', C.c_int64), ('audio_seconds', C.c_double), ('seconds', C.c_double), ('gpu_seconds', C.c_double)]
+
+
+LABEL_MISSING_FN = C.CFUNCTYPE(None, C.c_char_p, _vp)     # some_label_missing_fn
+
+
 AUDIO_WAV, AUDIO_FLAC, AUDIO_AIFF = 1, 2, 3
 PCM_U8, PCM_S16, PCM_S24, PCM_S32, PCM_F32, PCM_F64 = range(1, 7)
 PCM_S8, PCM_S16BE, PCM_S24BE, PCM_S32BE, PCM_F32BE, PCM_F64BE, PCM_ULAW, PCM_ALAW = range(7, 15)
@@ -235,6 +247,12 @@ EXPORTS = {
                                   C.POINTER(C.c_size_t)]),
     'some_notes_midi': (C.c_int, [_vp, C.c_int, C.c_double, C.c_double, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     'some_session_transcribe_encoded': (C.c_int, [_vp, C.POINTER(Encoded), C.c_int, C.POINTER(SlicerParams), _vp]),
+    'some_label_write': (C.c_int, [C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_double, C.c_char_p, C.c_char_p, C.c_int, _vp, C.c_size_t,
+                                   C.POINTER(C.c_size_t), _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    'some_notes_label': (C.c_int, [_vp, C.c_int, C.c_double, C.c_char_p, C.c_char_p, C.c_int, _vp, C.c_size_t,
+                                   C.POINTER(C.c_size_t), _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    'some_session_label_dataset': (C.c_int, [_vp, C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.POINTER(LabelParams),
+                                             LABEL_MISSING_FN, _vp, C.POINTER(LabelReport)]),
     'some_row_stats': (C.c_int, [C.POINTER(RowStatsArgs), _vp]),
     'some_col_means': (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, _vp]),
     'some_forward': (C.c_int, [C.POINTER(ModelC), C.POINTER(WorkspaceC), C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp,

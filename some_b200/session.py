@@ -34,11 +34,41 @@ class Curves(NamedTuple):
     note_index: np.ndarray    # i32: the 1-based note of the frame
 
 
+def _label_call(fn, *args) -> Tuple[str, str]:
+    """Runs some_label_write / some_notes_label (their leading arguments in ``args``): asks for the sizes, then fills."""
+    lib = _lib.load()
+    n_seq, n_dur = C.c_size_t(), C.c_size_t()
+    _lib.check(getattr(lib, fn)(*args, None, 0, C.byref(n_seq), None, 0, C.byref(n_dur)), fn)
+    seq, dur = C.create_string_buffer(n_seq.value), C.create_string_buffer(n_dur.value)
+    _lib.check(getattr(lib, fn)(*args, seq, n_seq.value, C.byref(n_seq), dur, n_dur.value, C.byref(n_dur)), fn)
+    return seq.value.decode('utf8'), dur.value.decode('utf8')
+
+
+def label_write(offsets: Sequence[float], segments: Sequence[Dict[str, np.ndarray]], timestep: float, ph_dur: str, ph_num: str,
+                round_midi: bool = False) -> Tuple[str, str]:
+    """some_label_write: the ``note_seq`` / ``note_dur`` fields of transcriptions.csv for one item, what
+    ``batch.row_notes(ph_dur, ph_num, batch.note_timeline(offsets, segments), round_midi)`` returns for segments whose
+    ``note_dur`` is ``note_frames * timestep`` (each segment's ``note_frames``, int32, are the durations passed)."""
+    counts = np.array([len(sg['note_frames']) for sg in segments] or [0], dtype=np.int32)
+    midi = np.ascontiguousarray(np.concatenate([sg['note_midi'] for sg in segments] or [[]]), dtype=np.float32)
+    frames = np.ascontiguousarray(np.concatenate([sg['note_frames'] for sg in segments] or [[]]), dtype=np.int32)
+    rest = np.ascontiguousarray(np.concatenate([sg['note_rest'] for sg in segments] or [[]]), dtype=np.uint8)
+    offs = np.ascontiguousarray(np.asarray(offsets, dtype=np.float64).reshape(-1))
+    if offs.shape[0] != len(segments):
+        raise ValueError(f'label_write: {offs.shape[0]} offsets for {len(segments)} segments')
+    return _label_call('some_label_write', len(segments), offs.ctypes.data, counts.ctypes.data, midi.ctypes.data,
+                       frames.ctypes.data, rest.ctypes.data, float(timestep), ph_dur.encode('utf8'), ph_num.encode('utf8'),
+                       int(bool(round_midi)))
+
+
 class Notes:
-    """A caller-owned result object (some_notes_create / some_notes_destroy)."""
+    """A caller-owned result object (some_notes_create / some_notes_destroy).  A session call that fills it records the
+    session's sample rate and timestep on it, for label()."""
 
     handle = None
     _frames = False
+    sample_rate = None
+    timestep = None
 
     def __init__(self):
         self.lib = _lib.load()
@@ -77,6 +107,15 @@ class Notes:
 
     def __del__(self):
         self.close()
+
+    def label(self, ph_dur: str, ph_num: str, round_midi: bool = False) -> Tuple[str, str]:
+        """some_notes_label: the ``note_seq`` / ``note_dur`` fields of transcriptions.csv for the recording whose chunks this
+        object holds, with its row's ``ph_dur`` / ``ph_num`` fields: ``batch.row_notes(ph_dur, ph_num,
+        batch.note_timeline(offsets, segments), round_midi)`` of the same notes."""
+        if self.sample_rate is None:
+            raise ValueError('Notes.label: not filled by a session call')
+        return _label_call('some_notes_label', self.handle, int(self.sample_rate), float(self.timestep), ph_dur.encode('utf8'),
+                           ph_num.encode('utf8'), int(bool(round_midi)))
 
     def results(self, timestep: float) -> Tuple[List[Tuple[int, int]], List[Dict[str, np.ndarray]]]:
         """(sample range of every clip, notes of every clip) copied out of the native object."""
@@ -208,14 +247,17 @@ class Session:
 
     def _results(self, notes: Notes, frames: bool):
         """(offsets in seconds, ranges, notes), and the curves when `frames`."""
+        notes.sample_rate, notes.timestep = self.sample_rate, self.timestep
         ranges, res = notes.results(self.timestep)
         offsets = [a / self.sample_rate for a, _ in ranges]
         return (offsets, ranges, res, notes.curves()) if frames else (offsets, ranges, res)
 
-    def transcribe_encoded(self, items: Sequence, params: Optional[_lib.SlicerParams] = None, frames: bool = False):
+    def transcribe_encoded(self, items: Sequence, params: Optional[_lib.SlicerParams] = None, frames: bool = False,
+                           notes: Optional[Sequence[Notes]] = None):
         """some_session_transcribe_encoded: WAV, FLAC or AIFF files (bytes, or paths to read) -> one (chunk offsets in seconds, chunk
         sample ranges, per-chunk notes) per item, what transcribe_sliced returns for audio.load(file, sr=None, mono=True).
-        The files are decoded, resampled, sliced and transcribed in one GPU step."""
+        The files are decoded, resampled, sliced and transcribed in one GPU step.  ``notes``: one caller-owned Notes per item
+        to fill (and keep, e.g. for Notes.label); by default the call uses its own."""
         datas = []
         for it in items:
             if isinstance(it, (bytes, bytearray, memoryview)):
@@ -227,7 +269,10 @@ class Session:
         bufs = [C.create_string_buffer(d, len(d)) if d else None for d in datas]
         enc = (_lib.Encoded * max(k, 1))(*[_lib.Encoded(C.cast(b, C.c_void_p) if b is not None else None, len(d))
                                            for b, d in zip(bufs, datas)])
-        notes = [Notes() for _ in range(k)]
+        own = notes is None
+        if not own and len(notes) != k:
+            raise ValueError(f'transcribe_encoded: {k} items, {len(notes)} Notes')
+        notes = [Notes() for _ in range(k)] if own else list(notes)
         try:
             for n in notes:
                 n.set_frames(frames)
@@ -236,8 +281,32 @@ class Session:
                                                                 outs), 'some_session_transcribe_encoded')
             return [self._results(n, frames) for n in notes]
         finally:
-            for n in notes:
-                n.close()
+            if own:
+                for n in notes:
+                    n.close()
+
+    def label_dataset(self, dataset, csv=None, round_midi: bool = False, overwrite: bool = False, budget: Optional[int] = None,
+                      params: Optional[_lib.SlicerParams] = None, report: Optional[dict] = None):
+        """some_session_label_dataset: batch_infer.py's command on a DiffSinger dataset (``transcriptions.csv`` and ``wavs/``),
+        writing ``csv`` (default: the dataset's own transcriptions.csv) byte for byte as
+        ``batch.batch_infer_dataset(..., load_audio=audio.load_native)`` does, and printing its warning for every missing
+        audio file.  ``budget``: frames per GPU step (default SOME_SESSION_STEP_SAMPLES / hop); the output does not depend on
+        it.  ``report``: a dict to receive the call's counts and times (some_label_report).  Returns the output path."""
+        import pathlib
+
+        def missing(path, _user):
+            print(f"WARNING: audio file does not exist: '{os.fsdecode(path)}'")
+
+        cb = _lib.LABEL_MISSING_FN(missing)
+        lp = _lib.LabelParams(C.pointer(params) if params is not None else None, int(budget or 0))
+        rep = _lib.LabelReport()
+        _lib.check(self.lib.some_session_label_dataset(self.handle, os.fsencode(os.fspath(dataset)),
+                                                       None if csv is None else os.fsencode(os.fspath(csv)), int(bool(round_midi)),
+                                                       int(bool(overwrite)), C.byref(lp), cb, None, C.byref(rep)),
+                   'some_session_label_dataset')
+        if report is not None:
+            report.update({name: getattr(rep, name) for name, _ in _lib.LabelReport._fields_})
+        return pathlib.Path(csv) if csv is not None else pathlib.Path(dataset) / 'transcriptions.csv'
 
     def stream(self, sample_rate: Optional[int] = None, params: Optional[_lib.SlicerParams] = None) -> 'Stream':
         """some_stream_open: a recording pushed while it arrives (see Stream)."""
