@@ -323,87 +323,6 @@ def test_dwconv_bn_silu(lib):
             r0 += t
 
 
-@pytest.mark.parametrize('impl', ['some_attention_varlen'])
-@pytest.mark.parametrize('frames', [[1], [64, 65, 127, 128, 129], [700, 3, 259], [2584]])
-def test_attention_varlen(lib, frames, impl):
-    torch.manual_seed(7)
-    cu = _cu(frames)
-    m = int(cu[-1])
-    qkv = [(torch.randn(m, 1536, device=DEV) * 1.5).to(torch.bfloat16) for _ in range(2)]
-    out = [torch.full((m, 512), float('nan'), device=DEV, dtype=torch.bfloat16) for _ in range(2)]
-    a = _lib.AttnArgs()
-    a.qkv, a.out = _lib.pair(*qkv), _lib.pair(*out)
-    a.groups, a.B, a.M, a.cu_frames, a.max_frames = 2, len(frames), m, cu.data_ptr(), max(frames)
-    _lib.check(getattr(lib, impl)(C.byref(a), stream()), impl)
-    torch.cuda.synchronize()
-    for i in range(2):
-        r0 = 0
-        for t in frames:
-            z = qkv[i][r0:r0 + t].float()
-            q, k, v = (z[:, j * 512:(j + 1) * 512].reshape(t, 8, 64).transpose(0, 1) for j in range(3))
-            ref = torch.nn.functional.scaled_dot_product_attention(q[None], k[None], v[None])[0]
-            ref = ref.transpose(0, 1).reshape(t, 512)
-            # P is rounded to bf16 before P.V, output rounded to bf16
-            torch.testing.assert_close(out[i][r0:r0 + t].float(), ref, atol=2e-2, rtol=2e-2)
-            r0 += t
-
-
-def test_attention_growing_max_forces_rescale(lib):
-    """Scores whose row maximum jumps by far more than 2^8 from one key tile to the next: exercises the lazy
-    O-rescale path of the attention kernel on every tile (a race there shows up as wrong rows)."""
-    torch.manual_seed(8)
-    frames = [1500, 333]
-    cu = _cu(frames)
-    m = int(cu[-1])
-    qkv = torch.randn(m, 1536, device=DEV) * 0.5
-    ramp = torch.cat([torch.arange(t, device=DEV, dtype=torch.float32) / 64.0 for t in frames])   # grows with the key index
-    qkv[:, 512:1024] += ramp[:, None] * torch.sign(torch.randn(1, 512, device=DEV))
-    qkv[:, :512] = qkv[:, :512].abs() * torch.sign(qkv[0:1, 512:1024] - 0.0 + 1e-3) * 2.0
-    qkv = qkv.to(torch.bfloat16)
-    out = torch.full((m, 512), float('nan'), device=DEV, dtype=torch.bfloat16)
-    a = _lib.AttnArgs()
-    a.qkv, a.out = _lib.pair(qkv), _lib.pair(out)
-    a.groups, a.B, a.M, a.cu_frames, a.max_frames = 1, len(frames), m, cu.data_ptr(), max(frames)
-    for _ in range(3):      # repeat: the failure mode is timing dependent
-        out.fill_(float('nan'))
-        _lib.check(lib.some_attention_varlen(C.byref(a), stream()))
-        torch.cuda.synchronize()
-        r0 = 0
-        for t in frames:
-            z = qkv[r0:r0 + t].float()
-            q, k, v = (z[:, j * 512:(j + 1) * 512].reshape(t, 8, 64).transpose(0, 1) for j in range(3))
-            ref = torch.nn.functional.scaled_dot_product_attention(q[None], k[None], v[None])[0]
-            ref = ref.transpose(0, 1).reshape(t, 512)
-            torch.testing.assert_close(out[r0:r0 + t].float(), ref, atol=3e-2, rtol=3e-2)
-            r0 += t
-
-
-@pytest.mark.parametrize('outlier', [200, 206, 519, 1023])
-def test_attention_outlier_key_after_the_first_tile(lib, outlier):
-    """The exp pass runs against the group's stale reference maximum and a tile is redone only when its row sum gives an
-    overflow away (attention_tc.cu).  One key far above everything seen so far -- by more than 2^127 in the exponent, so the
-    first attempt produces +inf -- placed in a tile other than a group's first one, at a position handled by the MUFU path
-    (key index % 8 < 6) or by the polynomial path (% 8 in {6, 7}, which must clamp instead of wrapping around)."""
-    torch.manual_seed(9)
-    t = 1100
-    cu = _cu([t])
-    qkv = torch.randn(t, 1536, device=DEV) * 0.5
-    qkv[:, :512] = qkv[:, :512].abs()                         # q > 0, so a key of all + LARGE scores high against every query
-    qkv[outlier, 512:1024] = 40.0                             # score ~ 64 * 0.4 * 40 = 1000  ->  1000 / 8 * log2(e) = 180 > 127
-    qkv = qkv.to(torch.bfloat16)
-    out = torch.full((t, 512), float('nan'), device=DEV, dtype=torch.bfloat16)
-    a = _lib.AttnArgs()
-    a.qkv, a.out = _lib.pair(qkv), _lib.pair(out)
-    a.groups, a.B, a.M, a.cu_frames, a.max_frames = 1, 1, t, cu.data_ptr(), t
-    _lib.check(lib.some_attention_varlen(C.byref(a), stream()))
-    torch.cuda.synchronize()
-    z = qkv.float()
-    q, k, v = (z[:, j * 512:(j + 1) * 512].reshape(t, 8, 64).transpose(0, 1) for j in range(3))
-    ref = torch.nn.functional.scaled_dot_product_attention(q[None], k[None], v[None])[0].transpose(0, 1).reshape(t, 512)
-    assert torch.isfinite(out.float()).all()
-    torch.testing.assert_close(out.float(), ref, atol=2e-2, rtol=2e-2)     # every row is (almost) exactly v[outlier]
-
-
 def test_mel_matches_torch_stft(lib):
     from some_b200 import synth
     from some_b200.engine import Engine
