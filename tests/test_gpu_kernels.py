@@ -212,22 +212,6 @@ def test_gemm_ln_consumer(lib, kind, parts):
         assert float((out[i].float() - ref[i]).abs().mean()) < 6e-3
 
 
-def test_row_stats(lib):
-    torch.manual_seed(40)
-    m = 1003
-    x = [torch.randn(m, 512, device=DEV) * 2 - 0.3 for _ in range(2)]
-    xb = [torch.empty(m, 512, device=DEV, dtype=torch.bfloat16) for _ in range(2)]
-    st = [torch.full((m, _lib.LN_SLOTS, 2), float('nan'), device=DEV) for _ in range(2)]
-    a = _lib.RowStatsArgs()
-    a.x, a.out_bf16, a.ln_stats, a.groups, a.M = _lib.pair(*x), _lib.pair(*xb), _lib.pair(*st), 2, m
-    _lib.check(lib.some_row_stats(C.byref(a), stream()), 'some_row_stats')
-    torch.cuda.synchronize()
-    for i in range(2):
-        assert torch.equal(xb[i], x[i].to(torch.bfloat16))
-        torch.testing.assert_close(st[i][:, 0, 0], x[i].sum(1), atol=1e-3, rtol=1e-5)
-        torch.testing.assert_close(st[i][:, 0, 1], (x[i] * x[i]).sum(1), atol=1e-2, rtol=1e-5)
-
-
 @pytest.mark.parametrize('normalised', [False, True])
 def test_col_means_match_and_repeat_bit_for_bit(lib, normalised):
     """The load-time bias correction is built from these means: they must not depend on the run (fixed summation order)."""
@@ -267,60 +251,10 @@ def test_gemm_heads(lib, n, epi):
     torch.testing.assert_close(out, ref, atol=2e-4, rtol=2e-4)
 
 
-def test_layernorm_and_bound_head(lib):
-    torch.manual_seed(5)
-    m = 1003
-    x = [torch.randn(m, 512, device=DEV) * 3 + 1.5 for _ in range(2)]
-    g = [torch.rand(512, device=DEV) + 0.5 for _ in range(2)]
-    b = [torch.randn(512, device=DEV) * 0.1 for _ in range(2)]
-    ob = [torch.empty(m, 512, device=DEV, dtype=torch.bfloat16) for _ in range(2)]
-    of = [torch.empty(m, 512, device=DEV) for _ in range(2)]
-    a = _lib.LnArgs()
-    a.x, a.gamma, a.beta = _lib.pair(*x), _lib.pair(*g), _lib.pair(*b)
-    a.out_bf16, a.out_f32, a.groups, a.M = _lib.pair(*ob), _lib.pair(*of), 2, m
-    _lib.check(lib.some_layernorm(C.byref(a), stream()))
-    torch.cuda.synchronize()
-    for i in range(2):
-        ref = torch.nn.functional.layer_norm(x[i], (512,), g[i], b[i], 1e-5)
-        torch.testing.assert_close(of[i], ref, atol=1e-5, rtol=1e-5)
-        torch.testing.assert_close(ob[i].float(), ref, atol=2e-2, rtol=1e-2)   # bf16 rounding
-    w = torch.randn(512, device=DEV) / 512 ** 0.5
-    bounds = torch.empty(m, device=DEV)
-    _lib.check(lib.some_bound_head(x[0].data_ptr(), g[0].data_ptr(), b[0].data_ptr(), w.data_ptr(), 0.3, m,
-                                   bounds.data_ptr(), stream()))
-    torch.cuda.synchronize()
-    ref = torch.sigmoid(torch.nn.functional.layer_norm(x[0], (512,), g[0], b[0], 1e-5) @ w + 0.3)
-    torch.testing.assert_close(bounds, ref, atol=1e-5, rtol=1e-5)
-
-
 def _cu(frames):
     cu = np.zeros(len(frames) + 1, dtype=np.int32)
     np.cumsum(frames, out=cu[1:])
     return torch.from_numpy(cu).to(DEV)
-
-
-def test_dwconv_bn_silu(lib):
-    torch.manual_seed(6)
-    frames = [1, 17, 128, 129, 300, 31]
-    cu = _cu(frames)
-    m = int(cu[-1])
-    x = [torch.randn(m, 512, device=DEV).to(torch.bfloat16) for _ in range(2)]
-    w = [torch.randn(31, 512, device=DEV) * 0.2 for _ in range(2)]
-    b = [torch.randn(512, device=DEV) * 0.1 for _ in range(2)]
-    out = [torch.full((m, 512), float('nan'), device=DEV, dtype=torch.bfloat16) for _ in range(2)]
-    a = _lib.DwconvArgs()
-    a.x, a.w, a.b, a.out = _lib.pair(*x), _lib.pair(*w), _lib.pair(*b), _lib.pair(*out)
-    a.groups, a.B, a.cu_frames, a.max_frames = 2, len(frames), cu.data_ptr(), max(frames)
-    _lib.check(lib.some_dwconv_bn_silu(C.byref(a), stream()))
-    torch.cuda.synchronize()
-    for i in range(2):
-        r0 = 0
-        for t in frames:
-            xi = x[i][r0:r0 + t].float().t().unsqueeze(0)                       # [1, 512, t]
-            wi = w[i].t().unsqueeze(1)                                          # [512, 1, 31]
-            ref = torch.nn.functional.silu(torch.nn.functional.conv1d(xi, wi, b[i], padding=15, groups=512))[0].t()
-            torch.testing.assert_close(out[i][r0:r0 + t].float(), ref, atol=3e-2, rtol=2e-2)   # bf16 out
-            r0 += t
 
 
 def test_mel_matches_torch_stft(lib):
