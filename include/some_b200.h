@@ -491,6 +491,34 @@ long long some_pcm_decode_bytes(int K);
 int some_pcm_decode_pack(const some_pcm_item* items, int K, void* desc);
 int some_pcm_decode(const void* desc, const void* desc_d, cudaStream_t stream);
 
+/* ---- K-downmix (csrc/downmix.cu): librosa.to_mono of float32 audio already in device memory, many recordings in one launch.
+ * Output sample f of an item is np.mean(y, axis=0) in float32 of librosa's (channels, frames) view y, bit for bit.  numpy's
+ * order depends on the layout:
+ *   SOME_DOWNMIX_MONO         a one-dimensional recording (one channel): the value itself;
+ *   SOME_DOWNMIX_PLANAR       frames contiguous, channel c at data + c * channel_stride (>= frames): the channels added in
+ *                             order starting from +0.0 (an all -0.0 frame gives +0.0), then / channels;
+ *   SOME_DOWNMIX_INTERLEAVED  channels contiguous, frame f at data + f * channels: numpy's pairwise sum, the order of
+ *                             some_pcm_decode's mono output; an item of one frame reads channel c at data + c * channel_stride
+ *                             (numpy reduces a lone frame in this order whatever its strides).
+ * some_downmix_layout names the layout of `channels` x `frames` floats with the given strides in floats (channel_stride 0 with
+ * one channel: a one-dimensional recording), or refuses any other stride pattern (host only, no CUDA call).  Packed and
+ * launched like some_pcm_decode: some_downmix_pack checks every item (the message names it) into host memory of
+ * some_downmix_bytes(K) bytes; some_downmix launches from it and its device copy desc_d (16-byte aligned).  The native session
+ * down-mixes device audio with the same launch (some_session_transcribe_device). */
+enum { SOME_DOWNMIX_MONO = 0, SOME_DOWNMIX_PLANAR = 1, SOME_DOWNMIX_INTERLEAVED = 2 };
+typedef struct {
+  const float* data;             /* device: channel 0 of frame 0 */
+  long long frames;              /* samples per channel */
+  int channels;                  /* 1..128 */
+  int layout;                    /* SOME_DOWNMIX_* */
+  long long channel_stride;      /* floats between channels: planar, and an interleaved item of one frame */
+  float* out;                    /* device: frames floats */
+} some_downmix_item;
+int some_downmix_layout(int channels, long long frames, long long channel_stride, long long frame_stride, int* layout);
+long long some_downmix_bytes(int K);
+int some_downmix_pack(const some_downmix_item* items, int K, void* desc);
+int some_downmix(const void* desc, const void* desc_d, cudaStream_t stream);
+
 /* ---- MIDI bytes (host, no CUDA call): the Standard MIDI File some_b200.midi.build_midi_file(offsets, segments,
  * tempo).to_bytes() writes, with note_dur seconds = (double)note_dur * timestep.  Chunk c holds notes
  * [sum counts[0 .. c), + counts[c]).  Ticks follow infer_utils.build_midi_file: offsets * tempo * 8 rounded half to even,
@@ -1062,6 +1090,53 @@ int some_stream_get_meta(const some_stream* st, some_audio_meta* meta, long long
  * touches the same stream or some_notes, and run after every earlier call on their streams. */
 int some_stream_peek(some_stream* st, some_notes* out);
 int some_stream_peek_many(some_stream* const* streams, int count, some_notes* const* out);
+
+/* ---- Audio already on the GPU: float32 recordings in device memory (a vocal stem a separation model left there, often stereo)
+ * into the session and its PCM streams, down-mixed as librosa.to_mono does, with no host copy.  An item is `channels` x
+ * `frames` floats; sample (c, f) lies at data + c * channel_stride + f * frame_stride.  The layout follows from the strides
+ * (some_downmix_layout): a one-dimensional recording (one channel, channel_stride 0, frame_stride 1), planar (frame_stride 1,
+ * channel_stride >= frames: librosa's C-contiguous [channels, n], or a view of one with a larger channel stride) or
+ * interleaved (channel_stride 1, frame_stride = channels: librosa's [channels, n] view of an [n, channels] array); any other
+ * stride pattern is refused.  The mono samples are np.mean(y, axis=0) of that (channels, frames) view in float32, bit for bit,
+ * in numpy's order for the layout (K-downmix).
+ *   some_session_transcribe_device: for item i, out[i] receives what some_session_transcribe_sliced(s, m, frames,
+ * sample_rate, params, out[i]) gives for its host down-mix m = np.mean(y, axis=0): the same chunk ranges, bit-identical notes
+ * and, with some_notes_set_frames, bit-identical frame curves.  Results do not depend on the other items.  The call is one
+ * recordings request (see "Calls from several threads"): it shares a step with sliced and encoded calls, counting each item's
+ * model-rate samples against SOME_SESSION_STEP_SAMPLES; the step down-mixes every device item with one some_downmix launch
+ * into the recording buffer, then resamples, cuts and transcribes as for host recordings.
+ *   some_stream_push_device: the effect of some_stream_push of the item's down-mixed samples; sample_rate must equal the
+ * stream's.  Host and device pushes may be mixed on one stream and split in any way; the chunks stay those of
+ * some_session_transcribe_sliced.  The stream step down-mixes device items straight into the stream's window.
+ * some_stream_push_device_many is some_stream_push_many with device items (and its refusals, encoded streams included); it
+ * shares a step with any PCM push request.
+ *   Ordering: at the call, an event is recorded on each item's `stream` (0: the legacy default stream of `device`), and the
+ * session's stream waits on it before its first read of the item; nothing else is enqueued on the caller's streams, and the
+ * caller need not synchronise.  When a call returns, the session no longer reads its items: the caller may overwrite or free
+ * them.  Items may lie on any visible device; an item on another device than the session's first is copied to it
+ * (cudaMemcpyPeerAsync, packed) before the down-mix; peer access is used when the application has enabled it, not required.
+ *   Memory: besides what the same host call holds, the session keeps (grow-only) room for the packed copies of a step's items
+ * on other devices; items on its own device are read where they lie.
+ *   Refused before any GPU work, with the index i in the message and no out[i] touched: the refusals of the host calls (NULL
+ * arrays, count < 0, NULL or shared some_notes, finished or encoded streams, ...); data NULL with frames > 0, or frames < 0;
+ * channels outside 1..128; a stride pattern that is none of the three layouts; data that cudaPointerGetAttributes does not
+ * report as device memory of `device` (a host pointer, for one); a rate pair the resampler refuses or a recording too short to
+ * resample.  The session stays usable after a refusal.  count == 0 does nothing. */
+typedef struct {
+  const float* data;        /* device memory of `device` */
+  int device;
+  long long frames;
+  int channels;             /* 1..128 */
+  long long channel_stride; /* in floats; the layout follows from the two strides */
+  long long frame_stride;
+  int sample_rate;
+  cudaStream_t stream;      /* the stream that produced `data` (0: legacy default stream of `device`) */
+} some_device_audio;
+int some_session_transcribe_device(some_session* s, const some_device_audio* items, int count, const some_slicer_params* params,
+                                   some_notes* const* out);
+int some_stream_push_device(some_stream* st, const some_device_audio* a, some_notes* out);
+int some_stream_push_device_many(some_stream* const* streams, const some_device_audio* items, const int* finish, int count,
+                                 some_notes* const* out);
 
 #ifdef __cplusplus
 }

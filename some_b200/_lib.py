@@ -171,6 +171,19 @@ class PcmItem(C.Structure):
                 ('reserved', C.c_int), ('out', _vp)]
 
 
+DOWNMIX_MONO, DOWNMIX_PLANAR, DOWNMIX_INTERLEAVED = range(3)      # SOME_DOWNMIX_*
+
+
+class DownmixItem(C.Structure):
+    _fields_ = [('data', _vp), ('frames', C.c_longlong), ('channels', C.c_int), ('layout', C.c_int),
+                ('channel_stride', C.c_longlong), ('out', _vp)]
+
+
+class DeviceAudio(C.Structure):
+    _fields_ = [('data', _vp), ('device', C.c_int), ('frames', C.c_longlong), ('channels', C.c_int),
+                ('channel_stride', C.c_longlong), ('frame_stride', C.c_longlong), ('sample_rate', C.c_int), ('stream', _vp)]
+
+
 class Encoded(C.Structure):
     _fields_ = [('data', _vp), ('n_bytes', C.c_longlong)]
 
@@ -243,6 +256,10 @@ EXPORTS = {
     'some_pcm_decode_bytes': (C.c_longlong, [C.c_int]),
     'some_pcm_decode_pack': (C.c_int, [C.POINTER(PcmItem), C.c_int, _vp]),
     'some_pcm_decode': (C.c_int, [_vp, _vp, _vp]),
+    'some_downmix_layout': (C.c_int, [C.c_int, C.c_longlong, C.c_longlong, C.c_longlong, C.POINTER(C.c_int)]),
+    'some_downmix_bytes': (C.c_longlong, [C.c_int]),
+    'some_downmix_pack': (C.c_int, [C.POINTER(DownmixItem), C.c_int, _vp]),
+    'some_downmix': (C.c_int, [_vp, _vp, _vp]),
     'some_midi_write': (C.c_int, [C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_double, C.c_double, _vp, C.c_size_t,
                                   C.POINTER(C.c_size_t)]),
     'some_notes_midi': (C.c_int, [_vp, C.c_int, C.c_double, C.c_double, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
@@ -309,6 +326,9 @@ EXPORTS = {
     'some_stream_get_meta': (C.c_int, [_vp, C.POINTER(AudioMeta), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]),
     'some_stream_peek': (C.c_int, [_vp, _vp]),
     'some_stream_peek_many': (C.c_int, [_vp, C.c_int, _vp]),
+    'some_session_transcribe_device': (C.c_int, [_vp, C.POINTER(DeviceAudio), C.c_int, C.POINTER(SlicerParams), _vp]),
+    'some_stream_push_device': (C.c_int, [_vp, C.POINTER(DeviceAudio), _vp]),
+    'some_stream_push_device_many': (C.c_int, [_vp, C.POINTER(DeviceAudio), _vp, C.c_int, _vp]),
 }
 
 _lib = None

@@ -444,3 +444,70 @@ def load_native(path, sr=None):
     the caller wants (batch.batch_infer_dataset passes it) and is ignored: a loader that returns (waveform, rate) has the
     dataset driver resample on the device, straight into the batch's wave buffer."""
     return load(path, sr=None)
+
+
+# ---------------------------------------------------------------------------------------------- float32 audio on the device
+def is_cuda_tensor(x) -> bool:
+    """Whether ``x`` is a CUDA torch tensor (without importing torch when the caller has not)."""
+    import sys
+    torch = sys.modules.get('torch')
+    return torch is not None and isinstance(x, torch.Tensor) and x.is_cuda
+
+
+def device_layout(t, index: int, who: str) -> Tuple[int, int, int, int, int]:
+    """(channels, frames, channel stride, frame stride, layout) of a float32 recording tensor, ``[n]`` or librosa's
+    ``[channels, n]``, read from its shape and ``stride()`` (some_downmix_layout: mono, planar or interleaved).  Raises
+    ValueError naming item ``index`` for another dtype, rank or stride pattern.  Host only: CPU tensors are mapped too."""
+    import torch
+    from . import _lib
+    where = f'{who}: item {index}'
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f'{where}: a torch tensor expected, got {type(t).__name__}')
+    if t.dtype != torch.float32:
+        raise ValueError(f'{where}: float32 audio expected, got {t.dtype}')
+    if t.dim() == 1:
+        ch, n, cs, fs = 1, int(t.shape[0]), 0, int(t.stride(0))
+    elif t.dim() == 2:
+        (ch, n), (cs, fs) = (int(v) for v in t.shape), (int(v) for v in t.stride())
+    else:
+        raise ValueError(f'{where}: [n] or [channels, n] expected, got shape {tuple(t.shape)}')
+    lib = _lib.load()
+    layout = C.c_int()
+    if lib.some_downmix_layout(ch, n, cs, fs, C.byref(layout)) != 0:
+        raise ValueError(f'{where}: {lib.some_last_error().decode("utf8", "replace")}')
+    return ch, n, cs, fs, layout.value
+
+
+def device_audio(t, index: int, who: str, sample_rate: int):
+    """The some_device_audio descriptor of CUDA float32 recording ``t`` (see device_layout) at ``sample_rate``, produced on
+    the current stream of its device; ValueError naming item ``index`` for a CPU tensor or what device_layout refuses."""
+    import torch
+    from . import _lib
+    ch, n, cs, fs, _ = device_layout(t, index, who)
+    if not t.is_cuda:
+        raise ValueError(f'{who}: item {index}: a CUDA tensor expected, got one on {t.device}')
+    stream = torch.cuda.current_stream(t.device).cuda_stream
+    return _lib.DeviceAudio(t.data_ptr() if n else None, t.device.index, n, ch, cs, fs, int(sample_rate), stream or None)
+
+
+def downmix_into(items: Sequence[Tuple[object, object, int]], who: str = 'downmix_into') -> None:
+    """One some_downmix launch on the current stream of the destinations' device: item (t, dst, at) writes np.mean(y,
+    axis=0) in float32 of the CUDA float32 recording t ([n] or librosa's [channels, n], on dst's device) to dst[at : at +
+    frames], bit for bit."""
+    import torch
+    from . import _lib
+    if not items:
+        return
+    lib = _lib.load()
+    dev = items[0][1].device
+    arr = (_lib.DownmixItem * len(items))()
+    for k, (t, dst, at) in enumerate(items):
+        ch, n, cs, _, layout = device_layout(t, k, who)
+        if t.device != dev or dst.device != dev or dst.dtype != torch.float32 or at < 0 or at + n > dst.numel():
+            raise ValueError(f'{who}: item {k}: a recording on {t.device} into {dst.numel()} floats of {dst.device} at {at}')
+        arr[k] = _lib.DownmixItem(t.data_ptr() if n else None, n, ch, layout, cs, dst.data_ptr() + 4 * at if n else None)
+    desc = np.zeros(int(lib.some_downmix_bytes(len(items))), np.uint8)
+    _lib.check(lib.some_downmix_pack(arr, len(items), desc.ctypes.data), 'some_downmix_pack')
+    desc_d = torch.from_numpy(desc).to(dev)
+    _lib.check(lib.some_downmix(desc.ctypes.data, desc_d.data_ptr(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+               'some_downmix')

@@ -196,12 +196,17 @@ def row_notes(ph_dur_field: str, ph_num_field: str, notes: List[dict], round_mid
 def stage_recordings(eng, target_sr: int, waveforms: Sequence, rates: Optional[Sequence[Optional[int]]]):
     """Uploads mono recordings (numpy arrays, or ``audio.EncodedAudio`` FLAC records) into ONE device buffer at
     ``target_sr``, as transcribe_recordings describes: recordings at another rate are resampled on the device, FLAC records
-    decoded there.  Call on the engine's device.  Returns (wave_d, bases int64 [n + 1], lens, flac_status): recording i is
+    decoded there, and CUDA float32 tensors (``[n]`` or librosa's ``[channels, n]``) down-mixed there by one some_downmix
+    launch per destination, with no host copy.  Call on the engine's device.  Returns (wave_d, bases int64 [n + 1], lens, flac_status): recording i is
     wave_d[bases[i] : bases[i] + lens[i]]; the FLAC status words are checked with audio._check_status once the stream has
     passed them, as ``staged`` does."""
     import torch
     enc = {i: w for i, w in enumerate(waveforms) if isinstance(w, audio.EncodedAudio)}
-    waves = [None if i in enc else np.ascontiguousarray(w, dtype=np.float32) for i, w in enumerate(waveforms)]
+    here = torch.empty(0, device=eng.device).device                            # with its index
+    dev = {i: w for i, w in enumerate(waveforms) if audio.is_cuda_tensor(w)}    # on another device: copied to the engine's
+    dev = {i: t if t.device == here else t.to(here) for i, t in dev.items()}
+    dev_frames = {i: audio.device_layout(t, i, 'stage_recordings')[1] for i, t in dev.items()}
+    waves = [None if i in enc or i in dev else np.ascontiguousarray(w, dtype=np.float32) for i, w in enumerate(waveforms)]
     for w in waves:
         assert w is None or w.ndim == 1, 'mono recordings expected (librosa.load(..., mono=True), batch_infer.py:51)'
     if rates is None:
@@ -215,7 +220,8 @@ def stage_recordings(eng, target_sr: int, waveforms: Sequence, rates: Optional[S
     if enc:                                                        # scan + chain: one device-to-host copy, one sync
         flac = audio.FlacBatch(list(enc.values()), eng.device)
     slot = {i: k for k, i in enumerate(enc)}                       # recording -> its index in the FlacBatch
-    native_lens = [flac.lengths[slot[i]] if i in enc else int(w.shape[0]) for i, w in enumerate(waves)]
+    native_lens = [flac.lengths[slot[i]] if i in enc else dev_frames[i] if i in dev else int(w.shape[0])
+                   for i, w in enumerate(waves)]
     lens = [audio.resampled_length(n, r, target_sr) for n, r in zip(native_lens, rates)]
     bases = np.zeros(len(waves) + 1, dtype=np.int64)
     np.cumsum([(n + 3) & ~3 for n in lens], out=bases[1:])
@@ -224,6 +230,7 @@ def stage_recordings(eng, target_sr: int, waveforms: Sequence, rates: Optional[S
         if n and r == target_sr and w is not None:
             src = torch.from_numpy(w)
             wave_d[b:b + n].copy_(src, non_blocking=src.is_pinned())
+    audio.downmix_into([(dev[i], wave_d, int(bases[i])) for i in dev if rates[i] == target_sr], 'stage_recordings')
     flac_status = []
     direct = {slot[i]: int(bases[i]) for i in enc if rates[i] == target_sr}
     if direct:
@@ -234,8 +241,9 @@ def stage_recordings(eng, target_sr: int, waveforms: Sequence, rates: Optional[S
         np.cumsum([native_lens[i] for i in group], out=starts[1:])
         native_d = torch.empty(max(int(starts[-1]), 1), dtype=torch.float32, device=eng.device)
         for i, a in zip(group, starts):
-            if i not in enc:
+            if i not in enc and i not in dev:
                 native_d[a:a + native_lens[i]].copy_(torch.from_numpy(waves[i]))
+        audio.downmix_into([(dev[i], native_d, int(a)) for i, a in zip(group, starts) if i in dev], 'stage_recordings')
         to_decode = {slot[i]: int(a) for i, a in zip(group, starts) if i in enc}
         if to_decode:
             flac_status.append(flac.emit(native_d, to_decode))

@@ -1,4 +1,5 @@
-// The down-mix of librosa.to_mono, shared by the FLAC emitter (flac.cu) and the PCM decoder (pcm.cu).
+// The down-mix of librosa.to_mono, shared by the FLAC emitter (flac.cu), the PCM decoder (pcm.cu) and the float32 down-mix of
+// audio already on the device (downmix.cu).
 #pragma once
 
 namespace some {
@@ -31,6 +32,24 @@ __device__ __forceinline__ float mono_mean(int ch, F value) {
     for (; i < ch; ++i) sum = __fadd_rn(sum, value(i));
   }
   return __fdiv_rn(__fadd_rn(0.f, sum), static_cast<float>(ch));
+}
+
+// np.mean(y, axis=0) in float32 for a (channels, n) array whose frames are contiguous (a C-contiguous [channels, n] array,
+// or a view of one with a larger channel stride), n >= 2: numpy adds the rows one after another into an output that starts
+// from the identity +0.0 (so an all -0.0 frame gives +0.0, also for one channel), then divides by the channel count.  The
+// order differs from mono_mean's from 8 channels up.  N frames at once, so that their loads are in flight together:
+// value(c, k) returns channel c of frame k, mean[k] receives frame k's mean.  1 <= ch.
+template <int N, class F>
+__device__ __forceinline__ void mono_mean_planar(int ch, F value, float (&mean)[N]) {
+  float sum[N];
+#pragma unroll
+  for (int k = 0; k < N; ++k) sum[k] = 0.f;
+#pragma unroll 2
+  for (int c = 0; c < ch; ++c)
+#pragma unroll
+    for (int k = 0; k < N; ++k) sum[k] = __fadd_rn(sum[k], value(c, k));
+#pragma unroll
+  for (int k = 0; k < N; ++k) mean[k] = __fdiv_rn(sum[k], static_cast<float>(ch));
 }
 
 }  // namespace some

@@ -373,6 +373,7 @@ struct some_session {
   // the encoded calls' Decode: the audio bytes, the FLAC candidate list, scan workspace and int32 scratch
   DevBuf enc_d, flac_frames_d, flac_ws_d, flac_scratch_d;
   PinBuf enc_h, flac_frames_h;
+  DevBuf peer_d;                          // the packed copies of a step's device audio that lies on other devices
   std::vector<std::unique_ptr<Replica>> reps;
   // lane r runs replica r's share of a step (lane 0 on the calling thread, the only lane of a one-device session); with
   // several replicas, `fed` is recorded on replica 0's stream once the front end has written the chunks the others copy
@@ -1126,6 +1127,9 @@ int slice_ranges(const SliceShape& sh, const float* rms, const some_slicer_frame
 struct RecItem {
   const float* host = nullptr;
   const uint8_t* bytes = nullptr;
+  const some_device_audio* dev = nullptr;   // the device call: its item, the item's layout and the event its producer recorded
+  int layout = 0;
+  cudaEvent_t ready = nullptr;
   some_audio_meta m{};        // of the file; the sliced call sets only its rate
   int64_t n = 0;              // samples at its rate (FLAC without a stated length: known after the chain)
   SliceShape sh;
@@ -1245,6 +1249,74 @@ struct StepWindows {
     if (frames)
       SOME_CUDA(cudaMemcpyAsync(s->rms_h.p, s->rms_d.p, 4ull * frames, cudaMemcpyDeviceToHost, s->stream), "RMS download");
     return 0;
+  }
+};
+
+// The device audio of a step (some_session_transcribe_device, some_stream_push_device*), down-mixed by one some_downmix launch
+// into the session's buffers:
+//   add     the descriptor region of k items in the step's upload;
+//   push    an item, with where its frames mono samples go (on the session's device) and the event its producer recorded;
+//   fill    after every push: room for the packed copies of the items on other devices, and the descriptors;
+//   launch  after the upload is sent: the session's stream waits on every item's event, copies the items on other devices
+//           (cudaMemcpyPeerAsync: channel c of a planar item to c * frames) and launches the down-mix.
+struct Downmix {
+  std::vector<some_downmix_item> items;
+  std::vector<const some_device_audio*> src;
+  std::vector<cudaEvent_t> ready;
+  size_t off = 0;
+  int k = 0;
+
+  void add(Upload& up, int count) {
+    k = count;
+    if (k) off = up.add(static_cast<size_t>(some_downmix_bytes(k)));
+  }
+  void push(const some_device_audio& a, int layout, cudaEvent_t ev, float* out) {
+    items.push_back(some_downmix_item{a.data, a.frames, a.channels, layout, a.channel_stride, out});
+    src.push_back(&a), ready.push_back(ev);
+  }
+  // A copied item's channels lie `rows` floats apart (rows 0: the item is copied as one block).
+  static int64_t rows(const some_downmix_item& it) {
+    if (it.channels == 1) return 0;
+    return it.layout == SOME_DOWNMIX_PLANAR ? it.frames : it.layout == SOME_DOWNMIX_INTERLEAVED && it.frames == 1 ? 1 : 0;
+  }
+  bool remote(const some_session* s, size_t j) const { return src[j]->device != s->device && items[j].frames > 0; }
+  int fill(some_session* s, const Upload& up) {
+    SOME_REQUIRE(static_cast<int>(items.size()) == k, "session: %zu device items, %d placed", items.size(), k);
+    if (k == 0) return 0;
+    int64_t total = 0;
+    for (size_t j = 0; j < items.size(); ++j)
+      if (remote(s, j)) total += align4(items[j].frames * items[j].channels);
+    if (total && s->peer_d.ensure(4ull * total + 16, "the copies of device audio")) return -1;
+    float* at = static_cast<float*>(s->peer_d.p);
+    for (size_t j = 0; j < items.size(); ++j)
+      if (remote(s, j)) {
+        some_downmix_item& it = items[j];
+        it.data = at;
+        if (rows(it)) it.channel_stride = rows(it);
+        at += align4(it.frames * it.channels);
+      }
+    return some_downmix_pack(items.data(), k, up.h(off));
+  }
+  int launch(some_session* s, const Upload& up) const {
+    if (k == 0) return 0;
+    for (cudaEvent_t e : ready)
+      if (e) SOME_CUDA(cudaStreamWaitEvent(s->stream, e, 0), "waiting for the device audio's stream");
+    for (size_t j = 0; j < items.size(); ++j) {
+      if (!remote(s, j)) continue;
+      const some_device_audio& a = *src[j];
+      const some_downmix_item& it = items[j];
+      float* dst = const_cast<float*>(it.data);
+      const int64_t r = rows(it);
+      if (r) {
+        for (int c = 0; c < it.channels; ++c)
+          SOME_CUDA(cudaMemcpyPeerAsync(dst + c * r, s->device, a.data + c * a.channel_stride, a.device, 4ull * r, s->stream),
+                    "device audio copy");
+      } else {
+        SOME_CUDA(cudaMemcpyPeerAsync(dst, s->device, a.data, a.device, 4ull * it.frames * it.channels, s->stream),
+                  "device audio copy");
+      }
+    }
+    return some_downmix(up.h(off), up.d(off), s->stream);
   }
 };
 
@@ -1428,6 +1500,9 @@ struct StepItem {
   int64_t n;
   bool final;
   some_notes* out;
+  const some_device_audio* dev = nullptr;   // a device push: its item (n = its frames), layout and producer's event
+  int layout = 0;
+  cudaEvent_t ready = nullptr;
   int64_t up = 0;               // where its samples lie in the upload (floats)
   int64_t rms0 = 0, nf = 0;     // its new RMS frames in the session's RMS buffer
   int c0 = 0, c1 = 0;           // its chunks in the step's batch
@@ -1650,6 +1725,7 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
   const int sr = s->info.sample_rate;
   StepWindows win;
   std::vector<ScatterParams> sc;
+  Downmix dm;
   int64_t up_floats = 0;
   for (StepItem& it : items) {
     some_stream* st = it.st;
@@ -1688,7 +1764,9 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
       dst = st->wave.at(st->received);
       st->wave.len += it.n, st->received += it.n, st->fixed = st->received;
     }
-    if (it.n) {
+    if (it.n && it.dev) {
+      dm.push(*it.dev, it.layout, it.ready, dst);           // down-mixed straight into the window
+    } else if (it.n) {
       it.up = up_floats;
       up_floats += align4(it.n);
       sc.push_back({nullptr, dst, it.n});
@@ -1708,6 +1786,7 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
   const size_t smp_off = up.add(4ull * up_floats);
   const size_t sc_off = up.add(windows_bytes<ScatterParams>(ks));
   if (dec) dec->add(up);
+  dm.add(up, static_cast<int>(dm.items.size()));
   if (win.place(s, up, "the stream upload")) return -1;
   std::vector<HostSpan> spans;
   {
@@ -1715,7 +1794,7 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
     long long* tile0 = windows_tile0(up.h(sc_off));
     int j = 0;
     for (const StepItem& it : items)
-      if (it.n) {
+      if (it.n && !it.dev) {
         ps[j] = sc[j];
         ps[j].src = reinterpret_cast<const float*>(up.d(smp_off)) + it.up;
         tile0[j + 1] = (it.n + kScatterTile - 1) / kScatterTile;
@@ -1726,6 +1805,7 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
   }
   float* samples_d = reinterpret_cast<float*>(up.d(smp_off));
   if (dec && dec->fill(s, up, samples_d, [&](int j) { return items[j].up; })) return -1;
+  if (dm.fill(s, up)) return -1;
   copy_to_pinned(*s->pool, spans, size_t(1) << 20);          // the samples, in pieces of up to 1 MB
   if (up.send("stream upload") || (dec && dec->launch(s, up))) return -1;
   if (ks) {
@@ -1734,7 +1814,7 @@ int streams_step(some_session* s, std::vector<StepItem>& items, Decode* dec = nu
         windows_params<ScatterParams>(up.d(sc_off), ks), windows_tile0(up.d(sc_off)), ks);
     if (check_launch("stream upload scatter")) return -1;
   }
-  if (win.launch(s, up)) return -1;
+  if (dm.launch(s, up) || win.launch(s, up)) return -1;
   SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");   // also frees the upload buffer for the next step
   if (dec) {
     std::vector<std::pair<int, std::string>> failed;
@@ -2218,7 +2298,7 @@ int recordings_step(some_session* s, const std::vector<Request*>& g) {
   std::vector<int> flac;                  // the refs of the FLAC files, in upload order
   for (int k = 0; k < static_cast<int>(refs.size()); ++k) {
     RecItem& it = item(refs[k]);
-    if (it.host) continue;
+    if (it.host || it.dev) continue;
     ws.push_back({&it.m, it.bytes + it.m.data_offset, it.m.data_bytes, &it.up});
     if (!pcm_container(it.m)) flac.push_back(k);
   }
@@ -2266,7 +2346,7 @@ int recordings_step(some_session* s, const std::vector<Request*>& g) {
     const int j = static_cast<int>(rec.items.size());
     rec_of[k] = j, ref_of.push_back(k);
     rec.items.push_back({it.m.rate, it.n, it.sh, &f.rq->sl, it.out});
-    if (!it.host && pcm_container(it.m)) {
+    if (!it.host && !it.dev && pcm_container(it.m)) {
       dec.pcm.push_back(some_pcm_item{dec.bytes_d + it.up, it.n, it.m.channels, it.m.kind, 1, 0, nullptr});
       dec.pcm_of.push_back(j);
     }
@@ -2284,17 +2364,21 @@ int recordings_step(some_session* s, const std::vector<Request*>& g) {
   }
   Upload up{s};
   if (encoded) dec.add(up);
+  Downmix dm;
+  dm.add(up, static_cast<int>(std::count_if(ref_of.begin(), ref_of.end(), [&](int k) { return item(refs[k]).dev != nullptr; })));
   if (rec.place(s, up)) return -1;
   std::vector<Staged> staged;
   for (size_t j = 0; j < rec.items.size(); ++j) {
     const RecItem& it = item(refs[ref_of[j]]);
     if (it.host) staged.push_back({rec.base + rec.items[j].x, it.host, it.n});
+    if (it.dev) dm.push(*it.dev, it.layout, it.ready, rec.base + rec.items[j].x);
   }
   if ((!staged.empty() && upload_staged(s, staged)) ||
-      (encoded && dec.fill(s, up, rec.base, [&](int j) { return rec.items[j].x; })) || up.send("descriptor upload") ||
-      (encoded && dec.launch(s, up)) || rec.win.launch(s, up))
+      (encoded && dec.fill(s, up, rec.base, [&](int j) { return rec.items[j].x; })) || dm.fill(s, up) ||
+      up.send("descriptor upload") || (encoded && dec.launch(s, up)) || dm.launch(s, up) || rec.win.launch(s, up))
     return -1;
-  if (encoded || rec.win.frames) SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");   // with a recording to cut
+  // with a recording to cut; with device audio, so that the call returns only once its items have been read
+  if (encoded || rec.win.frames || dm.k) SOME_CUDA(cudaStreamSynchronize(s->stream), "synchronise");
   if (encoded) {
     std::vector<std::pair<int, std::string>> failed;
     if (dec.check(s, up, failed)) return -1;
@@ -2487,3 +2571,141 @@ int submit(some_session* s, Request& rq) {
   return rq.rc;
 }
 }  // namespace
+
+// ---------------------------------------------------------------------------------------------------- audio on the GPU
+namespace {
+// An item of device audio, checked before any GPU work (prefix: the call and the item, for the message): its frames,
+// channels and strides (*layout: some_downmix_layout's), and that its data is device memory of its device.
+int check_device_audio(const some_device_audio& a, const std::string& prefix, int* layout) {
+  const char* p = prefix.c_str();
+  SOME_REQUIRE(a.frames >= 0, "%s%lld frames", p, a.frames);
+  SOME_REQUIRE(a.frames == 0 || a.data != nullptr, "%sdata is NULL with %lld frames", p, a.frames);
+  if (some_downmix_layout(a.channels, a.frames, a.channel_stride, a.frame_stride, layout)) {
+    const std::string m = some_last_error();
+    set_error("%s%s", p, m.c_str());
+    return -1;
+  }
+  if (a.frames == 0) return 0;
+  int n_dev = 0;
+  cudaError_t e = cudaGetDeviceCount(&n_dev);
+  SOME_REQUIRE(e == cudaSuccess && a.device >= 0 && a.device < n_dev, "%sno CUDA device %d", p, a.device);
+  cudaPointerAttributes at{};
+  e = cudaPointerGetAttributes(&at, a.data);
+  if (e != cudaSuccess) cudaGetLastError();      // not a pointer the runtime knows: clear the error, refuse below
+  SOME_REQUIRE(e == cudaSuccess && at.type == cudaMemoryTypeDevice && at.device == a.device,
+               "%sdata %p is not device memory of device %d (%s)", p, static_cast<const void*>(a.data), a.device,
+               e != cudaSuccess ? cudaGetErrorString(e)
+               : at.type == cudaMemoryTypeDevice ? "it lies on another device"
+               : at.type == cudaMemoryTypeManaged ? "managed memory"
+               : "host memory");
+  return 0;
+}
+
+// The events a call records on its items' streams (one per item with frames), destroyed when the call returns: by then the
+// session's stream has passed its waits on them.
+struct ReadyEvents {
+  std::vector<cudaEvent_t> ev;
+  ~ReadyEvents() {
+    for (cudaEvent_t e : ev) cudaEventDestroy(e);
+  }
+  // Records the event item `a` is read after: at this point of a.stream, on a.device.
+  int record(const some_device_audio& a, const std::string& prefix, cudaEvent_t* out) {
+    *out = nullptr;
+    if (a.frames == 0) return 0;
+    DeviceScope scope(a.device);
+    cudaError_t e = scope.err;
+    cudaEvent_t r = nullptr;
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&r, cudaEventDisableTiming);
+    if (e == cudaSuccess) ev.push_back(r), e = cudaEventRecord(r, a.stream);
+    SOME_REQUIRE(e == cudaSuccess, "%srecording an event on the item's stream: %s", prefix.c_str(), cudaGetErrorString(e));
+    *out = r;
+    return 0;
+  }
+};
+
+// The checks of a device push to stream st, before any stream changes.
+int check_push_device(const some_stream* st, const some_device_audio& a, const std::string& prefix, int* layout) {
+  SOME_REQUIRE(a.sample_rate == st->rate, "%sthe audio is at %d Hz, the stream at %d Hz", prefix.c_str(), a.sample_rate,
+               st->rate);
+  return check_device_audio(a, prefix, layout);
+}
+}  // namespace
+
+extern "C" int some_session_transcribe_device(some_session* s, const some_device_audio* items, int count,
+                                              const some_slicer_params* params, some_notes* const* out) {
+  const char* who = "some_session_transcribe_device";
+  SOME_REQUIRE(s != nullptr && items != nullptr && out != nullptr && count >= 0, "%s: bad arguments", who);
+  if (count == 0) return 0;
+  const int sr = s->info.sample_rate;
+  some_slicer_frames sl;
+  if (some_slicer_derive(sr, params, &sl)) return -1;
+  // every item is checked before any GPU work
+  std::vector<RecItem> its(count);
+  Request rq{Request::RECORDINGS};
+  rq.recs = &its, rq.sl = sl;
+  std::map<const void*, int> seen_notes;
+  for (int i = 0; i < count; ++i) {
+    const some_device_audio& a = items[i];
+    const std::string prefix = std::string(who) + ": item " + std::to_string(i) + ": ";
+    SOME_REQUIRE(out[i] != nullptr, "%sNULL notes", prefix.c_str());
+    const auto shared = seen_notes.emplace(out[i], i);
+    SOME_REQUIRE(shared.second, "%sshares its some_notes with item %d", prefix.c_str(), shared.first->second);
+    SOME_REQUIRE(a.sample_rate > 0, "%ssample rate %d", prefix.c_str(), a.sample_rate);
+    RecItem& it = its[i];
+    if (check_device_audio(a, prefix, &it.layout)) return -1;
+    if (check_rates(a.sample_rate, sr)) {
+      const std::string m = some_last_error();
+      set_error("%s%s", prefix.c_str(), m.c_str());
+      return -1;
+    }
+    const std::string at = std::string(who) + ": item " + std::to_string(i);
+    if (slice_shape(a.frames, a.sample_rate, sr, sl, at.c_str(), &it.sh)) return -1;
+    it.dev = &a, it.m.rate = a.sample_rate, it.n = a.frames, it.out = out[i];
+    rq.samples += it.sh.n_out;
+    rq.touches.push_back(out[i]);
+  }
+  ReadyEvents ready;
+  for (int i = 0; i < count; ++i)
+    if (ready.record(items[i], std::string(who) + ": item " + std::to_string(i) + ": ", &its[i].ready)) return -1;
+  return submit(s, rq);
+}
+
+extern "C" int some_stream_push_device(some_stream* st, const some_device_audio* a, some_notes* out) {
+  const char* who = "some_stream_push_device";
+  SOME_REQUIRE(st != nullptr && a != nullptr && out != nullptr, "%s: bad arguments", who);
+  SOME_REQUIRE(!st->walk, "%s: an encoded stream takes bytes (some_stream_push_bytes)", who);
+  SOME_REQUIRE(!st->finished, "%s: the stream has finished", who);
+  const std::string prefix = std::string(who) + ": ";
+  std::vector<StepItem> items{StepItem{st, nullptr, a->frames, false, out}};
+  if (check_push_device(st, *a, prefix, &items[0].layout)) return -1;
+  items[0].dev = a;
+  ReadyEvents ready;
+  if (ready.record(*a, prefix, &items[0].ready)) return -1;
+  return stream_call(st->s, items);
+}
+
+extern "C" int some_stream_push_device_many(some_stream* const* streams, const some_device_audio* items, const int* finish,
+                                            int count, some_notes* const* out) {
+  const char* who = "some_stream_push_device_many";
+  SOME_REQUIRE(streams != nullptr && items != nullptr && out != nullptr && count >= 0, "%s: bad arguments", who);
+  if (count == 0) return 0;
+  std::vector<const float*> data(count);
+  std::vector<long long> n(count);
+  for (int i = 0; i < count; ++i) data[i] = items[i].data, n[i] = items[i].frames;
+  if (check_many(streams, data.data(), n.data(), finish, count, out, false, who)) return -1;
+  std::vector<StepItem> step;
+  step.reserve(count);
+  for (int i = 0; i < count; ++i) {
+    const bool final = finish && finish[i];
+    step.push_back(StepItem{streams[i], nullptr, items[i].frames, final, out[i]});
+    step.back().dev = &items[i];
+    if (check_push_device(streams[i], items[i], std::string(who) + ": stream " + std::to_string(i) + ": ", &step.back().layout))
+      return -1;
+  }
+  ReadyEvents ready;
+  for (int i = 0; i < count; ++i)
+    if (ready.record(items[i], std::string(who) + ": stream " + std::to_string(i) + ": ", &step[i].ready)) return -1;
+  for (int i = 0; i < count; ++i)
+    if (step[i].final) streams[i]->finished = true;
+  return stream_call(streams[0]->s, step);
+}

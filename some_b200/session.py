@@ -20,7 +20,7 @@ from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from . import _lib
+from . import _lib, audio
 # The slicer's parameters and host decisions are defined in some_b200.slicer; they stay importable from here because
 # transcribe_sliced and stream take slicer_params(...), and existing callers import them with the session.
 from .slicer import SlicerStream, slicer_frames, slicer_params, slicer_ranges  # noqa: F401
@@ -285,6 +285,59 @@ class Session:
                 for n in notes:
                     n.close()
 
+    def transcribe_device(self, tensors: Sequence, rates: Optional[Sequence[Optional[int]]] = None,
+                          params: Optional[_lib.SlicerParams] = None, frames: bool = False,
+                          notes: Optional[Sequence[Notes]] = None):
+        """some_session_transcribe_device: CUDA float32 recordings, ``[n]`` or librosa's ``[channels, n]`` (the layout is read
+        from ``stride()``: planar, or the ``[channels, n]`` view of an ``[n, channels]`` array) -> one (chunk offsets in
+        seconds, chunk sample ranges, per-chunk notes) per recording, what transcribe_sliced returns for
+        ``np.mean(y, axis=0)`` of its host copy, with no host copy.  ``rates``: each recording's rate (default: the model's).
+        Each tensor is read after the work its device's current stream holds at the call; when the call returns the
+        session no longer reads them.  Other dtypes, CPU tensors and other stride patterns raise ValueError naming the
+        index."""
+        k = len(tensors)
+        if rates is None:
+            rates = [None] * k
+        if len(rates) != k:
+            raise ValueError(f'transcribe_device: {k} recordings, {len(rates)} rates')
+        descs = [audio.device_audio(t, i, 'transcribe_device', int(r or self.sample_rate))
+                 for i, (t, r) in enumerate(zip(tensors, rates))]
+        arr = (_lib.DeviceAudio * max(k, 1))(*descs)
+        own = notes is None
+        if not own and len(notes) != k:
+            raise ValueError(f'transcribe_device: {k} recordings, {len(notes)} Notes')
+        notes = [Notes() for _ in range(k)] if own else list(notes)
+        try:
+            for n in notes:
+                n.set_frames(frames)
+            outs = (C.c_void_p * max(k, 1))(*[n.handle for n in notes])
+            _lib.check(self.lib.some_session_transcribe_device(self.handle, arr, k,
+                                                               C.byref(params) if params is not None else None, outs),
+                       'some_session_transcribe_device')
+            return [self._results(n, frames) for n in notes]
+        finally:
+            if own:
+                for n in notes:
+                    n.close()
+
+    def push_device_many(self, items: Sequence[Tuple['Stream', object]], finish: Optional[Sequence[bool]] = None,
+                         frames: bool = False):
+        """some_stream_push_device_many: push_many with CUDA float32 tensors (as Stream.push takes them) in place of host
+        samples; each tensor is at its stream's rate."""
+        k = len(items)
+        descs = [audio.device_audio(t, i, 'push_device_many', st.rate) for i, (st, t) in enumerate(items)]
+        arr = (_lib.DeviceAudio * max(k, 1))(*descs)
+        streams = (C.c_void_p * max(k, 1))(*[st.handle for st, _ in items])
+        outs = (C.c_void_p * max(k, 1))(*[st.notes.handle for st, _ in items])
+        fin = None if finish is None else np.array([bool(f) for f in finish] or [0], dtype=np.int32)
+        if fin is not None and len(finish) != k:
+            raise ValueError(f'push_device_many: {k} items, {len(finish)} finish flags')
+        for st, _ in items:
+            st.notes.set_frames(frames)
+        _lib.check(self.lib.some_stream_push_device_many(streams, arr, None if fin is None else fin.ctypes.data, k, outs),
+                   'some_stream_push_device_many')
+        return [st._results(frames=frames) for st, _ in items]
+
     def label_dataset(self, dataset, csv=None, round_midi: bool = False, overwrite: bool = False, budget: Optional[int] = None,
                       params: Optional[_lib.SlicerParams] = None, report: Optional[dict] = None):
         """some_session_label_dataset: batch_infer.py's command on a DiffSinger dataset (``transcriptions.csv`` and ``wavs/``),
@@ -379,6 +432,7 @@ class Stream:
     handle = None
     notes = None
     peeked = None
+    rate = 0                  # of the pushed samples (an encoded stream's comes from its header)
 
     def __init__(self, session: Session, sample_rate: Optional[int] = None, params: Optional[_lib.SlicerParams] = None):
         self.lib, self.session = session.lib, session
@@ -386,6 +440,7 @@ class Stream:
         _lib.check(self.lib.some_stream_open(session.handle, int(sample_rate or session.sample_rate),
                                              C.byref(params) if params is not None else None, C.byref(h)), 'some_stream_open')
         self.handle = h
+        self.rate = int(sample_rate or session.sample_rate)
         self.notes = Notes()
         session._streams.add(self)
 
@@ -407,6 +462,14 @@ class Stream:
         return self._results(self.peeked, frames)
 
     def push(self, samples: np.ndarray, frames: bool = False):
+        """some_stream_push; a CUDA float32 tensor (``[n]`` or librosa's ``[channels, n]``, at the stream's rate) goes to
+        some_stream_push_device instead: its down-mix is pushed, read on the device after the work its device's current
+        stream holds at the call."""
+        if audio.is_cuda_tensor(samples):
+            a = audio.device_audio(samples, 0, 'Stream.push', self.rate)
+            self.notes.set_frames(frames)
+            _lib.check(self.lib.some_stream_push_device(self.handle, C.byref(a), self.notes.handle), 'some_stream_push_device')
+            return self._results(frames=frames)
         x = np.ascontiguousarray(samples, dtype=np.float32)
         self.notes.set_frames(frames)
         _lib.check(self.lib.some_stream_push(self.handle, x.ctypes.data, int(x.shape[0]), self.notes.handle), 'some_stream_push')
